@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — denoiser-steps/sec of the NaturalSpeech2 hot path on B200 (BASELINE.json metric).
+"""bench.py — denoiser-steps/sec of the NaturalSpeech2 hot path on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -17,13 +17,13 @@ Printed JSON (one line, rank 0): the base contract keys plus
                 mean launch time measured with CUDA events inside real steps, against BOTH measured bf16 peaks of
                 MEASURED_PEAKS.json (burst and sustained); step-level fractions beside it
   parity        the step's own output checked in the run: the first CPU_SAMPLE_BATCH samples of the SAME inputs go
-                through the reference (baseline/_ref, fp32 on the host) and are compared with the GPU prediction
+                through the reference (oracle/_ref, fp32 on the host) and are compared with the GPU prediction
   cpu_baseline  the reference's own CPU path timed on that bounded sample (N=1 only)
   e2e           the same metric with HOST buffers: pinned-host -> device copy of the step's inputs and device ->
                 pinned-host copy of the full prediction inside the timed region (double-buffered on side streams)
   secondary     the other quantities BASELINE.json's metric names: RVQ Mcodes/s (configs[3], 1M frames, bit-exact
                 sample check, own roofline) and the conditional denoiser (configs[2], B=16) steps/s
-`--impl reference` times the reference arm: the UNMODIFIED reference (pip-installed into baseline/_ref, third-party
+`--impl reference` times the reference arm: the UNMODIFIED reference (pip-installed into oracle/_ref, third-party
 imports it does not need on this path stubbed) on the host cores, same metric/unit/config; rank 0 only.
 """
 from __future__ import annotations
@@ -56,15 +56,15 @@ CPU_SAMPLE_BATCH = 4   # bounded sample of the 32-sample workload step for the i
 def build_config(world: int) -> dict:
     """Identical for both arms (the driver compares them)."""
     return {"workload": WORKLOAD, "global_batch": BATCH * world, "seq_len": SEQ, "parallelism": f"dp{world}",
-            "l2": "no flush needed: each step streams ~1.3 GB of activations + 0.5 GB of weights, >> 126 MB L2"}
+            "l2": "no flush needed: each step streams ~1.3 GB of activations + 0.5 GB of weights, >> 50 MB L2"}
 
 
 def _peaks():
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         return json.loads(p.read_text()), "measured (MEASURED_PEAKS.json)"
-    return ({"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0},
-            "fallback (B200_PROFILING.md)")
+    return ({"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0},
+            "fallback: NVIDIA H100 SXM data sheet (dense bf16, 700 W), not measured")
 
 
 def _ncu_traffic():
@@ -128,7 +128,7 @@ class ClockSampler:
 
 
 # ------------------------------------------------------------------------------------------------------
-# the reference (baseline/_ref) on the host
+# the reference (oracle/_ref) on the host
 # ------------------------------------------------------------------------------------------------------
 def _host_threads() -> int:
     """CPU threads this process may really use: affinity mask, capped by the cgroup CPU quota (oversubscribing a
@@ -144,10 +144,10 @@ def _host_threads() -> int:
 
 
 def import_reference():
-    """The unmodified reference package from baseline/_ref (`pip install --no-deps --target baseline/_ref`, recorded
+    """The unmodified reference package from oracle/_ref (`pip install --no-deps --target oracle/_ref`, recorded
     in DESIGN.md).  Third-party modules it imports at module scope but never touches on the denoiser path are
     stubbed (SURVEY Appendix A).  Returns the `naturalspeech2_pytorch.naturalspeech2_pytorch` module or None."""
-    ref_dir = ROOT / "baseline" / "_ref"
+    ref_dir = ROOT / "oracle" / "_ref"
     if not (ref_dir / "naturalspeech2_pytorch").exists():
         return None
     import torch
@@ -189,7 +189,7 @@ def import_reference():
 
 
 class HostReference:
-    """The reference denoiser on the host cores: baseline/_ref when importable (kind 'reference'), else the
+    """The reference denoiser on the host cores: oracle/_ref when importable (kind 'reference'), else the
     torch port of the oracle (kind 'port').  Same fp32 weights as the GPU model (state_dict keys are identical)."""
 
     def __init__(self, state_dict=None):
@@ -205,7 +205,7 @@ class HostReference:
             self.kind = "reference"
             self.model = self.ns2.Model(**CFG).eval()
             self.model.load_state_dict(sd)
-            self.desc = "unmodified reference Model.forward from baseline/_ref, torch fp32 CPU"
+            self.desc = "unmodified reference Model.forward from oracle/_ref, torch fp32 CPU"
         else:
             from oracle import denoiser_oracle, denoiser_torch_port
             self.kind = "port"
@@ -289,13 +289,13 @@ def secondary_rvq(dev, peaks):
     ref = rvq_oracle.encode(x[idx.to(dev)].cpu().numpy(), cb.numpy())
     rows_diff = int((out[idx.to(dev)].cpu().numpy() != ref).any(axis=1).sum())
     flops = 2.0 * F * Q * K * 128
-    burst = float(peaks.get("bf16_tflops", 1590.0))
+    burst = float(peaks.get("bf16_tflops", 989.0))
     return {"metric": "RVQ Mcodes/sec", "value": round(F * Q / (ms * 1e-3) / 1e6, 1), "unit": "Mcodes/s",
             "workload": "configs[3]: 8 quantizers x 1024 codes x dim 128, 1,048,576 frames, exact (bit-exact) indices",
             "ms_per_launch": round(ms, 3), "bit_exact_rows_diff_of_4096": rows_diff,
             "roofline": {"bound": "tensor", "achieved": round(flops / (ms * 1e-3) / 1e12, 1), "peak": burst,
                          "unit": "TFLOP/s", "frac": round(flops / (ms * 1e-3) / 1e12 / burst, 4),
-                         "note": "fp16 tcgen05 distance filter + exact re-score; algorithmic 2*F*Q*K*d FLOPs vs "
+                         "note": "fp16 wgmma distance filter + exact re-score; algorithmic 2*F*Q*K*d FLOPs vs "
                                  "burst bf16 peak (kernel timed alone)"}}
 
 
@@ -373,10 +373,10 @@ def secondary_aligner(dev, peaks):
                                  "expansion kernel",
                         "algorithmic_bytes": 3 * b * t_x * t_y * 4,
                         "achieved_GBps": round(3 * b * t_x * t_y * 4 / (ms * 1e-3) / 1e9, 1),
-                        "peak_GBps": float(peaks.get("hbm_gbs", 6650.0))}}
+                        "peak_GBps": float(peaks.get("hbm_gbs", 3350.0))}}
     try:
         if import_reference() is None:
-            raise RuntimeError("baseline/_ref is not present")
+            raise RuntimeError("oracle/_ref is not present")
         import time
         from naturalspeech2_pytorch.aligner import maximum_path as ref_mas
         torch.set_num_threads(_host_threads())
@@ -421,7 +421,7 @@ def secondary_prompt_encoder(dev, peaks):
     D, Di, depth = 512, 1365, 6
     tr_flops = depth * (2.0 * Np * D * 3 * D + 4.0 * Np * Np * D + 2.0 * Np * D * D + 2.0 * Np * D * 2 * Di + 2.0 * Np * Di * D)
     flops = B * (conv_flops + tr_flops)
-    burst = float(peaks.get("bf16_tflops", 1590.0))
+    burst = float(peaks.get("bf16_tflops", 989.0))
     out = {"metric": "prompts/sec", "unit": "prompts/s", "value": round(B / (ms * 1e-3), 1), "ms_per_batch": round(ms, 4),
            "workload": "SpeechPromptEncoder(dim_codebook=128) default dims, prompt batch (16, 103, 128), forward only",
            "isfinite": bool(torch.isfinite(y).all()),
@@ -432,7 +432,7 @@ def secondary_prompt_encoder(dev, peaks):
     try:
         ns2 = import_reference()
         if ns2 is None:
-            raise RuntimeError("baseline/_ref is not present")
+            raise RuntimeError("oracle/_ref is not present")
         torch.set_num_threads(_host_threads())
         ref = ns2.SpeechPromptEncoder(dim_codebook=Dc).eval()
         ref.load_state_dict(enc.state_dict())
@@ -626,6 +626,8 @@ def run_ours(args):
     value = world * args.steps / (ms_total / 1e3)
     gpu_head = pred[:CPU_SAMPLE_BATCH].float().cpu()
     loss_value = float(losses[(args.steps - 1) & 1].item()) / world
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, pred, losses[(args.steps - 1) & 1])
 
     # ------------------------------- e2e: host buffers in, host buffers out --------------------------
     model.use_cuda_graphs = not args.no_cuda_graphs   # the public API call replays the model's own captured graph
@@ -697,13 +699,13 @@ def run_ours(args):
         model._prof = None
         conv_mean = statistics.mean(by_name["ff_conv"])
         peaks, peak_src = _peaks()
-        burst = float(peaks.get("bf16_tflops", 1590.0))
+        burst = float(peaks.get("bf16_tflops", 989.0))
         sus = float(peaks.get("bf16_tflops_sustained", burst))
         achieved = CONV_FLOPS_PER_LAUNCH / (conv_mean * 1e-3) / 1e12
         step_tf = FLOPS_PER_SAMPLE * BATCH / (ms_per_step * 1e-3) / 1e12
         traffic, traffic_src = _ncu_traffic()
         roof = {"bound": "tensor",
-                "kernel": "ns2::gemm2_kernel<256,1,NS2_EPI_BF16> (CTA-pair tcgen05 GEMM; FFN causal conv k=3 as 3 "
+                "kernel": "ns2::gemm_kernel<256,1,NS2_EPI_BF16> (wgmma GEMM; FFN causal conv k=3 as 3 "
                           "shifted-row segments)",
                 "achieved": round(achieved, 1), "peak": burst, "unit": "TFLOP/s", "frac": round(achieved / burst, 4),
                 "frac_burst": round(achieved / burst, 4), "frac_sustained": round(achieved / sus, 4),
@@ -742,6 +744,24 @@ def run_ours(args):
         _emit(line)
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_ROWS = 8192   # (sample, position) rows of the prediction written by --dump-outputs: 16 MB of float32
+
+
+def dump_outputs(out_dir, pred, loss):
+    """What the timed step returned in its last iteration: the denoiser prediction (a fixed, seeded sample of DUMP_ROWS
+    of its BATCH x SEQ rows, in ascending row order) and the batch-mean MSE loss.  The inputs are seeded, so two builds
+    run with the same arguments can be compared output for output."""
+    import numpy as np
+    import torch
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    rows = torch.randperm(BATCH * SEQ, generator=torch.Generator().manual_seed(1234))[:DUMP_ROWS].sort().values
+    flat = pred.detach().reshape(BATCH * SEQ, -1).float().cpu()
+    np.save(d / "pred_rows.npy", flat[rows].numpy().astype(np.float32))
+    np.save(d / "pred_row_index.npy", rows.numpy().astype(np.float64))
+    np.save(d / "loss.npy", np.array([float(loss.item())], dtype=np.float64))
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -816,6 +836,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-secondary", action="store_true")
     ap.add_argument("--no-cuda-graphs", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs to DIR/<name>.npy")
     ap.add_argument("--ref-max-batch", type=int, default=BATCH,
                     help="reference arm: cap on the per-step sample batch (tests use 2)")
     args = ap.parse_args()

@@ -1,4 +1,4 @@
-/* ns2_b200.h — C ABI of libns2b200.so: the sm_100a kernels behind the NaturalSpeech2 denoiser hot path.
+/* ns2_b200.h — C ABI of libns2b200.so: the sm_90a kernels behind the NaturalSpeech2 denoiser hot path.
  *
  * The reference (lucidrains/naturalspeech2-pytorch @ 659bec7) has no FFI of its own; its boundary for this
  * path is Python (nn.Module classes).  Each entry point below replaces the PyTorch library calls the
@@ -13,8 +13,8 @@
  *  - activations are token-major (batch, position, channel) with the channel contiguous;
  *  - "bf16" buffers hold IEEE bfloat16, "f32" IEEE binary32, codes are int64 (as in the reference).
  */
-#ifndef NS2_B200_H_
-#define NS2_B200_H_
+#ifndef NS2_H100_H_
+#define NS2_H100_H_
 
 #include <stdint.h>
 
@@ -29,13 +29,13 @@ typedef void* ns2_stream_t; /* cudaStream_t */
 const char* ns2_last_error(void);
 int ns2_abi_version(void);
 /* Size the persistent grids of every kernel for at most `sms` SMs (rounded down to an even count; 0 = all SMs, the
- * default).  The GEMM / attention kernels run one CTA (pair) per SM for the whole launch, so a concurrent kernel that
+ * default).  The GEMM / attention kernels run one CTA per SM for the whole launch, so a concurrent kernel that
  * holds a few SMs - NCCL's all-reduce of the gradients during the backward pass (ns2.py:1723-1726, 1886) - would delay
  * whole CTAs by a full tile loop; leaving those SMs out of the grid avoids that.  Returns the previous limit. */
 int ns2_set_sm_limit(int sms);
 
 /* ------------------------------------------------------------------------------------------------
- * 1. Segmented tcgen05 GEMM with fused epilogues.
+ * 1. Segmented wgmma GEMM with fused epilogues.
  *
  * Computes, for every group g, batch b, position n and output channel j
  *     acc_a[b,n,j] = sum over segments s with segs[s].acc == a, k < segs[s].k_len of
@@ -98,16 +98,15 @@ typedef struct ns2_gemm_args {
   int64_t film_batch_stride;
   int32_t film_group_stride;
   int32_t flags;           /* 0, or NS2_GEMM_FLAG_* */
-  void* debug_timeline;    /* bring-up aid, normally NULL: device buffer of 64*8 int64 receiving clock64 stamps of CTA
-                              pair 0 of the CTA-pair kernel (tools/gemm_timeline.py) */
+  void* debug_timeline;    /* reserved, ignored (keeps the struct layout of ABI v3) */
 } ns2_gemm_args;
 
-#define NS2_GEMM_FLAG_SKIP_EPILOGUE 1  /* measurement aid: run the TMA/MMA mainloop only, write nothing (CTA-pair kernel) */
+#define NS2_GEMM_FLAG_SKIP_EPILOGUE 1  /* measurement aid: run the TMA/MMA mainloop only, write nothing */
 #define NS2_GEMM_FLAG_SILU 4 /* BF16 / F32 epilogues: out = silu(acc + bias) (+ resid) — Conv1d + nn.SiLU of the prompt
                                encoder (ns2.py:316-320) and CausalConv1d + SiLU of the phoneme encoder (ns2.py:255-257) */
-#define NS2_GEMM_FLAG_NARROW_LAST 8 /* tuning / A-B tests (CTA-pair kernel, n % 256 != 0): schedule the partial-width n-tiles
+#define NS2_GEMM_FLAG_NARROW_LAST 8 /* tuning / A-B tests (groups == 1, n % BN != 0): schedule the partial-width n-tiles
                                       after all full-width ones instead of n-fastest */
-#define NS2_GEMM_FLAG_WAVENET_ONE_PASS 2 /* tuning / A-B tests: WAVENET with two 256-column accumulators and a single epilogue pass */
+#define NS2_GEMM_FLAG_WAVENET_ONE_PASS 2 /* accepted and ignored: WAVENET tiles always hold both accumulators */
 
 int ns2_gemm(const ns2_gemm_args* args, ns2_stream_t stream);
 
@@ -146,19 +145,20 @@ typedef struct ns2_attn_args {
   void* out;     int64_t o_row_stride, o_batch_stride;
   int32_t batches, heads, q_len, kv_len, dim_head;
   float scale;
-  int32_t kernel;   /* NS2_ATTN_AUTO, or force one implementation (tests / tuning) */
-  void* debug_timeline; /* bring-up aid, normally NULL: device buffer of 64*16 int64 receiving clock64 stamps of CTA 0
-                           of the two-tile kernel (tools/attn_timeline.py) */
+  int32_t kernel;   /* one of NS2_ATTN_*; validated, every value runs the same sm_90a kernel */
+  void* debug_timeline; /* reserved, ignored (keeps the struct layout of ABI v3) */
   float* lse;           /* optional (batches, heads, q_len) f32: log2-domain log-sum-exp of the scaled score rows,
                            saved for ns2_attn_bwd */
 } ns2_attn_args;
 
-#define NS2_ATTN_AUTO 0            /* two-tile kernel when q_len > 128 and kv_len > 64, else one-tile */
-#define NS2_ATTN_ONE_TILE 1        /* 128 queries x 64-key tiles per CTA, P staged in shared memory */
-#define NS2_ATTN_TWO_TILE 2        /* persistent, 2 x 128 queries x 128-key tiles, P and O in tensor memory */
-#define NS2_ATTN_TWO_TILE_POLY2 3  /* same, 2 of every 8 exponentials on the FMA pipe (degree-3 polynomial) */
-#define NS2_ATTN_TWO_TILE_POLY4 4  /* same, 4 of every 8 */
-#define NS2_ATTN_TWO_TILE_LOCKSTEP 5 /* two-tile without the exponential-section turn taking (A/B measurement) */
+/* Kernel selectors of ABI v3.  On sm_90a one kernel (128 queries x 128-key tiles per CTA, P kept in registers as the
+ * wgmma A operand) serves every shape, so all selectors give identical results. */
+#define NS2_ATTN_AUTO 0
+#define NS2_ATTN_ONE_TILE 1
+#define NS2_ATTN_TWO_TILE 2
+#define NS2_ATTN_TWO_TILE_POLY2 3
+#define NS2_ATTN_TWO_TILE_POLY4 4
+#define NS2_ATTN_TWO_TILE_LOCKSTEP 5
 
 int ns2_attn_fwd(const ns2_attn_args* args, ns2_stream_t stream);
 
@@ -295,7 +295,7 @@ int ns2_x_start(const float* x, const float* pred, const float* alpha, const flo
  * 7. Residual vector quantisation (Encodec RVQ encode/decode; third-party code reached from
  *    ns2.py:1445,1611 via audiolm_pytorch.EncodecWrapper -> encodec ResidualVectorQuantizer).
  *    ns2_rvq_prepare : codebooks f32 (Q, K, d) -> cb_f16: NS2_RVQ_PREPARED_HALFS(Q, K, d) fp16 values = the copy
- *                      (Q, K, d) scaled by 2^-e_q followed by the (Q, K, 16) norm blocks (||c||^2 as an fp16 hi/lo pair,
+ *                      (Q, K, d) scaled by 2^-e_q, codes permuted inside each 128-code chunk, followed by the (Q, K, 16) norm blocks (||c||^2 as an fp16 hi/lo pair,
  *                      laid out for the tensor core); ||c||^2 f32 (Q, K); meta f32 (Q, 2) = {max_k ||c_k||, 2^e_q}
  *    ns2_rvq_encode  : frames f32 (F, d) -> codes int64 (F, Q); residual chain in fp32, nearest
  *                      codeword by exact squared L2 distance, ties -> lowest index.  d must be 128,
@@ -379,4 +379,4 @@ int64_t ns2_launch_count(void);
 #ifdef __cplusplus
 }
 #endif
-#endif /* NS2_B200_H_ */
+#endif /* NS2_H100_H_ */

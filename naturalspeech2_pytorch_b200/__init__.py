@@ -1,4 +1,4 @@
-"""B200-native (sm_100a) implementation of the NaturalSpeech2 denoiser hot path.
+"""H100-native (sm_90a) implementation of the NaturalSpeech2 denoiser hot path.
 
 Public names mirror naturalspeech2_pytorch/__init__.py:8-24 for the path this package accelerates:
 `Model` (the denoiser) and, once imported below, `NaturalSpeech2` (diffusion wrapper) and `EncodecRVQ`

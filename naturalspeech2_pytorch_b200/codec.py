@@ -1,7 +1,7 @@
-"""`EncodecRVQ`: the residual-VQ step of the Encodec codec on sm_100a, behind the duck-type that
+"""`EncodecRVQ`: the residual-VQ step of the Encodec codec on sm_90a, behind the duck-type that
 `NaturalSpeech2` expects from `audiolm_pytorch.EncodecWrapper` (ns2.py:1213-1214, 1244-1246, 1445, 1496, 1611).
 
-In scope (SURVEY a16): nearest-codeword search over Q sequential residual stages (`ops.rvq_encode`, tcgen05
+In scope (SURVEY a16): nearest-codeword search over Q sequential residual stages (`ops.rvq_encode`, wgmma
 distance filter + exact fp64 re-score => bit-exact indices) and the sum-of-codewords decode (`ops.rvq_decode`).
 Out of scope: Encodec's SEANet conv/LSTM encoder and decoder (pretrained weights are not available offline and
 the north star does not name them).  They plug in as callables:

@@ -1,16 +1,13 @@
-// Flash attention forward on tcgen05 for sm_100a (non-causal, unmasked, dim_head = 64).
+// Flash attention forward on wgmma for sm_90a (non-causal, unmasked, dim_head = 64).
 // Replaces Attend.forward / F.scaled_dot_product_attention (attend.py:77-155) for the only configuration
 // the denoiser uses: mask=None, causal=False, dropout=0 (SURVEY T9).
 //
-// One CTA per (batch, head, 128-query tile); 192 threads:
-//   warps 0-3  softmax: thread r owns query row r (TMEM lane r): tcgen05.ld S -> online softmax in fp32 ->
-//              P (bf16) written to shared memory in the 128B-swizzled K-major layout UMMA expects ->
-//              running output kept in registers, rescaled and accumulated from the per-tile P.V product
-//   warp 4     TMA producer: Q once, then K_j / V_j tiles (128 keys x 64) through a 2-stage ring
-//   warp 5     tcgen05.mma issuer: S_j = Q.K_j^T (both K-major), O_j = P_j.V_j (V is the MN-major operand:
-//              its rows are keys = the reduction dimension, so no transpose of V is ever materialised)
-// 64-key tiles; S (TMEM), P (smem) and O_j (TMEM) are double-buffered so S_{j+1} and S_{j+2} are computed while the
-// softmax warps process tile j.  Two CTAs are co-resident per SM.
+// One CTA per (batch, head, 128-query tile); 384 threads:
+//   warpgroup 0     TMA producer (warp 0): Q once, then K_j / V_j tiles (128 keys x 64) through a KVS-stage ring
+//   warpgroups 1-2  softmax warpgroups, 64 query rows each: S = Q K_j^T by wgmma (both operands K-major in shared
+//                   memory, fp32 accumulator fragments in registers) -> online softmax in fp32 -> P packed to bf16
+//                   straight from the S fragments into the A-operand fragments of O += P V_j (register-A wgmma; V is
+//                   the MN-major B operand: its rows are keys = the reduction dimension, so V is never transposed)
 #include "ptx.cuh"
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
@@ -22,22 +19,18 @@ namespace ns2 {
 extern std::atomic<long long> g_launches;
 
 namespace attn {
-constexpr int BQ = 128;   // queries per CTA
-constexpr int BKV = 64;   // keys per tile
+constexpr int BQ = 128;   // queries per CTA (64 per softmax warpgroup)
+constexpr int BKV = 128;  // keys per tile
 constexpr int DH = 64;
-constexpr int KVS = 4;    // K/V ring depth
+constexpr int KVS = 3;    // K/V ring depth
 constexpr int Q_BYTES = BQ * DH * 2;         // 16 KB
-constexpr int KV_BYTES = BKV * DH * 2;       // 8 KB each for K and V
-constexpr int P_BYTES = BQ * BKV * 2;        // 16 KB: one 64-key swizzle atom
+constexpr int KV_BYTES = BKV * DH * 2;       // 16 KB each for K and V
 constexpr int OFF_Q = 0;
 constexpr int OFF_K = OFF_Q + Q_BYTES;                 // KVS stages
 constexpr int OFF_V = OFF_K + KVS * KV_BYTES;          // KVS stages
-constexpr int OFF_P = OFF_V + KVS * KV_BYTES;          // 2 buffers
-constexpr int OFF_BAR = OFF_P + 2 * P_BYTES;
-constexpr int SMEM_BYTES = OFF_BAR + 256;              // 112.25 KB -> two CTAs per SM
-constexpr int TMEM_COLS = 256;                         // two CTAs per SM share the 512 columns
-constexpr int TM_S = 0;     // S buffers at columns 0 and 64
-constexpr int TM_O = 128;   // O_j buffers at columns 128 and 192
+constexpr int OFF_BAR = OFF_V + KVS * KV_BYTES;
+constexpr int SMEM_BYTES = OFF_BAR + 256;              // 112.25 KB
+constexpr int THREADS = 384;
 }  // namespace attn
 
 struct AttnDev {
@@ -49,33 +42,19 @@ struct AttnDev {
   float* lse;   // optional (batches, heads, q_len): log2-domain log-sum-exp of the scaled scores, for the backward pass
 };
 
-// bf16 pair from two non-negative finite floats with round-half-up done on the integer pipe (IADD + PRMT): the
-// F2FP conversion shares the 16-lane XU pipe with ex2, which bounds the softmax throughput.
-__device__ __forceinline__ uint32_t pack_bf16x2_pos(float lo, float hi) {
-  return __byte_perm(__float_as_uint(lo) + 0x8000u, __float_as_uint(hi) + 0x8000u, 0x7632);
-}
-
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
 
-// One-pass online-softmax flash attention on 64-key tiles.  S and P are double-buffered (TMEM / smem) so that the
-// tensor core computes S_{j+1}, S_{j+2} while the softmax warps work on tile j and never waits for them in steady
-// state; the per-tile P.V product is folded into the register-resident output one tile late.
-// Two CTAs are resident per SM (112 KB smem, 256 TMEM columns each).
-__global__ void __launch_bounds__(192, 2) attn_fwd_kernel(const __grid_constant__ AttnDev p) {
+__global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid_constant__ AttnDev p) {
   using namespace attn;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* q_full = bars + 0;
   uint64_t* kv_full = bars + 1;            // [KVS]
-  uint64_t* kv_empty = bars + 1 + KVS;     // [KVS]
-  uint64_t* s_full = bars + 1 + 2 * KVS;   // [2]
-  uint64_t* p_full = bars + 3 + 2 * KVS;   // [2] 128 arrivals: P_j written and S_j consumed
-  uint64_t* o_full = bars + 5 + 2 * KVS;   // [2]
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 7 + 2 * KVS);
+  uint64_t* kv_empty = bars + 1 + KVS;     // [KVS] one arrive per softmax warp
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * BQ;
@@ -83,37 +62,27 @@ __global__ void __launch_bounds__(192, 2) attn_fwd_kernel(const __grid_constant_
   const int b = blockIdx.z;
   const int T = (p.kv_len + BKV - 1) / BKV;
 
-  if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) {
-    printf("ns2 attn: dynamic shared memory is not 1024-byte aligned\n");
-    __trap();
-  }
-  if (warp == 4 && lane == 0) {
+  if (threadIdx.x == 0) {
+    if ((smem_u32(smem) & 1023u) != 0) {
+      printf("ns2 attn: dynamic shared memory is not 1024-byte aligned\n");
+      __trap();
+    }
     tma_prefetch_desc(&p.tmQ);
     tma_prefetch_desc(&p.tmK);
     tma_prefetch_desc(&p.tmV);
-  }
-  if (warp == 5 && lane == 0) {
     mbar_init(smem_u32(q_full), 1);
     for (int i = 0; i < KVS; ++i) {
       mbar_init(smem_u32(&kv_full[i]), 1);
-      mbar_init(smem_u32(&kv_empty[i]), 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(&s_full[i]), 1);
-      mbar_init(smem_u32(&p_full[i]), 128);
-      mbar_init(smem_u32(&o_full[i]), 1);
+      mbar_init(smem_u32(&kv_empty[i]), 8);
     }
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc(smem_u32(tmem_holder), TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
 
-  if (warp == 4) {
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     // ================================ TMA producer ================================
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       mbar_arrive_expect_tx(smem_u32(q_full), Q_BYTES);
       tma_load_3d(smem_u32(smem + OFF_Q), &p.tmQ, smem_u32(q_full), head * DH, q0, b);
       for (int j = 0; j < T; ++j) {
@@ -126,643 +95,106 @@ __global__ void __launch_bounds__(192, 2) attn_fwd_kernel(const __grid_constant_
         tma_load_3d(smem_u32(smem + OFF_V + st * KV_BYTES), &p.tmV, fb, head * DH, j * BKV, b);
       }
     }
-  } else if (warp == 5) {
-    // ================================ MMA issuer ==================================
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma_idesc_f16(BQ, BKV, 1, 0, 0);
-      constexpr uint32_t idesc_o = umma_idesc_f16(BQ, DH, 1, 0, /*V is MN-major*/ 1);
-      const uint64_t dq = umma_desc_sw128(smem_u32(smem + OFF_Q), 16, 1024);
-      auto issue_s = [&](int j) {
-        const int st = j % KVS;
-        mbar_wait(smem_u32(&kv_full[st]), (j / KVS) & 1);
-        tc_fence_after();
-        const uint64_t dk = umma_desc_sw128(smem_u32(smem + OFF_K + st * KV_BYTES), 16, 1024);
-#pragma unroll
-        for (int k = 0; k < DH / 16; ++k)
-          tc_mma_f16(tmem_base + TM_S + (j & 1) * BKV, dq + 2 * k, dk + 2 * k, idesc_s, k > 0);
-        tc_commit(smem_u32(&s_full[j & 1]));
-      };
-      mbar_wait(smem_u32(q_full), 0);
-      issue_s(0);
-      if (T > 1) issue_s(1);
-      for (int j = 0; j < T; ++j) {
-        const int bsel = j & 1;
-        const int st = j % KVS;
-        // P_j is in smem and the softmax warps are done reading S_j
-        mbar_wait(smem_u32(&p_full[bsel]), (j >> 1) & 1);
-        tc_fence_after();
-        const uint32_t pbase = smem_u32(smem + OFF_P + bsel * P_BYTES);
-        const uint32_t vbase = smem_u32(smem + OFF_V + st * KV_BYTES);
-#pragma unroll
-        for (int k = 0; k < BKV / 16; ++k) {
-          // A = P: K-major, one 64-key atom, 32 bytes per 16-key step
-          const uint64_t dp = umma_desc_sw128(pbase + k * 32, 16, 1024);
-          // B = V: MN-major (64 dh contiguous per key row of 128 B); 16 keys = 2048 bytes per step
-          const uint64_t dv = umma_desc_sw128(vbase + k * 2048, 1024, 1024);
-          tc_mma_f16(tmem_base + TM_O + bsel * DH, dp, dv, idesc_o, k > 0);
-        }
-        tc_commit(smem_u32(&o_full[bsel]));
-        tc_commit(smem_u32(&kv_empty[st]));
-        if (j + 2 < T) issue_s(j + 2);  // S buffer `bsel` is free again
-      }
-    }
   } else {
-    // ================================ softmax warps ===============================
-    const int row = warp * 32 + lane;
-    const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    // ================================ softmax warpgroups ===============================
+    const int w = (warp >> 2) - 1;              // query rows [64 w, 64 w + 64) of the tile
+    const int r0 = 64 * w + 16 * (warp & 3) + (lane >> 2);   // this thread's rows: r0 and r0 + 8
+    const int c2 = 2 * (lane & 3);
     const float c = p.scale_log2e;
-    float o_acc[DH];
+    float o_acc[DH / 2];
 #pragma unroll
-    for (int i = 0; i < DH; ++i) o_acc[i] = 0.f;
-    float m_run = -INFINITY, l_run = 0.f, a_prev = 0.f;
-
-    auto accumulate_o = [&](int jprev, float a) {
-      const int bs = jprev & 1;
-      mbar_wait(smem_u32(&o_full[bs]), (jprev >> 1) & 1);
-      tc_fence_after();
-      uint32_t r0[32], r1[32];
-      tmem_ld32(lane_addr + TM_O + bs * DH, r0);
-      tmem_ld32(lane_addr + TM_O + bs * DH + 32, r1);
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        o_acc[i] = fmaf(o_acc[i], a, __uint_as_float(r0[i]));
-        o_acc[32 + i] = fmaf(o_acc[32 + i], a, __uint_as_float(r1[i]));
-      }
-    };
+    for (int i = 0; i < DH / 2; ++i) o_acc[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // l_run: this thread's partial row sums
+    const uint64_t dq = gmma_desc_sw128(smem_u32(smem + OFF_Q + w * (64 * 128)), 16, 1024);
+    mbar_wait(smem_u32(q_full), 0);
 
     for (int j = 0; j < T; ++j) {
-      const int bsel = j & 1;
-      mbar_wait(smem_u32(&s_full[bsel]), (j >> 1) & 1);
-      tc_fence_after();
-      const int valid = p.kv_len - j * BKV;  // columns >= valid are padding keys
-      const bool full = valid >= BKV;
-      const uint32_t s_addr = lane_addr + TM_S + bsel * BKV;
-      // S_j is read from TMEM exactly once (TMEM reads run at ~64 B/clk per SM and were the bottleneck of the
-      // two-pass version): 64 scores stay in registers for both the maximum and the exponentials
-      uint32_t r0[32], r1[32];
-      tmem_ld32(s_addr, r0);
-      tmem_ld32(s_addr + 32, r1);
-      tmem_ld_wait();
-      float m_tile;
+      const int st = j % KVS;
+      mbar_wait(smem_u32(&kv_full[st]), (j / KVS) & 1);
+      float s[BKV / 2];
       {
-        float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;
-        if (full) {
+        const uint64_t dk = gmma_desc_sw128(smem_u32(smem + OFF_K + st * KV_BYTES), 16, 1024);
+        wgmma_fence();
 #pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            m0 = fmaxf(m0, __uint_as_float(r0[i]));
-            m1 = fmaxf(m1, __uint_as_float(r0[i + 1]));
-            m2 = fmaxf(m2, __uint_as_float(r1[i]));
-            m3 = fmaxf(m3, __uint_as_float(r1[i + 1]));
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            if (i < valid) m0 = fmaxf(m0, __uint_as_float(r0[i]));
-            if (32 + i < valid) m1 = fmaxf(m1, __uint_as_float(r1[i]));
-          }
-        }
-        m_tile = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
+        for (int k = 0; k < DH / 16; ++k) wgmma_bf16_ss_n128<0, 0>(s, dq + 2 * k, dk + 2 * k, k > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_hold(s);
       }
-      const float m_new = fmaxf(m_run, m_tile * c);
-      const float a = ex2_approx(m_run - m_new);  // 0 on the first tile (m_run = -inf)
-      // probabilities -> bf16 -> swizzled smem; row sum in fp32 (4 independent chains)
-      // (P buffer `bsel` was last read by P.V of tile j-2, whose completion was awaited in iteration j-1)
-      float l_tile;
+      const int valid = p.kv_len - j * BKV;  // columns >= valid are padding keys (TMA zero-filled): excluded
+      if (valid < BKV) {
+#pragma unroll
+        for (int jj = 0; jj < BKV / 8; ++jj)
+#pragma unroll
+          for (int e = 0; e < 4; ++e)
+            if (8 * jj + c2 + (e & 1) >= valid) s[4 * jj + e] = -INFINITY;
+      }
+      float a[2], m_new[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        float m = -INFINITY;
+#pragma unroll
+        for (int jj = 0; jj < BKV / 8; ++jj) m = fmaxf(m, fmaxf(s[4 * jj + 2 * i], s[4 * jj + 2 * i + 1]));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));   // the four threads of a quad share the row
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+        m_new[i] = fmaxf(m_run[i], m * c);
+        a[i] = ex2_approx(m_run[i] - m_new[i]);   // 0 on the first tile (m_run = -inf)
+        m_run[i] = m_new[i];
+        l_run[i] *= a[i];
+      }
+#pragma unroll
+      for (int jj = 0; jj < DH / 8; ++jj) {
+        o_acc[4 * jj + 0] *= a[0];
+        o_acc[4 * jj + 1] *= a[0];
+        o_acc[4 * jj + 2] *= a[1];
+        o_acc[4 * jj + 3] *= a[1];
+      }
+      // P = exp2(s c - m) -> bf16 A fragments (16 keys per k-step: S fragments 2k and 2k + 1)
+      uint32_t pa[BKV / 16][4];
+#pragma unroll
+      for (int jj = 0; jj < BKV / 8; ++jj) {
+        const float p0 = ex2_approx(fmaf(s[4 * jj + 0], c, -m_new[0]));
+        const float p1 = ex2_approx(fmaf(s[4 * jj + 1], c, -m_new[0]));
+        const float p2 = ex2_approx(fmaf(s[4 * jj + 2], c, -m_new[1]));
+        const float p3 = ex2_approx(fmaf(s[4 * jj + 3], c, -m_new[1]));
+        l_run[0] += p0 + p1;
+        l_run[1] += p2 + p3;
+        pa[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(p0, p1);
+        pa[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(p2, p3);
+      }
       {
-        uint8_t* prow = smem + OFF_P + bsel * P_BYTES + row * 128;
-        float l0 = 0.f, l1 = 0.f, l2 = 0.f, l3 = 0.f;
-        auto chunk32 = [&](const uint32_t (&r)[32], int cc) {
-          uint32_t pk[16];
-          if (full) {
-#pragma unroll
-            for (int i = 0; i < 16; i += 2) {
-              const float p0 = ex2_approx(fmaf(__uint_as_float(r[2 * i]), c, -m_new));
-              const float p1 = ex2_approx(fmaf(__uint_as_float(r[2 * i + 1]), c, -m_new));
-              const float p2 = ex2_approx(fmaf(__uint_as_float(r[2 * i + 2]), c, -m_new));
-              const float p3 = ex2_approx(fmaf(__uint_as_float(r[2 * i + 3]), c, -m_new));
-              l0 += p0; l1 += p1; l2 += p2; l3 += p3;
-              pk[i] = pack_bf16x2_pos(p0, p1);
-              pk[i + 1] = pack_bf16x2_pos(p2, p3);
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const int c0 = cc * 32 + 2 * i;
-              const float p0 = (c0 < valid) ? ex2_approx(fmaf(__uint_as_float(r[2 * i]), c, -m_new)) : 0.f;
-              const float p1 =
-                  (c0 + 1 < valid) ? ex2_approx(fmaf(__uint_as_float(r[2 * i + 1]), c, -m_new)) : 0.f;
-              l0 += p0; l1 += p1;
-              pk[i] = pack_bf16x2_pos(p0, p1);
-            }
-          }
-          // 32 columns = 4 chunks of 16 bytes of the 128-byte row; chunk index XOR-swizzled with row&7
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int chunk = cc * 4 + q;
-            *reinterpret_cast<uint4*>(prow + ((chunk ^ (row & 7)) << 4)) =
-                make_uint4(pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
-          }
-        };
-        chunk32(r0, 0);
-        chunk32(r1, 1);
-        l_tile = (l0 + l1) + (l2 + l3);
-      }
-      l_run = fmaf(l_run, a, l_tile);
-      m_run = m_new;
-      // publish P_j: generic-proxy writes -> async proxy, TMEM reads of S_j ordered before the next MMA
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(smem_u32(&p_full[bsel]));
-      // fold in the previous tile's P.V while the tensor core works on this one
-      if (j > 0) accumulate_o(j - 1, a_prev);
-      a_prev = a;
-    }
-    accumulate_o(T - 1, a_prev);
-
-    if (q0 + row < p.q_len) {
-      const float inv = 1.0f / l_run;
-      if (p.lse != nullptr)
-        p.lse[(static_cast<long long>(b) * gridDim.y + head) * p.q_len + q0 + row] = m_run + log2f(l_run);
-      __nv_bfloat16* op = p.out + static_cast<long long>(b) * p.o_bs +
-                          static_cast<long long>(q0 + row) * p.o_rs + head * DH;
-      uint4* o4 = reinterpret_cast<uint4*>(op);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        uint4 w;
-        w.x = pack_bf16x2(o_acc[8 * i + 0] * inv, o_acc[8 * i + 1] * inv);
-        w.y = pack_bf16x2(o_acc[8 * i + 2] * inv, o_acc[8 * i + 3] * inv);
-        w.z = pack_bf16x2(o_acc[8 * i + 4] * inv, o_acc[8 * i + 5] * inv);
-        w.w = pack_bf16x2(o_acc[8 * i + 6] * inv, o_acc[8 * i + 7] * inv);
-        o4[i] = w;
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
-}
-
-
-// =====================================================================================================
-// Two-tile kernel (the self-attention path): persistent CTAs, 320 threads.
-//   warps 0-3   softmax warpgroup 0: query rows [q0, q0+128) of the work item, thread r <-> TMEM lane r
-//   warps 4-7   softmax warpgroup 1: query rows [q0+128, q0+256)
-//   warp 8      TMA producer: Q pair (double-buffered across work items) + K_j/V_j tiles (128 keys) through a ring
-//   warp 9      tcgen05.mma issuer
-// Per 128-key tile and warpgroup w:  S^w = Q^w K_j^T (SS MMA, fp32 in TMEM) -> the warpgroup reads its 128 scores into
-// registers (S is free again at once, so S^w_{j+1} is computed while the exponentials of tile j are evaluated) ->
-// row max with LAZY rescaling (the running max only moves when it grows by > 2^8; the accumulator in TMEM is rescaled
-// in place by the row's own thread in that rare case) -> P = exp2(s*c - m) packed to bf16 and written back to TENSOR
-// MEMORY (tcgen05.st) -> O^w += P V_j with P as the TMEM A operand and V the MN-major B operand, accumulating in TMEM
-// across all key tiles.  The tensor core is never on the softmax warps' critical path after the first tile; the kernel
-// runs at the rate the two warpgroups evaluate exponentials (MUFU ex2 + an FMA-pipe polynomial for POLY of every 8).
-// TMEM columns: S0 [0,128) S1 [128,256) O0 [256,320) O1 [320,384) P0 [384,448) P1 [448,512).
-// =====================================================================================================
-namespace attn2 {
-constexpr int BQ = 128;      // query rows per warpgroup
-constexpr int BKV = 128;     // keys per tile
-constexpr int DH = 64;
-constexpr int KVS = 4;       // K/V ring depth
-constexpr int Q_BYTES = BQ * DH * 2;          // 16 KB per query tile
-constexpr int KV_BYTES = BKV * DH * 2;        // 16 KB each for K and V
-constexpr int OFF_Q = 0;                               // [2 stages][2 tiles]
-constexpr int OFF_K = OFF_Q + 4 * Q_BYTES;             // [KVS]
-constexpr int OFF_V = OFF_K + KVS * KV_BYTES;          // [KVS]
-constexpr int OFF_BAR = OFF_V + KVS * KV_BYTES;
-constexpr int SMEM_BYTES = OFF_BAR + 256;              // 192.25 KB -> one CTA per SM
-constexpr int TM_S = 0, TM_O = 256, TM_P = 384;
-constexpr int THREADS = 384;     // 2 softmax warpgroups + 1 auxiliary warpgroup (TMA warp, MMA warp, 2 idle)
-constexpr float LAZY = 8.0f;  // log2 units
-}  // namespace attn2
-
-struct Attn2Dev {
-  CUtensorMap tmQ, tmK, tmV;
-  __nv_bfloat16* out;
-  long long o_rs, o_bs;
-  int q_len, kv_len, heads;
-  int q_pairs, num_items;
-  float scale_log2e;
-  float* lse;            // optional (batches, heads, q_len), see AttnDev
-  long long* timeline;   // bring-up aid (ns2_attn_args.debug_timeline): clock64 stamps of CTA 0, else NULL
-};
-
-// timeline layout: [tile g < 64][16 slots]; softmax warp 0 / warp 4 lane 0 and the MMA thread of CTA 0 write
-#define NS2_ATT_STAMP(slot)                                                                          \
-  do {                                                                                               \
-    if (p.timeline != nullptr && blockIdx.x == 0 && g < 64) p.timeline[g * 16 + (slot)] = clock64(); \
-  } while (0)
-
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
-}
-__device__ __forceinline__ unsigned long long pack_f32x2(float lo, float hi) {
-  unsigned long long r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack_f32x2(unsigned long long v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ unsigned long long fma_f32x2(unsigned long long a, unsigned long long b,
-                                                        unsigned long long c) {
-  unsigned long long r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
-__device__ __forceinline__ unsigned long long add_f32x2(unsigned long long a, unsigned long long b) {
-  unsigned long long r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ uint32_t cvt_bf16x2(float lo, float hi) {
-  uint32_t r;
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-  return r;
-}
-
-// 2^x for a pair on the FMA pipe (Cody-Waite: n = round(x), f = x - n in [-0.5, 0.5], degree-3 minimax polynomial for
-// 2^f, exponent patched with integer adds).  Inputs must be >= -125 (callers clamp); relative error 1.1e-4, far below
-// the bf16 rounding (2^-9) applied to the result.
-__device__ __forceinline__ void exp2_poly_x2(unsigned long long x, float& y0, float& y1) {
-  const unsigned long long magic = pack_f32x2(12582912.0f, 12582912.0f);  // 1.5 * 2^23
-  const unsigned long long neg1 = pack_f32x2(-1.0f, -1.0f);
-  const unsigned long long t = add_f32x2(x, magic);          // integer part in the low mantissa bits
-  const unsigned long long n = fma_f32x2(magic, neg1, t);    // n = t - magic
-  const unsigned long long f = fma_f32x2(n, neg1, x);        // f = x - n
-  unsigned long long p = fma_f32x2(pack_f32x2(0.05550410866f, 0.05550410866f), f,
-                                   pack_f32x2(0.24022650696f, 0.24022650696f));
-  p = fma_f32x2(p, f, pack_f32x2(0.69314718056f, 0.69314718056f));
-  p = fma_f32x2(p, f, pack_f32x2(1.0f, 1.0f));
-  float p0, p1, t0, t1;
-  unpack_f32x2(p, p0, p1);
-  unpack_f32x2(t, t0, t1);
-  y0 = __uint_as_float(__float_as_uint(p0) + (__float_as_uint(t0) << 23));
-  y1 = __uint_as_float(__float_as_uint(p1) + (__float_as_uint(t1) << 23));
-}
-
-// POLY: how many of every 8 consecutive exponentials are evaluated on the FMA pipe instead of MUFU (0, 2 or 4)
-// STAGGER: the two warps that share an SM sub-partition (same TMEM lane quarter, one per warpgroup) take turns in the
-//          exponential section, so that one warp's MUFU-bound phase overlaps the other's load / max / store phases
-//          instead of both fighting for the MUFU at the same time and then both leaving it idle
-template <int POLY, bool STAGGER>
-__global__ void __launch_bounds__(attn2::THREADS, 1) attn2_fwd_kernel(const __grid_constant__ Attn2Dev p) {
-  using namespace attn2;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
-  uint64_t* q_full = bars + 0;              // [2]
-  uint64_t* q_empty = bars + 2;             // [2]
-  uint64_t* kv_full = bars + 4;             // [KVS]
-  uint64_t* kv_empty = bars + 4 + KVS;      // [KVS]
-  uint64_t* s_full = bars + 4 + 2 * KVS;    // [2] MMA -> softmax: S^w ready
-  uint64_t* s_free = bars + 6 + 2 * KVS;    // [2] softmax -> MMA: S^w is in registers (4 warp arrivals)
-  uint64_t* p_full = bars + 8 + 2 * KVS;    // [2] softmax -> MMA: P^w is in TMEM (4 warp arrivals)
-  uint64_t* o_full = bars + 10 + 2 * KVS;   // [2] MMA -> softmax: O^w += P^w V complete
-  uint64_t* turn = bars + 12 + 2 * KVS;     // [2][4] warp (w, quarter) has finished its exponential section
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 20 + 2 * KVS);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int T = (p.kv_len + BKV - 1) / BKV;
-  const int my_items = (p.num_items - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) /
-                       static_cast<int>(gridDim.x);
-
-  if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) {
-    printf("ns2 attn2: dynamic shared memory is not 1024-byte aligned\n");
-    __trap();
-  }
-  if (warp == 8 && lane == 0) {
-    tma_prefetch_desc(&p.tmQ);
-    tma_prefetch_desc(&p.tmK);
-    tma_prefetch_desc(&p.tmV);
-  }
-  if (warp == 9 && lane == 0) {
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(&q_full[i]), 1);
-      mbar_init(smem_u32(&q_empty[i]), 1);
-      mbar_init(smem_u32(&s_full[i]), 1);
-      mbar_init(smem_u32(&s_free[i]), 4);
-      mbar_init(smem_u32(&p_full[i]), 4);
-      mbar_init(smem_u32(&o_full[i]), 1);
-    }
-    for (int i = 0; i < KVS; ++i) {
-      mbar_init(smem_u32(&kv_full[i]), 1);
-      mbar_init(smem_u32(&kv_empty[i]), 1);
-    }
-    for (int i = 0; i < 8; ++i) mbar_init(smem_u32(&turn[i]), 1);
-    fence_barrier_init();
-  }
-  if (warp == 8) tmem_alloc(smem_u32(tmem_holder), 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
-
-  auto decode = [&](int it, int& b, int& head, int& q0) {
-    const int item = static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x);
-    const int qp = item % p.q_pairs;
-    const int bh = item / p.q_pairs;
-    head = bh % p.heads;
-    b = bh / p.heads;
-    q0 = qp * 2 * BQ;
-  };
-
-  // register budget (setmaxnreg): the softmax warpgroups keep a whole 128-score row and its packed probabilities in
-  // registers; the auxiliary warpgroup gives its share up
-  if (warp >= 8) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-    // Both service warps run their loops CONVERGED (all 32 lanes, warp-uniform operands) and elect one lane per
-    // asynchronous instruction: tcgen05.mma / TMA take their operands from uniform registers, and when they are issued
-    // from a single-lane divergent region the compiler wraps each one in an ELECT / R2UR / BRA.U.ANY loop that costs
-    // ~117 cycles per instruction (profiles/r02_ubench_mma.txt) — more than the MMA itself.
-    if (warp == 8) {
-      // ================================ TMA producer ================================
-      uint32_t g = 0;  // global key-tile counter of this CTA
-      for (int it = 0; it < my_items; ++it) {
-        int b, head, q0;
-        decode(it, b, head, q0);
-        const int qs = it & 1;
-        mbar_wait(smem_u32(&q_empty[qs]), ((it >> 1) & 1) ^ 1);
-        if (elect_one()) {
-          const uint32_t qb = smem_u32(&q_full[qs]);
-          mbar_arrive_expect_tx(qb, 2 * Q_BYTES);
-          tma_load_3d(smem_u32(smem + OFF_Q + (qs * 2 + 0) * Q_BYTES), &p.tmQ, qb, head * DH, q0, b);
-          tma_load_3d(smem_u32(smem + OFF_Q + (qs * 2 + 1) * Q_BYTES), &p.tmQ, qb, head * DH, q0 + BQ, b);
-        }
-        __syncwarp();
-        for (int j = 0; j < T; ++j, ++g) {
-          const int st = g % KVS;
-          mbar_wait(smem_u32(&kv_empty[st]), ((g / KVS) & 1) ^ 1);
-          if (elect_one()) {
-            const uint32_t fb = smem_u32(&kv_full[st]);
-            mbar_arrive_expect_tx(fb, 2 * KV_BYTES);
-            tma_load_3d(smem_u32(smem + OFF_K + st * KV_BYTES), &p.tmK, fb, head * DH, j * BKV, b);
-            tma_load_3d(smem_u32(smem + OFF_V + st * KV_BYTES), &p.tmV, fb, head * DH, j * BKV, b);
-          }
-          __syncwarp();
-        }
-      }
-    } else if (warp == 9) {
-      // ================================ MMA issuer ==================================
-      constexpr uint32_t idesc_s = umma_idesc_f16(BQ, BKV, 1, 0, 0);
-      constexpr uint32_t idesc_o = umma_idesc_f16(BQ, DH, 1, 0, /*V is MN-major*/ 1);
-      const int total = my_items * T;
-      // S for global tile gs (item gs / T, key tile gs % T), both warpgroups
-      auto issue_s = [&](int gs) {
-        const int g = gs;   // for NS2_ATT_STAMP
-        const int it = gs / T, j = gs - it * T;
-        const int qs = it & 1;
-        if (j == 0) mbar_wait(smem_u32(&q_full[qs]), (it >> 1) & 1);
-        const int st = gs % KVS;
-        mbar_wait(smem_u32(&kv_full[st]), (gs / KVS) & 1);
-        tc_fence_after();
-        const uint64_t dk = umma_desc_sw128(smem_u32(smem + OFF_K + st * KV_BYTES), 16, 1024);
-#pragma unroll
-        for (int w = 0; w < 2; ++w) {
-          if (gs > 0) {  // the warpgroup has pulled S^w of the previous tile into registers
-            mbar_wait(smem_u32(&s_free[w]), (gs - 1) & 1);
-            tc_fence_after();
-          }
-          const uint64_t dq = umma_desc_sw128(smem_u32(smem + OFF_Q + (qs * 2 + w) * Q_BYTES), 16, 1024);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < DH / 16; ++k)
-              tc_mma_f16(tmem_base + TM_S + w * BKV, dq + 2 * k, dk + 2 * k, idesc_s, k > 0);
-            tc_commit(smem_u32(&s_full[w]));
-            NS2_ATT_STAMP(12 + w);
-          }
-          __syncwarp();
-        }
-        if (j == T - 1) {
-          if (elect_one()) tc_commit(smem_u32(&q_empty[qs]));  // every S of this item has been issued
-          __syncwarp();
-        }
-      };
-      if (total > 0) issue_s(0);
-      for (int g = 0; g < total; ++g) {
-        if (g + 1 < total) issue_s(g + 1);
-        const int j = g % T;
-        const int st = g % KVS;
         const uint32_t vbase = smem_u32(smem + OFF_V + st * KV_BYTES);
+        wgmma_fence();
 #pragma unroll
-        for (int w = 0; w < 2; ++w) {
-          mbar_wait(smem_u32(&p_full[w]), g & 1);
-          tc_fence_after();
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < BKV / 16; ++k) {
-              // A = P^w from TMEM: 16 keys = 8 packed columns per step; B = V: 16 keys = 2048 bytes per step
-              const uint64_t dv = umma_desc_sw128(vbase + k * 2048, 1024, 1024);
-              tc_mma_f16_ts(tmem_base + TM_O + w * DH, tmem_base + TM_P + w * (BKV / 2) + k * 8, dv, idesc_o,
-                            (j > 0) | (k > 0));
-            }
-            tc_commit(smem_u32(&o_full[w]));
-            NS2_ATT_STAMP(14 + w);
-          }
-          __syncwarp();
-        }
-        if (elect_one()) tc_commit(smem_u32(&kv_empty[st]));
-        __syncwarp();
+        for (int k = 0; k < BKV / 16; ++k)   // B = V: MN-major (64 dh contiguous per key row); 16 keys = 2048 bytes
+          wgmma_bf16_rs_n64<1>(o_acc, pa[k], gmma_desc_sw128(vbase + k * 2048, 1024, 1024), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_hold(o_acc);
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(&kv_empty[st]));
     }
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 208;");
-    // ================================ softmax warpgroups ==========================
-    const int w = warp >> 2;                      // warpgroup = query tile
-    const int qw = warp & 3;                      // TMEM lane quarter
-    const int row = qw * 32 + lane;               // row inside the 128-row tile
-    const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(qw * 32) << 16);
-    const uint32_t s_addr = lane_addr + TM_S + w * BKV;
-    const uint32_t o_addr = lane_addr + TM_O + w * DH;
-    const uint32_t p_addr = lane_addr + TM_P + w * (BKV / 2);
-    const float c = p.scale_log2e;
-    const unsigned long long c2 = pack_f32x2(c, c);
-    uint32_t g = 0;
-    for (int it = 0; it < my_items; ++it) {
-      int b, head, q0;
-      decode(it, b, head, q0);
-      float m_run = -INFINITY, l_run = 0.f;
-      for (int j = 0; j < T; ++j, ++g) {
-        const bool stamp = (qw == 0 && lane == 0);
-        if (stamp) NS2_ATT_STAMP(w * 6 + 0);
-        mbar_wait(smem_u32(&s_full[w]), g & 1);
-        tc_fence_after();
-        if (stamp) NS2_ATT_STAMP(w * 6 + 1);
-        float s[BKV];
-        {
-          uint32_t r0[32], r1[32], r2[32], r3[32];
-          tmem_ld32(s_addr, r0);
-          tmem_ld32(s_addr + 32, r1);
-          tmem_ld32(s_addr + 64, r2);
-          tmem_ld32(s_addr + 96, r3);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            s[i] = __uint_as_float(r0[i]);
-            s[32 + i] = __uint_as_float(r1[i]);
-            s[64 + i] = __uint_as_float(r2[i]);
-            s[96 + i] = __uint_as_float(r3[i]);
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&s_free[w]));   // S^w may be overwritten by the next tile's MMA
-        if (stamp) NS2_ATT_STAMP(w * 6 + 2);
-        const int valid = p.kv_len - j * BKV;
-        if (valid < BKV) {  // padding keys of the last tile (TMA zero-filled): exclude them
-#pragma unroll
-          for (int i = 0; i < BKV; ++i)
-            if (i >= valid) s[i] = -INFINITY;
-        }
-        float m0 = s[0], m1 = s[1], m2 = s[2], m3 = s[3];
-#pragma unroll
-        for (int i = 4; i < BKV; i += 8) {
-          m0 = fmax3(m0, s[i], s[i + 1]);
-          m1 = fmax3(m1, s[i + 2], s[i + 3]);
-          if (i + 4 < BKV) {
-            m2 = fmax3(m2, s[i + 4], s[i + 5]);
-            m3 = fmax3(m3, s[i + 6], s[i + 7]);
-          }
-        }
-        const float m_tile = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3)) * c;
-        // lazy rescaling: keep the stale maximum unless the true one exceeds it by more than 2^LAZY
-        const bool grow = m_tile > m_run + LAZY;
-        if (__any_sync(0xffffffffu, grow && j > 0)) {
-          // rare: rescale this row's accumulator in TMEM (needs the previous P.V to have completed)
-          mbar_wait(smem_u32(&o_full[w]), (g - 1) & 1);
-          tc_fence_after();
-          const float a = grow ? exp2f(m_run - m_tile) : 1.0f;
-#pragma unroll 1
-          for (int cc = 0; cc < DH; cc += 16) {   // 16 columns at a time: the 128 scores stay live in registers
-            uint32_t o[16];
-            tmem_ld16(o_addr + cc, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * a);
-            tmem_st16(o_addr + cc, o);
-          }
-          tmem_st_wait();
-          if (grow) {
-            l_run *= a;
-            m_run = m_tile;
-          }
-        } else if (grow) {  // first tile of the item: nothing accumulated yet
-          m_run = m_tile;
-          l_run = 0.f;
-        }
-        if constexpr (STAGGER) {
-          // strict alternation per lane quarter: warpgroup 0's tile g, warpgroup 1's tile g, warpgroup 0's tile g+1 ...
-          if (w == 0) {
-            if (g > 0) mbar_wait(smem_u32(&turn[4 + qw]), (g - 1) & 1);
-          } else {
-            mbar_wait(smem_u32(&turn[qw]), g & 1);
-          }
-        }
-        if (stamp) NS2_ATT_STAMP(w * 6 + 3);
-        // the P buffer is read by the previous tile's P.V until o_full flips (long done by now)
-        if (j > 0) {
-          mbar_wait(smem_u32(&o_full[w]), (g - 1) & 1);
-          tc_fence_after();
-        }
-        if (stamp) NS2_ATT_STAMP(w * 6 + 4);
-        // P = exp2(s*c - m) -> bf16 pairs; row sum in fp32
-        const unsigned long long nm2 = pack_f32x2(-m_run, -m_run);
-        unsigned long long lsum0 = 0ull, lsum1 = 0ull;  // two packed (0.f, 0.f) accumulators
-        uint32_t pk_lo[32], pk_hi[32];   // packed bf16 pairs of keys [0,64) and [64,128)
-#pragma unroll
-        for (int i = 0; i < BKV; i += 8) {
-          float e[8];
-#pragma unroll
-          for (int q = 0; q < 8; q += 2) {
-            unsigned long long x = fma_f32x2(pack_f32x2(s[i + q], s[i + q + 1]), c2, nm2);
-            if (q < POLY) {
-              float x0, x1;
-              unpack_f32x2(x, x0, x1);
-              x = pack_f32x2(fmaxf(x0, -125.0f), fmaxf(x1, -125.0f));
-              exp2_poly_x2(x, e[q], e[q + 1]);
-            } else {
-              float x0, x1;
-              unpack_f32x2(x, x0, x1);
-              e[q] = ex2_approx(x0);
-              e[q + 1] = ex2_approx(x1);
-            }
-          }
-          lsum0 = add_f32x2(lsum0, pack_f32x2(e[0], e[1]));
-          lsum1 = add_f32x2(lsum1, pack_f32x2(e[2], e[3]));
-          lsum0 = add_f32x2(lsum0, pack_f32x2(e[4], e[5]));
-          lsum1 = add_f32x2(lsum1, pack_f32x2(e[6], e[7]));
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const uint32_t v = cvt_bf16x2(e[2 * q], e[2 * q + 1]);
-            if (i < BKV / 2) pk_lo[i / 2 + q] = v;
-            else pk_hi[(i - BKV / 2) / 2 + q] = v;
-          }
-          if (i == BKV / 2 - 8) tmem_st32(p_addr, pk_lo);   // first half of P goes out while the second is computed
-        }
-        if constexpr (STAGGER) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(&turn[w * 4 + qw]));
-        }
-        {
-          float a0, a1, b0, b1;
-          unpack_f32x2(lsum0, a0, a1);
-          unpack_f32x2(lsum1, b0, b1);
-          l_run += (a0 + a1) + (b0 + b1);
-        }
-        tmem_st32(p_addr + 32, pk_hi);
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&p_full[w]));
-        if (stamp) NS2_ATT_STAMP(w * 6 + 5);
-      }
-      // ---- epilogue of the work item: O / l -> bf16 -> global ----
-      mbar_wait(smem_u32(&o_full[w]), (g - 1) & 1);
-      tc_fence_after();
-      uint32_t o0[32], o1[32];
-      tmem_ld32(o_addr, o0);
-      tmem_ld32(o_addr + 32, o1);
-      tmem_ld_wait();
-      const int qrow = q0 + w * BQ + row;
-      if (qrow < p.q_len) {
-        const float inv = 1.0f / l_run;
-        if (p.lse != nullptr)
-          p.lse[(static_cast<long long>(b) * p.heads + head) * p.q_len + qrow] = m_run + log2f(l_run);
-        __nv_bfloat16* op = p.out + static_cast<long long>(b) * p.o_bs + static_cast<long long>(qrow) * p.o_rs +
-                            head * DH;
-        uint4* o4 = reinterpret_cast<uint4*>(op);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          uint4 v;
-          v.x = pack_bf16x2(__uint_as_float(o0[8 * i + 0]) * inv, __uint_as_float(o0[8 * i + 1]) * inv);
-          v.y = pack_bf16x2(__uint_as_float(o0[8 * i + 2]) * inv, __uint_as_float(o0[8 * i + 3]) * inv);
-          v.z = pack_bf16x2(__uint_as_float(o0[8 * i + 4]) * inv, __uint_as_float(o0[8 * i + 5]) * inv);
-          v.w = pack_bf16x2(__uint_as_float(o0[8 * i + 6]) * inv, __uint_as_float(o0[8 * i + 7]) * inv);
-          o4[i] = v;
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          uint4 v;
-          v.x = pack_bf16x2(__uint_as_float(o1[8 * i + 0]) * inv, __uint_as_float(o1[8 * i + 1]) * inv);
-          v.y = pack_bf16x2(__uint_as_float(o1[8 * i + 2]) * inv, __uint_as_float(o1[8 * i + 3]) * inv);
-          v.z = pack_bf16x2(__uint_as_float(o1[8 * i + 4]) * inv, __uint_as_float(o1[8 * i + 5]) * inv);
-          v.w = pack_bf16x2(__uint_as_float(o1[8 * i + 6]) * inv, __uint_as_float(o1[8 * i + 7]) * inv);
-          o4[4 + i] = v;
-        }
-      }
-    }
-  }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 8) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      float l = l_run[i];
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      const int qrow = q0 + r0 + 8 * i;
+      if (qrow < p.q_len) {
+        const float inv = 1.0f / l;
+        if (p.lse != nullptr && (lane & 3) == 0)
+          p.lse[(static_cast<long long>(b) * gridDim.y + head) * p.q_len + qrow] = m_run[i] + log2f(l);
+        __nv_bfloat16* op = p.out + static_cast<long long>(b) * p.o_bs + static_cast<long long>(qrow) * p.o_rs +
+                            head * DH + c2;
+#pragma unroll
+        for (int jj = 0; jj < DH / 8; ++jj)
+          *reinterpret_cast<uint32_t*>(op + 8 * jj) =
+              pack_bf16x2(o_acc[4 * jj + 2 * i] * inv, o_acc[4 * jj + 2 * i + 1] * inv);
+      }
+    }
   }
 }
 
@@ -777,6 +209,9 @@ extern "C" int ns2_attn_fwd(const ns2_attn_args* a, ns2_stream_t stream_) {
   NS2_REQUIRE(a->o_row_stride % 8 == 0 && a->o_batch_stride % 8 == 0 &&
                   (reinterpret_cast<uintptr_t>(a->out) & 15) == 0,
               "attn_fwd: out must be 16-byte aligned with strides multiple of 8");
+  // one kernel for every problem shape; the selector is still validated so callers get the same errors as before
+  NS2_REQUIRE(a->kernel >= NS2_ATTN_AUTO && a->kernel <= NS2_ATTN_TWO_TILE_LOCKSTEP,
+              "attn_fwd: unknown kernel selector %d", a->kernel);
   AttnDev dev;
   memset(&dev, 0, sizeof(dev));
   const uint32_t box[3] = {64, attn::BQ, 1};
@@ -803,63 +238,9 @@ extern "C" int ns2_attn_fwd(const ns2_attn_args* a, ns2_stream_t stream_) {
   dev.kv_len = a->kv_len;
   dev.scale_log2e = a->scale * 1.4426950408889634f;
   dev.lse = a->lse;
-
-  // kernel choice: the two-tile kernel (256 queries x 128-key tiles per CTA, P and O in TMEM) for self-attention sized
-  // problems; the single-tile kernel (128 queries x 64-key tiles) for short key sequences (cross attention over the 32
-  // perceiver latents) and short query sequences (the perceiver itself).  args->kernel overrides (tests, tuning).
-  int kernel = a->kernel;
-  if (kernel == NS2_ATTN_AUTO) kernel = (a->kv_len > 64 && a->q_len > 128) ? NS2_ATTN_TWO_TILE : NS2_ATTN_ONE_TILE;
-  NS2_REQUIRE(kernel >= NS2_ATTN_ONE_TILE && kernel <= NS2_ATTN_TWO_TILE_LOCKSTEP,
-              "attn_fwd: unknown kernel selector %d", a->kernel);
-  if (kernel == NS2_ATTN_ONE_TILE) {
-    NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel, attn::SMEM_BYTES));
-    dim3 grid((a->q_len + attn::BQ - 1) / attn::BQ, a->heads, a->batches);
-    attn_fwd_kernel<<<grid, 192, attn::SMEM_BYTES, stream>>>(dev);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    NS2_CUDA_CHECK(cudaGetLastError());
-    return kOk;
-  }
-  Attn2Dev d2;
-  memset(&d2, 0, sizeof(d2));
-  {
-    const uint32_t box2[3] = {64, attn2::BQ, 1};   // Q tiles and K/V tiles are all 128 rows x 64 columns
-    const uint64_t qdims[3] = {(uint64_t)a->heads * 64, (uint64_t)a->q_len, (uint64_t)a->batches};
-    const uint64_t qstr[3] = {2, (uint64_t)a->q_row_stride * 2, (uint64_t)a->q_batch_stride * 2};
-    int rc = make_tmap_16bit(&d2.tmQ, a->q, 3, qdims, qstr, box2);
-    if (rc != kOk) return rc;
-    const uint64_t kdims[3] = {(uint64_t)a->heads * 64, (uint64_t)a->kv_len, (uint64_t)a->batches};
-    const uint64_t kstr[3] = {2, (uint64_t)a->k_row_stride * 2, (uint64_t)a->k_batch_stride * 2};
-    const uint64_t vstr[3] = {2, (uint64_t)a->v_row_stride * 2, (uint64_t)a->v_batch_stride * 2};
-    rc = make_tmap_16bit(&d2.tmK, a->k, 3, kdims, kstr, box2);
-    if (rc != kOk) return rc;
-    rc = make_tmap_16bit(&d2.tmV, a->v, 3, kdims, vstr, box2);
-    if (rc != kOk) return rc;
-  }
-  d2.out = reinterpret_cast<__nv_bfloat16*>(a->out);
-  d2.o_rs = a->o_row_stride;
-  d2.o_bs = a->o_batch_stride;
-  d2.q_len = a->q_len;
-  d2.kv_len = a->kv_len;
-  d2.heads = a->heads;
-  d2.q_pairs = (a->q_len + 2 * attn2::BQ - 1) / (2 * attn2::BQ);
-  d2.num_items = d2.q_pairs * a->heads * a->batches;
-  d2.scale_log2e = a->scale * 1.4426950408889634f;
-  d2.timeline = reinterpret_cast<long long*>(a->debug_timeline);
-  d2.lse = a->lse;
-  const int grid2 = d2.num_items < num_sms() ? d2.num_items : num_sms();
-  auto launch2 = [&](auto kern) -> int {
-    NS2_CUDA_CHECK(set_max_smem_once(kern, attn2::SMEM_BYTES));
-    kern<<<grid2, attn2::THREADS, attn2::SMEM_BYTES, stream>>>(d2);
-    return kOk;
-  };
-  int rc2;
-  switch (kernel) {
-    case NS2_ATTN_TWO_TILE: rc2 = launch2(attn2_fwd_kernel<0, true>); break;
-    case NS2_ATTN_TWO_TILE_POLY2: rc2 = launch2(attn2_fwd_kernel<2, true>); break;
-    case NS2_ATTN_TWO_TILE_POLY4: rc2 = launch2(attn2_fwd_kernel<4, true>); break;
-    default: rc2 = launch2(attn2_fwd_kernel<0, false>); break;
-  }
-  if (rc2 != kOk) return rc2;
+  NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel, attn::SMEM_BYTES));
+  dim3 grid((a->q_len + attn::BQ - 1) / attn::BQ, a->heads, a->batches);
+  attn_fwd_kernel<<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   NS2_CUDA_CHECK(cudaGetLastError());
   return kOk;

@@ -1,4 +1,4 @@
-// Flash-attention backward on tcgen05 for sm_100a (non-causal, unmasked, dim_head = 64) — the backward of
+// Flash-attention backward on wgmma for sm_90a (non-causal, unmasked, dim_head = 64) — the backward of
 // Attend.forward / F.scaled_dot_product_attention (attend.py:77-155) that autograd runs for the reference's
 // loss.backward() (README.md:63, ns2.py:1886).
 //
@@ -6,16 +6,15 @@
 //   dV = P^T dO               dP = dO V^T               D = rowsum(dO * O)   (ns2_attn_bwd_delta)
 //   dS = P * (dP - D) * scale dQ = dS K                 dK = dS^T Q
 //
-// One CTA per (batch, head, 128-key tile j); it walks over the 128-query tiles i.  192 threads:
-//   warps 0-3  thread r <-> query row r of the current tile: S and dP are read from TMEM in 64-column halves, P and dS
-//              are written (bf16) to 128B-swizzled shared memory; later the same warps drain dQ_i (TMEM -> smem -> TMA
-//              fp32 reduce-add into the dQ accumulator, because every key tile contributes to every query row)
-//   warp 4     TMA producer: K_j, V_j once; Q_i, dO_i through a 2-stage ring
-//   warp 5     tcgen05.mma issuer (converged, elect_one)
-// All five products run on the tensor cores; the operands whose contraction index is the row index of the stored
-// tile (P, dS for dV/dK; dO, Q, K as B operands) are consumed as MN-major operands, so nothing is ever transposed.
-// dK_j / dV_j accumulate in TMEM over all query tiles and are stored once at the end.
-// TMEM columns: S [0,128) dP [128,256) dV [256,320) dK [320,384) dQ [384,448).
+// One CTA per (batch, head, 128-key tile j); it walks over the 64-query tiles i.  384 threads:
+//   warpgroup 0     TMA producer (warp 0): K_j, V_j once; Q_i, dO_i through a 2-stage ring
+//   warpgroups 1-2  warpgroup w owns keys [64 (w-1), 64 w) of the tile.  S^T = K Q_i^T and dP^T = V dO_i^T come out of
+//                   wgmma with the keys as accumulator rows, so P^T and dS^T are formed in registers and feed
+//                   dV += P^T dO_i and dK += dS^T Q_i directly as register A operands (dO_i, Q_i are MN-major B
+//                   operands: nothing is ever transposed).  dS^T also goes to 128B-swizzled shared memory, from where
+//                   dQ_i (partial over this warpgroup's keys) = dS K is computed with dS as the MN-major A operand and
+//                   added into the fp32 dQ accumulator with global reductions (every key tile contributes to every
+//                   query row).  dK_j / dV_j stay in registers over all query tiles and are stored once at the end.
 #include "ptx.cuh"
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
@@ -27,24 +26,23 @@ namespace ns2 {
 extern std::atomic<long long> g_launches;
 
 namespace ab {
-constexpr int BQ = 128, BKV = 128, DH = 64;
-constexpr int T16 = BQ * DH * 2;            // 16 KB: a [128 rows][64 x bf16] tile
-constexpr int ATOM = BQ * 128;              // 16 KB: a [128 rows][128 B] swizzle atom of P / dS (64 keys wide)
-constexpr int OFF_K = 0, OFF_V = T16;
-constexpr int OFF_Q = 2 * T16;              // [2 stages]
-constexpr int OFF_DO = 4 * T16;             // [2 stages]
-constexpr int OFF_P = 6 * T16;              // 2 atoms
-constexpr int OFF_DS = OFF_P + 2 * ATOM;    // 2 atoms
-constexpr int OFF_STG = OFF_DS + 2 * ATOM;  // dQ staging: 4 warps x 2 boxes x 4 KB
-constexpr int OFF_BAR = OFF_STG + 4 * 2 * 4096;
-constexpr int SMEM_BYTES = OFF_BAR + 256;   // 192.25 KB
-constexpr int TM_S = 0, TM_DP = 128, TM_DV = 256, TM_DK = 320, TM_DQ = 384;
+constexpr int BQ = 64, BKV = 128, DH = 64;
+constexpr int KV_BYTES = BKV * DH * 2;      // 16 KB: a [128 keys][64 x bf16] tile
+constexpr int QT_BYTES = BQ * DH * 2;       // 8 KB: a [64 queries][64 x bf16] tile
+constexpr int OFF_K = 0, OFF_V = KV_BYTES;
+constexpr int OFF_Q = 2 * KV_BYTES;                 // [2 stages]
+constexpr int OFF_DO = OFF_Q + 2 * QT_BYTES;        // [2 stages]
+constexpr int OFF_DS = OFF_DO + 2 * QT_BYTES;       // dS^T: [128 keys][64 queries] bf16, 128B-swizzled rows
+constexpr int OFF_BAR = OFF_DS + BKV * BQ * 2;
+constexpr int SMEM_BYTES = OFF_BAR + 256;           // 80.25 KB
+constexpr int THREADS = 384;
 }  // namespace ab
 
 struct AttnBwdDev {
-  CUtensorMap tmQ, tmK, tmV, tmDO, tmDQ;   // tmDQ: fp32 dQ accumulator (inner, q_len, batch), box {32, 32, 1}
+  CUtensorMap tmQ, tmK, tmV, tmDO;
   const float* lse;     // (batches, heads, q_len): log2-domain log-sum-exp of the scaled scores
   const float* delta;   // (batches, heads, q_len): rowsum(dO * O)
+  float* dq;            // (batches, q_len, heads * 64) fp32 accumulator
   __nv_bfloat16* dk;
   __nv_bfloat16* dv;
   long long dk_rs, dk_bs, dv_rs, dv_bs;
@@ -58,248 +56,173 @@ __device__ __forceinline__ float ab_ex2(float x) {
   return y;
 }
 
-__global__ void __launch_bounds__(192, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdDev p) {
+__global__ void __launch_bounds__(ab::THREADS, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdDev p) {
   using namespace ab;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* kv_full = bars + 0;
   uint64_t* q_full = bars + 1;     // [2]
-  uint64_t* q_empty = bars + 3;    // [2]
-  uint64_t* sdp_full = bars + 5;   // MMA -> softmax: S_i and dP_i are in TMEM
-  uint64_t* pds_full = bars + 6;   // softmax -> MMA: P_i, dS_i are in shared memory (4 warp arrivals)
-  uint64_t* dq_full = bars + 7;    // MMA -> softmax: dQ_i complete (also: P / dS buffers and the Q/dO stage are free)
-  uint64_t* dq_free = bars + 8;    // softmax -> MMA: dQ_i has been drained from TMEM (4 warp arrivals)
-  uint64_t* fin_full = bars + 9;   // MMA -> softmax: dK_j, dV_j complete
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 10);
+  uint64_t* q_empty = bars + 3;    // [2] one arrive per consumer warp
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int j = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
   const int TQ = (p.q_len + BQ - 1) / BQ;
 
-  if (warp == 4 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmQ);
     tma_prefetch_desc(&p.tmK);
     tma_prefetch_desc(&p.tmV);
     tma_prefetch_desc(&p.tmDO);
-    tma_prefetch_desc(&p.tmDQ);
-  }
-  if (warp == 5 && lane == 0) {
     mbar_init(smem_u32(kv_full), 1);
     for (int i = 0; i < 2; ++i) {
       mbar_init(smem_u32(&q_full[i]), 1);
-      mbar_init(smem_u32(&q_empty[i]), 1);
+      mbar_init(smem_u32(&q_empty[i]), 8);
     }
-    mbar_init(smem_u32(sdp_full), 1);
-    mbar_init(smem_u32(pds_full), 4);
-    mbar_init(smem_u32(dq_full), 1);
-    mbar_init(smem_u32(dq_free), 4);
-    mbar_init(smem_u32(fin_full), 1);
     fence_barrier_init();
   }
-  if (warp == 4) tmem_alloc(smem_u32(tmem_holder), 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
 
-  if (warp == 4) {
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     // ================================ TMA producer ================================
-    if (elect_one()) {
-      mbar_arrive_expect_tx(smem_u32(kv_full), 2 * T16);
-      tma_load_3d(smem_u32(smem + OFF_K), &p.tmK, smem_u32(kv_full), head * DH, j * BKV, b);
-      tma_load_3d(smem_u32(smem + OFF_V), &p.tmV, smem_u32(kv_full), head * DH, j * BKV, b);
-    }
-    __syncwarp();
-    for (int i = 0; i < TQ; ++i) {
-      const int st = i & 1;
-      mbar_wait(smem_u32(&q_empty[st]), ((i >> 1) & 1) ^ 1);
+    if (warp == 0) {
       if (elect_one()) {
-        const uint32_t fb = smem_u32(&q_full[st]);
-        mbar_arrive_expect_tx(fb, 2 * T16);
-        tma_load_3d(smem_u32(smem + OFF_Q + st * T16), &p.tmQ, fb, head * DH, i * BQ, b);
-        tma_load_3d(smem_u32(smem + OFF_DO + st * T16), &p.tmDO, fb, head * DH, i * BQ, b);
+        mbar_arrive_expect_tx(smem_u32(kv_full), 2 * KV_BYTES);
+        tma_load_3d(smem_u32(smem + OFF_K), &p.tmK, smem_u32(kv_full), head * DH, j * BKV, b);
+        tma_load_3d(smem_u32(smem + OFF_V), &p.tmV, smem_u32(kv_full), head * DH, j * BKV, b);
       }
       __syncwarp();
-    }
-  } else if (warp == 5) {
-    // ================================ MMA issuer ==================================
-    constexpr uint32_t id_s = umma_idesc_f16(BQ, BKV, 1, 0, 0);    // S = Q K^T, dP = dO V^T (both K-major)
-    constexpr uint32_t id_t = umma_idesc_f16(BKV, DH, 1, 1, 1);    // dV = P^T dO, dK = dS^T Q (both MN-major)
-    constexpr uint32_t id_q = umma_idesc_f16(BQ, DH, 1, 0, 1);     // dQ = dS K (A K-major, B MN-major)
-    const uint32_t k_s = smem_u32(smem + OFF_K), v_s = smem_u32(smem + OFF_V);
-    const uint32_t p_s = smem_u32(smem + OFF_P), ds_s = smem_u32(smem + OFF_DS);
-    auto issue_sdp = [&](int i) {
-      const int st = i & 1;
-      mbar_wait(smem_u32(&q_full[st]), (i >> 1) & 1);
-      tc_fence_after();
-      const uint32_t q_s = smem_u32(smem + OFF_Q + st * T16), do_s = smem_u32(smem + OFF_DO + st * T16);
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < DH / 16; ++k)
-          tc_mma_f16(tmem_base + TM_S, umma_desc_sw128(q_s, 16, 1024) + 2 * k, umma_desc_sw128(k_s, 16, 1024) + 2 * k,
-                     id_s, k > 0);
-#pragma unroll
-        for (int k = 0; k < DH / 16; ++k)
-          tc_mma_f16(tmem_base + TM_DP, umma_desc_sw128(do_s, 16, 1024) + 2 * k,
-                     umma_desc_sw128(v_s, 16, 1024) + 2 * k, id_s, k > 0);
-        tc_commit(smem_u32(sdp_full));
+      for (int i = 0; i < TQ; ++i) {
+        const int st = i & 1;
+        mbar_wait(smem_u32(&q_empty[st]), ((i >> 1) & 1) ^ 1);
+        if (elect_one()) {
+          const uint32_t fb = smem_u32(&q_full[st]);
+          mbar_arrive_expect_tx(fb, 2 * QT_BYTES);
+          tma_load_3d(smem_u32(smem + OFF_Q + st * QT_BYTES), &p.tmQ, fb, head * DH, i * BQ, b);
+          tma_load_3d(smem_u32(smem + OFF_DO + st * QT_BYTES), &p.tmDO, fb, head * DH, i * BQ, b);
+        }
+        __syncwarp();
       }
-      __syncwarp();
-    };
-    mbar_wait(smem_u32(kv_full), 0);
-    tc_fence_after();
-    issue_sdp(0);
-    for (int i = 0; i < TQ; ++i) {
-      const int st = i & 1;
-      const uint32_t q_s = smem_u32(smem + OFF_Q + st * T16), do_s = smem_u32(smem + OFF_DO + st * T16);
-      mbar_wait(smem_u32(pds_full), i & 1);
-      if (i > 0) mbar_wait(smem_u32(dq_free), (i - 1) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < BQ / 16; ++k) {   // contraction over the 128 query rows, 16 per step = 2048 bytes
-          tc_mma_f16(tmem_base + TM_DV, umma_desc_sw128(p_s + k * 2048, ATOM, 1024),
-                     umma_desc_sw128(do_s + k * 2048, 1024, 1024), id_t, (i > 0) | (k > 0));
-        }
-#pragma unroll
-        for (int k = 0; k < BQ / 16; ++k) {
-          tc_mma_f16(tmem_base + TM_DK, umma_desc_sw128(ds_s + k * 2048, ATOM, 1024),
-                     umma_desc_sw128(q_s + k * 2048, 1024, 1024), id_t, (i > 0) | (k > 0));
-        }
-#pragma unroll
-        for (int k = 0; k < BKV / 16; ++k) {  // contraction over the 128 keys: atom k/4, 32 bytes per step inside it
-          tc_mma_f16(tmem_base + TM_DQ, umma_desc_sw128(ds_s + (k >> 2) * ATOM + (k & 3) * 32, 16, 1024),
-                     umma_desc_sw128(k_s + k * 2048, 1024, 1024), id_q, k > 0);
-        }
-        tc_commit(smem_u32(dq_full));
-        tc_commit(smem_u32(&q_empty[st]));
-        if (i == TQ - 1) tc_commit(smem_u32(fin_full));
-      }
-      __syncwarp();
-      if (i + 1 < TQ) issue_sdp(i + 1);   // S / dP of the next tile queue up behind this tile's products
     }
   } else {
-    // ================================ softmax / gradient warps =====================
-    const int row = warp * 32 + lane;
-    const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    // ================================ gradient warpgroups ===============================
+    const int w = (warp >> 2) - 1;
+    const int kr0 = 64 * w + 16 * (warp & 3) + (lane >> 2);   // this thread's key rows (in the tile): kr0, kr0 + 8
+    const int c2 = 2 * (lane & 3);
     const int valid = p.kv_len - j * BKV;   // keys of this tile that exist
-    const uint32_t stg = smem_u32(smem + OFF_STG + warp * 2 * 4096);
-    uint32_t stg_count = 0;
+    const uint32_t k_s = smem_u32(smem + OFF_K) + w * (64 * 128), v_s = smem_u32(smem + OFF_V) + w * (64 * 128);
+    const uint32_t ds_s = smem_u32(smem + OFF_DS) + w * (64 * 128);
+    uint8_t* ds_rows = smem + OFF_DS;
+    const long long inner = static_cast<long long>(p.heads) * DH;
+    float dv_acc[DH / 2], dk_acc[DH / 2];
+#pragma unroll
+    for (int i = 0; i < DH / 2; ++i) {
+      dv_acc[i] = 0.f;
+      dk_acc[i] = 0.f;
+    }
+    mbar_wait(smem_u32(kv_full), 0);
     for (int i = 0; i < TQ; ++i) {
-      const int q = i * BQ + row;
-      const bool q_ok = q < p.q_len;
-      const long long sidx = (static_cast<long long>(b) * p.heads + head) * p.q_len + q;
-      const float L = q_ok ? __ldg(p.lse + sidx) : INFINITY;
-      const float Dl = q_ok ? __ldg(p.delta + sidx) : 0.f;
-      mbar_wait(smem_u32(sdp_full), i & 1);
-      tc_fence_after();
-      // the P / dS buffers were read by the previous tile's MMAs, whose completion dq_full(i-1) has signalled (awaited below)
-#pragma unroll 1
-      for (int h = 0; h < 2; ++h) {   // 64 keys at a time (register budget)
-        uint32_t s0[32], s1[32], d0[32], d1[32];
-        tmem_ld32(lane_addr + TM_S + h * 64, s0);
-        tmem_ld32(lane_addr + TM_S + h * 64 + 32, s1);
-        tmem_ld32(lane_addr + TM_DP + h * 64, d0);
-        tmem_ld32(lane_addr + TM_DP + h * 64 + 32, d1);
-        tmem_ld_wait();
-        uint8_t* prow = smem + OFF_P + h * ATOM + row * 128;
-        uint8_t* drow = smem + OFF_DS + h * ATOM + row * 128;
+      const int st = i & 1;
+      mbar_wait(smem_u32(&q_full[st]), (i >> 1) & 1);
+      const uint32_t q_s = smem_u32(smem + OFF_Q + st * QT_BYTES), do_s = smem_u32(smem + OFF_DO + st * QT_BYTES);
+      // S^T = K Q_i^T, dP^T = V dO_i^T (keys x queries; both operands K-major)
+      float s[BQ / 2], dp[BQ / 2];
+      wgmma_fence();
 #pragma unroll
-        for (int c = 0; c < 8; ++c) {   // 8 keys per 16-byte chunk
-          uint32_t pw[4], dw[4];
+      for (int k = 0; k < DH / 16; ++k)
+        wgmma_bf16_ss_n64<0, 0>(s, gmma_desc_sw128(k_s, 16, 1024) + 2 * k, gmma_desc_sw128(q_s, 16, 1024) + 2 * k,
+                                k > 0 ? 1u : 0u);
 #pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            float pv[2], dv[2];
+      for (int k = 0; k < DH / 16; ++k)
+        wgmma_bf16_ss_n64<0, 0>(dp, gmma_desc_sw128(v_s, 16, 1024) + 2 * k, gmma_desc_sw128(do_s, 16, 1024) + 2 * k,
+                                k > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_hold(s);
+      wgmma_hold(dp);
+      // P^T, dS^T -> bf16 register A fragments (16 queries per k-step) and dS^T -> shared memory
+      uint32_t pa[BQ / 16][4], da[BQ / 16][4];
 #pragma unroll
-            for (int t = 0; t < 2; ++t) {
-              const int col = c * 8 + e * 2 + t;            // 0..63
-              const float sv = __uint_as_float(col < 32 ? s0[col] : s1[col - 32]);
-              const float dpv = __uint_as_float(col < 32 ? d0[col] : d1[col - 32]);
-              float pp = ab_ex2(fmaf(sv, p.scale_log2e, -L));
-              if (h * 64 + col >= valid) pp = 0.f;
-              pv[t] = pp;
-              dv[t] = pp * (dpv - Dl) * p.scale;
-            }
-            pw[e] = pack_bf16x2(pv[0], pv[1]);
-            dw[e] = pack_bf16x2(dv[0], dv[1]);
-          }
-          *reinterpret_cast<uint4*>(prow + ((c ^ (row & 7)) << 4)) = make_uint4(pw[0], pw[1], pw[2], pw[3]);
-          *reinterpret_cast<uint4*>(drow + ((c ^ (row & 7)) << 4)) = make_uint4(dw[0], dw[1], dw[2], dw[3]);
+      for (int jj = 0; jj < BQ / 8; ++jj) {
+        const int qc = 8 * jj + c2;   // query column (in the tile) of elements e = 0, 1
+        float L[2], Dl[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int q = i * BQ + qc + e;
+          const bool q_ok = q < p.q_len;
+          const long long sidx = (static_cast<long long>(b) * p.heads + head) * p.q_len + q;
+          L[e] = q_ok ? __ldg(p.lse + sidx) : INFINITY;
+          Dl[e] = q_ok ? __ldg(p.delta + sidx) : 0.f;
+        }
+        float pv[4], dv[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {   // e = 2 r + t: key row kr0 + 8 r, query column qc + t
+          const int r = e >> 1, t = e & 1;
+          float pp = ab_ex2(fmaf(s[4 * jj + e], p.scale_log2e, -L[t]));
+          if (kr0 + 8 * r >= valid) pp = 0.f;
+          pv[e] = pp;
+          dv[e] = pp * (dp[4 * jj + e] - Dl[t]) * p.scale;
+        }
+        pa[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(pv[0], pv[1]);
+        pa[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(pv[2], pv[3]);
+        const uint32_t d0 = pack_bf16x2(dv[0], dv[1]), d1 = pack_bf16x2(dv[2], dv[3]);
+        da[jj >> 1][(jj & 1) * 2 + 0] = d0;
+        da[jj >> 1][(jj & 1) * 2 + 1] = d1;
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int key = kr0 + 8 * r;
+          *reinterpret_cast<uint32_t*>(ds_rows + key * 128 + ((jj ^ (key & 7)) << 4) + c2 * 2) = r ? d1 : d0;
         }
       }
       fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(pds_full));
-      // ---- drain dQ_i: TMEM -> swizzled staging -> TMA fp32 reduce-add into the dQ accumulator ----
-      mbar_wait(smem_u32(dq_full), i & 1);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < DH; c += 32) {
-        uint32_t r[32];
-        tmem_ld32(lane_addr + TM_DQ + c, r);
-        tmem_ld_wait();
-        if (elect_one()) tma_store_wait_read<1>();
-        __syncwarp();
-        const uint32_t box = stg + (stg_count & 1) * 4096;
+      warpgroup_bar(w);
+      // dV += P^T dO_i, dK += dS^T Q_i (B operands MN-major: 16 queries = 2048 bytes per step);
+      // dQ_i = dS K over this warpgroup's keys (A = dS^T in smem: MN-major; B = K: MN-major; 16 keys per step)
+      float dq[DH / 2];
+      wgmma_fence();
 #pragma unroll
-        for (int qq = 0; qq < 8; ++qq) {
-          const uint32_t addr = box + lane * 128 + ((qq ^ (lane & 7)) << 4);
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[4 * qq]), "r"(r[4 * qq + 1]),
-                       "r"(r[4 * qq + 2]), "r"(r[4 * qq + 3])
-                       : "memory");
-        }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (elect_one()) {
-          tma_reduce_add_3d(&p.tmDQ, box, head * DH + c, i * BQ + warp * 32, b);
-          tma_store_commit();
-        }
-        __syncwarp();
-        ++stg_count;
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(dq_free));
-    }
-    // ---- dK_j, dV_j: thread r <-> key row r ----
-    mbar_wait(smem_u32(fin_full), 0);
-    tc_fence_after();
-    const int key = j * BKV + row;
-#pragma unroll 1
-    for (int which = 0; which < 2; ++which) {
-      uint32_t r0[32], r1[32];
-      const uint32_t ta = lane_addr + (which == 0 ? TM_DV : TM_DK);
-      tmem_ld32(ta, r0);
-      tmem_ld32(ta + 32, r1);
-      tmem_ld_wait();
-      if (key < p.kv_len) {
-        __nv_bfloat16* base = which == 0 ? p.dv : p.dk;
-        const long long rs = which == 0 ? p.dv_rs : p.dk_rs, bs = which == 0 ? p.dv_bs : p.dk_bs;
-        uint4* o4 = reinterpret_cast<uint4*>(base + static_cast<long long>(b) * bs + static_cast<long long>(key) * rs +
-                                             head * DH);
+      for (int k = 0; k < BQ / 16; ++k) wgmma_bf16_rs_n64<1>(dv_acc, pa[k], gmma_desc_sw128(do_s + k * 2048, 1024, 1024), 1u);
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          o4[i] = make_uint4(pack_bf16x2(__uint_as_float(r0[8 * i]), __uint_as_float(r0[8 * i + 1])),
-                             pack_bf16x2(__uint_as_float(r0[8 * i + 2]), __uint_as_float(r0[8 * i + 3])),
-                             pack_bf16x2(__uint_as_float(r0[8 * i + 4]), __uint_as_float(r0[8 * i + 5])),
-                             pack_bf16x2(__uint_as_float(r0[8 * i + 6]), __uint_as_float(r0[8 * i + 7])));
-          o4[4 + i] = make_uint4(pack_bf16x2(__uint_as_float(r1[8 * i]), __uint_as_float(r1[8 * i + 1])),
-                                 pack_bf16x2(__uint_as_float(r1[8 * i + 2]), __uint_as_float(r1[8 * i + 3])),
-                                 pack_bf16x2(__uint_as_float(r1[8 * i + 4]), __uint_as_float(r1[8 * i + 5])),
-                                 pack_bf16x2(__uint_as_float(r1[8 * i + 6]), __uint_as_float(r1[8 * i + 7])));
+      for (int k = 0; k < BQ / 16; ++k) wgmma_bf16_rs_n64<1>(dk_acc, da[k], gmma_desc_sw128(q_s + k * 2048, 1024, 1024), 1u);
+#pragma unroll
+      for (int k = 0; k < 64 / 16; ++k)
+        wgmma_bf16_ss_n64<1, 1>(dq, gmma_desc_sw128(ds_s + k * 2048, 1024, 1024),
+                                gmma_desc_sw128(k_s + k * 2048, 1024, 1024), k > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_hold(dv_acc);
+      wgmma_hold(dk_acc);
+      wgmma_hold(dq);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(&q_empty[st]));   // Q_i / dO_i may be overwritten
+      warpgroup_bar(w);                                      // dS^T may be overwritten by the next tile
+      // dQ accumulator += this warpgroup's partial (rows = queries 16 ww + lane/4 + 8 r of the tile)
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int q = i * BQ + 16 * (warp & 3) + (lane >> 2) + 8 * r;
+        if (q >= p.q_len) continue;
+        float* dst = p.dq + (static_cast<long long>(b) * p.q_len + q) * inner + head * DH + c2;
+#pragma unroll
+        for (int jj = 0; jj < DH / 8; ++jj) {
+          atomicAdd(dst + 8 * jj, dq[4 * jj + 2 * r]);
+          atomicAdd(dst + 8 * jj + 1, dq[4 * jj + 2 * r + 1]);
         }
       }
     }
-    if (elect_one()) tma_store_wait_all();
-    __syncwarp();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+    // ---- dK_j, dV_j -> bf16 ----
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int key = j * BKV + kr0 + 8 * r;
+      if (key >= p.kv_len) continue;
+      __nv_bfloat16* pv = p.dv + static_cast<long long>(b) * p.dv_bs + static_cast<long long>(key) * p.dv_rs + head * DH + c2;
+      __nv_bfloat16* pk = p.dk + static_cast<long long>(b) * p.dk_bs + static_cast<long long>(key) * p.dk_rs + head * DH + c2;
+#pragma unroll
+      for (int jj = 0; jj < DH / 8; ++jj) {
+        *reinterpret_cast<uint32_t*>(pv + 8 * jj) = pack_bf16x2(dv_acc[4 * jj + 2 * r], dv_acc[4 * jj + 2 * r + 1]);
+        *reinterpret_cast<uint32_t*>(pk + 8 * jj) = pack_bf16x2(dk_acc[4 * jj + 2 * r], dk_acc[4 * jj + 2 * r + 1]);
+      }
+    }
   }
 }
 
@@ -343,24 +266,19 @@ extern "C" int ns2_attn_bwd(const ns2_attn_bwd_args* a, ns2_stream_t stream_) {
   }
   AttnBwdDev dev;
   memset(&dev, 0, sizeof(dev));
-  const uint32_t box[3] = {64, 128, 1};
   const uint64_t inner = (uint64_t)a->heads * 64;
-  auto map16 = [&](CUtensorMap* m, const void* ptr, int len, int64_t rs, int64_t bs) {
+  auto map16 = [&](CUtensorMap* m, const void* ptr, int len, int64_t rs, int64_t bs, uint32_t rows) {
     const uint64_t dims[3] = {inner, (uint64_t)len, (uint64_t)a->batches};
     const uint64_t str[3] = {2, (uint64_t)rs * 2, (uint64_t)bs * 2};
+    const uint32_t box[3] = {64, rows, 1};
     return make_tmap_16bit(m, ptr, 3, dims, str, box);
   };
   int rc;
-  if ((rc = map16(&dev.tmQ, a->q, a->q_len, a->q_row_stride, a->q_batch_stride)) != kOk) return rc;
-  if ((rc = map16(&dev.tmK, a->k, a->kv_len, a->k_row_stride, a->k_batch_stride)) != kOk) return rc;
-  if ((rc = map16(&dev.tmV, a->v, a->kv_len, a->v_row_stride, a->v_batch_stride)) != kOk) return rc;
-  if ((rc = map16(&dev.tmDO, a->d_o, a->q_len, a->do_row_stride, a->do_batch_stride)) != kOk) return rc;
-  {
-    const uint64_t dims[3] = {inner, (uint64_t)a->q_len, (uint64_t)a->batches};
-    const uint64_t str[3] = {4, inner * 4, inner * (uint64_t)a->q_len * 4};
-    const uint32_t qbox[3] = {32, 32, 1};
-    if ((rc = make_tmap_f32(&dev.tmDQ, a->dq_accum, 3, dims, str, qbox)) != kOk) return rc;
-  }
+  if ((rc = map16(&dev.tmQ, a->q, a->q_len, a->q_row_stride, a->q_batch_stride, ab::BQ)) != kOk) return rc;
+  if ((rc = map16(&dev.tmK, a->k, a->kv_len, a->k_row_stride, a->k_batch_stride, ab::BKV)) != kOk) return rc;
+  if ((rc = map16(&dev.tmV, a->v, a->kv_len, a->v_row_stride, a->v_batch_stride, ab::BKV)) != kOk) return rc;
+  if ((rc = map16(&dev.tmDO, a->d_o, a->q_len, a->do_row_stride, a->do_batch_stride, ab::BQ)) != kOk) return rc;
+  dev.dq = a->dq_accum;
   dev.lse = a->lse;
   dev.delta = a->delta;
   dev.dk = reinterpret_cast<__nv_bfloat16*>(a->dk);
@@ -376,7 +294,7 @@ extern "C" int ns2_attn_bwd(const ns2_attn_bwd_args* a, ns2_stream_t stream_) {
   dev.scale_log2e = a->scale * 1.4426950408889634f;
   NS2_CUDA_CHECK(set_max_smem_once(attn_bwd_kernel, ab::SMEM_BYTES));
   dim3 grid((a->kv_len + ab::BKV - 1) / ab::BKV, a->heads, a->batches);
-  attn_bwd_kernel<<<grid, 192, ab::SMEM_BYTES, stream>>>(dev);
+  attn_bwd_kernel<<<grid, ab::THREADS, ab::SMEM_BYTES, stream>>>(dev);
   g_launches.fetch_add(2, std::memory_order_relaxed);
   NS2_CUDA_CHECK(cudaGetLastError());
   return kOk;

@@ -12,7 +12,7 @@ namespace ns2 {
 
 std::atomic<long long> g_launches{0};
 
-// CTAs per SM of the streaming RMSNorm grid: 76 registers -> 3 resident, two generations measured best on B200
+// CTAs per SM of the streaming RMSNorm grid: 76 registers -> 3 resident
 // (19.5 us vs 20.1 at 3, 20.5 at 4, 23.3 for one CTA per 8 rows; 32768 x 512 rows, profiles/r02j_rmsnorm_stream.txt)
 constexpr int kRmsnormCtasPerSm = 6;
 

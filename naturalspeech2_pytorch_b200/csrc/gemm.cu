@@ -1,20 +1,13 @@
-// Segmented tcgen05 GEMM for sm_100a with fused epilogues (see include/ns2_b200.h, section 1).
+// Segmented wgmma GEMM for sm_90a with fused epilogues (see include/ns2_b200.h, section 1).
 //
-// Two kernels share the pipeline structure and the epilogue code:
-//   gemm2_kernel  CTA PAIRS (cluster of 2, tcgen05 cta_group::2): the pair owns a 256-position x BN tile; each CTA
-//                 stages its own 128 A rows and HALF of the B tile, so per-SM shared-memory traffic per MMA is halved
-//                 — the 1-CTA kernel is smem-bandwidth bound (operand reads + TMA fills ~ 192-256 B/clk vs 128 B/clk).
-//                 Used whenever a batch has more than 128 positions.
-//   gemm_kernel   single CTA, 128 x BN tile: the small-M problems (FiLM GEMM, perceiver, cross-attention K/V).
-// Both are persistent (one CTA per SM), 256 threads, warp-specialised:
-//   warp 0     TMA producer: A tile (128 positions x 64 channels, 3-D map so that shifted rows of a causal conv that
-//              fall before position 0 are zero-filled by the TMA unit) + B tile
-//   warp 1     tcgen05.mma issuer (one elected lane; leader CTA only in the pair kernel), accumulators in TMEM,
-//              double-buffered across tiles
-//   warp 2     TMEM allocator
-//   warps 4-7  epilogue: tcgen05.ld -> registers -> bias / residual / GEGLU / FiLM+gate -> global
-// Three pipelines: smem ring (full/empty mbarriers, TMA <-> MMA), TMEM double buffer (tmem_full/empty,
-// MMA <-> epilogue), static round-robin tile scheduler (n fastest so co-resident CTAs share A rows in L2).
+// gemm_kernel: persistent (one CTA per SM), 384 threads, warp-specialised, 128 positions x BN columns per tile:
+//   warpgroup 0    TMA producer (warp 0): A tile (128 positions x 64 channels, 3-D map so that shifted rows of a causal
+//                  conv that fall before position 0 are zero-filled by the TMA unit) + B tile (BN rows x 64 channels)
+//                  through a smem ring (full / empty mbarriers)
+//   warpgroups 1-2 consumers: warpgroup w owns positions [64 (w-1), 64 w) of the tile, issues wgmma m64nBNk16 from the
+//                  shared-memory ring into register accumulators, then runs the epilogue (bias / residual / GEGLU /
+//                  FiLM + gate) straight from the accumulator fragments to global memory
+// Tiles are handed out by a static round robin, n fastest so co-resident CTAs share A rows in L2.
 //
 // Replaces, in the reference: nn.Linear GEMMs (ns2.py:1021,1024,1051-1053,783,613,731) and
 // CausalConv1d (ns2.py:583-595) incl. the WavenetResBlock body (ns2.py:619-636) and GEGLU (1004-1007).
@@ -34,10 +27,8 @@ constexpr int BK = 64;
 struct GemmDev {
   CUtensorMap tmA;
   CUtensorMap tmB;
-  CUtensorMap tmOut;   // pair kernel: TMA store / reduce-add target (3-D: columns, positions, batch)
-  int reduce_add;      // pair kernel, F32 epilogue with resid == out: out += acc + bias via TMA reduce-add
   int tiles_n, tiles_per_batch, tiles_m, num_tiles;
-  int narrow_last;     // pair kernel, groups == 1, n % BN != 0: schedule the partial-width n-tiles after all full-width ones
+  int narrow_last;     // groups == 1, n % BN != 0: schedule the partial-width n-tiles after all full-width ones
   int a_rows, n, groups;
   int a_gcs, b_grs, out_gcs;
   int dil[NS2_GEMM_MAX_GROUPS];
@@ -54,30 +45,18 @@ struct GemmDev {
   int film_gs;
   int act;            // BF16 / F32 epilogues: 0 = none, 1 = SiLU applied to acc + bias (ns2_gemm_args.flags & NS2_GEMM_FLAG_SILU)
   int skip_epilogue;  // measurement aid (ns2_gemm_args.flags & NS2_GEMM_FLAG_SKIP_EPILOGUE): mainloop-only timing
-  long long* timeline;  // bring-up aid (ns2_gemm_args.debug_timeline): clock64 stamps of CTA pair 0, else NULL
 };
-
-// timeline layout: [tile ti < 64][8 slots] of the leader CTA of pair 0 (tools/gemm_timeline.py)
-#define NS2_GEMM_STAMP(slot)                                                                             \
-  do {                                                                                                   \
-    if (p.timeline != nullptr && pair == 0 && leader && ti < 64) p.timeline[ti * 8 + (slot)] = clock64(); \
-  } while (0)
 
 struct TileCoord {
   int g, b, n0, n_tile;
 };
 
-// ROWS = positions covered by one tile (128 for a single CTA, 256 for a CTA pair)
-template <int ROWS>
 __device__ __forceinline__ TileCoord decode_tile(const GemmDev& p, int tile) {
   TileCoord t;
   int m_tile;
   if (p.narrow_last) {
-    // The last n-tile of every row block is narrower (n % BN columns) and its MMAs are cheaper.  With the plain
-    // n-fastest order and the static tile -> pair round robin those cheap tiles land on a subset of the pairs (FFN
-    // conv: tiles_n = 6, 74 pairs -> only odd pairs ever see one) and the launch still lasts ceil(tiles / pairs) FULL
-    // tiles.  Full-width tiles first (n fastest, so a row block's activations stay hot in L2), then all narrow ones:
-    // every pair ends on cheap tiles and the longest pair does 9 full + 2 narrow instead of 11 full (FFN conv, cfg2).
+    // The last n-tile of every row block is narrower (n % BN columns).  Full-width tiles first (n fastest, so a row
+    // block's activations stay hot in L2), then all narrow ones, so that every CTA ends on the narrow tiles.
     const int wide_n = p.tiles_n - 1;
     const int wide_total = p.tiles_m * wide_n;
     t.g = 0;
@@ -96,1025 +75,217 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmDev& p, int tile) {
     t.n_tile = r - m_tile * p.tiles_n;
   }
   t.b = m_tile / p.tiles_per_batch;
-  t.n0 = (m_tile - t.b * p.tiles_per_batch) * ROWS;
+  t.n0 = (m_tile - t.b * p.tiles_per_batch) * BM;
   return t;
 }
 
 // ------------------------------------------------------------------------------------------------
-// epilogue pieces (shared by both kernels)
+// epilogue: straight from the wgmma accumulator fragments.  Thread (warp ww of the consumer warpgroup, lane l) holds
+// rows r0 = 16 ww + l/4 and r0 + 8 of its warpgroup's 64 rows, columns 8j + 2(l%4) + {0, 1}:  acc[4j + 2i + k].
 // ------------------------------------------------------------------------------------------------
-template <int W>
-__device__ __forceinline__ void tmem_load_f32(uint32_t taddr, float (&v)[W]) {
-  static_assert(W == 32 || W == 16, "chunk width");
-  if constexpr (W == 32) {
-    uint32_t r[32];
-    tmem_ld32(taddr, r);
-    tmem_ld_wait();
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-  } else {
-    uint32_t r[16];
-    tmem_ld16(taddr, r);
-    tmem_ld_wait();
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-  }
+__device__ __forceinline__ float silu_f(float v) { return __fdividef(v, 1.0f + __expf(-v)); }
+
+// tanh(z) * sigmoid(z) with ONE MUFU: u = tanh(z/2); sigmoid = (1 + u)/2; tanh(z) = 2u / (1 + u^2), the reciprocal of
+// w = 1 + u^2 in [1, 2] by a linear seed + two Newton steps on the FMA pipe (rel. err < 2e-5)
+__device__ __forceinline__ float wavenet_gate(float z) {
+  const float u = tanh_fast(0.5f * z);
+  const float w = fmaf(u, u, 1.0f);
+  float r = fmaf(-0.47058824f, w, 1.4117647f);     // 24/17 - 8/17 w: |1 - w r| <= 1/17 on [1, 2]
+  r = r * fmaf(-w, r, 2.0f);
+  r = r * fmaf(-w, r, 2.0f);
+  return (u * r) * (1.0f + u);
 }
 
-template <int W>
-__device__ __forceinline__ void add_vec(float (&v)[W], const float* __restrict__ src) {
-  const float4* s4 = reinterpret_cast<const float4*>(src);
-#pragma unroll
-  for (int i = 0; i < W / 4; ++i) {
-    const float4 b4 = __ldg(s4 + i);
-    v[4 * i + 0] += b4.x;
-    v[4 * i + 1] += b4.y;
-    v[4 * i + 2] += b4.z;
-    v[4 * i + 3] += b4.w;
-  }
-}
-
-// SiLU of conv / linear outputs (nn.SiLU after the SpeechPromptEncoder convs, ns2.py:316-320)
-template <int W>
-__device__ __forceinline__ void silu_vec(float (&v)[W]) {
-#pragma unroll
-  for (int i = 0; i < W; ++i) v[i] = __fdividef(v[i], 1.0f + __expf(-v[i]));
-}
-
-template <int W>
-__device__ __forceinline__ void store_bf16(const float (&v)[W], __nv_bfloat16* dst) {
-  uint4* o4 = reinterpret_cast<uint4*>(dst);
-#pragma unroll
-  for (int i = 0; i < W / 8; ++i) {
-    uint4 w;
-    w.x = pack_bf16x2(v[8 * i + 0], v[8 * i + 1]);
-    w.y = pack_bf16x2(v[8 * i + 2], v[8 * i + 3]);
-    w.z = pack_bf16x2(v[8 * i + 4], v[8 * i + 5]);
-    w.w = pack_bf16x2(v[8 * i + 6], v[8 * i + 7]);
-    o4[i] = w;
-  }
-}
-
-template <int W>
-__device__ __forceinline__ void store_f32(const float (&v)[W], float* dst) {
-  float4* o4 = reinterpret_cast<float4*>(dst);
-#pragma unroll
-  for (int i = 0; i < W / 4; ++i)
-    o4[i] = make_float4(v[4 * i + 0], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-}
-
-// one chunk of W accumulator columns starting at tile column `tc` of the BF16 / F32 epilogues
-template <int W, int EPI>
-__device__ __forceinline__ void epi_plain_chunk(const GemmDev& p, const TileCoord& t, int tile_col0, int tc,
-                                                uint32_t taddr, bool row_ok, long long grow) {
-  const int col0 = tile_col0 + tc;
-  float v[W];
-  tmem_load_f32<W>(taddr + tc, v);
-  if (p.bias != nullptr) add_vec<W>(v, p.bias + t.g * p.b_grs + col0);
-  if (p.act != 0) silu_vec<W>(v);
-  if (!row_ok) return;
-  if constexpr (EPI == NS2_EPI_BF16) {
-    store_bf16<W>(v, reinterpret_cast<__nv_bfloat16*>(p.out) + grow * p.out_rs + t.g * p.out_gcs + col0);
-  } else {
-    if (p.resid != nullptr) add_vec<W>(v, p.resid + grow * p.resid_rs + t.g * p.out_gcs + col0);
-    store_f32<W>(v, reinterpret_cast<float*>(p.out) + grow * p.out_rs + t.g * p.out_gcs + col0);
-  }
-}
-
-// Full epilogue of one 128-row x BN accumulator tile held in this CTA's TMEM.
-//   taddr: TMEM address of (first lane of this warp, first column of the accumulator stage)
-//   npos : position (row inside the batch) owned by this thread
 template <int BN, int NACC, int EPI>
-__device__ __forceinline__ void epilogue_tile(const GemmDev& p, const TileCoord& t, uint32_t taddr, int npos) {
-  const bool row_ok = npos < p.a_rows;
-  const long long grow = static_cast<long long>(t.b) * p.a_rows + npos;
+__device__ __forceinline__ void epilogue_tile(const GemmDev& p, const TileCoord& t, const float (&acc)[NACC][BN / 2],
+                                              int row_base, int c2) {
   const int tile_col0 = t.n_tile * BN;
-  if constexpr (EPI == NS2_EPI_BF16 || EPI == NS2_EPI_F32) {
-#pragma unroll 1
-    for (int tc = 0; tc + 32 <= BN; tc += 32) {
-      if (tile_col0 + tc >= p.n) break;
-      epi_plain_chunk<32, EPI>(p, t, tile_col0, tc, taddr, row_ok, grow);
-    }
-    if constexpr (BN % 32 != 0) {
-      constexpr int tc = BN - 16;
-      if (tile_col0 + tc < p.n) epi_plain_chunk<16, EPI>(p, t, tile_col0, tc, taddr, row_ok, grow);
-    }
-  } else if constexpr (EPI == NS2_EPI_GEGLU) {
-    static_assert(EPI != NS2_EPI_GEGLU || BN == 256, "GEGLU tiles pair 128 value + 128 gate rows");
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-      const int pcol0 = tile_col0 + c * 32;  // packed (value) column
-      if (pcol0 >= p.n) break;
-      float xv[32], gv[32];
-      {
-        uint32_t rv[32], rg[32];
-        tmem_ld32(taddr + c * 32, rv);
-        tmem_ld32(taddr + 128 + c * 32, rg);
-        tmem_ld_wait();
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          xv[i] = __uint_as_float(rv[i]);
-          gv[i] = __uint_as_float(rg[i]);
+  for (int i = 0; i < 2; ++i) {
+    const int npos = row_base + 8 * i;
+    if (npos >= p.a_rows) continue;
+    const long long grow = static_cast<long long>(t.b) * p.a_rows + npos;
+    if constexpr (EPI == NS2_EPI_BF16 || EPI == NS2_EPI_F32) {
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = tile_col0 + 8 * j + c2;
+        if (tile_col0 + 8 * j >= p.n) break;   // n is a multiple of 32: 8-column groups are all in or all out
+        float v0 = acc[0][4 * j + 2 * i], v1 = acc[0][4 * j + 2 * i + 1];
+        if (p.bias != nullptr) {
+          const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + col));
+          v0 += bb.x;
+          v1 += bb.y;
         }
-      }
-      add_vec<32>(xv, p.bias + t.g * p.b_grs + pcol0);
-      add_vec<32>(gv, p.bias + t.g * p.b_grs + pcol0 + 128);
-#pragma unroll
-      for (int i = 0; i < 32; ++i) xv[i] *= gelu_erf(gv[i]);
-      if (row_ok)
-        store_bf16<32>(xv, reinterpret_cast<__nv_bfloat16*>(p.out) + grow * p.out_rs + t.g * p.out_gcs +
-                               t.n_tile * 128 + c * 32);
-    }
-  } else {  // NS2_EPI_WAVENET
-    static_assert(EPI != NS2_EPI_WAVENET || NACC == 2, "wavenet block needs conv + res accumulators");
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      const int col0 = tile_col0 + c * 32;
-      if (col0 >= p.n) break;
-      float y[32], rr[32];
-      {
-        uint32_t rc[32], r1[32];
-        tmem_ld32(taddr + c * 32, rc);
-        tmem_ld32(taddr + BN + c * 32, r1);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          y[i] = __uint_as_float(rc[i]);
-          rr[i] = __uint_as_float(r1[i]);
+        if (p.act != 0) {
+          v0 = silu_f(v0);
+          v1 = silu_f(v1);
         }
-      }
-      const float* b0 = p.bias + t.g * p.b_grs + col0;
-      add_vec<32>(y, b0);
-      add_vec<32>(rr, b0 + p.bias1_off);
-      const float4* gm = reinterpret_cast<const float4*>(p.film + t.b * p.film_bs + t.g * p.film_gs + col0);
-      const float4* bt = reinterpret_cast<const float4*>(p.film + t.b * p.film_bs + t.g * p.film_gs + col0 + p.n);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float4 g4 = __ldg(gm + i), b4 = __ldg(bt + i);
-        const float ga[4] = {g4.x, g4.y, g4.z, g4.w}, be[4] = {b4.x, b4.y, b4.z, b4.w};
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float z = fmaf(y[4 * i + j], ga[j], be[j]);
-          y[4 * i + j] = tanhf(z) * sigmoid_f(z) + rr[4 * i + j];
-        }
-      }
-      if (row_ok)
-        store_bf16<32>(y, reinterpret_cast<__nv_bfloat16*>(p.out) + grow * p.out_rs + t.g * p.out_gcs + col0);
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// pair-kernel epilogue: registers -> 128B-swizzled smem staging (per warp, double-buffered) -> TMA store.
-// Per-thread scattered 16-byte global stores (the single-CTA epilogue above) cost ~10k cycles per 128x256 tile
-// in the LSU; the bulk stores are issued by one lane per warp and overlap with the next chunk's math.
-// ------------------------------------------------------------------------------------------------
-constexpr int STG_BYTES = 32 * 128;  // one box: 32 rows x 128 bytes
-
-struct Stager {
-  uint32_t base;      // smem address of this warp's two staging boxes
-  uint32_t count;     // boxes issued so far
-  int lane;
-  __device__ __forceinline__ uint32_t acquire() {
-    // the box used two stores ago must have been read out by the TMA engine (bulk groups belong to the elected lane)
-    if (elect_one()) tma_store_wait_read<1>();
-    __syncwarp();
-    return base + (count & 1) * STG_BYTES;
-  }
-  // thread writes 16-byte piece j (0..7) of its 128-byte row
-  __device__ __forceinline__ void put(uint32_t box, int j, uint4 v) const {
-    const uint32_t addr = box + lane * 128 + ((j ^ (lane & 7)) << 4);
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
-                 : "memory");
-  }
-  __device__ __forceinline__ void submit(const CUtensorMap* m, uint32_t box, int c0, int c1, int c2, bool reduce) {
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (elect_one()) {   // converged warp + elected lane: no per-instruction uniformisation loop (see gemm_kernel)
-      if (reduce) tma_reduce_add_3d(m, box, c0, c1, c2);
-      else tma_store_3d(m, box, c0, c1, c2);
-      tma_store_commit();
-    }
-    __syncwarp();
-    ++count;
-  }
-};
-
-__device__ __forceinline__ void put_bf16x32(const Stager& st, uint32_t box, int half, const float (&v)[32]) {
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    uint4 w;
-    w.x = pack_bf16x2(v[8 * q + 0], v[8 * q + 1]);
-    w.y = pack_bf16x2(v[8 * q + 2], v[8 * q + 3]);
-    w.z = pack_bf16x2(v[8 * q + 4], v[8 * q + 5]);
-    w.w = pack_bf16x2(v[8 * q + 6], v[8 * q + 7]);
-    st.put(box, half * 4 + q, w);
-  }
-}
-
-// taddr: TMEM address (first lane of this warp, first column of the accumulator stage); row0: first position of
-// this warp's 32 rows.  Returns after the last TMEM read of the tile (stores may still be in flight).
-template <int BN, int NACC, int EPI>
-__device__ __forceinline__ void epilogue_tile_tma(const GemmDev& p, const TileCoord& t, uint32_t taddr, int row0,
-                                                  Stager& st) {
-  const int tile_col0 = t.n_tile * BN;
-  if constexpr (EPI == NS2_EPI_BF16) {
-#pragma unroll 1
-    for (int oc = 0; oc < BN; oc += 64) {
-      if (tile_col0 + oc >= p.n) break;
-      const uint32_t box = st.acquire();
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float v[32];
-        tmem_load_f32<32>(taddr + oc + h * 32, v);
-        if (p.bias != nullptr) add_vec<32>(v, p.bias + t.g * p.b_grs + tile_col0 + oc + h * 32);
-        if (p.act != 0) silu_vec<32>(v);
-        put_bf16x32(st, box, h, v);
-      }
-      st.submit(&p.tmOut, box, t.g * p.out_gcs + tile_col0 + oc, row0, t.b, false);
-    }
-  } else if constexpr (EPI == NS2_EPI_F32) {
-#pragma unroll 1
-    for (int oc = 0; oc < BN; oc += 32) {
-      if (tile_col0 + oc >= p.n) break;
-      const uint32_t box = st.acquire();
-      float v[32];
-      tmem_load_f32<32>(taddr + oc, v);
-      if (p.bias != nullptr) add_vec<32>(v, p.bias + t.g * p.b_grs + tile_col0 + oc);
-      if (p.act != 0) silu_vec<32>(v);
-#pragma unroll
-      for (int q = 0; q < 8; ++q)
-        st.put(box, q, make_uint4(__float_as_uint(v[4 * q]), __float_as_uint(v[4 * q + 1]),
-                                  __float_as_uint(v[4 * q + 2]), __float_as_uint(v[4 * q + 3])));
-      st.submit(&p.tmOut, box, t.g * p.out_gcs + tile_col0 + oc, row0, t.b, p.reduce_add != 0);
-    }
-  } else if constexpr (EPI == NS2_EPI_GEGLU) {
-    static_assert(EPI != NS2_EPI_GEGLU || BN == 256, "GEGLU tiles pair 128 value + 128 gate rows");
-#pragma unroll 1
-    for (int oc = 0; oc < 128; oc += 64) {  // output columns of this tile
-      const uint32_t box = st.acquire();
-#pragma unroll 1
-      for (int h = 0; h < 2; ++h) {
-        const int c = oc + h * 32;
-        float xv[32], gv[32];
-        {
-          uint32_t rv[32], rg[32];
-          tmem_ld32(taddr + c, rv);
-          tmem_ld32(taddr + 128 + c, rg);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            xv[i] = __uint_as_float(rv[i]);
-            gv[i] = __uint_as_float(rg[i]);
+        if constexpr (EPI == NS2_EPI_BF16) {
+          *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + grow * p.out_rs + t.g * p.out_gcs +
+                                       col) = pack_bf16x2(v0, v1);
+        } else {
+          if (p.resid != nullptr) {
+            const float2 rr = *reinterpret_cast<const float2*>(p.resid + grow * p.resid_rs + t.g * p.out_gcs + col);
+            v0 += rr.x;
+            v1 += rr.y;
           }
-        }
-        add_vec<32>(xv, p.bias + t.g * p.b_grs + tile_col0 + c);
-        add_vec<32>(gv, p.bias + t.g * p.b_grs + tile_col0 + c + 128);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) xv[i] *= gelu_erf_fast(gv[i]);
-        put_bf16x32(st, box, h, xv);
-      }
-      st.submit(&p.tmOut, box, t.g * p.out_gcs + t.n_tile * 128 + oc, row0, t.b, false);
-    }
-  } else {  // NS2_EPI_WAVENET
-    static_assert(EPI != NS2_EPI_WAVENET || NACC == 2, "wavenet block needs conv + res accumulators");
-#pragma unroll 1
-    for (int oc = 0; oc < BN; oc += 64) {
-      if (tile_col0 + oc >= p.n) break;
-      const uint32_t box = st.acquire();
-#pragma unroll 1
-      for (int h = 0; h < 2; ++h) {
-        const int c = oc + h * 32;
-        const int col0 = tile_col0 + c;
-        float y[32], rr[32];
-        {
-          uint32_t rc[32], r1[32];
-          tmem_ld32(taddr + c, rc);
-          tmem_ld32(taddr + BN + c, r1);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            y[i] = __uint_as_float(rc[i]);
-            rr[i] = __uint_as_float(r1[i]);
-          }
-        }
-        const float* b0 = p.bias + t.g * p.b_grs + col0;
-        add_vec<32>(y, b0);
-        add_vec<32>(rr, b0 + p.bias1_off);
-        const float4* gm = reinterpret_cast<const float4*>(p.film + t.b * p.film_bs + t.g * p.film_gs + col0);
-        const float4* bt = reinterpret_cast<const float4*>(p.film + t.b * p.film_bs + t.g * p.film_gs + col0 + p.n);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 g4 = __ldg(gm + i), b4 = __ldg(bt + i);
-          const float ga[4] = {g4.x, g4.y, g4.z, g4.w}, be[4] = {b4.x, b4.y, b4.z, b4.w};
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float z = fmaf(y[4 * i + j], ga[j], be[j]);
-            y[4 * i + j] = fmaf(tanh_fast(z), sigmoid_fast(z), rr[4 * i + j]);
-          }
-        }
-        put_bf16x32(st, box, h, y);
-      }
-      st.submit(&p.tmOut, box, t.g * p.out_gcs + tile_col0 + oc, row0, t.b, false);
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// pair-kernel epilogue, 8 warps per CTA: warp e (0..7) owns TMEM lane quarter e & 3 (32 positions) and column half
-// e >> 2 of the tile, so every SM sub-partition has two epilogue warps to hide each other's TMEM / shared-memory
-// latencies.  Inside a warp the 32-column steps are software-pipelined: the tcgen05.ld of step s+1 is in flight while
-// step s is being computed and staged.  registers -> 128B-swizzled smem staging (per warp, double-buffered) -> TMA.
-// ------------------------------------------------------------------------------------------------
-// taddr: TMEM address (first lane of this warp's quarter, first column of the accumulator stage); row0: first position
-// of this warp's 32 rows; hsel: column half.  Returns after the last TMEM read of the tile (stores may be in flight).
-template <int BN, int NACC, int EPI>
-__device__ __forceinline__ void epilogue_tile_tma8(const GemmDev& p, const TileCoord& t, uint32_t taddr, int row0,
-                                                   int hsel, Stager& st, int bias_off = 0) {
-  const int tile_col0 = t.n_tile * BN;
-  constexpr bool kTwo = (EPI == NS2_EPI_GEGLU || EPI == NS2_EPI_WAVENET);   // two accumulator regions per step
-  constexpr int HALF = (EPI == NS2_EPI_GEGLU) ? 64 : BN / 2;                // output columns of this warp per tile
-  constexpr int STEPS = HALF / 32;
-  const int c_base = hsel * HALF;                                           // first (value) column of this warp
-  constexpr int SECOND = (EPI == NS2_EPI_GEGLU) ? 128 : BN;                 // column offset of the second region
-  // steps whose columns lie inside the matrix (n is a multiple of 32; a partial last n-tile is narrower)
-  int nsteps = 0;
-#pragma unroll
-  for (int s = 0; s < STEPS; ++s)
-    if (tile_col0 + ((EPI == NS2_EPI_GEGLU) ? 0 : c_base + s * 32) < p.n) nsteps = s + 1;
-  if (nsteps == 0) return;
-
-  uint32_t ra[2][32], rb[2][32];
-  auto load = [&](int s, int buf) {
-    tmem_ld32(taddr + c_base + s * 32, ra[buf]);
-    if constexpr (kTwo) tmem_ld32(taddr + SECOND + c_base + s * 32, rb[buf]);
-  };
-  load(0, 0);
-  uint32_t box = 0;
-#pragma unroll
-  for (int s = 0; s < STEPS; ++s) {
-    if (s < nsteps) {
-      const int buf = s & 1;
-      tmem_ld_wait();
-      if (s + 1 < STEPS && s + 1 < nsteps) load(s + 1, buf ^ 1);   // in flight during this step's math
-      const int c = c_base + s * 32;                               // tile column of this step
-      float v[32];
-      if constexpr (EPI == NS2_EPI_BF16 || EPI == NS2_EPI_F32) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(ra[buf][i]);
-        if (p.bias != nullptr) add_vec<32>(v, p.bias + bias_off + t.g * p.b_grs + tile_col0 + c);
-        if (p.act != 0) silu_vec<32>(v);
-      } else if constexpr (EPI == NS2_EPI_GEGLU) {
-        const float4* bv4 = reinterpret_cast<const float4*>(p.bias + t.g * p.b_grs + tile_col0 + c);
-        const float4* bg4 = bv4 + 32;   // gate bias: + 128 columns
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {   // 4 columns at a time: keeps the bias temporaries out of the register peak
-          const float4 bv = __ldg(bv4 + q), bg = __ldg(bg4 + q);
-          const float bva[4] = {bv.x, bv.y, bv.z, bv.w}, bga[4] = {bg.x, bg.y, bg.z, bg.w};
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int i = 4 * q + j;
-            v[i] = (__uint_as_float(ra[buf][i]) + bva[j]) * gelu_erf_fast(__uint_as_float(rb[buf][i]) + bga[j]);
-          }
-        }
-      } else {  // NS2_EPI_WAVENET: y = tanh(z) sigmoid(z) + res, z = conv * gamma + beta   (ns2.py:619-636)
-        const int col0 = tile_col0 + c;
-        const float4* b04 = reinterpret_cast<const float4*>(p.bias + t.g * p.b_grs + col0);
-        const float4* b14 = reinterpret_cast<const float4*>(p.bias + t.g * p.b_grs + col0 + p.bias1_off);
-        const float4* ga4 = reinterpret_cast<const float4*>(p.film + t.b * p.film_bs + t.g * p.film_gs + col0);
-        const float4* be4 = reinterpret_cast<const float4*>(p.film + t.b * p.film_bs + t.g * p.film_gs + col0 + p.n);
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const float4 b0 = __ldg(b04 + q), b1 = __ldg(b14 + q), g4 = __ldg(ga4 + q), e4 = __ldg(be4 + q);
-          const float b0a[4] = {b0.x, b0.y, b0.z, b0.w}, b1a[4] = {b1.x, b1.y, b1.z, b1.w};
-          const float gaa[4] = {g4.x, g4.y, g4.z, g4.w}, bea[4] = {e4.x, e4.y, e4.z, e4.w};
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int i = 4 * q + j;
-            const float z = fmaf(__uint_as_float(ra[buf][i]) + b0a[j], gaa[j], bea[j]);
-            // tanh(z) * sigmoid(z) with ONE MUFU: u = tanh(z/2); sigmoid = (1 + u)/2; tanh(z) = 2u / (1 + u^2), the
-            // reciprocal of w = 1 + u^2 in [1, 2] by a linear seed + two Newton steps on the FMA pipe (rel. err < 2e-5)
-            const float u = tanh_fast(0.5f * z);
-            const float w = fmaf(u, u, 1.0f);
-            float r = fmaf(-0.47058824f, w, 1.4117647f);     // 24/17 - 8/17 w: |1 - w r| <= 1/17 on [1, 2]
-            r = r * fmaf(-w, r, 2.0f);
-            r = r * fmaf(-w, r, 2.0f);
-            const float gate = (u * r) * (1.0f + u);          // = tanh(z) * sigmoid(z)
-            v[i] = gate + (__uint_as_float(rb[buf][i]) + b1a[j]);
-          }
+          *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + grow * p.out_rs + t.g * p.out_gcs + col) =
+              make_float2(v0, v1);
         }
       }
-      // ---- stage + store ----
-      if constexpr (EPI == NS2_EPI_F32) {
-        box = st.acquire();
+    } else if constexpr (EPI == NS2_EPI_GEGLU) {
+      static_assert(EPI != NS2_EPI_GEGLU || BN == 256, "GEGLU tiles pair 128 value + 128 gate rows");
 #pragma unroll
-        for (int q = 0; q < 8; ++q)
-          st.put(box, q, make_uint4(__float_as_uint(v[4 * q]), __float_as_uint(v[4 * q + 1]),
-                                    __float_as_uint(v[4 * q + 2]), __float_as_uint(v[4 * q + 3])));
-        st.submit(&p.tmOut, box, t.g * p.out_gcs + tile_col0 + c, row0, t.b, p.reduce_add != 0);
-      } else {
-        if ((s & 1) == 0) box = st.acquire();
-        put_bf16x32(st, box, s & 1, v);
-        if ((s & 1) == 1 || s + 1 == nsteps) {
-          const int oc = c - (s & 1) * 32;   // first output column of the 64-column box
-          const int out_col = (EPI == NS2_EPI_GEGLU) ? t.n_tile * 128 + oc : tile_col0 + oc;
-          st.submit(&p.tmOut, box, t.g * p.out_gcs + out_col, row0, t.b, false);
-        }
+      for (int j = 0; j < 16; ++j) {
+        const int c = 8 * j + c2;   // value column inside the tile; its gate is column c + 128 (fragment j + 16)
+        const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + tile_col0 + c));
+        const float2 bg = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + tile_col0 + c + 128));
+        const float v0 = (acc[0][4 * j + 2 * i] + bv.x) * gelu_erf(acc[0][4 * (j + 16) + 2 * i] + bg.x);
+        const float v1 = (acc[0][4 * j + 2 * i + 1] + bv.y) * gelu_erf(acc[0][4 * (j + 16) + 2 * i + 1] + bg.y);
+        *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + grow * p.out_rs + t.g * p.out_gcs +
+                                     t.n_tile * 128 + c) = pack_bf16x2(v0, v1);
+      }
+    } else {  // NS2_EPI_WAVENET: y = tanh(z) sigmoid(z) + res, z = (conv + b0) * gamma + beta   (ns2.py:619-636)
+      static_assert(EPI != NS2_EPI_WAVENET || NACC == 2, "wavenet block needs conv + res accumulators");
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        if (tile_col0 + 8 * j >= p.n) break;
+        const int col = tile_col0 + 8 * j + c2;
+        const float2 b0 = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + col));
+        const float2 b1 = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + col + p.bias1_off));
+        const float* fp = p.film + t.b * p.film_bs + t.g * p.film_gs + col;
+        const float2 ga = __ldg(reinterpret_cast<const float2*>(fp));
+        const float2 be = __ldg(reinterpret_cast<const float2*>(fp + p.n));
+        const float z0 = fmaf(acc[0][4 * j + 2 * i] + b0.x, ga.x, be.x);
+        const float z1 = fmaf(acc[0][4 * j + 2 * i + 1] + b0.y, ga.y, be.y);
+        const float y0 = wavenet_gate(z0) + (acc[NACC - 1][4 * j + 2 * i] + b1.x);
+        const float y1 = wavenet_gate(z1) + (acc[NACC - 1][4 * j + 2 * i + 1] + b1.y);
+        *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + grow * p.out_rs + t.g * p.out_gcs +
+                                     col) = pack_bf16x2(y0, y1);
       }
     }
   }
 }
 
 // ------------------------------------------------------------------------------------------------
-// single-CTA kernel
+// kernel
 // ------------------------------------------------------------------------------------------------
 template <int BN, int NACC>
 struct GemmCfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BN == 256) ? 4 : 6;
-  static constexpr int ACC_COLS = BN * NACC;  // TMEM columns per accumulation stage
-  static constexpr int TMEM_COLS = (2 * ACC_COLS > 256) ? 512 : 256;
+  static constexpr int STAGES = (192 * 1024) / STAGE_BYTES;   // 4 stages of 48 KB (BN 256), 6 of 32 KB (BN 128)
+  static constexpr int THREADS = 384;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
+template <int BN>
+__device__ __forceinline__ void wgmma_tile_k16(float (&d)[BN / 2], uint64_t da, uint64_t db) {
+  if constexpr (BN == 256) wgmma_bf16_ss_n256<0, 0>(d, da, db, 1);
+  else wgmma_bf16_ss_n128<0, 0>(d, da, db, 1);
+}
+
 template <int BN, int NACC, int EPI>
-__global__ void __launch_bounds__(256, 1) gemm_kernel(const __grid_constant__ GemmDev p) {
+__global__ void __launch_bounds__(GemmCfg<BN, NACC>::THREADS, 1) gemm_kernel(const __grid_constant__ GemmDev p) {
   using Cfg = GemmCfg<BN, NACC>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
-  uint64_t* full_bar = bars;                          // [STAGES]
-  uint64_t* empty_bar = bars + Cfg::STAGES;           // [STAGES]
-  uint64_t* tfull_bar = bars + 2 * Cfg::STAGES;       // [2]
-  uint64_t* tempty_bar = bars + 2 * Cfg::STAGES + 2;  // [2]
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 2 * Cfg::STAGES + 4);
+  uint64_t* full_bar = bars;                 // [STAGES]
+  uint64_t* empty_bar = bars + Cfg::STAGES;  // [STAGES] one arrive per consumer warp
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmA);
     tma_prefetch_desc(&p.tmB);
-  }
-  if (warp == 1 && lane == 0) {
     for (int i = 0; i < Cfg::STAGES; ++i) {
       mbar_init(smem_u32(&full_bar[i]), 1);
-      mbar_init(smem_u32(&empty_bar[i]), 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(&tfull_bar[i]), 1);
-      mbar_init(smem_u32(&tempty_bar[i]), 4);  // one arrive per epilogue warp
+      mbar_init(smem_u32(&empty_bar[i]), 8);
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(tmem_holder), Cfg::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
-
-  // The two service warps run CONVERGED (all 32 lanes execute the loops on warp-uniform values) and elect one lane per
-  // TMA / tcgen05 instruction.  Issued from a single-lane divergent region, every UTMALDG / UTCHMMA is wrapped by the
-  // compiler in an ELECT / R2UR / BRA.U.ANY loop costing ~117 cycles (profiles/r02_ubench_mma.txt): 4 MMAs per k-block
-  // then take 468 cycles to ISSUE against 512 cycles of tensor work, which is what capped round 1's mainloop.
-  if (warp == 0) {
-    // =============================== TMA producer ===============================
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      const TileCoord t = decode_tile<BM>(p, tile);
-      const int dil = p.dil[t.g];
-      for (int s = 0; s < p.num_segs; ++s) {
-        const ns2_gemm_seg sg = p.segs[s];
-        const int row0 = t.n0 - sg.shift_units * dil;
-        const int a_c0 = t.g * p.a_gcs + sg.a_col_off;
-        const int b_r0 = t.g * p.b_grs + t.n_tile * BN;
-        const int kblocks = (sg.k_len + BK - 1) / BK;
-        for (int kb = 0; kb < kblocks; ++kb, ++it) {
-          const uint32_t stage = it % Cfg::STAGES;
-          const uint32_t phase = (it / Cfg::STAGES) & 1;
-          mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1);
-          if (elect_one()) {
-            const uint32_t fb = smem_u32(&full_bar[stage]);
-            mbar_arrive_expect_tx(fb, Cfg::STAGE_BYTES);
-            uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-            tma_load_3d(smem_u32(sa), &p.tmA, fb, a_c0 + kb * BK, row0, t.b);
-            tma_load_2d(smem_u32(sa + Cfg::A_BYTES), &p.tmB, fb, sg.b_col_off + kb * BK, b_r0);
-          }
-          __syncwarp();
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // =============================== MMA issuer =================================
-    constexpr uint32_t idesc = umma_idesc_f16(BM, BN, /*bf16*/ 1, 0, 0);
-    uint32_t it = 0;
-    uint32_t ti = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++ti) {
-      const uint32_t as = ti & 1;
-      const uint32_t aphase = (ti >> 1) & 1;
-      mbar_wait(smem_u32(&tempty_bar[as]), aphase ^ 1);
-      tc_fence_after();
-      uint32_t started = 0;  // bit a set once accumulator a has received its first MMA
-      for (int s = 0; s < p.num_segs; ++s) {
-        const int acc = p.segs[s].acc;
-        const uint32_t d_tmem = tmem_base + as * Cfg::ACC_COLS + acc * BN;
-        const int kblocks = (p.segs[s].k_len + BK - 1) / BK;
-        for (int kb = 0; kb < kblocks; ++kb, ++it) {
-          const uint32_t stage = it % Cfg::STAGES;
-          const uint32_t phase = (it / Cfg::STAGES) & 1;
-          mbar_wait(smem_u32(&full_bar[stage]), phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-          const uint64_t da = umma_desc_sw128(sa, 16, 1024);
-          const uint64_t db = umma_desc_sw128(sa + Cfg::A_BYTES, 16, 1024);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              // advancing 16 elements (32 bytes) along K inside the 128-byte swizzle atom
-              tc_mma_f16(d_tmem, da + 2 * k, db + 2 * k, idesc, ((started >> acc) & 1) | (k > 0));
-            }
-            tc_commit(smem_u32(&empty_bar[stage]));  // frees the smem slot when these MMAs retire
-          }
-          __syncwarp();
-          started |= 1u << acc;
-        }
-      }
-      if (elect_one()) tc_commit(smem_u32(&tfull_bar[as]));  // accumulators of this tile complete
-      __syncwarp();
-    }
-  } else if (warp >= 4) {
-    // =============================== epilogue ===================================
-    const int ew = warp - 4;  // == warp % 4: the TMEM lane quarter this warp may read
-    uint32_t ti = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++ti) {
-      const TileCoord t = decode_tile<BM>(p, tile);
-      const uint32_t as = ti & 1;
-      const uint32_t aphase = (ti >> 1) & 1;
-      mbar_wait(smem_u32(&tfull_bar[as]), aphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + as * Cfg::ACC_COLS;
-      epilogue_tile<BN, NACC, EPI>(p, t, taddr, t.n0 + ew * 32 + lane);
-      // release this accumulator stage back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&tempty_bar[as]));
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// CTA-pair kernel (cluster of 2, cta_group::2)
-// ------------------------------------------------------------------------------------------------
-template <int BN, int NACC>
-struct Gemm2Cfg {
-  static constexpr int A_BYTES = BM * BK * 2;            // this CTA's 128 rows
-  static constexpr int B_BYTES = (BN / 2) * BK * 2;      // this CTA's half of the B tile
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;  // multiple of 1024 for BN in {128, 176, 256}
-  static constexpr int EPI_WARPS = 8;                    // two per SM sub-partition (lane quarter x column half)
-  static constexpr int THREADS = (4 + EPI_WARPS) * 32;
-  static constexpr int STG_TOTAL = EPI_WARPS * 2 * STG_BYTES;   // 2 staging boxes per epilogue warp
-  static constexpr int STAGES = (160 * 1024) / STAGE_BYTES > 8 ? 8 : (160 * 1024) / STAGE_BYTES;
-  static constexpr int ACC_COLS = BN * NACC;
-  // accumulators are double-buffered across tiles when two sets fit the 512 TMEM columns; the 256-wide two-accumulator
-  // (wavenet) tile uses all 512 columns, so its epilogue and the next tile's MMAs take turns
-  static constexpr int ACC_STAGES = (2 * ACC_COLS <= 512) ? 2 : 1;
-  static constexpr int ACC_STRIDE = (ACC_STAGES == 1) ? 0 : ((ACC_COLS <= 128) ? 128 : 256);
-  static constexpr int TMEM_COLS = (ACC_STAGES == 1) ? 512 : 2 * ACC_STRIDE;
-  static constexpr int OFF_STG = STAGES * STAGE_BYTES;
-  static constexpr int OFF_BAR = OFF_STG + STG_TOTAL;
-  static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
-  static_assert(STAGE_BYTES % 1024 == 0, "stage must keep 1024-byte alignment of the swizzled tiles");
-  static_assert(ACC_COLS <= 512, "accumulators of one tile must fit the 512 TMEM columns");
-};
-
-template <int BN, int NACC, int EPI>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(Gemm2Cfg<BN, NACC>::THREADS, 1)
-    gemm2_kernel(const __grid_constant__ GemmDev p) {
-  using Cfg = Gemm2Cfg<BN, NACC>;
-  extern __shared__ uint8_t smem_raw[];
-  // identical carve-up in both CTAs of the pair (the dynamic smem base offset is the same for every CTA of a launch)
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
-  uint64_t* full_bar = bars;                          // [STAGES]  used in the leader CTA only
-  uint64_t* empty_bar = bars + Cfg::STAGES;           // [STAGES]  one per CTA, signalled by multicast commit
-  uint64_t* tfull_bar = bars + 2 * Cfg::STAGES;       // [2]       one per CTA, multicast commit
-  uint64_t* tempty_bar = bars + 2 * Cfg::STAGES + 2;  // [2]       leader only: 16 arrivals (8 warps x 2 CTAs)
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 2 * Cfg::STAGES + 4);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int pair = blockIdx.x >> 1;
-  const int num_pairs = gridDim.x >> 1;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&p.tmA);
-    tma_prefetch_desc(&p.tmB);
-    tma_prefetch_desc(&p.tmOut);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < Cfg::STAGES; ++i) {
-      mbar_init(smem_u32(&full_bar[i]), 1);
-      mbar_init(smem_u32(&empty_bar[i]), 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(&tfull_bar[i]), 1);
-      mbar_init(smem_u32(&tempty_bar[i]), 2 * Cfg::EPI_WARPS);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc_2cta(smem_u32(tmem_holder), Cfg::TMEM_COLS);
-  tc_fence_before();
-  __syncwarp();
-  cluster_sync_all();  // barriers of BOTH CTAs are initialised before any remote arrive / TMA signal
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
-
-  // register budget (setmaxnreg): the service warpgroup (TMA, MMA, TMEM allocator, one idle warp) gives registers to the
-  // two epilogue warpgroups, whose software-pipelined steps hold two sets of accumulator fragments
-  if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 80;");
-  if (warp == 0) {
-    // =============================== TMA producer (both CTAs; converged, see gemm_kernel) ===================
-    uint32_t it = 0;
-    for (int tile = pair; tile < p.num_tiles; tile += num_pairs) {
-      const TileCoord t = decode_tile<2 * BM>(p, tile);
-      const int dil = p.dil[t.g];
-      // a partial last n-tile is computed with N = bn_eff: each CTA then supplies bn_eff/2 B rows
-      const int bn_eff = (p.n - t.n_tile * BN) < BN ? (p.n - t.n_tile * BN) : BN;
-      const int b_r0 = t.g * p.b_grs + t.n_tile * BN + static_cast<int>(rank) * (bn_eff / 2);
-      for (int s = 0; s < p.num_segs; ++s) {
-        const ns2_gemm_seg sg = p.segs[s];
-        const int row0 = t.n0 + static_cast<int>(rank) * BM - sg.shift_units * dil;
-        const int a_c0 = t.g * p.a_gcs + sg.a_col_off;
-        const int kblocks = (sg.k_len + BK - 1) / BK;
-        for (int kb = 0; kb < kblocks; ++kb, ++it) {
-          const uint32_t stage = it % Cfg::STAGES;
-          const uint32_t phase = (it / Cfg::STAGES) & 1;
-          mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1);
-          if (elect_one()) {
-            // the transaction bytes of both CTAs are counted on the leader's barrier
-            const uint32_t fb_leader = mapa_shared(smem_u32(&full_bar[stage]), 0);
-            if (leader) mbar_arrive_expect_tx(smem_u32(&full_bar[stage]), 2 * Cfg::STAGE_BYTES);
-            uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-            tma_load_3d_2sm(smem_u32(sa), &p.tmA, fb_leader, a_c0 + kb * BK, row0, t.b);
-            tma_load_2d_2sm(smem_u32(sa + Cfg::A_BYTES), &p.tmB, fb_leader, sg.b_col_off + kb * BK, b_r0);
-          }
-          __syncwarp();
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // =============================== MMA issuer (leader CTA only; converged) ================
-    if (leader) {
-      uint32_t it = 0;
-      uint32_t ti = 0;
-      for (int tile = pair; tile < p.num_tiles; tile += num_pairs, ++ti) {
-        const int n_tile = decode_tile<2 * BM>(p, tile).n_tile;
-        const int bn_eff = (p.n - n_tile * BN) < BN ? (p.n - n_tile * BN) : BN;
-        const uint32_t idesc = umma_idesc_f16(2 * BM, bn_eff, /*bf16*/ 1, 0, 0);
-        const uint32_t as = (Cfg::ACC_STAGES == 2) ? (ti & 1) : 0;
-        const uint32_t aphase = (Cfg::ACC_STAGES == 2) ? ((ti >> 1) & 1) : (ti & 1);
-        if (lane == 0) NS2_GEMM_STAMP(0);
-        mbar_wait(smem_u32(&tempty_bar[as]), aphase ^ 1);
-        tc_fence_after();
-        if (lane == 0) NS2_GEMM_STAMP(1);
-        uint32_t started = 0;
-        for (int s = 0; s < p.num_segs; ++s) {
-          const int acc = p.segs[s].acc;
-          const uint32_t d_tmem = tmem_base + as * Cfg::ACC_STRIDE + acc * BN;
-          const int kblocks = (p.segs[s].k_len + BK - 1) / BK;
-          for (int kb = 0; kb < kblocks; ++kb, ++it) {
-            const uint32_t stage = it % Cfg::STAGES;
-            const uint32_t phase = (it / Cfg::STAGES) & 1;
-            mbar_wait(smem_u32(&full_bar[stage]), phase);
-            tc_fence_after();
-            const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-            const uint64_t da = umma_desc_sw128(sa, 16, 1024);
-            const uint64_t db = umma_desc_sw128(sa + Cfg::A_BYTES, 16, 1024);
-            if (elect_one()) {
-#pragma unroll
-              for (int k = 0; k < BK / 16; ++k)
-                tc_mma_f16_2cta(d_tmem, da + 2 * k, db + 2 * k, idesc, ((started >> acc) & 1) | (k > 0));
-              tc_commit_2cta(smem_u32(&empty_bar[stage]), 0b11);  // frees the slot in both CTAs
-            }
-            __syncwarp();
-            started |= 1u << acc;
-          }
-        }
-        if (elect_one()) tc_commit_2cta(smem_u32(&tfull_bar[as]), 0b11);  // both CTAs' epilogues may read their rows
-        __syncwarp();
-        if (lane == 0) NS2_GEMM_STAMP(2);
-      }
-    }
-  }
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 208;");
-    // =============================== epilogue (both CTAs, 8 warps each) =======================
-    const int ew = warp - 4;
-    const int quarter = ew & 3;   // == warp % 4: the TMEM lane quarter this warp may read
-    const int hsel = ew >> 2;     // column half of the tile
-    Stager st;
-    st.base = smem_u32(smem + Cfg::OFF_STG + ew * 2 * STG_BYTES);
-    st.count = 0;
-    st.lane = lane;
-    uint32_t ti = 0;
-    for (int tile = pair; tile < p.num_tiles; tile += num_pairs, ++ti) {
-      const TileCoord t = decode_tile<2 * BM>(p, tile);
-      const uint32_t as = (Cfg::ACC_STAGES == 2) ? (ti & 1) : 0;
-      const uint32_t aphase = (Cfg::ACC_STAGES == 2) ? ((ti >> 1) & 1) : (ti & 1);
-      if (ew == 0 && lane == 0) NS2_GEMM_STAMP(3);
-      if (ew == 7 && lane == 0) NS2_GEMM_STAMP(6);
-      mbar_wait(smem_u32(&tfull_bar[as]), aphase);
-      tc_fence_after();
-      if (ew == 0 && lane == 0) NS2_GEMM_STAMP(4);
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + as * Cfg::ACC_STRIDE;
-      if (!p.skip_epilogue)
-        epilogue_tile_tma8<BN, NACC, EPI>(p, t, taddr, t.n0 + static_cast<int>(rank) * BM + quarter * 32, hsel, st);
-      // all TMEM reads of this tile are complete: hand the accumulator stage back to the leader's MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(mapa_shared(smem_u32(&tempty_bar[as]), 0));
-      if (ew == 0 && lane == 0) NS2_GEMM_STAMP(5);
-      if (ew == 7 && lane == 0) NS2_GEMM_STAMP(7);
-    }
-    if (elect_one()) tma_store_wait_all();  // staging smem must outlive the bulk stores that read it
-    __syncwarp();
-  }
-
-  // neither CTA may free TMEM / exit while its peer can still touch it (MMA writes, remote barrier arrives)
-  tc_fence_before();
-  __syncwarp();  // the cluster barrier is .aligned: every warp must be converged when it executes it
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2cta(tmem_base, Cfg::TMEM_COLS);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Wavenet residual block on CTA pairs, TWO-PASS accumulator (gemm2w_kernel).
-// y = tanh(z) sigmoid(z) + res(x),  z = (conv3(x) + b0) * gamma + beta   (ns2.py:619-636)
-// gemm2_kernel keeps conv3(x) and res(x) in two 256-column accumulators, i.e. all 512 TMEM columns: the epilogue
-// and the next tile's MMAs take turns (1.9 ms vs 1.45 ms mainloop-only per step).  Here one 256-column accumulator
-// serves both: phase 1 accumulates conv3(x); epilogue pass 1 replaces it IN TENSOR MEMORY by the gate value
-// (tcgen05.ld -> gate -> tcgen05.st); phase 2 accumulates res(x) on top; pass 2 adds the residual bias and stores
-// bf16.  Two accumulator stages fit, and tiles go through the pipeline in pairs (a, b):
-//     MMA:       P1(a)  P1(b)            P2(a)        P2(b)         P1(a') ...
-//     epilogue:         pass1(a)  pass1(b)     pass2(a)      pass2(b)
-// so every epilogue pass runs under MMAs of the other stage.
-// ------------------------------------------------------------------------------------------------
-template <int DUMMY>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(Gemm2Cfg<256, 1>::THREADS, 1)
-    gemm2w_kernel(const __grid_constant__ GemmDev p) {
-  using Cfg = Gemm2Cfg<256, 1>;
-  constexpr int BN = 256;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
-  uint64_t* full_bar = bars;                           // [STAGES]  leader only
-  uint64_t* empty_bar = bars + Cfg::STAGES;            // [STAGES]  one per CTA, multicast commit
-  uint64_t* tfull1_bar = bars + 2 * Cfg::STAGES;       // [2] phase 1 complete (per CTA, multicast commit)
-  uint64_t* tfull2_bar = tfull1_bar + 2;               // [2] phase 2 complete
-  uint64_t* gready_bar = tfull2_bar + 2;               // [2] leader only: gate values are in TMEM (16 arrivals)
-  uint64_t* tempty_bar = gready_bar + 2;               // [2] leader only: accumulator stage drained (16 arrivals)
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int pair = blockIdx.x >> 1;
-  const int num_pairs = gridDim.x >> 1;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&p.tmA);
-    tma_prefetch_desc(&p.tmB);
-    tma_prefetch_desc(&p.tmOut);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < Cfg::STAGES; ++i) {
-      mbar_init(smem_u32(&full_bar[i]), 1);
-      mbar_init(smem_u32(&empty_bar[i]), 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(&tfull1_bar[i]), 1);
-      mbar_init(smem_u32(&tfull2_bar[i]), 1);
-      mbar_init(smem_u32(&gready_bar[i]), 2 * Cfg::EPI_WARPS);
-      mbar_init(smem_u32(&tempty_bar[i]), 2 * Cfg::EPI_WARPS);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc_2cta(smem_u32(tmem_holder), 512);
-  tc_fence_before();
-  __syncwarp();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
 
   if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 80;");
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (warp == 0) {
-      // =============================== TMA producer (both CTAs; converged) ===================
+      // =============================== TMA producer (converged, one elected lane issues) ===============================
       uint32_t it = 0;
-      auto load_phase = [&](int tile, int want_acc) {
-        const TileCoord t = decode_tile<2 * BM>(p, tile);
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        const TileCoord t = decode_tile(p, tile);
         const int dil = p.dil[t.g];
-        const int bn_eff = (p.n - t.n_tile * BN) < BN ? (p.n - t.n_tile * BN) : BN;
-        const int b_r0 = t.g * p.b_grs + t.n_tile * BN + static_cast<int>(rank) * (bn_eff / 2);
         for (int s = 0; s < p.num_segs; ++s) {
           const ns2_gemm_seg sg = p.segs[s];
-          if (sg.acc != want_acc) continue;
-          const int row0 = t.n0 + static_cast<int>(rank) * BM - sg.shift_units * dil;
+          const int row0 = t.n0 - sg.shift_units * dil;
           const int a_c0 = t.g * p.a_gcs + sg.a_col_off;
+          const int b_r0 = t.g * p.b_grs + t.n_tile * BN;
           const int kblocks = (sg.k_len + BK - 1) / BK;
           for (int kb = 0; kb < kblocks; ++kb, ++it) {
             const uint32_t stage = it % Cfg::STAGES;
             const uint32_t phase = (it / Cfg::STAGES) & 1;
             mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1);
             if (elect_one()) {
-              const uint32_t fb_leader = mapa_shared(smem_u32(&full_bar[stage]), 0);
-              if (leader) mbar_arrive_expect_tx(smem_u32(&full_bar[stage]), 2 * Cfg::STAGE_BYTES);
+              const uint32_t fb = smem_u32(&full_bar[stage]);
+              mbar_arrive_expect_tx(fb, Cfg::STAGE_BYTES);
               uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-              tma_load_3d_2sm(smem_u32(sa), &p.tmA, fb_leader, a_c0 + kb * BK, row0, t.b);
-              tma_load_2d_2sm(smem_u32(sa + Cfg::A_BYTES), &p.tmB, fb_leader, sg.b_col_off + kb * BK, b_r0);
+              tma_load_3d(smem_u32(sa), &p.tmA, fb, a_c0 + kb * BK, row0, t.b);
+              tma_load_2d(smem_u32(sa + Cfg::A_BYTES), &p.tmB, fb, sg.b_col_off + kb * BK, b_r0);
             }
-            __syncwarp();
-          }
-        }
-      };
-      for (int t0 = pair; t0 < p.num_tiles; t0 += 2 * num_pairs) {
-        const int t1 = t0 + num_pairs;
-        const bool has1 = t1 < p.num_tiles;
-        load_phase(t0, 0);
-        if (has1) load_phase(t1, 0);
-        load_phase(t0, 1);
-        if (has1) load_phase(t1, 1);
-      }
-    } else if (warp == 1) {
-      // =============================== MMA issuer (leader CTA only; converged) ================
-      if (leader) {
-        uint32_t it = 0, grp = 0;
-        auto mma_phase = [&](int tile, int want_acc, uint32_t d_tmem) {
-          const int n_tile = decode_tile<2 * BM>(p, tile).n_tile;
-          const int bn_eff = (p.n - n_tile * BN) < BN ? (p.n - n_tile * BN) : BN;
-          const uint32_t idesc = umma_idesc_f16(2 * BM, bn_eff, /*bf16*/ 1, 0, 0);
-          uint32_t started = want_acc;   // phase 2 accumulates on top of the gate values from its first MMA on
-          for (int s = 0; s < p.num_segs; ++s) {
-            if (p.segs[s].acc != want_acc) continue;
-            const int kblocks = (p.segs[s].k_len + BK - 1) / BK;
-            for (int kb = 0; kb < kblocks; ++kb, ++it) {
-              const uint32_t stage = it % Cfg::STAGES;
-              const uint32_t phase = (it / Cfg::STAGES) & 1;
-              mbar_wait(smem_u32(&full_bar[stage]), phase);
-              tc_fence_after();
-              const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-              const uint64_t da = umma_desc_sw128(sa, 16, 1024);
-              const uint64_t db = umma_desc_sw128(sa + Cfg::A_BYTES, 16, 1024);
-              if (elect_one()) {
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k)
-                  tc_mma_f16_2cta(d_tmem, da + 2 * k, db + 2 * k, idesc, started | (k > 0));
-                tc_commit_2cta(smem_u32(&empty_bar[stage]), 0b11);
-              }
-              __syncwarp();
-              started = 1;
-            }
-          }
-        };
-        for (int t0 = pair; t0 < p.num_tiles; t0 += 2 * num_pairs, ++grp) {
-          const int t1 = t0 + num_pairs;
-          const bool has1 = t1 < p.num_tiles;
-          const uint32_t ph = grp & 1;
-          mbar_wait(smem_u32(&tempty_bar[0]), ph ^ 1);
-          tc_fence_after();
-          mma_phase(t0, 0, tmem_base);
-          if (elect_one()) tc_commit_2cta(smem_u32(&tfull1_bar[0]), 0b11);
-          __syncwarp();
-          if (has1) {
-            mbar_wait(smem_u32(&tempty_bar[1]), ph ^ 1);
-            tc_fence_after();
-            mma_phase(t1, 0, tmem_base + 256);
-            if (elect_one()) tc_commit_2cta(smem_u32(&tfull1_bar[1]), 0b11);
-            __syncwarp();
-          }
-          mbar_wait(smem_u32(&gready_bar[0]), ph);
-          tc_fence_after();
-          mma_phase(t0, 1, tmem_base);
-          if (elect_one()) tc_commit_2cta(smem_u32(&tfull2_bar[0]), 0b11);
-          __syncwarp();
-          if (has1) {
-            mbar_wait(smem_u32(&gready_bar[1]), ph);
-            tc_fence_after();
-            mma_phase(t1, 1, tmem_base + 256);
-            if (elect_one()) tc_commit_2cta(smem_u32(&tfull2_bar[1]), 0b11);
             __syncwarp();
           }
         }
       }
     }
   } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 208;");
-    // =============================== epilogue (both CTAs, 8 warps each) =======================
-    const int ew = warp - 4;
-    const int quarter = ew & 3;
-    const int hsel = ew >> 2;
-    Stager st;
-    st.base = smem_u32(smem + Cfg::OFF_STG + ew * 2 * STG_BYTES);
-    st.count = 0;
-    st.lane = lane;
-    const uint32_t lane_base = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    // pass 1: accumulator -> gate value, in place.  This warp owns columns [128 hsel, 128 hsel + 128) of its 32 rows.
-    auto pass1 = [&](int tile, uint32_t taddr) {
-      const TileCoord t = decode_tile<2 * BM>(p, tile);
-      const int tile_col0 = t.n_tile * BN;
-      uint32_t ra[2][32];
-      tmem_ld32(taddr + hsel * 128, ra[0]);
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    // =============================== consumers: wgmma mainloop + epilogue ===============================
+    const int cw = (warp >> 2) - 1;   // consumer warpgroup: rows [64 cw, 64 cw + 64) of the tile
+    const int ww = warp & 3;
+    float acc[NACC][BN / 2];
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      const TileCoord t = decode_tile(p, tile);
 #pragma unroll
-      for (int s = 0; s < 4; ++s) {
-        const int buf = s & 1;
-        const int c = hsel * 128 + s * 32;
-        tmem_ld_wait();
-        if (s + 1 < 4) tmem_ld32(taddr + c + 32, ra[buf ^ 1]);
-        if (tile_col0 + c < p.n) {   // a partial last n-tile is narrower (n is a multiple of 32)
-          const int col0 = tile_col0 + c;
-          const float4* b04 = reinterpret_cast<const float4*>(p.bias + t.g * p.b_grs + col0);
-          const float4* ga4 = reinterpret_cast<const float4*>(p.film + t.b * p.film_bs + t.g * p.film_gs + col0);
-          const float4* be4 = reinterpret_cast<const float4*>(p.film + t.b * p.film_bs + t.g * p.film_gs + col0 + p.n);
-          uint32_t gv[32];
+      for (int a = 0; a < NACC; ++a)
 #pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const float4 b0 = __ldg(b04 + q), g4 = __ldg(ga4 + q), e4 = __ldg(be4 + q);
-            const float b0a[4] = {b0.x, b0.y, b0.z, b0.w};
-            const float gaa[4] = {g4.x, g4.y, g4.z, g4.w}, bea[4] = {e4.x, e4.y, e4.z, e4.w};
+        for (int i = 0; i < BN / 2; ++i) acc[a][i] = 0.f;
+      int prev_stage = -1;
+      for (int s = 0; s < p.num_segs; ++s) {
+        const int sel = p.segs[s].acc;
+        const int kblocks = (p.segs[s].k_len + BK - 1) / BK;
+        for (int kb = 0; kb < kblocks; ++kb, ++it) {
+          const uint32_t stage = it % Cfg::STAGES;
+          const uint32_t phase = (it / Cfg::STAGES) & 1;
+          mbar_wait(smem_u32(&full_bar[stage]), phase);
+          const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
+          const uint64_t da = gmma_desc_sw128(sa + cw * (64 * 128), 16, 1024);
+          const uint64_t db = gmma_desc_sw128(sa + Cfg::A_BYTES, 16, 1024);
+          wgmma_fence();
+          if (NACC == 1 || sel == 0) {
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const int i = 4 * q + j;
-              const float z = fmaf(__uint_as_float(ra[buf][i]) + b0a[j], gaa[j], bea[j]);
-              // tanh(z) * sigmoid(z) with ONE MUFU: u = tanh(z/2); sigmoid = (1 + u)/2; tanh(z) = 2u / (1 + u^2), the
-              // reciprocal of w = 1 + u^2 in [1, 2] by a linear seed + two Newton steps (rel. err < 2e-5)
-              const float u = tanh_fast(0.5f * z);
-              const float w = fmaf(u, u, 1.0f);
-              float r = fmaf(-0.47058824f, w, 1.4117647f);
-              r = r * fmaf(-w, r, 2.0f);
-              r = r * fmaf(-w, r, 2.0f);
-              gv[i] = __float_as_uint((u * r) * (1.0f + u));
-            }
+            for (int k = 0; k < BK / 16; ++k) wgmma_tile_k16<BN>(acc[0], da + 2 * k, db + 2 * k);
+          } else {
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k) wgmma_tile_k16<BN>(acc[NACC - 1], da + 2 * k, db + 2 * k);
           }
-          tmem_st32(taddr + c, gv);
+          wgmma_commit();
+          // the previous k-block's MMAs have retired: its smem slot goes back to the producer
+          wgmma_wait<1>();
+          if (prev_stage >= 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev_stage]));
+          prev_stage = static_cast<int>(stage);
         }
       }
-      tmem_st_wait();
-    };
-    uint32_t grp = 0;
-    for (int t0 = pair; t0 < p.num_tiles; t0 += 2 * num_pairs, ++grp) {
-      const int t1 = t0 + num_pairs;
-      const bool has1 = t1 < p.num_tiles;
-      const uint32_t ph = grp & 1;
-      for (int x = 0; x < (has1 ? 2 : 1); ++x) {
-        mbar_wait(smem_u32(&tfull1_bar[x]), ph);
-        tc_fence_after();
-        if (!p.skip_epilogue) pass1(x ? t1 : t0, lane_base + x * 256);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(mapa_shared(smem_u32(&gready_bar[x]), 0));
-      }
-      for (int x = 0; x < (has1 ? 2 : 1); ++x) {
-        const TileCoord t = decode_tile<2 * BM>(p, x ? t1 : t0);
-        mbar_wait(smem_u32(&tfull2_bar[x]), ph);
-        tc_fence_after();
-        // pass 2: gate + res(x) is in the accumulator: + residual bias -> bf16 -> TMA store
-        if (!p.skip_epilogue)
-          epilogue_tile_tma8<BN, 1, NS2_EPI_BF16>(p, t, lane_base + x * 256,
-                                                  t.n0 + static_cast<int>(rank) * BM + quarter * 32, hsel, st, p.bias1_off);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(mapa_shared(smem_u32(&tempty_bar[x]), 0));
-      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int a = 0; a < NACC; ++a) wgmma_hold(acc[a]);
+      if (prev_stage >= 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev_stage]));
+      if (!p.skip_epilogue)
+        epilogue_tile<BN, NACC, EPI>(p, t, acc, t.n0 + cw * 64 + ww * 16 + (lane >> 2), 2 * (lane & 3));
     }
-    if (elect_one()) tma_store_wait_all();
-    __syncwarp();
-  }
-
-  tc_fence_before();
-  __syncwarp();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2cta(tmem_base, 512);
   }
 }
 
@@ -1127,32 +298,7 @@ static int launch_gemm(const GemmDev& dev, cudaStream_t stream) {
   auto kern = gemm_kernel<BN, NACC, EPI>;
   NS2_CUDA_CHECK(set_max_smem_once(kern, Cfg::SMEM_BYTES));
   const int grid = dev.num_tiles < num_sms() ? dev.num_tiles : num_sms();
-  kern<<<grid, 256, Cfg::SMEM_BYTES, stream>>>(dev);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
-}
-
-template <int BN, int NACC, int EPI>
-static int launch_gemm2(const GemmDev& dev, cudaStream_t stream) {
-  using Cfg = Gemm2Cfg<BN, NACC>;
-  auto kern = gemm2_kernel<BN, NACC, EPI>;
-  NS2_CUDA_CHECK(set_max_smem_once(kern, Cfg::SMEM_BYTES));
-  int pairs = num_sms() / 2;
-  if (dev.num_tiles < pairs) pairs = dev.num_tiles;
-  kern<<<2 * pairs, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(dev);  // __cluster_dims__(2,1,1)
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
-}
-
-static int launch_gemm2w(const GemmDev& dev, cudaStream_t stream) {
-  using Cfg = Gemm2Cfg<256, 1>;
-  auto kern = gemm2w_kernel<0>;
-  NS2_CUDA_CHECK(set_max_smem_once(kern, Cfg::SMEM_BYTES));
-  int pairs = num_sms() / 2;
-  if (dev.num_tiles < pairs) pairs = dev.num_tiles;
-  kern<<<2 * pairs, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(dev);  // __cluster_dims__(2,1,1)
+  kern<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(dev);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   NS2_CUDA_CHECK(cudaGetLastError());
   return kOk;
@@ -1203,21 +349,11 @@ extern "C" int ns2_gemm(const ns2_gemm_args* a, ns2_stream_t stream_) {
     NS2_REQUIRE(a->resid_row_stride % 4 == 0 && (reinterpret_cast<uintptr_t>(a->resid) & 15) == 0,
                 "ns2_gemm: resid must be 16-byte aligned");
 
-  // ---- kernel / tile selection ----
-  const int n_out = (a->epilogue == NS2_EPI_GEGLU) ? a->n / 2 : a->n;
-  const bool out_f32 = a->epilogue == NS2_EPI_F32;
-  // CTA pairs need > 128 positions per batch to fill both halves; their TMA-store epilogue needs whole 128-byte
-  // column chunks and can only fold a residual that aliases the output (reduce-add)
-  bool pair = a->a_rows > BM;
-  if (!out_f32 && n_out % 64 != 0) pair = false;
-  if (out_f32 && a->resid != nullptr && a->resid != a->out) pair = false;
-  if (out_f32 && a->resid != nullptr && a->resid_row_stride != a->out_row_stride) pair = false;
+  // ---- tile selection ----
   int bn;
-  if (a->epilogue == NS2_EPI_WAVENET) bn = (pair && a->n % 256 == 0) ? 256 : 128;
-  else if (a->epilogue == NS2_EPI_GEGLU) bn = 256;
-  else if (pair) bn = a->n >= 256 ? 256 : 128;
-  else bn = (a->n % 256 == 0 && a->n >= 1024) ? 256 : 128;
-  const int tile_rows = pair ? 2 * BM : BM;
+  if (a->epilogue == NS2_EPI_WAVENET) bn = 128;      // two 64-register accumulator fragments per thread
+  else if (a->epilogue == NS2_EPI_GEGLU) bn = 256;   // 128 value + 128 gate columns
+  else bn = a->n >= 256 ? 256 : 128;
 
   GemmDev dev;
   memset(&dev, 0, sizeof(dev));
@@ -1231,27 +367,15 @@ extern "C" int ns2_gemm(const ns2_gemm_args* a, ns2_stream_t stream_) {
   {
     const uint64_t dims[2] = {(uint64_t)a->b_cols, (uint64_t)a->b_rows};
     const uint64_t strides[2] = {2, (uint64_t)a->b_row_stride * 2};
-    const uint32_t box[2] = {BK, (uint32_t)(pair ? bn / 2 : bn)};
+    const uint32_t box[2] = {BK, (uint32_t)bn};
     int rc = make_tmap_16bit(&dev.tmB, a->B, 2, dims, strides, box);
     if (rc != kOk) return rc;
   }
-  if (pair) {
-    const uint64_t es = out_f32 ? 4 : 2;
-    const uint64_t dims[3] = {(uint64_t)(a->groups - 1) * a->out_group_col_stride + n_out, (uint64_t)a->a_rows,
-                              (uint64_t)a->a_batches};
-    const uint64_t strides[3] = {es, (uint64_t)a->out_row_stride * es,
-                                 (uint64_t)a->a_rows * a->out_row_stride * es};
-    const uint32_t box[3] = {(uint32_t)(128 / es), 32, 1};
-    int rc = out_f32 ? make_tmap_f32(&dev.tmOut, a->out, 3, dims, strides, box)
-                     : make_tmap_16bit(&dev.tmOut, a->out, 3, dims, strides, box);
-    if (rc != kOk) return rc;
-    dev.reduce_add = (out_f32 && a->resid != nullptr) ? 1 : 0;
-  }
   dev.tiles_n = (a->n + bn - 1) / bn;
-  dev.tiles_per_batch = (a->a_rows + tile_rows - 1) / tile_rows;
+  dev.tiles_per_batch = (a->a_rows + BM - 1) / BM;
   dev.tiles_m = dev.tiles_per_batch * a->a_batches;
   dev.num_tiles = dev.tiles_m * dev.tiles_n * a->groups;
-  dev.narrow_last = ((a->flags & NS2_GEMM_FLAG_NARROW_LAST) && pair && a->groups == 1 && dev.tiles_n > 1 && a->n % bn != 0) ? 1 : 0;
+  dev.narrow_last = ((a->flags & NS2_GEMM_FLAG_NARROW_LAST) && a->groups == 1 && dev.tiles_n > 1 && a->n % bn != 0) ? 1 : 0;
   dev.a_rows = a->a_rows;
   dev.n = a->n;
   dev.groups = a->groups;
@@ -1274,28 +398,7 @@ extern "C" int ns2_gemm(const ns2_gemm_args* a, ns2_stream_t stream_) {
   NS2_REQUIRE(dev.act == 0 || a->epilogue == NS2_EPI_BF16 || a->epilogue == NS2_EPI_F32,
               "ns2_gemm: NS2_GEMM_FLAG_SILU only applies to the BF16 / F32 epilogues");
   dev.skip_epilogue = (a->flags & NS2_GEMM_FLAG_SKIP_EPILOGUE) ? 1 : 0;
-  dev.timeline = reinterpret_cast<long long*>(a->debug_timeline);
 
-  if (pair) {
-    switch (a->epilogue) {
-      case NS2_EPI_BF16:
-        return bn == 256 ? launch_gemm2<256, 1, NS2_EPI_BF16>(dev, stream)
-                         : launch_gemm2<128, 1, NS2_EPI_BF16>(dev, stream);
-      case NS2_EPI_F32:
-        return bn == 256 ? launch_gemm2<256, 1, NS2_EPI_F32>(dev, stream)
-                         : launch_gemm2<128, 1, NS2_EPI_F32>(dev, stream);
-      case NS2_EPI_GEGLU:
-        return launch_gemm2<256, 1, NS2_EPI_GEGLU>(dev, stream);
-      case NS2_EPI_WAVENET:
-        // 256-wide tiles: the two-pass single-accumulator kernel (epilogue fully under the MMAs) unless the caller
-        // asks for the two-accumulator tile (A/B measurements)
-        if (bn == 256 && !(a->flags & NS2_GEMM_FLAG_WAVENET_ONE_PASS)) return launch_gemm2w(dev, stream);
-        return bn == 256 ? launch_gemm2<256, 2, NS2_EPI_WAVENET>(dev, stream)
-                         : launch_gemm2<128, 2, NS2_EPI_WAVENET>(dev, stream);
-      default:
-        return set_error(kErrInvalidArg, "ns2_gemm: unknown epilogue %d", a->epilogue);
-    }
-  }
   switch (a->epilogue) {
     case NS2_EPI_BF16:
       return bn == 256 ? launch_gemm<256, 1, NS2_EPI_BF16>(dev, stream)

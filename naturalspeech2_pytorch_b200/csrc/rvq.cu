@@ -1,10 +1,10 @@
-// Residual vector quantisation (Encodec RVQ encode / decode) for sm_100a.
+// Residual vector quantisation (Encodec RVQ encode / decode) for sm_90a.
 //
 // Reference behaviour (third-party code behind audiolm_pytorch.EncodecWrapper, reached from ns2.py:1445,1611;
 // restated in oracle/rvq_oracle.py from encodec's EuclideanCodebook.quantize + ResidualVectorQuantization):
 //   for q in 0..Q-1:  idx = argmin_k ||r - C_q[k]||^2 (first minimum wins);  r -= C_q[idx]
 //
-// The distance contraction runs on tcgen05 tensor cores in fp16 (fp32 accumulate) as a *filter*:
+// The distance contraction runs on the tensor cores (wgmma) in fp16 (fp32 accumulate) as a *filter*:
 //   s~_k = ||c_k||^2 - 2 r.c_k     with a rigorous bound |s~_k - s_k| <= E = 2 * 1.05 * 2^-10 * ||r|| * max_k ||c_k|| + ...
 // The whole score comes out of the tensor core: besides the 128 latent dims the MMA contracts one extra K block that
 // carries ||c_k||^2 (split into an fp16 hi/lo pair, prepared once per codebook) against a per-row power of two, so
@@ -14,13 +14,15 @@
 // (ties -> lowest index) — bit-exact against the fp64 oracle — while >99% of the flops stay on tensor cores.
 //
 // One CTA per 128 frames, 320 threads:
-//   warps 0-7  scan threads: two threads per frame (TMEM lane), each scanning 64 of every 128 score columns with a
-//              branch-free top-4 on packed (score|index) keys; fp32 residuals live in padded shared memory for all
-//              Q stages; the same threads build the fp16 A tile, re-score near-ties in fp64 (per lane, or
-//              warp-cooperatively for crowded 32-code blocks / bands) and subtract the chosen fp32 codeword
+//   warps 0-7  scan threads = two warpgroups; warpgroup w computes D[64 frames x 128 codes] per chunk with 8 + 1
+//              wgmma m64n128k16 into registers.  The prepared fp16 codebook stores the codes of every 128-code chunk
+//              permuted (see rvq_perm) so that each thread's accumulator columns are one contiguous 32-code block for
+//              each of its two frames; it scans them with a branch-free top-2 on packed (score|index) keys.  fp32
+//              residuals live in padded shared memory for all Q stages; the same threads build the fp16 A tile,
+//              re-score near-ties in fp64 (per lane, or warp-cooperatively for crowded 32-code blocks / bands) and
+//              subtract the chosen fp32 codeword
 //   warp 8     TMA producer: streams the fp16 codebooks (128 codes x 128 dims + the 4 KB norm block per chunk) through
 //              a 3-deep ring
-//   warp 9     tcgen05.mma issuer: D[128 frames x 128 codes] per chunk (8 + 1 MMAs), double-buffered in TMEM
 #include "ptx.cuh"
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
@@ -43,7 +45,7 @@ constexpr int MAX_K = 2048;
 constexpr int OFF_A = 0;
 constexpr int OFF_B = OFF_A + A_BYTES;
 constexpr int X_BYTES = 4096;         // norm block of one chunk / of the A tile: [16 row groups][2 K halves][8 rows][8 fp16]
-                                      // = the canonical un-swizzled K-major UMMA layout (SBO 256 B, LBO 128 B)
+                                      // = the canonical un-swizzled K-major GMMA layout (SBO 256 B, LBO 128 B)
 constexpr int OFF_BX = OFF_B + RING * B_BYTES;       // norm blocks of the ring stages
 constexpr int OFF_AX = OFF_BX + RING * X_BYTES;      // per-row power of two (K half 0, elements 0 and 1), rest zero
 constexpr int OFF_R = OFF_AX + X_BYTES;              // fp32 residuals, row-major padded: 67.6 KB
@@ -55,8 +57,7 @@ constexpr int OFF_BAR = OFF_CAND + (4 + BF) * 4;     // queue of ambiguous rows:
 constexpr int OFF_META = OFF_BAR + 256;             // per-stage {max ||c||, 2^e} of the first 32 stages
 constexpr int OFF_TL = OFF_META + 256;               // bring-up timeline of CTA 0: 32 stages x 8 clock64 stamps
 constexpr int SMEM_BYTES = OFF_TL + 2048;
-constexpr int TMEM_COLS = 256;
-constexpr int SCAN_THREADS = 256;     // warps 0-7: quarter = warp & 3 (TMEM lanes), column half = warp >> 2
+constexpr int SCAN_THREADS = 256;     // warps 0-7: quarter = warp & 3, column half = warp >> 2 (A tile / residual rows)
 }  // namespace rvq
 
 struct RvqDev {
@@ -176,6 +177,11 @@ __device__ __forceinline__ void warp_argmin(double& d, int& k) {
   }
 }
 
+// Column n of a prepared 128-code chunk holds code rvq_perm(n) of the chunk: accumulator column 8j + 2c + k (fragment
+// element 4j + k of the thread with lane % 4 == c) is code 32c + 2j + k, so thread c of a quad sees codes [32c, 32c+32).
+__host__ __device__ __forceinline__ int rvq_perm(int n) { return ((n >> 1) & 3) * 32 + (n >> 3) * 2 + (n & 1); }
+__host__ __device__ __forceinline__ int rvq_perm_inv(int m) { return ((m & 31) >> 1) * 8 + (m >> 5) * 2 + (m & 1); }
+
 // Approximate scores are carried as "keys": the fp32 score with its low mantissa bits replaced by the code index,
 // so that min/max on the keys sorts (score, index) pairs without branches or separate index registers.
 // Low 11 bits = index (K <= 2048); the 2^-12 relative truncation is folded into the re-score margin.
@@ -197,11 +203,7 @@ __global__ void __launch_bounds__(320, 1) rvq_encode_kernel(const __grid_constan
                                                                    // stores inside the measured phases
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* b_full = bars + 0;    // [RING]
-  uint64_t* b_empty = bars + 3;   // [RING]
-  uint64_t* a_full = bars + 6;    // scan threads -> MMA: A tile of this stage written
-  uint64_t* d_full = bars + 7;    // [2]
-  uint64_t* d_empty = bars + 9;   // [2]
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 11);
+  uint64_t* b_empty = bars + 3;   // [RING] one arrive per scan warp
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long f0 = static_cast<long long>(blockIdx.x) * BF;
@@ -211,20 +213,11 @@ __global__ void __launch_bounds__(320, 1) rvq_encode_kernel(const __grid_constan
   if (warp == 9 && lane == 0) {
     for (int i = 0; i < RING; ++i) {
       mbar_init(smem_u32(&b_full[i]), 1);
-      mbar_init(smem_u32(&b_empty[i]), 1);
-    }
-    mbar_init(smem_u32(a_full), SCAN_THREADS);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(&d_full[i]), 1);
-      mbar_init(smem_u32(&d_empty[i]), SCAN_THREADS);
+      mbar_init(smem_u32(&b_empty[i]), 8);
     }
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc(smem_u32(tmem_holder), TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
 
   if (warp == 8) {
     // ================================ TMA producer ================================
@@ -245,41 +238,13 @@ __global__ void __launch_bounds__(320, 1) rvq_encode_kernel(const __grid_constan
         }
       }
     }
-  } else if (warp == 9) {
-    // ================================ MMA issuer ==================================
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(BF, BC, /*fp16*/ 0, 0, 0);
-      const uint32_t abase = smem_u32(smem + OFF_A);
-      uint32_t it = 0;
-      for (int q = 0; q < p.Q; ++q) {
-        mbar_wait_backoff(smem_u32(a_full), q & 1, 100);
-        tc_fence_after();
-        for (int c = 0; c < chunks; ++c, ++it) {
-          const uint32_t st = it % RING, ph = (it / RING) & 1;
-          const uint32_t buf = it & 1, dph = (it >> 1) & 1;
-          mbar_wait(smem_u32(&b_full[st]), ph);
-          mbar_wait(smem_u32(&d_empty[buf]), dph ^ 1);
-          tc_fence_after();
-          const uint32_t bbase = smem_u32(smem + OFF_B + st * B_BYTES);
-#pragma unroll
-          for (int k = 0; k < D / 16; ++k) {
-            const uint32_t off = (k >> 2) * (128 * 128) + (k & 3) * 32;  // atom, 16-dim step inside it
-            tc_mma_f16(tmem_base + buf * BC, umma_desc_sw128(abase + off, 16, 1024),
-                       umma_desc_sw128(bbase + off, 16, 1024), idesc, k > 0);
-          }
-          // + 2^(e-ex+6) * (hi_k + lo_k) = ||c_k||^2 * 2^-(e+ex+1): the norm term of the score
-          tc_mma_f16(tmem_base + buf * BC, umma_desc_plain(smem_u32(smem + OFF_AX), 128, 256),
-                     umma_desc_plain(smem_u32(smem + OFF_BX + st * X_BYTES), 128, 256), idesc, 1);
-          tc_commit(smem_u32(&b_empty[st]));
-          tc_commit(smem_u32(&d_full[buf]));
-        }
-      }
-    }
-  } else {
+  } else if (warp < 8) {
     // ================================ scan threads ================================
     const int quarter = warp & 3, half = warp >> 2;
     const int row = quarter * 32 + lane;       // frame owned (together with the thread of the other half)
-    const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
+    const int wgi = warp >> 2;                 // warpgroup: accumulator rows [64 wgi, 64 wgi + 64)
+    const int frow = 64 * wgi + 16 * quarter + (lane >> 2);   // accumulator rows of this thread: frow, frow + 8
+    const int qc = lane & 3;                                  // 32-code block of every chunk this thread scans
 
     float* rrow = R + row * RSTRIDE;
     // cooperative, coalesced load of the 128 frames: warp w fills rows [16w, 16w+16)
@@ -356,20 +321,20 @@ __global__ void __launch_bounds__(320, 1) rvq_encode_kernel(const __grid_constan
         }
       }
       fence_proxy_async_smem();
-      mbar_arrive(smem_u32(a_full));
+      scan_barrier();  // [B1'] the A tile (written by both warpgroups) is complete
       if (threadIdx.x == 0) NS2_RVQ_STAMP(1);
 
-      // ---- scan this thread's 64 columns of every 128-code chunk: branch-free top-8 on packed keys ----
-      // The accumulator already is the (scaled) score, so a key is one LOP3: (bits & ~31) | index.  The two 32-column
-      // TMEM loads of a chunk are software-pipelined against the compare/select work, and the accumulator buffer is
-      // handed back to the MMA warp as soon as its last column sits in registers.
-      float g[8];
+      // ---- scan this thread's 32-code block of every 128-code chunk, for both of its frames: branch-free top-8 on
+      // packed keys.  The accumulator already is the (scaled) score, so a key is one LOP3: (bits & ~31) | index. ----
+      float ga[8], gb[8];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) g[i] = INFINITY;
-      auto scan32 = [&](const uint32_t (&v)[32], int sub_id) {
-        // local top-2 of the 32 scores, index i in the low 5 bits.  FMNMX / LOP3 share the half-rate ALU pipe, which
-        // bounds this loop: a tracker (a0 <= a1) absorbs a PAIR of keys in 5 min/max (2.5 per key instead of 3):
-        //   m = min(k0,k1), M = max(k0,k1);  a1' = min3(a1, max(a0, m), M);  a0' = min(a0, m).   Two trackers for ILP.
+      for (int i = 0; i < 8; ++i) {
+        ga[i] = INFINITY;
+        gb[i] = INFINITY;
+      }
+      auto scan32 = [&](const uint32_t (&v)[32], int sub_id, float (&g)[8]) {
+        // local top-2 of the 32 scores, index i in the low 5 bits.  A tracker (a0 <= a1) absorbs a PAIR of keys in
+        // 5 min/max:  m = min(k0,k1), M = max(k0,k1);  a1' = min3(a1, max(a0, m), M);  a0' = min(a0, m).  Two trackers.
         float a0 = INFINITY, a1 = INFINITY, b0 = INFINITY, b1 = INFINITY;
 #pragma unroll
         for (int i = 0; i < 32; i += 4) {
@@ -386,38 +351,67 @@ __global__ void __launch_bounds__(320, 1) rvq_encode_kernel(const __grid_constan
         }
         const float l0 = fminf(a0, b0);
         const float l1 = fminf(fmaxf(a0, b0), fminf(a1, b1));
-        // widen the index field to 11 bits (block id above the 5 local bits) and merge into the global top-8
+        // widen the index field to 11 bits (block id above the 5 local bits) and merge into the top-8
         const uint32_t blk = static_cast<uint32_t>(sub_id) << 5;
         insert8(__uint_as_float((__float_as_uint(l0) & 0xFFFFF81Fu) | blk), g);
         insert8(__uint_as_float((__float_as_uint(l1) & 0xFFFFF81Fu) | blk), g);
       };
       {
-        uint32_t v0[32], v1[32];
-        mbar_wait(smem_u32(&d_full[it & 1]), (it >> 1) & 1);
-        tc_fence_after();
-        tmem_ld32(lane_addr + (it & 1) * BC + half * 64, v0);
+        const uint32_t abase = smem_u32(smem + OFF_A) + wgi * (64 * 128);
+        const uint64_t dax = gmma_desc_plain(smem_u32(smem + OFF_AX) + wgi * (8 * 256), 128, 256);
 #pragma unroll 1
         for (int c = 0; c < chunks; ++c, ++it) {
-          const uint32_t buf = it & 1;
-          tmem_ld_wait();                                              // v0 = columns [0, 32) of this chunk
-          tmem_ld32(lane_addr + buf * BC + half * 64 + 32, v1);
-          scan32(v0, c * 4 + half * 2);                                // code = sub_id * 32 + i
-          tmem_ld_wait();                                              // v1 = columns [32, 64)
-          tc_fence_before();
-          mbar_arrive(smem_u32(&d_empty[buf]));                        // every TMEM read of this buffer is complete
-          if (c + 1 < chunks) {
-            const uint32_t nit = it + 1;
-            mbar_wait(smem_u32(&d_full[nit & 1]), (nit >> 1) & 1);
-            tc_fence_after();
-            tmem_ld32(lane_addr + (nit & 1) * BC + half * 64, v0);
+          const uint32_t st = it % RING, ph = (it / RING) & 1;
+          mbar_wait(smem_u32(&b_full[st]), ph);
+          const uint32_t bbase = smem_u32(smem + OFF_B + st * B_BYTES);
+          float d[BC / 2];
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < D / 16; ++k) {
+            const uint32_t aoff = (k >> 2) * (BF * 128) + (k & 3) * 32;   // atom, 16-dim step inside it
+            const uint32_t boff = (k >> 2) * (BC * 128) + (k & 3) * 32;
+            wgmma_f16_ss_n128<0, 0>(d, gmma_desc_sw128(abase + aoff, 16, 1024), gmma_desc_sw128(bbase + boff, 16, 1024),
+                                    k > 0 ? 1u : 0u);
           }
-          scan32(v1, c * 4 + half * 2 + 1);
+          // + 2^(e-ex+6) * (hi_k + lo_k) = ||c_k||^2 * 2^-(e+ex+1): the norm term of the score
+          wgmma_f16_ss_n128<0, 0>(d, dax, gmma_desc_plain(smem_u32(smem + OFF_BX + st * X_BYTES), 128, 256), 1u);
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_hold(d);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(smem_u32(&b_empty[st]));   // the ring slot may be refilled
+          uint32_t va[32], vb[32];
+#pragma unroll
+          for (int l = 0; l < 32; ++l) {
+            va[l] = __float_as_uint(d[4 * (l >> 1) + (l & 1)]);       // frame frow,     code 32 qc + l
+            vb[l] = __float_as_uint(d[4 * (l >> 1) + 2 + (l & 1)]);   // frame frow + 8, code 32 qc + l
+          }
+          scan32(va, c * 4 + qc, ga);
+          scan32(vb, c * 4 + qc, gb);
         }
       }
+      // blocks 4c + {0, 1} form column half 0, 4c + {2, 3} half 1: merge the lists of the lane pair (lane ^ 1)
       {
-        float4* kd = reinterpret_cast<float4*>(keys_s + (half * BF + row) * 8);
-        kd[0] = make_float4(g[0], g[1], g[2], g[3]);
-        kd[1] = make_float4(g[4], g[5], g[6], g[7]);
+        float oa[8], ob[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          oa[i] = __shfl_xor_sync(0xffffffffu, ga[i], 1);
+          ob[i] = __shfl_xor_sync(0xffffffffu, gb[i], 1);
+        }
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          insert8(oa[i], ga);
+          insert8(ob[i], gb);
+        }
+        if ((qc & 1) == 0) {
+          const int hsel = qc >> 1;
+          float4* kd = reinterpret_cast<float4*>(keys_s + (hsel * BF + frow) * 8);
+          kd[0] = make_float4(ga[0], ga[1], ga[2], ga[3]);
+          kd[1] = make_float4(ga[4], ga[5], ga[6], ga[7]);
+          float4* ke = reinterpret_cast<float4*>(keys_s + (hsel * BF + frow + 8) * 8);
+          ke[0] = make_float4(gb[0], gb[1], gb[2], gb[3]);
+          ke[1] = make_float4(gb[4], gb[5], gb[6], gb[7]);
+        }
       }
       if (threadIdx.x == 0) NS2_RVQ_STAMP(2);
       scan_barrier();  // [B2] both halves' key lists are published
@@ -632,18 +626,13 @@ __global__ void __launch_bounds__(320, 1) rvq_encode_kernel(const __grid_constan
     }
   }
 
-  tc_fence_before();
   __syncthreads();
   if (p.stats != nullptr && blockIdx.x == 0 && threadIdx.x < 256 && static_cast<int>(threadIdx.x) < p.Q * 8)
     p.stats[4 + threadIdx.x] = tl_s[threadIdx.x];
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------
-// prepare: fp16 copy scaled by a per-quantiser power of two, ||c||^2, max ||c||, and the fp16 hi/lo norm blocks the
+// prepare: fp16 copy (codes permuted inside each 128-code chunk, see rvq_perm) scaled by a per-quantiser power of two, ||c||^2, max ||c||, and the fp16 hi/lo norm blocks the
 // encode kernel contracts as a ninth K block (layout: rvq::X_BYTES per 128-code chunk, see OFF_BX)
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) rvq_prepare_kernel(const float* __restrict__ cb, int K, int D,
@@ -670,8 +659,11 @@ __global__ void __launch_bounds__(256) rvq_prepare_kernel(const float* __restric
   }
   __syncthreads();
   const float inv = 1.0f / s_scale;
-  for (int i = threadIdx.x; i < K * D; i += blockDim.x)
-    cb16[static_cast<long long>(q) * K * D + i] = __float2half_rn(c[i] * inv);
+  for (int i = threadIdx.x; i < K * D; i += blockDim.x) {   // row n of the fp16 copy holds code rvq_perm(n) of its chunk
+    const int n = i / D;
+    const int src = ((n & ~127) | rvq_perm(n & 127)) * D + (i - n * D);
+    cb16[static_cast<long long>(q) * K * D + i] = __float2half_rn(c[src] * inv);
+  }
   // ||c||^2 in fp64, rounded once to fp32; one warp per code
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float nmax = 0.f;
@@ -688,7 +680,8 @@ __global__ void __launch_bounds__(256) rvq_prepare_kernel(const float* __restric
       const float val = static_cast<float>(s) * inv * inv * 0.0078125f;
       const __half hi = __float2half_rn(val);
       const __half lo = __float2half_rn(val - __half2float(hi));
-      __half* blk = cbx + (static_cast<long long>(q) * (K / 128) + k / 128) * 2048 + ((k & 127) >> 3) * 128 + (k & 7) * 8;
+      const int n = rvq_perm_inv(k & 127);   // column of the chunk that holds code k
+      __half* blk = cbx + (static_cast<long long>(q) * (K / 128) + k / 128) * 2048 + (n >> 3) * 128 + (n & 7) * 8;
       if (lane < 8) blk[lane] = lane == 0 ? hi : (lane == 1 ? lo : __float2half_rn(0.f));   // K half 0
       else if (lane < 16) blk[64 + lane - 8] = __float2half_rn(0.f);                        // K half 1
     }

@@ -1,4 +1,4 @@
-// Weight-gradient GEMM on tcgen05 for sm_100a (backward of every Linear / CausalConv1d on the hot path):
+// Weight-gradient GEMM on wgmma for sm_90a (backward of every Linear / CausalConv1d on the hot path):
 //
 //     dW[g][n, k] += sum over batches b and positions m of  dY[b, m, g*dy_gcs + n] * X[b, m - shift*dil[g], g*x_gcs + x_col_off + k]
 //
@@ -9,11 +9,12 @@
 // "transposed" bits — no transpose is ever materialised.  Out-of-range positions of a shifted tap are zero-filled by the
 // TMA unit (the 3-D map ends each batch), exactly as in the forward conv.
 //
-// One CTA per (128 x BN output tile, split of the position range), 192 threads:
-//   warp 0   TMA producer (converged, elect_one): dY tile (2 swizzle atoms) + X tile (BN/64 atoms) per 64 positions
-//   warp 1   tcgen05.mma issuer: D[128 x BN] fp32 in TMEM, 4 MMAs per 64 positions
-//   warps 2-5 epilogue: TMEM -> registers -> swizzled smem staging -> TMA reduce-add (fp32 +=) into dW
-// Partial sums of the position splits meet in L2 through the reduce-add, which is also what makes the call accumulate
+// One CTA per (128 x BN output tile, split of the position range), 384 threads:
+//   warpgroup 0     TMA producer (warp 0, converged, elect_one): dY tile (2 swizzle atoms) + X tile (BN/64 atoms) per
+//                   64 positions
+//   warpgroups 1-2  wgmma m64nBNk16: warpgroup w accumulates dW rows [64 (w-1), 64 w) of the tile in registers, then
+//                   adds them into dW with fp32 global reductions
+// Partial sums of the position splits meet in L2 through the reductions, which is also what makes the call accumulate
 // into an existing gradient (autograd's .grad semantics).
 #include "ptx.cuh"
 #include "host_common.h"
@@ -29,21 +30,23 @@ namespace wg {
 constexpr int BM = 128;           // dW rows per tile (output channels n)
 constexpr int BKP = 64;           // positions per pipeline stage
 constexpr int ATOM = 64 * BKP * 2;  // one [64 positions][64 channels] bf16 swizzle atom: 8 KB
-constexpr int STG_BYTES = 32 * 128;
+constexpr int THREADS = 384;
 template <int BN>
 struct Cfg {
   static constexpr int A_BYTES = 2 * ATOM;              // 128 n-channels
   static constexpr int B_BYTES = (BN / 64) * ATOM;      // BN k-channels
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = (BN == 256) ? 4 : 6;
-  static constexpr int OFF_STG = STAGES * STAGE_BYTES;
-  static constexpr int OFF_BAR = OFF_STG + 4 * 2 * STG_BYTES;
+  static constexpr int OFF_BAR = STAGES * STAGE_BYTES;
   static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
 };
 }  // namespace wg
 
 struct WgradDev {
-  CUtensorMap tmDy, tmX, tmOut;
+  float* dW;
+  long long dw_rs;
+  int n, k;
+  CUtensorMap tmDy, tmX;
   int tiles_n, tiles_k, groups, splits;
   int rows, batches;          // positions per batch, batches
   int blocks_per_batch;       // ceil(rows / 64)
@@ -53,7 +56,7 @@ struct WgradDev {
 };
 
 template <int BN>
-__global__ void __launch_bounds__(192, 1) wgrad_kernel(const __grid_constant__ WgradDev p) {
+__global__ void __launch_bounds__(wg::THREADS, 1) wgrad_kernel(const __grid_constant__ WgradDev p) {
   using namespace wg;
   using C = Cfg<BN>;
   extern __shared__ uint8_t smem_raw[];
@@ -61,8 +64,6 @@ __global__ void __launch_bounds__(192, 1) wgrad_kernel(const __grid_constant__ W
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + C::STAGES;
-  uint64_t* done_bar = bars + 2 * C::STAGES;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 2 * C::STAGES + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   // tile / split decode
@@ -75,116 +76,90 @@ __global__ void __launch_bounds__(192, 1) wgrad_kernel(const __grid_constant__ W
   const int blk0 = blockIdx.y * per_split;
   const int blk1 = (blk0 + per_split < total_blocks) ? blk0 + per_split : total_blocks;
   const int nblk = blk1 - blk0;
+  if (nblk <= 0) return;  // empty split (more splits than position blocks): nothing to add
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmDy);
     tma_prefetch_desc(&p.tmX);
-    tma_prefetch_desc(&p.tmOut);
-  }
-  if (warp == 1 && lane == 0) {
     for (int i = 0; i < C::STAGES; ++i) {
       mbar_init(smem_u32(&full_bar[i]), 1);
-      mbar_init(smem_u32(&empty_bar[i]), 1);
+      mbar_init(smem_u32(&empty_bar[i]), 8);
     }
-    mbar_init(smem_u32(done_bar), 1);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(tmem_holder), BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
-  if (nblk <= 0) {  // empty split (more splits than position blocks): nothing to add
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, BN);
-    return;
-  }
 
-  if (warp == 0) {
-    // =============================== TMA producer ===============================
-    const int shift = p.shift_units * p.dil[g];
-    const int dy_c0 = g * p.dy_gcs + tn * BM;
-    const int x_c0 = g * p.x_gcs + p.x_col_off + tk * BN;
-    for (int i = 0; i < nblk; ++i) {
-      const int blk = blk0 + i;
-      const int b = blk / p.blocks_per_batch;
-      const int m0 = (blk - b * p.blocks_per_batch) * BKP;
-      const uint32_t stage = i % C::STAGES, phase = (i / C::STAGES) & 1;
-      mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1);
-      if (elect_one()) {
-        const uint32_t fb = smem_u32(&full_bar[stage]);
-        mbar_arrive_expect_tx(fb, C::STAGE_BYTES);
-        const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES);
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == 0) {
+      // =============================== TMA producer ===============================
+      const int shift = p.shift_units * p.dil[g];
+      const int dy_c0 = g * p.dy_gcs + tn * BM;
+      const int x_c0 = g * p.x_gcs + p.x_col_off + tk * BN;
+      for (int i = 0; i < nblk; ++i) {
+        const int blk = blk0 + i;
+        const int b = blk / p.blocks_per_batch;
+        const int m0 = (blk - b * p.blocks_per_batch) * BKP;
+        const uint32_t stage = i % C::STAGES, phase = (i / C::STAGES) & 1;
+        mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1);
+        if (elect_one()) {
+          const uint32_t fb = smem_u32(&full_bar[stage]);
+          mbar_arrive_expect_tx(fb, C::STAGE_BYTES);
+          const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES);
 #pragma unroll
-        for (int a = 0; a < 2; ++a) tma_load_3d(sa + a * ATOM, &p.tmDy, fb, dy_c0 + a * 64, m0, b);
+          for (int a = 0; a < 2; ++a) tma_load_3d(sa + a * ATOM, &p.tmDy, fb, dy_c0 + a * 64, m0, b);
 #pragma unroll
-        for (int a = 0; a < BN / 64; ++a)
-          tma_load_3d(sa + C::A_BYTES + a * ATOM, &p.tmX, fb, x_c0 + a * 64, m0 - shift, b);
+          for (int a = 0; a < BN / 64; ++a)
+            tma_load_3d(sa + C::A_BYTES + a * ATOM, &p.tmX, fb, x_c0 + a * 64, m0 - shift, b);
+        }
+        __syncwarp();
       }
-      __syncwarp();
     }
-  } else if (warp == 1) {
-    // =============================== MMA issuer =================================
-    constexpr uint32_t idesc = umma_idesc_f16(BM, BN, /*bf16*/ 1, /*A MN-major*/ 1, /*B MN-major*/ 1);
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    // =============================== wgmma consumers ===============================
+    const int cw = (warp >> 2) - 1;   // dW rows [64 cw, 64 cw + 64) of the tile = swizzle atom cw of the dY tile
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int prev_stage = -1;
     for (int i = 0; i < nblk; ++i) {
       const uint32_t stage = i % C::STAGES, phase = (i / C::STAGES) & 1;
       mbar_wait(smem_u32(&full_bar[stage]), phase);
-      tc_fence_after();
       const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES);
-      if (elect_one()) {
+      wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BKP / 16; ++k) {
-          // 16 positions = two 8-row groups of 1024 bytes; LBO = distance between 64-channel atoms
-          const uint64_t da = umma_desc_sw128(sa + k * 2048, ATOM, 1024);
-          const uint64_t db = umma_desc_sw128(sa + C::A_BYTES + k * 2048, ATOM, 1024);
-          tc_mma_f16(tmem_base, da, db, idesc, (i > 0) | (k > 0));
+      for (int k = 0; k < BKP / 16; ++k) {
+        // 16 positions = two 8-row groups of 1024 bytes; LBO = distance between 64-channel atoms
+        const uint64_t da = gmma_desc_sw128(sa + cw * ATOM + k * 2048, ATOM, 1024);
+        const uint64_t db = gmma_desc_sw128(sa + C::A_BYTES + k * 2048, ATOM, 1024);
+        if constexpr (BN == 256) wgmma_bf16_ss_n256<1, 1>(acc, da, db, 1u);
+        else wgmma_bf16_ss_n128<1, 1>(acc, da, db, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev_stage >= 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev_stage]));
+      prev_stage = static_cast<int>(stage);
+    }
+    wgmma_wait<0>();
+    wgmma_hold(acc);
+    // ---- dW += acc (fp32 reductions in L2) ----
+    const int row_base = tn * BM + cw * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int c2 = 2 * (lane & 3);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int n = row_base + 8 * r;
+      if (n >= p.n) continue;
+      float* drow = p.dW + (static_cast<long long>(g) * p.out_grs + n) * p.dw_rs;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = tk * BN + 8 * j + c2;
+        if (col < p.k) {
+          atomicAdd(drow + col, acc[4 * j + 2 * r]);
+          atomicAdd(drow + col + 1, acc[4 * j + 2 * r + 1]);
         }
-        tc_commit(smem_u32(&empty_bar[stage]));
-        if (i == nblk - 1) tc_commit(smem_u32(done_bar));
       }
-      __syncwarp();
     }
-  } else {
-    // =============================== epilogue ===================================
-    const int ew = warp & 3;   // TMEM lane quarter this warp may read (warps 2..5 -> quarters 2,3,0,1)
-    mbar_wait(smem_u32(done_bar), 0);
-    tc_fence_after();
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(ew * 32) << 16);
-    const uint32_t stg = smem_u32(smem + C::OFF_STG + (warp - 2) * 2 * STG_BYTES);
-    const int out_row = g * p.out_grs + tn * BM + ew * 32;
-    uint32_t count = 0;
-#pragma unroll 1
-    for (int c = 0; c < BN; c += 32) {
-      uint32_t r[32];
-      tmem_ld32(taddr + c, r);
-      tmem_ld_wait();
-      if (elect_one()) tma_store_wait_read<1>();
-      __syncwarp();
-      const uint32_t box = stg + (count & 1) * STG_BYTES;
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const uint32_t addr = box + lane * 128 + ((q ^ (lane & 7)) << 4);
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[4 * q]), "r"(r[4 * q + 1]),
-                     "r"(r[4 * q + 2]), "r"(r[4 * q + 3])
-                     : "memory");
-      }
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (elect_one()) {
-        tma_reduce_add_2d(&p.tmOut, box, tk * BN + c, out_row);
-        tma_store_commit();
-      }
-      __syncwarp();
-      ++count;
-    }
-    if (elect_one()) tma_store_wait_all();
-    __syncwarp();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, BN);
   }
 }
 
@@ -217,13 +192,10 @@ extern "C" int ns2_wgrad(const ns2_wgrad_args* a, ns2_stream_t stream_) {
     int rc = make_tmap_16bit(&dev.tmX, a->X, 3, dims, str, box);
     if (rc != kOk) return rc;
   }
-  {
-    const uint64_t dims[2] = {(uint64_t)a->k, (uint64_t)(a->groups - 1) * a->dw_group_row_stride + a->n};
-    const uint64_t str[2] = {4, (uint64_t)a->dw_row_stride * 4};
-    const uint32_t obox[2] = {32, 32};
-    int rc = make_tmap_f32(&dev.tmOut, a->dW, 2, dims, str, obox);
-    if (rc != kOk) return rc;
-  }
+  dev.dW = a->dW;
+  dev.dw_rs = a->dw_row_stride;
+  dev.n = a->n;
+  dev.k = a->k;
   dev.tiles_n = (a->n + wg::BM - 1) / wg::BM;
   dev.tiles_k = (a->k + bn - 1) / bn;
   dev.groups = a->groups;
@@ -247,10 +219,10 @@ extern "C" int ns2_wgrad(const ns2_wgrad_args* a, ns2_stream_t stream_) {
   dim3 grid(tiles, splits);
   if (bn == 256) {
     NS2_CUDA_CHECK(set_max_smem_once(wgrad_kernel<256>, wg::Cfg<256>::SMEM_BYTES));
-    wgrad_kernel<256><<<grid, 192, wg::Cfg<256>::SMEM_BYTES, stream>>>(dev);
+    wgrad_kernel<256><<<grid, wg::THREADS, wg::Cfg<256>::SMEM_BYTES, stream>>>(dev);
   } else {
     NS2_CUDA_CHECK(set_max_smem_once(wgrad_kernel<128>, wg::Cfg<128>::SMEM_BYTES));
-    wgrad_kernel<128><<<grid, 192, wg::Cfg<128>::SMEM_BYTES, stream>>>(dev);
+    wgrad_kernel<128><<<grid, wg::THREADS, wg::Cfg<128>::SMEM_BYTES, stream>>>(dev);
   }
   g_launches.fetch_add(1, std::memory_order_relaxed);
   NS2_CUDA_CHECK(cudaGetLastError());

@@ -2,7 +2,7 @@
 naturalspeech2_pytorch.NaturalSpeech2 (ns2.py:1160-1684): `forward` (training loss), `sample`, `ddim_sample`.
 
 Scope (SURVEY section 8): the per-timestep path — schedules, q-sample, v-target, per-sample MSE, min-SNR
-weight, the DDIM update and classifier-free guidance — runs on the sm_100a kernels (`ops.q_sample`,
+weight, the DDIM update and classifier-free guidance — runs on the sm_90a kernels (`ops.q_sample`,
 `Model.forward`, `ops.mse_rows`, `ops.ddim_step`, `ops.cfg_combine`).  The once-per-sample conditioning encoders
 of the reference (PhonemeEncoder, SpeechPromptEncoder, DurationPitchPredictor, Aligner; ns2.py:228-527,
 aligner.py) are out of scope: for a conditional model pass their outputs directly (`prompt_enc=`, `cond=`) or

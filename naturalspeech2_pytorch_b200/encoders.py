@@ -1,4 +1,4 @@
-"""Per-sample conditioning encoders of NaturalSpeech2 on the sm_100a kernels (SURVEY section 8, row f3).
+"""Per-sample conditioning encoders of NaturalSpeech2 on the sm_90a kernels (SURVEY section 8, row f3).
 
 `SpeechPromptEncoder` (ns2.py:289-341) and `PhonemeEncoder` (ns2.py:228-287) run once per sample BEFORE the denoiser
 loop (`NaturalSpeech2.forward` ns2.py:1537-1539, `sample` 1474-1476).  Both are a stack of k=9 convolutions with SiLU
@@ -6,7 +6,7 @@ followed by the plain `Transformer` (ns2.py:1073-1117: RMSNorm -> Attention -> +
 +res).  Same constructor arguments, same parameter names and shapes as the reference, so a reference state_dict loads
 unchanged; the module tree only HOLDS parameters, the math goes through `ops` (libns2b200.so):
 
-  Conv1d(k=9, padding=4) + SiLU   one segmented tcgen05 GEMM with nine shifted-row segments (TMA zero fill = the
+  Conv1d(k=9, padding=4) + SiLU   one segmented wgmma GEMM with nine shifted-row segments (TMA zero fill = the
                                   "same" padding), SiLU in the epilogue (NS2_GEMM_FLAG_SILU)
   CausalConv1d(k=9) + SiLU        the same GEMM with shifts 8..0 (left padding only, ns2.py:583-595)
   nn.Embedding                    ops.embedding_bf16 (gather + padding substitution)
@@ -135,9 +135,9 @@ class _EncoderBase(nn.Module):
 
 def _check_transformer_dims(dim: int, dim_head: int):
     if dim_head != 64:
-        raise NotImplementedError("the sm_100a attention kernel is specialised for dim_head=64")
+        raise NotImplementedError("the sm_90a attention kernel is specialised for dim_head=64")
     if dim % 128 != 0 or dim > 1024:
-        raise NotImplementedError("transformer dim must be a multiple of 128 (<= 1024) for the sm_100a kernels")
+        raise NotImplementedError("transformer dim must be a multiple of 128 (<= 1024) for the sm_90a kernels")
 
 
 class SpeechPromptEncoder(_EncoderBase):
@@ -228,7 +228,7 @@ class PhonemeEncoder(_EncoderBase):
     @torch.no_grad()
     def forward(self, x, mask=None) -> torch.Tensor:
         if mask is not None:
-            raise NotImplementedError("PhonemeEncoder: attention masks are not supported by the sm_100a attention kernel")
+            raise NotImplementedError("PhonemeEncoder: attention masks are not supported by the sm_90a attention kernel")
         if isinstance(x, (list, tuple)):
             assert self.tokenizer is not None
             x = self.tokenizer.texts_to_tensor_ids(x).to(self.token_emb.weight.device)
@@ -382,7 +382,7 @@ class DurationPitchPredictor(_EncoderBase):
     @torch.no_grad()
     def forward(self, x, encoded_prompts: torch.Tensor, prompt_mask=None):
         if prompt_mask is not None:
-            raise NotImplementedError("DurationPitchPredictor: prompt masks are not supported by the sm_100a attention kernel")
+            raise NotImplementedError("DurationPitchPredictor: prompt masks are not supported by the sm_90a attention kernel")
         if isinstance(x, (list, tuple)):
             assert self.tokenizer is not None
             x = self.tokenizer.texts_to_tensor_ids(x).to(encoded_prompts.device)

@@ -1,7 +1,7 @@
-"""Switching an existing reference object over to the sm_100a path (INTEGRATION.md).
+"""Switching an existing reference object over to the sm_90a path (INTEGRATION.md).
 
 `accelerate(ref_model)` reads the constructor arguments back out of a `naturalspeech2_pytorch.Model` instance
-(ns2.py:811-905 stores them as attributes / module shapes), builds the B200 `Model` with the same configuration,
+(ns2.py:811-905 stores them as attributes / module shapes), builds the H100 `Model` with the same configuration,
 loads the reference's state_dict (the parameter names and shapes are identical, SURVEY Appendix B) and returns it.
 `patch_reference(ref_model)` additionally rebinds `forward` / `forward_with_cond_scale` of the reference object, so
 that code holding the reference instance (e.g. a reference `NaturalSpeech2` wrapper) runs the CUDA kernels unchanged.
@@ -43,7 +43,7 @@ def infer_model_kwargs(ref: nn.Module) -> dict:
 
 
 def accelerate(ref: nn.Module, device=None) -> Model:
-    """B200 `Model` with the configuration and the weights of the reference `Model` instance `ref`."""
+    """H100 `Model` with the configuration and the weights of the reference `Model` instance `ref`."""
     fast = Model(**infer_model_kwargs(ref))
     fast.load_state_dict(ref.state_dict())
     if device is None:
@@ -52,7 +52,7 @@ def accelerate(ref: nn.Module, device=None) -> Model:
 
 
 def patch_reference(ref: nn.Module, device="cuda") -> Model:
-    """Rebind `ref.forward` / `ref.forward_with_cond_scale` to the B200 model built from `ref` (returned).  The
+    """Rebind `ref.forward` / `ref.forward_with_cond_scale` to the H100 model built from `ref` (returned).  The
     reference object keeps its parameters; call `fast.load_state_dict(ref.state_dict())` again after updating them."""
     fast = accelerate(ref, device=device)
 

@@ -1,4 +1,4 @@
-"""`Model`: the NaturalSpeech2 denoiser (time FiLM -> Wavenet -> conditionable Transformer) on sm_100a kernels.
+"""`Model`: the NaturalSpeech2 denoiser (time FiLM -> Wavenet -> conditionable Transformer) on sm_90a kernels.
 
 Drop-in for `naturalspeech2_pytorch.Model` (ns2.py:811-1000): same constructor, same `forward` /
 `forward_with_cond_scale` signatures, same parameter names and shapes (SURVEY Appendix B), so a reference
@@ -154,16 +154,16 @@ def _prob_mask_like(shape, prob, device):
 
 
 class Model(nn.Module):
-    """B200 denoiser; constructor and call signatures of ns2.py:811-937."""
+    """H100 denoiser; constructor and call signatures of ns2.py:811-937."""
 
     def __init__(self, dim, *, depth, dim_head=64, heads=8, ff_mult=4, wavenet_layers=8,
                  wavenet_stacks=4, dim_cond_mult=4, use_flash_attn=True, dim_prompt=None,
                  num_latents_m=32, resampler_depth=2, cond_drop_prob=0., condition_on_prompt=False):
         super().__init__()
         if dim_head != 64:
-            raise NotImplementedError("the sm_100a attention kernel is specialised for dim_head=64")
+            raise NotImplementedError("the sm_90a attention kernel is specialised for dim_head=64")
         if dim % 128 != 0 or dim > 1024:
-            raise NotImplementedError("dim must be a multiple of 128 (<= 1024) for the sm_100a kernels")
+            raise NotImplementedError("dim must be a multiple of 128 (<= 1024) for the sm_90a kernels")
         if not 1 <= wavenet_layers <= 8:
             raise NotImplementedError("wavenet_layers must be in [1, 8] (one launch covers <= 8 dilation columns)")
         self.dim = dim
@@ -571,7 +571,7 @@ class Model(nn.Module):
         if prompt_mask is not None:
             raise NotImplementedError("prompt_mask is unsupported (the reference itself fails on it, SURVEY T9)")
         if not x.is_cuda:
-            raise RuntimeError("naturalspeech2_pytorch_b200.Model runs on CUDA (sm_100a) tensors only")
+            raise RuntimeError("naturalspeech2_pytorch_b200.Model runs on CUDA (sm_90a) tensors only")
         B, N, D = x.shape
         assert D == self.dim, f"expected last dim {self.dim}, got {D}"
         dev = x.device

@@ -3,8 +3,8 @@
 `loss.backward()` is how the reference is used (README.md:60-63, ns2.py:1886).  Here `Model.forward` records ONE autograd
 node (`DenoiserFunction`) when gradients are enabled; its backward walks the network in reverse and launches, per layer,
   * dgrad GEMMs     ns2_gemm on transposed weight packs (anti-causal shifts for the causal convs),
-  * wgrad GEMMs     ns2_wgrad (tcgen05, MN-major operands, fp32 reduce-add into the packed gradient),
-  * attention bwd   ns2_attn_bwd (tcgen05 flash backward from the saved log-sum-exp),
+  * wgrad GEMMs     ns2_wgrad (wgmma, MN-major operands, fp32 reduce-add into the packed gradient),
+  * attention bwd   ns2_attn_bwd (wgmma flash backward from the saved log-sum-exp),
   * the element-wise backward kernels of csrc/backward.cu (RMSNorm+FiLM, GEGLU, Wavenet gate, bias column sums).
 Pre-activations that the fused forward epilogues never materialise (GEGLU's value/gate pair, the Wavenet conv output
 before FiLM) are recomputed with plain-epilogue GEMMs instead of being stored.  Gradients come out in the packed bf16

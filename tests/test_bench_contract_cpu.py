@@ -16,8 +16,8 @@ def test_reference_arm_json_contract():
     d = json.loads(line)
     assert d["impl"] == "reference" and d["metric"] == "denoiser-steps/sec" and d["unit"] == "steps/s"
     assert d["higher_is_better"] is True and d["value"] > 0
-    # baseline/_ref (the pip-installed reference) when present, else the oracle port
-    expect_kind = "reference" if (ROOT / "baseline" / "_ref" / "naturalspeech2_pytorch").exists() else "port"
+    # oracle/_ref (the pip-installed reference) when present, else the oracle port
+    expect_kind = "reference" if (ROOT / "oracle" / "_ref" / "naturalspeech2_pytorch").exists() else "port"
     assert d["cpu_baseline"]["kind"] == expect_kind
     assert d["cpu_baseline"]["cores"] >= 1 and d["cpu_baseline"]["value"] == d["value"]
     assert d["steps"] == 2 and d["sample_batch"] == 2 and d["extrapolated"] is True

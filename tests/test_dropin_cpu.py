@@ -1,4 +1,4 @@
-"""CPU: drop-in surface against the UNMODIFIED reference (pip-installed into baseline/_ref; it travels to the GPU box).
+"""CPU: drop-in surface against the UNMODIFIED reference (pip-installed into oracle/_ref; it travels to the GPU box).
 
 For BASELINE configs[0..2] (README model, cfg2, cfg3) and a small conditional model: identical `state_dict` keys and
 shapes, identical `forward` / `forward_with_cond_scale` parameter lists (the reference's parameters must all be
@@ -19,7 +19,7 @@ sys.path.insert(0, str(ROOT))
 import bench  # noqa: E402
 
 ns2 = bench.import_reference()
-pytestmark = pytest.mark.skipif(ns2 is None, reason="baseline/_ref (pip-installed reference) is not present")
+pytestmark = pytest.mark.skipif(ns2 is None, reason="oracle/_ref (pip-installed reference) is not present")
 
 CONFIGS = {
     "cfg1_readme": dict(dim=128, depth=6),
@@ -85,7 +85,7 @@ def test_call_signatures_cover_the_reference():
 
 
 def test_patch_reference_rebinds_forward():
-    """`patch_reference` on a real (CPU) reference instance: the bound methods are replaced and the B200 model carries
+    """`patch_reference` on a real (CPU) reference instance: the bound methods are replaced and the H100 model carries
     the reference's weights; calling it without a GPU must raise (there is no CPU fallback)."""
     from naturalspeech2_pytorch_b200.integration import patch_reference
     kw = dict(dim=128, depth=1, heads=2, wavenet_layers=2, wavenet_stacks=2)

@@ -163,7 +163,8 @@ typedef struct ns2_attn_args {
 int ns2_attn_fwd(const ns2_attn_args* args, ns2_stream_t stream);
 
 /* Backward of the above (autograd of F.scaled_dot_product_attention, reached from loss.backward(), ns2.py:1886):
- *   dq_accum (batches, q_len, heads*64) f32, contiguous, must be ZERO on entry (every key tile adds its share);
+ *   dq_accum (batches, q_len, heads*64) f32, contiguous: dQ is ADDED to it (every key tile adds its share; zero it for
+ *   a plain gradient);
  *   dk / dv: bf16, same layout conventions as k / v;  lse from ns2_attn_fwd;  delta: scratch (batches, heads, q_len) f32. */
 typedef struct ns2_attn_bwd_args {
   const void* q; int64_t q_row_stride, q_batch_stride;

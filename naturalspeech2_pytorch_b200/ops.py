@@ -559,7 +559,7 @@ def rvq_ce(frames: torch.Tensor, codebooks: torch.Tensor, cn2: torch.Tensor, own
 # --------------------------------------------------------------------------------------------------
 def attention_bwd(q, k, v, o, d_o, lse, dq_accum, dk, dv, *, heads: int, scale: Optional[float] = None,
                   delta: Optional[torch.Tensor] = None):
-    """(dq_accum f32 (B, Nq, inner) += dQ, dk, dv bf16) of softmax(q k^T scale) v given d_o; dq_accum must be zeroed."""
+    """(dq_accum f32 (B, Nq, inner) += dQ, dk, dv bf16) of softmax(q k^T scale) v given d_o; zero dq_accum for a plain dQ."""
     lib = _lib.load()
     for name, t in (("q", q), ("k", k), ("v", v), ("o", o), ("d_o", d_o), ("dk", dk), ("dv", dv)):
         _req(t, torch.bfloat16, name)

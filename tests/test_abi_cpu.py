@@ -53,6 +53,22 @@ def test_argument_validation_without_gpu(lib):
     assert lib.ns2_film_wgrad(None, 8, None, 33, 8, 8, None, 0, None) < 0
 
 
+@pytest.mark.parametrize("k", [
+    4096,   # above MAX_K = 2048, the 11-bit code index of the encoder's packed keys
+    192,    # not a multiple of the 128-code chunk
+])
+def test_rvq_rejects_unsupported_codebook_size_before_launch(lib, k):
+    """The codebook-size checks are host-side: a clean error and no kernel launch (dummy non-NULL device pointers are
+    never dereferenced)."""
+    before = lib.ns2_launch_count()
+    assert lib.ns2_rvq_encode(16, 4, 128, 16, 16, 16, 16, 1, k, 16, None, None) < 0
+    assert b"codebook size" in lib.ns2_last_error()
+    if k % 128:
+        assert lib.ns2_rvq_prepare(16, 1, k, 128, 16, 16, 16, None) < 0
+        assert b"codebook size" in lib.ns2_last_error()
+    assert lib.ns2_launch_count() == before
+
+
 def test_struct_layout_matches_header():
     """ctypes mirrors of the C structs: sizes are what a C compiler produces for include/ns2_b200.h."""
     import subprocess, tempfile, textwrap

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define NS2_ABI_VERSION 3
+#define NS2_ABI_VERSION 4
 
 typedef void* ns2_stream_t; /* cudaStream_t */
 
@@ -359,6 +359,32 @@ int ns2_film_wgrad(const float* dfilm, int64_t dfilm_batch_stride /* elements be
                    int32_t accumulate /* 0: dw = ..., dw need not be initialised; 1: dw += ... */, ns2_stream_t stream);
 /*    ns2_accum_bf16       : acc (f32) += t (bf16); acc_bf16 (optional) = bf16(acc)   (joins a branch gradient) */
 int ns2_accum_bf16(float* acc, const void* t_bf16, int64_t count, void* acc_bf16, ns2_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * 8b. Backward of the conditioning front end (SpeechPromptEncoder ns2.py:289-341, PhonemeEncoder 228-287, pitch
+ *     embedding and length regulation 1449-1455, 1581-1583): the diffusion loss reaches them through
+ *     Model(prompt=prompt_enc, cond=cond) (ns2.py:1635, 1886).  Convolution dgrad / wgrad are ns2_gemm / ns2_wgrad
+ *     ("same" padding: negative shift_units); attention, RMSNorm(gamma) and GEGLU reuse section 8.
+ *    ns2_silu_bwd             : dpre = dout * s * (1 + pre * (1 - s)), s = sigmoid(pre), all bf16, `count` elements
+ *                               (even); dpre may alias pre.  nn.SiLU after each k=9 conv (ns2.py:255-257, 316-320)
+ *    ns2_embedding_bwd        : dtable[id(r), :] += de[r, :] (f32, atomics), id(r) = ids[r] < 0 ? pad_id : ids[r]
+ *                               — nn.Embedding backward of the phoneme table (ns2.py:253, 279-282); the pad row
+ *                               receives gradient (the reference's table has no padding_idx)
+ *    ns2_expand_encodings_bwd : transpose of ns2_expand_encodings given d cond token-major f32 (batch, length, dim)
+ *                               with row stride dcond_row_stride:  dphon[b, m, :] += sum over frames n with
+ *                               idx[b, n] == m of dcond[b, n, :];  dtable[coarse[b, m], :] += the same sums (atomics).
+ *                               Frames with idx < 0 add nothing; either output may be NULL
+ *    ns2_add_rows_bcast       : x[b, r, :] += scale * v[b, :] for f32 x (batch, rows, dim) — the gradient of a
+ *                               mean over rows (prompt mean-pool, ns2.py:858-862) added to a per-row gradient
+ * ------------------------------------------------------------------------------------------------ */
+int ns2_silu_bwd(const void* pre_bf16, const void* dout_bf16, int64_t count, void* dpre_bf16, ns2_stream_t stream);
+int ns2_embedding_bwd(const int64_t* ids, int64_t rows, const float* de, int32_t num_rows, int32_t dim, int32_t pad_id,
+                      float* dtable, ns2_stream_t stream);
+int ns2_expand_encodings_bwd(const float* dcond, int64_t dcond_row_stride, const int32_t* coarse, int32_t table_rows,
+                             const int32_t* idx, int32_t batch, int32_t t_text, int32_t dim, int32_t length, float* dphon,
+                             float* dtable, ns2_stream_t stream);
+int ns2_add_rows_bcast(float* x, int32_t batch, int32_t rows, int32_t dim, const float* v, float scale,
+                       ns2_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * 9. Monotonic alignment search: `maximum_path(value, mask)` of naturalspeech2_pytorch/aligner.py:88-122 (called from

@@ -17,7 +17,7 @@ NS2_MSE_SCRATCH_PER_SAMPLE = 64
 NS2_RVQ_STATS_LEN = 260
 NS2_OBJ_V, NS2_OBJ_EPS, NS2_OBJ_X0 = 0, 1, 2
 NS2_GEMM_FLAG_SKIP_EPILOGUE, NS2_GEMM_FLAG_WAVENET_ONE_PASS, NS2_GEMM_FLAG_SILU = 1, 2, 4
-NS2_ABI_VERSION = 3
+NS2_ABI_VERSION = 4
 
 
 class GemmSeg(C.Structure):
@@ -118,6 +118,10 @@ SIGNATURES = {
     "ns2_mse_bwd": (C.c_int, [_P, _P, _P, _I32, _I64, _P, _P, _P]),
     "ns2_film_wgrad": (C.c_int, [_P, _I64, _P, _I32, _I64, _I32, _P, _I32, _P]),
     "ns2_accum_bf16": (C.c_int, [_P, _P, _I64, _P, _P]),
+    "ns2_silu_bwd": (C.c_int, [_P, _P, _I64, _P, _P]),
+    "ns2_embedding_bwd": (C.c_int, [_P, _I64, _P, _I32, _I32, _I32, _P, _P]),
+    "ns2_expand_encodings_bwd": (C.c_int, [_P, _I64, _P, _I32, _P, _I32, _I32, _I32, _I32, _P, _P, _P]),
+    "ns2_add_rows_bcast": (C.c_int, [_P, _I32, _I32, _I32, _P, _F, _P]),
     "ns2_rvq_prepare": (C.c_int, [_P, _I32, _I32, _I32, _P, _P, _P, _P]),
     "ns2_rvq_encode": (C.c_int, [_P, _I64, _I32, _P, _P, _P, _P, _I32, _I32, _P, _P, _P]),
     "ns2_rvq_decode": (C.c_int, [_P, _I64, _I32, _I32, _I32, _P, _P, _P]),

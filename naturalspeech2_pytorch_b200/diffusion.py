@@ -238,19 +238,21 @@ class NaturalSpeech2(nn.Module):
     # training loss (differentiable: `loss.backward()` runs the hand-written backward kernels)
     # ------------------------------------------------------------------------------------------
     def forward(self, audio, text=None, text_lens=None, mel=None, mel_lens=None, codes=None, prompt=None,
-                pitch=None, *args, prompt_enc=None, cond=None, times=None, noise=None, **kwargs):
+                pitch=None, *args, prompt_enc=None, cond=None, times=None, noise=None, duration=None, **kwargs):
         """ns2.py:1503-1684 -> scalar diffusion loss (the only term the reference returns, SURVEY T11).
-        Extra keyword-only arguments: `prompt_enc`/`cond` (precomputed conditioning) and `times`/`noise`
-        (inject the two random draws of ns2.py:1621,1625 — used by the parity tests)."""
+        Extra keyword-only arguments: `prompt_enc`/`cond` (precomputed conditioning), `times`/`noise`
+        (inject the two random draws of ns2.py:1621,1625 — used by the parity tests) and `duration` (per-phoneme frame
+        counts, handed to the conditioner only when given: encoders.Conditioner takes them in place of an aligner)."""
         is_raw_audio = audio.ndim == 2
         if self.conditional and not (_exists(prompt_enc) and _exists(cond)):
             if not _exists(self.conditioner):
                 raise NotImplementedError(
                     "conditional training needs prompt_enc= and cond= or a `conditioner` callable (the "
                     "reference's encoders + aligner are outside the accelerated path)")
+            extra = {} if duration is None else {"duration": duration}
             prompt_enc, cond = self.conditioner(audio=audio, text=text, text_lens=text_lens, mel=mel,
                                                 mel_lens=mel_lens, prompt=self.process_prompt(prompt),
-                                                pitch=pitch, mode="train")
+                                                pitch=pitch, mode="train", **extra)
         assert not (is_raw_audio and not _exists(self.codec)), \
             "codec must be passed in if one were to train on raw audio"
         if is_raw_audio:

@@ -13,16 +13,27 @@ unchanged; the module tree only HOLDS parameters, the math goes through `ops` (l
   Transformer layer               RMSNorm kernel -> fused QKV GEMM -> flash attention -> out-proj GEMM (+residual,
                                   fp32 stream) -> RMSNorm -> GEGLU GEMM -> out GEMM (+residual)
 
-Forward / inference only (dropout is the identity in eval mode; the reference's training-mode dropout and the
-backward of these encoders are not restated).  Attention masks are not supported (`mask=None` is what
-NaturalSpeech2.forward / .sample pass, ns2.py:1475-1476, 1538-1539).  Numerics follow the denoiser: bf16 tensor-core
-operands, fp32 accumulation, fp32 residual stream and norm statistics.
+Training: in `train()` mode with gradients enabled (and parameters that require them) `SpeechPromptEncoder.forward` and
+`PhonemeEncoder.forward` record ONE autograd node each (`_EncoderFunction`, the pattern of training.DenoiserFunction).
+Its forward runs exactly the inference kernels (bit-identical output) and keeps the activations the backward needs;
+its backward walks the encoder in reverse:
+  plain Transformer      out-proj / FF wgrad + dgrad GEMMs on transposed packs, attention_bwd, geglu_bwd (on a
+                         plain-epilogue recomputation of the GEGLU input), rmsnorm_film_bwd(gamma=...)
+  k=9 conv + SiLU        pre-activation recomputed with a plain-epilogue GEMM, ops.silu_bwd, one ops.wgrad per tap
+                         ("same" padding: shifts +4..-4, causal: 8..0), dgrad = one nine-segment GEMM with mirrored
+                         shifts (the prompt encoder's first conv needs none: its input comes from the codec)
+  nn.Embedding           ops.embedding_bwd (scatter-add; the pad row receives gradient, as in the reference)
+Dropout stays the identity in training, as in the denoiser (the reference's conv / attention dropout is not drawn).
+Attention masks are not supported (`mask=None` is what NaturalSpeech2.forward / .sample pass, ns2.py:1475-1476,
+1538-1539).  Numerics follow the denoiser: bf16 tensor-core operands, fp32 accumulation, fp32 residual stream and norm
+statistics.
 """
 from __future__ import annotations
 
 from typing import Dict, Optional, Sequence, Tuple
 
 import torch
+import torch.nn.functional as F
 from torch import nn
 
 from . import _lib, ops
@@ -58,12 +69,56 @@ def _conv_segs(c_in: int, kernel: int, first_shift: int):
     return [(0, t * c_in, c_in, first_shift - t, 0) for t in range(kernel)]
 
 
+def _conv_dgrad_segs(c_out: int, kernel: int, first_shift: int):
+    """Segments of the input gradient of `_conv_segs` on the transposed pack ([in][tap][out]): tap t reads d out at
+    n + (first_shift - t), the mirrored shift."""
+    return [(0, t * c_out, c_out, t - first_shift, 0) for t in range(kernel)]
+
+
+def _transpose_conv(w: torch.Tensor, kernel: int) -> torch.Tensor:
+    """(O, k*I) tap-major pack -> (I, k*O) [in][tap][out] pack for the dgrad GEMM."""
+    O = w.shape[0]
+    return w.view(O, kernel, -1).permute(2, 1, 0).reshape(-1, kernel * O).contiguous()
+
+
+def _records_graph(m: nn.Module) -> bool:
+    return m.training and torch.is_grad_enabled() and any(p.requires_grad for p in m.parameters())
+
+
+class _EncoderFunction(torch.autograd.Function):
+    """One autograd node for a whole encoder: forward = the inference kernels keeping activations, backward = the
+    hand-written kernels (`_train_backward`).  `reducer` (parallel.GradReducer or None) receives the parameter
+    gradients when the backward ends."""
+
+    @staticmethod
+    def forward(ctx, enc, reducer, x, *params):
+        with torch.no_grad():
+            out, saved = enc._train_forward(x)
+        ctx.enc, ctx.reducer, ctx.saved = enc, reducer, saved
+        return out
+
+    @staticmethod
+    def backward(ctx, d_out):
+        enc = ctx.enc
+        with torch.no_grad():
+            grads = enc._train_backward(ctx.saved, d_out)
+        ctx.saved = None
+        missing = [n for n, _ in enc.named_parameters() if n not in grads]
+        if missing:
+            raise RuntimeError(f"encoder backward produced no gradient for {missing[:4]}...")
+        if ctx.reducer is not None:
+            ctx.reducer.reduce_all(grads)
+            ctx.reducer.finish()
+        return (None, None, None, *[grads[n].reshape(p.shape).to(p.dtype) for n, p in enc.named_parameters()])
+
+
 class _EncoderBase(nn.Module):
-    """Packing cache + the shared transformer forward."""
+    """Packing cache + the shared transformer forward / backward."""
 
     def _init_cache(self):
         self._packed: Optional[Dict[str, torch.Tensor]] = None
         self._packed_sig = None
+        self.grad_reducer = None   # parallel.GradReducer: all-reduce of this encoder's gradients (data parallel)
         self.register_load_state_dict_post_hook(lambda module, incompatible: module.invalidate_packed())
 
     def invalidate_packed(self) -> None:
@@ -83,6 +138,20 @@ class _EncoderBase(nn.Module):
                 self._packed = self._pack()
             self._packed_sig = sig
         return self._packed
+
+    def packed_transposed(self) -> Dict[str, torch.Tensor]:
+        """bf16 transposed twins of `packed()` for the dgrad GEMMs of the backward pass, rebuilt with it."""
+        P = self.packed()
+        if getattr(self, "_packed_T_of", None) is not P:
+            with torch.no_grad():
+                self._packed_T = self._pack_transposed(P)
+            self._packed_T_of = P
+        return self._packed_T
+
+    def _pack_transposed_transformer(self, P, T, depth: int) -> None:
+        for l in range(depth):
+            for k in ("qkv", "o", "w1", "w2"):
+                T[f"l{l}_{k}"] = P[f"l{l}_{k}"].t().contiguous()
 
     # ---- transformer ----
     def _pack_transformer(self, P: Dict[str, torch.Tensor], tr: _PlainTransformerParams, dim: int) -> None:
@@ -132,6 +201,106 @@ class _EncoderBase(nn.Module):
             return out
         return x
 
+    def _transformer_train(self, x: torch.Tensor, tr: _PlainTransformerParams, P, heads: int) -> list:
+        """`_transformer` (same kernels, same order: bit-identical x) keeping every layer's activations."""
+        if "final_g" in P:
+            raise NotImplementedError("training a Transformer with final_norm=True is not supported")
+        B, N, D = x.shape
+        dev, bf = x.device, torch.bfloat16
+        e = lambda *s, dt=bf: torch.empty(*s, device=dev, dtype=dt)  # noqa: E731
+        inner = heads * 64
+        layers = []
+        for l in range(len(tr.layers)):
+            Dp = P[f"l{l}_w2"].shape[1]
+            L = {"x_in": x.clone()}
+            L["h1"] = ops.rmsnorm_film(x, e(B, N, D), gamma=P[f"l{l}_g1"])
+            L["qkv"] = ops.gemm(L["h1"], P[f"l{l}_qkv"], e(B, N, 3 * inner), n=3 * inner, epilogue=ops.EPI_BF16)
+            L["lse"] = e(B, heads, N, dt=torch.float32)
+            qkv = L["qkv"]
+            L["o"] = ops.attention(qkv[:, :, :inner], qkv[:, :, inner:2 * inner], qkv[:, :, 2 * inner:], e(B, N, inner),
+                                   heads=heads, lse=L["lse"])
+            ops.gemm(L["o"], P[f"l{l}_o"], x, n=D, epilogue=ops.EPI_F32, resid=x)
+            L["x_mid"] = x.clone()
+            L["h2"] = ops.rmsnorm_film(x, e(B, N, D), gamma=P[f"l{l}_g2"])
+            L["g"] = ops.gemm(L["h2"], P[f"l{l}_w1"], e(B, N, Dp), n=2 * Dp, epilogue=ops.EPI_GEGLU, bias=P[f"l{l}_b1"])
+            ops.gemm(L["g"], P[f"l{l}_w2"], x, n=D, epilogue=ops.EPI_F32, bias=P[f"l{l}_b2"], resid=x)
+            layers.append(L)
+        return layers
+
+    def _transformer_backward(self, layers: list, tr: _PlainTransformerParams, P, T, heads: int, dxr: torch.Tensor,
+                              dxr_bf: torch.Tensor, grads: Dict[str, torch.Tensor]) -> None:
+        """Transformer backward (ns2.py:1110-1115): dxr (fp32 gradient of the output, updated in place) becomes the
+        gradient of the input; dxr_bf its bf16 copy.  Parameter gradients go to `grads` under the reference's names."""
+        B, N, D = dxr.shape
+        dev, bf = dxr.device, torch.bfloat16
+        e = lambda *s: torch.empty(*s, device=dev, dtype=bf)  # noqa: E731
+        z = lambda *s: torch.zeros(*s, device=dev, dtype=torch.float32)  # noqa: E731
+        inner = heads * 64
+        for l in reversed(range(len(tr.layers))):
+            L = layers[l]
+            pfx = f"transformer.layers.{l}."
+            ff = tr.layers[l][3]
+            Di = ff[-1].weight.shape[1]
+            Dp = P[f"l{l}_w2"].shape[1]
+            # ---- feed-forward: x += W2 GEGLU(W1 RMSNorm(x) + b1) + b2 ----
+            grads[pfx + f"3.{len(ff) - 1}.weight"] = ops.wgrad(dxr_bf, L["g"], z(D, Dp), n=D, k=Dp)[:, :Di]
+            grads[pfx + f"3.{len(ff) - 1}.bias"] = ops.colsum(dxr_bf, z(D))
+            d_g = ops.gemm(dxr_bf, T[f"l{l}_w2"], e(B, N, Dp), n=Dp, epilogue=ops.EPI_BF16)
+            pre = ops.gemm(L["h2"], P[f"l{l}_w1"], e(B, N, 2 * Dp), n=2 * Dp, epilogue=ops.EPI_BF16, bias=P[f"l{l}_b1"])
+            ops.geglu_bwd(pre, d_g)                                                      # pre <- d pre
+            dW1 = ops.wgrad(pre, L["h2"], z(2 * Dp, D), n=2 * Dp, k=D).view(Dp // 128, 2, 128, D)
+            db1 = ops.colsum(pre, z(2 * Dp)).view(Dp // 128, 2, 128)
+            grads[pfx + "3.0.weight"] = torch.cat((dW1[:, 0].reshape(Dp, D)[:Di], dW1[:, 1].reshape(Dp, D)[:Di]), dim=0)
+            grads[pfx + "3.0.bias"] = torch.cat((db1[:, 0].reshape(Dp)[:Di], db1[:, 1].reshape(Dp)[:Di]), dim=0)
+            dh2 = ops.gemm(pre, T[f"l{l}_w1"], e(B, N, D), n=D, epilogue=ops.EPI_BF16)
+            dg2 = z(D)
+            ops.rmsnorm_film_bwd(L["x_mid"], dh2, dxr, dxr_bf, rows_per_batch=N, gamma=P[f"l{l}_g2"], dgamma=dg2)
+            grads[pfx + "2.gamma"] = dg2
+            # ---- attention: x += Wo attn(Wqkv RMSNorm(x)) ----
+            grads[pfx + "1.to_out.weight"] = ops.wgrad(dxr_bf, L["o"], z(D, inner), n=D, k=inner)
+            d_o = ops.gemm(dxr_bf, T[f"l{l}_o"], e(B, N, inner), n=inner, epilogue=ops.EPI_BF16)
+            qkv = L["qkv"]
+            d_qkv = e(B, N, 3 * inner)
+            dq = z(B, N, inner)
+            ops.attention_bwd(qkv[:, :, :inner], qkv[:, :, inner:2 * inner], qkv[:, :, 2 * inner:], L["o"], d_o, L["lse"],
+                              dq, d_qkv[:, :, inner:2 * inner], d_qkv[:, :, 2 * inner:], heads=heads)
+            d_qkv[:, :, :inner].copy_(dq)   # fp32 accumulator -> bf16 slot (layout glue)
+            dWqkv = ops.wgrad(d_qkv, L["h1"], z(3 * inner, D), n=3 * inner, k=D)
+            grads[pfx + "1.to_q.weight"] = dWqkv[:inner]
+            grads[pfx + "1.to_kv.weight"] = dWqkv[inner:]
+            dh1 = ops.gemm(d_qkv, T[f"l{l}_qkv"], e(B, N, D), n=D, epilogue=ops.EPI_BF16)
+            dg1 = z(D)
+            ops.rmsnorm_film_bwd(L["x_in"], dh1, dxr, dxr_bf, rows_per_batch=N, gamma=P[f"l{l}_g1"], dgamma=dg1)
+            grads[pfx + "0.gamma"] = dg1
+
+    def _conv_silu_backward(self, x_in: torch.Tensor, w: torch.Tensor, w_t: Optional[torch.Tensor], bias: torch.Tensor,
+                            d_out: torch.Tensor, first_shift: int, grads: Dict[str, torch.Tensor], name: str,
+                            d_in_f32: bool = False) -> Optional[torch.Tensor]:
+        """Backward of out = silu(conv_k(x_in) + bias) (segmented GEMM): d_out bf16 (B, N, C_out) -> weight / bias
+        gradients under `name`, and d x_in ((B, N, C_in) bf16, or fp32 with d_in_f32) when the transposed pack w_t is
+        given."""
+        B, N, c_in = x_in.shape
+        c_out = w.shape[0]
+        k = w.shape[1] // c_in
+        dev = x_in.device
+        pre = ops.gemm(x_in, w, torch.empty(B, N, c_out, device=dev, dtype=torch.bfloat16), n=c_out,
+                       epilogue=ops.EPI_BF16, segs=_conv_segs(c_in, k, first_shift), bias=bias)   # recompute
+        ops.silu_bwd(pre, d_out)                                                                  # pre <- d pre
+        dW = torch.zeros(c_out, k * c_in, device=dev)
+        for t in range(k):   # tap t multiplies x[n - (first_shift - t)]
+            ops.wgrad(pre, x_in, dW[:, t * c_in:(t + 1) * c_in], n=c_out, k=c_in, shift_units=first_shift - t)
+        grads[name + ".weight"] = dW.view(c_out, k, c_in).permute(0, 2, 1)
+        grads[name + ".bias"] = ops.colsum(pre, torch.zeros(c_out, device=dev))
+        if w_t is None:
+            return None
+        out = torch.empty(B, N, c_in, device=dev, dtype=torch.float32 if d_in_f32 else torch.bfloat16)
+        return ops.gemm(pre, w_t, out, n=c_in, epilogue=ops.EPI_F32 if d_in_f32 else ops.EPI_BF16,
+                        segs=_conv_dgrad_segs(c_out, k, first_shift))
+
+    def _start_backward(self, d_out: torch.Tensor):
+        dxr = d_out.float().contiguous().clone()        # fp32 residual-stream gradient, updated in place
+        return dxr, ops.cast_bf16(dxr, torch.empty(dxr.shape, device=dxr.device, dtype=torch.bfloat16))
+
 
 def _check_transformer_dims(dim: int, dim_head: int):
     if dim_head != 64:
@@ -175,23 +344,52 @@ class SpeechPromptEncoder(_EncoderBase):
         self._pack_transformer(P, self.transformer, self.dim_out)
         return P
 
-    @torch.no_grad()
+    def _pack_transposed(self, P) -> Dict[str, torch.Tensor]:
+        T = {f"c{i}_w": _transpose_conv(P[f"c{i}_w"], self.kernel_size) for i in range(1, len(self._convs()))}
+        self._pack_transposed_transformer(P, T, len(self.transformer.layers))
+        return T
+
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         assert x.shape[-1] == self.dim
         if not x.is_cuda:
             raise ValueError("SpeechPromptEncoder: input must be a CUDA tensor (the ns2_b200 ops have no CPU path)")
+        if _records_graph(self):
+            return _EncoderFunction.apply(self, self.grad_reducer, x, *self.parameters())
+        with torch.no_grad():
+            return self._train_forward(x, keep=False)[0]
+
+    def _train_forward(self, x: torch.Tensor, keep: bool = True):
+        """Inference forward; with keep=True also the activations of `_train_backward` (same kernels, same output)."""
         P = self.packed()
         B, N, _ = x.shape
         dev, bf = x.device, torch.bfloat16
         h = ops.cast_bf16(x.float().contiguous(), torch.empty(B, N, self.dim, device=dev, dtype=bf))
         convs = self._convs()
+        conv_in = []
         for i, c in enumerate(convs):
             last = i == len(convs) - 1
             out = torch.empty(B, N, c.out_channels, device=dev, dtype=torch.float32 if last else bf)
             ops.gemm(h, P[f"c{i}_w"], out, n=c.out_channels, epilogue=ops.EPI_F32 if last else ops.EPI_BF16,
                      segs=_conv_segs(c.in_channels, self.kernel_size, self.padding), bias=P[f"c{i}_b"], flags=_SILU)
+            if keep:
+                conv_in.append(h)
             h = out
-        return self._transformer(h, self.transformer, P, self.heads)
+        if not keep:
+            return self._transformer(h, self.transformer, P, self.heads), None
+        layers = self._transformer_train(h, self.transformer, P, self.heads)
+        return h, {"conv_in": conv_in, "layers": layers}
+
+    def _train_backward(self, S, d_out: torch.Tensor) -> Dict[str, torch.Tensor]:
+        P, T = self.packed(), self.packed_transposed()
+        grads: Dict[str, torch.Tensor] = {}
+        dxr, dxr_bf = self._start_backward(d_out)
+        self._transformer_backward(S["layers"], self.transformer, P, T, self.heads, dxr, dxr_bf, grads)
+        d_h = dxr_bf                        # gradient of the last conv's (SiLU) output
+        for i in reversed(range(len(self._convs()))):
+            # conv i is module conv.{2i+1} (Rearrange, then [Conv1d, SiLU] pairs); its input needs no gradient for i = 0
+            d_h = self._conv_silu_backward(S["conv_in"][i], P[f"c{i}_w"], T.get(f"c{i}_w"), P[f"c{i}_b"], d_h,
+                                           self.padding, grads, f"conv.{2 * i + 1}")
+        return grads
 
 
 class PhonemeEncoder(_EncoderBase):
@@ -225,7 +423,11 @@ class PhonemeEncoder(_EncoderBase):
         self._pack_transformer(P, self.transformer, self.dim_hidden)
         return P
 
-    @torch.no_grad()
+    def _pack_transposed(self, P) -> Dict[str, torch.Tensor]:
+        T = {"c_w": _transpose_conv(P["c_w"], self.kernel_size)}
+        self._pack_transposed_transformer(P, T, len(self.transformer.layers))
+        return T
+
     def forward(self, x, mask=None) -> torch.Tensor:
         if mask is not None:
             raise NotImplementedError("PhonemeEncoder: attention masks are not supported by the sm_90a attention kernel")
@@ -234,16 +436,36 @@ class PhonemeEncoder(_EncoderBase):
             x = self.tokenizer.texts_to_tensor_ids(x).to(self.token_emb.weight.device)
         if not x.is_cuda:
             raise ValueError("PhonemeEncoder: input must be a CUDA tensor (the ns2_b200 ops have no CPU path)")
+        if _records_graph(self):
+            return _EncoderFunction.apply(self, self.grad_reducer, x, *self.parameters())
+        with torch.no_grad():
+            return self._train_forward(x, keep=False)[0]
+
+    def _train_forward(self, x: torch.Tensor, keep: bool = True):
+        """Inference forward; with keep=True also the activations of `_train_backward` (same kernels, same output)."""
         P = self.packed()
         B, T = x.shape
         dev, bf = x.device, torch.bfloat16
-        e = ops.embedding_bf16(x.long().contiguous(), P["emb"], torch.empty(B, T, self.dim, device=dev, dtype=bf),
-                               self.pad_id)
+        ids = x.long().contiguous()
+        e = ops.embedding_bf16(ids, P["emb"], torch.empty(B, T, self.dim, device=dev, dtype=bf), self.pad_id)
         h = torch.empty(B, T, self.dim_hidden, device=dev, dtype=torch.float32)
         # CausalConv1d: left padding dilation*(k-1) (ns2.py:592-595) -> tap t reads position n - (k-1-t)
         ops.gemm(e, P["c_w"], h, n=self.dim_hidden, epilogue=ops.EPI_F32,
                  segs=_conv_segs(self.dim, self.kernel_size, self.kernel_size - 1), bias=P["c_b"], flags=_SILU)
-        return self._transformer(h, self.transformer, P, self.heads)
+        if not keep:
+            return self._transformer(h, self.transformer, P, self.heads), None
+        layers = self._transformer_train(h, self.transformer, P, self.heads)
+        return h, {"ids": ids, "emb": e, "layers": layers}
+
+    def _train_backward(self, S, d_out: torch.Tensor) -> Dict[str, torch.Tensor]:
+        P, T = self.packed(), self.packed_transposed()
+        grads: Dict[str, torch.Tensor] = {}
+        dxr, dxr_bf = self._start_backward(d_out)
+        self._transformer_backward(S["layers"], self.transformer, P, T, self.heads, dxr, dxr_bf, grads)
+        d_e = self._conv_silu_backward(S["emb"], P["c_w"], T["c_w"], P["c_b"], dxr_bf, self.kernel_size - 1, grads,
+                                       "conv.1", d_in_f32=True)
+        grads["token_emb.weight"] = ops.embedding_bwd(S["ids"], d_e, torch.zeros_like(P["emb"]), self.pad_id)
+        return grads
 
 
 # --------------------------------------------------------------------------------------------------
@@ -418,33 +640,89 @@ def f0_to_coarse(f0: torch.Tensor, f0_bin: int = 256, f0_max: float = 1100.0, f0
     return (f0_mel + 0.5).int()
 
 
-def frames_to_text_index(duration: torch.Tensor) -> torch.Tensor:
+def average_over_durations(values: torch.Tensor, durs: torch.Tensor) -> torch.Tensor:
+    """Per-phoneme mean of frame-level values (utils/utils.py:4-26): values (B, C, L), durs (B, T) frame counts ->
+    (B, C, T).  Only NONZERO frames are averaged (unvoiced pitch is 0); a phoneme without one gets 0.  Prefix sums over
+    the frames, differenced at each phoneme's [start, end) — (B, T)-sized host glue like f0_to_coarse."""
+    B, C, _ = values.shape
+    end = durs.cumsum(dim=1).long()
+    start = torch.cat((torch.zeros_like(end[:, :1]), end[:, :-1]), dim=1)
+    gather_at = lambda t, at: t.gather(2, at[:, None, :].expand(B, C, at.shape[1]))  # noqa: E731
+    zero_col = torch.zeros(B, C, 1, dtype=values.dtype, device=values.device)
+    prefix = torch.cat((zero_col, values.cumsum(dim=2)), dim=2)
+    voiced = torch.cat((zero_col.long(), (values != 0.0).cumsum(dim=2)), dim=2)
+    total = (gather_at(prefix, end) - gather_at(prefix, start)).to(values.dtype)
+    count = (gather_at(voiced, end) - gather_at(voiced, start)).to(values.dtype)
+    return torch.where(count == 0.0, count, total / count).to(values.dtype)
+
+
+def frames_to_text_index(duration: torch.Tensor, length: Optional[int] = None) -> torch.Tensor:
     """The hard alignment of generate_mask_from_repeats (ns2.py:87-104) as one text index per frame: (B, L) int32,
-    L = max total duration, -1 past a sample's own length.  mask[b, i, n] of the reference == (idx[b, n] == i)."""
+    L = `length` or else the max total duration, -1 past a sample's own length.  mask[b, i, n] of the reference ==
+    (idx[b, n] == i)."""
     repeats = duration.int()
     cumsum = repeats.cumsum(dim=-1)
     lengths = cumsum[:, -1]
-    L = int(lengths.amax().item())
+    L = int(lengths.amax().item()) if length is None else int(length)
     seq = torch.arange(L, device=duration.device).unsqueeze(0).expand(duration.shape[0], L).contiguous()
     idx = torch.searchsorted(cumsum, seq, right=True)          # first i with cumsum[i] > n
     idx = torch.where(seq < lengths.unsqueeze(-1), idx, torch.full_like(idx, -1))
     return idx.int().contiguous()
 
 
+class _ExpandFunction(torch.autograd.Function):
+    """Length regulation with a backward: d phoneme_enc and d pitch_table through ops.expand_encodings_bwd."""
+
+    @staticmethod
+    def forward(ctx, phoneme_enc, pitch_table, coarse, idx, reducer):
+        ctx.save_for_backward(coarse, idx)
+        ctx.reducer, ctx.shapes = reducer, (tuple(phoneme_enc.shape), tuple(pitch_table.shape))
+        ctx.dtypes = (phoneme_enc.dtype, pitch_table.dtype)
+        return ops.expand_encodings(phoneme_enc.detach().float().contiguous(), coarse,
+                                    pitch_table.detach().float().contiguous(), idx)
+
+    @staticmethod
+    def backward(ctx, d_cond):
+        coarse, idx = ctx.saved_tensors
+        d_tok = d_cond.float().transpose(1, 2)          # (B, L, D): the denoiser hands over a token-major buffer
+        if d_tok.stride(2) != 1:
+            d_tok = d_tok.contiguous()
+        dev = d_cond.device
+        d_phon = torch.zeros(ctx.shapes[0], device=dev) if ctx.needs_input_grad[0] else None
+        d_table = torch.zeros(ctx.shapes[1], device=dev) if ctx.needs_input_grad[1] else None
+        ops.expand_encodings_bwd(d_tok, coarse, idx, d_phon, d_table)
+        if ctx.reducer is not None and d_table is not None:
+            ctx.reducer.reduce(d_table)
+            ctx.reducer.finish()
+        return (d_phon.to(ctx.dtypes[0]) if d_phon is not None else None,
+                d_table.to(ctx.dtypes[1]) if d_table is not None else None, None, None, None)
+
+
 def expand_encodings(phoneme_enc: torch.Tensor, duration: torch.Tensor, pitch: torch.Tensor,
-                     pitch_table: torch.Tensor) -> torch.Tensor:
-    """cond (B, D, L) of ns2.py:1478-1483: phoneme encodings + coarse-pitch embeddings repeated `duration` frames."""
-    idx = frames_to_text_index(duration)
+                     pitch_table: torch.Tensor, length: Optional[int] = None, reducer=None) -> torch.Tensor:
+    """cond (B, D, L) of ns2.py:1478-1483: phoneme encodings + coarse-pitch embeddings repeated `duration` frames.
+    pitch: per-phoneme (B, T) f0.  L = `length` (frames past a sample's total duration are 0) or the max total duration.
+    Differentiable with respect to phoneme_enc and pitch_table when autograd tracks them (`reducer`: GradReducer that
+    receives the pitch table's gradient)."""
+    idx = frames_to_text_index(duration, length)
     coarse = f0_to_coarse(pitch.float()).contiguous()
+    if torch.is_grad_enabled() and (phoneme_enc.requires_grad or pitch_table.requires_grad):
+        return _ExpandFunction.apply(phoneme_enc, pitch_table, coarse, idx, reducer)
     return ops.expand_encodings(phoneme_enc.float().contiguous(), coarse, pitch_table.detach().float().contiguous(), idx)
 
 
 class Conditioner(nn.Module):
-    """The per-sample conditional front end of `NaturalSpeech2.sample` (ns2.py:1472-1483) as the `conditioner`
-    callable of `naturalspeech2_pytorch_b200.NaturalSpeech2`: prompt latents + phoneme ids -> (prompt_enc, cond).
-    Sub-module names follow the reference's NaturalSpeech2 attributes (ns2.py:1231-1236), so the matching slices of a
-    reference checkpoint load with `load_state_dict(..., strict=False)`.  The training-time front end (mel, pitch
-    extraction, aligner network, ns2.py:1537-1583) is not built: `mode="train"` raises."""
+    """The per-sample conditional front end of NaturalSpeech2 (ns2.py:1472-1483 sampling, 1537-1583 training) as the
+    `conditioner` callable of `naturalspeech2_pytorch_b200.NaturalSpeech2`: prompt latents + phoneme ids -> (prompt_enc,
+    cond).  Sub-module names follow the reference's NaturalSpeech2 attributes (ns2.py:1231-1236), so the matching slices
+    of a reference checkpoint load with `load_state_dict(..., strict=False)`.
+
+    mode="train" takes the durations from the caller: `duration` (B, T) frame counts per phoneme (the reference
+    aligner's `aln_hard`, from an external aligner or the reference's Aligner) and frame-level `pitch` (B, L) /
+    (B, 1, L).  The aligner network, its losses and the duration / pitch predictor are not run: in the reference they
+    only feed `aux_loss`, which is never returned (ns2.py:1600-1602), so the diffusion loss is the only gradient path
+    into the prompt encoder, the phoneme encoder and `pitch_emb`.  `grad_reducer` (parallel.GradReducer) all-reduces
+    their gradients in data-parallel training."""
 
     def __init__(self, *, dim_codebook=128, num_phoneme_tokens=None, tokenizer=None, duration_pitch_dim=512,
                  pitch_emb_dim=256, pitch_emb_pp_hidden_dim=512):
@@ -453,14 +731,62 @@ class Conditioner(nn.Module):
         self.prompt_enc = SpeechPromptEncoder(dim_codebook=dim_codebook)
         self.duration_pitch = DurationPitchPredictor(dim=duration_pitch_dim)
         self.pitch_emb = nn.Embedding(pitch_emb_dim, pitch_emb_pp_hidden_dim)
+        self.grad_reducer = None
 
-    @torch.no_grad()
-    def forward(self, prompt=None, text=None, text_lens=None, mode="sample", **unused):
+    @property
+    def grad_reducer(self):
+        return self._grad_reducer
+
+    @grad_reducer.setter
+    def grad_reducer(self, reducer):
+        self._grad_reducer = reducer
+        self.prompt_enc.grad_reducer = reducer
+        self.phoneme_enc.grad_reducer = reducer
+
+    def forward(self, prompt=None, text=None, text_lens=None, mode="sample", pitch=None, duration=None, **unused):
+        if mode == "train":
+            return self._forward_train(prompt, text, pitch, duration)
         if mode != "sample":
-            raise NotImplementedError("Conditioner: only the sampling front end (ns2.py:1472-1483) is built")
+            raise NotImplementedError(f"Conditioner: unknown mode {mode!r} (sample | train)")
         assert prompt is not None and text is not None
+        with torch.no_grad():
+            prompt_enc = self.prompt_enc(prompt)
+            phoneme_enc = self.phoneme_enc(text)
+            duration, pitch = self.duration_pitch(phoneme_enc, prompt_enc)
+            cond = expand_encodings(phoneme_enc, duration, pitch, self.pitch_emb.weight)
+        return prompt_enc, cond
+
+    def _forward_train(self, prompt, text, pitch, duration):
+        """ns2.py:1538-1583 with the aligner's hard durations given: prompt_enc = prompt_enc(prompt), cond =
+        expand_encodings(phoneme_enc(text), durations, average_over_durations(pitch, durations)) with L = pitch frames."""
+        if duration is None:
+            raise NotImplementedError(
+                "Conditioner(mode='train') needs duration=(B, T) frame counts per phoneme (the aligner's aln_hard): the "
+                "aligner network is not built, durations come from the caller")
+        if prompt is None or text is None or pitch is None:
+            raise ValueError("Conditioner(mode='train') needs prompt=, text= and frame-level pitch= (B, L) or (B, 1, L)")
+        if isinstance(text, (list, tuple)):
+            raise ValueError("Conditioner(mode='train') takes phoneme ids (B, T), not strings")
+        if pitch.dim() == 2:
+            pitch = pitch.unsqueeze(1)
+        if pitch.dim() != 3 or pitch.shape[1] != 1:
+            raise ValueError(f"pitch must be (B, L) or (B, 1, L), got {tuple(pitch.shape)}")
+        B, T = text.shape
+        L = pitch.shape[-1]
+        if tuple(duration.shape) != (B, T) or pitch.shape[0] != B:
+            raise ValueError(f"duration must be (B, T) = {(B, T)} and pitch (B, 1, L); got {tuple(duration.shape)}, "
+                             f"{tuple(pitch.shape)}")
+        if duration.is_floating_point() and not bool((duration == duration.round()).all()):
+            raise ValueError("duration must hold whole frame counts")
+        if bool((duration < 0).any()):
+            raise ValueError("duration must be non-negative")
+        total = duration.long().sum(dim=-1)
+        if bool((total > L).any()):
+            raise ValueError(f"durations sum to {int(total.max())} frames, past the {L} frames of pitch")
         prompt_enc = self.prompt_enc(prompt)
         phoneme_enc = self.phoneme_enc(text)
-        duration, pitch = self.duration_pitch(phoneme_enc, prompt_enc)
-        cond = expand_encodings(phoneme_enc, duration, pitch, self.pitch_emb.weight)
+        with torch.no_grad():
+            ph_pitch = average_over_durations(pitch.float(), duration)[:, 0]      # (B, T), ns2.py:1581
+        cond = expand_encodings(phoneme_enc, duration, ph_pitch, self.pitch_emb.weight, length=L,
+                                reducer=self._grad_reducer)
         return prompt_enc, cond

@@ -712,6 +712,77 @@ def accum_bf16(acc, t, acc_bf=None):
 
 
 # --------------------------------------------------------------------------------------------------
+# backward of the conditioning front end (encoders, pitch embedding, length regulation)
+# --------------------------------------------------------------------------------------------------
+def silu_bwd(pre: torch.Tensor, dout: torch.Tensor, dpre: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """d pre of out = silu(pre) given d out; pre, dout, dpre bf16 contiguous of one size.  dpre defaults to pre (in place)."""
+    lib = _lib.load()
+    dpre = pre if dpre is None else dpre
+    for name, t in (("pre", pre), ("dout", dout), ("dpre", dpre)):
+        _req(t, torch.bfloat16, name)
+        if not t.is_contiguous() or t.numel() != pre.numel():
+            raise ValueError("silu_bwd needs contiguous tensors of equal size")
+    check(lib.ns2_silu_bwd(pre.data_ptr(), dout.data_ptr(), pre.numel(), dpre.data_ptr(), _stream(dpre)), "ns2_silu_bwd")
+    return dpre
+
+
+def embedding_bwd(ids: torch.Tensor, de: torch.Tensor, dtable: torch.Tensor, pad_id: int) -> torch.Tensor:
+    """dtable[ids < 0 ? pad_id : ids] += de (f32, accumulated): the backward of `embedding_bf16`."""
+    lib = _lib.load()
+    _req(ids, torch.int64, "ids")
+    _req(de, torch.float32, "de")
+    _req(dtable, torch.float32, "dtable")
+    if not (ids.is_contiguous() and de.is_contiguous() and dtable.is_contiguous()) or dtable.dim() != 2:
+        raise ValueError("embedding_bwd needs contiguous tensors and a 2-D table")
+    if de.numel() != ids.numel() * dtable.shape[1]:
+        raise ValueError("de must hold one table row per id")
+    check(lib.ns2_embedding_bwd(ids.data_ptr(), ids.numel(), de.data_ptr(), dtable.shape[0], dtable.shape[1], int(pad_id),
+                                dtable.data_ptr(), _stream(dtable)), "ns2_embedding_bwd")
+    return dtable
+
+
+def expand_encodings_bwd(dcond: torch.Tensor, coarse: torch.Tensor, idx: torch.Tensor, dphon: Optional[torch.Tensor],
+                         dtable: Optional[torch.Tensor]):
+    """Backward of `expand_encodings` given d cond TOKEN-MAJOR (B, L, D) f32 (unit channel stride, uniform row stride):
+    dphon (B, T, D) += per-phoneme sums over its frames; dtable[coarse] += the same sums.  Both accumulate."""
+    lib = _lib.load()
+    _req(dcond, torch.float32, "dcond")
+    _req(coarse, torch.int32, "coarse")
+    _req(idx, torch.int32, "idx")
+    B, L, D = dcond.shape
+    if dcond.stride(2) != 1 or (B > 1 and dcond.stride(0) != L * dcond.stride(1)):
+        raise ValueError("dcond must be (B, L, D) with unit channel stride and uniformly strided rows")
+    T = coarse.shape[1]
+    if not (coarse.is_contiguous() and idx.is_contiguous()) or coarse.shape[0] != B or tuple(idx.shape) != (B, L):
+        raise ValueError("expand_encodings_bwd: coarse (B, T) and idx (B, L) must be contiguous int32")
+    rows = 1
+    for name, t in (("dphon", dphon), ("dtable", dtable)):
+        if t is not None:
+            _req(t, torch.float32, name)
+            if not t.is_contiguous() or t.shape[-1] != D:
+                raise ValueError(f"{name} must be contiguous with D columns")
+    if dphon is not None and tuple(dphon.shape) != (B, T, D):
+        raise ValueError("dphon must be (B, T, D)")
+    if dtable is not None:
+        rows = dtable.shape[0]
+    check(lib.ns2_expand_encodings_bwd(dcond.data_ptr(), max(dcond.stride(1), D), coarse.data_ptr(), rows, idx.data_ptr(),
+                                       B, T, D, L, _ptr(dphon), _ptr(dtable), _stream(dcond)), "ns2_expand_encodings_bwd")
+    return dphon, dtable
+
+
+def add_rows_bcast(x: torch.Tensor, v: torch.Tensor, scale: float = 1.0) -> torch.Tensor:
+    """x[b, r, :] += scale * v[b, :] in place; x (B, R, D) f32 contiguous, v (B, D) f32 contiguous."""
+    lib = _lib.load()
+    _req(x, torch.float32, "x")
+    _req(v, torch.float32, "v")
+    B, R, D = x.shape
+    if not (x.is_contiguous() and v.is_contiguous()) or tuple(v.shape) != (B, D):
+        raise ValueError("add_rows_bcast: x (B, R, D) and v (B, D) must be contiguous")
+    check(lib.ns2_add_rows_bcast(x.data_ptr(), B, R, D, v.data_ptr(), float(scale), _stream(x)), "ns2_add_rows_bcast")
+    return x
+
+
+# --------------------------------------------------------------------------------------------------
 # Monotonic alignment search (aligner.py:88-122)
 # --------------------------------------------------------------------------------------------------
 def maximum_path(value: torch.Tensor, mask: torch.Tensor, neg_const: float = float("-inf"), *,

@@ -16,6 +16,10 @@ The (B,)-sized conditioning vectors — timestep embedding (LearnedSinusoidalPos
 839-843) and prompt vector (mean-pool + Linear + SiLU, ns2.py:858-862) — are differentiated with torch autograd on a
 recomputation: 32 x 2048 values each, host-side glue like the noise schedules.  `prompt_mask` is unsupported (as in
 the inference path).
+When autograd asks for them (an encoder upstream: encoders.Conditioner in train mode) the backward also returns
+d loss / d prompt (perceiver context projection dgrad + the mean-pool's share, spread by ops.add_rows_bcast) and
+d loss / d cond (one dgrad GEMM through the aligned-condition projection, token-major, handed over as a channel-first
+view); otherwise nothing extra runs.  `x` and `times` stay non-differentiable (latents come from the codec).
 """
 from __future__ import annotations
 
@@ -57,6 +61,9 @@ def pack_transposed(model) -> Dict[str, torch.Tensor]:
     T["pred_w"] = t(P["pred_w"])
     T["wn_init_w"] = P["wn_init_w"].view(D, 3, D).permute(2, 1, 0).reshape(D, 3 * D).contiguous()   # [in][tap][out]
     if model.condition_on_prompt:
+        T["cond_w"] = t(P["cond_w"])                                   # (dim_prompt, D): d cond
+        if "pr_proj_w" in P:
+            T["pr_proj_w"] = t(P["pr_proj_w"])                         # (dim_prompt, D): d prompt
         T["x_kv_all"] = t(P["x_kv_all"])                               # (D, depth*2*inner)
         for l in range(model.depth):
             T[f"l{l}_xq"] = t(P[f"l{l}_xq"])
@@ -202,10 +209,14 @@ def train_forward(model, x: torch.Tensor, times: torch.Tensor, prompt=None, cond
     return out, S
 
 
-def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None) -> Dict[str, torch.Tensor]:
+def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grads=None) -> Dict[str, torch.Tensor]:
     """Gradients of every parameter (keys of `model.named_parameters()`), given d(loss)/d(prediction).
     `reducer` (parallel.GradReducer): finished gradient buffers are handed over layer by layer, so that their
-    all-reduce overlaps the rest of the backward pass."""
+    all-reduce overlaps the rest of the backward pass.
+    `input_grads`: a dict whose keys "prompt" / "cond" (present = wanted) receive d(loss)/d(prompt) (B, Np, dim_prompt)
+    and d(loss)/d(cond) (B, dim_prompt, Lc) — per-sample gradients, kept out of the reducer."""
+    want_prompt = input_grads is not None and "prompt" in input_grads
+    want_cond = input_grads is not None and "cond" in input_grads
     flush = (lambda: reducer.reduce_all(grads)) if reducer is not None else (lambda: None)
     B, N = S["B"], S["N"]
     D, G, inner, H = model.dim, model.wavenet_layers, model.inner, model.heads
@@ -303,7 +314,15 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None) -> Dict[st
         flush()   # this layer's gradients are final: their all-reduce overlaps the layers still to come
 
     if conditional:
-        _conditioning_backward_tokens(model, S, T, d_xkv, grads)
+        # d of the perceiver context: bf16 d(proj) when it has a projection, else fp32 d(prompt)
+        d_ctx = _conditioning_backward_tokens(model, S, T, d_xkv, grads)
+        if want_prompt:
+            # d prompt, term (a): through the perceiver's context projection (identity when dim_prompt == dim)
+            if "pr_proj_w" in P:
+                input_grads["prompt"] = ops.gemm(d_ctx, T["pr_proj_w"], e(B, S["pr_Np"], model.dim_prompt, dt=torch.float32),
+                                                 n=model.dim_prompt, epilogue=ops.EPI_F32)
+            else:
+                input_grads["prompt"] = d_ctx
     # ---- wavenet: final 1x1 conv, skip sum, 4 stacks of 8 dilation columns, init conv ----
     grads["wavenet.final_conv.weight"] = ops.wgrad(dxr_bf, S["skip"], z(D, D), n=D, k=D).unsqueeze(-1)
     grads["wavenet.final_conv.bias"] = ops.colsum(dxr_bf, z(D))
@@ -375,6 +394,12 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None) -> Dict[st
         grads["cond_to_model_dim.weight"] = ops.wgrad(d_cp, S["cond_bf"], z(D, model.dim_prompt), n=D,
                                                       k=model.dim_prompt).unsqueeze(-1)
         grads["cond_to_model_dim.bias"] = ops.colsum(d_cp, z(D))
+        if want_cond:
+            # d cond = d_cp @ W (1x1 conv dgrad), token-major; curtailed frames (n >= N) stay exact zeros.  Returned as
+            # the channel-first view cond has, so nothing is transposed.
+            d_cond = ops.gemm(d_cp, T["cond_w"], e(B, Lc, model.dim_prompt, dt=torch.float32), n=model.dim_prompt,
+                              epilogue=ops.EPI_F32)
+            input_grads["cond"] = d_cond.permute(0, 2, 1)
 
     # ---- FiLM projections (one stacked matrix) and the timestep embedding ----
     rows = film.shape[1]
@@ -389,8 +414,11 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None) -> Dict[st
         with torch.enable_grad():
             lw = lin.weight.detach().float().requires_grad_(True)
             lb = lin.bias.detach().float().requires_grad_(True)
-            F.silu(F.linear(S["prompt_mean"], lw, lb)).backward(d_pc * (~S["drop"])[:, None])
+            mean = S["prompt_mean"].detach().requires_grad_(want_prompt)
+            F.silu(F.linear(mean, lw, lb)).backward(d_pc * (~S["drop"])[:, None])
         grads["to_prompt_cond.1.weight"], grads["to_prompt_cond.1.bias"] = lw.grad, lb.grad
+        if want_prompt:   # d prompt, term (b): the mean-pool spreads d mean evenly over the prompt rows
+            ops.add_rows_bcast(input_grads["prompt"], mean.grad.contiguous(), 1.0 / S["pr_Np"])
         dt = dt[:, :model.dim_time]
     off = 0
     for s in range(nst):
@@ -482,6 +510,8 @@ def _conditioning_backward_tokens(model, S, T, d_xkv, grads):
         grads["perceiver_resampler.proj_context.weight"] = ops.wgrad(d_proj_bf, S["pr_p_bf"], z(D, model.dim_prompt), n=D,
                                                                      k=model.dim_prompt)
         grads["perceiver_resampler.proj_context.bias"] = ops.colsum(d_proj_bf, z(D))
+        return d_proj_bf
+    return d_proj
 
 
 class DenoiserFunction(torch.autograd.Function):
@@ -493,18 +523,27 @@ class DenoiserFunction(torch.autograd.Function):
             out, saved = train_forward(model, x, times, prompt, cond, cond_drop_prob)
         ctx.model, ctx.saved = model, saved
         ctx.names = [n for n, _ in model.named_parameters()]
+        ctx.in_dtypes = (prompt.dtype if prompt is not None else None, cond.dtype if cond is not None else None)
         return out
 
     @staticmethod
     def backward(ctx, d_out):
+        # d prompt / d cond only when autograd asks for them (an encoder upstream): otherwise no extra kernel runs
+        inputs = {k: None for k, i in (("prompt", 3), ("cond", 4)) if ctx.needs_input_grad[i]}
         with torch.no_grad():
-            grads = train_backward(ctx.model, ctx.saved, d_out, getattr(ctx.model, "grad_reducer", None))
+            grads = train_backward(ctx.model, ctx.saved, d_out, getattr(ctx.model, "grad_reducer", None),
+                                   input_grads=inputs or None)
         ctx.saved = None
         missing = [n for n in ctx.names if n not in grads]
         if missing:
             raise RuntimeError(f"backward produced no gradient for {missing[:4]}...")
-        return (None, None, None, None, None, None, *[grads[n].reshape(p.shape).to(p.dtype)
-                                    for n, p in ctx.model.named_parameters()])
+        d_prompt, d_cond = inputs.get("prompt"), inputs.get("cond")
+        if d_prompt is not None:
+            d_prompt = d_prompt.to(ctx.in_dtypes[0])
+        if d_cond is not None:
+            d_cond = d_cond.to(ctx.in_dtypes[1])
+        return (None, None, None, d_prompt, d_cond, None, *[grads[n].reshape(p.shape).to(p.dtype)
+                                                          for n, p in ctx.model.named_parameters()])
 
 
 class MseRowsFunction(torch.autograd.Function):

@@ -1,0 +1,110 @@
+#!/usr/bin/env python
+"""Conditional training step with the conditioning front end in the loop, timed beside the same step without it.
+
+    python tools/train_cond_bench.py [--steps K] [--warmup W]
+
+  cond_e2e   configs[4] training step (cfg3 denoiser Model(512, depth 12, heads 8, dim_prompt 512), B=32, N=1024) with
+             SpeechPromptEncoder(dim_codebook=128) on (32, 103, 128) prompt latents, PhonemeEncoder on 100 phoneme ids
+             per sample, durations summing to <= 1024 frames, backward through everything (encoders, pitch embedding,
+             the denoiser's input gradients) and fused AdamW over the trained parameters
+  cfg5       the same denoiser step on precomputed (prompt_enc, cond) — bench.py's secondary train_cfg5 workload
+Prints one JSON line: ms / steps per second of both, the encoders' measured share of the step (1 - cfg5 / cond_e2e),
+the card name and its enforced power limit (part of every number).
+"""
+import argparse
+import json
+import subprocess
+import sys
+from pathlib import Path
+
+import torch
+
+sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
+from naturalspeech2_pytorch_b200 import Model, NaturalSpeech2  # noqa: E402
+from naturalspeech2_pytorch_b200.encoders import Conditioner  # noqa: E402
+
+CFG3 = dict(dim=512, depth=12, heads=8, dim_prompt=512, condition_on_prompt=True)
+B, SEQ, NP, T, TOKENS = 32, 1024, 103, 100, 150
+
+
+def card(dev):
+    out = {"name": torch.cuda.get_device_name(dev)}
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(dev.index)],
+                           capture_output=True, text=True, timeout=10)
+        out["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
+    except Exception as e:
+        out["power_limit_w"] = None
+        out["power_limit_error"] = f"{type(e).__name__}: {e}"
+    return out
+
+
+def timed(step, steps, warmup):
+    for _ in range(warmup):
+        step()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(steps):
+        loss = step()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / steps, float(loss)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=3)
+    args = ap.parse_args()
+    dev = torch.device("cuda", 0)
+    torch.manual_seed(0)
+    model = Model(**CFG3).to(dev).train()
+    g = torch.Generator().manual_seed(200)
+    lat = torch.randn(B, SEQ, 512, generator=g).to(dev)
+
+    # ---- cfg5: denoiser on precomputed conditioning ----
+    ns = NaturalSpeech2(model, target_sample_hz=24000)
+    prompt_enc = torch.randn(B, NP, 512, generator=g).to(dev)
+    cond = torch.randn(B, 512, SEQ, generator=g).to(dev)
+    opt = torch.optim.AdamW(model.parameters(), lr=1e-4, fused=True)
+
+    def step_cfg5():
+        opt.zero_grad(set_to_none=True)
+        loss = ns(lat, prompt_enc=prompt_enc, cond=cond)
+        loss.backward()
+        opt.step()
+        return loss.detach()
+
+    ms5, loss5 = timed(step_cfg5, args.steps, args.warmup)
+    del opt
+
+    # ---- cond_e2e: the encoders trained jointly ----
+    cond_net = Conditioner(dim_codebook=128, num_phoneme_tokens=TOKENS).to(dev).train()
+    ns = NaturalSpeech2(model, target_sample_hz=24000, conditioner=cond_net)
+    trained = [*model.parameters(), *cond_net.prompt_enc.parameters(), *cond_net.phoneme_enc.parameters(),
+               *cond_net.pitch_emb.parameters()]   # the duration / pitch predictor only feeds the discarded aux loss
+    opt = torch.optim.AdamW(trained, lr=1e-4, fused=True)
+    prompt = torch.randn(B, NP, 128, generator=g).to(dev)
+    text = torch.randint(0, TOKENS, (B, T), generator=g).to(dev)
+    dur = torch.randint(0, 20, (B, T), generator=g)
+    dur = (dur.float() * (SEQ / dur.sum(-1, keepdim=True).clamp_min(1))).floor().long().to(dev)   # <= SEQ frames
+    pitch = (torch.rand(B, SEQ, generator=g) * 300 + 80).to(dev)
+
+    def step_e2e():
+        opt.zero_grad(set_to_none=True)
+        loss = ns(lat, text=text, prompt=prompt, pitch=pitch, duration=dur)
+        loss.backward()
+        opt.step()
+        return loss.detach()
+
+    ms_e2e, loss_e2e = timed(step_e2e, args.steps, args.warmup)
+    print(json.dumps({
+        "cond_e2e": {"ms_per_step": round(ms_e2e, 3), "steps_per_s": round(1e3 / ms_e2e, 3), "loss": round(loss_e2e, 5)},
+        "cfg5": {"ms_per_step": round(ms5, 3), "steps_per_s": round(1e3 / ms5, 3), "loss": round(loss5, 5)},
+        "encoder_share_of_step": round(1.0 - ms5 / ms_e2e, 4), "steps": args.steps, "warmup": args.warmup,
+        "batch": B, "card": card(dev)}))
+
+
+if __name__ == "__main__":
+    main()

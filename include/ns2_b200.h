@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define NS2_ABI_VERSION 4
+#define NS2_ABI_VERSION 5
 
 typedef void* ns2_stream_t; /* cudaStream_t */
 
@@ -323,6 +323,22 @@ int ns2_rvq_decode(const int64_t* codes, int64_t num_frames, int32_t q, int32_t 
 int ns2_rvq_ce(const float* frames, int64_t num_frames, int32_t d, const float* codebooks,
                const float* cb_norm2, int32_t q, int32_t k, const int64_t* own_codes,
                const int64_t* target_codes, float* ce_scratch, float* loss, ns2_stream_t stream);
+/*    ns2_rvq_ce_bwd  : gradient of ns2_rvq_ce's loss with respect to `frames` (ns2.py:1682, `codec.rq(x_start, codes)`
+ *                      differentiated through x_start).  The subtracted codewords are constants (vector-quantize-pytorch
+ *                      subtracts `quantized.detach()`), so every stage's residual has d r_q / d frames = I and
+ *                        d_frames[f] = row_scale[f / rows_per_sample] * sum_q d_loss / count_q * (u_t - sum_k p_k u_k),
+ *                      u_k = (r_q - c_k) / ||r_q - c_k|| (0 where the distance is 0, torch.cdist's convention),
+ *                      p = softmax(-||r_q - c_k||), t = target_codes[f, q]; stages whose target is -1 add nothing, a
+ *                      stage with no valid target (count_q = 0) adds nothing.  `d_loss` (1 float) and the counts are read
+ *                      on the device: no host synchronisation.  row_scale: optional (num_frames / rows_per_sample) f32,
+ *                      NULL = 1 (NaturalSpeech2 folds d x_start / d pred into it).  coef_scratch: q floats.
+ *                      d_frames: num_frames rows of out_stride floats (>= 128, multiple of 4, 16-byte aligned); only the
+ *                      first 128 columns of valid rows are written.  Deterministic (no atomics). */
+int ns2_rvq_ce_bwd(const float* frames, int64_t num_frames, int32_t d, const float* codebooks,
+                   const float* cb_norm2, int32_t q, int32_t k, const int64_t* own_codes,
+                   const int64_t* target_codes, const float* d_loss, const float* row_scale,
+                   int64_t rows_per_sample, float* coef_scratch, float* d_frames, int64_t out_stride,
+                   ns2_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * 8. Backward pass (what autograd runs for the reference's loss.backward(), README.md:63, ns2.py:1886).

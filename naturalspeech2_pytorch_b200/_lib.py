@@ -17,7 +17,7 @@ NS2_MSE_SCRATCH_PER_SAMPLE = 64
 NS2_RVQ_STATS_LEN = 260
 NS2_OBJ_V, NS2_OBJ_EPS, NS2_OBJ_X0 = 0, 1, 2
 NS2_GEMM_FLAG_SKIP_EPILOGUE, NS2_GEMM_FLAG_WAVENET_ONE_PASS, NS2_GEMM_FLAG_SILU = 1, 2, 4
-NS2_ABI_VERSION = 4
+NS2_ABI_VERSION = 5
 
 
 class GemmSeg(C.Structure):
@@ -128,6 +128,7 @@ SIGNATURES = {
     "ns2_maximum_path_workspace_bytes": (C.c_int64, [_I32, _I32, _I32]),
     "ns2_maximum_path": (C.c_int, [_P, _P, _I32, _I32, _I32, _F, _P, _I64, _P, _P, _P]),
     "ns2_rvq_ce": (C.c_int, [_P, _I64, _I32, _P, _P, _I32, _I32, _P, _P, _P, _P, _P]),
+    "ns2_rvq_ce_bwd": (C.c_int, [_P, _I64, _I32, _P, _P, _I32, _I32, _P, _P, _P, _P, _I64, _P, _P, _I64, _P]),
 }
 
 _lib = None

@@ -85,17 +85,44 @@ class EncodecRVQ(nn.Module):
             return emb
         return self.decoder(emb)
 
-    @torch.no_grad()
     def rq(self, x: torch.Tensor, codes: torch.Tensor):
         """The call `NaturalSpeech2.forward` makes when rvq_cross_entropy_loss_weight != 0 (ns2.py:1682):
         `_, ce_loss = codec.rq(x_start, codes)` — vector-quantize-pytorch's ResidualVQ.forward(x, indices=codes).
         Per stage: logits = -||r_q - c_k|| (Euclidean), cross-entropy against codes[..., q] (ignore_index -1),
-        residual chain through the codec's own nearest codewords; returns (quantized, summed CE loss)."""
+        residual chain through the codec's own nearest codewords; returns (quantized, summed CE loss).
+        The loss is differentiable in `x` when gradients are enabled and `x` requires them (one autograd node whose
+        backward is `ops.rvq_ce_bwd`); `quantized` and the codebooks are constants, as in the reference (its subtracted
+        codewords are detached and the codebooks are buffers)."""
         shp = x.shape[:-1]
-        flat = x.reshape(-1, 128).float().contiguous()
         tgt = codes.reshape(-1, self.num_quantizers).to(torch.int64).contiguous()
-        prep = self._prep()
-        own = ops.rvq_encode(flat, self.codebooks, prep)
-        loss = ops.rvq_ce(flat, self.codebooks, prep[1], own, tgt)
-        emb = ops.rvq_decode(own, self.codebooks)
+        if torch.is_grad_enabled() and x.requires_grad:
+            loss, own = RqCrossEntropyFunction.apply(x.reshape(-1, 128).float().contiguous(), self, tgt)
+        else:
+            with torch.no_grad():
+                flat = x.reshape(-1, 128).float().contiguous()
+                prep = self._prep()
+                own = ops.rvq_encode(flat, self.codebooks, prep)
+                loss = ops.rvq_ce(flat, self.codebooks, prep[1], own, tgt)
+        with torch.no_grad():
+            emb = ops.rvq_decode(own, self.codebooks)
         return emb.view(*shp, 128), loss
+
+
+class RqCrossEntropyFunction(torch.autograd.Function):
+    """`EncodecRVQ.rq`'s cross-entropy loss as one autograd node: the forward runs the same kernels as the no-grad path
+    (own codes, then the CE head), the backward is one `ops.rvq_ce_bwd` call.  Returns (loss, own codes)."""
+
+    @staticmethod
+    def forward(ctx, flat, codec, tgt):
+        prep = codec._prep()
+        own = ops.rvq_encode(flat, codec.codebooks, prep)
+        loss = ops.rvq_ce(flat, codec.codebooks, prep[1], own, tgt)
+        ctx.save_for_backward(flat, codec.codebooks, prep[1], own, tgt)
+        ctx.mark_non_differentiable(own)
+        return loss, own
+
+    @staticmethod
+    def backward(ctx, d_loss, _d_own):
+        flat, codebooks, cn2, own, tgt = ctx.saved_tensors
+        d = ops.rvq_ce_bwd(flat, codebooks, cn2, own, tgt, d_loss.float().reshape(1).contiguous())
+        return d, None, None

@@ -8,7 +8,9 @@ of the reference (PhonemeEncoder, SpeechPromptEncoder, DurationPitchPredictor, A
 aligner.py) are out of scope: for a conditional model pass their outputs directly (`prompt_enc=`, `cond=`) or
 give a `conditioner` callable that produces them (e.g. the reference modules, see INTEGRATION.md).
 
-`forward` is forward-only in this round (no autograd graph; backward kernels are row f1 of SURVEY 8f).
+`forward` returns a differentiable loss: the denoiser records one autograd node (training.DenoiserFunction), and with
+rvq_cross_entropy_loss_weight > 0 the RVQ cross-entropy term records another (`XStartCrossEntropyFunction`) whose
+backward hands d pred to the denoiser's, as the reference's autograd does.
 """
 from __future__ import annotations
 
@@ -21,6 +23,7 @@ import torch
 from torch import nn
 
 from . import ops
+from .codec import EncodecRVQ
 from .model import Model
 
 
@@ -296,9 +299,51 @@ class NaturalSpeech2(nn.Module):
         if self.rvq_cross_entropy_loss_weight == 0 or not _exists(codes):   # ns2.py:1670-1671
             return loss
         # cross entropy of the predicted x_start against the codec's codes (ns2.py:1673-1684)
-        x_start = torch.empty_like(audio)
-        ops.x_start_from_pred(audio, pred.detach(), alpha, sigma, x_start, objective=self.objective)
-        _, ce_loss = self.codec.rq(x_start, codes)
+        if pred.requires_grad and isinstance(self.codec, EncodecRVQ):
+            ce_loss = XStartCrossEntropyFunction.apply(pred, audio, alpha, sigma, self.codec, codes, self.objective)
+        else:   # no gradient wanted, or a codec other than EncodecRVQ (its `rq` gets a constant x_start)
+            x_start = torch.empty_like(audio)
+            ops.x_start_from_pred(audio, pred.detach(), alpha, sigma, x_start, objective=self.objective)
+            _, ce_loss = self.codec.rq(x_start, codes)
         return loss + self.rvq_cross_entropy_loss_weight * ce_loss
 
     p_losses = forward  # the name BASELINE.json's north_star uses; the reference inlines it in forward
+
+
+def x_start_pred_coef(alpha: torch.Tensor, sigma: torch.Tensor, objective: str) -> Optional[torch.Tensor]:
+    """Per-sample d x_start / d pred of ns2.py:1673-1680 ((B,)-sized glue): -sigma (v), -sigma / max(alpha, 1e-10)
+    (eps, safe_div ns2.py:1122-1123), None = 1 (x0)."""
+    if objective == "v":
+        return (-sigma).contiguous()
+    if objective == "eps":
+        return (-sigma / alpha.clamp(min=1e-10)).contiguous()
+    return None
+
+
+class XStartCrossEntropyFunction(torch.autograd.Function):
+    """ns2.py:1673-1682 as one autograd node: x_start from the model output, then `codec.rq`'s CE loss.  The forward
+    launches the kernels of the no-grad path (ops.x_start_from_pred, the codec's own codes, ops.rvq_ce), so the loss
+    is bit-identical to it; the backward is one `ops.rvq_ce_bwd` call whose per-sample row scale is d x_start / d pred,
+    so it returns d pred directly."""
+
+    @staticmethod
+    def forward(ctx, pred, audio, alpha, sigma, codec, codes, objective):
+        x_start = torch.empty_like(audio)
+        ops.x_start_from_pred(audio, pred.detach(), alpha, sigma, x_start, objective=objective)
+        flat = x_start.view(-1, 128)
+        tgt = codes.reshape(-1, codec.num_quantizers).to(torch.int64).contiguous()
+        prep = codec._prep()
+        own = ops.rvq_encode(flat, codec.codebooks, prep)
+        loss = ops.rvq_ce(flat, codec.codebooks, prep[1], own, tgt)
+        coef = x_start_pred_coef(alpha, sigma, objective)
+        ctx.save_for_backward(flat, codec.codebooks, prep[1], own, tgt, coef)
+        ctx.rows_per_sample = audio.shape[1]
+        return loss
+
+    @staticmethod
+    def backward(ctx, d_loss):
+        flat, codebooks, cn2, own, tgt, coef = ctx.saved_tensors
+        d_pred = ops.rvq_ce_bwd(flat, codebooks, cn2, own, tgt, d_loss.float().reshape(1).contiguous(), row_scale=coef,
+                                rows_per_sample=ctx.rows_per_sample)
+        n = ctx.rows_per_sample
+        return d_pred.view(flat.shape[0] // n, n, 128), None, None, None, None, None, None

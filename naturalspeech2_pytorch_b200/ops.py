@@ -554,6 +554,40 @@ def rvq_ce(frames: torch.Tensor, codebooks: torch.Tensor, cn2: torch.Tensor, own
     return loss
 
 
+def rvq_ce_bwd(frames: torch.Tensor, codebooks: torch.Tensor, cn2: torch.Tensor, own_codes: torch.Tensor,
+               target_codes: torch.Tensor, d_loss: torch.Tensor, row_scale: Optional[torch.Tensor] = None,
+               rows_per_sample: int = 1, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """d loss / d frames of `rvq_ce` given d_loss (1-element f32 on the device): frames (F, 128) f32 -> (F, 128) f32.
+    `row_scale` (optional, F / rows_per_sample f32) multiplies each sample's rows; `out` may be a (F, >= 128) f32 view
+    with unit column stride (only its first 128 columns are written)."""
+    lib = _lib.load()
+    _req(frames, torch.float32, "frames")
+    _req(d_loss, torch.float32, "d_loss")
+    cb = codebooks.contiguous()
+    Q, K, D = cb.shape
+    fr = frames.contiguous()
+    F = fr.shape[0]
+    for name, t in (("own_codes", own_codes), ("target_codes", target_codes)):
+        if not (t.is_cuda and t.dtype == torch.int64 and t.is_contiguous() and tuple(t.shape) == (F, Q)):
+            raise ValueError(f"{name} must be a contiguous CUDA int64 tensor of shape (F, Q)")
+    if d_loss.numel() != 1:
+        raise ValueError("d_loss must hold one element")
+    if row_scale is not None:
+        _req(row_scale, torch.float32, "row_scale")
+        if not row_scale.is_contiguous() or rows_per_sample <= 0 or row_scale.numel() * rows_per_sample < F:
+            raise ValueError("row_scale must be contiguous with one value per rows_per_sample rows")
+    if out is None:
+        out = torch.empty((F, D), device=fr.device, dtype=torch.float32)
+    _req(out, torch.float32, "out")
+    if out.dim() != 2 or out.shape[0] != F or out.shape[1] < D:
+        raise ValueError("out must be (F, >= 128)")
+    coef = torch.empty(Q, device=fr.device, dtype=torch.float32)
+    check(lib.ns2_rvq_ce_bwd(fr.data_ptr(), F, D, cb.data_ptr(), cn2.data_ptr(), Q, K, own_codes.data_ptr(),
+                             target_codes.data_ptr(), d_loss.data_ptr(), _ptr(row_scale), int(rows_per_sample),
+                             coef.data_ptr(), out.data_ptr(), out.stride(0), _stream(fr)), "ns2_rvq_ce_bwd")
+    return out
+
+
 # --------------------------------------------------------------------------------------------------
 # backward pass
 # --------------------------------------------------------------------------------------------------

@@ -48,7 +48,9 @@ int ns2_set_sm_limit(int sms);
  *
  * Epilogues (all accumulate in fp32):
  *   NS2_EPI_BF16     out_bf16 = acc0 + bias
- *   NS2_EPI_F32      out_f32  = acc0 + bias (+ resid_f32)           residual add of ns2.py:799,805,809
+ *   NS2_EPI_F32      out_f32  = acc0 + bias (+ resid_f32)           residual add of ns2.py:799,805,809;
+ *                    with resid == out (same row stride) the sum is formed by a TMA reduce-add into out
+ *                    (one fp32 add of the same operands) and resid is never loaded
  *   NS2_EPI_GEGLU    out_bf16[j] = gelu_erf(acc0[gate j] + bias) * (acc0[val j] + bias)   ns2.py:1004-1007;
  *                    B rows must be packed so that each 256-row tile holds 128 value rows followed by
  *                    the 128 matching gate rows (see pack_geglu_weight in the Python host code);

@@ -63,10 +63,7 @@ __global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid
   const int T = (p.kv_len + BKV - 1) / BKV;
 
   if (threadIdx.x == 0) {
-    if ((smem_u32(smem) & 1023u) != 0) {
-      printf("ns2 attn: dynamic shared memory is not 1024-byte aligned\n");
-      __trap();
-    }
+    if ((smem_u32(smem) & 1023u) != 0) __trap();   // dynamic smem not 1024-byte aligned (no printf: see mbar_wait)
     tma_prefetch_desc(&p.tmQ);
     tma_prefetch_desc(&p.tmK);
     tma_prefetch_desc(&p.tmV);

@@ -6,7 +6,8 @@
 //                  through a smem ring (full / empty mbarriers)
 //   warpgroups 1-2 consumers: warpgroup w owns positions [64 (w-1), 64 w) of the tile, issues wgmma m64nBNk16 from the
 //                  shared-memory ring into register accumulators, then runs the epilogue (bias / residual / GEGLU /
-//                  FiLM + gate) straight from the accumulator fragments to global memory
+//                  FiLM + gate) in registers, stages the results in shared memory (two 8 KB boxes per warpgroup)
+//                  and writes them with TMA stores; the in-place fp32 residual is added by TMA reduce-add at L2
 // Tiles are handed out by a static round robin, n fastest so co-resident CTAs share A rows in L2.
 //
 // Replaces, in the reference: nn.Linear GEMMs (ns2.py:1021,1024,1051-1053,783,613,731) and
@@ -16,6 +17,7 @@
 #include "../../include/ns2_b200.h"
 
 #include <atomic>
+#include <type_traits>
 
 namespace ns2 {
 
@@ -27,6 +29,7 @@ constexpr int BK = 64;
 struct GemmDev {
   CUtensorMap tmA;
   CUtensorMap tmB;
+  CUtensorMap tmOut;   // TMA store / reduce-add target: (columns, group, position, batch), clipped at n and a_rows
   int tiles_n, tiles_per_batch, tiles_m, num_tiles;
   int narrow_last;     // groups == 1, n % BN != 0: schedule the partial-width n-tiles after all full-width ones
   int a_rows, n, groups;
@@ -40,6 +43,7 @@ struct GemmDev {
   long long out_rs;
   const float* resid;
   long long resid_rs;
+  int resid_in_place;  // F32 with resid == out (same row stride): out += acc + bias by TMA reduce-add, resid never read
   const float* film;
   long long film_bs;
   int film_gs;
@@ -80,8 +84,10 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmDev& p, int tile) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// epilogue: straight from the wgmma accumulator fragments.  Thread (warp ww of the consumer warpgroup, lane l) holds
-// rows r0 = 16 ww + l/4 and r0 + 8 of its warpgroup's 64 rows, columns 8j + 2(l%4) + {0, 1}:  acc[4j + 2i + k].
+// epilogue: accumulator fragments -> finished values in registers -> 128-byte-swizzled shared-memory staging box
+// (64 rows x 128 bytes per consumer warpgroup, double-buffered) -> TMA store, or a TMA reduce-add for the in-place
+// residual update.  Thread (warp ww of the consumer warpgroup, lane l) holds rows 16 ww + l/4 + 8i of its warpgroup's
+// 64 rows, columns 8j + 2(l%4) + k:  acc[4j + 2i + k].
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float silu_f(float v) { return __fdividef(v, 1.0f + __expf(-v)); }
 
@@ -96,74 +102,150 @@ __device__ __forceinline__ float wavenet_gate(float z) {
   return (u * r) * (1.0f + u);
 }
 
-template <int BN, int NACC, int EPI>
-__device__ __forceinline__ void epilogue_tile(const GemmDev& p, const TileCoord& t, const float (&acc)[NACC][BN / 2],
-                                              int row_base, int c2) {
-  const int tile_col0 = t.n_tile * BN;
+constexpr int STG_BYTES = 64 * 128;   // one staging box: 64 rows x (64 bf16 | 32 fp32) columns
+
+// Column groups jj, jj + 1 (jj even) of a bf16 box, o[2 jj + i] = bf16 pair k = 0, 1 of box row 16 ww + l/4 + 8i,
+// columns 8 jj + 2(l%4) + k.  Row r of the box is 128 bytes whose 16-byte piece c sits at c ^ (r % 8) (the TMA
+// 128-byte swizzle).  stmatrix writes one 8-row x 16-byte matrix per phase, and the 8 rows land on 8 different pieces:
+// no bank conflicts.  Written pair by pair, as soon as computed, so that only 4 packed values are live at a time.
+__device__ __forceinline__ void stage_bf16_pair(uint32_t buf, const uint32_t (&o)[16], int jj, int ww, int lane) {
+  const int m = lane >> 3;                                  // matrix whose row address this lane supplies
+  const uint32_t row_addr = buf + (16 * ww + 8 * (m & 1) + (lane & 7)) * 128;
+  const int piece = jj + (m >> 1);
+  stmatrix_x4(row_addr + ((piece ^ (lane & 7)) << 4), o[2 * jj], o[2 * jj + 1], o[2 * jj + 2], o[2 * jj + 3]);
+}
+// Same box layout with one 4-byte store per pair: a warp's 8 rows x 4 lanes land on piece jj ^ (row % 8), word l % 4,
+// i.e. 32 different banks.  Used where stmatrix's four-register operands would cost the kernel its wgmma overlap.
+__device__ __forceinline__ void stage_bf16_single(uint32_t buf, uint32_t v, int jj, int i, int ww, int lane) {
+  const int r = lane >> 2;
+  st_shared_b32(buf + (16 * ww + 8 * i + r) * 128 + ((jj ^ r) << 4) + 4 * (lane & 3), v);
+}
+
+// fp32, o[4 jj + 2i + k]: 8-byte stores, one half-warp per phase = box rows r = l/4 in 0..3 (or 4..7).  Column group jj is a 32-byte
+// piece pair, swizzled to pair jj ^ (r / 2): rows 2s and 2s + 1 would share it.  Lanes on odd rows store group jj ^ 3
+// while the others store jj, which puts the 4 rows of a phase on 4 different pairs: no bank conflicts.
+__device__ __forceinline__ void stage_f32(uint32_t buf, const float (&o)[16], int ww, int lane) {
+  const int r = lane >> 2;
+  const bool odd = (r & 1) != 0;
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
-    const int npos = row_base + 8 * i;
-    if (npos >= p.a_rows) continue;
-    const long long grow = static_cast<long long>(t.b) * p.a_rows + npos;
-    if constexpr (EPI == NS2_EPI_BF16 || EPI == NS2_EPI_F32) {
+    const uint32_t row_addr = buf + (16 * ww + 8 * i + r) * 128 + 8 * (lane & 1);
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int col = tile_col0 + 8 * j + c2;
-        if (tile_col0 + 8 * j >= p.n) break;   // n is a multiple of 32: 8-column groups are all in or all out
-        float v0 = acc[0][4 * j + 2 * i], v1 = acc[0][4 * j + 2 * i + 1];
-        if (p.bias != nullptr) {
-          const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + col));
-          v0 += bb.x;
-          v1 += bb.y;
-        }
-        if (p.act != 0) {
-          v0 = silu_f(v0);
-          v1 = silu_f(v1);
-        }
-        if constexpr (EPI == NS2_EPI_BF16) {
-          *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + grow * p.out_rs + t.g * p.out_gcs +
-                                       col) = pack_bf16x2(v0, v1);
-        } else {
-          if (p.resid != nullptr) {
-            const float2 rr = *reinterpret_cast<const float2*>(p.resid + grow * p.resid_rs + t.g * p.out_gcs + col);
-            v0 += rr.x;
-            v1 += rr.y;
+    for (int s = 0; s < 4; ++s) {
+      const int jj = odd ? (s ^ 3) : s;
+      const float a = odd ? o[4 * (s ^ 3) + 2 * i] : o[4 * s + 2 * i];
+      const float b = odd ? o[4 * (s ^ 3) + 2 * i + 1] : o[4 * s + 2 * i + 1];
+      st_shared_v2_f32(row_addr + (((2 * jj + ((lane & 3) >> 1)) ^ r) << 4), a, b);
+    }
+  }
+}
+
+// One tile of one consumer warpgroup.  stg: its two staging boxes; nbox: boxes it has issued so far.  Only the
+// warpgroup's first thread (`leader`) issues and waits on bulk groups; the box written now was last read by the store
+// issued two boxes ago, which the leader waited for before the previous box's barrier.
+template <int BN, int NACC, int EPI>
+__device__ __forceinline__ void epilogue_tile(const GemmDev& p, const TileCoord& t, const float (&acc)[NACC][BN / 2],
+                                              int cw, int ww, int lane, bool leader, uint32_t stg, uint32_t& nbox) {
+  constexpr int CW = EPI == NS2_EPI_F32 ? 32 : 64;                   // output columns per staging box
+  constexpr int OUT_COLS = EPI == NS2_EPI_GEGLU ? 128 : BN;         // output columns of the tile
+  // First position of this warpgroup's rows.  When it is past a_rows the stores below are clipped away entirely; the
+  // warpgroup still runs the epilogue, because returning early (a divergent path around the accumulator reads) makes
+  // ptxas serialize the WAVENET kernel's wgmma (C7520).
+  const int row0 = t.n0 + cw * 64;
+  const int out_col0 = t.n_tile * OUT_COLS;
+  const int out_n = EPI == NS2_EPI_GEGLU ? p.n / 2 : p.n;
+  const int c2 = 2 * (lane & 3);
+  const int rr = row0 + 16 * ww + (lane >> 2);                      // position of this thread's i = 0 row
+#pragma unroll
+  for (int q = 0; q < OUT_COLS / CW; ++q) {
+    if (out_col0 + q * CW >= out_n) break;   // n is a multiple of 32: a box holds at least 32 valid columns
+    // finished values of this box: fp32 o[4 jj + 2i + k], or bf16 pairs o[2 jj + i] (packed at once: fewer live registers)
+    using OutT = std::conditional_t<EPI == NS2_EPI_F32, float, uint32_t>;
+    OutT o[16];
+    const uint32_t buf = stg + (nbox & 1) * STG_BYTES;
+    auto put = [&](int jj, int i, float v0, float v1) {
+      if constexpr (EPI == NS2_EPI_F32) {
+        o[4 * jj + 2 * i] = v0;
+        o[4 * jj + 2 * i + 1] = v1;
+      } else {
+        o[2 * jj + i] = pack_bf16x2(v0, v1);
+      }
+    };
+#pragma unroll
+    for (int jj = 0; jj < CW / 8; ++jj) {
+      const int j = q * (CW / 8) + jj;        // accumulator column group
+      const int col = out_col0 + 8 * j + c2;  // output column of k = 0 (value column for GEGLU)
+      if (out_col0 + 8 * j >= out_n) {        // right half of a 64-column box past n: clipped by the TMA store
+        put(jj, 0, 0.f, 0.f);
+        put(jj, 1, 0.f, 0.f);
+        if constexpr (EPI == NS2_EPI_BF16 || EPI == NS2_EPI_GEGLU)
+          if (jj & 1) stage_bf16_pair(buf, o, jj - 1, ww, lane);
+        continue;
+      }
+      if constexpr (EPI == NS2_EPI_BF16 || EPI == NS2_EPI_F32) {
+        float2 bb = make_float2(0.f, 0.f);
+        if (p.bias != nullptr) bb = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + col));
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          float v0 = acc[0][4 * j + 2 * i], v1 = acc[0][4 * j + 2 * i + 1];
+          if (p.bias != nullptr) {
+            v0 += bb.x;
+            v1 += bb.y;
           }
-          *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + grow * p.out_rs + t.g * p.out_gcs + col) =
-              make_float2(v0, v1);
+          if (p.act != 0) {
+            v0 = silu_f(v0);
+            v1 = silu_f(v1);
+          }
+          if constexpr (EPI == NS2_EPI_F32) {
+            // residual held elsewhere: read it here (the in-place residual is added by the TMA reduce-add instead)
+            if (p.resid != nullptr && !p.resid_in_place && rr + 8 * i < p.a_rows) {
+              const long long grow = static_cast<long long>(t.b) * p.a_rows + rr + 8 * i;
+              const float2 r2 = *reinterpret_cast<const float2*>(p.resid + grow * p.resid_rs + t.g * p.out_gcs + col);
+              v0 += r2.x;
+              v1 += r2.y;
+            }
+          }
+          put(jj, i, v0, v1);
         }
-      }
-    } else if constexpr (EPI == NS2_EPI_GEGLU) {
-      static_assert(EPI != NS2_EPI_GEGLU || BN == 256, "GEGLU tiles pair 128 value + 128 gate rows");
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
+      } else if constexpr (EPI == NS2_EPI_GEGLU) {
+        static_assert(EPI != NS2_EPI_GEGLU || BN == 256, "GEGLU tiles pair 128 value + 128 gate rows");
         const int c = 8 * j + c2;   // value column inside the tile; its gate is column c + 128 (fragment j + 16)
-        const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + tile_col0 + c));
-        const float2 bg = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + tile_col0 + c + 128));
-        const float v0 = (acc[0][4 * j + 2 * i] + bv.x) * gelu_erf(acc[0][4 * (j + 16) + 2 * i] + bg.x);
-        const float v1 = (acc[0][4 * j + 2 * i + 1] + bv.y) * gelu_erf(acc[0][4 * (j + 16) + 2 * i + 1] + bg.y);
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + grow * p.out_rs + t.g * p.out_gcs +
-                                     t.n_tile * 128 + c) = pack_bf16x2(v0, v1);
-      }
-    } else {  // NS2_EPI_WAVENET: y = tanh(z) sigmoid(z) + res, z = (conv + b0) * gamma + beta   (ns2.py:619-636)
-      static_assert(EPI != NS2_EPI_WAVENET || NACC == 2, "wavenet block needs conv + res accumulators");
+        const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + t.n_tile * BN + c));
+        const float2 bg = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + t.n_tile * BN + c + 128));
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        if (tile_col0 + 8 * j >= p.n) break;
-        const int col = tile_col0 + 8 * j + c2;
+        for (int i = 0; i < 2; ++i) {
+          put(jj, i, (acc[0][4 * j + 2 * i] + bv.x) * gelu_erf(acc[0][4 * (j + 16) + 2 * i] + bg.x),
+              (acc[0][4 * j + 2 * i + 1] + bv.y) * gelu_erf(acc[0][4 * (j + 16) + 2 * i + 1] + bg.y));
+        }
+      } else {  // NS2_EPI_WAVENET: y = tanh(z) sigmoid(z) + res, z = (conv + b0) * gamma + beta   (ns2.py:619-636)
+        static_assert(EPI != NS2_EPI_WAVENET || NACC == 2, "wavenet block needs conv + res accumulators");
         const float2 b0 = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + col));
         const float2 b1 = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + col + p.bias1_off));
         const float* fp = p.film + t.b * p.film_bs + t.g * p.film_gs + col;
         const float2 ga = __ldg(reinterpret_cast<const float2*>(fp));
         const float2 be = __ldg(reinterpret_cast<const float2*>(fp + p.n));
-        const float z0 = fmaf(acc[0][4 * j + 2 * i] + b0.x, ga.x, be.x);
-        const float z1 = fmaf(acc[0][4 * j + 2 * i + 1] + b0.y, ga.y, be.y);
-        const float y0 = wavenet_gate(z0) + (acc[NACC - 1][4 * j + 2 * i] + b1.x);
-        const float y1 = wavenet_gate(z1) + (acc[NACC - 1][4 * j + 2 * i + 1] + b1.y);
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + grow * p.out_rs + t.g * p.out_gcs +
-                                     col) = pack_bf16x2(y0, y1);
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const float z0 = fmaf(acc[0][4 * j + 2 * i] + b0.x, ga.x, be.x);
+          const float z1 = fmaf(acc[0][4 * j + 2 * i + 1] + b0.y, ga.y, be.y);
+          stage_bf16_single(buf, pack_bf16x2(wavenet_gate(z0) + (acc[NACC - 1][4 * j + 2 * i] + b1.x),
+                                             wavenet_gate(z1) + (acc[NACC - 1][4 * j + 2 * i + 1] + b1.y)),
+                            jj, i, ww, lane);
+        }
       }
+      if constexpr (EPI == NS2_EPI_BF16 || EPI == NS2_EPI_GEGLU)
+        if (jj & 1) stage_bf16_pair(buf, o, jj - 1, ww, lane);
     }
+    if constexpr (EPI == NS2_EPI_F32) stage_f32(buf, o, ww, lane);
+    fence_proxy_async_smem();                   // generic-proxy smem writes -> visible to the TMA unit
+    if (leader) tma_store_wait_read<0>();        // the previous box has been read: free for the next one
+    warpgroup_bar(cw);
+    if (leader) {
+      if (EPI == NS2_EPI_F32 && p.resid_in_place) tma_reduce_add_4d(&p.tmOut, buf, out_col0 + q * CW, t.g, row0, t.b);
+      else tma_store_4d(&p.tmOut, buf, out_col0 + q * CW, t.g, row0, t.b);
+      tma_store_commit();
+    }
+    ++nbox;
   }
 }
 
@@ -177,7 +259,10 @@ struct GemmCfg {
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = (192 * 1024) / STAGE_BYTES;   // 4 stages of 48 KB (BN 256), 6 of 32 KB (BN 128)
   static constexpr int THREADS = 384;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
+  static constexpr int STG_OFF = RING_BYTES;                        // 2 consumer warpgroups x 2 staging boxes
+  static constexpr int BAR_OFF = STG_OFF + 4 * STG_BYTES;
+  static constexpr int SMEM_BYTES = BAR_OFF + 1024 /*align slack*/ + 256 /*barriers*/;   // 225.25 KB of 227
 };
 
 template <int BN>
@@ -192,7 +277,7 @@ __global__ void __launch_bounds__(GemmCfg<BN, NACC>::THREADS, 1) gemm_kernel(con
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::BAR_OFF);
   uint64_t* full_bar = bars;                 // [STAGES]
   uint64_t* empty_bar = bars + Cfg::STAGES;  // [STAGES] one arrive per consumer warp
 
@@ -202,6 +287,7 @@ __global__ void __launch_bounds__(GemmCfg<BN, NACC>::THREADS, 1) gemm_kernel(con
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmA);
     tma_prefetch_desc(&p.tmB);
+    tma_prefetch_desc(&p.tmOut);
     for (int i = 0; i < Cfg::STAGES; ++i) {
       mbar_init(smem_u32(&full_bar[i]), 1);
       mbar_init(smem_u32(&empty_bar[i]), 8);
@@ -245,6 +331,9 @@ __global__ void __launch_bounds__(GemmCfg<BN, NACC>::THREADS, 1) gemm_kernel(con
     // =============================== consumers: wgmma mainloop + epilogue ===============================
     const int cw = (warp >> 2) - 1;   // consumer warpgroup: rows [64 cw, 64 cw + 64) of the tile
     const int ww = warp & 3;
+    const bool leader = (threadIdx.x & 127) == 0;   // issues and waits on this warpgroup's bulk stores
+    const uint32_t stg = smem_u32(smem + Cfg::STG_OFF + cw * 2 * STG_BYTES);
+    uint32_t nbox = 0;
     float acc[NACC][BN / 2];
     uint32_t it = 0;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
@@ -283,9 +372,9 @@ __global__ void __launch_bounds__(GemmCfg<BN, NACC>::THREADS, 1) gemm_kernel(con
 #pragma unroll
       for (int a = 0; a < NACC; ++a) wgmma_hold(acc[a]);
       if (prev_stage >= 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev_stage]));
-      if (!p.skip_epilogue)
-        epilogue_tile<BN, NACC, EPI>(p, t, acc, t.n0 + cw * 64 + ww * 16 + (lane >> 2), 2 * (lane & 3));
+      if (!p.skip_epilogue) epilogue_tile<BN, NACC, EPI>(p, t, acc, cw, ww, lane, leader, stg, nbox);
     }
+    if (leader) tma_store_wait_all();   // shared memory must outlive the reads of the last stores
   }
 }
 
@@ -371,6 +460,22 @@ extern "C" int ns2_gemm(const ns2_gemm_args* a, ns2_stream_t stream_) {
     int rc = make_tmap_16bit(&dev.tmB, a->B, 2, dims, strides, box);
     if (rc != kOk) return rc;
   }
+  {
+    // (columns, group, position, batch): columns clip at n (n / 2 for GEGLU) inside every group, positions at a_rows,
+    // so a partial tile writes nothing into the next group's columns or the next batch's rows.  One box = one
+    // consumer warpgroup's 64 positions x 128 bytes.
+    const bool f32 = a->epilogue == NS2_EPI_F32;
+    const uint64_t esz = f32 ? 4 : 2;
+    const uint64_t out_cols = a->epilogue == NS2_EPI_GEGLU ? a->n / 2 : a->n;
+    const uint64_t row_bytes = (uint64_t)a->out_row_stride * esz;
+    const uint64_t dims[4] = {out_cols, (uint64_t)a->groups, (uint64_t)a->a_rows, (uint64_t)a->a_batches};
+    const uint64_t strides[4] = {esz, a->groups > 1 ? (uint64_t)a->out_group_col_stride * esz : row_bytes, row_bytes,
+                                 (uint64_t)a->a_rows * row_bytes};
+    const uint32_t box[4] = {(uint32_t)(128 / esz), 1, 64, 1};
+    int rc = f32 ? make_tmap_f32(&dev.tmOut, a->out, 4, dims, strides, box)
+                 : make_tmap_16bit(&dev.tmOut, a->out, 4, dims, strides, box);
+    if (rc != kOk) return rc;
+  }
   dev.tiles_n = (a->n + bn - 1) / bn;
   dev.tiles_per_batch = (a->a_rows + BM - 1) / BM;
   dev.tiles_m = dev.tiles_per_batch * a->a_batches;
@@ -391,6 +496,8 @@ extern "C" int ns2_gemm(const ns2_gemm_args* a, ns2_stream_t stream_) {
   dev.out_rs = a->out_row_stride;
   dev.resid = a->resid;
   dev.resid_rs = a->resid_row_stride;
+  dev.resid_in_place = (a->epilogue == NS2_EPI_F32 && a->resid != nullptr && a->resid == a->out &&
+                        a->resid_row_stride == a->out_row_stride) ? 1 : 0;
   dev.film = a->film;
   dev.film_bs = a->film_batch_stride;
   dev.film_gs = a->film_group_stride;

@@ -63,16 +63,15 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
 }
 // Bounded wait: a pipeline bug must surface as a trapped launch (an error the host sees), never as a
 // hung GPU.  ~2e9 SM cycles is about a second; no legitimate wait in these kernels is near that.
+// A timeout shows up only as a failed launch (cudaErrorLaunchFailure / illegal instruction on the next
+// synchronising call), with no device-side message: any function call here, printf included, makes ptxas
+// serialize every wgmma of the calling kernel (warning C7510), so the branch holds nothing but the trap.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   uint32_t it = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (((++it) & 0xfff) == 0 && (clock64() - t0) > 2000000000LL) {
-      printf("ns2: mbarrier wait timed out (block %d thread %d bar 0x%x parity %u)\n", blockIdx.x,
-             threadIdx.x, bar, parity);
-      __trap();
-    }
+    if (((++it) & 0xfff) == 0 && (clock64() - t0) > 2000000000LL) __trap();
   }
 }
 
@@ -84,11 +83,7 @@ __device__ __forceinline__ void mbar_wait_backoff(uint32_t bar, uint32_t parity,
   uint32_t it = 0;
   while (!mbar_try_wait(bar, parity)) {
     __nanosleep(ns);
-    if (((++it) & 0xfff) == 0 && (clock64() - t0) > 2000000000LL) {
-      printf("ns2: mbarrier wait timed out (block %d thread %d bar 0x%x parity %u)\n", blockIdx.x,
-             threadIdx.x, bar, parity);
-      __trap();
-    }
+    if (((++it) & 0xfff) == 0 && (clock64() - t0) > 2000000000LL) __trap();
   }
 }
 
@@ -121,25 +116,19 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, 
 }
 
 // TMA stores (smem -> global, bulk async-group completion).  OOB parts of the box are clipped by the TMA unit.
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
                    reinterpret_cast<uint64_t>(m)),
-               "r"(src), "r"(c0), "r"(c1), "r"(c2)
+               "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
 // global[tile] += smem[tile] (element-wise fp32 add performed at L2): the residual-stream update
-__device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2) {
+__device__ __forceinline__ void tma_reduce_add_4d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3) {
   asm volatile(
-      "cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+      "cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
           reinterpret_cast<uint64_t>(m)),
-      "r"(src), "r"(c0), "r"(c1), "r"(c2)
+      "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
-}
-__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* m, uint32_t src, int c0, int c1) {
-  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(src), "r"(c0), "r"(c1)
-               : "memory");
 }
 // plain 1-D bulk copy global -> shared (16-byte aligned, size % 16 == 0), completion on an mbarrier like the tensor loads
 __device__ __forceinline__ void bulk_load_1d(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t mbar) {
@@ -182,6 +171,20 @@ __device__ __forceinline__ uint64_t gmma_desc_plain(uint32_t smem_addr, uint32_t
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
   return d;
+}
+
+// stmatrix.x4: four 8x8 b16 matrices; register k of lane l = row l/4, columns 2(l%4)+{0,1} of matrix k (the wgmma
+// accumulator fragment layout), lane l gives the shared address of row l%8 of matrix l/8
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
+}
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void st_shared_v2_f32(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
 
 // named barrier over the 128 threads of one warpgroup (ids 8..11 are reserved for this)

@@ -190,10 +190,7 @@ __global__ void __launch_bounds__(320, 1) rvq_encode_kernel(const __grid_constan
   // declared 1024-byte aligned (checked below) and indexed directly so the compiler keeps every access in the
   // shared state space (LDS/STS instead of generic LD/ST)
   extern __shared__ __align__(1024) uint8_t smem[];
-  if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) {
-    printf("ns2 rvq: dynamic shared memory is not 1024-byte aligned\n");
-    __trap();
-  }
+  if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) __trap();   // no printf: see mbar_wait in ptx.cuh
   float* R = reinterpret_cast<float*>(smem + OFF_R);
   float* keys_s = reinterpret_cast<float*>(smem + OFF_KEYS);
   float4* rowp_s = reinterpret_cast<float4*>(smem + OFF_ROWP);

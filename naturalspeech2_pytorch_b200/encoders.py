@@ -15,10 +15,10 @@ unchanged; the module tree only HOLDS parameters, the math goes through `ops` (l
 
 Training: in `train()` mode with gradients enabled (and parameters that require them) `SpeechPromptEncoder.forward` and
 `PhonemeEncoder.forward` record ONE autograd node each (`_EncoderFunction`, the pattern of training.DenoiserFunction).
-Its forward runs exactly the inference kernels (bit-identical output) and keeps the activations the backward needs;
-its backward walks the encoder in reverse:
-  plain Transformer      out-proj / FF wgrad + dgrad GEMMs on transposed packs, attention_bwd, geglu_bwd (on a
-                         plain-epilogue recomputation of the GEGLU input), rmsnorm_film_bwd(gamma=...)
+Its forward is the inference forward (`_forward` and `_transformer`) given a `saved` dict, which keeps the activations
+the backward needs (bit-identical output); its backward walks the encoder in reverse:
+  plain Transformer      out-proj / FF wgrad + dgrad GEMMs on transposed packs, training.attention_backward and
+                         training.geglu_backward (shared with the denoiser's backward), rmsnorm_film_bwd(gamma=...)
   k=9 conv + SiLU        pre-activation recomputed with a plain-epilogue GEMM, ops.silu_bwd, one ops.wgrad per tap
                          ("same" padding: shifts +4..-4, causal: 8..0), dgrad = one nine-segment GEMM with mirrored
                          shifts (the prompt encoder's first conv needs none: its input comes from the codec)
@@ -37,7 +37,9 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import _lib, ops
-from .model import _AttentionParams, _NoParam, _RMSNormParams, _feedforward_params, _round_up
+from .ops import conv_dgrad_segs as _conv_dgrad_segs, conv_segs as _conv_segs
+from .model import _AttentionParams, _NoParam, _RMSNormParams, _bf, _feedforward_params, _pack_geglu
+from .training import _transpose_conv, attention_backward, geglu_backward
 
 _SILU = _lib.NS2_GEMM_FLAG_SILU
 
@@ -54,31 +56,10 @@ class _PlainTransformerParams(nn.Module):
         self.norm = _RMSNormParams(dim) if final_norm else nn.Identity()
 
 
-def _bf(t: torch.Tensor) -> torch.Tensor:
-    return t.detach().to(torch.bfloat16).contiguous()
-
-
 def _pack_conv(w: torch.Tensor) -> torch.Tensor:
     """(O, I, k) -> (O, k*I) bf16, tap t at columns [t*I, (t+1)*I)."""
     O, I, k = w.shape
     return _bf(w.detach().permute(0, 2, 1).reshape(O, k * I))
-
-
-def _conv_segs(c_in: int, kernel: int, first_shift: int):
-    """Segments of a stride-1 convolution: tap t reads position n - (first_shift - t)."""
-    return [(0, t * c_in, c_in, first_shift - t, 0) for t in range(kernel)]
-
-
-def _conv_dgrad_segs(c_out: int, kernel: int, first_shift: int):
-    """Segments of the input gradient of `_conv_segs` on the transposed pack ([in][tap][out]): tap t reads d out at
-    n + (first_shift - t), the mirrored shift."""
-    return [(0, t * c_out, c_out, t - first_shift, 0) for t in range(kernel)]
-
-
-def _transpose_conv(w: torch.Tensor, kernel: int) -> torch.Tensor:
-    """(O, k*I) tap-major pack -> (I, k*O) [in][tap][out] pack for the dgrad GEMM."""
-    O = w.shape[0]
-    return w.view(O, kernel, -1).permute(2, 1, 0).reshape(-1, kernel * O).contiguous()
 
 
 def _records_graph(m: nn.Module) -> bool:
@@ -153,6 +134,11 @@ class _EncoderBase(nn.Module):
             for k in ("qkv", "o", "w1", "w2"):
                 T[f"l{l}_{k}"] = P[f"l{l}_{k}"].t().contiguous()
 
+    def _train_forward(self, x: torch.Tensor):
+        """`_forward` keeping the activations `_train_backward` reads -> (output, record)."""
+        saved = {}
+        return self._forward(x, saved), saved
+
     # ---- transformer ----
     def _pack_transformer(self, P: Dict[str, torch.Tensor], tr: _PlainTransformerParams, dim: int) -> None:
         for l, (n1, attn, n2, ff) in enumerate(tr.layers):
@@ -160,82 +146,56 @@ class _EncoderBase(nn.Module):
             P[f"l{l}_g2"] = n2.gamma.detach().float().contiguous()
             P[f"l{l}_qkv"] = _bf(torch.cat((attn.to_q.weight, attn.to_kv.weight), dim=0))
             P[f"l{l}_o"] = _bf(attn.to_out.weight)
-            lin1, lin2 = ff[0], ff[-1]
-            Di = lin2.weight.shape[1]
-            Dp = _round_up(Di, 128)
-            dev = lin1.weight.device
-            wv, wg = torch.zeros(Dp, dim, device=dev), torch.zeros(Dp, dim, device=dev)
-            wv[:Di], wg[:Di] = lin1.weight[:Di], lin1.weight[Di:]   # first half = value, second = gate (ns2.py:1006)
-            bv, bg = torch.zeros(Dp, device=dev), torch.zeros(Dp, device=dev)
-            bv[:Di], bg[:Di] = lin1.bias[:Di], lin1.bias[Di:]
-            P[f"l{l}_w1"] = _bf(torch.stack((wv.view(-1, 128, dim), wg.view(-1, 128, dim)), dim=1).reshape(2 * Dp, dim))
-            P[f"l{l}_b1"] = torch.stack((bv.view(-1, 128), bg.view(-1, 128)), dim=1).reshape(2 * Dp).float().contiguous()
-            w2 = torch.zeros(dim, Dp, device=dev)
-            w2[:, :Di] = lin2.weight
-            P[f"l{l}_w2"] = _bf(w2)
-            P[f"l{l}_b2"] = lin2.bias.detach().float().contiguous()
+            for k, v in _pack_geglu(ff[0], ff[-1]).items():
+                P[f"l{l}_{k}"] = v
         if isinstance(tr.norm, _RMSNormParams):
             P["final_g"] = tr.norm.gamma.detach().float().contiguous()
 
-    def _transformer(self, x: torch.Tensor, tr: _PlainTransformerParams, P, heads: int) -> torch.Tensor:
-        """Transformer.forward (ns2.py:1110-1115) on the fp32 residual stream x (B, N, D), updated in place."""
+    def _transformer(self, x: torch.Tensor, tr: _PlainTransformerParams, P, heads: int,
+                     saved: Optional[dict] = None) -> torch.Tensor:
+        """Transformer.forward (ns2.py:1110-1115) on the fp32 residual stream x (B, N, D), updated in place.  With `saved`
+        every layer's activations go to saved["layers"] in fresh tensors (`_transformer_backward` reads them)."""
+        keep = saved is not None
+        if keep and "final_g" in P:
+            raise NotImplementedError("training a Transformer with final_norm=True is not supported")
         B, N, D = x.shape
-        dev, bf = x.device, torch.bfloat16
+        dev = x.device
+        e = lambda *s, dt=torch.bfloat16: torch.empty(*s, device=dev, dtype=dt)  # noqa: E731
         inner = heads * 64
-        Dp = P["l0_w2"].shape[1] if len(tr.layers) else 0
-        h = torch.empty(B, N, D, device=dev, dtype=bf)
-        qkv = torch.empty(B, N, 3 * inner, device=dev, dtype=bf)
-        o = torch.empty(B, N, inner, device=dev, dtype=bf)
-        g = torch.empty(B, N, Dp, device=dev, dtype=bf)
+        layers = []
         for l in range(len(tr.layers)):
-            ops.rmsnorm_film(x, h, gamma=P[f"l{l}_g1"])
-            ops.gemm(h, P[f"l{l}_qkv"], qkv, n=3 * inner, epilogue=ops.EPI_BF16)
-            ops.attention(qkv[:, :, :inner], qkv[:, :, inner:2 * inner], qkv[:, :, 2 * inner:], o, heads=heads)
-            ops.gemm(o, P[f"l{l}_o"], x, n=D, epilogue=ops.EPI_F32, resid=x)
-            ops.rmsnorm_film(x, h, gamma=P[f"l{l}_g2"])
-            ops.gemm(h, P[f"l{l}_w1"], g, n=2 * Dp, epilogue=ops.EPI_GEGLU, bias=P[f"l{l}_b1"])
-            ops.gemm(g, P[f"l{l}_w2"], x, n=D, epilogue=ops.EPI_F32, bias=P[f"l{l}_b2"], resid=x)
+            if keep or l == 0:   # inference reuses the first layer's buffers
+                Dp = P[f"l{l}_w2"].shape[1]
+                L = {"h1": e(B, N, D), "qkv": e(B, N, 3 * inner), "ao": e(B, N, inner), "ff_g": e(B, N, Dp),
+                     "lse": e(B, heads, N, dt=torch.float32) if keep else None}
+                L["h2"] = e(B, N, D) if keep else L["h1"]
+                layers.append(L)
+            if keep:
+                L["x_in"] = x.clone()
+            ops.rmsnorm_film(x, L["h1"], gamma=P[f"l{l}_g1"])
+            qkv = ops.gemm(L["h1"], P[f"l{l}_qkv"], L["qkv"], n=3 * inner, epilogue=ops.EPI_BF16)
+            ops.attention(qkv[:, :, :inner], qkv[:, :, inner:2 * inner], qkv[:, :, 2 * inner:], L["ao"], heads=heads,
+                          lse=L["lse"])
+            ops.gemm(L["ao"], P[f"l{l}_o"], x, n=D, epilogue=ops.EPI_F32, resid=x)
+            if keep:
+                L["x_mid"] = x.clone()
+            ops.rmsnorm_film(x, L["h2"], gamma=P[f"l{l}_g2"])
+            ops.gemm(L["h2"], P[f"l{l}_w1"], L["ff_g"], n=2 * Dp, epilogue=ops.EPI_GEGLU, bias=P[f"l{l}_b1"])
+            ops.gemm(L["ff_g"], P[f"l{l}_w2"], x, n=D, epilogue=ops.EPI_F32, bias=P[f"l{l}_b2"], resid=x)
+        if keep:
+            saved["layers"] = layers
         if "final_g" in P:
             out = torch.empty_like(x)
             ops.rmsnorm_f32(x, out, P["final_g"])
             return out
         return x
 
-    def _transformer_train(self, x: torch.Tensor, tr: _PlainTransformerParams, P, heads: int) -> list:
-        """`_transformer` (same kernels, same order: bit-identical x) keeping every layer's activations."""
-        if "final_g" in P:
-            raise NotImplementedError("training a Transformer with final_norm=True is not supported")
-        B, N, D = x.shape
-        dev, bf = x.device, torch.bfloat16
-        e = lambda *s, dt=bf: torch.empty(*s, device=dev, dtype=dt)  # noqa: E731
-        inner = heads * 64
-        layers = []
-        for l in range(len(tr.layers)):
-            Dp = P[f"l{l}_w2"].shape[1]
-            L = {"x_in": x.clone()}
-            L["h1"] = ops.rmsnorm_film(x, e(B, N, D), gamma=P[f"l{l}_g1"])
-            L["qkv"] = ops.gemm(L["h1"], P[f"l{l}_qkv"], e(B, N, 3 * inner), n=3 * inner, epilogue=ops.EPI_BF16)
-            L["lse"] = e(B, heads, N, dt=torch.float32)
-            qkv = L["qkv"]
-            L["o"] = ops.attention(qkv[:, :, :inner], qkv[:, :, inner:2 * inner], qkv[:, :, 2 * inner:], e(B, N, inner),
-                                   heads=heads, lse=L["lse"])
-            ops.gemm(L["o"], P[f"l{l}_o"], x, n=D, epilogue=ops.EPI_F32, resid=x)
-            L["x_mid"] = x.clone()
-            L["h2"] = ops.rmsnorm_film(x, e(B, N, D), gamma=P[f"l{l}_g2"])
-            L["g"] = ops.gemm(L["h2"], P[f"l{l}_w1"], e(B, N, Dp), n=2 * Dp, epilogue=ops.EPI_GEGLU, bias=P[f"l{l}_b1"])
-            ops.gemm(L["g"], P[f"l{l}_w2"], x, n=D, epilogue=ops.EPI_F32, bias=P[f"l{l}_b2"], resid=x)
-            layers.append(L)
-        return layers
-
     def _transformer_backward(self, layers: list, tr: _PlainTransformerParams, P, T, heads: int, dxr: torch.Tensor,
                               dxr_bf: torch.Tensor, grads: Dict[str, torch.Tensor]) -> None:
         """Transformer backward (ns2.py:1110-1115): dxr (fp32 gradient of the output, updated in place) becomes the
         gradient of the input; dxr_bf its bf16 copy.  Parameter gradients go to `grads` under the reference's names."""
         B, N, D = dxr.shape
-        dev, bf = dxr.device, torch.bfloat16
-        e = lambda *s: torch.empty(*s, device=dev, dtype=bf)  # noqa: E731
-        z = lambda *s: torch.zeros(*s, device=dev, dtype=torch.float32)  # noqa: E731
-        inner = heads * 64
+        dev = dxr.device
         for l in reversed(range(len(tr.layers))):
             L = layers[l]
             pfx = f"transformer.layers.{l}."
@@ -243,34 +203,19 @@ class _EncoderBase(nn.Module):
             Di = ff[-1].weight.shape[1]
             Dp = P[f"l{l}_w2"].shape[1]
             # ---- feed-forward: x += W2 GEGLU(W1 RMSNorm(x) + b1) + b2 ----
-            grads[pfx + f"3.{len(ff) - 1}.weight"] = ops.wgrad(dxr_bf, L["g"], z(D, Dp), n=D, k=Dp)[:, :Di]
-            grads[pfx + f"3.{len(ff) - 1}.bias"] = ops.colsum(dxr_bf, z(D))
-            d_g = ops.gemm(dxr_bf, T[f"l{l}_w2"], e(B, N, Dp), n=Dp, epilogue=ops.EPI_BF16)
-            pre = ops.gemm(L["h2"], P[f"l{l}_w1"], e(B, N, 2 * Dp), n=2 * Dp, epilogue=ops.EPI_BF16, bias=P[f"l{l}_b1"])
-            ops.geglu_bwd(pre, d_g)                                                      # pre <- d pre
-            dW1 = ops.wgrad(pre, L["h2"], z(2 * Dp, D), n=2 * Dp, k=D).view(Dp // 128, 2, 128, D)
-            db1 = ops.colsum(pre, z(2 * Dp)).view(Dp // 128, 2, 128)
-            grads[pfx + "3.0.weight"] = torch.cat((dW1[:, 0].reshape(Dp, D)[:Di], dW1[:, 1].reshape(Dp, D)[:Di]), dim=0)
-            grads[pfx + "3.0.bias"] = torch.cat((db1[:, 0].reshape(Dp)[:Di], db1[:, 1].reshape(Dp)[:Di]), dim=0)
-            dh2 = ops.gemm(pre, T[f"l{l}_w1"], e(B, N, D), n=D, epilogue=ops.EPI_BF16)
-            dg2 = z(D)
+            grads[pfx + f"3.{len(ff) - 1}.weight"] = ops.wgrad(dxr_bf, L["ff_g"], torch.zeros(D, Dp, device=dev), n=D,
+                                                               k=Dp)[:, :Di]
+            grads[pfx + f"3.{len(ff) - 1}.bias"] = ops.colsum(dxr_bf, torch.zeros(D, device=dev))
+            d_g = ops.gemm(dxr_bf, T[f"l{l}_w2"], torch.empty(B, N, Dp, device=dev, dtype=torch.bfloat16), n=Dp,
+                           epilogue=ops.EPI_BF16)
+            dh2 = geglu_backward(L["h2"], d_g, P[f"l{l}_w1"], P[f"l{l}_b1"], T[f"l{l}_w1"], Di, grads, pfx + "3.0")
+            dg2 = torch.zeros(D, device=dev)
             ops.rmsnorm_film_bwd(L["x_mid"], dh2, dxr, dxr_bf, rows_per_batch=N, gamma=P[f"l{l}_g2"], dgamma=dg2)
             grads[pfx + "2.gamma"] = dg2
             # ---- attention: x += Wo attn(Wqkv RMSNorm(x)) ----
-            grads[pfx + "1.to_out.weight"] = ops.wgrad(dxr_bf, L["o"], z(D, inner), n=D, k=inner)
-            d_o = ops.gemm(dxr_bf, T[f"l{l}_o"], e(B, N, inner), n=inner, epilogue=ops.EPI_BF16)
-            qkv = L["qkv"]
-            d_qkv = e(B, N, 3 * inner)
-            dq = z(B, N, inner)
-            ops.attention_bwd(qkv[:, :, :inner], qkv[:, :, inner:2 * inner], qkv[:, :, 2 * inner:], L["o"], d_o, L["lse"],
-                              dq, d_qkv[:, :, inner:2 * inner], d_qkv[:, :, 2 * inner:], heads=heads)
-            d_qkv[:, :, :inner].copy_(dq)   # fp32 accumulator -> bf16 slot (layout glue)
-            dWqkv = ops.wgrad(d_qkv, L["h1"], z(3 * inner, D), n=3 * inner, k=D)
-            grads[pfx + "1.to_q.weight"] = dWqkv[:inner]
-            grads[pfx + "1.to_kv.weight"] = dWqkv[inner:]
-            dh1 = ops.gemm(d_qkv, T[f"l{l}_qkv"], e(B, N, D), n=D, epilogue=ops.EPI_BF16)
-            dg1 = z(D)
-            ops.rmsnorm_film_bwd(L["x_in"], dh1, dxr, dxr_bf, rows_per_batch=N, gamma=P[f"l{l}_g1"], dgamma=dg1)
+            dg1 = torch.zeros(D, device=dev)
+            attention_backward(L, dxr, dxr_bf, T[f"l{l}_o"], T[f"l{l}_qkv"], heads, grads, pfx + "1.",
+                               gamma=P[f"l{l}_g1"], dgamma=dg1)
             grads[pfx + "0.gamma"] = dg1
 
     def _conv_silu_backward(self, x_in: torch.Tensor, w: torch.Tensor, w_t: Optional[torch.Tensor], bias: torch.Tensor,
@@ -356,10 +301,10 @@ class SpeechPromptEncoder(_EncoderBase):
         if _records_graph(self):
             return _EncoderFunction.apply(self, self.grad_reducer, x, *self.parameters())
         with torch.no_grad():
-            return self._train_forward(x, keep=False)[0]
+            return self._forward(x)
 
-    def _train_forward(self, x: torch.Tensor, keep: bool = True):
-        """Inference forward; with keep=True also the activations of `_train_backward` (same kernels, same output)."""
+    def _forward(self, x: torch.Tensor, saved: Optional[dict] = None) -> torch.Tensor:
+        """The forward; with `saved` it also records the activations `_train_backward` reads (same kernels, same output)."""
         P = self.packed()
         B, N, _ = x.shape
         dev, bf = x.device, torch.bfloat16
@@ -371,13 +316,12 @@ class SpeechPromptEncoder(_EncoderBase):
             out = torch.empty(B, N, c.out_channels, device=dev, dtype=torch.float32 if last else bf)
             ops.gemm(h, P[f"c{i}_w"], out, n=c.out_channels, epilogue=ops.EPI_F32 if last else ops.EPI_BF16,
                      segs=_conv_segs(c.in_channels, self.kernel_size, self.padding), bias=P[f"c{i}_b"], flags=_SILU)
-            if keep:
+            if saved is not None:
                 conv_in.append(h)
             h = out
-        if not keep:
-            return self._transformer(h, self.transformer, P, self.heads), None
-        layers = self._transformer_train(h, self.transformer, P, self.heads)
-        return h, {"conv_in": conv_in, "layers": layers}
+        if saved is not None:
+            saved["conv_in"] = conv_in
+        return self._transformer(h, self.transformer, P, self.heads, saved)
 
     def _train_backward(self, S, d_out: torch.Tensor) -> Dict[str, torch.Tensor]:
         P, T = self.packed(), self.packed_transposed()
@@ -439,10 +383,10 @@ class PhonemeEncoder(_EncoderBase):
         if _records_graph(self):
             return _EncoderFunction.apply(self, self.grad_reducer, x, *self.parameters())
         with torch.no_grad():
-            return self._train_forward(x, keep=False)[0]
+            return self._forward(x)
 
-    def _train_forward(self, x: torch.Tensor, keep: bool = True):
-        """Inference forward; with keep=True also the activations of `_train_backward` (same kernels, same output)."""
+    def _forward(self, x: torch.Tensor, saved: Optional[dict] = None) -> torch.Tensor:
+        """The forward; with `saved` it also records the activations `_train_backward` reads (same kernels, same output)."""
         P = self.packed()
         B, T = x.shape
         dev, bf = x.device, torch.bfloat16
@@ -452,10 +396,9 @@ class PhonemeEncoder(_EncoderBase):
         # CausalConv1d: left padding dilation*(k-1) (ns2.py:592-595) -> tap t reads position n - (k-1-t)
         ops.gemm(e, P["c_w"], h, n=self.dim_hidden, epilogue=ops.EPI_F32,
                  segs=_conv_segs(self.dim, self.kernel_size, self.kernel_size - 1), bias=P["c_b"], flags=_SILU)
-        if not keep:
-            return self._transformer(h, self.transformer, P, self.heads), None
-        layers = self._transformer_train(h, self.transformer, P, self.heads)
-        return h, {"ids": ids, "emb": e, "layers": layers}
+        if saved is not None:
+            saved.update(ids=ids, emb=e)
+        return self._transformer(h, self.transformer, P, self.heads, saved)
 
     def _train_backward(self, S, d_out: torch.Tensor) -> Dict[str, torch.Tensor]:
         P, T = self.packed(), self.packed_transposed()

@@ -38,6 +38,30 @@ def _round_up(v: int, m: int) -> int:
     return (v + m - 1) // m * m
 
 
+def _bf(t):
+    return t.detach().to(torch.bfloat16).contiguous()
+
+
+def _pack_geglu(lin1: nn.Linear, lin2: nn.Linear) -> Dict[str, torch.Tensor]:
+    """GEGLU FeedForward Linear pair (ns2.py:1001-1025) -> {w1, b1, w2, b2}: the inner width zero-padded to Dp, a multiple
+    of 128, and lin1's value and gate rows interleaved in 128-row tiles, so that one EPI_GEGLU tile holds a value block
+    and its gate block.  `training.geglu_backward` turns the gradient of this layout back into lin1's."""
+    D, Di = lin1.weight.shape[1], lin2.weight.shape[1]
+    Dp = _round_up(Di, 128)
+    dev = lin1.weight.device
+    wv = torch.zeros(Dp, D, device=dev)
+    wg = torch.zeros(Dp, D, device=dev)
+    wv[:Di], wg[:Di] = lin1.weight[:Di], lin1.weight[Di:]  # first half = value, second = gate (ns2.py:1006)
+    bv = torch.zeros(Dp, device=dev)
+    bg = torch.zeros(Dp, device=dev)
+    bv[:Di], bg[:Di] = lin1.bias[:Di], lin1.bias[Di:]
+    w1 = torch.stack((wv.view(-1, 128, D), wg.view(-1, 128, D)), dim=1).reshape(2 * Dp, D)
+    b1 = torch.stack((bv.view(-1, 128), bg.view(-1, 128)), dim=1).reshape(2 * Dp)
+    w2 = torch.zeros(D, Dp, device=dev)
+    w2[:, :Di] = lin2.weight
+    return {"w1": _bf(w1), "b1": b1.float().contiguous(), "w2": _bf(w2), "b2": lin2.bias.detach().float().contiguous()}
+
+
 class _NoParam(nn.Module):
     """Placeholder keeping Sequential indices aligned with the reference (Reduce / Rearrange / GEGLU / SiLU)."""
 
@@ -254,10 +278,6 @@ class Model(nn.Module):
         return self._packed
 
     @staticmethod
-    def _bf(t):
-        return t.detach().to(torch.bfloat16).contiguous()
-
-    @staticmethod
     def _conv3_pack(w, k_pad=None, o_pad=None):
         """(O, I, 3) -> (O_pad, 3*I_pad) with tap t at columns [t*I_pad, t*I_pad + I); zero padded."""
         O, I, _ = w.shape
@@ -266,31 +286,6 @@ class Model(nn.Module):
         out = w.new_zeros(o_pad, 3 * k_pad)
         for t in range(3):
             out[:O, t * k_pad:t * k_pad + I] = w[:, :, t]
-        return out
-
-    def _pack_ff(self, ff: nn.Sequential, conv: bool) -> Dict[str, torch.Tensor]:
-        D, Di = self.dim, self.ff_inner
-        Dp = _round_up(Di, 128)
-        lin1, lin2 = ff[0], ff[-1]
-        dev = lin1.weight.device
-        wv = torch.zeros(Dp, D, device=dev)
-        wg = torch.zeros(Dp, D, device=dev)
-        wv[:Di], wg[:Di] = lin1.weight[:Di], lin1.weight[Di:]  # first half = value, second = gate (ns2.py:1006)
-        bv = torch.zeros(Dp, device=dev)
-        bg = torch.zeros(Dp, device=dev)
-        bv[:Di], bg[:Di] = lin1.bias[:Di], lin1.bias[Di:]
-        w1 = torch.stack((wv.view(-1, 128, D), wg.view(-1, 128, D)), dim=1).reshape(2 * Dp, D)
-        b1 = torch.stack((bv.view(-1, 128), bg.view(-1, 128)), dim=1).reshape(2 * Dp)
-        w2 = torch.zeros(D, Dp, device=dev)
-        w2[:, :Di] = lin2.weight
-        out = {"w1": self._bf(w1), "b1": b1.float().contiguous(), "w2": self._bf(w2),
-               "b2": lin2.bias.detach().float().contiguous()}
-        if conv:
-            c = ff[2][1]
-            out["wc"] = self._bf(self._conv3_pack(c.weight, k_pad=Dp, o_pad=Dp))
-            bc = torch.zeros(Dp, device=dev)
-            bc[:Di] = c.bias
-            out["bc"] = bc
         return out
 
     def _pack(self) -> Dict[str, torch.Tensor]:
@@ -309,11 +304,11 @@ class Model(nn.Module):
                 if layer[idx] is not None:
                     film_w.append(layer[idx].to_gamma_beta.weight)
                     film_b.append(layer[idx].to_gamma_beta.bias)
-        P["film_w"] = self._bf(torch.cat(film_w, dim=0))
+        P["film_w"] = _bf(torch.cat(film_w, dim=0))
         P["film_b"] = torch.cat(film_b, dim=0).detach().float().contiguous()
         # ---- wavenet ----
         wn = self.wavenet
-        P["wn_init_w"] = self._bf(self._conv3_pack(wn.init_conv.weight))
+        P["wn_init_w"] = _bf(self._conv3_pack(wn.init_conv.weight))
         P["wn_init_b"] = wn.init_conv.bias.detach().float().contiguous()
         for s, st in enumerate(wn.stacks):
             ws, bc, br = [], [], []
@@ -321,42 +316,47 @@ class Model(nn.Module):
                 ws.append(torch.cat((self._conv3_pack(blk.conv.weight), blk.res_conv.weight[:, :, 0]), dim=1))
                 bc.append(blk.conv.bias)
                 br.append(blk.res_conv.bias)
-            P[f"wn{s}_w"] = self._bf(torch.cat(ws, dim=0))                      # (G*D, 4*D)
+            P[f"wn{s}_w"] = _bf(torch.cat(ws, dim=0))                      # (G*D, 4*D)
             P[f"wn{s}_b"] = torch.cat(bc + br).detach().float().contiguous()   # [conv biases | res biases]
         last = wn.stacks[-1]
-        P["wn_skip_w"] = self._bf(torch.cat([b.skip_conv.weight[:, :, 0] for b in last.blocks], dim=1))
+        P["wn_skip_w"] = _bf(torch.cat([b.skip_conv.weight[:, :, 0] for b in last.blocks], dim=1))
         P["wn_skip_b"] = torch.stack([b.skip_conv.bias for b in last.blocks]).sum(0).detach().float().contiguous()
-        P["wn_final_w"] = self._bf(wn.final_conv.weight[:, :, 0])
+        P["wn_final_w"] = _bf(wn.final_conv.weight[:, :, 0])
         P["wn_final_b"] = wn.final_conv.bias.detach().float().contiguous()
         # ---- transformer ----
         kv_all = []
         for l, layer in enumerate(self.transformer.layers):
             attn = layer[1]
-            P[f"l{l}_qkv"] = self._bf(torch.cat((attn.to_q.weight, attn.to_kv.weight), dim=0))
-            P[f"l{l}_o"] = self._bf(attn.to_out.weight)
+            P[f"l{l}_qkv"] = _bf(torch.cat((attn.to_q.weight, attn.to_kv.weight), dim=0))
+            P[f"l{l}_o"] = _bf(attn.to_out.weight)
             if layer[3] is not None:
-                P[f"l{l}_xq"] = self._bf(layer[3].to_q.weight)
-                P[f"l{l}_xo"] = self._bf(layer[3].to_out.weight)
+                P[f"l{l}_xq"] = _bf(layer[3].to_q.weight)
+                P[f"l{l}_xo"] = _bf(layer[3].to_out.weight)
                 kv_all.append(layer[3].to_kv.weight)
-            for k, v in self._pack_ff(layer[5], conv=True).items():
+            ff = layer[5]
+            for k, v in _pack_geglu(ff[0], ff[-1]).items():
                 P[f"l{l}_ff_{k}"] = v
+            conv, Dp = ff[2][1], P[f"l{l}_ff_w2"].shape[1]
+            P[f"l{l}_ff_wc"] = _bf(self._conv3_pack(conv.weight, k_pad=Dp, o_pad=Dp))
+            P[f"l{l}_ff_bc"] = torch.zeros(Dp, device=conv.bias.device)
+            P[f"l{l}_ff_bc"][:self.ff_inner] = conv.bias
         if kv_all:
-            P["x_kv_all"] = self._bf(torch.cat(kv_all, dim=0))  # (depth*2*inner, D): cross K/V of all layers
+            P["x_kv_all"] = _bf(torch.cat(kv_all, dim=0))  # (depth*2*inner, D): cross K/V of all layers
         P["pred_gamma"] = self.transformer.to_pred[0].gamma.detach().float().contiguous()
-        P["pred_w"] = self._bf(self.transformer.to_pred[1].weight)
+        P["pred_w"] = _bf(self.transformer.to_pred[1].weight)
         # ---- conditioning ----
         if self.condition_on_prompt:
             pr = self.perceiver_resampler
             if isinstance(pr.proj_context, nn.Linear):
-                P["pr_proj_w"] = self._bf(pr.proj_context.weight)
+                P["pr_proj_w"] = _bf(pr.proj_context.weight)
                 P["pr_proj_b"] = pr.proj_context.bias.detach().float().contiguous()
             for i, (attn, ff) in enumerate(pr.layers):
-                P[f"pr{i}_q"] = self._bf(attn.to_q.weight)
-                P[f"pr{i}_kv"] = self._bf(attn.to_kv.weight)
-                P[f"pr{i}_o"] = self._bf(attn.to_out.weight)
-                for k, v in self._pack_ff(ff, conv=False).items():
+                P[f"pr{i}_q"] = _bf(attn.to_q.weight)
+                P[f"pr{i}_kv"] = _bf(attn.to_kv.weight)
+                P[f"pr{i}_o"] = _bf(attn.to_out.weight)
+                for k, v in _pack_geglu(ff[0], ff[-1]).items():
                     P[f"pr{i}_ff_{k}"] = v
-            P["cond_w"] = self._bf(self.cond_to_model_dim.weight[:, :, 0])
+            P["cond_w"] = _bf(self.cond_to_model_dim.weight[:, :, 0])
             P["cond_b"] = self.cond_to_model_dim.bias.detach().float().contiguous()
         return P
 
@@ -396,46 +396,49 @@ class Model(nn.Module):
     # ----------------------------------------------------------------------------------------------
     # conditioning (timestep-invariant; cache across sampling steps via `precompute_conditioning`)
     # ----------------------------------------------------------------------------------------------
-    def _perceiver(self, prompt: torch.Tensor) -> torch.Tensor:
-        """PerceiverResampler.forward (ns2.py:568-579) -> (B, M, D) fp32."""
-        P, D, M, inner, H = self.packed(), self.dim, self.num_latents_m, self.inner, self.heads
+    def _perceiver(self, prompt: torch.Tensor, P: Dict[str, torch.Tensor], saved: Optional[dict] = None) -> torch.Tensor:
+        """PerceiverResampler.forward (ns2.py:568-579) -> (B, M, D) fp32.  With `saved`, every layer's activations are
+        kept (fresh buffers per layer) for `training._conditioning_backward_tokens`."""
+        D, M, inner, H = self.dim, self.num_latents_m, self.inner, self.heads
         pr = self.perceiver_resampler
         B, Np, _ = prompt.shape
         dev = prompt.device
-        bf = torch.bfloat16
-        ctx_len = M + Np
-        cat = torch.empty(B, ctx_len, D, device=dev, dtype=bf)  # [latents ; projected prompt]
-        p_bf = ops.cast_bf16(prompt.contiguous().float(), torch.empty(B, Np, self.dim_prompt, device=dev, dtype=bf))
+        e = lambda *s, dt=torch.bfloat16: torch.empty(*s, device=dev, dtype=dt)  # noqa: E731
+        keep = saved is not None
+        p_bf = ops.cast_bf16(prompt.contiguous().float(), e(B, Np, self.dim_prompt))
+        proj = p_bf
         if "pr_proj_w" in P:
-            proj = ops.gemm(p_bf, P["pr_proj_w"], torch.empty(B, Np, D, device=dev, dtype=bf), n=D,
-                            epilogue=ops.EPI_BF16, bias=P["pr_proj_b"])
-            cat[:, M:].copy_(proj)
-        else:
-            cat[:, M:].copy_(p_bf)
+            proj = ops.gemm(p_bf, P["pr_proj_w"], e(B, Np, D), n=D, epilogue=ops.EPI_BF16, bias=P["pr_proj_b"])
         lat = pr.latents.detach().float().unsqueeze(0).expand(B, M, D).contiguous()
-        lat_bf = torch.empty(B, M, D, device=dev, dtype=bf)
-        q = torch.empty(B, M, inner, device=dev, dtype=bf)
-        kv = torch.empty(B, ctx_len, 2 * inner, device=dev, dtype=bf)
-        o = torch.empty(B, M, inner, device=dev, dtype=bf)
         Dp = _round_up(self.ff_inner, 128)
-        g = torch.empty(B, M, Dp, device=dev, dtype=bf)
+        layers = []
         for i in range(len(pr.layers)):
-            ops.cast_bf16(lat, lat_bf)
-            cat[:, :M].copy_(lat_bf)  # cross_attn_include_queries: keys = cat(latents, context) (ns2.py:1060-1061)
-            ops.gemm(lat_bf, P[f"pr{i}_q"], q, n=inner, epilogue=ops.EPI_BF16)
-            ops.gemm(cat, P[f"pr{i}_kv"], kv, n=2 * inner, epilogue=ops.EPI_BF16)
-            ops.attention(q, kv[:, :, :inner], kv[:, :, inner:], o, heads=H)
-            ops.gemm(o, P[f"pr{i}_o"], lat, n=D, epilogue=ops.EPI_F32, resid=lat)
-            ops.cast_bf16(lat, lat_bf)
-            ops.gemm(lat_bf, P[f"pr{i}_ff_w1"], g, n=2 * Dp, epilogue=ops.EPI_GEGLU, bias=P[f"pr{i}_ff_b1"])
-            ops.gemm(g, P[f"pr{i}_ff_w2"], lat, n=D, epilogue=ops.EPI_F32, bias=P[f"pr{i}_ff_b2"], resid=lat)
-        out = torch.empty(B, M, D, device=dev, dtype=torch.float32)
+            if keep or i == 0:   # inference reuses the first layer's buffers
+                L = {"lat_bf": e(B, M, D), "cat": e(B, M + Np, D), "q": e(B, M, inner), "kv": e(B, M + Np, 2 * inner),
+                     "lse": e(B, H, M, dt=torch.float32) if keep else None, "o": e(B, M, inner), "g": e(B, M, Dp)}
+                L["lat_bf2"] = e(B, M, D) if keep else L["lat_bf"]
+                L["cat"][:, M:].copy_(proj)   # [latents ; projected prompt]
+                layers.append(L)
+            ops.cast_bf16(lat, L["lat_bf"])
+            L["cat"][:, :M].copy_(L["lat_bf"])  # cross_attn_include_queries: keys = cat(latents, context) (ns2.py:1060-1061)
+            ops.gemm(L["lat_bf"], P[f"pr{i}_q"], L["q"], n=inner, epilogue=ops.EPI_BF16)
+            ops.gemm(L["cat"], P[f"pr{i}_kv"], L["kv"], n=2 * inner, epilogue=ops.EPI_BF16)
+            ops.attention(L["q"], L["kv"][:, :, :inner], L["kv"][:, :, inner:], L["o"], heads=H, lse=L["lse"])
+            ops.gemm(L["o"], P[f"pr{i}_o"], lat, n=D, epilogue=ops.EPI_F32, resid=lat)
+            ops.cast_bf16(lat, L["lat_bf2"])
+            ops.gemm(L["lat_bf2"], P[f"pr{i}_ff_w1"], L["g"], n=2 * Dp, epilogue=ops.EPI_GEGLU, bias=P[f"pr{i}_ff_b1"])
+            ops.gemm(L["g"], P[f"pr{i}_ff_w2"], lat, n=D, epilogue=ops.EPI_F32, bias=P[f"pr{i}_ff_b2"], resid=lat)
+        if keep:
+            saved.update(pr_layers=layers, pr_lat=lat, pr_p_bf=p_bf, pr_Np=Np)
+        out = e(B, M, D, dt=torch.float32)
         ops.rmsnorm_f32(lat, out, pr.norm.gamma.detach().float().contiguous())
         return out
 
-    def precompute_conditioning(self, prompt: torch.Tensor, cond: torch.Tensor, length: int) -> dict:
+    def precompute_conditioning(self, prompt: torch.Tensor, cond: torch.Tensor, length: int,
+                                saved: Optional[dict] = None) -> dict:
         """Everything in `forward` that depends on (prompt, cond) but not on the timestep or x:
-        prompt FiLM vector, perceiver latents, projected aligned condition (ns2.py:947-992)."""
+        prompt FiLM vector, perceiver latents, projected aligned condition (ns2.py:947-992).  `saved`: see
+        `_forward_impl`."""
         assert self.condition_on_prompt
         P, D = self.packed(), self.dim
         B = prompt.shape[0]
@@ -446,12 +449,14 @@ class Model(nn.Module):
         prompt_cond = ops.small_linear(mean, lin.weight.detach().float().contiguous(),
                                        lin.bias.detach().float().contiguous(),
                                        torch.empty(B, self.dim_time, device=dev), act=1)
-        tokens = self._perceiver(prompt)
+        tokens = self._perceiver(prompt, P, saved)
         L = cond.shape[-1]
-        c_bf = ops.transpose_cast(cond.float().contiguous(), torch.empty(B, L, self.dim_prompt, device=dev,
-                                                                         dtype=torch.bfloat16))
-        cond_proj = ops.gemm(c_bf, P["cond_w"], torch.empty(B, L, D, device=dev), n=D, epilogue=ops.EPI_F32,
+        cond_bf = ops.transpose_cast(cond.float().contiguous(), torch.empty(B, L, self.dim_prompt, device=dev,
+                                                                            dtype=torch.bfloat16))
+        cond_proj = ops.gemm(cond_bf, P["cond_w"], torch.empty(B, L, D, device=dev), n=D, epilogue=ops.EPI_F32,
                              bias=P["cond_b"])
+        if saved is not None:
+            saved.update(prompt_mean=mean, cond_bf=cond_bf, Lc=L)
         return Conditioning(prompt_cond=prompt_cond, tokens=tokens, cond_proj=cond_proj, length=length)
 
     def _run(self, name, fn, *args, **kwargs):
@@ -567,7 +572,12 @@ class Model(nn.Module):
 
     @torch.no_grad()
     def _forward_impl(self, x, times, prompt=None, prompt_mask=None, cond=None, cond_drop_prob=None,
-                      _conditioning: Optional[dict] = None, out: Optional[torch.Tensor] = None):
+                      _conditioning: Optional[dict] = None, out: Optional[torch.Tensor] = None,
+                      saved: Optional[dict] = None):
+        """The denoiser's forward.  Without `saved` every intermediate lives in the per-shape workspace, so the call can
+        be captured in a CUDA graph.  With `saved` (a dict; the training forward of `training.DenoiserFunction`) the
+        workspace is not touched: each activation `training.train_backward` reads goes to a fresh tensor recorded
+        there, together with the residual stream before each branch and the attention log-sum-exps."""
         if prompt_mask is not None:
             raise NotImplementedError("prompt_mask is unsupported (the reference itself fails on it, SURVEY T9)")
         if not x.is_cuda:
@@ -576,14 +586,21 @@ class Model(nn.Module):
         assert D == self.dim, f"expected last dim {self.dim}, got {D}"
         dev = x.device
         P = self.packed()
-        ws = self._workspace(B, N, dev)
         G, inner, H = self.wavenet_layers, self.inner, self.heads
+        Dp = _round_up(self.ff_inner, 128)
+        keep = saved is not None
+        if keep:
+            buf = lambda name, *s, dt=torch.bfloat16: torch.empty(*s, device=dev, dtype=dt)  # noqa: E731
+        else:
+            ws = self._workspace(B, N, dev)
+            buf = lambda name, *s, dt=None: ws[name]  # noqa: E731
         cond_drop_prob = self.cond_drop_prob if cond_drop_prob is None else cond_drop_prob
 
         # ---- time / prompt conditioning vector t: (B, dim_cond) ----
-        t = ws["t"]
+        times = times.float().contiguous()
+        t = buf("t", B, self.dim_cond, dt=torch.float32)
         tc = self.to_time_cond
-        self._run("time_cond", ops.time_cond, times.float().contiguous(), tc[0].weights.detach().float().contiguous(),
+        self._run("time_cond", ops.time_cond, times, tc[0].weights.detach().float().contiguous(),
                       tc[1].weight.detach().float().contiguous(), tc[1].bias.detach().float().contiguous(),
                       t[:, :self.dim_time])
         c_tokens = None
@@ -592,72 +609,96 @@ class Model(nn.Module):
             if _conditioning is None:
                 assert _exists(prompt), "prompt is required when condition_on_prompt=True"
                 assert _exists(cond), "cond is required when condition_on_prompt=True"
-                _conditioning = self.precompute_conditioning(prompt, cond, N)
+                _conditioning = self.precompute_conditioning(prompt, cond, N, saved)
             # two independent draws, in the reference's order (ns2.py:950, 980): kept in torch for RNG-stream parity
             drop_mask = _prob_mask_like((B,), cond_drop_prob, dev)
             cond_drop_mask = _prob_mask_like((B,), cond_drop_prob, dev)
             ops.select_rows(drop_mask, self.null_prompt_cond.detach().float().contiguous(),
                             _conditioning["prompt_cond"], t[:, self.dim_time:])
             c_tokens = ops.select_rows(drop_mask, self.null_prompt_tokens.detach().float().contiguous(),
-                                       _conditioning["tokens"], ws["c_bf"])
+                                       _conditioning["tokens"], buf("c_bf", B, self.num_latents_m, D))
+            if keep:
+                saved.update(drop=drop_mask, cdrop=cond_drop_mask, c_bf=c_tokens)
 
         # ---- all FiLM (gamma, beta) vectors in one GEMM ----
-        self._run("cast", ops.cast_bf16, t, ws["t_bf"])
-        film = self._run("film", ops.gemm, ws["t_bf"], P["film_w"], ws["film"], n=P["film_w"].shape[0], epilogue=ops.EPI_F32,
-                        bias=P["film_b"])[0]  # (B, rows)
+        rows = P["film_w"].shape[0]
+        t_bf = self._run("cast", ops.cast_bf16, t, buf("t_bf", 1, B, self.dim_cond))
+        film = self._run("film", ops.gemm, t_bf, P["film_w"], buf("film", 1, B, rows, dt=torch.float32), n=rows,
+                         epilogue=ops.EPI_F32, bias=P["film_b"])[0]  # (B, rows)
 
         # ---- wavenet ----
         if self.condition_on_prompt:
             # x + pad_or_curtail(where(cond_drop_mask, null_cond, cond_proj)) -> bf16 in one pass (ns2.py:982-992)
-            x_bf = self._run("cast", ops.cond_inject, x.float().contiguous(), _conditioning["cond_proj"], ws["x_bf"],
-                             drop_mask=cond_drop_mask, null_cond=self.null_cond.detach().float().reshape(-1))
+            x_bf = self._run("cast", ops.cond_inject, x.float().contiguous(), _conditioning["cond_proj"],
+                             buf("x_bf", B, N, D), drop_mask=cond_drop_mask,
+                             null_cond=self.null_cond.detach().float().reshape(-1))
         else:
-            x_bf = self._run("cast", ops.cast_bf16, x.float().contiguous(), ws["x_bf"])
-        h = self._run("wn_init", ops.gemm, x_bf, P["wn_init_w"], ws["h"], n=D, epilogue=ops.EPI_BF16, bias=P["wn_init_b"],
-                     segs=ops.conv3_segs(D))
+            x_bf = self._run("cast", ops.cast_bf16, x.float().contiguous(), buf("x_bf", B, N, D))
+        h0 = self._run("wn_init", ops.gemm, x_bf, P["wn_init_w"], buf("h", B, N, D), n=D, epilogue=ops.EPI_BF16,
+                       bias=P["wn_init_b"], segs=ops.conv3_segs(D))
         segs = ops.conv3_segs(D) + [(0, 3 * D, D, 0, 1)]
         dil = [2 ** i for i in range(G)]
-        src, bufs = h, (ws["wn_a"], ws["wn_b"])
+        src, stack_out = h0, []
         for s in range(self.wavenet_stacks):
-            dst = bufs[s % 2]
+            dst = buf(("wn_a", "wn_b")[s % 2], B, N, G * D)
             self._run("wn_stack", ops.gemm, src, P[f"wn{s}_w"], dst, n=D, epilogue=ops.EPI_WAVENET, bias=P[f"wn{s}_b"],
                      bias1_off=G * D, segs=segs, film=film[:, s * G * 2 * D:], film_group_stride=2 * D,
                      groups=G, a_group_col_stride=0 if s == 0 else D, b_group_row_stride=D,
                      out_group_col_stride=D, dil=dil)
+            stack_out.append(dst)
             src = dst
-        skip = self._run("wn_skip", ops.gemm, src, P["wn_skip_w"], ws["h"], n=D, epilogue=ops.EPI_BF16, bias=P["wn_skip_b"])
-        xr = self._run("wn_final", ops.gemm, skip, P["wn_final_w"], ws["x_res"], n=D, epilogue=ops.EPI_F32, bias=P["wn_final_b"])
+        skip = self._run("wn_skip", ops.gemm, src, P["wn_skip_w"], buf("h", B, N, D), n=D, epilogue=ops.EPI_BF16,
+                         bias=P["wn_skip_b"])
+        xr = self._run("wn_final", ops.gemm, skip, P["wn_final_w"], buf("x_res", B, N, D, dt=torch.float32), n=D,
+                       epilogue=ops.EPI_F32, bias=P["wn_final_b"])
+        if keep:
+            saved.update(B=B, N=N, times=times, t=t, film=film, x_bf=x_bf, h0=h0, stack_out=stack_out, skip=skip)
 
         # ---- transformer ----
+        lse = lambda: torch.empty(B, H, N, device=dev, dtype=torch.float32) if keep else None  # noqa: E731
         if c_tokens is not None:
-            self._run("x_kv", ops.gemm, ws["c_bf"], P["x_kv_all"], ws["xkv"], n=self.depth * 2 * inner, epilogue=ops.EPI_BF16)
-        qkv, ao = ws["qkv"], ws["attn_o"]
-        Dp = ws["ff_g"].shape[-1]
+            xkv = self._run("x_kv", ops.gemm, c_tokens, P["x_kv_all"], buf("xkv", B, self.num_latents_m, self.depth * 2 * inner),
+                            n=self.depth * 2 * inner, epilogue=ops.EPI_BF16)
+            if keep:
+                saved["xkv"] = xkv
         npl = self._norms_per_layer
+        layers = []
         for l in range(self.depth):
             fo = self._film_tr_off + l * npl * 2 * D
-            self._run("norm", ops.rmsnorm_film, xr, ws["h"], film=film[:, fo:fo + 2 * D])
-            self._run("qkv", ops.gemm, ws["h"], P[f"l{l}_qkv"], qkv, n=3 * inner, epilogue=ops.EPI_BF16)
-            self._run("attn", ops.attention, qkv[:, :, :inner], qkv[:, :, inner:2 * inner], qkv[:, :, 2 * inner:], ao, heads=H)
-            self._run("attn_out", ops.gemm, ao, P[f"l{l}_o"], xr, n=D, epilogue=ops.EPI_F32, resid=xr)
-            j = 1
-            if c_tokens is not None:
+            L = {"x_in": xr.clone()} if keep else {}
+            L["h1"] = self._run("norm", ops.rmsnorm_film, xr, buf("h", B, N, D), film=film[:, fo:fo + 2 * D])
+            qkv = L["qkv"] = self._run("qkv", ops.gemm, L["h1"], P[f"l{l}_qkv"], buf("qkv", B, N, 3 * inner),
+                                       n=3 * inner, epilogue=ops.EPI_BF16)
+            L["lse"] = lse()
+            L["ao"] = self._run("attn", ops.attention, qkv[:, :, :inner], qkv[:, :, inner:2 * inner],
+                                qkv[:, :, 2 * inner:], buf("attn_o", B, N, inner), heads=H, lse=L["lse"])
+            self._run("attn_out", ops.gemm, L["ao"], P[f"l{l}_o"], xr, n=D, epilogue=ops.EPI_F32, resid=xr)
+            if c_tokens is not None:   # cross attention over the perceiver latents (ns2.py:800-803)
                 fo2 = fo + 2 * D
-                self._run("norm", ops.rmsnorm_film, xr, ws["h"], film=film[:, fo2:fo2 + 2 * D])
-                self._run("x_q", ops.gemm, ws["h"], P[f"l{l}_xq"], ws["xq"], n=inner, epilogue=ops.EPI_BF16)
-                kv = ws["xkv"][:, :, l * 2 * inner:(l + 1) * 2 * inner]
-                self._run("x_attn", ops.attention, ws["xq"], kv[:, :, :inner], kv[:, :, inner:], ao, heads=H)
-                self._run("x_out", ops.gemm, ao, P[f"l{l}_xo"], xr, n=D, epilogue=ops.EPI_F32, resid=xr)
-                j = 2
-            fo3 = fo + j * 2 * D
-            self._run("norm", ops.rmsnorm_film, xr, ws["h"], film=film[:, fo3:fo3 + 2 * D])
-            self._run("ff_in", ops.gemm, ws["h"], P[f"l{l}_ff_w1"], ws["ff_g"], n=2 * Dp, epilogue=ops.EPI_GEGLU,
-                     bias=P[f"l{l}_ff_b1"])
-            self._run("ff_conv", ops.gemm, ws["ff_g"], P[f"l{l}_ff_wc"], ws["ff_c"], n=Dp, epilogue=ops.EPI_BF16,
-                     bias=P[f"l{l}_ff_bc"], segs=ops.conv3_segs(Dp))
-            self._run("ff_out", ops.gemm, ws["ff_c"], P[f"l{l}_ff_w2"], xr, n=D, epilogue=ops.EPI_F32, bias=P[f"l{l}_ff_b2"],
-                     resid=xr)
-        self._run("norm", ops.rmsnorm_film, xr, ws["h"], gamma=P["pred_gamma"])
+                if keep:
+                    L["x_c"] = xr.clone()
+                L["h_x"] = self._run("norm", ops.rmsnorm_film, xr, buf("h", B, N, D), film=film[:, fo2:fo2 + 2 * D])
+                L["xq"] = self._run("x_q", ops.gemm, L["h_x"], P[f"l{l}_xq"], buf("xq", B, N, inner), n=inner,
+                                    epilogue=ops.EPI_BF16)
+                kv = xkv[:, :, l * 2 * inner:(l + 1) * 2 * inner]
+                L["lse2"] = lse()
+                L["ao2"] = self._run("x_attn", ops.attention, L["xq"], kv[:, :, :inner], kv[:, :, inner:],
+                                     buf("attn_o", B, N, inner), heads=H, lse=L["lse2"])
+                self._run("x_out", ops.gemm, L["ao2"], P[f"l{l}_xo"], xr, n=D, epilogue=ops.EPI_F32, resid=xr)
+            if keep:
+                L["x_mid"] = xr.clone()
+            fo3 = fo + (npl - 1) * 2 * D
+            L["h2"] = self._run("norm", ops.rmsnorm_film, xr, buf("h", B, N, D), film=film[:, fo3:fo3 + 2 * D])
+            L["ff_g"] = self._run("ff_in", ops.gemm, L["h2"], P[f"l{l}_ff_w1"], buf("ff_g", B, N, Dp), n=2 * Dp,
+                                  epilogue=ops.EPI_GEGLU, bias=P[f"l{l}_ff_b1"])
+            L["ff_c"] = self._run("ff_conv", ops.gemm, L["ff_g"], P[f"l{l}_ff_wc"], buf("ff_c", B, N, Dp), n=Dp,
+                                  epilogue=ops.EPI_BF16, bias=P[f"l{l}_ff_bc"], segs=ops.conv3_segs(Dp))
+            self._run("ff_out", ops.gemm, L["ff_c"], P[f"l{l}_ff_w2"], xr, n=D, epilogue=ops.EPI_F32,
+                      bias=P[f"l{l}_ff_b2"], resid=xr)
+            layers.append(L)
+        hf = self._run("norm", ops.rmsnorm_film, xr, buf("h", B, N, D), gamma=P["pred_gamma"])
+        if keep:
+            saved.update(layers=layers, x_final=xr, hf=hf)
         if out is None:
             out = torch.empty(B, N, D, device=dev, dtype=torch.float32)   # fresh tensor, like the reference
-        return self._run("pred", ops.gemm, ws["h"], P["pred_w"], out, n=D, epilogue=ops.EPI_F32)
+        return self._run("pred", ops.gemm, hf, P["pred_w"], out, n=D, epilogue=ops.EPI_F32)

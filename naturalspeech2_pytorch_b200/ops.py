@@ -147,12 +147,22 @@ def wgrad(dy: torch.Tensor, x: torch.Tensor, dw: torch.Tensor, *, n: int, k: int
     return dw
 
 
-def conv3_segs(k_len: int, tap_stride: Optional[int] = None, acc: int = 0, a_col_off: int = 0,
-               b_col_off: int = 0) -> list:
-    """Segments of a causal k=3 conv whose packed weight holds tap t at columns [t*tap_stride, +k_len):
-    tap t multiplies x[n - (2 - t) * dilation]   (CausalConv1d, ns2.py:583-595)."""
-    ts = k_len if tap_stride is None else tap_stride
-    return [(a_col_off, b_col_off + t * ts, k_len, 2 - t, acc) for t in range(3)]
+def conv_segs(c_in: int, kernel: int, first_shift: int) -> list:
+    """Segments of a stride-1 convolution whose packed weight holds tap t at columns [t*c_in, (t+1)*c_in): tap t reads
+    x[n - (first_shift - t) * dilation].  Causal k=3 (CausalConv1d, ns2.py:583-595): first_shift = 2; "same" padding p:
+    first_shift = p."""
+    return [(0, t * c_in, c_in, first_shift - t, 0) for t in range(kernel)]
+
+
+def conv3_segs(c_in: int) -> list:
+    """`conv_segs` of the denoiser's causal k=3 convs (CausalConv1d, ns2.py:583-595)."""
+    return conv_segs(c_in, 3, 2)
+
+
+def conv_dgrad_segs(c_out: int, kernel: int, first_shift: int) -> list:
+    """Segments of the input gradient of a `conv_segs` convolution on the transposed pack ([in][tap][out]): tap t reads
+    d out at n + (first_shift - t), the mirrored shift."""
+    return [(0, t * c_out, c_out, t - first_shift, 0) for t in range(kernel)]
 
 
 # --------------------------------------------------------------------------------------------------

@@ -1,7 +1,9 @@
-"""Training step of the denoiser: forward with saved activations + hand-written backward (SURVEY rows a18 / f1).
+"""Training step of the denoiser: hand-written backward of `Model._forward_impl` (SURVEY rows a18 / f1).
 
 `loss.backward()` is how the reference is used (README.md:60-63, ns2.py:1886).  Here `Model.forward` records ONE autograd
-node (`DenoiserFunction`) when gradients are enabled; its backward walks the network in reverse and launches, per layer,
+node (`DenoiserFunction`) when gradients are enabled.  Its forward is the inference forward, `Model._forward_impl`, given
+a `saved` dict: the same kernels in the same order (bit-identical output) with the activations the backward needs kept in
+fresh tensors.  Its backward walks the network in reverse and launches, per layer,
   * dgrad GEMMs     ns2_gemm on transposed weight packs (anti-causal shifts for the causal convs),
   * wgrad GEMMs     ns2_wgrad (wgmma, MN-major operands, fp32 reduce-add into the packed gradient),
   * attention bwd   ns2_attn_bwd (wgmma flash backward from the saved log-sum-exp),
@@ -9,6 +11,7 @@ node (`DenoiserFunction`) when gradients are enabled; its backward walks the net
 Pre-activations that the fused forward epilogues never materialise (GEGLU's value/gate pair, the Wavenet conv output
 before FiLM) are recomputed with plain-epilogue GEMMs instead of being stored.  Gradients come out in the packed bf16
 layouts' fp32 twins and are scattered back to the reference's parameter shapes (same keys as the state_dict).
+`geglu_backward` and `attention_backward` are shared with the encoders' backward (encoders.py).
 
 Scope: unconditional and conditional denoisers (BASELINE configs[1], configs[2]/[4]): perceiver resampler, cross
 attention, prompt FiLM vector, aligned-condition projection and the classifier-free-guidance null parameters included.
@@ -24,18 +27,21 @@ view); otherwise nothing extra runs.  `x` and `times` stay non-differentiable (l
 from __future__ import annotations
 
 import math
-from typing import Dict, List
+from typing import Dict
 
 import torch
 import torch.nn.functional as F
 
 from . import ops
+from .model import _round_up
 
 bf = torch.bfloat16
 
 
-def _round_up(v: int, m: int) -> int:
-    return (v + m - 1) // m * m
+def _transpose_conv(w: torch.Tensor, kernel: int) -> torch.Tensor:
+    """(O, k*I) tap-major conv pack -> (I, k*O) [in][tap][out] pack for the dgrad GEMM."""
+    O = w.shape[0]
+    return w.view(O, kernel, -1).permute(2, 1, 0).reshape(-1, kernel * O).contiguous()
 
 
 def pack_transposed(model) -> Dict[str, torch.Tensor]:
@@ -54,12 +60,10 @@ def pack_transposed(model) -> Dict[str, torch.Tensor]:
         T[f"l{l}_qkv"] = t(P[f"l{l}_qkv"])                              # (D, 3*inner)
         T[f"l{l}_o"] = t(P[f"l{l}_o"])                                  # (inner, D)
         T[f"l{l}_ff_w1"] = t(P[f"l{l}_ff_w1"])                          # (D, 2*Dp)
-        wc = P[f"l{l}_ff_wc"]                                           # (Dp, 3*Dp) tap-major columns
-        Dp = wc.shape[0]
-        T[f"l{l}_ff_wc"] = wc.view(Dp, 3, Dp).permute(2, 1, 0).reshape(Dp, 3 * Dp).contiguous()   # [in][tap][out]
+        T[f"l{l}_ff_wc"] = _transpose_conv(P[f"l{l}_ff_wc"], 3)         # (Dp, 3*Dp)
         T[f"l{l}_ff_w2"] = t(P[f"l{l}_ff_w2"])                          # (Dp, D)
     T["pred_w"] = t(P["pred_w"])
-    T["wn_init_w"] = P["wn_init_w"].view(D, 3, D).permute(2, 1, 0).reshape(D, 3 * D).contiguous()   # [in][tap][out]
+    T["wn_init_w"] = _transpose_conv(P["wn_init_w"], 3)
     if model.condition_on_prompt:
         T["cond_w"] = t(P["cond_w"])                                   # (dim_prompt, D): d cond
         if "pr_proj_w" in P:
@@ -74,139 +78,43 @@ def pack_transposed(model) -> Dict[str, torch.Tensor]:
     return T
 
 
-def _perceiver_forward(model, prompt_f, S):
-    """PerceiverResampler.forward (ns2.py:568-579) keeping per-layer activations -> tokens (B, M, D) fp32."""
-    P, D, M, inner, H = model.packed(), model.dim, model.num_latents_m, model.inner, model.heads
-    pr = model.perceiver_resampler
-    B, Np, _ = prompt_f.shape
-    dev = prompt_f.device
-    e = lambda *s, dt=bf: torch.empty(*s, device=dev, dtype=dt)
-    ctx = M + Np
-    Dp = _round_up(model.ff_inner, 128)
-    p_bf = ops.cast_bf16(prompt_f, e(B, Np, model.dim_prompt))
-    if "pr_proj_w" in P:
-        proj = ops.gemm(p_bf, P["pr_proj_w"], e(B, Np, D), n=D, epilogue=ops.EPI_BF16, bias=P["pr_proj_b"])
-    else:
-        proj = p_bf
-    lat = pr.latents.detach().float().unsqueeze(0).expand(B, M, D).contiguous()
-    layers = []
-    for i in range(len(pr.layers)):
-        L = {}
-        L["lat_bf"] = ops.cast_bf16(lat, e(B, M, D))
-        cat = e(B, ctx, D)
-        cat[:, :M].copy_(L["lat_bf"])     # cross_attn_include_queries: keys = cat(latents, context) (ns2.py:1060-1061)
-        cat[:, M:].copy_(proj)
-        L["cat"] = cat
-        L["q"] = ops.gemm(L["lat_bf"], P[f"pr{i}_q"], e(B, M, inner), n=inner, epilogue=ops.EPI_BF16)
-        L["kv"] = ops.gemm(cat, P[f"pr{i}_kv"], e(B, ctx, 2 * inner), n=2 * inner, epilogue=ops.EPI_BF16)
-        L["lse"] = e(B, H, M, dt=torch.float32)
-        L["o"] = ops.attention(L["q"], L["kv"][:, :, :inner], L["kv"][:, :, inner:], e(B, M, inner), heads=H, lse=L["lse"])
-        ops.gemm(L["o"], P[f"pr{i}_o"], lat, n=D, epilogue=ops.EPI_F32, resid=lat)
-        L["lat_bf2"] = ops.cast_bf16(lat, e(B, M, D))
-        L["g"] = ops.gemm(L["lat_bf2"], P[f"pr{i}_ff_w1"], e(B, M, Dp), n=2 * Dp, epilogue=ops.EPI_GEGLU, bias=P[f"pr{i}_ff_b1"])
-        ops.gemm(L["g"], P[f"pr{i}_ff_w2"], lat, n=D, epilogue=ops.EPI_F32, bias=P[f"pr{i}_ff_b2"], resid=lat)
-        layers.append(L)
-    S.update(pr_layers=layers, pr_lat=lat, pr_p_bf=p_bf, pr_Np=Np)
-    return ops.rmsnorm_f32(lat, e(B, M, D, dt=torch.float32), pr.norm.gamma.detach().float().contiguous())
+def geglu_backward(h, d_g, w1, b1, w1_t, Di: int, grads: Dict[str, torch.Tensor], name: str) -> torch.Tensor:
+    """Backward of g = GEGLU(h @ w1^T + b1), w1 / b1 packed by `model._pack_geglu` (inner width Di padded to Dp): the
+    pre-activation is recomputed with a plain-epilogue GEMM, lin1's gradients go to grads[name + ".weight" / ".bias"] in
+    the reference's layout (value rows, then gate rows), and d h (bf16) is returned."""
+    B, N, D = h.shape
+    Dp = w1.shape[0] // 2
+    dev = h.device
+    pre = ops.gemm(h, w1, torch.empty(B, N, 2 * Dp, device=dev, dtype=bf), n=2 * Dp, epilogue=ops.EPI_BF16, bias=b1)
+    ops.geglu_bwd(pre, d_g)                                                              # pre <- d pre
+    dW1 = ops.wgrad(pre, h, torch.zeros(2 * Dp, D, device=dev), n=2 * Dp, k=D).view(Dp // 128, 2, 128, D)
+    db1 = ops.colsum(pre, torch.zeros(2 * Dp, device=dev)).view(Dp // 128, 2, 128)
+    grads[name + ".weight"] = torch.cat((dW1[:, 0].reshape(Dp, D)[:Di], dW1[:, 1].reshape(Dp, D)[:Di]), dim=0)
+    grads[name + ".bias"] = torch.cat((db1[:, 0].reshape(Dp)[:Di], db1[:, 1].reshape(Dp)[:Di]), dim=0)
+    return ops.gemm(pre, w1_t, torch.empty(B, N, D, device=dev, dtype=bf), n=D, epilogue=ops.EPI_BF16)
 
 
-def train_forward(model, x: torch.Tensor, times: torch.Tensor, prompt=None, cond=None, cond_drop_prob=None):
-    """Same arithmetic as `Model._forward_impl` (ns2.py:929-1000), keeping what the backward needs."""
-    from .model import _prob_mask_like
-    B, N, D = x.shape
-    dev = x.device
-    P = model.packed()
-    G, inner, H = model.wavenet_layers, model.inner, model.heads
-    Dp = _round_up(model.ff_inner, 128)
-    e = lambda *s, dt=bf: torch.empty(*s, device=dev, dtype=dt)
-    S: Dict[str, object] = {"B": B, "N": N}
-    tc = model.to_time_cond
-    t = e(B, model.dim_cond, dt=torch.float32)
-    ops.time_cond(times.float().contiguous(), tc[0].weights.detach().float().contiguous(),
-                  tc[1].weight.detach().float().contiguous(), tc[1].bias.detach().float().contiguous(),
-                  t[:, :model.dim_time])
-    conditional = model.condition_on_prompt
-    c_bf = None
-    if conditional:
-        assert prompt is not None and cond is not None, "prompt and cond are required when condition_on_prompt=True"
-        M = model.num_latents_m
-        p_eff = model.cond_drop_prob if cond_drop_prob is None else cond_drop_prob
-        drop = _prob_mask_like((B,), p_eff, dev)          # same two draws, same order as the reference (ns2.py:950, 980)
-        cdrop = _prob_mask_like((B,), p_eff, dev)
-        prompt_f = prompt.float().contiguous()
-        mean = ops.mean_rows(prompt_f, e(B, model.dim_prompt, dt=torch.float32))
-        lin = model.to_prompt_cond[1]
-        raw_pc = ops.small_linear(mean, lin.weight.detach().float().contiguous(), lin.bias.detach().float().contiguous(),
-                                  e(B, model.dim_time, dt=torch.float32), act=1)
-        ops.select_rows(drop, model.null_prompt_cond.detach().float().contiguous(), raw_pc, t[:, model.dim_time:])
-        tokens = _perceiver_forward(model, prompt_f, S)
-        c_bf = ops.select_rows(drop, model.null_prompt_tokens.detach().float().contiguous(), tokens, e(B, M, D))
-        Lc = cond.shape[-1]
-        cond_bf = ops.transpose_cast(cond.float().contiguous(), e(B, Lc, model.dim_prompt))
-        cond_proj = ops.gemm(cond_bf, P["cond_w"], e(B, Lc, D, dt=torch.float32), n=D, epilogue=ops.EPI_F32, bias=P["cond_b"])
-        S.update(drop=drop, cdrop=cdrop, prompt_mean=mean, c_bf=c_bf, cond_bf=cond_bf, Lc=Lc)
-    t_bf = ops.cast_bf16(t, e(1, B, model.dim_cond))
-    film = ops.gemm(t_bf, P["film_w"], e(1, B, P["film_w"].shape[0], dt=torch.float32), n=P["film_w"].shape[0],
-                    epilogue=ops.EPI_F32, bias=P["film_b"])[0]
-    S.update(times=times.float().contiguous(), t=t, film=film)
-    # ---- wavenet ----
-    if conditional:
-        x_bf = ops.cond_inject(x.float().contiguous(), cond_proj, e(B, N, D), drop_mask=cdrop,
-                               null_cond=model.null_cond.detach().float().reshape(-1))
-    else:
-        x_bf = ops.cast_bf16(x.float().contiguous(), e(B, N, D))
-    h0 = ops.gemm(x_bf, P["wn_init_w"], e(B, N, D), n=D, epilogue=ops.EPI_BF16, bias=P["wn_init_b"], segs=ops.conv3_segs(D))
-    segs = ops.conv3_segs(D) + [(0, 3 * D, D, 0, 1)]
-    dil = [2 ** i for i in range(G)]
-    src, stack_out = h0, []
-    for s in range(model.wavenet_stacks):
-        dst = e(B, N, G * D)
-        ops.gemm(src, P[f"wn{s}_w"], dst, n=D, epilogue=ops.EPI_WAVENET, bias=P[f"wn{s}_b"], bias1_off=G * D, segs=segs,
-                 film=film[:, s * G * 2 * D:], film_group_stride=2 * D, groups=G,
-                 a_group_col_stride=0 if s == 0 else D, b_group_row_stride=D, out_group_col_stride=D, dil=dil)
-        stack_out.append(dst)
-        src = dst
-    skip = ops.gemm(src, P["wn_skip_w"], e(B, N, D), n=D, epilogue=ops.EPI_BF16, bias=P["wn_skip_b"])
-    xr = ops.gemm(skip, P["wn_final_w"], e(B, N, D, dt=torch.float32), n=D, epilogue=ops.EPI_F32, bias=P["wn_final_b"])
-    S.update(x_bf=x_bf, h0=h0, stack_out=stack_out, skip=skip)
-    # ---- transformer ----
-    layers: List[dict] = []
-    npl = model._norms_per_layer
-    if conditional:
-        S["xkv"] = ops.gemm(c_bf, P["x_kv_all"], e(B, model.num_latents_m, model.depth * 2 * inner),
-                            n=model.depth * 2 * inner, epilogue=ops.EPI_BF16)
-    for l in range(model.depth):
-        fo = model._film_tr_off + l * npl * 2 * D
-        L: Dict[str, torch.Tensor] = {"x_in": xr.clone()}
-        L["h1"] = ops.rmsnorm_film(xr, e(B, N, D), film=film[:, fo:fo + 2 * D])
-        L["qkv"] = ops.gemm(L["h1"], P[f"l{l}_qkv"], e(B, N, 3 * inner), n=3 * inner, epilogue=ops.EPI_BF16)
-        L["lse"] = e(B, H, N, dt=torch.float32)
-        qkv = L["qkv"]
-        L["ao"] = ops.attention(qkv[:, :, :inner], qkv[:, :, inner:2 * inner], qkv[:, :, 2 * inner:], e(B, N, inner),
-                                heads=H, lse=L["lse"])
-        ops.gemm(L["ao"], P[f"l{l}_o"], xr, n=D, epilogue=ops.EPI_F32, resid=xr)
-        if conditional:   # cross attention over the perceiver latents (ns2.py:800-803)
-            fo2 = fo + 2 * D
-            L["x_c"] = xr.clone()
-            L["h_x"] = ops.rmsnorm_film(xr, e(B, N, D), film=film[:, fo2:fo2 + 2 * D])
-            L["xq"] = ops.gemm(L["h_x"], P[f"l{l}_xq"], e(B, N, inner), n=inner, epilogue=ops.EPI_BF16)
-            kv = S["xkv"][:, :, l * 2 * inner:(l + 1) * 2 * inner]
-            L["lse2"] = e(B, H, N, dt=torch.float32)
-            L["ao2"] = ops.attention(L["xq"], kv[:, :, :inner], kv[:, :, inner:], e(B, N, inner), heads=H, lse=L["lse2"])
-            ops.gemm(L["ao2"], P[f"l{l}_xo"], xr, n=D, epilogue=ops.EPI_F32, resid=xr)
-        L["x_mid"] = xr.clone()
-        fo3 = fo + (npl - 1) * 2 * D
-        L["h2"] = ops.rmsnorm_film(xr, e(B, N, D), film=film[:, fo3:fo3 + 2 * D])
-        L["ff_g"] = ops.gemm(L["h2"], P[f"l{l}_ff_w1"], e(B, N, Dp), n=2 * Dp, epilogue=ops.EPI_GEGLU, bias=P[f"l{l}_ff_b1"])
-        L["ff_c"] = ops.gemm(L["ff_g"], P[f"l{l}_ff_wc"], e(B, N, Dp), n=Dp, epilogue=ops.EPI_BF16, bias=P[f"l{l}_ff_bc"],
-                             segs=ops.conv3_segs(Dp))
-        ops.gemm(L["ff_c"], P[f"l{l}_ff_w2"], xr, n=D, epilogue=ops.EPI_F32, bias=P[f"l{l}_ff_b2"], resid=xr)
-        layers.append(L)
-    S["x_final"] = xr
-    S["hf"] = ops.rmsnorm_film(xr, e(B, N, D), gamma=P["pred_gamma"])
-    out = ops.gemm(S["hf"], P["pred_w"], e(B, N, D, dt=torch.float32), n=D, epilogue=ops.EPI_F32)
-    S["layers"] = layers
-    return out, S
+def attention_backward(L: dict, dxr, dxr_bf, w_o_t, w_qkv_t, heads: int, grads: Dict[str, torch.Tensor], name: str,
+                       **norm) -> None:
+    """Backward of x += Wo attn(Wqkv h1), h1 = RMSNorm(x_in), from the layer record L (x_in, h1, qkv, lse, ao):
+    to_out / to_q / to_kv gradients go to grads[name + ...]; dxr (fp32, in place) and dxr_bf become the gradient of x_in.
+    `norm` is the RMSNorm's part of ops.rmsnorm_film_bwd: film= / dfilm= or gamma= / dgamma=."""
+    B, N, D = dxr.shape
+    inner = heads * 64
+    dev = dxr.device
+    grads[name + "to_out.weight"] = ops.wgrad(dxr_bf, L["ao"], torch.zeros(D, inner, device=dev), n=D, k=inner)
+    d_ao = ops.gemm(dxr_bf, w_o_t, torch.empty(B, N, inner, device=dev, dtype=bf), n=inner, epilogue=ops.EPI_BF16)
+    qkv = L["qkv"]
+    d_qkv = torch.empty(B, N, 3 * inner, device=dev, dtype=bf)
+    dq = torch.zeros(B, N, inner, device=dev)
+    ops.attention_bwd(qkv[:, :, :inner], qkv[:, :, inner:2 * inner], qkv[:, :, 2 * inner:], L["ao"], d_ao, L["lse"],
+                      dq, d_qkv[:, :, inner:2 * inner], d_qkv[:, :, 2 * inner:], heads=heads)
+    d_qkv[:, :, :inner].copy_(dq)   # fp32 accumulator -> bf16 slot (layout glue)
+    dWqkv = ops.wgrad(d_qkv, L["h1"], torch.zeros(3 * inner, D, device=dev), n=3 * inner, k=D)
+    grads[name + "to_q.weight"] = dWqkv[:inner]
+    grads[name + "to_kv.weight"] = dWqkv[inner:]
+    dh1 = ops.gemm(d_qkv, w_qkv_t, torch.empty(B, N, D, device=dev, dtype=bf), n=D, epilogue=ops.EPI_BF16)
+    ops.rmsnorm_film_bwd(L["x_in"], dh1, dxr, dxr_bf, rows_per_batch=N, **norm)
 
 
 def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grads=None) -> Dict[str, torch.Tensor]:
@@ -248,7 +156,6 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grad
     if conditional:
         M = model.num_latents_m
         d_xkv = e(B, M, model.depth * 2 * inner)
-    pre = e(B, N, 2 * Dp)
     for l in reversed(range(model.depth)):
         L = S["layers"][l]
         pfx = f"transformer.layers.{l}."
@@ -264,15 +171,8 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grad
             ops.wgrad(d_c, L["ff_g"], dWc[:, tap * Dp:(tap + 1) * Dp], n=Dp, k=Dp, shift_units=2 - tap)
         grads[pfx + "5.2.1.weight"] = dWc.view(Dp, 3, Dp)[:Di, :, :Di].permute(0, 2, 1)
         grads[pfx + "5.2.1.bias"] = ops.colsum(d_c, z(Dp))[:Di]
-        d_g = ops.gemm(d_c, T[f"l{l}_ff_wc"], e(B, N, Dp), n=Dp, epilogue=ops.EPI_BF16,
-                       segs=[(0, tap * Dp, Dp, -(2 - tap), 0) for tap in range(3)])
-        ops.gemm(L["h2"], P[f"l{l}_ff_w1"], pre, n=2 * Dp, epilogue=ops.EPI_BF16, bias=P[f"l{l}_ff_b1"])   # recompute
-        ops.geglu_bwd(pre, d_g)                                                                              # pre <- d pre
-        dW1 = ops.wgrad(pre, L["h2"], z(2 * Dp, D), n=2 * Dp, k=D).view(Dp // 128, 2, 128, D)
-        db1 = ops.colsum(pre, z(2 * Dp)).view(Dp // 128, 2, 128)
-        grads[pfx + "5.0.weight"] = torch.cat((dW1[:, 0].reshape(Dp, D)[:Di], dW1[:, 1].reshape(Dp, D)[:Di]), dim=0)
-        grads[pfx + "5.0.bias"] = torch.cat((db1[:, 0].reshape(Dp)[:Di], db1[:, 1].reshape(Dp)[:Di]), dim=0)
-        dh2 = ops.gemm(pre, T[f"l{l}_ff_w1"], e(B, N, D), n=D, epilogue=ops.EPI_BF16)
+        d_g = ops.gemm(d_c, T[f"l{l}_ff_wc"], e(B, N, Dp), n=Dp, epilogue=ops.EPI_BF16, segs=ops.conv_dgrad_segs(Dp, 3, 2))
+        dh2 = geglu_backward(L["h2"], d_g, P[f"l{l}_ff_w1"], P[f"l{l}_ff_b1"], T[f"l{l}_ff_w1"], Di, grads, pfx + "5.0")
         ops.rmsnorm_film_bwd(L["x_mid"], dh2, dxr, dxr_bf, rows_per_batch=N, film=film[:, fo3:fo3 + 2 * D],
                              dfilm=dfilm[:, fo3:fo3 + 2 * D])
         # ---- cross-attention branch: x += Wxo attn(Wxq h_x, Wxkv c) ----
@@ -291,20 +191,8 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grad
             ops.rmsnorm_film_bwd(L["x_c"], dh_x, dxr, dxr_bf, rows_per_batch=N, film=film[:, fo2:fo2 + 2 * D],
                                  dfilm=dfilm[:, fo2:fo2 + 2 * D])
         # ---- attention branch: x += Wo attn(Wqkv h1) ----
-        grads[pfx + "1.to_out.weight"] = ops.wgrad(dxr_bf, L["ao"], z(D, inner), n=D, k=inner)
-        d_ao = ops.gemm(dxr_bf, T[f"l{l}_o"], e(B, N, inner), n=inner, epilogue=ops.EPI_BF16)
-        qkv = L["qkv"]
-        d_qkv = e(B, N, 3 * inner)
-        dq_acc = z(B, N, inner)
-        ops.attention_bwd(qkv[:, :, :inner], qkv[:, :, inner:2 * inner], qkv[:, :, 2 * inner:], L["ao"], d_ao, L["lse"],
-                          dq_acc, d_qkv[:, :, inner:2 * inner], d_qkv[:, :, 2 * inner:], heads=H)
-        d_qkv[:, :, :inner].copy_(dq_acc)   # fp32 accumulator -> bf16 slot (layout glue)
-        dWqkv = ops.wgrad(d_qkv, L["h1"], z(3 * inner, D), n=3 * inner, k=D)
-        grads[pfx + "1.to_q.weight"] = dWqkv[:inner]
-        grads[pfx + "1.to_kv.weight"] = dWqkv[inner:]
-        dh1 = ops.gemm(d_qkv, T[f"l{l}_qkv"], e(B, N, D), n=D, epilogue=ops.EPI_BF16)
-        ops.rmsnorm_film_bwd(L["x_in"], dh1, dxr, dxr_bf, rows_per_batch=N, film=film[:, fo:fo + 2 * D],
-                             dfilm=dfilm[:, fo:fo + 2 * D])
+        attention_backward(L, dxr, dxr_bf, T[f"l{l}_o"], T[f"l{l}_qkv"], H, grads, pfx + "1.",
+                           film=film[:, fo:fo + 2 * D], dfilm=dfilm[:, fo:fo + 2 * D])
         # FiLM projections of this layer's norms: their rows of dfilm are final now, so the weight gradient (the largest
         # gradient buffers of the model) joins this layer's all-reduce instead of trailing the whole backward
         dWl = ops.film_wgrad(dfilm[:, fo:fo + npl * 2 * D], t_cond, torch.empty(npl * 2 * D, model.dim_cond, device=dev),
@@ -367,7 +255,7 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grad
             grads[blk + "conv.bias"] = dbc[g * D:(g + 1) * D]
             grads[blk + "res_conv.bias"] = dbr[g * D:(g + 1) * D]
         # d(input of every column): anti-causal taps on dc + the transposed 1x1 on dy
-        segs = [(0, tap * D, D, -(2 - tap), 0) for tap in range(3)] + [(G * D, 3 * D, D, 0, 0)]
+        segs = ops.conv_dgrad_segs(D, 3, 2) + [(G * D, 3 * D, D, 0, 0)]
         d_in = e(B, N, G * D)
         ops.gemm(dcy, T[f"wn{s}_w"], d_in, n=D, epilogue=ops.EPI_BF16, segs=segs, groups=G, a_group_col_stride=D,
                  b_group_row_stride=D, out_group_col_stride=D, dil=dil)
@@ -383,8 +271,7 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grad
     grads["wavenet.init_conv.bias"] = ops.colsum(d_h0, z(D))
     if conditional:
         # x_in = x + pad_or_curtail(where(cdrop, null_cond, cond_proj)) (ns2.py:978-992): d x_in from the init conv's dgrad
-        d_xin = ops.gemm(d_h0, T["wn_init_w"], e(B, N, D), n=D, epilogue=ops.EPI_BF16,
-                         segs=[(0, tap * D, D, -(2 - tap), 0) for tap in range(3)])
+        d_xin = ops.gemm(d_h0, T["wn_init_w"], e(B, N, D), n=D, epilogue=ops.EPI_BF16, segs=ops.conv_dgrad_segs(D, 3, 2))
         Lc = S["Lc"]
         n_used = min(Lc, N)
         keep = (~S["cdrop"])[:, None, None]
@@ -475,7 +362,6 @@ def _conditioning_backward_tokens(model, S, T, d_xkv, grads):
     Np = S["pr_Np"]
     ctx = M + Np
     d_proj = z(B, Np, D)
-    pre = e(B, M, 2 * Dp)
     for i in reversed(range(len(pr.layers))):
         L = S["pr_layers"][i]
         pfx = f"perceiver_resampler.layers.{i}."
@@ -483,13 +369,8 @@ def _conditioning_backward_tokens(model, S, T, d_xkv, grads):
         grads[pfx + "1.2.weight"] = ops.wgrad(dlat_bf, L["g"], z(D, Dp), n=D, k=Dp)[:, :Di]
         grads[pfx + "1.2.bias"] = ops.colsum(dlat_bf, z(D))
         d_g = ops.gemm(dlat_bf, T[f"pr{i}_ff_w2"], e(B, M, Dp), n=Dp, epilogue=ops.EPI_BF16)
-        ops.gemm(L["lat_bf2"], P[f"pr{i}_ff_w1"], pre, n=2 * Dp, epilogue=ops.EPI_BF16, bias=P[f"pr{i}_ff_b1"])
-        ops.geglu_bwd(pre, d_g)
-        dW1 = ops.wgrad(pre, L["lat_bf2"], z(2 * Dp, D), n=2 * Dp, k=D).view(Dp // 128, 2, 128, D)
-        db1 = ops.colsum(pre, z(2 * Dp)).view(Dp // 128, 2, 128)
-        grads[pfx + "1.0.weight"] = torch.cat((dW1[:, 0].reshape(Dp, D)[:Di], dW1[:, 1].reshape(Dp, D)[:Di]), dim=0)
-        grads[pfx + "1.0.bias"] = torch.cat((db1[:, 0].reshape(Dp)[:Di], db1[:, 1].reshape(Dp)[:Di]), dim=0)
-        ops.accum_bf16(dlat, ops.gemm(pre, T[f"pr{i}_ff_w1"], e(B, M, D), n=D, epilogue=ops.EPI_BF16), dlat_bf)
+        ops.accum_bf16(dlat, geglu_backward(L["lat_bf2"], d_g, P[f"pr{i}_ff_w1"], P[f"pr{i}_ff_b1"], T[f"pr{i}_ff_w1"], Di,
+                                            grads, pfx + "1.0"), dlat_bf)
         # attention over cat(latents, projected prompt): lat += Wo attn(Wq lat, Wkv cat)
         grads[pfx + "0.to_out.weight"] = ops.wgrad(dlat_bf, L["o"], z(D, inner), n=D, k=inner)
         d_o = ops.gemm(dlat_bf, T[f"pr{i}_o"], e(B, M, inner), n=inner, epilogue=ops.EPI_BF16)
@@ -519,8 +400,8 @@ class DenoiserFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, model, x, times, prompt, cond, cond_drop_prob, *params):
-        with torch.no_grad():
-            out, saved = train_forward(model, x, times, prompt, cond, cond_drop_prob)
+        saved = {}
+        out = model._forward_impl(x, times, prompt, cond=cond, cond_drop_prob=cond_drop_prob, saved=saved)
         ctx.model, ctx.saved = model, saved
         ctx.names = [n for n, _ in model.named_parameters()]
         ctx.in_dtypes = (prompt.dtype if prompt is not None else None, cond.dtype if cond is not None else None)

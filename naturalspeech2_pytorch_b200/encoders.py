@@ -17,11 +17,12 @@ Training: in `train()` mode with gradients enabled (and parameters that require 
 `PhonemeEncoder.forward` record ONE autograd node each (`_EncoderFunction`, the pattern of training.DenoiserFunction).
 Its forward is the inference forward (`_forward` and `_transformer`) given a `saved` dict, which keeps the activations
 the backward needs (bit-identical output); its backward walks the encoder in reverse:
-  plain Transformer      out-proj / FF wgrad + dgrad GEMMs on transposed packs, training.attention_backward and
-                         training.geglu_backward (shared with the denoiser's backward), rmsnorm_film_bwd(gamma=...)
-  k=9 conv + SiLU        pre-activation recomputed with a plain-epilogue GEMM, ops.silu_bwd, one ops.wgrad per tap
-                         ("same" padding: shifts +4..-4, causal: 8..0), dgrad = one nine-segment GEMM with mirrored
-                         shifts (the prompt encoder's first conv needs none: its input comes from the codec)
+  plain Transformer      training.ff_backward and training.attention_backward (shared with the denoiser's backward)
+                         on the transposed packs, rmsnorm_film_bwd(gamma=...)
+  k=9 conv + SiLU        pre-activation recomputed with a plain-epilogue GEMM, ops.silu_bwd, then training.conv_backward:
+                         one ops.wgrad per tap ("same" padding: shifts +4..-4, causal: 8..0), dgrad = one nine-segment
+                         GEMM with mirrored shifts (the prompt encoder's first conv needs none: its input comes from the
+                         codec)
   nn.Embedding           ops.embedding_bwd (scatter-add; the pad row receives gradient, as in the reference)
 Dropout stays the identity in training, as in the denoiser (the reference's conv / attention dropout is not drawn).
 Attention masks are not supported (`mask=None` is what NaturalSpeech2.forward / .sample pass, ns2.py:1475-1476,
@@ -37,9 +38,10 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import _lib, ops
-from .ops import conv_dgrad_segs as _conv_dgrad_segs, conv_segs as _conv_segs
-from .model import _AttentionParams, _NoParam, _RMSNormParams, _bf, _feedforward_params, _pack_geglu
-from .training import _transpose_conv, attention_backward, geglu_backward
+from .ops import conv_segs as _conv_segs
+from .model import (_AttentionParams, _NoParam, _PackedCache, _RMSNormParams, _bf, _feedforward_params, _pack_conv,
+                    _pack_geglu, _records_graph, _transpose_conv)
+from .training import attention_backward, conv_backward, ff_backward, param_grads
 
 _SILU = _lib.NS2_GEMM_FLAG_SILU
 
@@ -56,16 +58,6 @@ class _PlainTransformerParams(nn.Module):
         self.norm = _RMSNormParams(dim) if final_norm else nn.Identity()
 
 
-def _pack_conv(w: torch.Tensor) -> torch.Tensor:
-    """(O, I, k) -> (O, k*I) bf16, tap t at columns [t*I, (t+1)*I)."""
-    O, I, k = w.shape
-    return _bf(w.detach().permute(0, 2, 1).reshape(O, k * I))
-
-
-def _records_graph(m: nn.Module) -> bool:
-    return m.training and torch.is_grad_enabled() and any(p.requires_grad for p in m.parameters())
-
-
 class _EncoderFunction(torch.autograd.Function):
     """One autograd node for a whole encoder: forward = the inference kernels keeping activations, backward = the
     hand-written kernels (`_train_backward`).  `reducer` (parallel.GradReducer or None) receives the parameter
@@ -80,54 +72,18 @@ class _EncoderFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, d_out):
-        enc = ctx.enc
         with torch.no_grad():
-            grads = enc._train_backward(ctx.saved, d_out)
+            grads = ctx.enc._train_backward(ctx.saved, d_out)
         ctx.saved = None
-        missing = [n for n, _ in enc.named_parameters() if n not in grads]
-        if missing:
-            raise RuntimeError(f"encoder backward produced no gradient for {missing[:4]}...")
-        if ctx.reducer is not None:
-            ctx.reducer.reduce_all(grads)
-            ctx.reducer.finish()
-        return (None, None, None, *[grads[n].reshape(p.shape).to(p.dtype) for n, p in enc.named_parameters()])
+        return (None, None, None, *param_grads(ctx.enc, grads, ctx.reducer))
 
 
-class _EncoderBase(nn.Module):
-    """Packing cache + the shared transformer forward / backward."""
+class _EncoderBase(_PackedCache):
+    """The shared transformer forward / backward of the encoders."""
 
-    def _init_cache(self):
-        self._packed: Optional[Dict[str, torch.Tensor]] = None
-        self._packed_sig = None
+    def __init__(self):
+        super().__init__()
         self.grad_reducer = None   # parallel.GradReducer: all-reduce of this encoder's gradients (data parallel)
-        self.register_load_state_dict_post_hook(lambda module, incompatible: module.invalidate_packed())
-
-    def invalidate_packed(self) -> None:
-        self._packed = None
-        self._packed_sig = None
-
-    def _apply(self, fn, *args, **kwargs):
-        out = super()._apply(fn, *args, **kwargs)
-        if hasattr(self, "_packed"):
-            self.invalidate_packed()
-        return out
-
-    def packed(self) -> Dict[str, torch.Tensor]:
-        sig = tuple((p.data_ptr(), p._version) for p in self.parameters())
-        if self._packed is None or sig != self._packed_sig:
-            with torch.no_grad():
-                self._packed = self._pack()
-            self._packed_sig = sig
-        return self._packed
-
-    def packed_transposed(self) -> Dict[str, torch.Tensor]:
-        """bf16 transposed twins of `packed()` for the dgrad GEMMs of the backward pass, rebuilt with it."""
-        P = self.packed()
-        if getattr(self, "_packed_T_of", None) is not P:
-            with torch.no_grad():
-                self._packed_T = self._pack_transposed(P)
-            self._packed_T_of = P
-        return self._packed_T
 
     def _pack_transposed_transformer(self, P, T, depth: int) -> None:
         for l in range(depth):
@@ -194,53 +150,36 @@ class _EncoderBase(nn.Module):
                               dxr_bf: torch.Tensor, grads: Dict[str, torch.Tensor]) -> None:
         """Transformer backward (ns2.py:1110-1115): dxr (fp32 gradient of the output, updated in place) becomes the
         gradient of the input; dxr_bf its bf16 copy.  Parameter gradients go to `grads` under the reference's names."""
-        B, N, D = dxr.shape
-        dev = dxr.device
+        _, N, D = dxr.shape
+
+        def norm_backward(x_in, dh, gamma, key):
+            grads[key] = dgamma = torch.zeros(D, device=dxr.device)
+            ops.rmsnorm_film_bwd(x_in, dh, dxr, dxr_bf, rows_per_batch=N, gamma=gamma, dgamma=dgamma)
+
         for l in reversed(range(len(tr.layers))):
             L = layers[l]
             pfx = f"transformer.layers.{l}."
-            ff = tr.layers[l][3]
-            Di = ff[-1].weight.shape[1]
-            Dp = P[f"l{l}_w2"].shape[1]
             # ---- feed-forward: x += W2 GEGLU(W1 RMSNorm(x) + b1) + b2 ----
-            grads[pfx + f"3.{len(ff) - 1}.weight"] = ops.wgrad(dxr_bf, L["ff_g"], torch.zeros(D, Dp, device=dev), n=D,
-                                                               k=Dp)[:, :Di]
-            grads[pfx + f"3.{len(ff) - 1}.bias"] = ops.colsum(dxr_bf, torch.zeros(D, device=dev))
-            d_g = ops.gemm(dxr_bf, T[f"l{l}_w2"], torch.empty(B, N, Dp, device=dev, dtype=torch.bfloat16), n=Dp,
-                           epilogue=ops.EPI_BF16)
-            dh2 = geglu_backward(L["h2"], d_g, P[f"l{l}_w1"], P[f"l{l}_b1"], T[f"l{l}_w1"], Di, grads, pfx + "3.0")
-            dg2 = torch.zeros(D, device=dev)
-            ops.rmsnorm_film_bwd(L["x_mid"], dh2, dxr, dxr_bf, rows_per_batch=N, gamma=P[f"l{l}_g2"], dgamma=dg2)
-            grads[pfx + "2.gamma"] = dg2
+            dh2 = ff_backward(dxr_bf, L["h2"], L["ff_g"], None, P, T, f"l{l}_", tr.layers[l][3][-1].weight.shape[1],
+                              grads, pfx + "3.")
+            norm_backward(L["x_mid"], dh2, P[f"l{l}_g2"], pfx + "2.gamma")
             # ---- attention: x += Wo attn(Wqkv RMSNorm(x)) ----
-            dg1 = torch.zeros(D, device=dev)
-            attention_backward(L, dxr, dxr_bf, T[f"l{l}_o"], T[f"l{l}_qkv"], heads, grads, pfx + "1.",
-                               gamma=P[f"l{l}_g1"], dgamma=dg1)
-            grads[pfx + "0.gamma"] = dg1
+            dh1, _ = attention_backward(dxr_bf, L["h1"], L["ao"], L["lse"], L["qkv"], None, T[f"l{l}_o"], T[f"l{l}_qkv"],
+                                        heads, grads, pfx + "1.")
+            norm_backward(L["x_in"], dh1, P[f"l{l}_g1"], pfx + "0.gamma")
 
     def _conv_silu_backward(self, x_in: torch.Tensor, w: torch.Tensor, w_t: Optional[torch.Tensor], bias: torch.Tensor,
                             d_out: torch.Tensor, first_shift: int, grads: Dict[str, torch.Tensor], name: str,
-                            d_in_f32: bool = False) -> Optional[torch.Tensor]:
+                            dtype=torch.bfloat16) -> Optional[torch.Tensor]:
         """Backward of out = silu(conv_k(x_in) + bias) (segmented GEMM): d_out bf16 (B, N, C_out) -> weight / bias
-        gradients under `name`, and d x_in ((B, N, C_in) bf16, or fp32 with d_in_f32) when the transposed pack w_t is
-        given."""
+        gradients under `name`, and d x_in ((B, N, C_in) of `dtype`) when the transposed pack w_t is given."""
         B, N, c_in = x_in.shape
         c_out = w.shape[0]
         k = w.shape[1] // c_in
-        dev = x_in.device
-        pre = ops.gemm(x_in, w, torch.empty(B, N, c_out, device=dev, dtype=torch.bfloat16), n=c_out,
+        pre = ops.gemm(x_in, w, torch.empty(B, N, c_out, device=x_in.device, dtype=torch.bfloat16), n=c_out,
                        epilogue=ops.EPI_BF16, segs=_conv_segs(c_in, k, first_shift), bias=bias)   # recompute
         ops.silu_bwd(pre, d_out)                                                                  # pre <- d pre
-        dW = torch.zeros(c_out, k * c_in, device=dev)
-        for t in range(k):   # tap t multiplies x[n - (first_shift - t)]
-            ops.wgrad(pre, x_in, dW[:, t * c_in:(t + 1) * c_in], n=c_out, k=c_in, shift_units=first_shift - t)
-        grads[name + ".weight"] = dW.view(c_out, k, c_in).permute(0, 2, 1)
-        grads[name + ".bias"] = ops.colsum(pre, torch.zeros(c_out, device=dev))
-        if w_t is None:
-            return None
-        out = torch.empty(B, N, c_in, device=dev, dtype=torch.float32 if d_in_f32 else torch.bfloat16)
-        return ops.gemm(pre, w_t, out, n=c_in, epilogue=ops.EPI_F32 if d_in_f32 else ops.EPI_BF16,
-                        segs=_conv_dgrad_segs(c_out, k, first_shift))
+        return conv_backward(pre, x_in, grads, name, w_t, k, first_shift, dtype=dtype)
 
     def _start_backward(self, d_out: torch.Tensor):
         dxr = d_out.float().contiguous().clone()        # fp32 residual-stream gradient, updated in place
@@ -276,7 +215,6 @@ class SpeechPromptEncoder(_EncoderBase):
         mods.append(_NoParam())                              # Rearrange back
         self.conv = nn.Sequential(*mods)
         self.transformer = _PlainTransformerParams(dims[-1], depth, dim_head, heads)
-        self._init_cache()
 
     def _convs(self):
         return [m for m in self.conv if isinstance(m, nn.Conv1d)]
@@ -358,7 +296,6 @@ class PhonemeEncoder(_EncoderBase):
         self.pad_id = num_tokens
         self.conv = nn.Sequential(_NoParam(), nn.Conv1d(dim, dim_hidden, kernel_size), _NoParam(), _NoParam(), _NoParam())
         self.transformer = _PlainTransformerParams(dim_hidden, depth, dim_head, heads)
-        self._init_cache()
 
     def _pack(self) -> Dict[str, torch.Tensor]:
         c = self.conv[1]
@@ -406,7 +343,7 @@ class PhonemeEncoder(_EncoderBase):
         dxr, dxr_bf = self._start_backward(d_out)
         self._transformer_backward(S["layers"], self.transformer, P, T, self.heads, dxr, dxr_bf, grads)
         d_e = self._conv_silu_backward(S["emb"], P["c_w"], T["c_w"], P["c_b"], dxr_bf, self.kernel_size - 1, grads,
-                                       "conv.1", d_in_f32=True)
+                                       "conv.1", dtype=torch.float32)
         grads["token_emb.weight"] = ops.embedding_bwd(S["ids"], d_e, torch.zeros_like(P["emb"]), self.pad_id)
         return grads
 
@@ -479,7 +416,6 @@ class DurationPitchPredictor(_EncoderBase):
                                   num_convs_per_resnet_block, num_convolutions_per_block)
         self.to_pitch_pred = mk()
         self.to_duration_pred = mk()
-        self._init_cache()
 
     def _pack(self) -> Dict[str, torch.Tensor]:
         P: Dict[str, torch.Tensor] = {}

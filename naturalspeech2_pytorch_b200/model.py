@@ -62,6 +62,65 @@ def _pack_geglu(lin1: nn.Linear, lin2: nn.Linear) -> Dict[str, torch.Tensor]:
     return {"w1": _bf(w1), "b1": b1.float().contiguous(), "w2": _bf(w2), "b2": lin2.bias.detach().float().contiguous()}
 
 
+def _pack_conv(w: torch.Tensor, i_pad: Optional[int] = None, o_pad: Optional[int] = None) -> torch.Tensor:
+    """Conv1d weight (O, I, k) -> bf16 (o_pad, k*i_pad), tap t at columns [t*i_pad, t*i_pad + I); zero padded."""
+    O, I, k = w.shape
+    i_pad, o_pad = i_pad or I, o_pad or O
+    out = w.new_zeros(o_pad, k, i_pad)
+    out[:O, :, :I] = w.detach().permute(0, 2, 1)
+    return _bf(out.view(o_pad, k * i_pad))
+
+
+def _transpose_conv(w: torch.Tensor, kernel: int) -> torch.Tensor:
+    """`_pack_conv` layout (O, k*I) -> (I, k*O) [in][tap][out] pack for the dgrad GEMM."""
+    O = w.shape[0]
+    return w.view(O, kernel, -1).permute(2, 1, 0).reshape(-1, kernel * O).contiguous()
+
+
+def _records_graph(m: nn.Module) -> bool:
+    """Whether a call of `m` records its hand-written autograd node: train mode, gradients on, a trainable parameter."""
+    return m.training and torch.is_grad_enabled() and any(p.requires_grad for p in m.parameters())
+
+
+class _PackedCache(nn.Module):
+    """Packed bf16 weights of a parameter-holding module: `_pack()` builds the forward packs and `_pack_transposed(P)`
+    their transposed twins for the dgrad GEMMs of the backward pass.  Both are rebuilt when a parameter changes."""
+
+    def __init__(self):
+        super().__init__()
+        self._packed: Optional[Dict[str, torch.Tensor]] = None
+        self._packed_sig = None
+        self._packed_T: Optional[Dict[str, torch.Tensor]] = None
+        self.register_load_state_dict_post_hook(lambda module, incompatible: module.invalidate_packed())
+
+    def invalidate_packed(self) -> None:
+        """Drop the packed weights.  Called automatically by `load_state_dict`, `.to()` / `.cuda()` / `.float()` and
+        whenever a parameter's version counter moves (optimizer steps, in-place ops).  Updates made THROUGH `.data`
+        (e.g. the `p.data.lerp_()` of ema_pytorch) do not bump the version counter: call this after them."""
+        self._packed = self._packed_sig = self._packed_T = None
+
+    def _apply(self, fn, *args, **kwargs):
+        out = super()._apply(fn, *args, **kwargs)
+        self.invalidate_packed()
+        return out
+
+    def packed(self) -> Dict[str, torch.Tensor]:
+        sig = tuple((p.data_ptr(), p._version) for p in self.parameters())
+        if self._packed is None or sig != self._packed_sig:
+            with torch.no_grad():
+                self._packed = self._pack()
+            self._packed_sig, self._packed_T = sig, None
+        return self._packed
+
+    def packed_transposed(self) -> Dict[str, torch.Tensor]:
+        """Transposed bf16 packs for the dgrad GEMMs of the backward pass (training.py), rebuilt with `packed()`."""
+        P = self.packed()
+        if self._packed_T is None:
+            with torch.no_grad():
+                self._packed_T = self._pack_transposed(P)
+        return self._packed_T
+
+
 class _NoParam(nn.Module):
     """Placeholder keeping Sequential indices aligned with the reference (Reduce / Rearrange / GEGLU / SiLU)."""
 
@@ -177,7 +236,7 @@ def _prob_mask_like(shape, prob, device):
     return torch.zeros(shape, device=device).float().uniform_(0, 1) < prob
 
 
-class Model(nn.Module):
+class Model(_PackedCache):
     """H100 denoiser; constructor and call signatures of ns2.py:811-937."""
 
     def __init__(self, dim, *, depth, dim_head=64, heads=8, ff_mult=4, wavenet_layers=8,
@@ -231,15 +290,12 @@ class Model(nn.Module):
         self.wavenet = _WavenetParams(dim, wavenet_stacks, wavenet_layers, dim_cond_mult)
         self.transformer = _TransformerParams(dim, depth, dim_head, heads, ff_mult, dim_cond_mult,
                                               cross_attn=condition_on_prompt)
-        self._packed: Optional[Dict[str, torch.Tensor]] = None
-        self._packed_sig = None
         self._ws: "OrderedDict[tuple, Dict[str, torch.Tensor]]" = OrderedDict()
         self.freeze_packed = False  # set True to skip the per-call parameter-version check (inference loops)
         self._prof = None           # bench.py: list collecting (op name, start event, end event)
         self.use_cuda_graphs = False  # replay one captured CUDA graph per problem shape instead of ~110 launches
         self._graphs: "OrderedDict[tuple, dict]" = OrderedDict()
         self.max_cached_shapes = 4  # LRU bound on per-(B, N) workspaces (~1.3 GB each at cfg2) and captured graphs
-        self.register_load_state_dict_post_hook(lambda module, incompatible: module.invalidate_packed())
 
     @property
     def device(self):
@@ -248,45 +304,21 @@ class Model(nn.Module):
     # ----------------------------------------------------------------------------------------------
     # weight packing: fp32 parameters -> bf16 tensor-core layouts (rebuilt whenever a parameter changes)
     # ----------------------------------------------------------------------------------------------
-    def _signature(self):
-        return tuple((p.data_ptr(), p._version) for p in self.parameters())
-
     def invalidate_packed(self) -> None:
-        """Drop the packed bf16 weights and every captured CUDA graph (they hold pointers into the packed copies).
-        Called automatically by `load_state_dict`, `.to()` / `.cuda()` / `.float()` and whenever a parameter's
-        version counter moves (optimizer steps, in-place ops).  Updates made THROUGH `.data` (e.g. the
-        `p.data.lerp_()` of ema_pytorch) do not bump the version counter: call this after them."""
-        self._packed = None
-        self._packed_sig = None
+        """`_PackedCache.invalidate_packed`, which here also drops every captured CUDA graph (they hold pointers into
+        the packed copies)."""
+        super().invalidate_packed()
         self._graphs.clear()
 
     def _apply(self, fn, *args, **kwargs):
         out = super()._apply(fn, *args, **kwargs)
-        if hasattr(self, "_graphs"):
-            self.invalidate_packed()
-            self._ws.clear()
+        self._ws.clear()
         return out
 
     def packed(self) -> Dict[str, torch.Tensor]:
         if self._packed is not None and self.freeze_packed:
             return self._packed
-        sig = self._signature()
-        if self._packed is None or sig != self._packed_sig:
-            with torch.no_grad():
-                self._packed = self._pack()
-            self._packed_sig = sig
-        return self._packed
-
-    @staticmethod
-    def _conv3_pack(w, k_pad=None, o_pad=None):
-        """(O, I, 3) -> (O_pad, 3*I_pad) with tap t at columns [t*I_pad, t*I_pad + I); zero padded."""
-        O, I, _ = w.shape
-        k_pad = k_pad or I
-        o_pad = o_pad or O
-        out = w.new_zeros(o_pad, 3 * k_pad)
-        for t in range(3):
-            out[:O, t * k_pad:t * k_pad + I] = w[:, :, t]
-        return out
+        return super().packed()
 
     def _pack(self) -> Dict[str, torch.Tensor]:
         D, G = self.dim, self.wavenet_layers
@@ -308,12 +340,12 @@ class Model(nn.Module):
         P["film_b"] = torch.cat(film_b, dim=0).detach().float().contiguous()
         # ---- wavenet ----
         wn = self.wavenet
-        P["wn_init_w"] = _bf(self._conv3_pack(wn.init_conv.weight))
+        P["wn_init_w"] = _pack_conv(wn.init_conv.weight)
         P["wn_init_b"] = wn.init_conv.bias.detach().float().contiguous()
         for s, st in enumerate(wn.stacks):
             ws, bc, br = [], [], []
             for blk in st.blocks:
-                ws.append(torch.cat((self._conv3_pack(blk.conv.weight), blk.res_conv.weight[:, :, 0]), dim=1))
+                ws.append(torch.cat((_pack_conv(blk.conv.weight), _bf(blk.res_conv.weight[:, :, 0])), dim=1))
                 bc.append(blk.conv.bias)
                 br.append(blk.res_conv.bias)
             P[f"wn{s}_w"] = _bf(torch.cat(ws, dim=0))                      # (G*D, 4*D)
@@ -337,7 +369,7 @@ class Model(nn.Module):
             for k, v in _pack_geglu(ff[0], ff[-1]).items():
                 P[f"l{l}_ff_{k}"] = v
             conv, Dp = ff[2][1], P[f"l{l}_ff_w2"].shape[1]
-            P[f"l{l}_ff_wc"] = _bf(self._conv3_pack(conv.weight, k_pad=Dp, o_pad=Dp))
+            P[f"l{l}_ff_wc"] = _pack_conv(conv.weight, Dp, Dp)
             P[f"l{l}_ff_bc"] = torch.zeros(Dp, device=conv.bias.device)
             P[f"l{l}_ff_bc"][:self.ff_inner] = conv.bias
         if kv_all:
@@ -359,6 +391,37 @@ class Model(nn.Module):
             P["cond_w"] = _bf(self.cond_to_model_dim.weight[:, :, 0])
             P["cond_b"] = self.cond_to_model_dim.bias.detach().float().contiguous()
         return P
+
+    def _pack_transposed(self, P: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        D, G = self.dim, self.wavenet_layers
+        T: Dict[str, torch.Tensor] = {}
+        t = lambda w: w.t().contiguous()  # noqa: E731
+        T["film_w"] = t(P["film_w"])                                        # (dim_cond, rows)
+        for s in range(self.wavenet_stacks):
+            w = P[f"wn{s}_w"].view(G, D, 4, D)                              # [group][out][tap0,tap1,tap2,res][in]
+            T[f"wn{s}_w"] = w.permute(0, 3, 2, 1).reshape(G * D, 4 * D).contiguous()   # [group][in][tap][out]
+        T["wn_skip_w"] = t(P["wn_skip_w"])                                  # (G*D, D)
+        T["wn_final_w"] = t(P["wn_final_w"])
+        for l in range(self.depth):
+            T[f"l{l}_qkv"] = t(P[f"l{l}_qkv"])                              # (D, 3*inner)
+            T[f"l{l}_o"] = t(P[f"l{l}_o"])                                  # (inner, D)
+            T[f"l{l}_ff_w1"] = t(P[f"l{l}_ff_w1"])                          # (D, 2*Dp)
+            T[f"l{l}_ff_wc"] = _transpose_conv(P[f"l{l}_ff_wc"], 3)         # (Dp, 3*Dp)
+            T[f"l{l}_ff_w2"] = t(P[f"l{l}_ff_w2"])                          # (Dp, D)
+        T["pred_w"] = t(P["pred_w"])
+        T["wn_init_w"] = _transpose_conv(P["wn_init_w"], 3)
+        if self.condition_on_prompt:
+            T["cond_w"] = t(P["cond_w"])                                   # (dim_prompt, D): d cond
+            if "pr_proj_w" in P:
+                T["pr_proj_w"] = t(P["pr_proj_w"])                         # (dim_prompt, D): d prompt
+            T["x_kv_all"] = t(P["x_kv_all"])                               # (D, depth*2*inner)
+            for l in range(self.depth):
+                T[f"l{l}_xq"] = t(P[f"l{l}_xq"])
+                T[f"l{l}_xo"] = t(P[f"l{l}_xo"])
+            for i in range(len(self.perceiver_resampler.layers)):
+                for k in ("q", "kv", "o", "ff_w1", "ff_w2"):
+                    T[f"pr{i}_{k}"] = t(P[f"pr{i}_{k}"])
+        return T
 
     # ----------------------------------------------------------------------------------------------
     # workspaces (stable addresses per problem shape so a forward can be captured in a CUDA graph)
@@ -481,16 +544,6 @@ class Model(nn.Module):
         null_logits = self.forward(*args, cond_drop_prob=1., **kwargs)
         return ops.cfg_combine(logits, null_logits, cond_scale, logits)   # in place into the (fresh) first output
 
-    def packed_transposed(self) -> Dict[str, torch.Tensor]:
-        """Transposed bf16 packs for the dgrad GEMMs of the backward pass (training.py), cached with `packed()`."""
-        P = self.packed()
-        if getattr(self, "_packed_T_of", None) is not P:
-            from .training import pack_transposed
-            with torch.no_grad():
-                self._packed_T = pack_transposed(self)
-            self._packed_T_of = P
-        return self._packed_T
-
     def forward(self, x, times, prompt=None, prompt_mask=None, cond=None, cond_drop_prob=None, *,
                 out: Optional[torch.Tensor] = None, _conditioning: Optional[dict] = None):
         """x (B, N, dim) fp32, times (B,) in [0, 1] -> (B, N, dim) fp32   (ns2.py:929-1000).
@@ -503,7 +556,7 @@ class Model(nn.Module):
         With `use_cuda_graphs` the whole step (every kernel launch below) is captured once per
         (B, N, drop-prob, conditioning shapes) and replayed; eligible when no RNG draw and no per-call host work is
         involved, i.e. unconditional models or cached conditioning with cond_drop_prob in {0, 1}."""
-        if self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+        if _records_graph(self):
             # training: one autograd node whose backward runs the hand-written kernels (training.py)
             from .training import DenoiserFunction
             if prompt_mask is not None or out is not None or _conditioning is not None:

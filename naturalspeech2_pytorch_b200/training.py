@@ -10,8 +10,9 @@ fresh tensors.  Its backward walks the network in reverse and launches, per laye
   * the element-wise backward kernels of csrc/backward.cu (RMSNorm+FiLM, GEGLU, Wavenet gate, bias column sums).
 Pre-activations that the fused forward epilogues never materialise (GEGLU's value/gate pair, the Wavenet conv output
 before FiLM) are recomputed with plain-epilogue GEMMs instead of being stored.  Gradients come out in the packed bf16
-layouts' fp32 twins and are scattered back to the reference's parameter shapes (same keys as the state_dict).
-`geglu_backward` and `attention_backward` are shared with the encoders' backward (encoders.py).
+layouts' fp32 twins, under the state_dict's keys; `param_grads` gives them the parameters' shapes.
+Each building block has one implementation, shared by the denoiser, the perceiver and the encoders (encoders.py):
+`linear_backward`, `conv_backward`, `ff_backward` (with `geglu_backward`) and `attention_backward`.
 
 Scope: unconditional and conditional denoisers (BASELINE configs[1], configs[2]/[4]): perceiver resampler, cross
 attention, prompt FiLM vector, aligned-condition projection and the classifier-free-guidance null parameters included.
@@ -27,55 +28,68 @@ view); otherwise nothing extra runs.  `x` and `times` stay non-differentiable (l
 from __future__ import annotations
 
 import math
-from typing import Dict
+from typing import Dict, Optional
 
 import torch
 import torch.nn.functional as F
 
 from . import ops
-from .model import _round_up
 
 bf = torch.bfloat16
 
 
-def _transpose_conv(w: torch.Tensor, kernel: int) -> torch.Tensor:
-    """(O, k*I) tap-major conv pack -> (I, k*O) [in][tap][out] pack for the dgrad GEMM."""
-    O = w.shape[0]
-    return w.view(O, kernel, -1).permute(2, 1, 0).reshape(-1, kernel * O).contiguous()
+def _wgrad(dy: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
+    """dW = dy^T x (fp32, (dy cols, x cols)) of a projection y = x W^T."""
+    n, k = dy.shape[-1], x.shape[-1]
+    return ops.wgrad(dy, x, torch.zeros(n, k, device=dy.device), n=n, k=k)
 
 
-def pack_transposed(model) -> Dict[str, torch.Tensor]:
-    """bf16 transposed twins of `Model.packed()` for the dgrad GEMMs (rebuilt whenever the forward packs are)."""
-    P = model.packed()
-    D, G = model.dim, model.wavenet_layers
-    T: Dict[str, torch.Tensor] = {}
-    t = lambda w: w.t().contiguous()
-    T["film_w"] = t(P["film_w"])                                        # (dim_cond, rows)
-    for s in range(model.wavenet_stacks):
-        w = P[f"wn{s}_w"].view(G, D, 4, D)                              # [group][out][tap0,tap1,tap2,res][in]
-        T[f"wn{s}_w"] = w.permute(0, 3, 2, 1).reshape(G * D, 4 * D).contiguous()   # [group][in][tap][out]
-    T["wn_skip_w"] = t(P["wn_skip_w"])                                  # (G*D, D)
-    T["wn_final_w"] = t(P["wn_final_w"])
-    for l in range(model.depth):
-        T[f"l{l}_qkv"] = t(P[f"l{l}_qkv"])                              # (D, 3*inner)
-        T[f"l{l}_o"] = t(P[f"l{l}_o"])                                  # (inner, D)
-        T[f"l{l}_ff_w1"] = t(P[f"l{l}_ff_w1"])                          # (D, 2*Dp)
-        T[f"l{l}_ff_wc"] = _transpose_conv(P[f"l{l}_ff_wc"], 3)         # (Dp, 3*Dp)
-        T[f"l{l}_ff_w2"] = t(P[f"l{l}_ff_w2"])                          # (Dp, D)
-    T["pred_w"] = t(P["pred_w"])
-    T["wn_init_w"] = _transpose_conv(P["wn_init_w"], 3)
-    if model.condition_on_prompt:
-        T["cond_w"] = t(P["cond_w"])                                   # (dim_prompt, D): d cond
-        if "pr_proj_w" in P:
-            T["pr_proj_w"] = t(P["pr_proj_w"])                         # (dim_prompt, D): d prompt
-        T["x_kv_all"] = t(P["x_kv_all"])                               # (D, depth*2*inner)
-        for l in range(model.depth):
-            T[f"l{l}_xq"] = t(P[f"l{l}_xq"])
-            T[f"l{l}_xo"] = t(P[f"l{l}_xo"])
-        for i in range(len(model.perceiver_resampler.layers)):
-            for k in ("q", "kv", "o", "ff_w1", "ff_w2"):
-                T[f"pr{i}_{k}"] = t(P[f"pr{i}_{k}"])
-    return T
+def _colsum(dy: torch.Tensor) -> torch.Tensor:
+    """Bias gradient: dy summed over every row (fp32)."""
+    return ops.colsum(dy, torch.zeros(dy.shape[-1], device=dy.device))
+
+
+def _dgrad(dy: torch.Tensor, w_t: torch.Tensor, dtype=bf, out=None, **gemm_args) -> torch.Tensor:
+    """d x = dy W on the transposed pack w_t (x cols, dy cols), into `out` or a fresh tensor of `dtype`."""
+    if out is None:
+        out = torch.empty(*dy.shape[:2], w_t.shape[0], device=dy.device, dtype=dtype)
+    return ops.gemm(dy, w_t, out, n=w_t.shape[0], epilogue=ops.EPI_F32 if out.dtype == torch.float32 else ops.EPI_BF16,
+                    **gemm_args)
+
+
+def linear_backward(dy, x, grads: Dict[str, torch.Tensor], name: str, w_t=None, bias: bool = True,
+                    width: Optional[int] = None, dtype=bf) -> Optional[torch.Tensor]:
+    """Backward of y = x W^T (+ b): grads[name + ".weight"] (its first `width` input columns when the pack is
+    zero-padded beyond the layer's width) and grads[name + ".bias"]; returns d x (of `dtype`) when the transposed pack
+    w_t is given."""
+    dw = _wgrad(dy, x)
+    grads[name + ".weight"] = dw if width is None else dw[:, :width]
+    if bias:
+        grads[name + ".bias"] = _colsum(dy)
+    return None if w_t is None else _dgrad(dy, w_t, dtype)
+
+
+def conv_wgrad(dy, x, dw, n: int, c_in: int, kernel: int, first_shift: int, **wgrad_args) -> torch.Tensor:
+    """dw[:, t*c_in:(t+1)*c_in] += the weight gradient of tap t of an `ops.conv_segs` convolution (tap t reads
+    x[n - (first_shift - t) * dilation]); returns those columns as the reference's (O, I, k) view.  `wgrad_args`: the
+    groups / strides / dilations of a grouped convolution."""
+    for t in range(kernel):
+        ops.wgrad(dy, x, dw[:, t * c_in:(t + 1) * c_in], n=n, k=c_in, shift_units=first_shift - t, **wgrad_args)
+    return dw[:, :kernel * c_in].view(dw.shape[0], kernel, c_in).permute(0, 2, 1)
+
+
+def conv_backward(dy, x, grads: Dict[str, torch.Tensor], name: str, w_t, kernel: int, first_shift: int,
+                  width: Optional[int] = None, dtype=bf) -> Optional[torch.Tensor]:
+    """Backward of y = conv(x) + b (stride 1, packed by `model._pack_conv`, tap t reads x[n - (first_shift - t)]):
+    grads[name + ".weight" / ".bias"] in the reference's layout (the first `width` channels when the pack is zero-padded
+    beyond the layer's width); returns d x (of `dtype`, mirrored shifts on the transposed pack) when w_t is given."""
+    c_out, c_in = dy.shape[-1], x.shape[-1]
+    dw = conv_wgrad(dy, x, torch.zeros(c_out, kernel * c_in, device=dy.device), c_out, c_in, kernel, first_shift)
+    db = _colsum(dy)
+    grads[name + ".weight"], grads[name + ".bias"] = (dw, db) if width is None else (dw[:width, :width], db[:width])
+    if w_t is None:
+        return None
+    return _dgrad(dy, w_t, dtype, segs=ops.conv_dgrad_segs(c_out, kernel, first_shift))
 
 
 def geglu_backward(h, d_g, w1, b1, w1_t, Di: int, grads: Dict[str, torch.Tensor], name: str) -> torch.Tensor:
@@ -84,37 +98,57 @@ def geglu_backward(h, d_g, w1, b1, w1_t, Di: int, grads: Dict[str, torch.Tensor]
     the reference's layout (value rows, then gate rows), and d h (bf16) is returned."""
     B, N, D = h.shape
     Dp = w1.shape[0] // 2
-    dev = h.device
-    pre = ops.gemm(h, w1, torch.empty(B, N, 2 * Dp, device=dev, dtype=bf), n=2 * Dp, epilogue=ops.EPI_BF16, bias=b1)
+    pre = ops.gemm(h, w1, torch.empty(B, N, 2 * Dp, device=h.device, dtype=bf), n=2 * Dp, epilogue=ops.EPI_BF16, bias=b1)
     ops.geglu_bwd(pre, d_g)                                                              # pre <- d pre
-    dW1 = ops.wgrad(pre, h, torch.zeros(2 * Dp, D, device=dev), n=2 * Dp, k=D).view(Dp // 128, 2, 128, D)
-    db1 = ops.colsum(pre, torch.zeros(2 * Dp, device=dev)).view(Dp // 128, 2, 128)
+    dW1 = _wgrad(pre, h).view(Dp // 128, 2, 128, D)
+    db1 = _colsum(pre).view(Dp // 128, 2, 128)
     grads[name + ".weight"] = torch.cat((dW1[:, 0].reshape(Dp, D)[:Di], dW1[:, 1].reshape(Dp, D)[:Di]), dim=0)
     grads[name + ".bias"] = torch.cat((db1[:, 0].reshape(Dp)[:Di], db1[:, 1].reshape(Dp)[:Di]), dim=0)
-    return ops.gemm(pre, w1_t, torch.empty(B, N, D, device=dev, dtype=bf), n=D, epilogue=ops.EPI_BF16)
+    return _dgrad(pre, w1_t)
 
 
-def attention_backward(L: dict, dxr, dxr_bf, w_o_t, w_qkv_t, heads: int, grads: Dict[str, torch.Tensor], name: str,
-                       **norm) -> None:
-    """Backward of x += Wo attn(Wqkv h1), h1 = RMSNorm(x_in), from the layer record L (x_in, h1, qkv, lse, ao):
-    to_out / to_q / to_kv gradients go to grads[name + ...]; dxr (fp32, in place) and dxr_bf become the gradient of x_in.
-    `norm` is the RMSNorm's part of ops.rmsnorm_film_bwd: film= / dfilm= or gamma= / dgamma=."""
-    B, N, D = dxr.shape
+def ff_backward(dy, h, g, c, P, T, pk: str, Di: int, grads: Dict[str, torch.Tensor], name: str) -> torch.Tensor:
+    """Backward of FeedForward (ns2.py:1009-1025) y = W2 [causal conv](GEGLU(W1 h + b1)) + b2 from the saved GEGLU output
+    g and, when the layer has the causal k=3 conv, its output c (None without it).  Weights are P / T[pk + "w1" / "b1" /
+    "wc" / "w2"], the inner width Di padded in the packs; gradients go to grads[name + Sequential index + ...].  Returns
+    d h (bf16)."""
+    d_g = linear_backward(dy, g if c is None else c, grads, name + ("2" if c is None else "3"), T[pk + "w2"], width=Di)
+    if c is not None:
+        d_g = conv_backward(d_g, g, grads, name + "2.1", T[pk + "wc"], 3, 2, width=Di)
+    return geglu_backward(h, d_g, P[pk + "w1"], P[pk + "b1"], T[pk + "w1"], Di, grads, name + "0")
+
+
+def attention_backward(dy, x, o, lse, q, kv, w_o_t, w_q_t, heads: int, grads: Dict[str, torch.Tensor], name: str,
+                       d_kv=None, x_kv=None, w_kv_t=None):
+    """Backward of y = Wo attn(Wq x, Wkv x_kv) (Attention, ns2.py:1029-1053, bias-free) from the forward's attention
+    output o and log-sum-exp.  to_out / to_q / to_kv gradients go to grads[name + ...]; returns (d x, d x_kv), bf16.
+      * self-attention: kv is None and q is the fused (B, N, 3*inner) qkv of one GEMM on x (transposed pack w_q_t),
+        so one wgrad and one dgrad cover q, k and v;
+      * cross-attention: d kv goes to `d_kv` (a fresh buffer when None).  Given the context x_kv and its transposed pack
+        w_kv_t, to_kv's gradient and d x_kv are computed too; otherwise d x_kv is None and to_kv is the caller's."""
+    B, N = dy.shape[:2]
     inner = heads * 64
-    dev = dxr.device
-    grads[name + "to_out.weight"] = ops.wgrad(dxr_bf, L["ao"], torch.zeros(D, inner, device=dev), n=D, k=inner)
-    d_ao = ops.gemm(dxr_bf, w_o_t, torch.empty(B, N, inner, device=dev, dtype=bf), n=inner, epilogue=ops.EPI_BF16)
-    qkv = L["qkv"]
-    d_qkv = torch.empty(B, N, 3 * inner, device=dev, dtype=bf)
+    dev = dy.device
+    grads[name + "to_out.weight"] = _wgrad(dy, o)
+    d_o = _dgrad(dy, w_o_t)
+    fused = kv is None
+    if fused:
+        d_q = torch.empty(B, N, 3 * inner, device=dev, dtype=bf)
+        q, kv, d_kv = q[:, :, :inner], q[:, :, inner:], d_q[:, :, inner:]
+    elif d_kv is None:
+        d_kv = torch.empty(B, kv.shape[1], 2 * inner, device=dev, dtype=bf)
     dq = torch.zeros(B, N, inner, device=dev)
-    ops.attention_bwd(qkv[:, :, :inner], qkv[:, :, inner:2 * inner], qkv[:, :, 2 * inner:], L["ao"], d_ao, L["lse"],
-                      dq, d_qkv[:, :, inner:2 * inner], d_qkv[:, :, 2 * inner:], heads=heads)
-    d_qkv[:, :, :inner].copy_(dq)   # fp32 accumulator -> bf16 slot (layout glue)
-    dWqkv = ops.wgrad(d_qkv, L["h1"], torch.zeros(3 * inner, D, device=dev), n=3 * inner, k=D)
-    grads[name + "to_q.weight"] = dWqkv[:inner]
-    grads[name + "to_kv.weight"] = dWqkv[inner:]
-    dh1 = ops.gemm(d_qkv, w_qkv_t, torch.empty(B, N, D, device=dev, dtype=bf), n=D, epilogue=ops.EPI_BF16)
-    ops.rmsnorm_film_bwd(L["x_in"], dh1, dxr, dxr_bf, rows_per_batch=N, **norm)
+    ops.attention_bwd(q, kv[:, :, :inner], kv[:, :, inner:], o, d_o, lse, dq, d_kv[:, :, :inner], d_kv[:, :, inner:],
+                      heads=heads)
+    if fused:
+        d_q[:, :, :inner].copy_(dq)   # fp32 accumulator -> bf16 slot (layout glue)
+        dw = _wgrad(d_q, x)
+        grads[name + "to_q.weight"], grads[name + "to_kv.weight"] = dw[:inner], dw[inner:]
+    else:
+        d_q = ops.cast_bf16(dq, torch.empty(B, N, inner, device=dev, dtype=bf))
+        grads[name + "to_q.weight"] = _wgrad(d_q, x)
+    d_x_kv = None if x_kv is None else linear_backward(d_kv, x_kv, grads, name + "to_kv", w_kv_t, bias=False)
+    return _dgrad(d_q, w_q_t), d_x_kv
 
 
 def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grads=None) -> Dict[str, torch.Tensor]:
@@ -129,7 +163,6 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grad
     B, N = S["B"], S["N"]
     D, G, inner, H = model.dim, model.wavenet_layers, model.inner, model.heads
     Di = model.ff_inner
-    Dp = _round_up(Di, 128)
     dev = d_out.device
     P = model.packed()
     T = model.packed_transposed()
@@ -143,8 +176,7 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grad
 
     # ---- to_pred: Linear (no bias) after RMSNorm(gamma) ----
     dout_bf = ops.cast_bf16(d_out.float().contiguous(), e(B, N, D))
-    grads["transformer.to_pred.1.weight"] = ops.wgrad(dout_bf, S["hf"], z(D, D), n=D, k=D)
-    dhf = ops.gemm(dout_bf, T["pred_w"], e(B, N, D), n=D, epilogue=ops.EPI_BF16)
+    dhf = linear_backward(dout_bf, S["hf"], grads, "transformer.to_pred.1", T["pred_w"], bias=False)
     dxr = z(B, N, D)                       # fp32 gradient of the residual stream
     dxr_bf = e(B, N, D)
     dgam = z(D)
@@ -156,43 +188,28 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grad
     if conditional:
         M = model.num_latents_m
         d_xkv = e(B, M, model.depth * 2 * inner)
+
+    def norm_backward(x_in, dh, fo):   # RMSNorm + FiLM whose (gamma, beta) are film[:, fo:fo + 2D]
+        ops.rmsnorm_film_bwd(x_in, dh, dxr, dxr_bf, rows_per_batch=N, film=film[:, fo:fo + 2 * D],
+                             dfilm=dfilm[:, fo:fo + 2 * D])
+
     for l in reversed(range(model.depth)):
         L = S["layers"][l]
         pfx = f"transformer.layers.{l}."
         fo = model._film_tr_off + l * npl * 2 * D
-        fo3 = fo + (npl - 1) * 2 * D
         # ---- feed-forward branch: x += W2 conv(GEGLU(W1 h2)) ----
-        dW2 = ops.wgrad(dxr_bf, L["ff_c"], z(D, Dp), n=D, k=Dp)
-        grads[pfx + "5.3.weight"] = dW2[:, :Di]
-        grads[pfx + "5.3.bias"] = ops.colsum(dxr_bf, z(D))
-        d_c = ops.gemm(dxr_bf, T[f"l{l}_ff_w2"], e(B, N, Dp), n=Dp, epilogue=ops.EPI_BF16)
-        dWc = z(Dp, 3 * Dp)
-        for tap in range(3):   # tap t multiplies g[n - (2 - t)]
-            ops.wgrad(d_c, L["ff_g"], dWc[:, tap * Dp:(tap + 1) * Dp], n=Dp, k=Dp, shift_units=2 - tap)
-        grads[pfx + "5.2.1.weight"] = dWc.view(Dp, 3, Dp)[:Di, :, :Di].permute(0, 2, 1)
-        grads[pfx + "5.2.1.bias"] = ops.colsum(d_c, z(Dp))[:Di]
-        d_g = ops.gemm(d_c, T[f"l{l}_ff_wc"], e(B, N, Dp), n=Dp, epilogue=ops.EPI_BF16, segs=ops.conv_dgrad_segs(Dp, 3, 2))
-        dh2 = geglu_backward(L["h2"], d_g, P[f"l{l}_ff_w1"], P[f"l{l}_ff_b1"], T[f"l{l}_ff_w1"], Di, grads, pfx + "5.0")
-        ops.rmsnorm_film_bwd(L["x_mid"], dh2, dxr, dxr_bf, rows_per_batch=N, film=film[:, fo3:fo3 + 2 * D],
-                             dfilm=dfilm[:, fo3:fo3 + 2 * D])
-        # ---- cross-attention branch: x += Wxo attn(Wxq h_x, Wxkv c) ----
+        dh2 = ff_backward(dxr_bf, L["h2"], L["ff_g"], L["ff_c"], P, T, f"l{l}_ff_", Di, grads, pfx + "5.")
+        norm_backward(L["x_mid"], dh2, fo + (npl - 1) * 2 * D)
+        # ---- cross-attention branch: x += Wxo attn(Wxq h_x, Wxkv c); Wxkv's gradient is taken for all layers at once ----
         if conditional:
-            fo2 = fo + 2 * D
-            grads[pfx + "3.to_out.weight"] = ops.wgrad(dxr_bf, L["ao2"], z(D, inner), n=D, k=inner)
-            d_ao2 = ops.gemm(dxr_bf, T[f"l{l}_xo"], e(B, N, inner), n=inner, epilogue=ops.EPI_BF16)
-            kv = S["xkv"][:, :, l * 2 * inner:(l + 1) * 2 * inner]
-            dkv = d_xkv[:, :, l * 2 * inner:(l + 1) * 2 * inner]
-            dq2 = z(B, N, inner)
-            ops.attention_bwd(L["xq"], kv[:, :, :inner], kv[:, :, inner:], L["ao2"], d_ao2, L["lse2"], dq2,
-                              dkv[:, :, :inner], dkv[:, :, inner:], heads=H)
-            dq2_bf = ops.cast_bf16(dq2, e(B, N, inner))
-            grads[pfx + "3.to_q.weight"] = ops.wgrad(dq2_bf, L["h_x"], z(inner, D), n=inner, k=D)
-            dh_x = ops.gemm(dq2_bf, T[f"l{l}_xq"], e(B, N, D), n=D, epilogue=ops.EPI_BF16)
-            ops.rmsnorm_film_bwd(L["x_c"], dh_x, dxr, dxr_bf, rows_per_batch=N, film=film[:, fo2:fo2 + 2 * D],
-                                 dfilm=dfilm[:, fo2:fo2 + 2 * D])
+            kv = slice(l * 2 * inner, (l + 1) * 2 * inner)
+            dh_x, _ = attention_backward(dxr_bf, L["h_x"], L["ao2"], L["lse2"], L["xq"], S["xkv"][:, :, kv], T[f"l{l}_xo"],
+                                         T[f"l{l}_xq"], H, grads, pfx + "3.", d_kv=d_xkv[:, :, kv])
+            norm_backward(L["x_c"], dh_x, fo + 2 * D)
         # ---- attention branch: x += Wo attn(Wqkv h1) ----
-        attention_backward(L, dxr, dxr_bf, T[f"l{l}_o"], T[f"l{l}_qkv"], H, grads, pfx + "1.",
-                           film=film[:, fo:fo + 2 * D], dfilm=dfilm[:, fo:fo + 2 * D])
+        dh1, _ = attention_backward(dxr_bf, L["h1"], L["ao"], L["lse"], L["qkv"], None, T[f"l{l}_o"], T[f"l{l}_qkv"], H,
+                                    grads, pfx + "1.")
+        norm_backward(L["x_in"], dh1, fo)
         # FiLM projections of this layer's norms: their rows of dfilm are final now, so the weight gradient (the largest
         # gradient buffers of the model) joins this layer's all-reduce instead of trailing the whole backward
         dWl = ops.film_wgrad(dfilm[:, fo:fo + npl * 2 * D], t_cond, torch.empty(npl * 2 * D, model.dim_cond, device=dev),
@@ -202,29 +219,22 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grad
         flush()   # this layer's gradients are final: their all-reduce overlaps the layers still to come
 
     if conditional:
-        # d of the perceiver context: bf16 d(proj) when it has a projection, else fp32 d(prompt)
-        d_ctx = _conditioning_backward_tokens(model, S, T, d_xkv, grads)
+        # d prompt, term (a): through the perceiver's context projection (identity when dim_prompt == dim)
+        d_prompt = _conditioning_backward_tokens(model, S, T, d_xkv, grads, want_prompt)
         if want_prompt:
-            # d prompt, term (a): through the perceiver's context projection (identity when dim_prompt == dim)
-            if "pr_proj_w" in P:
-                input_grads["prompt"] = ops.gemm(d_ctx, T["pr_proj_w"], e(B, S["pr_Np"], model.dim_prompt, dt=torch.float32),
-                                                 n=model.dim_prompt, epilogue=ops.EPI_F32)
-            else:
-                input_grads["prompt"] = d_ctx
+            input_grads["prompt"] = d_prompt
     # ---- wavenet: final 1x1 conv, skip sum, 4 stacks of 8 dilation columns, init conv ----
-    grads["wavenet.final_conv.weight"] = ops.wgrad(dxr_bf, S["skip"], z(D, D), n=D, k=D).unsqueeze(-1)
-    grads["wavenet.final_conv.bias"] = ops.colsum(dxr_bf, z(D))
-    d_skip = ops.gemm(dxr_bf, T["wn_final_w"], e(B, N, D), n=D, epilogue=ops.EPI_BF16)
-    last = S["stack_out"][-1]
-    dWskip = ops.wgrad(d_skip, last, z(D, G * D), n=D, k=G * D)
-    dbskip = ops.colsum(d_skip, z(D))
+    # (1x1 conv gradients keep the GEMM's 2-D shape; `param_grads` gives them the parameters' shapes)
+    d_skip = linear_backward(dxr_bf, S["skip"], grads, "wavenet.final_conv", T["wn_final_w"])
+    # the skip convs are one GEMM over the concatenated stack outputs with the summed bias: split its gradient
+    dWskip, dbskip = _wgrad(d_skip, S["stack_out"][-1]), _colsum(d_skip)
     nst = model.wavenet_stacks
     for g in range(G):
-        grads[f"wavenet.stacks.{nst - 1}.blocks.{g}.skip_conv.weight"] = dWskip[:, g * D:(g + 1) * D].unsqueeze(-1)
+        grads[f"wavenet.stacks.{nst - 1}.blocks.{g}.skip_conv.weight"] = dWskip[:, g * D:(g + 1) * D]
         grads[f"wavenet.stacks.{nst - 1}.blocks.{g}.skip_conv.bias"] = dbskip
     # dcy: [dc | dy] halves, so that one grouped dgrad GEMM reads the conv taps from dc and the 1x1 res conv from dy
     dcy = e(B, N, 2 * G * D)
-    ops.gemm(d_skip, T["wn_skip_w"], dcy[:, :, G * D:], n=G * D, epilogue=ops.EPI_BF16)     # d y of the last stack
+    _dgrad(d_skip, T["wn_skip_w"], out=dcy[:, :, G * D:])     # d y of the last stack
     c_pre = e(B, N, G * D)
     for s in reversed(range(nst)):
         x_in = S["stack_out"][s - 1] if s > 0 else S["h0"]
@@ -240,18 +250,16 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grad
                              accumulate=False)   # this stack's FiLM projections (see the transformer loop)
         for g in range(G):
             grads[f"wavenet.stacks.{s}.blocks.{g}.to_time_cond.weight"] = dWs[g * 2 * D:(g + 1) * 2 * D]
+        # [conv taps | res conv] of the G blocks in one (G*D, 4*D) buffer, like the forward pack
+        grouped = dict(groups=G, dy_group_col_stride=D, x_group_col_stride=gcs, dw_group_row_stride=D)
         dWp = z(G * D, 4 * D)
-        for tap in range(3):
-            ops.wgrad(dc, x_in, dWp[:, tap * D:(tap + 1) * D], n=D, k=D, shift_units=2 - tap, groups=G,
-                      dy_group_col_stride=D, x_group_col_stride=gcs, dw_group_row_stride=D, dil=dil)
-        ops.wgrad(dy, x_in, dWp[:, 3 * D:], n=D, k=D, groups=G, dy_group_col_stride=D, x_group_col_stride=gcs,
-                  dw_group_row_stride=D)
-        dbc, dbr = ops.colsum(dc, z(G * D)), ops.colsum(dy, z(G * D))
+        dWc = conv_wgrad(dc, x_in, dWp, D, D, 3, 2, dil=dil, **grouped)
+        ops.wgrad(dy, x_in, dWp[:, 3 * D:], n=D, k=D, **grouped)
+        dbc, dbr = _colsum(dc), _colsum(dy)
         for g in range(G):
             blk = f"wavenet.stacks.{s}.blocks.{g}."
-            w = dWp[g * D:(g + 1) * D]
-            grads[blk + "conv.weight"] = w[:, :3 * D].view(D, 3, D).permute(0, 2, 1)
-            grads[blk + "res_conv.weight"] = w[:, 3 * D:].unsqueeze(-1)
+            grads[blk + "conv.weight"] = dWc[g * D:(g + 1) * D]
+            grads[blk + "res_conv.weight"] = dWp[g * D:(g + 1) * D, 3 * D:]
             grads[blk + "conv.bias"] = dbc[g * D:(g + 1) * D]
             grads[blk + "res_conv.bias"] = dbr[g * D:(g + 1) * D]
         # d(input of every column): anti-causal taps on dc + the transposed 1x1 on dy
@@ -264,35 +272,27 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grad
             dcy[:, :, G * D:].copy_(d_in)       # becomes d y of the previous stack
         else:
             d_h0 = ops.group_sum(d_in, e(B, N, D), dim=D, groups=G)   # h0 feeds all columns
-    dWi = z(D, 3 * D)
-    for tap in range(3):
-        ops.wgrad(d_h0, S["x_bf"], dWi[:, tap * D:(tap + 1) * D], n=D, k=D, shift_units=2 - tap)
-    grads["wavenet.init_conv.weight"] = dWi.view(D, 3, D).permute(0, 2, 1)
-    grads["wavenet.init_conv.bias"] = ops.colsum(d_h0, z(D))
+    # x_in = x + pad_or_curtail(where(cdrop, null_cond, cond_proj)) (ns2.py:978-992): d x_in from the init conv's dgrad
+    d_xin = conv_backward(d_h0, S["x_bf"], grads, "wavenet.init_conv", T["wn_init_w"] if conditional else None, 3, 2)
     if conditional:
-        # x_in = x + pad_or_curtail(where(cdrop, null_cond, cond_proj)) (ns2.py:978-992): d x_in from the init conv's dgrad
-        d_xin = ops.gemm(d_h0, T["wn_init_w"], e(B, N, D), n=D, epilogue=ops.EPI_BF16, segs=ops.conv_dgrad_segs(D, 3, 2))
         Lc = S["Lc"]
         n_used = min(Lc, N)
         keep = (~S["cdrop"])[:, None, None]
         d_cp = torch.zeros(B, Lc, D, device=dev, dtype=bf)
         d_cp[:, :n_used] = torch.where(keep, d_xin[:, :n_used], torch.zeros((), device=dev, dtype=bf))   # masking glue
         grads["null_cond"] = (d_xin[:, :n_used].float() * S["cdrop"][:, None, None]).sum((0, 1)).unsqueeze(-1)
-        grads["cond_to_model_dim.weight"] = ops.wgrad(d_cp, S["cond_bf"], z(D, model.dim_prompt), n=D,
-                                                      k=model.dim_prompt).unsqueeze(-1)
-        grads["cond_to_model_dim.bias"] = ops.colsum(d_cp, z(D))
+        # d cond = d_cp @ W (1x1 conv dgrad), token-major; curtailed frames (n >= N) stay exact zeros.  Returned as the
+        # channel-first view cond has, so nothing is transposed.
+        d_cond = linear_backward(d_cp, S["cond_bf"], grads, "cond_to_model_dim", T["cond_w"] if want_cond else None,
+                                 dtype=torch.float32)
         if want_cond:
-            # d cond = d_cp @ W (1x1 conv dgrad), token-major; curtailed frames (n >= N) stay exact zeros.  Returned as
-            # the channel-first view cond has, so nothing is transposed.
-            d_cond = ops.gemm(d_cp, T["cond_w"], e(B, Lc, model.dim_prompt, dt=torch.float32), n=model.dim_prompt,
-                              epilogue=ops.EPI_F32)
             input_grads["cond"] = d_cond.permute(0, 2, 1)
 
     # ---- FiLM projections (one stacked matrix) and the timestep embedding ----
     rows = film.shape[1]
     dbf = dfilm.sum(0)
     dfilm_bf = ops.cast_bf16(dfilm, e(1, B, rows))
-    dt = ops.gemm(dfilm_bf, T["film_w"], e(1, B, model.dim_cond, dt=torch.float32), n=model.dim_cond, epilogue=ops.EPI_F32)[0]
+    dt = _dgrad(dfilm_bf, T["film_w"], torch.float32)[0]
     if conditional:
         # prompt FiLM vector: where(drop, null_prompt_cond, silu(Linear(mean(prompt)))) (ns2.py:952-962); (B,)-sized glue
         d_pc = dt[:, model.dim_time:]
@@ -335,20 +335,20 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grad
     return grads
 
 
-def _conditioning_backward_tokens(model, S, T, d_xkv, grads):
+def _conditioning_backward_tokens(model, S, T, d_xkv, grads, want_prompt: bool):
     """Backward of everything that produced the cross-attention context: the stacked K/V projection of all layers,
-    the null-token substitution and the PerceiverResampler (ns2.py:532-579, 964-968)."""
+    the null-token substitution and the PerceiverResampler (ns2.py:532-579, 964-968).  Returns d prompt (fp32) when
+    `want_prompt`, without its mean-pool term."""
     P = model.packed()
     B, D, M, inner, H = S["B"], model.dim, model.num_latents_m, model.inner, model.heads
-    Di = model.ff_inner
-    Dp = _round_up(Di, 128)
     dev = d_xkv.device
     e = lambda *s, dt=bf: torch.empty(*s, device=dev, dtype=dt)
     z = lambda *s: torch.zeros(*s, device=dev, dtype=torch.float32)
-    dWkv = ops.wgrad(d_xkv, S["c_bf"], z(model.depth * 2 * inner, D), n=model.depth * 2 * inner, k=D)
+    # one GEMM holds the cross-attention K/V projections of every layer: split its weight gradient
+    dWkv = _wgrad(d_xkv, S["c_bf"])
     for l in range(model.depth):
         grads[f"transformer.layers.{l}.3.to_kv.weight"] = dWkv[l * 2 * inner:(l + 1) * 2 * inner]
-    d_c = ops.gemm(d_xkv, T["x_kv_all"], e(B, M, D), n=D, epilogue=ops.EPI_BF16).float()
+    d_c = _dgrad(d_xkv, T["x_kv_all"]).float()
     drop = S["drop"]
     grads["null_prompt_tokens"] = (d_c * drop[:, None, None]).sum(0)
     d_tok = ops.cast_bf16((d_c * (~drop)[:, None, None]).contiguous(), e(B, M, D))
@@ -360,39 +360,37 @@ def _conditioning_backward_tokens(model, S, T, d_xkv, grads):
                          dgamma=dgam)
     grads["perceiver_resampler.norm.gamma"] = dgam
     Np = S["pr_Np"]
-    ctx = M + Np
     d_proj = z(B, Np, D)
     for i in reversed(range(len(pr.layers))):
         L = S["pr_layers"][i]
         pfx = f"perceiver_resampler.layers.{i}."
         # feed-forward (no conv, no pre-norm): lat += W2 GEGLU(W1 lat)
-        grads[pfx + "1.2.weight"] = ops.wgrad(dlat_bf, L["g"], z(D, Dp), n=D, k=Dp)[:, :Di]
-        grads[pfx + "1.2.bias"] = ops.colsum(dlat_bf, z(D))
-        d_g = ops.gemm(dlat_bf, T[f"pr{i}_ff_w2"], e(B, M, Dp), n=Dp, epilogue=ops.EPI_BF16)
-        ops.accum_bf16(dlat, geglu_backward(L["lat_bf2"], d_g, P[f"pr{i}_ff_w1"], P[f"pr{i}_ff_b1"], T[f"pr{i}_ff_w1"], Di,
-                                            grads, pfx + "1.0"), dlat_bf)
+        ops.accum_bf16(dlat, ff_backward(dlat_bf, L["lat_bf2"], L["g"], None, P, T, f"pr{i}_ff_", model.ff_inner, grads,
+                                         pfx + "1."), dlat_bf)
         # attention over cat(latents, projected prompt): lat += Wo attn(Wq lat, Wkv cat)
-        grads[pfx + "0.to_out.weight"] = ops.wgrad(dlat_bf, L["o"], z(D, inner), n=D, k=inner)
-        d_o = ops.gemm(dlat_bf, T[f"pr{i}_o"], e(B, M, inner), n=inner, epilogue=ops.EPI_BF16)
-        dq = z(B, M, inner)
-        d_kv = e(B, ctx, 2 * inner)
-        ops.attention_bwd(L["q"], L["kv"][:, :, :inner], L["kv"][:, :, inner:], L["o"], d_o, L["lse"], dq, d_kv[:, :, :inner],
-                          d_kv[:, :, inner:], heads=H)
-        dq_bf = ops.cast_bf16(dq, e(B, M, inner))
-        grads[pfx + "0.to_q.weight"] = ops.wgrad(dq_bf, L["lat_bf"], z(inner, D), n=inner, k=D)
-        grads[pfx + "0.to_kv.weight"] = ops.wgrad(d_kv, L["cat"], z(2 * inner, D), n=2 * inner, k=D)
-        d_cat = ops.gemm(d_kv, T[f"pr{i}_kv"], e(B, ctx, D), n=D, epilogue=ops.EPI_BF16)
-        ops.accum_bf16(dlat, ops.gemm(dq_bf, T[f"pr{i}_q"], e(B, M, D), n=D, epilogue=ops.EPI_BF16))
+        d_lat, d_cat = attention_backward(dlat_bf, L["lat_bf"], L["o"], L["lse"], L["q"], L["kv"], T[f"pr{i}_o"],
+                                          T[f"pr{i}_q"], H, grads, pfx + "0.", x_kv=L["cat"], w_kv_t=T[f"pr{i}_kv"])
+        ops.accum_bf16(dlat, d_lat)
         ops.accum_bf16(dlat, d_cat[:, :M].contiguous(), dlat_bf)
         ops.accum_bf16(d_proj, d_cat[:, M:].contiguous())
     grads["perceiver_resampler.latents"] = dlat.sum(0)
-    if "pr_proj_w" in P:
-        d_proj_bf = ops.cast_bf16(d_proj, e(B, Np, D))
-        grads["perceiver_resampler.proj_context.weight"] = ops.wgrad(d_proj_bf, S["pr_p_bf"], z(D, model.dim_prompt), n=D,
-                                                                     k=model.dim_prompt)
-        grads["perceiver_resampler.proj_context.bias"] = ops.colsum(d_proj_bf, z(D))
-        return d_proj_bf
-    return d_proj
+    if "pr_proj_w" not in P:
+        return d_proj
+    return linear_backward(ops.cast_bf16(d_proj, e(B, Np, D)), S["pr_p_bf"], grads, "perceiver_resampler.proj_context",
+                           T["pr_proj_w"] if want_prompt else None, dtype=torch.float32)
+
+
+def param_grads(module: torch.nn.Module, grads: Dict[str, torch.Tensor], reducer=None) -> list:
+    """The gradients of `module.parameters()` from a hand-written backward's `grads` (keys of `named_parameters()`), in
+    the parameters' shapes and dtypes; raises when one is missing.  `reducer` (parallel.GradReducer) all-reduces them
+    first."""
+    missing = [n for n, _ in module.named_parameters() if n not in grads]
+    if missing:
+        raise RuntimeError(f"{type(module).__name__} backward produced no gradient for {missing[:4]}...")
+    if reducer is not None:
+        reducer.reduce_all(grads)
+        reducer.finish()
+    return [grads[n].reshape(p.shape).to(p.dtype) for n, p in module.named_parameters()]
 
 
 class DenoiserFunction(torch.autograd.Function):
@@ -403,7 +401,6 @@ class DenoiserFunction(torch.autograd.Function):
         saved = {}
         out = model._forward_impl(x, times, prompt, cond=cond, cond_drop_prob=cond_drop_prob, saved=saved)
         ctx.model, ctx.saved = model, saved
-        ctx.names = [n for n, _ in model.named_parameters()]
         ctx.in_dtypes = (prompt.dtype if prompt is not None else None, cond.dtype if cond is not None else None)
         return out
 
@@ -415,16 +412,12 @@ class DenoiserFunction(torch.autograd.Function):
             grads = train_backward(ctx.model, ctx.saved, d_out, getattr(ctx.model, "grad_reducer", None),
                                    input_grads=inputs or None)
         ctx.saved = None
-        missing = [n for n in ctx.names if n not in grads]
-        if missing:
-            raise RuntimeError(f"backward produced no gradient for {missing[:4]}...")
         d_prompt, d_cond = inputs.get("prompt"), inputs.get("cond")
         if d_prompt is not None:
             d_prompt = d_prompt.to(ctx.in_dtypes[0])
         if d_cond is not None:
             d_cond = d_cond.to(ctx.in_dtypes[1])
-        return (None, None, None, d_prompt, d_cond, None, *[grads[n].reshape(p.shape).to(p.dtype)
-                                                          for n, p in ctx.model.named_parameters()])
+        return (None, None, None, d_prompt, d_cond, None, *param_grads(ctx.model, grads))
 
 
 class MseRowsFunction(torch.autograd.Function):

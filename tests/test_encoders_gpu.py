@@ -33,7 +33,8 @@ def test_silu_conv_gemm_matches_torch():
     >128 rows: CTA pair), bf16 and fp32 outputs, against torch fp32 conv1d on the bf16-rounded operands."""
     import torch.nn.functional as F
     from naturalspeech2_pytorch_b200 import _lib, ops
-    from naturalspeech2_pytorch_b200.encoders import _conv_segs, _pack_conv
+    from naturalspeech2_pytorch_b200.encoders import _conv_segs
+    from naturalspeech2_pytorch_b200.model import _pack_conv
     g = torch.Generator().manual_seed(3)
     for rows, c_in, c_out in ((103, 128, 256), (300, 256, 512), (1024, 64, 128)):
         x = torch.randn(2, rows, c_in, generator=g).bfloat16()

@@ -292,15 +292,6 @@ __global__ void __launch_bounds__(256) mse_bwd_kernel(const float4* __restrict__
   }
 }
 
-// fp32 -> (fp32 copy, bf16 copy): seeds the residual-stream gradient from a GEMM's fp32 output
-__global__ void __launch_bounds__(256) cast_pair_kernel(const float4* __restrict__ src, long long n4, uint2* __restrict__ out_bf) {
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n4;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const float4 v = __ldg(src + i);
-    out_bf[i] = make_uint2(f2_to_bf2(v.x, v.y), f2_to_bf2(v.z, v.w));
-  }
-}
-
 // acc (fp32) += t (bf16); acc_bf = bf16(acc): joins a branch gradient into a residual-stream gradient
 __global__ void __launch_bounds__(256) accum_bf16_kernel(float4* __restrict__ acc, const uint2* __restrict__ t, long long n4,
                                                          uint2* __restrict__ acc_bf) {

@@ -169,7 +169,10 @@ class NaturalSpeech2(nn.Module):
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph, capture_error_mode="thread_local"):
             step()
-        entry = {"graph": graph, "x": x, "ts": ts, "coef": coef, "cond": static_cond, "packed": model.packed()}
+        # the entry owns every buffer the graph reads or writes: v0 / v1 are written by each replay, and a buffer freed
+        # here would go back to the caching allocator while the graph still writes the prediction into it
+        entry = {"graph": graph, "x": x, "ts": ts, "coef": coef, "v": (v0, v1), "cond": static_cond,
+                 "packed": model.packed()}
         self._sampler_graphs[key] = entry
         return entry
 
@@ -178,7 +181,9 @@ class NaturalSpeech2(nn.Module):
         """ns2.py:1379-1431.  `noise` (optional) fixes the initial latent instead of drawing it.
         (`time_difference` only shifts a value the reference never reads again, ns2.py:1404-1406.)"""
         batch, device = shape[0], self.device
-        audio = torch.randn(shape, device=device) if noise is None else noise.to(device).float().clone()
+        # a dense, row-major copy: the eager loop updates it in place with ops.ddim_step, which reads flat arrays
+        audio = torch.randn(shape, device=device) if noise is None else \
+            noise.to(device).float().clone(memory_format=torch.contiguous_format)
         conditioning = None
         if self.conditional:
             assert _exists(prompt) and _exists(cond)

@@ -42,6 +42,18 @@ def _req(t: torch.Tensor, dtype: torch.dtype, name: str) -> None:
         raise ValueError(f"{name} must be contiguous in its last dimension")
 
 
+def _req_flat(t: torch.Tensor, dtype: torch.dtype, name: str, numel: int, align: int = 16) -> None:
+    """`t` is read or written as one flat array of `numel` elements, in vectors of `align` bytes (float4 loads of fp32
+    data, 4 x bf16 stores; align=1 for per-sample scalars read one element at a time)."""
+    _req(t, dtype, name)
+    if not t.is_contiguous():
+        raise ValueError(f"{name} must be contiguous")
+    if t.numel() != numel:
+        raise ValueError(f"{name} must hold {numel} elements, got {t.numel()}")
+    if t.data_ptr() % align:
+        raise ValueError(f"{name} must be {align}-byte aligned")
+
+
 def set_sm_limit(sms: int) -> int:
     """Size every kernel's persistent grid for at most `sms` SMs (0 = all).  Returns the previous limit."""
     return int(_lib.load().ns2_set_sm_limit(int(sms)))
@@ -223,10 +235,13 @@ def rmsnorm_film(x: torch.Tensor, out: torch.Tensor, *, gamma: Optional[torch.Te
 
 
 def rmsnorm_f32(x: torch.Tensor, out: torch.Tensor, gamma: Optional[torch.Tensor]) -> torch.Tensor:
+    """out (f32, x's shape) = RMSNorm(x) (* gamma) over the last dimension; x and out contiguous."""
     lib = _lib.load()
-    _req(x, torch.float32, "x")
-    _req(out, torch.float32, "out")
     D = x.shape[-1]
+    _req_flat(x, torch.float32, "x", x.numel())
+    _req_flat(out, torch.float32, "out", x.numel())
+    if gamma is not None:
+        _req_flat(gamma, torch.float32, "gamma", D)
     rows = x.numel() // D
     check(lib.ns2_rmsnorm_f32(x.data_ptr(), D, rows, D, _ptr(gamma), out.data_ptr(), D, _stream()),
           "ns2_rmsnorm_f32")
@@ -435,10 +450,10 @@ def q_sample(x0, noise, alpha, sigma, x_t, target=None, objective: str = "v"):
     lib = _lib.load()
     B = x0.shape[0]
     per = x0.numel() // B
-    for name, t in (("x0", x0), ("noise", noise), ("alpha", alpha), ("sigma", sigma), ("x_t", x_t)):
-        _req(t, torch.float32, name)
-    if target is not None:
-        _req(target, torch.float32, "target")
+    for name, t in (("x0", x0), ("noise", noise), ("x_t", x_t)) + ((("target", target),) if target is not None else ()):
+        _req_flat(t, torch.float32, name, x0.numel())
+    for name, t in (("alpha", alpha), ("sigma", sigma)):
+        _req_flat(t, torch.float32, name, B, align=1)
     check(lib.ns2_q_sample(x0.data_ptr(), noise.data_ptr(), alpha.data_ptr(), sigma.data_ptr(), B, per,
                            x_t.data_ptr(), _ptr(target), OBJECTIVES[objective], _stream()), "ns2_q_sample")
     return x_t, target
@@ -467,6 +482,10 @@ def ddim_step(x, v, alpha, sigma, alpha_next, sigma_next, objective: str = "v"):
     lib = _lib.load()
     B = x.shape[0]
     per = x.numel() // B
+    for name, t in (("x", x), ("v", v)):
+        _req_flat(t, torch.float32, name, x.numel())
+    for name, t in (("alpha", alpha), ("sigma", sigma), ("alpha_next", alpha_next), ("sigma_next", sigma_next)):
+        _req_flat(t, torch.float32, name, B, align=1)
     check(lib.ns2_ddim_step(x.data_ptr(), v.data_ptr(), alpha.data_ptr(), sigma.data_ptr(),
                             alpha_next.data_ptr(), sigma_next.data_ptr(), B, per, OBJECTIVES[objective],
                             _stream()),
@@ -479,15 +498,20 @@ def x_start_from_pred(x, pred, alpha, sigma, out, objective: str = "v"):
     lib = _lib.load()
     B = x.shape[0]
     per = x.numel() // B
-    for name, t in (("x", x), ("pred", pred), ("alpha", alpha), ("sigma", sigma), ("out", out)):
-        _req(t, torch.float32, name)
+    for name, t in (("x", x), ("pred", pred), ("out", out)):
+        _req_flat(t, torch.float32, name, x.numel())
+    for name, t in (("alpha", alpha), ("sigma", sigma)):
+        _req_flat(t, torch.float32, name, B, align=1)
     check(lib.ns2_x_start(x.data_ptr(), pred.data_ptr(), alpha.data_ptr(), sigma.data_ptr(), B, per, out.data_ptr(),
                           OBJECTIVES[objective], _stream(out)), "ns2_x_start")
     return out
 
 
 def cfg_combine(cond, null, scale, out):
+    """out = null + (cond - null) * scale (classifier-free guidance); out may be cond or null itself."""
     lib = _lib.load()
+    for name, t in (("cond", cond), ("null", null), ("out", out)):
+        _req_flat(t, torch.float32, name, cond.numel())
     check(lib.ns2_cfg_combine(cond.data_ptr(), null.data_ptr(), float(scale), cond.numel(),
                               out.data_ptr(), _stream()), "ns2_cfg_combine")
     return out
@@ -711,13 +735,14 @@ def group_sum(t, out, *, dim: int, groups: int):
 def mse_bwd(pred, target, coef, out_bf=None, out_f32=None):
     """coef[b] * (pred - target) as bf16 and/or f32: the seed of the backward pass."""
     lib = _lib.load()
-    for name, t in (("pred", pred), ("target", target), ("coef", coef)):
-        _req(t, torch.float32, name)
-    if out_bf is not None:
-        _req(out_bf, torch.bfloat16, "out_bf")
-    if out_f32 is not None:
-        _req(out_f32, torch.float32, "out_f32")
     B = pred.shape[0]
+    for name, t in (("pred", pred), ("target", target)):
+        _req_flat(t, torch.float32, name, pred.numel())
+    _req_flat(coef, torch.float32, "coef", B, align=1)
+    if out_bf is not None:
+        _req_flat(out_bf, torch.bfloat16, "out_bf", pred.numel(), align=8)
+    if out_f32 is not None:
+        _req_flat(out_f32, torch.float32, "out_f32", pred.numel())
     check(lib.ns2_mse_bwd(pred.data_ptr(), target.data_ptr(), coef.data_ptr(), B, pred.numel() // B, _ptr(out_bf),
                           _ptr(out_f32), _stream(pred)), "ns2_mse_bwd")
     return out_bf if out_bf is not None else out_f32

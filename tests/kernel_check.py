@@ -11,6 +11,7 @@ be widened until it passes everything.
 from __future__ import annotations
 
 import math
+from contextlib import contextmanager
 
 import torch
 
@@ -78,3 +79,26 @@ def shifted(x: torch.Tensor, s: int) -> torch.Tensor:
     elif -N < s < 0:
         y[:, :N + s] = x[:, -s:]
     return y
+
+
+def gen(seed: int, device: str = "cuda") -> torch.Generator:
+    return torch.Generator(device=device).manual_seed(seed)
+
+
+def nan_buf(shape, dtype=torch.float32, pad: int = 40, device: str = "cuda"):
+    """(buffer, contiguous window): the window is the buffer's first prod(shape) elements, the rest stays NaN."""
+    n = math.prod(shape)
+    buf = torch.full((n + pad,), float("nan"), device=device, dtype=dtype)
+    return buf, buf[:n].view(shape)
+
+
+@contextmanager
+def sm_limit(sms: int):
+    """Every kernel's persistent grid sized for at most `sms` SMs (0 = all) inside the block; yields the previous
+    limit and restores it on exit."""
+    from naturalspeech2_pytorch_b200 import ops
+    prev = ops.set_sm_limit(sms)
+    try:
+        yield prev
+    finally:
+        ops.set_sm_limit(prev)

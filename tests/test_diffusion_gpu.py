@@ -88,7 +88,10 @@ def test_conditional_requires_conditioning():
 
 def test_sampler_graph_matches_eager_loop():
     """The captured sampling step (forward(s) + guidance + DDIM update in one CUDA graph, schedule tables) gives the
-    same latents as the eager per-step loop, for unconditional and guided conditional sampling."""
+    same latents as the eager per-step loop, for unconditional and guided conditional sampling, whatever the order of
+    eager and graph calls on one model, and for the same noise passed as a transposed (B, D, N)-ordered view.  The graph
+    writes only into buffers its sampler owns: memory handed out by the caching allocator after the capture (the
+    sentinels) is never written by a later replay."""
     from naturalspeech2_pytorch_b200 import NaturalSpeech2
     for name, kw in (("uncond_small", {}), ("cond_small", dict(cond_scale=2.0))):
         z, kwargs, seed = load_model_golden(name)
@@ -97,11 +100,19 @@ def test_sampler_graph_matches_eager_loop():
         if kwargs.get("condition_on_prompt"):
             extra = dict(prompt_enc=torch.from_numpy(z["in_prompt"]).cuda(), cond=torch.from_numpy(z["in_cond"]).cuda())
         noise = torch.randn(2, 160, 128, generator=torch.Generator().manual_seed(5))
-        outs = []
-        for graphs in (False, True):
-            ns = NaturalSpeech2(model, target_sample_hz=24000, timesteps=3, cuda_graphs=graphs)
-            outs.append(ns.sample(length=160, batch_size=2, noise=noise, **extra, **kw))
-        assert torch.equal(outs[0], outs[1]), name
+        noise_t = noise.transpose(1, 2).contiguous().transpose(1, 2)
+        eager = NaturalSpeech2(model, target_sample_hz=24000, timesteps=3, cuda_graphs=False)
+        ns = NaturalSpeech2(model, target_sample_hz=24000, timesteps=3, cuda_graphs=True)
+        run = lambda sampler, nz: sampler.sample(length=160, batch_size=2, noise=nz, **extra, **kw)  # noqa: E731
+        ref = run(eager, noise)
+        assert torch.equal(run(eager, noise_t), ref), (name, "eager, transposed noise")
+        assert torch.equal(run(ns, noise), ref), (name, "graph captured after two eager samples")
+        sentinels = [torch.full((2, 160, 128), 7.0, device="cuda") for _ in range(8)]
+        assert torch.equal(run(ns, noise_t), ref), (name, "graph, transposed noise")
+        assert torch.equal(run(eager, noise), ref), (name, "eager after graph")
+        assert torch.equal(run(ns, noise), ref), (name, "graph after eager")
+        torch.cuda.synchronize()
+        assert all(bool((t == 7.0).all()) for t in sentinels), (name, "a replay wrote into memory it does not own")
         # a second call with other noise reuses the captured graph
         ns.sample(length=160, batch_size=2, **extra, **kw)
         assert len(ns._sampler_graphs) == 1
@@ -121,3 +132,4 @@ def test_loss_with_rvq_cross_entropy_term():
     with_ce = NaturalSpeech2(model, codec, timesteps=4, rvq_cross_entropy_loss_weight=0.5)(
         latents, codes=codes, times=times, noise=noise)
     assert torch.isfinite(with_ce) and float(with_ce) > float(base)
+

@@ -4,7 +4,9 @@ Same restatement of `Model.forward` (ns2.py:929-1000) as `denoiser_oracle.py`, e
 the reference itself calls (F.linear, F.conv1d, F.scaled_dot_product_attention, F.gelu ...), so that it runs on
 all host cores through MKL/oneDNN exactly like the reference's own CPU path.  It exists for `bench.py`'s
 `cpu_baseline` / `--impl reference` legs (the numpy oracle is the parity checker; numpy's BLAS use leaves most cores
-idle and would understate the reference).  `tests/test_oracle_cpu.py` pins it to the same goldens.
+idle and would understate the reference).  `tests/test_oracle_cpu.py` pins it to the same goldens, its autograd
+(`model_forward_autograd` in float64) to the reference's fp64 gradients; run on the GPU in float64 it is the reference
+of the hand-written backward at the benchmarked dims (tests/test_denoiser_backward_fp64_gpu.py).
 Only tests/ and bench.py's CPU legs may import this module.
 """
 from __future__ import annotations
@@ -63,8 +65,9 @@ def feedforward(P, prefix, x, causal_conv):
     return F.linear(h, P[prefix + last + "weight"], P[prefix + last + "bias"])
 
 
-def wavenet(P, cfg, x, t):
-    """Wavenet / WavenetStack / WavenetResBlock, ns2.py:597-725."""
+def wavenet(P, cfg, x, t, dilations=None):
+    """Wavenet / WavenetStack / WavenetResBlock, ns2.py:597-725.  `dilations`: optional (stacks, layers) table that
+    replaces the reference's 2**i."""
     x = causal_conv1d(x, P["wavenet.init_conv.weight"], P["wavenet.init_conv.bias"])
     inputs = [x] * cfg.wavenet_layers
     skips = None
@@ -78,7 +81,8 @@ def wavenet(P, cfg, x, t):
             g, b = tt[:, :dim, None], tt[:, dim:, None]
             xi = inputs[i]
             res = causal_conv1d(xi, P[pre + "res_conv.weight"], P[pre + "res_conv.bias"])
-            y = causal_conv1d(xi, P[pre + "conv.weight"], P[pre + "conv.bias"], 2 ** i)
+            y = causal_conv1d(xi, P[pre + "conv.weight"], P[pre + "conv.bias"],
+                              2 ** i if dilations is None else dilations[s][i])
             y = y * g + b
             y = y.tanh() * y.sigmoid() + res
             residuals.append(y)
@@ -116,7 +120,16 @@ def transformer(P, cfg, x, t, context=None):
 
 @torch.no_grad()
 def model_forward(P: Params, cfg, x, times, prompt=None, cond=None, drop_prompt=None, drop_cond=None):
-    """Model.forward, ns2.py:929-1000 (explicit CFG drop masks, None = keep everything)."""
+    """Model.forward, ns2.py:929-1000 (explicit CFG drop masks, None = keep everything), without autograd."""
+    return model_forward_autograd(P, cfg, x, times, prompt, cond, drop_prompt, drop_cond)
+
+
+def model_forward_autograd(P: Params, cfg, x, times, prompt=None, cond=None, drop_prompt=None, drop_cond=None,
+                           dilations=None):
+    """`model_forward` with autograd left as the caller has it: gradients reach every tensor of P, prompt and cond
+    that requires them, so that the port in float64 is a reference for the denoiser's backward.  Runs on the device
+    of `x`.  `dilations`: optional (stacks, layers) table of Wavenet dilations instead of the reference's 2**i, for
+    building a deliberately wrong reference."""
     B, N, D = x.shape
     xt = times[:, None]
     freqs = xt * P["to_time_cond.0.weights"][None] * 2 * math.pi
@@ -124,8 +137,8 @@ def model_forward(P: Params, cfg, x, times, prompt=None, cond=None, drop_prompt=
     t = F.silu(F.linear(t, P["to_time_cond.1.weight"], P["to_time_cond.1.bias"]))
     c = None
     if cfg.condition_on_prompt:
-        dp = torch.zeros(B, dtype=torch.bool) if drop_prompt is None else drop_prompt
-        dc = torch.zeros(B, dtype=torch.bool) if drop_cond is None else drop_cond
+        dp = torch.zeros(B, dtype=torch.bool, device=x.device) if drop_prompt is None else drop_prompt
+        dc = torch.zeros(B, dtype=torch.bool, device=x.device) if drop_cond is None else drop_cond
         pc = F.silu(F.linear(prompt.mean(dim=1), P["to_prompt_cond.1.weight"], P["to_prompt_cond.1.bias"]))
         pc = torch.where(dp[:, None], P["null_prompt_cond"][None], pc)
         t = torch.cat((t, pc), dim=-1)
@@ -137,5 +150,5 @@ def model_forward(P: Params, cfg, x, times, prompt=None, cond=None, drop_prompt=
         L = cp.shape[-1]
         cp = cp[..., :N] if L >= N else F.pad(cp, (0, N - L))
         xc = xc + cp
-    xc = wavenet(P, cfg, xc, t)
+    xc = wavenet(P, cfg, xc, t, dilations)
     return transformer(P, cfg, xc.transpose(1, 2), t, context=c)

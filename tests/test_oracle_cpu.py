@@ -142,6 +142,44 @@ def test_torch_port_matches_reference(name):
     assert err_stats(out.numpy(), z["out_fp64"])[0] < 1e-9
 
 
+@pytest.mark.parametrize("case", ["uncond_small", "cond_small"])
+def test_torch_port_autograd_matches_reference_gradients(case):
+    """`model_forward_autograd` in float64 is the reference of the GPU backward tests at the benchmarked dims
+    (tests/test_denoiser_backward_fp64_gpu.py): its autograd through the diffusion loss of make_golden.gradient_goldens
+    (sigmoid schedule, v target, min-SNR-5 weight) reproduces the reference's fp64 gradients — every parameter's norm
+    and every stored whole tensor."""
+    from naturalspeech2_pytorch_b200.diffusion import gamma_to_alpha_sigma, sigmoid_schedule
+    from oracle import denoiser_torch_port as tp
+    zd = np.load(GOLDEN / "diffusion_uncond_small.npz")
+    gz = np.load(GOLDEN / f"grads_{case}.npz")
+    zm, kwargs, seed = load_model_golden(case)
+    model = build_model(kwargs, seed)
+    P = {k: v.detach().double().requires_grad_(True) for k, v in model.named_parameters()}
+    latents, times, noise = (torch.from_numpy(zd[k]).double() for k in ("latents", "times", "noise"))
+    extra = {}
+    if kwargs.get("condition_on_prompt"):
+        extra = dict(prompt=torch.from_numpy(zm["in_prompt"]).double(), cond=torch.from_numpy(zm["in_cond"]).double())
+    gamma = sigmoid_schedule(times)
+    alpha, sigma = gamma_to_alpha_sigma(gamma[:, None, None], 1.)
+    pred = tp.model_forward_autograd(P, oracle_config(kwargs), alpha * latents + sigma * noise, times, **extra)
+    per_sample = ((pred - (alpha * noise - sigma * latents)) ** 2).reshape(pred.shape[0], -1).mean(dim=1)
+    snr = (alpha * alpha) / (sigma * sigma)
+    loss = (per_sample * (snr.clamp(max=5) / (snr + 1))).mean()   # the golden's broadcast, as make_golden.py writes it
+    assert abs(loss.item() - float(gz["loss"])) < 1e-9 * abs(float(gz["loss"]))
+    loss.backward()
+    names = [str(n) for n in gz["names"]]
+    assert set(names) == set(P)
+    for n, ref_norm in zip(names, gz["norms"]):
+        g = P[n].grad if P[n].grad is not None else torch.zeros_like(P[n])
+        assert abs(float(g.norm()) - float(ref_norm)) <= 1e-9 * max(float(ref_norm), 1e-6), (n, float(g.norm()), ref_norm)
+    stored = [k for k in gz.files if k.startswith("grad::")]
+    assert len(stored) == 13
+    for key in stored:
+        n = key[len("grad::"):]
+        ref = torch.from_numpy(gz[key]).double()   # stored as float32
+        assert float((P[n].grad - ref).abs().max()) <= 2 ** -23 * float(ref.abs().max()), n
+
+
 @pytest.mark.parametrize("name", BIG_MODEL_CASES)
 def test_torch_port_matches_reference_at_benchmarked_dims(name):
     """The port that bench.py uses as the in-run parity checker / CPU arm, pinned at dim 512 / heads 8 / seq 1024

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define NS2_ABI_VERSION 5
+#define NS2_ABI_VERSION 6
 
 typedef void* ns2_stream_t; /* cudaStream_t */
 
@@ -184,6 +184,34 @@ typedef struct ns2_attn_bwd_args {
 } ns2_attn_bwd_args;
 
 int ns2_attn_bwd(const ns2_attn_bwd_args* args, ns2_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * 2b. Dropout (training only).  One site's parameters: a 64-bit seed (Philox4x32-10 key = its low / high 32 bits),
+ *     the site number (one per dropout site of a forward call, reused by its backward) and the drop probability p.
+ *     An element is kept iff its Philox word is >= min(floor(p 2^32 + 0.5), 2^32 - 1) (computed in double from the
+ *     float p); kept values are scaled by (float)(1 / (1 - p)).  p must be in [0, 1); p = 0 runs the plain entry point.
+ *     Counter layouts (csrc/philox.cuh):
+ *       attention element (b, h, q, k), q' = q & ~8, k' = k & ~8:  ctr = ((k' >> 4) 8 + (k' & 7), (q' >> 4) 8 + (q' & 7),
+ *           b heads + h, site); its four words belong to (q', k'), (q', k' + 8), (q' + 8, k'), (q' + 8, k' + 8)
+ *       element-wise element i:  ctr = ((i >> 2) & 0xffffffff, i >> 34, 0xffffffff, site); word i & 3
+ *    ns2_attn_fwd_dropout : ns2_attn_fwd with dropout on the softmax probabilities (Attend, attend.py:106 SDPA
+ *                           dropout_p, attend.py:149 attn_dropout): out = ((P (.) M) V) / (1 - p); lse as without
+ *                           dropout (undropped probabilities, bit-identical)
+ *    ns2_attn_bwd_dropout : ns2_attn_bwd of that forward, the mask regenerated from (seed, site, b, h, q, k):
+ *                           dV = (P (.) M)^T dO / (1 - p), dP = (dO V^T) (.) M / (1 - p), dS = P (.) (dP - D), D from the
+ *                           dropped output o
+ *    ns2_dropout_f32      : x (n f32, in place) = x * keep * scale — the phoneme encoder's conv dropout
+ *                           (nn.Dropout, ns2.py:258) and its backward on the gradient
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct ns2_dropout {
+  uint64_t seed;
+  uint32_t site;
+  float p;
+} ns2_dropout;
+
+int ns2_attn_fwd_dropout(const ns2_attn_args* args, const ns2_dropout* dropout, ns2_stream_t stream);
+int ns2_attn_bwd_dropout(const ns2_attn_bwd_args* args, const ns2_dropout* dropout, ns2_stream_t stream);
+int ns2_dropout_f32(float* x, int64_t n, const ns2_dropout* dropout, ns2_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * 3. RMSNorm (+ learned gamma) (+ FiLM) : RMSNorm.forward ns2.py:736-746.

@@ -17,7 +17,7 @@ NS2_MSE_SCRATCH_PER_SAMPLE = 64
 NS2_RVQ_STATS_LEN = 260
 NS2_OBJ_V, NS2_OBJ_EPS, NS2_OBJ_X0 = 0, 1, 2
 NS2_GEMM_FLAG_SKIP_EPILOGUE, NS2_GEMM_FLAG_WAVENET_ONE_PASS, NS2_GEMM_FLAG_SILU = 1, 2, 4
-NS2_ABI_VERSION = 5
+NS2_ABI_VERSION = 6
 
 
 class GemmSeg(C.Structure):
@@ -80,6 +80,10 @@ class AttnBwdArgs(C.Structure):
     ]
 
 
+class Dropout(C.Structure):
+    _fields_ = [("seed", C.c_uint64), ("site", C.c_uint32), ("p", C.c_float)]
+
+
 _P, _I32, _I64, _F = C.c_void_p, C.c_int32, C.c_int64, C.c_float
 
 # name -> (restype, argtypes); every symbol include/ns2_b200.h declares
@@ -92,6 +96,9 @@ SIGNATURES = {
     "ns2_wgrad": (C.c_int, [C.POINTER(WgradArgs), _P]),
     "ns2_attn_fwd": (C.c_int, [C.POINTER(AttnArgs), _P]),
     "ns2_attn_bwd": (C.c_int, [C.POINTER(AttnBwdArgs), _P]),
+    "ns2_attn_fwd_dropout": (C.c_int, [C.POINTER(AttnArgs), C.POINTER(Dropout), _P]),
+    "ns2_attn_bwd_dropout": (C.c_int, [C.POINTER(AttnBwdArgs), C.POINTER(Dropout), _P]),
+    "ns2_dropout_f32": (C.c_int, [_P, _I64, C.POINTER(Dropout), _P]),
     "ns2_rmsnorm_film": (C.c_int, [_P, _I64, _I64, _I32, _I32, _P, _P, _I64, _P, _I64, _P]),
     "ns2_rmsnorm_f32": (C.c_int, [_P, _I64, _I64, _I32, _P, _P, _I64, _P]),
     "ns2_time_cond": (C.c_int, [_P, _I32, _P, _I32, _P, _P, _I32, _P, _I64, _P]),

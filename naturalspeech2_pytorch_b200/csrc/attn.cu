@@ -8,7 +8,14 @@
 //                   memory, fp32 accumulator fragments in registers) -> online softmax in fp32 -> P packed to bf16
 //                   straight from the S fragments into the A-operand fragments of O += P V_j (register-A wgmma; V is
 //                   the MN-major B operand: its rows are keys = the reduction dimension, so V is never transposed)
+//
+// attn_fwd_kernel<true> adds the attention dropout of Attend (attend.py:106 / 149: dropout on the softmax probabilities
+// while training).  The keep bits of a key tile come from Philox (philox.cuh), drawn while the S wgmma runs.  The row
+// sums l and the saved log-sum-exp use the undropped probabilities (lse is bit-identical to attn_fwd_kernel<false>'s),
+// each P element is multiplied by its keep bit before it becomes an A fragment of O += P V, and 1 / (1 - p) is applied
+// once, with 1 / l, when O is stored.
 #include "ptx.cuh"
+#include "philox.cuh"
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
 
@@ -40,6 +47,7 @@ struct AttnDev {
   int q_len, kv_len;
   float scale_log2e;
   float* lse;   // optional (batches, heads, q_len): log2-domain log-sum-exp of the scaled scores, for the backward pass
+  DropoutDev drop;   // attn_fwd_kernel<true> only
 };
 
 __device__ __forceinline__ float ex2_approx(float x) {
@@ -48,6 +56,9 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 
+__device__ __forceinline__ float keep_if(float x, uint32_t bits, int n) { return (bits >> n) & 1u ? x : 0.f; }
+
+template <bool DROPOUT>
 __global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid_constant__ AttnDev p) {
   using namespace attn;
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -110,12 +121,30 @@ __global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid
       const int st = j % KVS;
       mbar_wait(smem_u32(&kv_full[st]), (j / KVS) & 1);
       float s[BKV / 2];
+      uint32_t keep[2];   // DROPOUT: keep bit of S fragment element n = 4 jj + e is bit n & 31 of keep[n >> 5]
       {
         const uint64_t dk = gmma_desc_sw128(smem_u32(smem + OFF_K + st * KV_BYTES), 16, 1024);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < DH / 16; ++k) wgmma_bf16_ss_n128<0, 0>(s, dq + 2 * k, dk + 2 * k, k > 0 ? 1u : 0u);
         wgmma_commit();
+        if constexpr (DROPOUT) {   // one Philox block per (16-key group kk, column t): rows r0, r0 + 8 x keys k, k + 8
+          const uint32_t cq = philox_attn_index(q0 + r0), cbh = b * gridDim.y + head, th = p.drop.threshold;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {   // keep[h]: 16-key groups 4 h .. 4 h + 3
+            keep[h] = 0u;
+#pragma unroll 1   // one group at a time: unrolled, the Philox rounds of all groups would spill the accumulators
+            for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+              for (int t = 0; t < 2; ++t) {
+                const Philox4 r = philox4x32_10(philox_attn_index(j * BKV + 16 * (4 * h + kk) + c2 + t), cq, cbh,
+                                                p.drop.site, p.drop.key0, p.drop.key1);
+                const int n = 8 * kk + t;   // element 4 (2 kk) + t of the word; +4: key + 8; +2: row + 8
+                keep[h] |= (r.x >= th ? 1u : 0u) << n | (r.y >= th ? 1u : 0u) << (n + 4) |
+                           (r.z >= th ? 1u : 0u) << (n + 2) | (r.w >= th ? 1u : 0u) << (n + 6);
+              }
+          }
+        }
         wgmma_wait<0>();
         wgmma_hold(s);
       }
@@ -157,8 +186,15 @@ __global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid
         const float p3 = ex2_approx(fmaf(s[4 * jj + 3], c, -m_new[1]));
         l_run[0] += p0 + p1;
         l_run[1] += p2 + p3;
-        pa[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(p0, p1);
-        pa[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(p2, p3);
+        if constexpr (DROPOUT) {
+          const uint32_t kb = keep[jj >> 3];
+          const int n = (4 * jj) & 31;
+          pa[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(keep_if(p0, kb, n), keep_if(p1, kb, n + 1));
+          pa[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(keep_if(p2, kb, n + 2), keep_if(p3, kb, n + 3));
+        } else {
+          pa[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(p0, p1);
+          pa[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(p2, p3);
+        }
       }
       {
         const uint32_t vbase = smem_u32(smem + OFF_V + st * KV_BYTES);
@@ -181,7 +217,7 @@ __global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid
       l += __shfl_xor_sync(0xffffffffu, l, 2);
       const int qrow = q0 + r0 + 8 * i;
       if (qrow < p.q_len) {
-        const float inv = 1.0f / l;
+        const float inv = DROPOUT ? p.drop.scale / l : 1.0f / l;
         if (p.lse != nullptr && (lane & 3) == 0)
           p.lse[(static_cast<long long>(b) * gridDim.y + head) * p.q_len + qrow] = m_run[i] + log2f(l);
         __nv_bfloat16* op = p.out + static_cast<long long>(b) * p.o_bs + static_cast<long long>(qrow) * p.o_rs +
@@ -195,11 +231,8 @@ __global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid
   }
 }
 
-}  // namespace ns2
-
-extern "C" int ns2_attn_fwd(const ns2_attn_args* a, ns2_stream_t stream_) {
-  using namespace ns2;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+// drop == nullptr: the plain kernel; otherwise attn_fwd_kernel<true> with those dropout parameters.
+static int attn_fwd_launch(const ns2_attn_args* a, const DropoutDev* drop, cudaStream_t stream) {
   NS2_REQUIRE(a != nullptr && a->q && a->k && a->v && a->out, "attn_fwd: NULL pointer");
   NS2_REQUIRE(a->dim_head == 64, "attn_fwd: dim_head=%d, only 64 is supported", a->dim_head);
   NS2_REQUIRE(a->batches > 0 && a->heads > 0 && a->q_len > 0 && a->kv_len > 0, "attn_fwd: empty problem");
@@ -235,10 +268,31 @@ extern "C" int ns2_attn_fwd(const ns2_attn_args* a, ns2_stream_t stream_) {
   dev.kv_len = a->kv_len;
   dev.scale_log2e = a->scale * 1.4426950408889634f;
   dev.lse = a->lse;
-  NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel, attn::SMEM_BYTES));
   dim3 grid((a->q_len + attn::BQ - 1) / attn::BQ, a->heads, a->batches);
-  attn_fwd_kernel<<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
+  if (drop == nullptr) {
+    NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<false>, attn::SMEM_BYTES));
+    attn_fwd_kernel<false><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
+  } else {
+    dev.drop = *drop;
+    NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<true>, attn::SMEM_BYTES));
+    attn_fwd_kernel<true><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
+  }
   g_launches.fetch_add(1, std::memory_order_relaxed);
   NS2_CUDA_CHECK(cudaGetLastError());
   return kOk;
+}
+
+}  // namespace ns2
+
+extern "C" int ns2_attn_fwd(const ns2_attn_args* a, ns2_stream_t stream) {
+  return ns2::attn_fwd_launch(a, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int ns2_attn_fwd_dropout(const ns2_attn_args* a, const ns2_dropout* d, ns2_stream_t stream) {
+  using namespace ns2;
+  NS2_REQUIRE(d != nullptr, "attn_fwd_dropout: NULL dropout parameters");
+  DropoutDev drop;
+  NS2_REQUIRE(make_dropout_dev(d->seed, d->site, d->p, &drop), "attn_fwd_dropout: p=%g is not in [0, 1)",
+              static_cast<double>(d->p));
+  return attn_fwd_launch(a, d->p == 0.0f ? nullptr : &drop, static_cast<cudaStream_t>(stream));
 }

@@ -15,7 +15,13 @@
 //                   dQ_i (partial over this warpgroup's keys) = dS K is computed with dS as the MN-major A operand and
 //                   added into the fp32 dQ accumulator with global reductions (every key tile contributes to every
 //                   query row).  dK_j / dV_j stay in registers over all query tiles and are stored once at the end.
+//
+// attn_bwd_kernel<true> is the backward of attn_fwd_kernel<true> (attention dropout, mask M, s = 1 / (1 - p)).  It
+// regenerates M from (seed, site, b, h, q, k) with Philox (philox.cuh) while the S^T / dP^T wgmma run:
+//   dV = (P * M)^T dO s (s applied when dV is stored)    dP = (dO V^T) * M s    dS = P * (dP - D) * scale
+// with D = rowsum(dO * O) of the dropped output O, so attn_delta_kernel is unchanged.
 #include "ptx.cuh"
+#include "philox.cuh"
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
 
@@ -35,6 +41,8 @@ constexpr int OFF_DO = OFF_Q + 2 * QT_BYTES;        // [2 stages]
 constexpr int OFF_DS = OFF_DO + 2 * QT_BYTES;       // dS^T: [128 keys][64 queries] bf16, 128B-swizzled rows
 constexpr int OFF_BAR = OFF_DS + BKV * BQ * 2;
 constexpr int SMEM_BYTES = OFF_BAR + 256;           // 80.25 KB
+constexpr int OFF_KEEP = SMEM_BYTES;                // attn_bwd_kernel<true>: one keep-bit word per gradient thread
+constexpr int SMEM_BYTES_DROPOUT = OFF_KEEP + 256 * 4;
 constexpr int THREADS = 384;
 }  // namespace ab
 
@@ -48,6 +56,7 @@ struct AttnBwdDev {
   long long dk_rs, dk_bs, dv_rs, dv_bs;
   int q_len, kv_len, heads;
   float scale, scale_log2e;
+  DropoutDev drop;      // attn_bwd_kernel<true> only
 };
 
 __device__ __forceinline__ float ab_ex2(float x) {
@@ -56,6 +65,9 @@ __device__ __forceinline__ float ab_ex2(float x) {
   return y;
 }
 
+__device__ __forceinline__ float ab_keep_if(float x, uint32_t bits, int n) { return (bits >> n) & 1u ? x : 0.f; }
+
+template <bool DROPOUT>
 __global__ void __launch_bounds__(ab::THREADS, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdDev p) {
   using namespace ab;
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -126,6 +138,24 @@ __global__ void __launch_bounds__(ab::THREADS, 1) attn_bwd_kernel(const __grid_c
       const int st = i & 1;
       mbar_wait(smem_u32(&q_full[st]), (i >> 1) & 1);
       const uint32_t q_s = smem_u32(smem + OFF_Q + st * QT_BYTES), do_s = smem_u32(smem + OFF_DO + st * QT_BYTES);
+      // DROPOUT: keep bit of fragment element n = 4 jj + e (key row kr0 + 8 (e >> 1), query 8 jj + c2 + (e & 1)) is bit n
+      // of this thread's word at keep_s.  Drawn before the S^T / dP^T wgmma are issued (their accumulators are not live
+      // yet) and parked in shared memory, re-read per fragment column: a register held across the P^T / dS^T loop spills.
+      const uint32_t keep_s = smem_u32(smem + OFF_KEEP) + 4 * (threadIdx.x - 128);
+      if constexpr (DROPOUT) {   // one Philox block per (16-query group g >> 1, column g & 1): keys kr0, kr0 + 8 x queries q, q + 8
+        const uint32_t ck = philox_attn_index(j * BKV + kr0), cbh = b * p.heads + head, th = p.drop.threshold;
+        uint32_t keep = 0u;
+#pragma unroll 1   // one block at a time: unrolled, the Philox rounds would spill the accumulators
+        for (int g = 0; g < BQ / 8; ++g) {
+          const int qq = g >> 1, t = g & 1;
+          const Philox4 r = philox4x32_10(ck, philox_attn_index(i * BQ + 16 * qq + c2 + t), cbh, p.drop.site,
+                                          p.drop.key0, p.drop.key1);
+          const int n = 8 * qq + t;   // element 4 (2 qq) + t; +2: key + 8; +4: query + 8
+          keep |= (r.x >= th ? 1u : 0u) << n | (r.y >= th ? 1u : 0u) << (n + 2) | (r.z >= th ? 1u : 0u) << (n + 4) |
+                  (r.w >= th ? 1u : 0u) << (n + 6);
+        }
+        asm volatile("st.shared.u32 [%0], %1;" ::"r"(keep_s), "r"(keep));
+      }
       // S^T = K Q_i^T, dP^T = V dO_i^T (keys x queries; both operands K-major)
       float s[BQ / 2], dp[BQ / 2];
       wgmma_fence();
@@ -156,13 +186,20 @@ __global__ void __launch_bounds__(ab::THREADS, 1) attn_bwd_kernel(const __grid_c
           Dl[e] = q_ok ? __ldg(p.delta + sidx) : 0.f;
         }
         float pv[4], dv[4];
+        uint32_t keep = 0u;
+        if constexpr (DROPOUT) asm volatile("ld.shared.u32 %0, [%1];" : "=r"(keep) : "r"(keep_s));
 #pragma unroll
         for (int e = 0; e < 4; ++e) {   // e = 2 r + t: key row kr0 + 8 r, query column qc + t
           const int r = e >> 1, t = e & 1;
           float pp = ab_ex2(fmaf(s[4 * jj + e], p.scale_log2e, -L[t]));
           if (kr0 + 8 * r >= valid) pp = 0.f;
-          pv[e] = pp;
-          dv[e] = pp * (dp[4 * jj + e] - Dl[t]) * p.scale;
+          if constexpr (DROPOUT) {
+            pv[e] = ab_keep_if(pp, keep, 4 * jj + e);
+            dv[e] = pp * (ab_keep_if(dp[4 * jj + e], keep, 4 * jj + e) * p.drop.scale - Dl[t]) * p.scale;
+          } else {
+            pv[e] = pp;
+            dv[e] = pp * (dp[4 * jj + e] - Dl[t]) * p.scale;
+          }
         }
         pa[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(pv[0], pv[1]);
         pa[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(pv[2], pv[3]);
@@ -211,6 +248,10 @@ __global__ void __launch_bounds__(ab::THREADS, 1) attn_bwd_kernel(const __grid_c
       }
     }
     // ---- dK_j, dV_j -> bf16 ----
+    if constexpr (DROPOUT) {
+#pragma unroll
+      for (int i = 0; i < DH / 2; ++i) dv_acc[i] *= p.drop.scale;
+    }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const int key = j * BKV + kr0 + 8 * r;
@@ -247,11 +288,8 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const __nv_bfloat16* __
   }
 }
 
-}  // namespace ns2
-
-extern "C" int ns2_attn_bwd(const ns2_attn_bwd_args* a, ns2_stream_t stream_) {
-  using namespace ns2;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+// drop == nullptr: the plain kernel; otherwise attn_bwd_kernel<true> with those dropout parameters.
+static int attn_bwd_launch(const ns2_attn_bwd_args* a, const DropoutDev* drop, cudaStream_t stream) {
   NS2_REQUIRE(a != nullptr && a->q && a->k && a->v && a->o && a->d_o && a->lse && a->delta && a->dq_accum && a->dk && a->dv,
               "attn_bwd: NULL pointer");
   NS2_REQUIRE(a->dim_head == 64, "attn_bwd: dim_head=%d, only 64 is supported", a->dim_head);
@@ -292,10 +330,31 @@ extern "C" int ns2_attn_bwd(const ns2_attn_bwd_args* a, ns2_stream_t stream_) {
   dev.heads = a->heads;
   dev.scale = a->scale;
   dev.scale_log2e = a->scale * 1.4426950408889634f;
-  NS2_CUDA_CHECK(set_max_smem_once(attn_bwd_kernel, ab::SMEM_BYTES));
   dim3 grid((a->kv_len + ab::BKV - 1) / ab::BKV, a->heads, a->batches);
-  attn_bwd_kernel<<<grid, ab::THREADS, ab::SMEM_BYTES, stream>>>(dev);
+  if (drop == nullptr) {
+    NS2_CUDA_CHECK(set_max_smem_once(attn_bwd_kernel<false>, ab::SMEM_BYTES));
+    attn_bwd_kernel<false><<<grid, ab::THREADS, ab::SMEM_BYTES, stream>>>(dev);
+  } else {
+    dev.drop = *drop;
+    NS2_CUDA_CHECK(set_max_smem_once(attn_bwd_kernel<true>, ab::SMEM_BYTES_DROPOUT));
+    attn_bwd_kernel<true><<<grid, ab::THREADS, ab::SMEM_BYTES_DROPOUT, stream>>>(dev);
+  }
   g_launches.fetch_add(2, std::memory_order_relaxed);
   NS2_CUDA_CHECK(cudaGetLastError());
   return kOk;
+}
+
+}  // namespace ns2
+
+extern "C" int ns2_attn_bwd(const ns2_attn_bwd_args* a, ns2_stream_t stream) {
+  return ns2::attn_bwd_launch(a, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int ns2_attn_bwd_dropout(const ns2_attn_bwd_args* a, const ns2_dropout* d, ns2_stream_t stream) {
+  using namespace ns2;
+  NS2_REQUIRE(d != nullptr, "attn_bwd_dropout: NULL dropout parameters");
+  DropoutDev drop;
+  NS2_REQUIRE(make_dropout_dev(d->seed, d->site, d->p, &drop), "attn_bwd_dropout: p=%g is not in [0, 1)",
+              static_cast<double>(d->p));
+  return attn_bwd_launch(a, d->p == 0.0f ? nullptr : &drop, static_cast<cudaStream_t>(stream));
 }

@@ -9,8 +9,11 @@
 //   expand_encodings_bwd   the transpose of length regulation: segmented sums over each phoneme's frames, scattered to
 //                          the phoneme encodings and the coarse-pitch table (ns2.py:1449-1455)
 //   add_rows_bcast         d prompt of the prompt FiLM vector's mean-pool (Reduce 'b n d -> b d' mean, ns2.py:858-862)
+//   dropout_f32            the phoneme encoder's conv dropout (nn.Dropout after the causal conv's SiLU, ns2.py:258) on
+//                          the forward activation and, with the same mask, on its gradient (philox.cuh element stream)
 // All HBM-bound.  The scatters accumulate with fp32 atomics, so their summation order is not fixed.
 #include "host_common.h"
+#include "philox.cuh"
 #include "../../include/ns2_b200.h"
 
 #include <atomic>
@@ -114,6 +117,30 @@ __global__ void __launch_bounds__(256) add_rows_bcast_kernel(float* __restrict__
   }
 }
 
+// x[i] *= keep(i) ? scale : 0; one Philox block per 4 consecutive elements (the last group may be partial).
+__global__ void __launch_bounds__(256) dropout_f32_kernel(float* __restrict__ x, long long n, DropoutDev d) {
+  const long long groups = (n + 3) >> 2;
+  for (long long g = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; g < groups;
+       g += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const Philox4 r = philox4x32_10(static_cast<uint32_t>(g), static_cast<uint32_t>(g >> 32), 0xffffffffu, d.site,
+                                    d.key0, d.key1);
+    const float f0 = r.x >= d.threshold ? d.scale : 0.f, f1 = r.y >= d.threshold ? d.scale : 0.f;
+    const float f2 = r.z >= d.threshold ? d.scale : 0.f, f3 = r.w >= d.threshold ? d.scale : 0.f;
+    if (4 * g + 4 <= n) {
+      float4* p4 = reinterpret_cast<float4*>(x) + g;
+      float4 v = *p4;
+      v.x *= f0;
+      v.y *= f1;
+      v.z *= f2;
+      v.w *= f3;
+      *p4 = v;
+    } else {
+      const float f[3] = {f0, f1, f2};
+      for (long long i = 4 * g; i < n; ++i) x[i] *= f[i - 4 * g];
+    }
+  }
+}
+
 unsigned grid_cap(long long n) {
   long long g = (n + 255) / 256;
   const long long cap = static_cast<long long>(num_sms()) * 8;
@@ -177,6 +204,21 @@ extern "C" int ns2_add_rows_bcast(float* x, int32_t batch, int32_t rows, int32_t
   if (total == 0) return kOk;
   NS2_REQUIRE(x && v, "add_rows_bcast: null pointer");
   add_rows_bcast_kernel<<<grid_cap(total), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, rows, dim, v, scale, total);
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  NS2_CUDA_CHECK(cudaGetLastError());
+  return kOk;
+}
+
+extern "C" int ns2_dropout_f32(float* x, int64_t n, const ns2_dropout* dropout, ns2_stream_t stream) {
+  NS2_REQUIRE(dropout != nullptr, "dropout_f32: NULL dropout parameters");
+  DropoutDev d;
+  NS2_REQUIRE(make_dropout_dev(dropout->seed, dropout->site, dropout->p, &d), "dropout_f32: p=%g is not in [0, 1)",
+              static_cast<double>(dropout->p));
+  NS2_REQUIRE(n >= 0, "dropout_f32: negative size");
+  if (n == 0 || dropout->p == 0.0f) return kOk;
+  NS2_REQUIRE(x != nullptr, "dropout_f32: null pointer");
+  NS2_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "dropout_f32: x must be 16-byte aligned");
+  dropout_f32_kernel<<<grid_cap((n + 3) / 4), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, n, d);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   NS2_CUDA_CHECK(cudaGetLastError());
   return kOk;

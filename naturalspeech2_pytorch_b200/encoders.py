@@ -24,7 +24,14 @@ the backward needs (bit-identical output); its backward walks the encoder in rev
                          GEMM with mirrored shifts (the prompt encoder's first conv needs none: its input comes from the
                          codec)
   nn.Embedding           ops.embedding_bwd (scatter-add; the pad row receives gradient, as in the reference)
-Dropout stays the identity in training, as in the denoiser (the reference's conv / attention dropout is not drawn).
+Dropout: with `train_dropout` set (default False; `Conditioner(train_dropout=True)` sets it on both encoders) a call
+in train() mode - with or without autograd, like nn.Dropout - draws the reference's dropout: every transformer layer's
+attention drops softmax probabilities with p = `attn_dropout` (SpeechPromptEncoder's `dropout`, PhonemeEncoder's
+`attn_dropout`; Attend, attend.py:106 / 149), and the phoneme encoder drops its causal conv's SiLU output with p =
+`conv_dropout` (ns2.py:258).  The masks are Philox streams (include/ns2_b200.h section 2b) of one 64-bit seed drawn per
+call from torch's default CPU generator (no device sync; torch.manual_seed reproduces it); site 0 is the conv, site
+1 + l the attention of layer l.  The backward regenerates them from the seed in the record.  Without train_dropout, in
+eval() mode, or with p = 0 nothing is drawn and the kernels are those of inference.
 Attention masks are not supported (`mask=None` is what NaturalSpeech2.forward / .sample pass, ns2.py:1475-1476,
 1538-1539).  Numerics follow the denoiser: bf16 tensor-core operands, fp32 accumulation, fp32 residual stream and norm
 statistics.
@@ -84,6 +91,18 @@ class _EncoderBase(_PackedCache):
     def __init__(self):
         super().__init__()
         self.grad_reducer = None   # parallel.GradReducer: all-reduce of this encoder's gradients (data parallel)
+        self.train_dropout = False   # draw the reference's dropout in train() mode (see the module docstring)
+        self.attn_dropout = self.conv_dropout = 0.0
+
+    def _dropout_seed(self) -> Optional[int]:
+        """The call's 64-bit dropout seed, or None when this call draws no dropout (then nothing is drawn from the
+        generator, so the random stream of a run without dropout is unchanged)."""
+        if not (self.training and self.train_dropout and (self.attn_dropout > 0 or self.conv_dropout > 0)):
+            return None
+        return int(torch.randint(0, 2 ** 63 - 1, ()))
+
+    def _attn_dropout(self, seed: Optional[int], layer: int):
+        return None if seed is None else (seed, 1 + layer, self.attn_dropout)
 
     def _pack_transposed_transformer(self, P, T, depth: int) -> None:
         for l in range(depth):
@@ -108,9 +127,10 @@ class _EncoderBase(_PackedCache):
             P["final_g"] = tr.norm.gamma.detach().float().contiguous()
 
     def _transformer(self, x: torch.Tensor, tr: _PlainTransformerParams, P, heads: int,
-                     saved: Optional[dict] = None) -> torch.Tensor:
+                     saved: Optional[dict] = None, seed: Optional[int] = None) -> torch.Tensor:
         """Transformer.forward (ns2.py:1110-1115) on the fp32 residual stream x (B, N, D), updated in place.  With `saved`
-        every layer's activations go to saved["layers"] in fresh tensors (`_transformer_backward` reads them)."""
+        every layer's activations go to saved["layers"] in fresh tensors (`_transformer_backward` reads them).
+        seed: the call's dropout seed (None = no attention dropout)."""
         keep = saved is not None
         if keep and "final_g" in P:
             raise NotImplementedError("training a Transformer with final_norm=True is not supported")
@@ -131,7 +151,7 @@ class _EncoderBase(_PackedCache):
             ops.rmsnorm_film(x, L["h1"], gamma=P[f"l{l}_g1"])
             qkv = ops.gemm(L["h1"], P[f"l{l}_qkv"], L["qkv"], n=3 * inner, epilogue=ops.EPI_BF16)
             ops.attention(qkv[:, :, :inner], qkv[:, :, inner:2 * inner], qkv[:, :, 2 * inner:], L["ao"], heads=heads,
-                          lse=L["lse"])
+                          lse=L["lse"], dropout=self._attn_dropout(seed, l))
             ops.gemm(L["ao"], P[f"l{l}_o"], x, n=D, epilogue=ops.EPI_F32, resid=x)
             if keep:
                 L["x_mid"] = x.clone()
@@ -147,9 +167,10 @@ class _EncoderBase(_PackedCache):
         return x
 
     def _transformer_backward(self, layers: list, tr: _PlainTransformerParams, P, T, heads: int, dxr: torch.Tensor,
-                              dxr_bf: torch.Tensor, grads: Dict[str, torch.Tensor]) -> None:
+                              dxr_bf: torch.Tensor, grads: Dict[str, torch.Tensor], seed: Optional[int] = None) -> None:
         """Transformer backward (ns2.py:1110-1115): dxr (fp32 gradient of the output, updated in place) becomes the
-        gradient of the input; dxr_bf its bf16 copy.  Parameter gradients go to `grads` under the reference's names."""
+        gradient of the input; dxr_bf its bf16 copy.  Parameter gradients go to `grads` under the reference's names.
+        seed: the forward's dropout seed (its attention masks are regenerated)."""
         _, N, D = dxr.shape
 
         def norm_backward(x_in, dh, gamma, key):
@@ -165,7 +186,7 @@ class _EncoderBase(_PackedCache):
             norm_backward(L["x_mid"], dh2, P[f"l{l}_g2"], pfx + "2.gamma")
             # ---- attention: x += Wo attn(Wqkv RMSNorm(x)) ----
             dh1, _ = attention_backward(dxr_bf, L["h1"], L["ao"], L["lse"], L["qkv"], None, T[f"l{l}_o"], T[f"l{l}_qkv"],
-                                        heads, grads, pfx + "1.")
+                                        heads, grads, pfx + "1.", dropout=self._attn_dropout(seed, l))
             norm_backward(L["x_in"], dh1, P[f"l{l}_g1"], pfx + "0.gamma")
 
     def _conv_silu_backward(self, x_in: torch.Tensor, w: torch.Tensor, w_t: Optional[torch.Tensor], bias: torch.Tensor,
@@ -209,6 +230,7 @@ class SpeechPromptEncoder(_EncoderBase):
             raise NotImplementedError("channel counts must be multiples of 64 (tensor-core K blocks)")
         _check_transformer_dims(dims[-1], dim_head)
         self.kernel_size, self.padding, self.heads = kernel_size, padding, heads
+        self.attn_dropout = dropout   # the reference hands `dropout` to every Attention of its Transformer (ns2.py:332)
         mods = [_NoParam()]                                  # Rearrange('b n c -> b c n')
         for d_in, d_out in zip(dims[:-1], dims[1:]):
             mods.extend([nn.Conv1d(d_in, d_out, kernel_size, padding=padding), _NoParam()])   # conv, SiLU
@@ -257,15 +279,17 @@ class SpeechPromptEncoder(_EncoderBase):
             if saved is not None:
                 conv_in.append(h)
             h = out
+        seed = self._dropout_seed()
         if saved is not None:
-            saved["conv_in"] = conv_in
-        return self._transformer(h, self.transformer, P, self.heads, saved)
+            saved.update(conv_in=conv_in, dropout_seed=seed)
+        return self._transformer(h, self.transformer, P, self.heads, saved, seed)
 
     def _train_backward(self, S, d_out: torch.Tensor) -> Dict[str, torch.Tensor]:
         P, T = self.packed(), self.packed_transposed()
         grads: Dict[str, torch.Tensor] = {}
         dxr, dxr_bf = self._start_backward(d_out)
-        self._transformer_backward(S["layers"], self.transformer, P, T, self.heads, dxr, dxr_bf, grads)
+        self._transformer_backward(S["layers"], self.transformer, P, T, self.heads, dxr, dxr_bf, grads,
+                                   S["dropout_seed"])
         d_h = dxr_bf                        # gradient of the last conv's (SiLU) output
         for i in reversed(range(len(self._convs()))):
             # conv i is module conv.{2i+1} (Rearrange, then [Conv1d, SiLU] pairs); its input needs no gradient for i = 0
@@ -292,6 +316,7 @@ class PhonemeEncoder(_EncoderBase):
             raise NotImplementedError("dim must be a multiple of 64 (tensor-core K blocks)")
         _check_transformer_dims(dim_hidden, dim_head)
         self.dim, self.dim_hidden, self.kernel_size, self.heads = dim, dim_hidden, kernel_size, heads
+        self.conv_dropout, self.attn_dropout = conv_dropout, attn_dropout
         self.token_emb = nn.Embedding(num_tokens + 1, dim)
         self.pad_id = num_tokens
         self.conv = nn.Sequential(_NoParam(), nn.Conv1d(dim, dim_hidden, kernel_size), _NoParam(), _NoParam(), _NoParam())
@@ -333,15 +358,21 @@ class PhonemeEncoder(_EncoderBase):
         # CausalConv1d: left padding dilation*(k-1) (ns2.py:592-595) -> tap t reads position n - (k-1-t)
         ops.gemm(e, P["c_w"], h, n=self.dim_hidden, epilogue=ops.EPI_F32,
                  segs=_conv_segs(self.dim, self.kernel_size, self.kernel_size - 1), bias=P["c_b"], flags=_SILU)
+        seed = self._dropout_seed()
+        if seed is not None:
+            ops.dropout_(h, dropout=(seed, 0, self.conv_dropout))                   # nn.Dropout(conv_dropout), ns2.py:258
         if saved is not None:
-            saved.update(ids=ids, emb=e)
-        return self._transformer(h, self.transformer, P, self.heads, saved)
+            saved.update(ids=ids, emb=e, dropout_seed=seed)
+        return self._transformer(h, self.transformer, P, self.heads, saved, seed)
 
     def _train_backward(self, S, d_out: torch.Tensor) -> Dict[str, torch.Tensor]:
         P, T = self.packed(), self.packed_transposed()
         grads: Dict[str, torch.Tensor] = {}
         dxr, dxr_bf = self._start_backward(d_out)
-        self._transformer_backward(S["layers"], self.transformer, P, T, self.heads, dxr, dxr_bf, grads)
+        seed = S["dropout_seed"]
+        self._transformer_backward(S["layers"], self.transformer, P, T, self.heads, dxr, dxr_bf, grads, seed)
+        if seed is not None and self.conv_dropout > 0:   # the conv's dropout mask, on the fp32 gradient
+            ops.cast_bf16(ops.dropout_(dxr, dropout=(seed, 0, self.conv_dropout)), dxr_bf)
         d_e = self._conv_silu_backward(S["emb"], P["c_w"], T["c_w"], P["c_b"], dxr_bf, self.kernel_size - 1, grads,
                                        "conv.1", dtype=torch.float32)
         grads["token_emb.weight"] = ops.embedding_bwd(S["ids"], d_e, torch.zeros_like(P["emb"]), self.pad_id)
@@ -601,13 +632,17 @@ class Conditioner(nn.Module):
     (B, 1, L).  The aligner network, its losses and the duration / pitch predictor are not run: in the reference they
     only feed `aux_loss`, which is never returned (ns2.py:1600-1602), so the diffusion loss is the only gradient path
     into the prompt encoder, the phoneme encoder and `pitch_emb`.  `grad_reducer` (parallel.GradReducer) all-reduces
-    their gradients in data-parallel training."""
+    their gradients in data-parallel training.
+
+    train_dropout=True makes training draw the reference's dropout in both encoders (their `train_dropout`; see the
+    module docstring).  The default False keeps them deterministic, as before the option existed."""
 
     def __init__(self, *, dim_codebook=128, num_phoneme_tokens=None, tokenizer=None, duration_pitch_dim=512,
-                 pitch_emb_dim=256, pitch_emb_pp_hidden_dim=512):
+                 pitch_emb_dim=256, pitch_emb_pp_hidden_dim=512, train_dropout=False):
         super().__init__()
         self.phoneme_enc = PhonemeEncoder(tokenizer=tokenizer, num_tokens=num_phoneme_tokens)
         self.prompt_enc = SpeechPromptEncoder(dim_codebook=dim_codebook)
+        self.phoneme_enc.train_dropout = self.prompt_enc.train_dropout = bool(train_dropout)
         self.duration_pitch = DurationPitchPredictor(dim=duration_pitch_dim)
         self.pitch_emb = nn.Embedding(pitch_emb_dim, pitch_emb_pp_hidden_dim)
         self.grad_reducer = None

@@ -178,6 +178,37 @@ def conv_dgrad_segs(c_out: int, kernel: int, first_shift: int) -> list:
 
 
 # --------------------------------------------------------------------------------------------------
+# dropout (training): (seed, site, p) of one dropout site, see include/ns2_b200.h section 2b
+# --------------------------------------------------------------------------------------------------
+DropoutSpec = Tuple[int, int, float]   # (64-bit seed, site, p)
+
+
+def _dropout_args(dropout: Optional[DropoutSpec]) -> Optional["_lib.Dropout"]:
+    """ctypes parameters of `dropout`, or None when it draws nothing (None or p = 0: the plain entry point runs)."""
+    if dropout is None:
+        return None
+    seed, site, p = dropout
+    if not 0.0 <= float(p) < 1.0:
+        raise ValueError(f"dropout p must be in [0, 1), got {p}")
+    if not 0 <= int(seed) < 2 ** 64 or not 0 <= int(site) < 2 ** 32:
+        raise ValueError(f"dropout seed must fit in 64 bits and site in 32 bits, got {seed}, {site}")
+    if float(p) == 0.0:
+        return None
+    return _lib.Dropout(int(seed), int(site), float(p))
+
+
+def dropout_(x: torch.Tensor, *, dropout: Optional[DropoutSpec]) -> torch.Tensor:
+    """x (f32, contiguous, in place) *= keep * 1 / (1 - p): element i's keep bit is word i & 3 of Philox block i >> 2
+    of (seed, site).  Applying the same (seed, site, p) to a gradient gives the backward of the forward call."""
+    lib = _lib.load()
+    _req_flat(x, torch.float32, "x", x.numel())
+    d = _dropout_args(dropout)
+    if d is not None:
+        check(lib.ns2_dropout_f32(x.data_ptr(), x.numel(), C.byref(d), _stream(x)), "ns2_dropout_f32")
+    return x
+
+
+# --------------------------------------------------------------------------------------------------
 # attention
 # --------------------------------------------------------------------------------------------------
 ATTN_AUTO, ATTN_ONE_TILE, ATTN_TWO_TILE, ATTN_TWO_TILE_POLY2, ATTN_TWO_TILE_POLY4, ATTN_TWO_TILE_LOCKSTEP = 0, 1, 2, 3, 4, 5
@@ -185,8 +216,10 @@ ATTN_AUTO, ATTN_ONE_TILE, ATTN_TWO_TILE, ATTN_TWO_TILE_POLY2, ATTN_TWO_TILE_POLY
 
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tensor, *, heads: int,
               scale: Optional[float] = None, kernel: int = ATTN_AUTO,
-              debug_timeline: Optional[torch.Tensor] = None, lse: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """q: (B, Nq, heads*64), k/v: (B, Nk, heads*64) bf16 (strided views into a fused projection are fine)."""
+              debug_timeline: Optional[torch.Tensor] = None, lse: Optional[torch.Tensor] = None,
+              dropout: Optional[DropoutSpec] = None) -> torch.Tensor:
+    """q: (B, Nq, heads*64), k/v: (B, Nk, heads*64) bf16 (strided views into a fused projection are fine).
+    dropout=(seed, site, p): attention dropout on the softmax probabilities (lse stays that of the undropped ones)."""
     lib = _lib.load()
     for name, t in (("q", q), ("k", k), ("v", v), ("out", out)):
         _req(t, torch.bfloat16, name)
@@ -207,7 +240,11 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tens
         if not lse.is_contiguous() or tuple(lse.shape) != (q.shape[0], heads, q.shape[1]):
             raise ValueError("lse must be a contiguous (B, heads, Nq) float tensor")
     args.lse = _ptr(lse)
-    check(lib.ns2_attn_fwd(C.byref(args), _stream(out)), "ns2_attn_fwd")
+    d = _dropout_args(dropout)
+    if d is None:
+        check(lib.ns2_attn_fwd(C.byref(args), _stream(out)), "ns2_attn_fwd")
+    else:
+        check(lib.ns2_attn_fwd_dropout(C.byref(args), C.byref(d), _stream(out)), "ns2_attn_fwd_dropout")
     return out
 
 
@@ -626,8 +663,9 @@ def rvq_ce_bwd(frames: torch.Tensor, codebooks: torch.Tensor, cn2: torch.Tensor,
 # backward pass
 # --------------------------------------------------------------------------------------------------
 def attention_bwd(q, k, v, o, d_o, lse, dq_accum, dk, dv, *, heads: int, scale: Optional[float] = None,
-                  delta: Optional[torch.Tensor] = None):
-    """(dq_accum f32 (B, Nq, inner) += dQ, dk, dv bf16) of softmax(q k^T scale) v given d_o; zero dq_accum for a plain dQ."""
+                  delta: Optional[torch.Tensor] = None, dropout: Optional[DropoutSpec] = None):
+    """(dq_accum f32 (B, Nq, inner) += dQ, dk, dv bf16) of softmax(q k^T scale) v given d_o; zero dq_accum for a plain dQ.
+    dropout: the forward's (seed, site, p); the mask is regenerated, not stored."""
     lib = _lib.load()
     for name, t in (("q", q), ("k", k), ("v", v), ("o", o), ("d_o", d_o), ("dk", dk), ("dv", dv)):
         _req(t, torch.bfloat16, name)
@@ -651,7 +689,11 @@ def attention_bwd(q, k, v, o, d_o, lse, dq_accum, dk, dv, *, heads: int, scale: 
     a.dv, a.dv_row_stride, a.dv_batch_stride = dv.data_ptr(), dv.stride(1), dv.stride(0)
     a.batches, a.heads, a.q_len, a.kv_len, a.dim_head = B, heads, Nq, Nk, 64
     a.scale = float(scale if scale is not None else 64 ** -0.5)
-    check(lib.ns2_attn_bwd(C.byref(a), _stream(dq_accum)), "ns2_attn_bwd")
+    d = _dropout_args(dropout)
+    if d is None:
+        check(lib.ns2_attn_bwd(C.byref(a), _stream(dq_accum)), "ns2_attn_bwd")
+    else:
+        check(lib.ns2_attn_bwd_dropout(C.byref(a), C.byref(d), _stream(dq_accum)), "ns2_attn_bwd_dropout")
     return dq_accum, dk, dv
 
 

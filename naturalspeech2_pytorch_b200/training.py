@@ -119,13 +119,14 @@ def ff_backward(dy, h, g, c, P, T, pk: str, Di: int, grads: Dict[str, torch.Tens
 
 
 def attention_backward(dy, x, o, lse, q, kv, w_o_t, w_q_t, heads: int, grads: Dict[str, torch.Tensor], name: str,
-                       d_kv=None, x_kv=None, w_kv_t=None):
+                       d_kv=None, x_kv=None, w_kv_t=None, dropout=None):
     """Backward of y = Wo attn(Wq x, Wkv x_kv) (Attention, ns2.py:1029-1053, bias-free) from the forward's attention
     output o and log-sum-exp.  to_out / to_q / to_kv gradients go to grads[name + ...]; returns (d x, d x_kv), bf16.
       * self-attention: kv is None and q is the fused (B, N, 3*inner) qkv of one GEMM on x (transposed pack w_q_t),
         so one wgrad and one dgrad cover q, k and v;
       * cross-attention: d kv goes to `d_kv` (a fresh buffer when None).  Given the context x_kv and its transposed pack
-        w_kv_t, to_kv's gradient and d x_kv are computed too; otherwise d x_kv is None and to_kv is the caller's."""
+        w_kv_t, to_kv's gradient and d x_kv are computed too; otherwise d x_kv is None and to_kv is the caller's.
+    `dropout`: the forward's attention dropout (seed, site, p), or None (see ops.attention)."""
     B, N = dy.shape[:2]
     inner = heads * 64
     dev = dy.device
@@ -139,7 +140,7 @@ def attention_backward(dy, x, o, lse, q, kv, w_o_t, w_q_t, heads: int, grads: Di
         d_kv = torch.empty(B, kv.shape[1], 2 * inner, device=dev, dtype=bf)
     dq = torch.zeros(B, N, inner, device=dev)
     ops.attention_bwd(q, kv[:, :, :inner], kv[:, :, inner:], o, d_o, lse, dq, d_kv[:, :, :inner], d_kv[:, :, inner:],
-                      heads=heads)
+                      heads=heads, dropout=dropout)
     if fused:
         d_q[:, :, :inner].copy_(dq)   # fp32 accumulator -> bf16 slot (layout glue)
         dw = _wgrad(d_q, x)

@@ -56,6 +56,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--train-dropout", action="store_true",
+                    help="train the encoders with the reference's dropout (Conditioner(train_dropout=True))")
     args = ap.parse_args()
     dev = torch.device("cuda", 0)
     torch.manual_seed(0)
@@ -80,7 +82,7 @@ def main():
     del opt
 
     # ---- cond_e2e: the encoders trained jointly ----
-    cond_net = Conditioner(dim_codebook=128, num_phoneme_tokens=TOKENS).to(dev).train()
+    cond_net = Conditioner(dim_codebook=128, num_phoneme_tokens=TOKENS, train_dropout=args.train_dropout).to(dev).train()
     ns = NaturalSpeech2(model, target_sample_hz=24000, conditioner=cond_net)
     trained = [*model.parameters(), *cond_net.prompt_enc.parameters(), *cond_net.phoneme_enc.parameters(),
                *cond_net.pitch_emb.parameters()]   # the duration / pitch predictor only feeds the discarded aux loss
@@ -102,7 +104,8 @@ def main():
     print(json.dumps({
         "cond_e2e": {"ms_per_step": round(ms_e2e, 3), "steps_per_s": round(1e3 / ms_e2e, 3), "loss": round(loss_e2e, 5)},
         "cfg5": {"ms_per_step": round(ms5, 3), "steps_per_s": round(1e3 / ms5, 3), "loss": round(loss5, 5)},
-        "encoder_share_of_step": round(1.0 - ms5 / ms_e2e, 4), "steps": args.steps, "warmup": args.warmup,
+        "encoder_share_of_step": round(1.0 - ms5 / ms_e2e, 4), "train_dropout": args.train_dropout,
+        "steps": args.steps, "warmup": args.warmup,
         "batch": B, "card": card(dev)}))
 
 

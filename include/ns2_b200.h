@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define NS2_ABI_VERSION 6
+#define NS2_ABI_VERSION 7
 
 typedef void* ns2_stream_t; /* cudaStream_t */
 
@@ -99,16 +99,12 @@ typedef struct ns2_gemm_args {
   const float* film;       /* WAVENET: FiLM table */
   int64_t film_batch_stride;
   int32_t film_group_stride;
-  int32_t flags;           /* 0, or NS2_GEMM_FLAG_* */
-  void* debug_timeline;    /* reserved, ignored (keeps the struct layout of ABI v3) */
+  int32_t flags;           /* 0, or NS2_GEMM_FLAG_*; any other bit is an error */
 } ns2_gemm_args;
 
 #define NS2_GEMM_FLAG_SKIP_EPILOGUE 1  /* measurement aid: run the TMA/MMA mainloop only, write nothing */
 #define NS2_GEMM_FLAG_SILU 4 /* BF16 / F32 epilogues: out = silu(acc + bias) (+ resid) — Conv1d + nn.SiLU of the prompt
                                encoder (ns2.py:316-320) and CausalConv1d + SiLU of the phoneme encoder (ns2.py:255-257) */
-#define NS2_GEMM_FLAG_NARROW_LAST 8 /* tuning / A-B tests (groups == 1, n % BN != 0): schedule the partial-width n-tiles
-                                      after all full-width ones instead of n-fastest */
-#define NS2_GEMM_FLAG_WAVENET_ONE_PASS 2 /* accepted and ignored: WAVENET tiles always hold both accumulators */
 
 int ns2_gemm(const ns2_gemm_args* args, ns2_stream_t stream);
 
@@ -147,20 +143,9 @@ typedef struct ns2_attn_args {
   void* out;     int64_t o_row_stride, o_batch_stride;
   int32_t batches, heads, q_len, kv_len, dim_head;
   float scale;
-  int32_t kernel;   /* one of NS2_ATTN_*; validated, every value runs the same sm_90a kernel */
-  void* debug_timeline; /* reserved, ignored (keeps the struct layout of ABI v3) */
-  float* lse;           /* optional (batches, heads, q_len) f32: log2-domain log-sum-exp of the scaled score rows,
-                           saved for ns2_attn_bwd */
+  float* lse;    /* optional (batches, heads, q_len) f32: log2-domain log-sum-exp of the scaled score rows,
+                    saved for ns2_attn_bwd */
 } ns2_attn_args;
-
-/* Kernel selectors of ABI v3.  On sm_90a one kernel (128 queries x 128-key tiles per CTA, P kept in registers as the
- * wgmma A operand) serves every shape, so all selectors give identical results. */
-#define NS2_ATTN_AUTO 0
-#define NS2_ATTN_ONE_TILE 1
-#define NS2_ATTN_TWO_TILE 2
-#define NS2_ATTN_TWO_TILE_POLY2 3
-#define NS2_ATTN_TWO_TILE_POLY4 4
-#define NS2_ATTN_TWO_TILE_LOCKSTEP 5
 
 int ns2_attn_fwd(const ns2_attn_args* args, ns2_stream_t stream);
 
@@ -334,7 +319,7 @@ int ns2_x_start(const float* x, const float* pred, const float* alpha, const flo
  *    ns2_rvq_decode  : emb f32 (F, d) = sum_q codebooks[q, codes[f,q], :]  (summed in order q = 0..Q-1)
  * ------------------------------------------------------------------------------------------------ */
 #define NS2_RVQ_PREPARED_HALFS(q, k, d) ((long long)(q) * (k) * ((d) + 16))
-#define NS2_RVQ_STATS_LEN 260  /* 4 counters + 32 stages x 8 clock64 stamps of CTA 0 (bring-up timeline) */
+#define NS2_RVQ_STATS_LEN 4
 int ns2_rvq_prepare(const float* codebooks, int32_t q, int32_t k, int32_t d, void* cb_f16,
                     float* cb_norm2, float* cb_meta, ns2_stream_t stream);
 int ns2_rvq_encode(const float* frames, int64_t num_frames, int32_t d, const float* codebooks,

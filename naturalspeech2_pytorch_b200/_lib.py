@@ -14,10 +14,10 @@ NS2_EPI_BF16, NS2_EPI_F32, NS2_EPI_GEGLU, NS2_EPI_WAVENET = 0, 1, 2, 3
 NS2_GEMM_MAX_SEGS = 12
 NS2_GEMM_MAX_GROUPS = 8
 NS2_MSE_SCRATCH_PER_SAMPLE = 64
-NS2_RVQ_STATS_LEN = 260
+NS2_RVQ_STATS_LEN = 4
 NS2_OBJ_V, NS2_OBJ_EPS, NS2_OBJ_X0 = 0, 1, 2
-NS2_GEMM_FLAG_SKIP_EPILOGUE, NS2_GEMM_FLAG_WAVENET_ONE_PASS, NS2_GEMM_FLAG_SILU = 1, 2, 4
-NS2_ABI_VERSION = 6
+NS2_GEMM_FLAG_SKIP_EPILOGUE, NS2_GEMM_FLAG_SILU = 1, 4
+NS2_ABI_VERSION = 7
 
 
 class GemmSeg(C.Structure):
@@ -38,7 +38,7 @@ class GemmArgs(C.Structure):
         ("out", C.c_void_p), ("out_row_stride", C.c_int64),
         ("resid", C.c_void_p), ("resid_row_stride", C.c_int64),
         ("film", C.c_void_p), ("film_batch_stride", C.c_int64), ("film_group_stride", C.c_int32),
-        ("flags", C.c_int32), ("debug_timeline", C.c_void_p),
+        ("flags", C.c_int32),
     ]
 
 
@@ -60,8 +60,7 @@ class AttnArgs(C.Structure):
         ("v", C.c_void_p), ("v_row_stride", C.c_int64), ("v_batch_stride", C.c_int64),
         ("out", C.c_void_p), ("o_row_stride", C.c_int64), ("o_batch_stride", C.c_int64),
         ("batches", C.c_int32), ("heads", C.c_int32), ("q_len", C.c_int32), ("kv_len", C.c_int32),
-        ("dim_head", C.c_int32), ("scale", C.c_float), ("kernel", C.c_int32),
-        ("debug_timeline", C.c_void_p), ("lse", C.c_void_p),
+        ("dim_head", C.c_int32), ("scale", C.c_float), ("lse", C.c_void_p),
     ]
 
 

@@ -239,9 +239,6 @@ static int attn_fwd_launch(const ns2_attn_args* a, const DropoutDev* drop, cudaS
   NS2_REQUIRE(a->o_row_stride % 8 == 0 && a->o_batch_stride % 8 == 0 &&
                   (reinterpret_cast<uintptr_t>(a->out) & 15) == 0,
               "attn_fwd: out must be 16-byte aligned with strides multiple of 8");
-  // one kernel for every problem shape; the selector is still validated so callers get the same errors as before
-  NS2_REQUIRE(a->kernel >= NS2_ATTN_AUTO && a->kernel <= NS2_ATTN_TWO_TILE_LOCKSTEP,
-              "attn_fwd: unknown kernel selector %d", a->kernel);
   AttnDev dev;
   memset(&dev, 0, sizeof(dev));
   const uint32_t box[3] = {64, attn::BQ, 1};

@@ -31,7 +31,6 @@ struct GemmDev {
   CUtensorMap tmB;
   CUtensorMap tmOut;   // TMA store / reduce-add target: (columns, group, position, batch), clipped at n and a_rows
   int tiles_n, tiles_per_batch, tiles_m, num_tiles;
-  int narrow_last;     // groups == 1, n % BN != 0: schedule the partial-width n-tiles after all full-width ones
   int a_rows, n, groups;
   int a_gcs, b_grs, out_gcs;
   int dil[NS2_GEMM_MAX_GROUPS];
@@ -57,27 +56,11 @@ struct TileCoord {
 
 __device__ __forceinline__ TileCoord decode_tile(const GemmDev& p, int tile) {
   TileCoord t;
-  int m_tile;
-  if (p.narrow_last) {
-    // The last n-tile of every row block is narrower (n % BN columns).  Full-width tiles first (n fastest, so a row
-    // block's activations stay hot in L2), then all narrow ones, so that every CTA ends on the narrow tiles.
-    const int wide_n = p.tiles_n - 1;
-    const int wide_total = p.tiles_m * wide_n;
-    t.g = 0;
-    if (tile < wide_total) {
-      m_tile = tile / wide_n;
-      t.n_tile = tile - m_tile * wide_n;
-    } else {
-      m_tile = tile - wide_total;
-      t.n_tile = wide_n;
-    }
-  } else {
-    const int per_group = p.tiles_m * p.tiles_n;
-    t.g = tile / per_group;
-    const int r = tile - t.g * per_group;
-    m_tile = r / p.tiles_n;
-    t.n_tile = r - m_tile * p.tiles_n;
-  }
+  const int per_group = p.tiles_m * p.tiles_n;
+  t.g = tile / per_group;
+  const int r = tile - t.g * per_group;
+  const int m_tile = r / p.tiles_n;
+  t.n_tile = r - m_tile * p.tiles_n;
   t.b = m_tile / p.tiles_per_batch;
   t.n0 = (m_tile - t.b * p.tiles_per_batch) * BM;
   return t;
@@ -437,6 +420,8 @@ extern "C" int ns2_gemm(const ns2_gemm_args* a, ns2_stream_t stream_) {
   if (a->resid != nullptr)
     NS2_REQUIRE(a->resid_row_stride % 4 == 0 && (reinterpret_cast<uintptr_t>(a->resid) & 15) == 0,
                 "ns2_gemm: resid must be 16-byte aligned");
+  NS2_REQUIRE((a->flags & ~(NS2_GEMM_FLAG_SKIP_EPILOGUE | NS2_GEMM_FLAG_SILU)) == 0,
+              "ns2_gemm: unknown flags 0x%x (only NS2_GEMM_FLAG_SKIP_EPILOGUE and NS2_GEMM_FLAG_SILU exist)", a->flags);
 
   // ---- tile selection ----
   int bn;
@@ -480,7 +465,6 @@ extern "C" int ns2_gemm(const ns2_gemm_args* a, ns2_stream_t stream_) {
   dev.tiles_per_batch = (a->a_rows + BM - 1) / BM;
   dev.tiles_m = dev.tiles_per_batch * a->a_batches;
   dev.num_tiles = dev.tiles_m * dev.tiles_n * a->groups;
-  dev.narrow_last = ((a->flags & NS2_GEMM_FLAG_NARROW_LAST) && a->groups == 1 && dev.tiles_n > 1 && a->n % bn != 0) ? 1 : 0;
   dev.a_rows = a->a_rows;
   dev.n = a->n;
   dev.groups = a->groups;

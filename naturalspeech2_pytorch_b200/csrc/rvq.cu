@@ -51,12 +51,10 @@ constexpr int OFF_AX = OFF_BX + RING * X_BYTES;      // per-row power of two (K 
 constexpr int OFF_R = OFF_AX + X_BYTES;              // fp32 residuals, row-major padded: 67.6 KB
 constexpr int OFF_KEYS = OFF_R + BF * RSTRIDE * 4;   // top-8 keys of each column half: [half][row][8] floats (8 KB)
 constexpr int OFF_ROWP = OFF_KEYS + 2 * BF * 8 * 4;  // per-row {scale, unused, error bound in D units, force-exact flag}
-constexpr int OFF_SEL = OFF_ROWP + BF * 4 * 4;       // (unused)
-constexpr int OFF_CAND = OFF_SEL + BF * 4;           // CTA-wide queue of the rows that need the exact re-score
+constexpr int OFF_CAND = OFF_ROWP + BF * 4 * 4;      // CTA-wide queue of the rows that need the exact re-score
 constexpr int OFF_BAR = OFF_CAND + (4 + BF) * 4;     // queue of ambiguous rows: [count, pad x3, BF entries]
 constexpr int OFF_META = OFF_BAR + 256;             // per-stage {max ||c||, 2^e} of the first 32 stages
-constexpr int OFF_TL = OFF_META + 256;               // bring-up timeline of CTA 0: 32 stages x 8 clock64 stamps
-constexpr int SMEM_BYTES = OFF_TL + 2048;
+constexpr int SMEM_BYTES = OFF_META + 256;
 constexpr int SCAN_THREADS = 256;     // warps 0-7: quarter = warp & 3, column half = warp >> 2 (A tile / residual rows)
 }  // namespace rvq
 
@@ -111,12 +109,6 @@ __device__ __forceinline__ double coop_reduce(const float4 r, const float4 v) {
   for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
   return a;
 }
-
-// bring-up timeline: stats[4 + q*8 + slot] = clock64 of CTA 0 (tools/rvq_timeline.py); q < 32
-#define NS2_RVQ_STAMP(slot)                                                                              \
-  do {                                                                                                   \
-    if (p.stats != nullptr && blockIdx.x == 0 && q < 32) tl_s[q * 8 + (slot)] = clock64();               \
-  } while (0)
 
 // Half-warp variant: lane hl of a 16-lane half owns dims [8 hl, 8 hl + 8); fixed order, xor-butterfly inside the half
 // (equal inputs give bit-equal results); every lane of the half returns the full distance.
@@ -196,8 +188,6 @@ __global__ void __launch_bounds__(320, 1) rvq_encode_kernel(const __grid_constan
   float4* rowp_s = reinterpret_cast<float4*>(smem + OFF_ROWP);
   int* queue_s = reinterpret_cast<int*>(smem + OFF_CAND);   // [0] = count, [1 + i] = row | na << 8 | nb << 12 | force << 16
   float* meta_s = reinterpret_cast<float*>(smem + OFF_META);
-  long long* tl_s = reinterpret_cast<long long*>(smem + OFF_TL);   // stamps stay in smem until the end: no global
-                                                                   // stores inside the measured phases
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* b_full = bars + 0;    // [RING]
   uint64_t* b_empty = bars + 3;   // [RING] one arrive per scan warp
@@ -261,10 +251,7 @@ __global__ void __launch_bounds__(320, 1) rvq_encode_kernel(const __grid_constan
     uint32_t it = 0;
     for (int q = 0; q < p.Q; ++q) {
       scan_barrier();  // [B1] residuals of this stage are in place
-      if (threadIdx.x == 0) {
-        queue_s[0] = 0;   // filled after [B2]; the previous stage's last read was before [B1]
-        NS2_RVQ_STAMP(0);
-      }
+      if (threadIdx.x == 0) queue_s[0] = 0;   // filled after [B2]; the previous stage's last read was before [B1]
       // row scale (exact power of two into fp16 range), |r|^2 and the filter margin; both threads of a row compute
       // them redundantly from the same data in the same order (bit-identical), so no exchange is needed
       float xs_row;
@@ -319,7 +306,6 @@ __global__ void __launch_bounds__(320, 1) rvq_encode_kernel(const __grid_constan
       }
       fence_proxy_async_smem();
       scan_barrier();  // [B1'] the A tile (written by both warpgroups) is complete
-      if (threadIdx.x == 0) NS2_RVQ_STAMP(1);
 
       // ---- scan this thread's 32-code block of every 128-code chunk, for both of its frames: branch-free top-8 on
       // packed keys.  The accumulator already is the (scaled) score, so a key is one LOP3: (bits & ~31) | index. ----
@@ -410,9 +396,7 @@ __global__ void __launch_bounds__(320, 1) rvq_encode_kernel(const __grid_constan
           ke[1] = make_float4(gb[4], gb[5], gb[6], gb[7]);
         }
       }
-      if (threadIdx.x == 0) NS2_RVQ_STAMP(2);
       scan_barrier();  // [B2] both halves' key lists are published
-      if (threadIdx.x == 0) NS2_RVQ_STAMP(3);
 
       // ---- exact decision + residual update ----
       // Candidates = every code whose key is within the error band of the best key.  Each column half keeps its own
@@ -474,9 +458,7 @@ __global__ void __launch_bounds__(320, 1) rvq_encode_kernel(const __grid_constan
           *dst = v;
         }
       }
-      if (threadIdx.x == 0) NS2_RVQ_STAMP(4);
       scan_barrier();  // [B3] the queue of ambiguous rows is complete
-      if (threadIdx.x == 0) NS2_RVQ_STAMP(6);
       // One row per HALF-warp (lane hl of a half owns dims [8 hl, 8 hl + 8)), so a warp resolves two queue rows per
       // round in one instruction stream; the rare rows (crowded block / full scan / filter skipped) are redone by the
       // whole warp with the general routine.
@@ -611,7 +593,6 @@ __global__ void __launch_bounds__(320, 1) rvq_encode_kernel(const __grid_constan
             if ((rare >> (16 * hh)) & 1u) resolve_row_fullwarp(__shfl_sync(0xffffffffu, ent, 16 * hh));
         }
       }
-      if (threadIdx.x == 0) NS2_RVQ_STAMP(5);
     }
     if (p.stats != nullptr) {
       if (half == 0 && f0 + row < p.num_frames) atomicAdd(p.stats + 0, static_cast<unsigned long long>(p.Q));
@@ -622,10 +603,6 @@ __global__ void __launch_bounds__(320, 1) rvq_encode_kernel(const __grid_constan
       }
     }
   }
-
-  __syncthreads();
-  if (p.stats != nullptr && blockIdx.x == 0 && threadIdx.x < 256 && static_cast<int>(threadIdx.x) < p.Q * 8)
-    p.stats[4 + threadIdx.x] = tl_s[threadIdx.x];
 }
 
 // ------------------------------------------------------------------------------------------------

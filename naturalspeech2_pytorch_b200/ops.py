@@ -71,8 +71,7 @@ def gemm(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, n: int, epilogu
          resid: Optional[torch.Tensor] = None, film: Optional[torch.Tensor] = None,
          film_group_stride: int = 0, bias1_off: int = 0, groups: int = 1,
          a_group_col_stride: int = 0, b_group_row_stride: int = 0, out_group_col_stride: int = 0,
-         dil: Optional[Sequence[int]] = None, flags: int = 0,
-         debug_timeline: Optional[torch.Tensor] = None) -> torch.Tensor:
+         dil: Optional[Sequence[int]] = None, flags: int = 0) -> torch.Tensor:
     """out = epilogue(segmented_gemm(a, w)).  `a`: (batches, rows, cols) bf16 (may be a strided view),
     `w`: packed bf16 weight (rows, K).  See include/ns2_b200.h section 1 for the exact semantics."""
     lib = _lib.load()
@@ -125,7 +124,6 @@ def gemm(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, n: int, epilogu
     args.film = _ptr(film)
     args.film_group_stride = film_group_stride
     args.flags = int(flags)
-    args.debug_timeline = _ptr(debug_timeline)
     check(lib.ns2_gemm(C.byref(args), _stream(out)), "ns2_gemm")
     return out
 
@@ -211,12 +209,8 @@ def dropout_(x: torch.Tensor, *, dropout: Optional[DropoutSpec]) -> torch.Tensor
 # --------------------------------------------------------------------------------------------------
 # attention
 # --------------------------------------------------------------------------------------------------
-ATTN_AUTO, ATTN_ONE_TILE, ATTN_TWO_TILE, ATTN_TWO_TILE_POLY2, ATTN_TWO_TILE_POLY4, ATTN_TWO_TILE_LOCKSTEP = 0, 1, 2, 3, 4, 5
-
-
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tensor, *, heads: int,
-              scale: Optional[float] = None, kernel: int = ATTN_AUTO,
-              debug_timeline: Optional[torch.Tensor] = None, lse: Optional[torch.Tensor] = None,
+              scale: Optional[float] = None, lse: Optional[torch.Tensor] = None,
               dropout: Optional[DropoutSpec] = None) -> torch.Tensor:
     """q: (B, Nq, heads*64), k/v: (B, Nk, heads*64) bf16 (strided views into a fused projection are fine).
     dropout=(seed, site, p): attention dropout on the softmax probabilities (lse stays that of the undropped ones)."""
@@ -233,8 +227,6 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tens
     args.batches, args.heads = q.shape[0], heads
     args.q_len, args.kv_len, args.dim_head = q.shape[1], k.shape[1], 64
     args.scale = float(scale if scale is not None else 64 ** -0.5)
-    args.kernel = int(kernel)
-    args.debug_timeline = _ptr(debug_timeline)
     if lse is not None:
         _req(lse, torch.float32, "lse")
         if not lse.is_contiguous() or tuple(lse.shape) != (q.shape[0], heads, q.shape[1]):

@@ -39,6 +39,18 @@ def test_argument_validation_without_gpu(lib):
     a = GemmArgs()
     assert lib.ns2_gemm(ctypes.byref(a), None) < 0
     assert b"non-NULL" in lib.ns2_last_error()
+    # an otherwise valid call (dummy pointers, never dereferenced) with a flag bit the library does not define
+    a.A, a.B, a.out = 256, 512, 1024
+    a.a_batches, a.a_rows, a.a_cols, a.a_row_stride, a.a_batch_stride = 1, 128, 64, 64, 128 * 64
+    a.b_rows, a.b_cols, a.b_row_stride = 128, 64, 64
+    a.n, a.groups, a.num_segs, a.out_row_stride = 128, 1, 1, 128
+    a.segs[0].k_len = 64
+    before = lib.ns2_launch_count()
+    for flags in (2, 8):
+        a.flags = flags
+        assert lib.ns2_gemm(ctypes.byref(a), None) < 0
+        assert f"unknown flags 0x{flags:x}".encode() in lib.ns2_last_error()
+    assert lib.ns2_launch_count() == before
     t = AttnArgs()
     assert lib.ns2_attn_fwd(ctypes.byref(t), None) < 0
     assert lib.ns2_rvq_encode(None, 0, 128, None, None, None, None, 8, 1024, None, None, None) < 0

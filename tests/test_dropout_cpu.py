@@ -105,7 +105,7 @@ def test_dropout_struct_matches_header():
         subprocess.run(["gcc", "-I", str(ROOT / "include"), str(c), "-o", str(exe)], check=True)
         out = [int(v) for v in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
     assert out[:4] == [ctypes.sizeof(Dropout), Dropout.seed.offset, Dropout.site.offset, Dropout.p.offset]
-    assert out[4] == 6
+    assert out[4] == 7
 
 
 def test_train_dropout_defaults_off_and_conditioner_plumbs_it():

@@ -46,10 +46,13 @@ def _check_untouched(store, full, B, N, cols, what):
     assert_nan(store[B * N:], f"{what}: rows past the last batch")
 
 
-def _plain_case(B, N, K, n, *, flags=0, seed=0, check_f32=True):
+def _plain_case(B, N, K, n, *, flags=0, seed=0):
     from naturalspeech2_pytorch_b200 import ops
     g = _gen(seed)
-    a = (torch.randn(B, N, K, device=dev, generator=g) * 0.5).to(bf)
+    # a: columns [64, 64 + K) of a NaN-filled wider buffer, so a read outside the window (or past a K tail) shows
+    a_full = torch.full((B, N, K + 128), float("nan"), device=dev, dtype=bf)
+    a = a_full[..., 64:64 + K]
+    a.copy_(torch.randn(B, N, K, device=dev, generator=g) * 0.5)
     w = (torch.randn(n, K, device=dev, generator=g) / math.sqrt(K)).to(bf)
     bias = torch.randn(n, device=dev, generator=g)
     resid = torch.randn(B, N, n, device=dev, generator=g)
@@ -65,16 +68,13 @@ def _plain_case(B, N, K, n, *, flags=0, seed=0, check_f32=True):
     # bf16 out: 2^-8 |ref| output rounding + fp32 accumulation 2^-20 sqrt(K) sum|a||w| (kernel_check.acc_eps)
     assert_close(full[..., :n], post, U_BF16 * post.abs() + emag, U_BF16 + acc_eps(Kt[0]), "bf16")
     _check_untouched(store, full, B, N, n, "bf16")
-    out_bf = full[..., :n].clone()
-    if check_f32:
-        ref32 = post + resid.double()
-        store32, full32 = _out_buffer(B, N, n, 64, torch.float32)
-        ops.gemm(a, w, full32[..., :n], n=n, epilogue=ops.EPI_F32, bias=bias, resid=resid, flags=flags)
-        # fp32 out: 2^-23 |ref| rounding of the bias / residual adds + the same accumulation term
-        assert_close(full32[..., :n], ref32, U_F32 * (ref32.abs() + resid.double().abs()) + emag, acc_eps(Kt[0]) * 4,
-                     "f32+resid")
-        _check_untouched(store32, full32, B, N, n, "f32")
-    return a, w, bias, out_bf, post
+    ref32 = post + resid.double()
+    store32, full32 = _out_buffer(B, N, n, 64, torch.float32)
+    ops.gemm(a, w, full32[..., :n], n=n, epilogue=ops.EPI_F32, bias=bias, resid=resid, flags=flags)
+    # fp32 out: 2^-23 |ref| rounding of the bias / residual adds + the same accumulation term
+    assert_close(full32[..., :n], ref32, U_F32 * (ref32.abs() + resid.double().abs()) + emag, acc_eps(Kt[0]) * 4,
+                 "f32+resid")
+    _check_untouched(store32, full32, B, N, n, "f32")
 
 
 N_COLS = [
@@ -128,18 +128,6 @@ def test_gemm_silu_epilogue(n, N):
     _plain_case(2, N, 256, n, flags=4, seed=n + N)   # NS2_GEMM_FLAG_SILU, BF16 and F32 + resid
 
 
-@pytest.mark.parametrize("n", [
-    288,    # 1 wide + 1 narrow (32) n-tile per row block
-    1408,   # 5 wide + 1 narrow (128) n-tile per row block
-])
-def test_gemm_narrow_last_is_bit_identical(n):
-    from naturalspeech2_pytorch_b200 import ops
-    a, w, bias, out0, _ = _plain_case(3, 200, 192, n, flags=0, seed=n, check_f32=False)
-    out = torch.full_like(out0, float("nan"))
-    ops.gemm(a, w, out, n=n, epilogue=ops.EPI_BF16, bias=bias, flags=8)   # NS2_GEMM_FLAG_NARROW_LAST
-    assert torch.equal(out, out0)
-
-
 def test_gemm_sensitivity_drop_k_slice():
     """The bf16 and f32 tolerances reject a reference that misses one 16-wide K slice (one wgmma k-step)."""
     from naturalspeech2_pytorch_b200 import ops
@@ -183,16 +171,21 @@ def _conv_case(B, N, C, O, segs, dil, seed):
     return x, w, bias, full[..., :O].clone(), bound
 
 
-@pytest.mark.parametrize("N,dil", [
-    (300, 80),    # tap 0 shift 160: more than one 128-row tile
-    (300, 130),   # tap 0 shift 260, tap 1 shift 130: both cross a tile boundary
-    (100, 64),    # tap 0 shift 128 >= N: tap 0 reads only zero-filled rows
-    (100, 200),   # taps 0 and 1 (shifts 400, 200) both beyond the sequence
-    (65, 1),      # ordinary dil, warpgroup 2 holds one row
+@pytest.mark.parametrize("N,dil,dgrad", [
+    pytest.param(300, 80, False, id="300-80"),     # tap 0 shift 160: more than one 128-row tile
+    pytest.param(300, 130, False, id="300-130"),   # tap 0 shift 260, tap 1 shift 130: both cross a tile boundary
+    pytest.param(100, 64, False, id="100-64"),     # tap 0 shift 128 >= N: tap 0 reads only zero-filled rows
+    pytest.param(100, 200, False, id="100-200"),   # taps 0 and 1 (shifts 400, 200) both beyond the sequence
+    pytest.param(65, 1, False, id="65-1"),         # ordinary dil, warpgroup 2 holds one row
+    # the causal conv's input gradient (conv_dgrad_segs): shifts 0, -dil, -2 dil read rows after the output position
+    pytest.param(300, 4, True, id="dgrad-300-4"),      # the Wavenet backward's shape class
+    pytest.param(300, 130, True, id="dgrad-300-130"),  # taps 0 and 1 (shifts -260, -130) cross tile boundaries
+    pytest.param(100, 64, True, id="dgrad-100-64"),    # tap 0 shift -128: reaches past the sequence end, reads only zeros
 ])
-def test_gemm_conv3_long_shifts(N, dil):
+def test_gemm_conv3_long_shifts(N, dil, dgrad):
     from naturalspeech2_pytorch_b200 import ops
-    _conv_case(2, N, 128, 256, ops.conv3_segs(128), dil, seed=N + dil)
+    segs = ops.conv_dgrad_segs(128, 3, 2) if dgrad else ops.conv3_segs(128)
+    _conv_case(2, N, 128, 256, segs, dil, seed=N + dil + (7 if dgrad else 0))
 
 
 def test_gemm_conv_sensitivity_tap_shift():
@@ -338,6 +331,7 @@ def _wavenet(B, N, D, G, *, film_scale=1.0, seed=0, strided_film=False, tap_shif
     33,     # warpgroup 2 has no valid rows; dil >= 32 taps read only padding
     200,    # second tile: warpgroup 2 holds 8 rows
     1024,   # the benchmarked sequence length (8 row tiles)
+    4096,   # 192-512 tiles: persistent CTAs carry the ring and both accumulators across tiles
 ])
 def test_gemm_wavenet(G, D, N):
     store, full, ref, bound = _wavenet(2, N, D, G, seed=G * 10000 + N)

@@ -52,6 +52,7 @@ def _assert_increment(got, start, ref, mag, positions, what):
     32,     # BN=128, the only tile is 32 wide
     96,     # BN=128, the only tile is 96 wide
     224,    # BN=128, last tile 96 wide
+    512,    # BN=256 (k % 256 == 0), two full tiles
     1056,   # k > 1024 with k % 256 != 0: BN=256, last tile 32 wide
     1408,   # BN=256 (k > 1024), last tile 128 wide
 ])

@@ -2,8 +2,7 @@
 """Time the attention forward (and, with --bwd, the backward) with CUDA events, by default at the cfg2 shape
 (B=32, H=8, N=1024).  --dropout P runs the dropout kernels (Philox mask drawn in the forward, regenerated in the
 backward); --shape B,H,N another shape, e.g. 32,8,103 for the conditioning encoders' prompts.
-Usage: python tools/attn_bench.py [kernel_selector] [iters] [--dropout P] [--shape B,H,N] [--bwd]
-(every selector runs the same sm_90a kernel)"""
+Usage: python tools/attn_bench.py [iters] [--dropout P] [--shape B,H,N] [--bwd]"""
 import argparse
 import sys
 from pathlib import Path
@@ -13,13 +12,12 @@ import torch  # noqa: E402
 from naturalspeech2_pytorch_b200 import ops  # noqa: E402
 
 ap = argparse.ArgumentParser()
-ap.add_argument("kernel", nargs="?", type=int, default=ops.ATTN_AUTO)
 ap.add_argument("iters", nargs="?", type=int, default=5)
 ap.add_argument("--dropout", type=float, default=0.0)
 ap.add_argument("--shape", default="32,8,1024")
 ap.add_argument("--bwd", action="store_true")
 a = ap.parse_args()
-kern, iters = a.kernel, a.iters
+iters = a.iters
 B, H, N = (int(v) for v in a.shape.split(","))
 drop = (0x9E3779B97F4A7C15, 1, a.dropout) if a.dropout > 0 else None
 inner = H * 64
@@ -34,7 +32,7 @@ args = (qkv[:, :, :inner], qkv[:, :, inner:2 * inner], qkv[:, :, 2 * inner:], ou
 
 
 def fwd():
-    ops.attention(*args, heads=H, kernel=kern, lse=lse, dropout=drop)
+    ops.attention(*args, heads=H, lse=lse, dropout=drop)
 
 
 def bwd():
@@ -56,7 +54,7 @@ def timed(fn):
 tag = f"B{B} H{H} N{N} dropout {a.dropout:g}"
 us = timed(fwd)
 flops = 4.0 * B * H * N * N * 64
-print(f"kernel {kern} {tag}: {us:.1f} us/launch = {flops / us / 1e6:.0f} TFLOP/s (x12 layers = {us * 12 / 1e3:.3f} ms/step)")
+print(f"forward {tag}: {us:.1f} us/launch = {flops / us / 1e6:.0f} TFLOP/s (x12 layers = {us * 12 / 1e3:.3f} ms/step)")
 if a.bwd:
     fwd()
     us = timed(bwd)

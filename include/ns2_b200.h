@@ -431,6 +431,46 @@ int64_t ns2_maximum_path_workspace_bytes(int32_t batch, int32_t t_x, int32_t t_y
 int ns2_maximum_path(const float* value, const float* mask, int32_t batch, int32_t t_x, int32_t t_y, float neg_const,
                      void* workspace, int64_t workspace_bytes, int32_t* idx, float* path, ns2_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * 10. Encodec's SEANet decoder, 24 kHz model (`codec.decode(audio)`, ns2.py:1496-1499, reached through
+ *     audiolm_pytorch.EncodecWrapper.decode -> encodec SEANetDecoder; transformers' EncodecDecoder has the same
+ *     layers).  Convolutions with >= 64 channels, the transposed convolutions and the LSTM input projections are
+ *     ns2_gemm calls; these three entry points cover the rest.  Activations are token-major (batch, time, channel).
+ *    ns2_lstm_seq    : one layer of nn.LSTM(512, 512) over `steps` time steps with zero initial state (the decoder's
+ *                      SLSTM: encodec/modules/lstm.py, transformers EncodecLSTM), gate order i, f, g, o:
+ *                        gates = xproj[b, t, :] + W_hh h_{t-1};  c = f c + i g;  h_t = o tanh(c)
+ *                      xproj (batch, steps, 2048) f32 = x W_ih^T + b_ih + b_hh with its columns (and W_hh's rows)
+ *                      permuted to the kernel's order: column 128 c + 64 hf + 16 w + 8 i + q holds gate 2 hf + i of
+ *                      hidden unit 32 c + 8 w + q.  w_hh: those 2048 permuted rows x 512, bf16.  h_{t-1} enters the
+ *                      recurrence as bf16.  Writes out[b, t, :] = h_t (+ skip[b, t, :] when skip != NULL: the
+ *                      `lstm(x)[0] + x` of SLSTM) as f32 and/or bf16 (either may be NULL).  hidden must be 512.  One
+ *                      16-CTA cluster per 64 batch rows (needs a device that can hold such a cluster, else an error).
+ *    ns2_elu_pad     : out_bf16[b, r, 0:C] = bf16(act(xpad[b, r - pad])), r in [0, pad + length), act = ELU
+ *                      (nn.ELU, alpha 1) with NS2_ELU_PAD_ELU else identity; xpad is x reflect-padded on the left by
+ *                      `pad` (StreamableConv1d / EncodecConv1d causal padding, with their rule for inputs no longer
+ *                      than the pad: zeros are appended before reflecting).  NS2_ELU_PAD_RAW also writes bf16(xpad) in
+ *                      columns [C, 2C) (the un-activated input of a ResnetBlock shortcut).  C % 4 == 0.
+ *    ns2_seanet_tail : the decoder's last 32-channel stage at the sample rate, f32 throughout:
+ *                        z = shortcut(x) + conv1x1(ELU(conv3(ELU(x))))   (SEANetResnetBlock 32 -> 16 -> 32)
+ *                        out[b, t] = conv7(ELU(z))[t]                    (final StreamableConv1d 32 -> 1)
+ *                      causal, reflect-padded like ns2_elu_pad.  x: (batch, length, 32) f32.  params:
+ *                      NS2_SEANET_TAIL_PARAMS f32 (weight norm folded):  w3 [tap 3][in 32][out 16], b3 [16],
+ *                      w_shortcut [in 32][out 32], w_conv1 [in 16][out 32], b_shortcut + b_conv1 [32],
+ *                      w_final [tap 7][in 32], b_final, 3 zeros.
+ * ------------------------------------------------------------------------------------------------ */
+#define NS2_ELU_PAD_ELU 1
+#define NS2_ELU_PAD_RAW 2
+#define NS2_SEANET_TAIL_PARAMS 3348
+int ns2_lstm_seq(const float* xproj, int64_t xp_row_stride, int64_t xp_batch_stride, const void* w_hh, int32_t batch,
+                 int32_t steps, int32_t hidden, const float* skip, int64_t skip_row_stride, int64_t skip_batch_stride,
+                 float* out, int64_t out_row_stride, int64_t out_batch_stride, void* out_bf16, int64_t outbf_row_stride,
+                 int64_t outbf_batch_stride, ns2_stream_t stream);
+int ns2_elu_pad(const float* x, int64_t x_row_stride, int64_t x_batch_stride, int32_t batch, int32_t length,
+                int32_t channels, int32_t pad, int32_t flags, void* out_bf16, int64_t out_row_stride,
+                int64_t out_batch_stride, ns2_stream_t stream);
+int ns2_seanet_tail(const float* x, int64_t x_row_stride, int64_t x_batch_stride, int32_t batch, int32_t length,
+                    const float* params, float* out, int64_t out_batch_stride, ns2_stream_t stream);
+
 /* Number of kernel launches issued through this library since load (for bench.py's gpu_launches). */
 int64_t ns2_launch_count(void);
 

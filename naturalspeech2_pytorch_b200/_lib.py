@@ -17,6 +17,8 @@ NS2_MSE_SCRATCH_PER_SAMPLE = 64
 NS2_RVQ_STATS_LEN = 4
 NS2_OBJ_V, NS2_OBJ_EPS, NS2_OBJ_X0 = 0, 1, 2
 NS2_GEMM_FLAG_SKIP_EPILOGUE, NS2_GEMM_FLAG_SILU = 1, 4
+NS2_ELU_PAD_ELU, NS2_ELU_PAD_RAW = 1, 2
+NS2_SEANET_TAIL_PARAMS = 3348
 NS2_ABI_VERSION = 7
 
 
@@ -135,6 +137,10 @@ SIGNATURES = {
     "ns2_maximum_path": (C.c_int, [_P, _P, _I32, _I32, _I32, _F, _P, _I64, _P, _P, _P]),
     "ns2_rvq_ce": (C.c_int, [_P, _I64, _I32, _P, _P, _I32, _I32, _P, _P, _P, _P, _P]),
     "ns2_rvq_ce_bwd": (C.c_int, [_P, _I64, _I32, _P, _P, _I32, _I32, _P, _P, _P, _P, _I64, _P, _P, _I64, _P]),
+    "ns2_lstm_seq": (C.c_int, [_P, _I64, _I64, _P, _I32, _I32, _I32, _P, _I64, _I64, _P, _I64, _I64, _P, _I64, _I64,
+                               _P]),
+    "ns2_elu_pad": (C.c_int, [_P, _I64, _I64, _I32, _I32, _I32, _I32, _I32, _P, _I64, _I64, _P]),
+    "ns2_seanet_tail": (C.c_int, [_P, _I64, _I64, _I32, _I32, _P, _P, _I64, _P]),
 }
 
 _lib = None

@@ -3,10 +3,10 @@
 
 In scope (SURVEY a16): nearest-codeword search over Q sequential residual stages (`ops.rvq_encode`, wgmma
 distance filter + exact fp64 re-score => bit-exact indices) and the sum-of-codewords decode (`ops.rvq_decode`).
-Out of scope: Encodec's SEANet conv/LSTM encoder and decoder (pretrained weights are not available offline and
-the north star does not name them).  They plug in as callables:
+Encodec's SEANet encoder and decoder plug in as callables:
     encoder(raw_audio (B, T)) -> frames (B, N, 128)        decoder(emb (B, N, 128)) -> audio (B, 1, T)
-Without an encoder the codec accepts encoder-output frames (B, N, 128) directly.
+`seanet.SEANetDecoder` is the 24 kHz decoder on this library's kernels; the encoder is not built.  Without an encoder
+the codec accepts encoder-output frames (B, N, 128) directly; without a decoder `decode` returns the latents.
 """
 from __future__ import annotations
 

@@ -906,3 +906,77 @@ def maximum_path(value: torch.Tensor, mask: torch.Tensor, neg_const: float = flo
     check(lib.ns2_maximum_path(value.data_ptr(), mask.data_ptr(), b, t_x, t_y, float(neg_const), ws.data_ptr(),
                                ws_bytes, idx.data_ptr(), _ptr(path), _stream(value)), "ns2_maximum_path")
     return idx, path
+
+
+# --------------------------------------------------------------------------------------------------
+# SEANet decoder (Encodec 24 kHz): LSTM recurrence, conv operand preparation, 32-channel tail
+# --------------------------------------------------------------------------------------------------
+def _rows3(t: torch.Tensor, name: str, cols: int) -> Tuple[int, int]:
+    """(row stride, batch stride) of a (B, T, >= cols) view with unit channel stride."""
+    if t.dim() != 3 or t.shape[2] < cols or (t.shape[2] > 1 and t.stride(2) != 1):
+        raise ValueError(f"{name} must be a (B, T, >= {cols}) view with unit channel stride, got {tuple(t.shape)}")
+    return t.stride(1), t.stride(0)
+
+
+def lstm_seq(xproj: torch.Tensor, w_hh: torch.Tensor, *, skip: Optional[torch.Tensor] = None,
+             out: Optional[torch.Tensor] = None, out_bf16: Optional[torch.Tensor] = None) -> None:
+    """One nn.LSTM(512, 512) layer over the sequence: xproj (B, T, 2048) f32 holds x W_ih^T + b_ih + b_hh in the
+    kernel's gate order (see include/ns2_b200.h section 10), w_hh (2048, 512) bf16 in the same row order.
+    Writes h_t (+ skip) into out (B, T, 512) f32 and/or out_bf16 (B, T, 512) bf16; all may be strided views."""
+    lib = _lib.load()
+    _req(xproj, torch.float32, "xproj")
+    _req(w_hh, torch.bfloat16, "w_hh")
+    if tuple(w_hh.shape) != (2048, 512) or not w_hh.is_contiguous():
+        raise ValueError("w_hh must be a contiguous (2048, 512) bf16 tensor")
+    if out is None and out_bf16 is None:
+        raise ValueError("lstm_seq needs out and/or out_bf16")
+    B, T = xproj.shape[:2]
+    xrs, xbs = _rows3(xproj, "xproj", 2048)
+    strides = {}
+    for name, t, dt in (("skip", skip, torch.float32), ("out", out, torch.float32), ("out_bf16", out_bf16, torch.bfloat16)):
+        if t is None:
+            strides[name] = (0, 0)
+            continue
+        _req(t, dt, name)
+        if t.shape[:2] != (B, T):
+            raise ValueError(f"{name} must be (B, T, 512) like xproj's (B, T)")
+        strides[name] = _rows3(t, name, 512)
+    check(lib.ns2_lstm_seq(xproj.data_ptr(), xrs, xbs, w_hh.data_ptr(), B, T, 512, _ptr(skip), *strides["skip"],
+                           _ptr(out), *strides["out"], _ptr(out_bf16), *strides["out_bf16"], _stream(xproj)),
+          "ns2_lstm_seq")
+
+
+def elu_pad(x: torch.Tensor, out: torch.Tensor, *, pad: int, elu: bool = True, raw: bool = False) -> torch.Tensor:
+    """out[:, r, :C] = bf16(ELU(xpad[:, r - pad])) for r < pad + T (ELU only with elu=True), xpad = x reflect-padded
+    on the left (Encodec's causal padding); raw=True also writes bf16(xpad) in columns [C, 2C).  x (B, T, C) f32 and
+    out (B, pad + T, >= C or 2C) bf16 may be row-strided views (e.g. a GEMM output past its scratch rows)."""
+    lib = _lib.load()
+    _req(x, torch.float32, "x")
+    _req(out, torch.bfloat16, "out")
+    B, T, Cc = x.shape
+    xrs, xbs = _rows3(x, "x", Cc)
+    ors, obs = _rows3(out, "out", Cc * (2 if raw else 1))
+    if out.shape[0] != B or out.shape[1] != pad + T:
+        raise ValueError(f"out must have {pad + T} rows per batch element, got {tuple(out.shape)}")
+    flags = (_lib.NS2_ELU_PAD_ELU if elu else 0) | (_lib.NS2_ELU_PAD_RAW if raw else 0)
+    check(lib.ns2_elu_pad(x.data_ptr(), xrs, xbs, B, T, Cc, int(pad), flags, out.data_ptr(), ors, obs, _stream(out)),
+          "ns2_elu_pad")
+    return out
+
+
+def seanet_tail(x: torch.Tensor, params: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """out (B, T) f32 = conv7(ELU(ResnetBlock(x))) for x (B, T, 32) f32 (row-strided view allowed); params: the
+    NS2_SEANET_TAIL_PARAMS packed f32 weights (SEANetDecoder packs them)."""
+    lib = _lib.load()
+    _req(x, torch.float32, "x")
+    _req(out, torch.float32, "out")
+    _req_flat(params, torch.float32, "params", _lib.NS2_SEANET_TAIL_PARAMS)
+    B, T, Cc = x.shape
+    if Cc != 32:
+        raise ValueError("seanet_tail takes 32 channels")
+    xrs, xbs = _rows3(x, "x", 32)
+    if out.dim() != 2 or tuple(out.shape) != (B, T) or (T > 1 and out.stride(1) != 1):
+        raise ValueError("out must be (B, T) with unit time stride")
+    check(lib.ns2_seanet_tail(x.data_ptr(), xrs, xbs, B, T, params.data_ptr(), out.data_ptr(), out.stride(0),
+                              _stream(out)), "ns2_seanet_tail")
+    return out

@@ -1,0 +1,271 @@
+"""`SEANetDecoder`: Encodec's 24 kHz SEANet decoder on sm_90a, the `decoder` of `EncodecRVQ` — what
+`codec.decode(audio)` runs at the end of `NaturalSpeech2.sample` (ns2.py:1496-1499) to turn 75 Hz latents into 24 kHz
+audio.
+
+Layers (token-major activations (B, time, channels); every conv causal with reflect left padding, weight norm folded):
+    0       Conv1d k7 128 -> 512                      elu_pad (pad 6) + 7-segment GEMM
+    1       2-layer LSTM(512), lstm(x)[0] + x         input projection GEMM + ns2_lstm_seq per layer
+    2-3     ELU, ConvTranspose1d k16 s8 512 -> 256    elu_pad + 2-segment GEMM (taps [0, s) shift 0, [s, 2s) shift 1)
+    4       ResnetBlock(256, hidden 128)              elu_pad (ELU | raw, pad 2) + 3-segment GEMM, elu_pad, one GEMM
+                                                      for conv1x1 + shortcut over [ELU(x) | x | ELU(h)]
+    5-10    the same at 256 -> 128 (k10 s5) and 128 -> 64 (k8 s4)
+    11-12   ELU, ConvTranspose1d k4 s2 64 -> 32       elu_pad + 2-segment GEMM
+    13-15   ResnetBlock(32, hidden 16), ELU, Conv1d k7 32 -> 1      ns2_seanet_tail (fp32)
+GEMM operands are bf16 with fp32 accumulation; activations between layers, the LSTM cell state and the tail stay fp32.
+The state_dict has the keys and shapes of transformers' `EncodecDecoder`; `load_encodec_state_dict` takes Meta
+`encodec` (and audiolm's `EncodecWrapper.model.decoder`) keys.  Inference only: there is no backward.
+"""
+from __future__ import annotations
+
+import re
+from collections import OrderedDict
+from typing import Dict, Sequence
+
+import torch
+from torch import nn
+
+from . import _lib, ops
+from .model import _PackedCache
+
+RATIOS = (8, 5, 4, 2)
+
+# the 24 kHz Encodec model's decoder configuration (transformers EncodecConfig() defaults); nothing else is built
+SUPPORTED = dict(audio_channels=1, num_filters=32, upsampling_ratios=(8, 5, 4, 2), hidden_size=128, kernel_size=7,
+                 last_kernel_size=7, residual_kernel_size=3, dilation_growth_rate=2, num_residual_layers=1,
+                 compress=2, num_lstm_layers=2, use_causal_conv=True, pad_mode="reflect", norm_type="weight_norm",
+                 trim_right_ratio=1.0, use_conv_shortcut=True)
+
+
+def lstm_gate_perm() -> torch.Tensor:
+    """Row order of the packed LSTM weights (include/ns2_b200.h section 10): packed row 128 c + 64 hf + 16 w + 8 i + q
+    is PyTorch row (2 hf + i) * 512 + 32 c + 8 w + q (gate 2 hf + i of hidden unit 32 c + 8 w + q)."""
+    c, hf, w, i, q = torch.meshgrid(*(torch.arange(n) for n in (16, 2, 4, 2, 8)), indexing="ij")
+    return ((2 * hf + i) * 512 + 32 * c + 8 * w + q).reshape(-1)
+
+
+def fold_weight_norm(g: torch.Tensor, v: torch.Tensor) -> torch.Tensor:
+    """w = g v / ||v||, the norm over every dim but 0 (output channels of a Conv1d, input channels of a
+    ConvTranspose1d) - torch.nn.utils.parametrizations.weight_norm(dim=0)."""
+    return g * v / v.norm(dim=tuple(range(1, v.dim())), keepdim=True)
+
+
+def pack_conv_transpose(w: torch.Tensor, b: torch.Tensor, s: int):
+    """ConvTranspose1d(k = 2s, stride s) weight (C_in, C_out, 2s) and bias -> the 2-segment GEMM's bf16 pack
+    (s C_out, 2 C_in) and f32 bias: packed row r C_out + co, column j C_in + ci = w[ci, co, j s + r], so output frame
+    n, columns [r C_out, (r + 1) C_out) is output sample s n + r (segment j reads input frame n - j)."""
+    c_in, c_out = w.shape[0], w.shape[1]
+    packed = w.reshape(c_in, c_out, 2, s).permute(3, 1, 2, 0).reshape(s * c_out, 2 * c_in)
+    return packed.to(torch.bfloat16).contiguous(), b.float().repeat(s).contiguous()
+
+
+def pack_tail(w3, b3, w1, b1, w_sc, b_sc, w_f, b_f) -> torch.Tensor:
+    """Folded weights of the 32-channel ResnetBlock (conv3 (16, 32, 3), conv1x1 (32, 16, 1), shortcut (32, 32, 1)) and
+    of the final conv (1, 32, 7) -> the NS2_SEANET_TAIL_PARAMS f32 layout of ns2_seanet_tail."""
+    p = torch.cat([w3.permute(2, 1, 0).reshape(-1), b3, w_sc[:, :, 0].t().reshape(-1), w1[:, :, 0].t().reshape(-1),
+                   b_sc + b1, w_f[0].t().reshape(-1), b_f.reshape(1), b_f.new_zeros(3)])
+    assert p.numel() == _lib.NS2_SEANET_TAIL_PARAMS
+    return p.float().contiguous()
+
+
+class _WNConv(nn.Module):
+    """Parameter holder of EncodecConv1d / EncodecConvTranspose1d: `conv` is the weight-normed torch module."""
+
+    def __init__(self, c_in: int, c_out: int, kernel: int, stride: int = 1, transposed: bool = False):
+        super().__init__()
+        conv = nn.ConvTranspose1d(c_in, c_out, kernel, stride) if transposed else nn.Conv1d(c_in, c_out, kernel)
+        self.conv = nn.utils.parametrizations.weight_norm(conv)
+
+    def folded(self):
+        p = self.conv.parametrizations.weight
+        return fold_weight_norm(p.original0.float(), p.original1.float()), self.conv.bias.float()
+
+
+class _LSTMParams(nn.Module):
+    """Parameter holder of EncodecLSTM."""
+
+    def __init__(self, dim: int, layers: int):
+        super().__init__()
+        self.lstm = nn.LSTM(dim, dim, layers)
+
+
+class _ResnetParams(nn.Module):
+    """Parameter holder of EncodecResnetBlock: block = [ELU, conv k3 dim -> hidden, ELU, conv k1 hidden -> dim]."""
+
+    def __init__(self, dim: int, hidden: int, kernel: int):
+        super().__init__()
+        self.block = nn.ModuleList([nn.ELU(), _WNConv(dim, hidden, kernel), nn.ELU(), _WNConv(hidden, dim, 1)])
+        self.shortcut = _WNConv(dim, dim, 1)
+
+
+class SEANetDecoder(_PackedCache):
+    """Encodec's SEANet decoder (24 kHz model): (B, N, 128) summed codewords -> (B, 1, 320 N) audio, fp32.
+
+    The constructor takes transformers' `EncodecConfig` decoder fields; only the 24 kHz model's values are supported
+    (`SEANetDecoder.from_config(EncodecConfig())` or no arguments)."""
+
+    def __init__(self, *, audio_channels: int = 1, num_filters: int = 32, upsampling_ratios: Sequence[int] = RATIOS,
+                 hidden_size: int = 128, kernel_size: int = 7, last_kernel_size: int = 7, residual_kernel_size: int = 3,
+                 dilation_growth_rate: int = 2, num_residual_layers: int = 1, compress: int = 2,
+                 num_lstm_layers: int = 2, use_causal_conv: bool = True, pad_mode: str = "reflect",
+                 norm_type: str = "weight_norm", trim_right_ratio: float = 1.0, use_conv_shortcut: bool = True):
+        super().__init__()
+        given = dict(audio_channels=audio_channels, num_filters=num_filters,
+                     upsampling_ratios=tuple(int(r) for r in upsampling_ratios), hidden_size=hidden_size,
+                     kernel_size=kernel_size, last_kernel_size=last_kernel_size,
+                     residual_kernel_size=residual_kernel_size, dilation_growth_rate=dilation_growth_rate,
+                     num_residual_layers=num_residual_layers, compress=compress, num_lstm_layers=num_lstm_layers,
+                     use_causal_conv=bool(use_causal_conv), pad_mode=pad_mode, norm_type=norm_type,
+                     trim_right_ratio=float(trim_right_ratio), use_conv_shortcut=bool(use_conv_shortcut))
+        bad = {k: v for k, v in given.items() if v != SUPPORTED[k]}
+        if bad:
+            raise ValueError(f"SEANetDecoder supports only the 24 kHz Encodec decoder configuration; unsupported: {bad} "
+                             f"(expected {({k: SUPPORTED[k] for k in bad})})")
+        scale = 2 ** len(RATIOS)
+        layers = [_WNConv(hidden_size, scale * num_filters, kernel_size), _LSTMParams(scale * num_filters, num_lstm_layers)]
+        for r in RATIOS:
+            dim = scale * num_filters
+            layers += [nn.ELU(), _WNConv(dim, dim // 2, 2 * r, stride=r, transposed=True),
+                       _ResnetParams(dim // 2, dim // 2 // compress, residual_kernel_size)]
+            scale //= 2
+        layers += [nn.ELU(), _WNConv(num_filters, audio_channels, last_kernel_size)]
+        self.layers = nn.ModuleList(layers)
+        self._ws: "OrderedDict[tuple, Dict[str, torch.Tensor]]" = OrderedDict()
+        self.max_cached_shapes = 4  # LRU bound on per-(B, N) workspaces (~10 GB at (32, 1024))
+
+    @classmethod
+    def from_config(cls, config) -> "SEANetDecoder":
+        """From an object with transformers' `EncodecConfig` attribute names."""
+        return cls(**{k: getattr(config, k) for k in SUPPORTED})
+
+    def load_encodec_state_dict(self, sd: Dict[str, torch.Tensor], strict: bool = True):
+        """Load a Meta `encodec` SEANetDecoder state_dict (`EncodecModel.decoder`, also audiolm's
+        `EncodecWrapper.model.decoder`): `model.{i}.conv.conv.weight_g|weight_v|bias`, `model.{i}.convtr.convtr.*`,
+        `model.{i}.block.{j}.conv.conv.*`, `model.{i}.shortcut.conv.conv.*`, `model.1.lstm.*`.  A `decoder.` prefix
+        is stripped.  The mapping follows the upstream module layout; it has not been checked against a released
+        checkpoint, so load with strict=True and compare a decoded clip against the original decoder once."""
+        out = {}
+        for k, v in sd.items():
+            k = k[len("decoder."):] if k.startswith("decoder.") else k
+            m = re.fullmatch(r"model\.(\d+)\.(.*)", k)
+            if m is None:
+                raise KeyError(f"unexpected key {k!r} in an encodec decoder state_dict")
+            i, rest = m.group(1), m.group(2)
+            rest = re.sub(r"^(conv\.conv|convtr\.convtr)\.", "conv.", rest)
+            rest = re.sub(r"^(block\.\d+|shortcut)\.conv\.conv\.", r"\1.conv.", rest)
+            rest = re.sub(r"conv\.weight_g$", "conv.parametrizations.weight.original0", rest)
+            rest = re.sub(r"conv\.weight_v$", "conv.parametrizations.weight.original1", rest)
+            out[f"layers.{i}.{rest}"] = v
+        return self.load_state_dict(out, strict=strict)
+
+    @property
+    def device(self):
+        return next(self.parameters()).device
+
+    def _apply(self, fn, *args, **kwargs):
+        out = super()._apply(fn, *args, **kwargs)
+        self._ws.clear()
+        return out
+
+    # ----------------------------------------------------------------------------------------------
+    # weight packing (folded weight norm, bf16, K-major; rebuilt when a parameter changes)
+    # ----------------------------------------------------------------------------------------------
+    def _pack(self) -> Dict[str, torch.Tensor]:
+        bf = lambda t: t.to(torch.bfloat16).contiguous()
+        f32 = lambda t: t.float().contiguous()
+        P = {}
+        w, b = self.layers[0].folded()                              # (512, 128, 7)
+        P["c0_w"], P["c0_b"] = bf(w.permute(0, 2, 1).reshape(w.shape[0], -1)), f32(b)
+        lstm = self.layers[1].lstm
+        perm = lstm_gate_perm().to(w.device)
+        for l in range(2):
+            P[f"l{l}_wih"] = bf(getattr(lstm, f"weight_ih_l{l}")[perm])
+            P[f"l{l}_whh"] = bf(getattr(lstm, f"weight_hh_l{l}")[perm])
+            P[f"l{l}_b"] = f32((getattr(lstm, f"bias_ih_l{l}") + getattr(lstm, f"bias_hh_l{l}"))[perm])
+        for si, s in enumerate(RATIOS):
+            P[f"t{si}_w"], P[f"t{si}_b"] = pack_conv_transpose(*self.layers[3 + 3 * si].folded(), s)
+            blk = self.layers[4 + 3 * si]
+            w3, b3 = blk.block[1].folded()                          # (H, D, 3)
+            w1, b1 = blk.block[3].folded()                          # (D, H, 1)
+            ws, bs = blk.shortcut.folded()                          # (D, D, 1)
+            if si < len(RATIOS) - 1:
+                P[f"r{si}_w3"], P[f"r{si}_b3"] = bf(w3.permute(0, 2, 1).reshape(w3.shape[0], -1)), f32(b3)
+                P[f"r{si}_w1"] = bf(torch.cat([ws[:, :, 0], w1[:, :, 0]], dim=1))
+                P[f"r{si}_b1"] = f32(bs + b1)
+            else:
+                P["tail"] = pack_tail(w3, b3, w1, b1, ws, bs, *self.layers[15].folded())
+        return P
+
+    # ----------------------------------------------------------------------------------------------
+    # workspaces (per (B, N) shape, LRU-bounded)
+    # ----------------------------------------------------------------------------------------------
+    def _workspace(self, B: int, N: int, dev) -> Dict[str, torch.Tensor]:
+        key = (B, N, str(dev))
+        ws = self._ws.get(key)
+        if ws is not None:
+            self._ws.move_to_end(key)
+            return ws
+        while len(self._ws) >= self.max_cached_shapes:
+            self._ws.popitem(last=False)
+        e = lambda *s, dt=torch.bfloat16: torch.empty(*s, device=dev, dtype=dt)
+        f = torch.float32
+        ws = {"a0": e(B, N + 6, 128), "y0": e(B, N + 6, 512, dt=f), "xb": e(B, N, 512), "xp": e(B, N, 2048, dt=f),
+              "z": e(B, N, 512, dt=f)}
+        L = N
+        for si, s in enumerate(RATIOS):
+            c_in = 512 >> si
+            c_out, h = c_in // 2, c_in // 4
+            ws[f"at{si}"] = e(B, L, c_in)
+            ws[f"u{si}"] = e(B, L, s * c_out, dt=f)
+            L *= s
+            if si < len(RATIOS) - 1:
+                ws[f"blk{si}"] = e(B, L + 2, 2 * c_out + h)
+                ws[f"h{si}"] = e(B, L + 2, h, dt=f)
+                ws[f"z{si}"] = e(B, L + 2, c_out, dt=f)
+        self._ws[key] = ws
+        return ws
+
+    # ----------------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def forward(self, emb: torch.Tensor) -> torch.Tensor:
+        """emb (B, N, 128) -> audio (B, 1, 320 N) fp32."""
+        if emb.dim() != 3 or emb.shape[-1] != 128:
+            raise ValueError(f"SEANetDecoder takes (B, N, 128) latents, got {tuple(emb.shape)}")
+        B, N, _ = emb.shape
+        dev = emb.device
+        out = torch.empty(B, 1, 320 * N, device=dev, dtype=torch.float32)
+        if B == 0 or N == 0:
+            return out
+        with torch.cuda.device(dev):
+            P, ws = self.packed(), self._workspace(B, N, dev)
+            x = emb.float().contiguous()
+            ops.elu_pad(x, ws["a0"], pad=6, elu=False)
+            ops.gemm(ws["a0"], P["c0_w"], ws["y0"], n=512, epilogue=ops.EPI_F32, segs=ops.conv_segs(128, 7, 6),
+                     bias=P["c0_b"])
+            y0 = ws["y0"][:, 6:]
+            ops.elu_pad(y0, ws["xb"], pad=0, elu=False)
+            ops.gemm(ws["xb"], P["l0_wih"], ws["xp"], n=2048, epilogue=ops.EPI_F32, bias=P["l0_b"])
+            ops.lstm_seq(ws["xp"], P["l0_whh"], out_bf16=ws["xb"])
+            ops.gemm(ws["xb"], P["l1_wih"], ws["xp"], n=2048, epilogue=ops.EPI_F32, bias=P["l1_b"])
+            ops.lstm_seq(ws["xp"], P["l1_whh"], skip=y0, out=ws["z"])
+            z, L = ws["z"], N
+            for si, s in enumerate(RATIOS):
+                c_in = 512 >> si
+                c_out, h = c_in // 2, c_in // 4
+                at, u = ws[f"at{si}"], ws[f"u{si}"]
+                ops.elu_pad(z, at, pad=0, elu=True)
+                ops.gemm(at, P[f"t{si}_w"], u, n=s * c_out, epilogue=ops.EPI_F32,
+                         segs=[(0, 0, c_in, 0, 0), (0, c_in, c_in, 1, 0)], bias=P[f"t{si}_b"])
+                L *= s
+                u = u.view(B, L, c_out)
+                if si == len(RATIOS) - 1:
+                    ops.seanet_tail(u, P["tail"], out.view(B, L))
+                    break
+                blk, hb, zo = ws[f"blk{si}"], ws[f"h{si}"], ws[f"z{si}"]
+                ops.elu_pad(u, blk, pad=2, elu=True, raw=True)          # [ELU(x) | x], reflect-padded by 2
+                ops.gemm(blk, P[f"r{si}_w3"], hb, n=h, epilogue=ops.EPI_F32, segs=ops.conv_segs(c_out, 3, 2),
+                         bias=P[f"r{si}_b3"])
+                ops.elu_pad(hb[:, 2:], blk[:, 2:, 2 * c_out:], pad=0, elu=True)
+                ops.gemm(blk, P[f"r{si}_w1"], zo, n=c_out, epilogue=ops.EPI_F32,
+                         segs=[(c_out, 0, c_out, 0, 0), (2 * c_out, c_out, h, 0, 0)], bias=P[f"r{si}_b1"])
+                z = zo[:, 2:]
+        return out

@@ -434,8 +434,9 @@ int ns2_maximum_path(const float* value, const float* mask, int32_t batch, int32
 /* ------------------------------------------------------------------------------------------------
  * 10. Encodec's SEANet decoder, 24 kHz model (`codec.decode(audio)`, ns2.py:1496-1499, reached through
  *     audiolm_pytorch.EncodecWrapper.decode -> encodec SEANetDecoder; transformers' EncodecDecoder has the same
- *     layers).  Convolutions with >= 64 channels, the transposed convolutions and the LSTM input projections are
- *     ns2_gemm calls; these three entry points cover the rest.  Activations are token-major (batch, time, channel).
+ *     layers), and its SEANet encoder (`codec(raw_audio)`, transformers' EncodecEncoder).  Convolutions with >= 64
+ *     channels, the transposed and strided convolutions and the LSTM input projections are ns2_gemm calls; these
+ *     four entry points cover the rest.  Activations are token-major (batch, time, channel).
  *    ns2_lstm_seq    : one layer of nn.LSTM(512, 512) over `steps` time steps with zero initial state (the decoder's
  *                      SLSTM: encodec/modules/lstm.py, transformers EncodecLSTM), gate order i, f, g, o:
  *                        gates = xproj[b, t, :] + W_hh h_{t-1};  c = f c + i g;  h_t = o tanh(c)
@@ -457,10 +458,26 @@ int ns2_maximum_path(const float* value, const float* mask, int32_t batch, int32
  *                      NS2_SEANET_TAIL_PARAMS f32 (weight norm folded):  w3 [tap 3][in 32][out 16], b3 [16],
  *                      w_shortcut [in 32][out 32], w_conv1 [in 16][out 32], b_shortcut + b_conv1 [32],
  *                      w_final [tap 7][in 32], b_final, 3 zeros.
+ *    ns2_seanet_head : the encoder's first 32-channel stage at the sample rate (transformers EncodecEncoder layers
+ *                      0-2), f32 throughout, bf16 output:
+ *                        z0 = conv7(x)                                    (StreamableConv1d 1 -> 32)
+ *                        z1 = shortcut(z0) + conv1x1(ELU(conv3(ELU(z0)))) (SEANetResnetBlock 32 -> 16 -> 32)
+ *                        out_bf16[b, r, 0:32] = bf16(ELU(z1pad[b, r - 2])), r in [0, length + 2)
+ *                      causal, reflect-padded like ns2_elu_pad; z1pad is z1 reflect-padded by 2, so `out` is
+ *                      ns2_elu_pad(z1, pad = 2) and directly the A operand of the encoder's k4 stride-2 conv.
+ *                      x: (batch, length) f32 with batch stride x_batch_stride.  out: 16-byte aligned, row and batch
+ *                      strides multiples of 8.  params: NS2_SEANET_HEAD_PARAMS f32 (weight norm folded):
+ *                      w0 [tap 7][out 32], b0 [32], w3 [tap 3][in 32][out 16], b3 [16], w_shortcut [in 32][out 32],
+ *                      w_conv1 [in 16][out 32], b_shortcut + b_conv1 [32].
+ *    The encoder's strided convs (k = 2s, stride s, reflect left pad s) are 2-segment ns2_gemm calls: ns2_elu_pad
+ *    (pad = s) writes a contiguous (batch, L + s, C) buffer, viewed as (batch, L/s + 1, s C) rows; the weight packed
+ *    tap-major (C_out, 2 s C); segments {a 0, b 0, k sC, shift 1}, {a 0, b sC, k sC, shift 0}; output row m + 1 is
+ *    conv output m (row 0 is scratch).
  * ------------------------------------------------------------------------------------------------ */
 #define NS2_ELU_PAD_ELU 1
 #define NS2_ELU_PAD_RAW 2
 #define NS2_SEANET_TAIL_PARAMS 3348
+#define NS2_SEANET_HEAD_PARAMS 3376
 int ns2_lstm_seq(const float* xproj, int64_t xp_row_stride, int64_t xp_batch_stride, const void* w_hh, int32_t batch,
                  int32_t steps, int32_t hidden, const float* skip, int64_t skip_row_stride, int64_t skip_batch_stride,
                  float* out, int64_t out_row_stride, int64_t out_batch_stride, void* out_bf16, int64_t outbf_row_stride,
@@ -470,6 +487,8 @@ int ns2_elu_pad(const float* x, int64_t x_row_stride, int64_t x_batch_stride, in
                 int64_t out_batch_stride, ns2_stream_t stream);
 int ns2_seanet_tail(const float* x, int64_t x_row_stride, int64_t x_batch_stride, int32_t batch, int32_t length,
                     const float* params, float* out, int64_t out_batch_stride, ns2_stream_t stream);
+int ns2_seanet_head(const float* x, int64_t x_batch_stride, int32_t batch, int32_t length, const float* params,
+                    void* out_bf16, int64_t out_row_stride, int64_t out_batch_stride, ns2_stream_t stream);
 
 /* Number of kernel launches issued through this library since load (for bench.py's gpu_launches). */
 int64_t ns2_launch_count(void);

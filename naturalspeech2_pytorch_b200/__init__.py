@@ -8,7 +8,7 @@ from . import _lib, ops  # noqa: F401
 from .model import Model  # noqa: F401
 from .diffusion import NaturalSpeech2  # noqa: F401
 from .codec import EncodecRVQ  # noqa: F401
-from .seanet import SEANetDecoder  # noqa: F401
+from .seanet import SEANetDecoder, SEANetEncoder  # noqa: F401
 from . import parallel  # noqa: F401
 from .aligner import maximum_path  # noqa: F401
 from .encoders import (Conditioner, DurationPitchPredictor, PhonemeEncoder,  # noqa: F401

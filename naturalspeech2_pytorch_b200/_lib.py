@@ -19,6 +19,7 @@ NS2_OBJ_V, NS2_OBJ_EPS, NS2_OBJ_X0 = 0, 1, 2
 NS2_GEMM_FLAG_SKIP_EPILOGUE, NS2_GEMM_FLAG_SILU = 1, 4
 NS2_ELU_PAD_ELU, NS2_ELU_PAD_RAW = 1, 2
 NS2_SEANET_TAIL_PARAMS = 3348
+NS2_SEANET_HEAD_PARAMS = 3376
 NS2_ABI_VERSION = 7
 
 
@@ -141,6 +142,7 @@ SIGNATURES = {
                                _P]),
     "ns2_elu_pad": (C.c_int, [_P, _I64, _I64, _I32, _I32, _I32, _I32, _I32, _P, _I64, _I64, _P]),
     "ns2_seanet_tail": (C.c_int, [_P, _I64, _I64, _I32, _I32, _P, _P, _I64, _P]),
+    "ns2_seanet_head": (C.c_int, [_P, _I64, _I32, _I32, _P, _P, _I64, _I64, _P]),
 }
 
 _lib = None

@@ -5,12 +5,13 @@ In scope (SURVEY a16): nearest-codeword search over Q sequential residual stages
 distance filter + exact fp64 re-score => bit-exact indices) and the sum-of-codewords decode (`ops.rvq_decode`).
 Encodec's SEANet encoder and decoder plug in as callables:
     encoder(raw_audio (B, T)) -> frames (B, N, 128)        decoder(emb (B, N, 128)) -> audio (B, 1, T)
-`seanet.SEANetDecoder` is the 24 kHz decoder on this library's kernels; the encoder is not built.  Without an encoder
-the codec accepts encoder-output frames (B, N, 128) directly; without a decoder `decode` returns the latents.
+`seanet.SEANetEncoder` and `seanet.SEANetDecoder` are the 24 kHz encoder and decoder on this library's kernels;
+`EncodecRVQ.from_state_dict` builds the whole codec from one transformers `EncodecModel` state_dict.  Without an
+encoder the codec accepts encoder-output frames (B, N, 128) directly; without a decoder `decode` returns the latents.
 """
 from __future__ import annotations
 
-from typing import Callable, Optional
+from typing import Callable, Dict, Optional
 
 import torch
 from torch import nn
@@ -37,6 +38,19 @@ class EncodecRVQ(nn.Module):
         self._prepared = None
         self._prepared_key = None
 
+    @classmethod
+    def from_state_dict(cls, sd: Dict[str, torch.Tensor], *, num_quantizers: int = 8) -> "EncodecRVQ":
+        """The 24 kHz codec from a transformers `EncodecModel` state_dict: `SEANetEncoder` from `encoder.*`,
+        `SEANetDecoder` from `decoder.*`, and the first `num_quantizers` codebooks
+        `quantizer.layers.{q}.codebook.embed` (8 = the 6 kbps bandwidth).  Move the result with `.cuda()`."""
+        from .seanet import SEANetDecoder, SEANetEncoder
+        parts = {}
+        for name, module in (("encoder", SEANetEncoder()), ("decoder", SEANetDecoder())):
+            module.load_state_dict({k[len(name) + 1:]: v.float() for k, v in sd.items() if k.startswith(name + ".")})
+            parts[name] = module.eval()
+        cb = torch.stack([sd[f"quantizer.layers.{q}.codebook.embed"] for q in range(num_quantizers)])
+        return cls(cb, **parts)
+
     def _prep(self):
         key = (self.codebooks.data_ptr(), self.codebooks._version, str(self.codebooks.device))
         if self._prepared is None or key != self._prepared_key:
@@ -62,8 +76,8 @@ class EncodecRVQ(nn.Module):
         if x.ndim == 2:
             if self.encoder is None:
                 raise NotImplementedError(
-                    "raw audio needs an `encoder` callable (Encodec's SEANet encoder is outside the "
-                    "accelerated path); pass encoder-output frames (B, N, 128) instead")
+                    "raw audio needs an `encoder` callable (e.g. seanet.SEANetEncoder, or build the codec with "
+                    "EncodecRVQ.from_state_dict); pass encoder-output frames (B, N, 128) instead")
             m = self.seq_len_multiple_of
             T = x.shape[-1] // m * m
             x = x[..., -T:] if curtail_from_left else x[..., :T]

@@ -1,11 +1,14 @@
-// Kernels of Encodec's SEANet decoder (24 kHz model) that the segmented GEMM does not cover (include/ns2_b200.h,
-// section 10):
+// Kernels of Encodec's SEANet decoder and encoder (24 kHz model) that the segmented GEMM does not cover
+// (include/ns2_b200.h, section 10):
 //   lstm_seq_kernel   one layer of the decoder's 2-layer LSTM(512), the whole sequence in one launch: a 16-CTA cluster
 //                     per group of <= 64 batch rows, CTA c owning hidden units [32c, 32c + 32) of all four gates with
 //                     its 128 rows of W_hh resident in shared memory; h_t is exchanged through distributed shared memory
 //   elu_pad_kernel    ELU + causal reflect left padding + bf16 cast: the A operand of every conv GEMM
 //   seanet_tail_kernel the 32-channel stage at the full sample rate (last ResnetBlock, ELU, 32 -> 1 k7 conv), fp32
-// Convolutions with >= 64 channels, the transposed convolutions and the LSTM input projections run on ns2_gemm.
+//   seanet_head_kernel the encoder's 32-channel stage at the full sample rate (1 -> 32 k7 conv, ResnetBlock, ELU),
+//                      fp32, writing the bf16 A operand of the encoder's first strided conv
+// Convolutions with >= 64 channels, the transposed and strided convolutions and the LSTM input projections run on
+// ns2_gemm.
 #include "ptx.cuh"
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
@@ -395,6 +398,170 @@ __global__ void __launch_bounds__(kTailThreads) seanet_tail_kernel(const float* 
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// 4. Encoder head, the 32-channel stage at the full sample rate, fp32:
+//      z0 = conv7(x) (1 -> 32),  z1 = shortcut(z0) + conv1(ELU(conv3(ELU(z0)))),  out = bf16(ELU(z1)) reflect-padded
+//      by 2 (the A operand of the first strided conv's GEMM), every conv causal with reflect left padding.
+// One CTA = one batch element x kHeadOut positions t0 .. t0 + kHeadOut - 1 of z1; 128 threads.  Phase 1: thread r
+// computes z0 at window row r (position t0 - 2 + r); the conv3's reflected rows -1, -2 (first tile only) are computed
+// directly at their source positions 1, 2.  Phase 2: thread i < kHeadOut computes h and z1 at t0 + i from z0 rows
+// i .. i + 2 and writes output row t0 + i + 2; threads 1 and 2 of the first tile also write the reflected rows 1, 0.
+// x window: positions t0 - 8 .. t0 + kHeadOut - 1.  Parameters (NS2_SEANET_HEAD_PARAMS floats, input-major):
+//   w0 [7][32] (tap, out)  b0 [32]  w3 [3][32][16] (tap, in, out)  b3 [16]  wsc [32][32] (in, out)
+//   wc1 [16][32] (in, out)  b2 [32] = b_sc + b_c1
+// ------------------------------------------------------------------------------------------------
+constexpr int kHeadThreads = 128;
+constexpr int kHeadOut = kHeadThreads - 2;
+constexpr int kHeadXRows = kHeadOut + 8;
+constexpr int kHOffW0 = 0, kHOffB0 = 224, kHOffW3 = 256, kHOffB3 = 1792, kHOffWsc = 1808, kHOffWc1 = 2832,
+              kHOffB2 = 3344;
+static_assert(kHOffB2 + 32 == NS2_SEANET_HEAD_PARAMS, "head parameter layout");
+constexpr int kHeadSmemFloats = NS2_SEANET_HEAD_PARAMS + ((kHeadXRows + 3) & ~3) + 2 * kHeadThreads * 33;
+
+__global__ void __launch_bounds__(kHeadThreads) seanet_head_kernel(const float* __restrict__ x, long long x_bs,
+                                                                  int length, const float* __restrict__ prm,
+                                                                  __nv_bfloat16* __restrict__ out, long long o_rs,
+                                                                  long long o_bs) {
+  extern __shared__ float4 head_smem4[];
+  float* sp = reinterpret_cast<float*>(head_smem4);
+  float* sx = sp + NS2_SEANET_HEAD_PARAMS;           // x            [kHeadXRows]
+  float* sz = sx + ((kHeadXRows + 3) & ~3);          // z0           [128][33]
+  float* sze = sz + kHeadThreads * 33;               // ELU(z0)      [128][33]
+  const int tid = threadIdx.x;
+  const int b = blockIdx.y;
+  const int t0 = blockIdx.x * kHeadOut;
+  const float* xb = x + b * x_bs;
+
+  for (int i = tid; i < NS2_SEANET_HEAD_PARAMS / 4; i += kHeadThreads)
+    head_smem4[i] = __ldg(reinterpret_cast<const float4*>(prm) + i);
+  for (int i = tid; i < kHeadXRows; i += kHeadThreads) {
+    int t = t0 - 8 + i;
+    bool zero = t >= length || t < -6;
+    if (t < 0 && !zero) {  // the k7 conv's reflect pad (6), zero-extended when the input is that short
+      t = -t;
+      zero = t >= length;
+    }
+    sx[i] = zero ? 0.f : __ldg(xb + t);
+  }
+  __syncthreads();
+
+  {  // z0 = conv7(x) at window row tid
+    int src = t0 - 2 + tid;
+    if (src < 0) src = -src;  // the conv3's reflect pad (2) of z0
+    float acc[32];
+    if (src < length) {
+#pragma unroll
+      for (int o = 0; o < 32; ++o) acc[o] = sp[kHOffB0 + o];
+      const float* xr = sx + src - t0 + 2;
+#pragma unroll
+      for (int j = 0; j < 7; ++j) {
+        const float v = xr[j];
+        const float4* wr = reinterpret_cast<const float4*>(sp + kHOffW0 + j * 32);
+#pragma unroll
+        for (int o4 = 0; o4 < 8; ++o4) {
+          const float4 wv = wr[o4];
+          acc[4 * o4] = fmaf(wv.x, v, acc[4 * o4]);
+          acc[4 * o4 + 1] = fmaf(wv.y, v, acc[4 * o4 + 1]);
+          acc[4 * o4 + 2] = fmaf(wv.z, v, acc[4 * o4 + 2]);
+          acc[4 * o4 + 3] = fmaf(wv.w, v, acc[4 * o4 + 3]);
+        }
+      }
+    } else {  // past the end, or a reflected row of an input shorter than the pad (zero-extended)
+#pragma unroll
+      for (int o = 0; o < 32; ++o) acc[o] = 0.f;
+    }
+#pragma unroll
+    for (int o = 0; o < 32; ++o) {
+      sz[tid * 33 + o] = acc[o];
+      sze[tid * 33 + o] = elu_f(acc[o]);
+    }
+  }
+  __syncthreads();
+
+  if (tid >= kHeadOut) return;
+  const int t = t0 + tid;
+  __nv_bfloat16* ob = out + b * o_bs;
+  if (t >= length) {  // the reflected output rows of an input shorter than 3 samples are zero-extended
+    if (t0 == 0 && (tid == 1 || tid == 2)) {
+      uint4* o = reinterpret_cast<uint4*>(ob + (2 - tid) * o_rs);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) o[i] = make_uint4(0, 0, 0, 0);
+    }
+    return;
+  }
+  float hv[16];
+  {  // h = conv3(ELU(z0)) (32 -> 16), then ELU
+#pragma unroll
+    for (int o = 0; o < 16; ++o) hv[o] = sp[kHOffB3 + o];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      const float* zr = sze + (tid + j) * 33;
+#pragma unroll 8
+      for (int ci = 0; ci < 32; ++ci) {
+        const float v = zr[ci];
+        const float4* wr = reinterpret_cast<const float4*>(sp + kHOffW3 + (j * 32 + ci) * 16);
+#pragma unroll
+        for (int o4 = 0; o4 < 4; ++o4) {
+          const float4 wv = wr[o4];
+          hv[4 * o4] = fmaf(wv.x, v, hv[4 * o4]);
+          hv[4 * o4 + 1] = fmaf(wv.y, v, hv[4 * o4 + 1]);
+          hv[4 * o4 + 2] = fmaf(wv.z, v, hv[4 * o4 + 2]);
+          hv[4 * o4 + 3] = fmaf(wv.w, v, hv[4 * o4 + 3]);
+        }
+      }
+    }
+#pragma unroll
+    for (int o = 0; o < 16; ++o) hv[o] = elu_f(hv[o]);
+  }
+  float acc[32];
+#pragma unroll
+  for (int o = 0; o < 32; ++o) acc[o] = sp[kHOffB2 + o];
+  {  // z1 = shortcut(z0) + conv1(ELU(h)) (32 -> 32, 16 -> 32)
+    const float* zr = sz + (tid + 2) * 33;
+#pragma unroll 4
+    for (int ci = 0; ci < 32; ++ci) {
+      const float v = zr[ci];
+      const float4* wr = reinterpret_cast<const float4*>(sp + kHOffWsc + ci * 32);
+#pragma unroll
+      for (int o4 = 0; o4 < 8; ++o4) {
+        const float4 wv = wr[o4];
+        acc[4 * o4] = fmaf(wv.x, v, acc[4 * o4]);
+        acc[4 * o4 + 1] = fmaf(wv.y, v, acc[4 * o4 + 1]);
+        acc[4 * o4 + 2] = fmaf(wv.z, v, acc[4 * o4 + 2]);
+        acc[4 * o4 + 3] = fmaf(wv.w, v, acc[4 * o4 + 3]);
+      }
+    }
+#pragma unroll
+    for (int hc = 0; hc < 16; ++hc) {
+      const float v = hv[hc];
+      const float4* wr = reinterpret_cast<const float4*>(sp + kHOffWc1 + hc * 32);
+#pragma unroll
+      for (int o4 = 0; o4 < 8; ++o4) {
+        const float4 wv = wr[o4];
+        acc[4 * o4] = fmaf(wv.x, v, acc[4 * o4]);
+        acc[4 * o4 + 1] = fmaf(wv.y, v, acc[4 * o4 + 1]);
+        acc[4 * o4 + 2] = fmaf(wv.z, v, acc[4 * o4 + 2]);
+        acc[4 * o4 + 3] = fmaf(wv.w, v, acc[4 * o4 + 3]);
+      }
+    }
+  }
+  uint4 pk[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    pk[i] = make_uint4(pack_bf16x2(elu_f(acc[8 * i]), elu_f(acc[8 * i + 1])),
+                       pack_bf16x2(elu_f(acc[8 * i + 2]), elu_f(acc[8 * i + 3])),
+                       pack_bf16x2(elu_f(acc[8 * i + 4]), elu_f(acc[8 * i + 5])),
+                       pack_bf16x2(elu_f(acc[8 * i + 6]), elu_f(acc[8 * i + 7])));
+  uint4* o = reinterpret_cast<uint4*>(ob + (t + 2) * o_rs);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) o[i] = pk[i];
+  if (t == 1 || t == 2) {  // the next conv's reflect pad (2): output rows 1, 0 repeat z1 rows 1, 2
+    uint4* r = reinterpret_cast<uint4*>(ob + (2 - t) * o_rs);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) r[i] = pk[i];
+  }
+}
+
 }  // namespace ns2
 
 // ------------------------------------------------------------------------------------------------
@@ -478,6 +645,33 @@ extern "C" int ns2_seanet_tail(const float* x, int64_t x_row_stride, int64_t x_b
   seanet_tail_kernel<<<grid, kTailThreads, smem, static_cast<cudaStream_t>(stream)>>>(x, x_row_stride, x_batch_stride,
                                                                                       length, params, out,
                                                                                       out_batch_stride);
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  NS2_CUDA_CHECK(cudaGetLastError());
+  return kOk;
+}
+
+extern "C" int ns2_seanet_head(const float* x, int64_t x_batch_stride, int32_t batch, int32_t length,
+                               const float* params, void* out_bf16, int64_t out_row_stride, int64_t out_batch_stride,
+                               ns2_stream_t stream) {
+  using namespace ns2;
+  NS2_REQUIRE(batch >= 0 && length >= 0, "ns2_seanet_head: negative size");
+  if (batch == 0 || length == 0) return kOk;
+  NS2_REQUIRE(batch <= 65535, "ns2_seanet_head: batch=%d above 65535", batch);
+  NS2_REQUIRE(x != nullptr && params != nullptr && out_bf16 != nullptr, "ns2_seanet_head: NULL pointer");
+  NS2_REQUIRE(batch == 1 || x_batch_stride >= length, "ns2_seanet_head: x batch stride %lld below length %d",
+              (long long)x_batch_stride, length);
+  NS2_REQUIRE((reinterpret_cast<uintptr_t>(x) & 3) == 0 && (reinterpret_cast<uintptr_t>(params) & 15) == 0,
+              "ns2_seanet_head: x must be 4-byte and params 16-byte aligned");
+  NS2_REQUIRE(out_row_stride >= 32 && out_row_stride % 8 == 0 && out_batch_stride % 8 == 0 &&
+                  (reinterpret_cast<uintptr_t>(out_bf16) & 15) == 0,
+              "ns2_seanet_head: out (32 channels) must be 16-byte aligned with strides multiple of 8");
+  NS2_REQUIRE(batch == 1 || out_batch_stride >= (length + 2LL) * out_row_stride,
+              "ns2_seanet_head: out batch stride %lld below (length + 2) rows", (long long)out_batch_stride);
+  const int smem = kHeadSmemFloats * 4;
+  NS2_CUDA_CHECK(set_max_smem_once(seanet_head_kernel, smem));
+  const dim3 grid((length + kHeadOut - 1) / kHeadOut, batch);
+  seanet_head_kernel<<<grid, kHeadThreads, smem, static_cast<cudaStream_t>(stream)>>>(
+      x, x_batch_stride, length, params, static_cast<__nv_bfloat16*>(out_bf16), out_row_stride, out_batch_stride);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   NS2_CUDA_CHECK(cudaGetLastError());
   return kOk;

@@ -909,7 +909,7 @@ def maximum_path(value: torch.Tensor, mask: torch.Tensor, neg_const: float = flo
 
 
 # --------------------------------------------------------------------------------------------------
-# SEANet decoder (Encodec 24 kHz): LSTM recurrence, conv operand preparation, 32-channel tail
+# SEANet decoder and encoder (Encodec 24 kHz): LSTM recurrence, conv operand preparation, 32-channel tail and head
 # --------------------------------------------------------------------------------------------------
 def _rows3(t: torch.Tensor, name: str, cols: int) -> Tuple[int, int]:
     """(row stride, batch stride) of a (B, T, >= cols) view with unit channel stride."""
@@ -979,4 +979,23 @@ def seanet_tail(x: torch.Tensor, params: torch.Tensor, out: torch.Tensor) -> tor
         raise ValueError("out must be (B, T) with unit time stride")
     check(lib.ns2_seanet_tail(x.data_ptr(), xrs, xbs, B, T, params.data_ptr(), out.data_ptr(), out.stride(0),
                               _stream(out)), "ns2_seanet_tail")
+    return out
+
+
+def seanet_head(x: torch.Tensor, params: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """out (B, T + 2, 32) bf16 = elu_pad(ResnetBlock(conv7(x)), pad=2) for audio x (B, T) f32 (unit time stride,
+    any batch stride): the encoder's full-rate stage, ready as the first strided conv's A operand.  params: the
+    NS2_SEANET_HEAD_PARAMS packed f32 weights (SEANetEncoder packs them).  out may be a row-strided view."""
+    lib = _lib.load()
+    _req(x, torch.float32, "x")
+    _req(out, torch.bfloat16, "out")
+    _req_flat(params, torch.float32, "params", _lib.NS2_SEANET_HEAD_PARAMS)
+    if x.dim() != 2:
+        raise ValueError(f"seanet_head takes (B, T) audio, got {tuple(x.shape)}")
+    B, T = x.shape
+    ors, obs = _rows3(out, "out", 32)
+    if tuple(out.shape) != (B, T + 2, 32):
+        raise ValueError(f"out must be (B, T + 2, 32) = {(B, T + 2, 32)}, got {tuple(out.shape)}")
+    check(lib.ns2_seanet_head(x.data_ptr(), x.stride(0), B, T, params.data_ptr(), out.data_ptr(), ors, obs,
+                              _stream(out)), "ns2_seanet_head")
     return out

@@ -14,6 +14,10 @@ Layers (token-major activations (B, time, channels); every conv causal with refl
 GEMM operands are bf16 with fp32 accumulation; activations between layers, the LSTM cell state and the tail stay fp32.
 The state_dict has the keys and shapes of transformers' `EncodecDecoder`; `load_encodec_state_dict` takes Meta
 `encodec` (and audiolm's `EncodecWrapper.model.decoder`) keys.  Inference only: there is no backward.
+
+`SEANetEncoder` is the other direction, the `encoder` of `EncodecRVQ` (24 kHz audio -> 75 Hz frames, what
+`NaturalSpeech2.forward` and `process_prompt` run on raw audio): a full-rate fp32 head kernel (`ns2_seanet_head`), the
+strided convs as 2-segment GEMMs, the decoder's ResnetBlock and LSTM mapping; see its docstring.
 """
 from __future__ import annotations
 
@@ -29,7 +33,7 @@ from .model import _PackedCache
 
 RATIOS = (8, 5, 4, 2)
 
-# the 24 kHz Encodec model's decoder configuration (transformers EncodecConfig() defaults); nothing else is built
+# the 24 kHz Encodec model's SEANet configuration (transformers EncodecConfig() defaults); nothing else is built
 SUPPORTED = dict(audio_channels=1, num_filters=32, upsampling_ratios=(8, 5, 4, 2), hidden_size=128, kernel_size=7,
                  last_kernel_size=7, residual_kernel_size=3, dilation_growth_rate=2, num_residual_layers=1,
                  compress=2, num_lstm_layers=2, use_causal_conv=True, pad_mode="reflect", norm_type="weight_norm",
@@ -67,12 +71,59 @@ def pack_tail(w3, b3, w1, b1, w_sc, b_sc, w_f, b_f) -> torch.Tensor:
     return p.float().contiguous()
 
 
+def pack_head(w0, b0, w3, b3, w1, b1, w_sc, b_sc) -> torch.Tensor:
+    """Folded weights of the encoder's first conv (32, 1, 7) and of its 32-channel ResnetBlock (conv3 (16, 32, 3),
+    conv1x1 (32, 16, 1), shortcut (32, 32, 1)) -> the NS2_SEANET_HEAD_PARAMS f32 layout of ns2_seanet_head."""
+    p = torch.cat([w0[:, 0].t().reshape(-1), b0, w3.permute(2, 1, 0).reshape(-1), b3, w_sc[:, :, 0].t().reshape(-1),
+                   w1[:, :, 0].t().reshape(-1), b_sc + b1])
+    assert p.numel() == _lib.NS2_SEANET_HEAD_PARAMS
+    return p.float().contiguous()
+
+
+def pack_strided_conv(w: torch.Tensor) -> torch.Tensor:
+    """Conv1d(k = 2s, stride s) weight (C_out, C_in, 2s) -> the 2-segment GEMM's bf16 pack (C_out, 2s C_in), tap-major:
+    column j C_in + ci = w[co, ci, j].  With the input reflect-padded by s and viewed as rows of s samples, segment 0
+    (taps [0, s)) reads row m - 1 and segment 1 (taps [s, 2s)) row m: output row m + 1 is conv output m."""
+    return w.permute(0, 2, 1).reshape(w.shape[0], -1).to(torch.bfloat16).contiguous()
+
+
+def strided_conv_segs(s: int, c_in: int) -> list:
+    """`ns2_gemm` segments of `pack_strided_conv` (include/ns2_b200.h section 10)."""
+    return [(0, 0, s * c_in, 1, 0), (0, s * c_in, s * c_in, 0, 0)]
+
+
+def _check_config(cls_name: str, given: dict) -> None:
+    bad = {k: v for k, v in given.items() if v != SUPPORTED[k]}
+    if bad:
+        raise ValueError(f"{cls_name} supports only the 24 kHz Encodec configuration; unsupported: {bad} "
+                         f"(expected {({k: SUPPORTED[k] for k in bad})})")
+
+
+def encodec_keys_to_transformers(sd: Dict[str, torch.Tensor], part: str) -> Dict[str, torch.Tensor]:
+    """Meta `encodec` SEANet keys (`{part}.model.{i}.conv.conv.weight_g|weight_v|bias`, `model.{i}.convtr.convtr.*`,
+    `model.{i}.block.{j}.conv.conv.*`, `model.{i}.shortcut.conv.conv.*`, `model.{i}.lstm.*`; the `{part}.` prefix,
+    "encoder" or "decoder", is optional) -> transformers' `Encodec{Encoder,Decoder}` keys (`layers.{i}...`)."""
+    out = {}
+    for k, v in sd.items():
+        k = k[len(part) + 1:] if k.startswith(part + ".") else k
+        m = re.fullmatch(r"model\.(\d+)\.(.*)", k)
+        if m is None:
+            raise KeyError(f"unexpected key {k!r} in an encodec {part} state_dict")
+        i, rest = m.group(1), m.group(2)
+        rest = re.sub(r"^(conv\.conv|convtr\.convtr)\.", "conv.", rest)
+        rest = re.sub(r"^(block\.\d+|shortcut)\.conv\.conv\.", r"\1.conv.", rest)
+        rest = re.sub(r"conv\.weight_g$", "conv.parametrizations.weight.original0", rest)
+        rest = re.sub(r"conv\.weight_v$", "conv.parametrizations.weight.original1", rest)
+        out[f"layers.{i}.{rest}"] = v
+    return out
+
+
 class _WNConv(nn.Module):
     """Parameter holder of EncodecConv1d / EncodecConvTranspose1d: `conv` is the weight-normed torch module."""
 
     def __init__(self, c_in: int, c_out: int, kernel: int, stride: int = 1, transposed: bool = False):
         super().__init__()
-        conv = nn.ConvTranspose1d(c_in, c_out, kernel, stride) if transposed else nn.Conv1d(c_in, c_out, kernel)
+        conv = nn.ConvTranspose1d(c_in, c_out, kernel, stride) if transposed else nn.Conv1d(c_in, c_out, kernel, stride)
         self.conv = nn.utils.parametrizations.weight_norm(conv)
 
     def folded(self):
@@ -116,10 +167,7 @@ class SEANetDecoder(_PackedCache):
                      num_residual_layers=num_residual_layers, compress=compress, num_lstm_layers=num_lstm_layers,
                      use_causal_conv=bool(use_causal_conv), pad_mode=pad_mode, norm_type=norm_type,
                      trim_right_ratio=float(trim_right_ratio), use_conv_shortcut=bool(use_conv_shortcut))
-        bad = {k: v for k, v in given.items() if v != SUPPORTED[k]}
-        if bad:
-            raise ValueError(f"SEANetDecoder supports only the 24 kHz Encodec decoder configuration; unsupported: {bad} "
-                             f"(expected {({k: SUPPORTED[k] for k in bad})})")
+        _check_config("SEANetDecoder", given)
         scale = 2 ** len(RATIOS)
         layers = [_WNConv(hidden_size, scale * num_filters, kernel_size), _LSTMParams(scale * num_filters, num_lstm_layers)]
         for r in RATIOS:
@@ -143,19 +191,7 @@ class SEANetDecoder(_PackedCache):
         `model.{i}.block.{j}.conv.conv.*`, `model.{i}.shortcut.conv.conv.*`, `model.1.lstm.*`.  A `decoder.` prefix
         is stripped.  The mapping follows the upstream module layout; it has not been checked against a released
         checkpoint, so load with strict=True and compare a decoded clip against the original decoder once."""
-        out = {}
-        for k, v in sd.items():
-            k = k[len("decoder."):] if k.startswith("decoder.") else k
-            m = re.fullmatch(r"model\.(\d+)\.(.*)", k)
-            if m is None:
-                raise KeyError(f"unexpected key {k!r} in an encodec decoder state_dict")
-            i, rest = m.group(1), m.group(2)
-            rest = re.sub(r"^(conv\.conv|convtr\.convtr)\.", "conv.", rest)
-            rest = re.sub(r"^(block\.\d+|shortcut)\.conv\.conv\.", r"\1.conv.", rest)
-            rest = re.sub(r"conv\.weight_g$", "conv.parametrizations.weight.original0", rest)
-            rest = re.sub(r"conv\.weight_v$", "conv.parametrizations.weight.original1", rest)
-            out[f"layers.{i}.{rest}"] = v
-        return self.load_state_dict(out, strict=strict)
+        return self.load_state_dict(encodec_keys_to_transformers(sd, "decoder"), strict=strict)
 
     @property
     def device(self):
@@ -269,3 +305,183 @@ class SEANetDecoder(_PackedCache):
                          segs=[(c_out, 0, c_out, 0, 0), (2 * c_out, c_out, h, 0, 0)], bias=P[f"r{si}_b1"])
                 z = zo[:, 2:]
         return out
+
+
+class SEANetEncoder(_PackedCache):
+    """Encodec's SEANet encoder (24 kHz model): (B, T) or (B, 1, T) audio, T a multiple of 320 -> (B, T / 320, 128)
+    token-major frames, fp32 — the `encoder` callable of `EncodecRVQ`.
+
+    Layers (transformers `EncodecEncoder` indices; every conv causal with reflect left padding, weight norm folded):
+        0-2     Conv1d k7 1 -> 32, ResnetBlock(32, hidden 16), ELU      ns2_seanet_head (fp32, bf16 output)
+        3       Conv1d k4 stride 2 32 -> 64                             2-segment GEMM (`strided_conv_segs`)
+        4-5     ResnetBlock(64, hidden 32), ELU                         as in the decoder: elu_pad (ELU | raw, pad 2)
+                                                                        + 3-segment GEMM, elu_pad, one GEMM for
+                                                                        conv1x1 + shortcut, then elu_pad (pad s)
+        6-11    the same at k8 s4 64 -> 128, ResnetBlock(128); k10 s5 128 -> 256, ResnetBlock(256)
+        12      Conv1d k16 stride 8 256 -> 512                          2-segment GEMM
+        13      2-layer LSTM(512), lstm(x)[0] + x                       input projection GEMM + ns2_lstm_seq per layer
+        14-15   ELU, Conv1d k7 512 -> 128                               elu_pad (pad 6) + 7-segment GEMM, fp32 out
+    The constructor takes transformers' `EncodecConfig` fields; only the 24 kHz model's values are supported.  The
+    state_dict has the keys and shapes of transformers' `EncodecEncoder`.  Inference only: there is no backward."""
+
+    def __init__(self, *, audio_channels: int = 1, num_filters: int = 32, upsampling_ratios: Sequence[int] = RATIOS,
+                 hidden_size: int = 128, kernel_size: int = 7, last_kernel_size: int = 7, residual_kernel_size: int = 3,
+                 dilation_growth_rate: int = 2, num_residual_layers: int = 1, compress: int = 2,
+                 num_lstm_layers: int = 2, use_causal_conv: bool = True, pad_mode: str = "reflect",
+                 norm_type: str = "weight_norm", trim_right_ratio: float = 1.0, use_conv_shortcut: bool = True):
+        super().__init__()
+        given = dict(audio_channels=audio_channels, num_filters=num_filters,
+                     upsampling_ratios=tuple(int(r) for r in upsampling_ratios), hidden_size=hidden_size,
+                     kernel_size=kernel_size, last_kernel_size=last_kernel_size,
+                     residual_kernel_size=residual_kernel_size, dilation_growth_rate=dilation_growth_rate,
+                     num_residual_layers=num_residual_layers, compress=compress, num_lstm_layers=num_lstm_layers,
+                     use_causal_conv=bool(use_causal_conv), pad_mode=pad_mode, norm_type=norm_type,
+                     trim_right_ratio=float(trim_right_ratio), use_conv_shortcut=bool(use_conv_shortcut))
+        _check_config("SEANetEncoder", given)
+        layers = [_WNConv(audio_channels, num_filters, kernel_size)]
+        dim = num_filters
+        for r in reversed(RATIOS):
+            layers += [_ResnetParams(dim, dim // compress, residual_kernel_size), nn.ELU(),
+                       _WNConv(dim, 2 * dim, 2 * r, stride=r)]
+            dim *= 2
+        layers += [_LSTMParams(dim, num_lstm_layers), nn.ELU(), _WNConv(dim, hidden_size, last_kernel_size)]
+        self.layers = nn.ModuleList(layers)
+        self._ws: "OrderedDict[tuple, Dict[str, torch.Tensor]]" = OrderedDict()
+        self.max_cached_shapes = 4  # LRU bound on per-(B, T) workspaces (~6.5 GB at (32, 327680))
+
+    @classmethod
+    def from_config(cls, config) -> "SEANetEncoder":
+        """From an object with transformers' `EncodecConfig` attribute names."""
+        return cls(**{k: getattr(config, k) for k in SUPPORTED})
+
+    def load_encodec_state_dict(self, sd: Dict[str, torch.Tensor], strict: bool = True):
+        """Load a Meta `encodec` SEANetEncoder state_dict (`EncodecModel.encoder`, also audiolm's
+        `EncodecWrapper.model.encoder`): `model.{i}.conv.conv.weight_g|weight_v|bias`, `model.{i}.block.{j}.conv.conv.*`,
+        `model.{i}.shortcut.conv.conv.*`, `model.13.lstm.*`.  An `encoder.` prefix is stripped.  The mapping follows
+        the upstream module layout; it has not been checked against a released checkpoint, so load with strict=True
+        and compare the frames of one clip against the original encoder once."""
+        return self.load_state_dict(encodec_keys_to_transformers(sd, "encoder"), strict=strict)
+
+    @property
+    def device(self):
+        return next(self.parameters()).device
+
+    def _apply(self, fn, *args, **kwargs):
+        out = super()._apply(fn, *args, **kwargs)
+        self._ws.clear()
+        return out
+
+    # ----------------------------------------------------------------------------------------------
+    # weight packing (folded weight norm, bf16, K-major; rebuilt when a parameter changes)
+    # ----------------------------------------------------------------------------------------------
+    def _pack(self) -> Dict[str, torch.Tensor]:
+        bf = lambda t: t.to(torch.bfloat16).contiguous()
+        f32 = lambda t: t.float().contiguous()
+        P = {}
+        blk = self.layers[1]
+        P["head"] = pack_head(*self.layers[0].folded(), *blk.block[1].folded(), *blk.block[3].folded(),
+                              *blk.shortcut.folded())
+        for si in range(len(RATIOS)):
+            w, b = self.layers[3 + 3 * si].folded()                 # (2C, C, 2s)
+            P[f"s{si}_w"], P[f"s{si}_b"] = pack_strided_conv(w), f32(b)
+            if si < len(RATIOS) - 1:
+                blk = self.layers[4 + 3 * si]
+                w3, b3 = blk.block[1].folded()                      # (H, D, 3)
+                w1, b1 = blk.block[3].folded()                      # (D, H, 1)
+                ws, bs = blk.shortcut.folded()                      # (D, D, 1)
+                P[f"r{si}_w3"], P[f"r{si}_b3"] = bf(w3.permute(0, 2, 1).reshape(w3.shape[0], -1)), f32(b3)
+                P[f"r{si}_w1"] = bf(torch.cat([ws[:, :, 0], w1[:, :, 0]], dim=1))
+                P[f"r{si}_b1"] = f32(bs + b1)
+        lstm = self.layers[13].lstm
+        perm = lstm_gate_perm().to(w.device)
+        for l in range(2):
+            P[f"l{l}_wih"] = bf(getattr(lstm, f"weight_ih_l{l}")[perm])
+            P[f"l{l}_whh"] = bf(getattr(lstm, f"weight_hh_l{l}")[perm])
+            P[f"l{l}_b"] = f32((getattr(lstm, f"bias_ih_l{l}") + getattr(lstm, f"bias_hh_l{l}"))[perm])
+        w, b = self.layers[15].folded()                             # (128, 512, 7)
+        P["c15_w"], P["c15_b"] = bf(w.permute(0, 2, 1).reshape(w.shape[0], -1)), f32(b)
+        return P
+
+    # ----------------------------------------------------------------------------------------------
+    # workspaces (per (B, T) shape, LRU-bounded)
+    # ----------------------------------------------------------------------------------------------
+    def _workspace(self, B: int, T: int, dev) -> Dict[str, torch.Tensor]:
+        key = (B, T, str(dev))
+        ws = self._ws.get(key)
+        if ws is not None:
+            self._ws.move_to_end(key)
+            return ws
+        while len(self._ws) >= self.max_cached_shapes:
+            self._ws.popitem(last=False)
+        e = lambda *s, dt=torch.bfloat16: torch.empty(*s, device=dev, dtype=dt)
+        f = torch.float32
+        strides = tuple(reversed(RATIOS))
+        ws = {"a0": e(B, T + strides[0], 32)}
+        L = T
+        for si, s in enumerate(strides):
+            c_out = 64 << si
+            L //= s
+            ws[f"y{si}"] = e(B, L + 1, c_out, dt=f)                 # row 0: the strided GEMM's scratch row
+            if si < len(strides) - 1:
+                h = c_out // 2
+                ws[f"blk{si}"] = e(B, L + 2, 2 * c_out + h)
+                ws[f"h{si}"] = e(B, L + 2, h, dt=f)
+                ws[f"z{si}"] = e(B, L + 2, c_out, dt=f)
+                ws[f"a{si + 1}"] = e(B, L + strides[si + 1], c_out)
+        N = L
+        ws.update(xb=e(B, N, 512), xp=e(B, N, 2048, dt=f), lz=e(B, N, 512, dt=f), a15=e(B, N + 6, 512))
+        self._ws[key] = ws
+        return ws
+
+    # ----------------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def forward(self, audio: torch.Tensor) -> torch.Tensor:
+        """audio (B, T) or (B, 1, T), T % 320 == 0 -> frames (B, T / 320, 128) fp32, a new tensor per call."""
+        if audio.dim() == 3 and audio.shape[1] == 1:
+            audio = audio[:, 0]
+        if audio.dim() != 2:
+            raise ValueError(f"SEANetEncoder takes (B, T) or (B, 1, T) audio, got {tuple(audio.shape)}")
+        B, T = audio.shape
+        if T % 320:
+            raise ValueError(f"SEANetEncoder needs T % 320 == 0 (the product of the strides), got T={T}")
+        dev = audio.device
+        N = T // 320
+        if B == 0 or T == 0:
+            return torch.empty(B, N, 128, device=dev, dtype=torch.float32)
+        frames = torch.empty(B, N + 6, 128, device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            P, ws = self.packed(), self._workspace(B, T, dev)
+            x = audio.float()
+            if x.stride(1) != 1:
+                x = x.contiguous()
+            strides = tuple(reversed(RATIOS))
+            a, L, c_in = ws["a0"], T, 32
+            ops.seanet_head(x, P["head"], a)                       # bf16(ELU(z1)) reflect-padded by 2
+            for si, s in enumerate(strides):
+                c_out = 2 * c_in
+                L //= s
+                y = ws[f"y{si}"]
+                ops.gemm(a.view(B, L + 1, s * c_in), P[f"s{si}_w"], y, n=c_out, epilogue=ops.EPI_F32,
+                         segs=strided_conv_segs(s, c_in), bias=P[f"s{si}_b"])
+                y = y[:, 1:]
+                if si == len(strides) - 1:
+                    break
+                h = c_out // 2
+                blk, hb, zo, a = ws[f"blk{si}"], ws[f"h{si}"], ws[f"z{si}"], ws[f"a{si + 1}"]
+                ops.elu_pad(y, blk, pad=2, elu=True, raw=True)          # [ELU(x) | x], reflect-padded by 2
+                ops.gemm(blk, P[f"r{si}_w3"], hb, n=h, epilogue=ops.EPI_F32, segs=ops.conv_segs(c_out, 3, 2),
+                         bias=P[f"r{si}_b3"])
+                ops.elu_pad(hb[:, 2:], blk[:, 2:, 2 * c_out:], pad=0, elu=True)
+                ops.gemm(blk, P[f"r{si}_w1"], zo, n=c_out, epilogue=ops.EPI_F32,
+                         segs=[(c_out, 0, c_out, 0, 0), (2 * c_out, c_out, h, 0, 0)], bias=P[f"r{si}_b1"])
+                ops.elu_pad(zo[:, 2:], a, pad=strides[si + 1], elu=True)
+                c_in = c_out
+            ops.elu_pad(y, ws["xb"], pad=0, elu=False)
+            ops.gemm(ws["xb"], P["l0_wih"], ws["xp"], n=2048, epilogue=ops.EPI_F32, bias=P["l0_b"])
+            ops.lstm_seq(ws["xp"], P["l0_whh"], out_bf16=ws["xb"])
+            ops.gemm(ws["xb"], P["l1_wih"], ws["xp"], n=2048, epilogue=ops.EPI_F32, bias=P["l1_b"])
+            ops.lstm_seq(ws["xp"], P["l1_whh"], skip=y, out=ws["lz"])
+            ops.elu_pad(ws["lz"], ws["a15"], pad=6, elu=True)
+            ops.gemm(ws["a15"], P["c15_w"], frames, n=128, epilogue=ops.EPI_F32, segs=ops.conv_segs(512, 7, 6),
+                     bias=P["c15_b"])
+        return frames[:, 6:]

@@ -62,6 +62,29 @@ __device__ __forceinline__ void wgmma_lstm(float (&d)[NB / 2], uint64_t da, uint
 __device__ __forceinline__ float elu_f(float v) { return v > 0.f ? v : expm1f(v); }
 __device__ __forceinline__ float sigmoid_acc(float v) { return 1.0f / (1.0f + __expf(-v)); }
 
+// Source row of position t under a causal reflect left pad: rows [-pad, 0) mirror about row 0.  False where the row
+// reads as zero: beyond the pad, or at or past `length` (a reflected row of an input shorter than the pad is the
+// reflection of its zero extension).
+__device__ __forceinline__ bool reflect_src(int& t, int length, int pad) {
+  if (t < -pad) return false;
+  if (t < 0) t = -t;
+  return t < length;
+}
+
+// acc[o] += w[o] * v over a row of N weights: one float4 broadcast feeds four outputs
+template <int N>
+__device__ __forceinline__ void fma_row(float (&acc)[N], const float* w, float v) {
+  const float4* wr = reinterpret_cast<const float4*>(w);
+#pragma unroll
+  for (int o4 = 0; o4 < N / 4; ++o4) {
+    const float4 wv = wr[o4];
+    acc[4 * o4] = fmaf(wv.x, v, acc[4 * o4]);
+    acc[4 * o4 + 1] = fmaf(wv.y, v, acc[4 * o4 + 1]);
+    acc[4 * o4 + 2] = fmaf(wv.z, v, acc[4 * o4 + 2]);
+    acc[4 * o4 + 3] = fmaf(wv.w, v, acc[4 * o4 + 3]);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // 1. LSTM layer (nn.LSTM gate order i, f, g, o; zero initial state)
 //
@@ -250,13 +273,8 @@ __global__ void elu_pad_kernel(const float* __restrict__ x, long long x_rs, long
     const int r = static_cast<int>(rest % rows);
     const int b = static_cast<int>(rest / rows);
     int t = r - pad;
-    bool zero = false;
-    if (t < 0) {  // reflect about position 0; past the end of a short input the zero extension is reflected
-      t = -t;
-      zero = t >= length;
-    }
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (!zero) v = *reinterpret_cast<const float4*>(x + b * x_bs + t * x_rs + 4 * cc);
+    if (reflect_src(t, length, pad)) v = *reinterpret_cast<const float4*>(x + b * x_bs + t * x_rs + 4 * cc);
     __nv_bfloat16* o = out + b * o_bs + r * o_rs + 4 * cc;
     float4 e = v;
     if (flags & NS2_ELU_PAD_ELU) e = make_float4(elu_f(v.x), elu_f(v.y), elu_f(v.z), elu_f(v.w));
@@ -267,18 +285,49 @@ __global__ void elu_pad_kernel(const float* __restrict__ x, long long x_rs, long
 }
 
 // ------------------------------------------------------------------------------------------------
-// 3. 32-channel tail: z = shortcut(x) + conv1(ELU(conv3(ELU(x)))), y = conv7(ELU(z)), all causal with reflect padding.
-// One CTA = one batch element x kTailOut output samples; 128 threads, one window row each.  Window rows of z (and h)
-// cover t0 - 6 .. t0 + kTailOut - 1, x rows t0 - 8 .. t0 + kTailOut - 1.  Parameters (NS2_SEANET_TAIL_PARAMS floats,
-// packed input-major so that one float4 broadcast feeds four outputs):
+// 3. ResnetBlock(32, hidden 16) of the tail and head kernels, one position per thread, fp32:
+//      out = shortcut(x) + conv1(ELU(conv3(ELU(x))))
+// Parameters (kBlkFloats floats from the block's base, packed input-major for fma_row):
 //   w3 [3][32][16] (tap, in, out)  b3 [16]   wsc [32][32] (in, out)  wc1 [16][32] (in, out)  b2 [32] = b_sc + b_c1
-//   wf [7][32] (tap, in)           bf [4] (bf[0] = the final bias)
+// Each accumulator takes its bias first, then taps and input channels ascending, the shortcut before the conv1x1.
+// ------------------------------------------------------------------------------------------------
+constexpr int kBlkW3 = 0, kBlkB3 = 1536, kBlkWsc = 1552, kBlkWc1 = 2576, kBlkB2 = 3088, kBlkFloats = 3120;
+
+// h = b3 + conv3 over the three rows of ELU(x) (row stride 33) that start at xe
+__device__ __forceinline__ void resblock32_hidden(float (&h)[16], const float* blk, const float* xe) {
+#pragma unroll
+  for (int o = 0; o < 16; ++o) h[o] = blk[kBlkB3 + o];
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    const float* xr = xe + j * 33;
+#pragma unroll 8
+    for (int ci = 0; ci < 32; ++ci) fma_row(h, blk + kBlkW3 + (j * 32 + ci) * 16, xr[ci]);
+  }
+}
+
+// acc = b2 + shortcut(row x) + conv1(row eh = ELU(h)).  eh lives in shared memory in the tail (kUnrollH = 4) and in
+// registers in the head, where only the fully unrolled loop (kUnrollH = 16) keeps it there.
+template <int kUnrollH>
+__device__ __forceinline__ void resblock32_out(float (&acc)[32], const float* blk, const float* x, const float* eh) {
+#pragma unroll
+  for (int o = 0; o < 32; ++o) acc[o] = blk[kBlkB2 + o];
+#pragma unroll 4
+  for (int ci = 0; ci < 32; ++ci) fma_row(acc, blk + kBlkWsc + ci * 32, x[ci]);
+#pragma unroll kUnrollH
+  for (int hc = 0; hc < 16; ++hc) fma_row(acc, blk + kBlkWc1 + hc * 32, eh[hc]);
+}
+
+// ------------------------------------------------------------------------------------------------
+// 4. 32-channel tail: z = ResnetBlock(x), y = conv7(ELU(z)), all causal with reflect padding.
+// One CTA = one batch element x kTailOut output samples; 128 threads, one window row each.  Window rows of z (and h)
+// cover t0 - 6 .. t0 + kTailOut - 1, x rows t0 - 8 .. t0 + kTailOut - 1.  Parameters (NS2_SEANET_TAIL_PARAMS floats):
+//   the ResnetBlock's (section 3)  wf [7][32] (tap, in)  bf [4] (bf[0] = the final bias)
 // ------------------------------------------------------------------------------------------------
 constexpr int kTailThreads = 128;
 constexpr int kTailOut = kTailThreads - 6;
 constexpr int kTailXRows = kTailOut + 8;
-constexpr int kOffW3 = 0, kOffB3 = 1536, kOffWsc = 1552, kOffWc1 = 2576, kOffB2 = 3088, kOffWf = 3120, kOffBf = 3344;
-static_assert(kOffBf + 4 == NS2_SEANET_TAIL_PARAMS, "tail parameter layout");
+constexpr int kTailBlk = 0, kTailWf = kTailBlk + kBlkFloats, kTailBf = kTailWf + 7 * 32;
+static_assert(kTailBf + 4 == NS2_SEANET_TAIL_PARAMS, "tail parameter layout");
 constexpr int kTailSmemFloats = NS2_SEANET_TAIL_PARAMS + 2 * kTailXRows * 33 + kTailThreads * 17 + kTailThreads * 33;
 
 __global__ void __launch_bounds__(kTailThreads) seanet_tail_kernel(const float* __restrict__ x, long long x_rs,
@@ -301,13 +350,9 @@ __global__ void __launch_bounds__(kTailThreads) seanet_tail_kernel(const float* 
   for (int i = tid; i < kTailXRows * 8; i += kTailThreads) {
     const int r = i >> 3, c4 = (i & 7) * 4;
     int t = t0 - 8 + r;
-    bool zero = t >= length || t < -2;
-    if (t < 0 && !zero) {  // the k3 conv's reflect pad (2), zero-extended when the input is that short
-      t = -t;
-      zero = t >= length;
-    }
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (!zero) v = __ldg(reinterpret_cast<const float4*>(xb + t * x_rs + c4));
+    if (reflect_src(t, length, 2))  // the k3 conv's reflect pad
+      v = __ldg(reinterpret_cast<const float4*>(xb + t * x_rs + c4));
     float* d = sx + r * 33 + c4;
     float* e = sxe + r * 33 + c4;
     d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
@@ -318,62 +363,17 @@ __global__ void __launch_bounds__(kTailThreads) seanet_tail_kernel(const float* 
   const int hr = tid;                 // window row: t = t0 - 6 + hr
   const int t = t0 - 6 + hr;
   const bool live = t >= 0 && t < length;
+  const float* blk = sp + kTailBlk;
   {  // h = conv3(ELU(x)) (32 -> 16), stored as ELU(h)
     float acc[16];
-#pragma unroll
-    for (int o = 0; o < 16; ++o) acc[o] = sp[kOffB3 + o];
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-      const float* xr = sxe + (hr + j) * 33;
-#pragma unroll 8
-      for (int ci = 0; ci < 32; ++ci) {
-        const float v = xr[ci];
-        const float4* wr = reinterpret_cast<const float4*>(sp + kOffW3 + (j * 32 + ci) * 16);
-#pragma unroll
-        for (int o4 = 0; o4 < 4; ++o4) {
-          const float4 wv = wr[o4];
-          acc[4 * o4] = fmaf(wv.x, v, acc[4 * o4]);
-          acc[4 * o4 + 1] = fmaf(wv.y, v, acc[4 * o4 + 1]);
-          acc[4 * o4 + 2] = fmaf(wv.z, v, acc[4 * o4 + 2]);
-          acc[4 * o4 + 3] = fmaf(wv.w, v, acc[4 * o4 + 3]);
-        }
-      }
-    }
+    resblock32_hidden(acc, blk, sxe + hr * 33);
 #pragma unroll
     for (int o = 0; o < 16; ++o) sh[hr * 17 + o] = elu_f(acc[o]);
   }
   __syncthreads();
   {  // z = shortcut(x) + conv1(ELU(h)) (32 -> 32, 16 -> 32), stored as ELU(z); zero outside [0, length)
     float acc[32];
-#pragma unroll
-    for (int o = 0; o < 32; ++o) acc[o] = sp[kOffB2 + o];
-    const float* xr = sx + (hr + 2) * 33;
-#pragma unroll 4
-    for (int ci = 0; ci < 32; ++ci) {
-      const float v = xr[ci];
-      const float4* wr = reinterpret_cast<const float4*>(sp + kOffWsc + ci * 32);
-#pragma unroll
-      for (int o4 = 0; o4 < 8; ++o4) {
-        const float4 wv = wr[o4];
-        acc[4 * o4] = fmaf(wv.x, v, acc[4 * o4]);
-        acc[4 * o4 + 1] = fmaf(wv.y, v, acc[4 * o4 + 1]);
-        acc[4 * o4 + 2] = fmaf(wv.z, v, acc[4 * o4 + 2]);
-        acc[4 * o4 + 3] = fmaf(wv.w, v, acc[4 * o4 + 3]);
-      }
-    }
-#pragma unroll 4
-    for (int hc = 0; hc < 16; ++hc) {
-      const float v = sh[hr * 17 + hc];
-      const float4* wr = reinterpret_cast<const float4*>(sp + kOffWc1 + hc * 32);
-#pragma unroll
-      for (int o4 = 0; o4 < 8; ++o4) {
-        const float4 wv = wr[o4];
-        acc[4 * o4] = fmaf(wv.x, v, acc[4 * o4]);
-        acc[4 * o4 + 1] = fmaf(wv.y, v, acc[4 * o4 + 1]);
-        acc[4 * o4 + 2] = fmaf(wv.z, v, acc[4 * o4 + 2]);
-        acc[4 * o4 + 3] = fmaf(wv.w, v, acc[4 * o4 + 3]);
-      }
-    }
+    resblock32_out<4>(acc, blk, sx + (hr + 2) * 33, sh + hr * 17);
 #pragma unroll
     for (int o = 0; o < 32; ++o) sz[hr * 33 + o] = live ? elu_f(acc[o]) : 0.f;
   }
@@ -387,19 +387,19 @@ __global__ void __launch_bounds__(kTailThreads) seanet_tail_kernel(const float* 
     __syncthreads();
   }
   if (tid < kTailOut && t0 + tid < length) {  // y = conv7(ELU(z)) (32 -> 1)
-    float acc = sp[kOffBf];
+    float acc = sp[kTailBf];
 #pragma unroll
     for (int j = 0; j < 7; ++j) {
       const float* zr = sz + (tid + j) * 33;
 #pragma unroll 8
-      for (int ci = 0; ci < 32; ++ci) acc = fmaf(sp[kOffWf + j * 32 + ci], zr[ci], acc);
+      for (int ci = 0; ci < 32; ++ci) acc = fmaf(sp[kTailWf + j * 32 + ci], zr[ci], acc);
     }
     y[b * y_bs + t0 + tid] = acc;
   }
 }
 
 // ------------------------------------------------------------------------------------------------
-// 4. Encoder head, the 32-channel stage at the full sample rate, fp32:
+// 5. Encoder head, the 32-channel stage at the full sample rate, fp32:
 //      z0 = conv7(x) (1 -> 32),  z1 = shortcut(z0) + conv1(ELU(conv3(ELU(z0)))),  out = bf16(ELU(z1)) reflect-padded
 //      by 2 (the A operand of the first strided conv's GEMM), every conv causal with reflect left padding.
 // One CTA = one batch element x kHeadOut positions t0 .. t0 + kHeadOut - 1 of z1; 128 threads.  Phase 1: thread r
@@ -407,15 +407,13 @@ __global__ void __launch_bounds__(kTailThreads) seanet_tail_kernel(const float* 
 // directly at their source positions 1, 2.  Phase 2: thread i < kHeadOut computes h and z1 at t0 + i from z0 rows
 // i .. i + 2 and writes output row t0 + i + 2; threads 1 and 2 of the first tile also write the reflected rows 1, 0.
 // x window: positions t0 - 8 .. t0 + kHeadOut - 1.  Parameters (NS2_SEANET_HEAD_PARAMS floats, input-major):
-//   w0 [7][32] (tap, out)  b0 [32]  w3 [3][32][16] (tap, in, out)  b3 [16]  wsc [32][32] (in, out)
-//   wc1 [16][32] (in, out)  b2 [32] = b_sc + b_c1
+//   w0 [7][32] (tap, out)  b0 [32]  the ResnetBlock's (section 3)
 // ------------------------------------------------------------------------------------------------
 constexpr int kHeadThreads = 128;
 constexpr int kHeadOut = kHeadThreads - 2;
 constexpr int kHeadXRows = kHeadOut + 8;
-constexpr int kHOffW0 = 0, kHOffB0 = 224, kHOffW3 = 256, kHOffB3 = 1792, kHOffWsc = 1808, kHOffWc1 = 2832,
-              kHOffB2 = 3344;
-static_assert(kHOffB2 + 32 == NS2_SEANET_HEAD_PARAMS, "head parameter layout");
+constexpr int kHeadW0 = 0, kHeadB0 = kHeadW0 + 7 * 32, kHeadBlk = kHeadB0 + 32;
+static_assert(kHeadBlk + kBlkFloats == NS2_SEANET_HEAD_PARAMS, "head parameter layout");
 constexpr int kHeadSmemFloats = NS2_SEANET_HEAD_PARAMS + ((kHeadXRows + 3) & ~3) + 2 * kHeadThreads * 33;
 
 __global__ void __launch_bounds__(kHeadThreads) seanet_head_kernel(const float* __restrict__ x, long long x_bs,
@@ -436,12 +434,7 @@ __global__ void __launch_bounds__(kHeadThreads) seanet_head_kernel(const float* 
     head_smem4[i] = __ldg(reinterpret_cast<const float4*>(prm) + i);
   for (int i = tid; i < kHeadXRows; i += kHeadThreads) {
     int t = t0 - 8 + i;
-    bool zero = t >= length || t < -6;
-    if (t < 0 && !zero) {  // the k7 conv's reflect pad (6), zero-extended when the input is that short
-      t = -t;
-      zero = t >= length;
-    }
-    sx[i] = zero ? 0.f : __ldg(xb + t);
+    sx[i] = reflect_src(t, length, 6) ? __ldg(xb + t) : 0.f;  // the k7 conv's reflect pad
   }
   __syncthreads();
 
@@ -451,21 +444,10 @@ __global__ void __launch_bounds__(kHeadThreads) seanet_head_kernel(const float* 
     float acc[32];
     if (src < length) {
 #pragma unroll
-      for (int o = 0; o < 32; ++o) acc[o] = sp[kHOffB0 + o];
+      for (int o = 0; o < 32; ++o) acc[o] = sp[kHeadB0 + o];
       const float* xr = sx + src - t0 + 2;
 #pragma unroll
-      for (int j = 0; j < 7; ++j) {
-        const float v = xr[j];
-        const float4* wr = reinterpret_cast<const float4*>(sp + kHOffW0 + j * 32);
-#pragma unroll
-        for (int o4 = 0; o4 < 8; ++o4) {
-          const float4 wv = wr[o4];
-          acc[4 * o4] = fmaf(wv.x, v, acc[4 * o4]);
-          acc[4 * o4 + 1] = fmaf(wv.y, v, acc[4 * o4 + 1]);
-          acc[4 * o4 + 2] = fmaf(wv.z, v, acc[4 * o4 + 2]);
-          acc[4 * o4 + 3] = fmaf(wv.w, v, acc[4 * o4 + 3]);
-        }
-      }
+      for (int j = 0; j < 7; ++j) fma_row(acc, sp + kHeadW0 + j * 32, xr[j]);
     } else {  // past the end, or a reflected row of an input shorter than the pad (zero-extended)
 #pragma unroll
       for (int o = 0; o < 32; ++o) acc[o] = 0.f;
@@ -489,62 +471,13 @@ __global__ void __launch_bounds__(kHeadThreads) seanet_head_kernel(const float* 
     }
     return;
   }
-  float hv[16];
-  {  // h = conv3(ELU(z0)) (32 -> 16), then ELU
+  const float* blk = sp + kHeadBlk;
+  float hv[16];  // h = conv3(ELU(z0)) (32 -> 16), then ELU
+  resblock32_hidden(hv, blk, sze + tid * 33);
 #pragma unroll
-    for (int o = 0; o < 16; ++o) hv[o] = sp[kHOffB3 + o];
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-      const float* zr = sze + (tid + j) * 33;
-#pragma unroll 8
-      for (int ci = 0; ci < 32; ++ci) {
-        const float v = zr[ci];
-        const float4* wr = reinterpret_cast<const float4*>(sp + kHOffW3 + (j * 32 + ci) * 16);
-#pragma unroll
-        for (int o4 = 0; o4 < 4; ++o4) {
-          const float4 wv = wr[o4];
-          hv[4 * o4] = fmaf(wv.x, v, hv[4 * o4]);
-          hv[4 * o4 + 1] = fmaf(wv.y, v, hv[4 * o4 + 1]);
-          hv[4 * o4 + 2] = fmaf(wv.z, v, hv[4 * o4 + 2]);
-          hv[4 * o4 + 3] = fmaf(wv.w, v, hv[4 * o4 + 3]);
-        }
-      }
-    }
-#pragma unroll
-    for (int o = 0; o < 16; ++o) hv[o] = elu_f(hv[o]);
-  }
-  float acc[32];
-#pragma unroll
-  for (int o = 0; o < 32; ++o) acc[o] = sp[kHOffB2 + o];
-  {  // z1 = shortcut(z0) + conv1(ELU(h)) (32 -> 32, 16 -> 32)
-    const float* zr = sz + (tid + 2) * 33;
-#pragma unroll 4
-    for (int ci = 0; ci < 32; ++ci) {
-      const float v = zr[ci];
-      const float4* wr = reinterpret_cast<const float4*>(sp + kHOffWsc + ci * 32);
-#pragma unroll
-      for (int o4 = 0; o4 < 8; ++o4) {
-        const float4 wv = wr[o4];
-        acc[4 * o4] = fmaf(wv.x, v, acc[4 * o4]);
-        acc[4 * o4 + 1] = fmaf(wv.y, v, acc[4 * o4 + 1]);
-        acc[4 * o4 + 2] = fmaf(wv.z, v, acc[4 * o4 + 2]);
-        acc[4 * o4 + 3] = fmaf(wv.w, v, acc[4 * o4 + 3]);
-      }
-    }
-#pragma unroll
-    for (int hc = 0; hc < 16; ++hc) {
-      const float v = hv[hc];
-      const float4* wr = reinterpret_cast<const float4*>(sp + kHOffWc1 + hc * 32);
-#pragma unroll
-      for (int o4 = 0; o4 < 8; ++o4) {
-        const float4 wv = wr[o4];
-        acc[4 * o4] = fmaf(wv.x, v, acc[4 * o4]);
-        acc[4 * o4 + 1] = fmaf(wv.y, v, acc[4 * o4 + 1]);
-        acc[4 * o4 + 2] = fmaf(wv.z, v, acc[4 * o4 + 2]);
-        acc[4 * o4 + 3] = fmaf(wv.w, v, acc[4 * o4 + 3]);
-      }
-    }
-  }
+  for (int o = 0; o < 16; ++o) hv[o] = elu_f(hv[o]);
+  float acc[32];  // z1 = shortcut(z0) + conv1(ELU(h)) (32 -> 32, 16 -> 32)
+  resblock32_out<16>(acc, blk, sz + (tid + 2) * 33, hv);
   uint4 pk[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i)

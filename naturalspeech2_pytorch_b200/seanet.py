@@ -1,23 +1,18 @@
-"""`SEANetDecoder`: Encodec's 24 kHz SEANet decoder on sm_90a, the `decoder` of `EncodecRVQ` — what
-`codec.decode(audio)` runs at the end of `NaturalSpeech2.sample` (ns2.py:1496-1499) to turn 75 Hz latents into 24 kHz
-audio.
-
-Layers (token-major activations (B, time, channels); every conv causal with reflect left padding, weight norm folded):
-    0       Conv1d k7 128 -> 512                      elu_pad (pad 6) + 7-segment GEMM
-    1       2-layer LSTM(512), lstm(x)[0] + x         input projection GEMM + ns2_lstm_seq per layer
-    2-3     ELU, ConvTranspose1d k16 s8 512 -> 256    elu_pad + 2-segment GEMM (taps [0, s) shift 0, [s, 2s) shift 1)
-    4       ResnetBlock(256, hidden 128)              elu_pad (ELU | raw, pad 2) + 3-segment GEMM, elu_pad, one GEMM
-                                                      for conv1x1 + shortcut over [ELU(x) | x | ELU(h)]
-    5-10    the same at 256 -> 128 (k10 s5) and 128 -> 64 (k8 s4)
-    11-12   ELU, ConvTranspose1d k4 s2 64 -> 32       elu_pad + 2-segment GEMM
-    13-15   ResnetBlock(32, hidden 16), ELU, Conv1d k7 32 -> 1      ns2_seanet_tail (fp32)
-GEMM operands are bf16 with fp32 accumulation; activations between layers, the LSTM cell state and the tail stay fp32.
-The state_dict has the keys and shapes of transformers' `EncodecDecoder`; `load_encodec_state_dict` takes Meta
-`encodec` (and audiolm's `EncodecWrapper.model.decoder`) keys.  Inference only: there is no backward.
-
-`SEANetEncoder` is the other direction, the `encoder` of `EncodecRVQ` (24 kHz audio -> 75 Hz frames, what
-`NaturalSpeech2.forward` and `process_prompt` run on raw audio): a full-rate fp32 head kernel (`ns2_seanet_head`), the
-strided convs as 2-segment GEMMs, the decoder's ResnetBlock and LSTM mapping; see its docstring.
+"""Encodec's 24 kHz SEANet codec on sm_90a, both directions: `SEANetDecoder` is the `decoder` of `EncodecRVQ` (75 Hz
+latents -> 24 kHz audio, what `codec.decode(audio)` runs at the end of `NaturalSpeech2.sample`, ns2.py:1496-1499) and
+`SEANetEncoder` its `encoder` (24 kHz audio -> 75 Hz frames, what `NaturalSpeech2.forward` and `process_prompt` run on
+raw audio).  Each class docstring has its layer table; both are built from the same stages (`_SEANet`), on token-major
+activations (B, time, channels), every conv causal with reflect left padding, weight norm folded:
+    Conv1d k7                           elu_pad (pad 6) + 7-segment GEMM
+    2-layer LSTM(512), lstm(x)[0] + x   input projection GEMM + ns2_lstm_seq per layer
+    ResnetBlock(C, hidden C/2), C >= 64 elu_pad (ELU | raw, pad 2) + 3-segment GEMM, elu_pad, one GEMM for
+                                        conv1x1 + shortcut over [ELU(x) | x | ELU(h)]
+    ConvTranspose1d / Conv1d k 2s stride s      2-segment GEMM (`pack_conv_transpose`, `pack_strided_conv`)
+    the 32-channel stage at 24 kHz      one fp32 kernel: ns2_seanet_tail (decoder), ns2_seanet_head (encoder)
+GEMM operands are bf16 with fp32 accumulation; activations between layers, the LSTM cell state and the 32-channel
+kernels stay fp32.  The state_dicts have the keys and shapes of transformers' `EncodecDecoder` / `EncodecEncoder`;
+`load_encodec_state_dict` takes Meta `encodec` (and audiolm's `EncodecWrapper.model`) keys.  Inference only: there is
+no backward.
 """
 from __future__ import annotations
 
@@ -62,29 +57,42 @@ def pack_conv_transpose(w: torch.Tensor, b: torch.Tensor, s: int):
     return packed.to(torch.bfloat16).contiguous(), b.float().repeat(s).contiguous()
 
 
+def _pack_block32(w3, b3, w1, b1, w_sc, b_sc) -> torch.Tensor:
+    """Folded weights of the 32-channel ResnetBlock (conv3 (16, 32, 3), conv1x1 (32, 16, 1), shortcut (32, 32, 1)) ->
+    the 3120 floats both full-rate kernels read: w3 (tap, in, out) | b3 | shortcut (in, out) | conv1x1 (in, out) |
+    b_sc + b1."""
+    return torch.cat([w3.permute(2, 1, 0).reshape(-1), b3, w_sc[:, :, 0].t().reshape(-1), w1[:, :, 0].t().reshape(-1),
+                      b_sc + b1])
+
+
 def pack_tail(w3, b3, w1, b1, w_sc, b_sc, w_f, b_f) -> torch.Tensor:
-    """Folded weights of the 32-channel ResnetBlock (conv3 (16, 32, 3), conv1x1 (32, 16, 1), shortcut (32, 32, 1)) and
-    of the final conv (1, 32, 7) -> the NS2_SEANET_TAIL_PARAMS f32 layout of ns2_seanet_tail."""
-    p = torch.cat([w3.permute(2, 1, 0).reshape(-1), b3, w_sc[:, :, 0].t().reshape(-1), w1[:, :, 0].t().reshape(-1),
-                   b_sc + b1, w_f[0].t().reshape(-1), b_f.reshape(1), b_f.new_zeros(3)])
+    """Folded weights of the 32-channel ResnetBlock (`_pack_block32`) and of the final conv (1, 32, 7) -> the
+    NS2_SEANET_TAIL_PARAMS f32 layout of ns2_seanet_tail."""
+    p = torch.cat([_pack_block32(w3, b3, w1, b1, w_sc, b_sc), w_f[0].t().reshape(-1), b_f.reshape(1),
+                   b_f.new_zeros(3)])
     assert p.numel() == _lib.NS2_SEANET_TAIL_PARAMS
     return p.float().contiguous()
 
 
 def pack_head(w0, b0, w3, b3, w1, b1, w_sc, b_sc) -> torch.Tensor:
-    """Folded weights of the encoder's first conv (32, 1, 7) and of its 32-channel ResnetBlock (conv3 (16, 32, 3),
-    conv1x1 (32, 16, 1), shortcut (32, 32, 1)) -> the NS2_SEANET_HEAD_PARAMS f32 layout of ns2_seanet_head."""
-    p = torch.cat([w0[:, 0].t().reshape(-1), b0, w3.permute(2, 1, 0).reshape(-1), b3, w_sc[:, :, 0].t().reshape(-1),
-                   w1[:, :, 0].t().reshape(-1), b_sc + b1])
+    """Folded weights of the encoder's first conv (32, 1, 7) and of its 32-channel ResnetBlock (`_pack_block32`) -> the
+    NS2_SEANET_HEAD_PARAMS f32 layout of ns2_seanet_head."""
+    p = torch.cat([w0[:, 0].t().reshape(-1), b0, _pack_block32(w3, b3, w1, b1, w_sc, b_sc)])
     assert p.numel() == _lib.NS2_SEANET_HEAD_PARAMS
     return p.float().contiguous()
+
+
+def _pack_conv(w: torch.Tensor) -> torch.Tensor:
+    """Conv1d weight (C_out, C_in, k) -> the k-segment GEMM's bf16 pack (C_out, k C_in), tap-major: column
+    j C_in + ci = w[co, ci, j]."""
+    return w.permute(0, 2, 1).reshape(w.shape[0], -1).to(torch.bfloat16).contiguous()
 
 
 def pack_strided_conv(w: torch.Tensor) -> torch.Tensor:
     """Conv1d(k = 2s, stride s) weight (C_out, C_in, 2s) -> the 2-segment GEMM's bf16 pack (C_out, 2s C_in), tap-major:
     column j C_in + ci = w[co, ci, j].  With the input reflect-padded by s and viewed as rows of s samples, segment 0
     (taps [0, s)) reads row m - 1 and segment 1 (taps [s, 2s)) row m: output row m + 1 is conv output m."""
-    return w.permute(0, 2, 1).reshape(w.shape[0], -1).to(torch.bfloat16).contiguous()
+    return _pack_conv(w)
 
 
 def strided_conv_segs(s: int, c_in: int) -> list:
@@ -148,11 +156,12 @@ class _ResnetParams(nn.Module):
         self.shortcut = _WNConv(dim, dim, 1)
 
 
-class SEANetDecoder(_PackedCache):
-    """Encodec's SEANet decoder (24 kHz model): (B, N, 128) summed codewords -> (B, 1, 320 N) audio, fp32.
+class _SEANet(_PackedCache):
+    """What the two directions share: the constructor's configuration check, the per-shape workspace cache, and the
+    packing, workspace buffers and launches of the LSTM and ResnetBlock stages.  A subclass builds its `layers` (the
+    only registered sub-module, so the state_dict has transformers' keys), packs them, and runs them."""
 
-    The constructor takes transformers' `EncodecConfig` decoder fields; only the 24 kHz model's values are supported
-    (`SEANetDecoder.from_config(EncodecConfig())` or no arguments)."""
+    _part: str  # "decoder" or "encoder": the sub-module of Meta's EncodecModel this class loads
 
     def __init__(self, *, audio_channels: int = 1, num_filters: int = 32, upsampling_ratios: Sequence[int] = RATIOS,
                  hidden_size: int = 128, kernel_size: int = 7, last_kernel_size: int = 7, residual_kernel_size: int = 3,
@@ -167,31 +176,26 @@ class SEANetDecoder(_PackedCache):
                      num_residual_layers=num_residual_layers, compress=compress, num_lstm_layers=num_lstm_layers,
                      use_causal_conv=bool(use_causal_conv), pad_mode=pad_mode, norm_type=norm_type,
                      trim_right_ratio=float(trim_right_ratio), use_conv_shortcut=bool(use_conv_shortcut))
-        _check_config("SEANetDecoder", given)
-        scale = 2 ** len(RATIOS)
-        layers = [_WNConv(hidden_size, scale * num_filters, kernel_size), _LSTMParams(scale * num_filters, num_lstm_layers)]
-        for r in RATIOS:
-            dim = scale * num_filters
-            layers += [nn.ELU(), _WNConv(dim, dim // 2, 2 * r, stride=r, transposed=True),
-                       _ResnetParams(dim // 2, dim // 2 // compress, residual_kernel_size)]
-            scale //= 2
-        layers += [nn.ELU(), _WNConv(num_filters, audio_channels, last_kernel_size)]
-        self.layers = nn.ModuleList(layers)
+        _check_config(type(self).__name__, given)
+        self.layers = nn.ModuleList(self._build_layers(given))
         self._ws: "OrderedDict[tuple, Dict[str, torch.Tensor]]" = OrderedDict()
-        self.max_cached_shapes = 4  # LRU bound on per-(B, N) workspaces (~10 GB at (32, 1024))
+        # LRU bound on per-shape workspaces: ~10 GB each for the decoder at (B, N) = (32, 1024), ~6.5 GB each for the
+        # encoder at (B, T) = (32, 327680)
+        self.max_cached_shapes = 4
 
     @classmethod
-    def from_config(cls, config) -> "SEANetDecoder":
+    def from_config(cls, config):
         """From an object with transformers' `EncodecConfig` attribute names."""
         return cls(**{k: getattr(config, k) for k in SUPPORTED})
 
     def load_encodec_state_dict(self, sd: Dict[str, torch.Tensor], strict: bool = True):
-        """Load a Meta `encodec` SEANetDecoder state_dict (`EncodecModel.decoder`, also audiolm's
-        `EncodecWrapper.model.decoder`): `model.{i}.conv.conv.weight_g|weight_v|bias`, `model.{i}.convtr.convtr.*`,
-        `model.{i}.block.{j}.conv.conv.*`, `model.{i}.shortcut.conv.conv.*`, `model.1.lstm.*`.  A `decoder.` prefix
-        is stripped.  The mapping follows the upstream module layout; it has not been checked against a released
-        checkpoint, so load with strict=True and compare a decoded clip against the original decoder once."""
-        return self.load_state_dict(encodec_keys_to_transformers(sd, "decoder"), strict=strict)
+        """Load the state_dict of this direction's Meta `encodec` SEANet module (`EncodecModel.decoder` / `.encoder`,
+        also audiolm's `EncodecWrapper.model.decoder` / `.encoder`): `model.{i}.conv.conv.weight_g|weight_v|bias`,
+        `model.{i}.convtr.convtr.*`, `model.{i}.block.{j}.conv.conv.*`, `model.{i}.shortcut.conv.conv.*`,
+        `model.{i}.lstm.*`.  A `decoder.` / `encoder.` prefix is stripped.  The mapping follows the upstream module
+        layout; it has not been checked against a released checkpoint, so load with strict=True and compare the output
+        for one clip against the original module once."""
+        return self.load_state_dict(encodec_keys_to_transformers(sd, self._part), strict=strict)
 
     @property
     def device(self):
@@ -205,62 +209,125 @@ class SEANetDecoder(_PackedCache):
     # ----------------------------------------------------------------------------------------------
     # weight packing (folded weight norm, bf16, K-major; rebuilt when a parameter changes)
     # ----------------------------------------------------------------------------------------------
-    def _pack(self) -> Dict[str, torch.Tensor]:
-        bf = lambda t: t.to(torch.bfloat16).contiguous()
-        f32 = lambda t: t.float().contiguous()
-        P = {}
-        w, b = self.layers[0].folded()                              # (512, 128, 7)
-        P["c0_w"], P["c0_b"] = bf(w.permute(0, 2, 1).reshape(w.shape[0], -1)), f32(b)
-        lstm = self.layers[1].lstm
-        perm = lstm_gate_perm().to(w.device)
+    @staticmethod
+    def _pack_lstm(P: Dict[str, torch.Tensor], lstm: nn.LSTM) -> None:
+        perm = lstm_gate_perm().to(lstm.weight_ih_l0.device)
         for l in range(2):
-            P[f"l{l}_wih"] = bf(getattr(lstm, f"weight_ih_l{l}")[perm])
-            P[f"l{l}_whh"] = bf(getattr(lstm, f"weight_hh_l{l}")[perm])
-            P[f"l{l}_b"] = f32((getattr(lstm, f"bias_ih_l{l}") + getattr(lstm, f"bias_hh_l{l}"))[perm])
-        for si, s in enumerate(RATIOS):
-            P[f"t{si}_w"], P[f"t{si}_b"] = pack_conv_transpose(*self.layers[3 + 3 * si].folded(), s)
-            blk = self.layers[4 + 3 * si]
-            w3, b3 = blk.block[1].folded()                          # (H, D, 3)
-            w1, b1 = blk.block[3].folded()                          # (D, H, 1)
-            ws, bs = blk.shortcut.folded()                          # (D, D, 1)
-            if si < len(RATIOS) - 1:
-                P[f"r{si}_w3"], P[f"r{si}_b3"] = bf(w3.permute(0, 2, 1).reshape(w3.shape[0], -1)), f32(b3)
-                P[f"r{si}_w1"] = bf(torch.cat([ws[:, :, 0], w1[:, :, 0]], dim=1))
-                P[f"r{si}_b1"] = f32(bs + b1)
-            else:
-                P["tail"] = pack_tail(w3, b3, w1, b1, ws, bs, *self.layers[15].folded())
-        return P
+            P[f"l{l}_wih"] = getattr(lstm, f"weight_ih_l{l}")[perm].to(torch.bfloat16).contiguous()
+            P[f"l{l}_whh"] = getattr(lstm, f"weight_hh_l{l}")[perm].to(torch.bfloat16).contiguous()
+            P[f"l{l}_b"] = (getattr(lstm, f"bias_ih_l{l}") + getattr(lstm, f"bias_hh_l{l}"))[perm].float().contiguous()
+
+    @staticmethod
+    def _pack_resblock(P: Dict[str, torch.Tensor], si: int, blk: "_ResnetParams") -> None:
+        w3, b3 = blk.block[1].folded()                              # (H, D, 3)
+        w1, b1 = blk.block[3].folded()                              # (D, H, 1)
+        ws, bs = blk.shortcut.folded()                              # (D, D, 1)
+        P[f"r{si}_w3"], P[f"r{si}_b3"] = _pack_conv(w3), b3.float().contiguous()
+        P[f"r{si}_w1"] = torch.cat([ws[:, :, 0], w1[:, :, 0]], dim=1).to(torch.bfloat16).contiguous()
+        P[f"r{si}_b1"] = (bs + b1).float().contiguous()
 
     # ----------------------------------------------------------------------------------------------
-    # workspaces (per (B, N) shape, LRU-bounded)
+    # workspaces (per input shape, LRU-bounded)
     # ----------------------------------------------------------------------------------------------
-    def _workspace(self, B: int, N: int, dev) -> Dict[str, torch.Tensor]:
-        key = (B, N, str(dev))
+    def _workspace(self, B: int, n: int, dev) -> Dict[str, torch.Tensor]:
+        key = (B, n, str(dev))
         ws = self._ws.get(key)
         if ws is not None:
             self._ws.move_to_end(key)
             return ws
         while len(self._ws) >= self.max_cached_shapes:
             self._ws.popitem(last=False)
-        e = lambda *s, dt=torch.bfloat16: torch.empty(*s, device=dev, dtype=dt)
+        ws = self._ws[key] = self._alloc_workspace(
+            B, n, lambda *s, dt=torch.bfloat16: torch.empty(*s, device=dev, dtype=dt))
+        return ws
+
+    @staticmethod
+    def _resblock_ws(ws: Dict[str, torch.Tensor], e, si: int, B: int, L: int, c: int) -> None:
+        ws[f"blk{si}"] = e(B, L + 2, 2 * c + c // 2)                # [ELU(x) | x | ELU(h)], reflect-padded by 2
+        ws[f"h{si}"] = e(B, L + 2, c // 2, dt=torch.float32)
+        ws[f"z{si}"] = e(B, L + 2, c, dt=torch.float32)
+
+    # ----------------------------------------------------------------------------------------------
+    # stages
+    # ----------------------------------------------------------------------------------------------
+    @staticmethod
+    def _lstm_stage(P, ws, y: torch.Tensor, out: torch.Tensor) -> None:
+        """out = lstm(y)[0] + y, y and out (B, N, 512) fp32."""
+        ops.elu_pad(y, ws["xb"], pad=0, elu=False)
+        ops.gemm(ws["xb"], P["l0_wih"], ws["xp"], n=2048, epilogue=ops.EPI_F32, bias=P["l0_b"])
+        ops.lstm_seq(ws["xp"], P["l0_whh"], out_bf16=ws["xb"])
+        ops.gemm(ws["xb"], P["l1_wih"], ws["xp"], n=2048, epilogue=ops.EPI_F32, bias=P["l1_b"])
+        ops.lstm_seq(ws["xp"], P["l1_whh"], skip=y, out=out)
+
+    @staticmethod
+    def _resblock_stage(P, ws, si: int, x: torch.Tensor, c: int) -> torch.Tensor:
+        """ResnetBlock(c, hidden c / 2) of x (B, L, c) fp32 -> (B, L, c) fp32, a view of `z{si}`."""
+        h = c // 2
+        blk, hb, zo = ws[f"blk{si}"], ws[f"h{si}"], ws[f"z{si}"]
+        ops.elu_pad(x, blk, pad=2, elu=True, raw=True)              # [ELU(x) | x], reflect-padded by 2
+        ops.gemm(blk, P[f"r{si}_w3"], hb, n=h, epilogue=ops.EPI_F32, segs=ops.conv_segs(c, 3, 2), bias=P[f"r{si}_b3"])
+        ops.elu_pad(hb[:, 2:], blk[:, 2:, 2 * c:], pad=0, elu=True)
+        ops.gemm(blk, P[f"r{si}_w1"], zo, n=c, epilogue=ops.EPI_F32,
+                 segs=[(c, 0, c, 0, 0), (2 * c, c, h, 0, 0)], bias=P[f"r{si}_b1"])
+        return zo[:, 2:]
+
+
+class SEANetDecoder(_SEANet):
+    """Encodec's SEANet decoder (24 kHz model): (B, N, 128) summed codewords -> (B, 1, 320 N) audio, fp32.
+
+    Layers (transformers `EncodecDecoder` indices):
+        0       Conv1d k7 128 -> 512                  elu_pad (pad 6) + 7-segment GEMM
+        1       2-layer LSTM(512), lstm(x)[0] + x     the LSTM stage
+        2-3     ELU, ConvTranspose1d k16 s8 512 -> 256elu_pad + 2-segment GEMM (taps [0, s) shift 0, [s, 2s) shift 1)
+        4       ResnetBlock(256, hidden 128)          the ResnetBlock stage
+        5-10    the same at 256 -> 128 (k10 s5) and 128 -> 64 (k8 s4)
+        11-12   ELU, ConvTranspose1d k4 s2 64 -> 32   elu_pad + 2-segment GEMM
+        13-15   ResnetBlock(32, hidden 16), ELU, Conv1d k7 32 -> 1      ns2_seanet_tail (fp32)
+    The constructor takes transformers' `EncodecConfig` decoder fields; only the 24 kHz model's values are supported
+    (`SEANetDecoder.from_config(EncodecConfig())` or no arguments)."""
+
+    _part = "decoder"
+
+    def _build_layers(self, c: dict) -> list:
+        scale, nf = 2 ** len(RATIOS), c["num_filters"]
+        layers = [_WNConv(c["hidden_size"], scale * nf, c["kernel_size"]),
+                  _LSTMParams(scale * nf, c["num_lstm_layers"])]
+        for r in RATIOS:
+            dim = scale * nf
+            layers += [nn.ELU(), _WNConv(dim, dim // 2, 2 * r, stride=r, transposed=True),
+                       _ResnetParams(dim // 2, dim // 2 // c["compress"], c["residual_kernel_size"])]
+            scale //= 2
+        return layers + [nn.ELU(), _WNConv(nf, c["audio_channels"], c["last_kernel_size"])]
+
+    def _pack(self) -> Dict[str, torch.Tensor]:
+        P = {}
+        w, b = self.layers[0].folded()                              # (512, 128, 7)
+        P["c0_w"], P["c0_b"] = _pack_conv(w), b.float().contiguous()
+        self._pack_lstm(P, self.layers[1].lstm)
+        for si, s in enumerate(RATIOS):
+            P[f"t{si}_w"], P[f"t{si}_b"] = pack_conv_transpose(*self.layers[3 + 3 * si].folded(), s)
+            blk = self.layers[4 + 3 * si]
+            if si < len(RATIOS) - 1:
+                self._pack_resblock(P, si, blk)
+            else:
+                P["tail"] = pack_tail(*blk.block[1].folded(), *blk.block[3].folded(), *blk.shortcut.folded(),
+                                      *self.layers[15].folded())
+        return P
+
+    def _alloc_workspace(self, B: int, N: int, e) -> Dict[str, torch.Tensor]:
         f = torch.float32
         ws = {"a0": e(B, N + 6, 128), "y0": e(B, N + 6, 512, dt=f), "xb": e(B, N, 512), "xp": e(B, N, 2048, dt=f),
               "z": e(B, N, 512, dt=f)}
         L = N
         for si, s in enumerate(RATIOS):
             c_in = 512 >> si
-            c_out, h = c_in // 2, c_in // 4
             ws[f"at{si}"] = e(B, L, c_in)
-            ws[f"u{si}"] = e(B, L, s * c_out, dt=f)
+            ws[f"u{si}"] = e(B, L, s * c_in // 2, dt=f)
             L *= s
             if si < len(RATIOS) - 1:
-                ws[f"blk{si}"] = e(B, L + 2, 2 * c_out + h)
-                ws[f"h{si}"] = e(B, L + 2, h, dt=f)
-                ws[f"z{si}"] = e(B, L + 2, c_out, dt=f)
-        self._ws[key] = ws
+                self._resblock_ws(ws, e, si, B, L, c_in // 2)
         return ws
 
-    # ----------------------------------------------------------------------------------------------
     @torch.no_grad()
     def forward(self, emb: torch.Tensor) -> torch.Tensor:
         """emb (B, N, 128) -> audio (B, 1, 320 N) fp32."""
@@ -277,16 +344,11 @@ class SEANetDecoder(_PackedCache):
             ops.elu_pad(x, ws["a0"], pad=6, elu=False)
             ops.gemm(ws["a0"], P["c0_w"], ws["y0"], n=512, epilogue=ops.EPI_F32, segs=ops.conv_segs(128, 7, 6),
                      bias=P["c0_b"])
-            y0 = ws["y0"][:, 6:]
-            ops.elu_pad(y0, ws["xb"], pad=0, elu=False)
-            ops.gemm(ws["xb"], P["l0_wih"], ws["xp"], n=2048, epilogue=ops.EPI_F32, bias=P["l0_b"])
-            ops.lstm_seq(ws["xp"], P["l0_whh"], out_bf16=ws["xb"])
-            ops.gemm(ws["xb"], P["l1_wih"], ws["xp"], n=2048, epilogue=ops.EPI_F32, bias=P["l1_b"])
-            ops.lstm_seq(ws["xp"], P["l1_whh"], skip=y0, out=ws["z"])
+            self._lstm_stage(P, ws, ws["y0"][:, 6:], ws["z"])
             z, L = ws["z"], N
             for si, s in enumerate(RATIOS):
                 c_in = 512 >> si
-                c_out, h = c_in // 2, c_in // 4
+                c_out = c_in // 2
                 at, u = ws[f"at{si}"], ws[f"u{si}"]
                 ops.elu_pad(z, at, pad=0, elu=True)
                 ops.gemm(at, P[f"t{si}_w"], u, n=s * c_out, epilogue=ops.EPI_F32,
@@ -296,124 +358,52 @@ class SEANetDecoder(_PackedCache):
                 if si == len(RATIOS) - 1:
                     ops.seanet_tail(u, P["tail"], out.view(B, L))
                     break
-                blk, hb, zo = ws[f"blk{si}"], ws[f"h{si}"], ws[f"z{si}"]
-                ops.elu_pad(u, blk, pad=2, elu=True, raw=True)          # [ELU(x) | x], reflect-padded by 2
-                ops.gemm(blk, P[f"r{si}_w3"], hb, n=h, epilogue=ops.EPI_F32, segs=ops.conv_segs(c_out, 3, 2),
-                         bias=P[f"r{si}_b3"])
-                ops.elu_pad(hb[:, 2:], blk[:, 2:, 2 * c_out:], pad=0, elu=True)
-                ops.gemm(blk, P[f"r{si}_w1"], zo, n=c_out, epilogue=ops.EPI_F32,
-                         segs=[(c_out, 0, c_out, 0, 0), (2 * c_out, c_out, h, 0, 0)], bias=P[f"r{si}_b1"])
-                z = zo[:, 2:]
+                z = self._resblock_stage(P, ws, si, u, c_out)
         return out
 
 
-class SEANetEncoder(_PackedCache):
+class SEANetEncoder(_SEANet):
     """Encodec's SEANet encoder (24 kHz model): (B, T) or (B, 1, T) audio, T a multiple of 320 -> (B, T / 320, 128)
     token-major frames, fp32 — the `encoder` callable of `EncodecRVQ`.
 
-    Layers (transformers `EncodecEncoder` indices; every conv causal with reflect left padding, weight norm folded):
+    Layers (transformers `EncodecEncoder` indices):
         0-2     Conv1d k7 1 -> 32, ResnetBlock(32, hidden 16), ELU      ns2_seanet_head (fp32, bf16 output)
         3       Conv1d k4 stride 2 32 -> 64                             2-segment GEMM (`strided_conv_segs`)
-        4-5     ResnetBlock(64, hidden 32), ELU                         as in the decoder: elu_pad (ELU | raw, pad 2)
-                                                                        + 3-segment GEMM, elu_pad, one GEMM for
-                                                                        conv1x1 + shortcut, then elu_pad (pad s)
+        4-5     ResnetBlock(64, hidden 32), ELU                         the ResnetBlock stage, then elu_pad (pad s)
         6-11    the same at k8 s4 64 -> 128, ResnetBlock(128); k10 s5 128 -> 256, ResnetBlock(256)
         12      Conv1d k16 stride 8 256 -> 512                          2-segment GEMM
-        13      2-layer LSTM(512), lstm(x)[0] + x                       input projection GEMM + ns2_lstm_seq per layer
+        13      2-layer LSTM(512), lstm(x)[0] + x                       the LSTM stage
         14-15   ELU, Conv1d k7 512 -> 128                               elu_pad (pad 6) + 7-segment GEMM, fp32 out
-    The constructor takes transformers' `EncodecConfig` fields; only the 24 kHz model's values are supported.  The
-    state_dict has the keys and shapes of transformers' `EncodecEncoder`.  Inference only: there is no backward."""
+    The constructor takes transformers' `EncodecConfig` fields; only the 24 kHz model's values are supported."""
 
-    def __init__(self, *, audio_channels: int = 1, num_filters: int = 32, upsampling_ratios: Sequence[int] = RATIOS,
-                 hidden_size: int = 128, kernel_size: int = 7, last_kernel_size: int = 7, residual_kernel_size: int = 3,
-                 dilation_growth_rate: int = 2, num_residual_layers: int = 1, compress: int = 2,
-                 num_lstm_layers: int = 2, use_causal_conv: bool = True, pad_mode: str = "reflect",
-                 norm_type: str = "weight_norm", trim_right_ratio: float = 1.0, use_conv_shortcut: bool = True):
-        super().__init__()
-        given = dict(audio_channels=audio_channels, num_filters=num_filters,
-                     upsampling_ratios=tuple(int(r) for r in upsampling_ratios), hidden_size=hidden_size,
-                     kernel_size=kernel_size, last_kernel_size=last_kernel_size,
-                     residual_kernel_size=residual_kernel_size, dilation_growth_rate=dilation_growth_rate,
-                     num_residual_layers=num_residual_layers, compress=compress, num_lstm_layers=num_lstm_layers,
-                     use_causal_conv=bool(use_causal_conv), pad_mode=pad_mode, norm_type=norm_type,
-                     trim_right_ratio=float(trim_right_ratio), use_conv_shortcut=bool(use_conv_shortcut))
-        _check_config("SEANetEncoder", given)
-        layers = [_WNConv(audio_channels, num_filters, kernel_size)]
-        dim = num_filters
+    _part = "encoder"
+
+    def _build_layers(self, c: dict) -> list:
+        dim = c["num_filters"]
+        layers = [_WNConv(c["audio_channels"], dim, c["kernel_size"])]
         for r in reversed(RATIOS):
-            layers += [_ResnetParams(dim, dim // compress, residual_kernel_size), nn.ELU(),
+            layers += [_ResnetParams(dim, dim // c["compress"], c["residual_kernel_size"]), nn.ELU(),
                        _WNConv(dim, 2 * dim, 2 * r, stride=r)]
             dim *= 2
-        layers += [_LSTMParams(dim, num_lstm_layers), nn.ELU(), _WNConv(dim, hidden_size, last_kernel_size)]
-        self.layers = nn.ModuleList(layers)
-        self._ws: "OrderedDict[tuple, Dict[str, torch.Tensor]]" = OrderedDict()
-        self.max_cached_shapes = 4  # LRU bound on per-(B, T) workspaces (~6.5 GB at (32, 327680))
+        return layers + [_LSTMParams(dim, c["num_lstm_layers"]), nn.ELU(),
+                         _WNConv(dim, c["hidden_size"], c["last_kernel_size"])]
 
-    @classmethod
-    def from_config(cls, config) -> "SEANetEncoder":
-        """From an object with transformers' `EncodecConfig` attribute names."""
-        return cls(**{k: getattr(config, k) for k in SUPPORTED})
-
-    def load_encodec_state_dict(self, sd: Dict[str, torch.Tensor], strict: bool = True):
-        """Load a Meta `encodec` SEANetEncoder state_dict (`EncodecModel.encoder`, also audiolm's
-        `EncodecWrapper.model.encoder`): `model.{i}.conv.conv.weight_g|weight_v|bias`, `model.{i}.block.{j}.conv.conv.*`,
-        `model.{i}.shortcut.conv.conv.*`, `model.13.lstm.*`.  An `encoder.` prefix is stripped.  The mapping follows
-        the upstream module layout; it has not been checked against a released checkpoint, so load with strict=True
-        and compare the frames of one clip against the original encoder once."""
-        return self.load_state_dict(encodec_keys_to_transformers(sd, "encoder"), strict=strict)
-
-    @property
-    def device(self):
-        return next(self.parameters()).device
-
-    def _apply(self, fn, *args, **kwargs):
-        out = super()._apply(fn, *args, **kwargs)
-        self._ws.clear()
-        return out
-
-    # ----------------------------------------------------------------------------------------------
-    # weight packing (folded weight norm, bf16, K-major; rebuilt when a parameter changes)
-    # ----------------------------------------------------------------------------------------------
     def _pack(self) -> Dict[str, torch.Tensor]:
-        bf = lambda t: t.to(torch.bfloat16).contiguous()
-        f32 = lambda t: t.float().contiguous()
         P = {}
         blk = self.layers[1]
         P["head"] = pack_head(*self.layers[0].folded(), *blk.block[1].folded(), *blk.block[3].folded(),
                               *blk.shortcut.folded())
         for si in range(len(RATIOS)):
             w, b = self.layers[3 + 3 * si].folded()                 # (2C, C, 2s)
-            P[f"s{si}_w"], P[f"s{si}_b"] = pack_strided_conv(w), f32(b)
+            P[f"s{si}_w"], P[f"s{si}_b"] = pack_strided_conv(w), b.float().contiguous()
             if si < len(RATIOS) - 1:
-                blk = self.layers[4 + 3 * si]
-                w3, b3 = blk.block[1].folded()                      # (H, D, 3)
-                w1, b1 = blk.block[3].folded()                      # (D, H, 1)
-                ws, bs = blk.shortcut.folded()                      # (D, D, 1)
-                P[f"r{si}_w3"], P[f"r{si}_b3"] = bf(w3.permute(0, 2, 1).reshape(w3.shape[0], -1)), f32(b3)
-                P[f"r{si}_w1"] = bf(torch.cat([ws[:, :, 0], w1[:, :, 0]], dim=1))
-                P[f"r{si}_b1"] = f32(bs + b1)
-        lstm = self.layers[13].lstm
-        perm = lstm_gate_perm().to(w.device)
-        for l in range(2):
-            P[f"l{l}_wih"] = bf(getattr(lstm, f"weight_ih_l{l}")[perm])
-            P[f"l{l}_whh"] = bf(getattr(lstm, f"weight_hh_l{l}")[perm])
-            P[f"l{l}_b"] = f32((getattr(lstm, f"bias_ih_l{l}") + getattr(lstm, f"bias_hh_l{l}"))[perm])
+                self._pack_resblock(P, si, self.layers[4 + 3 * si])
+        self._pack_lstm(P, self.layers[13].lstm)
         w, b = self.layers[15].folded()                             # (128, 512, 7)
-        P["c15_w"], P["c15_b"] = bf(w.permute(0, 2, 1).reshape(w.shape[0], -1)), f32(b)
+        P["c15_w"], P["c15_b"] = _pack_conv(w), b.float().contiguous()
         return P
 
-    # ----------------------------------------------------------------------------------------------
-    # workspaces (per (B, T) shape, LRU-bounded)
-    # ----------------------------------------------------------------------------------------------
-    def _workspace(self, B: int, T: int, dev) -> Dict[str, torch.Tensor]:
-        key = (B, T, str(dev))
-        ws = self._ws.get(key)
-        if ws is not None:
-            self._ws.move_to_end(key)
-            return ws
-        while len(self._ws) >= self.max_cached_shapes:
-            self._ws.popitem(last=False)
-        e = lambda *s, dt=torch.bfloat16: torch.empty(*s, device=dev, dtype=dt)
+    def _alloc_workspace(self, B: int, T: int, e) -> Dict[str, torch.Tensor]:
         f = torch.float32
         strides = tuple(reversed(RATIOS))
         ws = {"a0": e(B, T + strides[0], 32)}
@@ -423,17 +413,12 @@ class SEANetEncoder(_PackedCache):
             L //= s
             ws[f"y{si}"] = e(B, L + 1, c_out, dt=f)                 # row 0: the strided GEMM's scratch row
             if si < len(strides) - 1:
-                h = c_out // 2
-                ws[f"blk{si}"] = e(B, L + 2, 2 * c_out + h)
-                ws[f"h{si}"] = e(B, L + 2, h, dt=f)
-                ws[f"z{si}"] = e(B, L + 2, c_out, dt=f)
+                self._resblock_ws(ws, e, si, B, L, c_out)
                 ws[f"a{si + 1}"] = e(B, L + strides[si + 1], c_out)
         N = L
         ws.update(xb=e(B, N, 512), xp=e(B, N, 2048, dt=f), lz=e(B, N, 512, dt=f), a15=e(B, N + 6, 512))
-        self._ws[key] = ws
         return ws
 
-    # ----------------------------------------------------------------------------------------------
     @torch.no_grad()
     def forward(self, audio: torch.Tensor) -> torch.Tensor:
         """audio (B, T) or (B, 1, T), T % 320 == 0 -> frames (B, T / 320, 128) fp32, a new tensor per call."""
@@ -466,21 +451,10 @@ class SEANetEncoder(_PackedCache):
                 y = y[:, 1:]
                 if si == len(strides) - 1:
                     break
-                h = c_out // 2
-                blk, hb, zo, a = ws[f"blk{si}"], ws[f"h{si}"], ws[f"z{si}"], ws[f"a{si + 1}"]
-                ops.elu_pad(y, blk, pad=2, elu=True, raw=True)          # [ELU(x) | x], reflect-padded by 2
-                ops.gemm(blk, P[f"r{si}_w3"], hb, n=h, epilogue=ops.EPI_F32, segs=ops.conv_segs(c_out, 3, 2),
-                         bias=P[f"r{si}_b3"])
-                ops.elu_pad(hb[:, 2:], blk[:, 2:, 2 * c_out:], pad=0, elu=True)
-                ops.gemm(blk, P[f"r{si}_w1"], zo, n=c_out, epilogue=ops.EPI_F32,
-                         segs=[(c_out, 0, c_out, 0, 0), (2 * c_out, c_out, h, 0, 0)], bias=P[f"r{si}_b1"])
-                ops.elu_pad(zo[:, 2:], a, pad=strides[si + 1], elu=True)
+                a = ws[f"a{si + 1}"]
+                ops.elu_pad(self._resblock_stage(P, ws, si, y, c_out), a, pad=strides[si + 1], elu=True)
                 c_in = c_out
-            ops.elu_pad(y, ws["xb"], pad=0, elu=False)
-            ops.gemm(ws["xb"], P["l0_wih"], ws["xp"], n=2048, epilogue=ops.EPI_F32, bias=P["l0_b"])
-            ops.lstm_seq(ws["xp"], P["l0_whh"], out_bf16=ws["xb"])
-            ops.gemm(ws["xb"], P["l1_wih"], ws["xp"], n=2048, epilogue=ops.EPI_F32, bias=P["l1_b"])
-            ops.lstm_seq(ws["xp"], P["l1_whh"], skip=y, out=ws["lz"])
+            self._lstm_stage(P, ws, y, ws["lz"])
             ops.elu_pad(ws["lz"], ws["a15"], pad=6, elu=True)
             ops.gemm(ws["a15"], P["c15_w"], frames, n=128, epilogue=ops.EPI_F32, segs=ops.conv_segs(512, 7, 6),
                      bias=P["c15_b"])

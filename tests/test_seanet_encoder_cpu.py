@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from golden.make_golden_seanet_encoder import CASES, audio, filled_state_dict
-import seanet_encoder_oracle
+import seanet_oracle
 
 
 @pytest.fixture(scope="module")
@@ -26,7 +26,7 @@ def keys_shapes(golden):
 @pytest.mark.parametrize("case", sorted(CASES))
 def test_oracle_matches_transformers_fp64(golden, keys_shapes, case):
     B, N = CASES[case]
-    f = seanet_encoder_oracle.encode(filled_state_dict(keys_shapes), audio(B, N), dtype=torch.float64)
+    f = seanet_oracle.encode(filled_state_dict(keys_shapes), audio(B, N), dtype=torch.float64)
     assert tuple(f.shape) == (B, N, 128)
     ref = torch.from_numpy(golden[f"{case}_f64"])
     assert float((f - ref).abs().max()) <= 1e-9 * max(1.0, float(ref.abs().max()))
@@ -35,8 +35,8 @@ def test_oracle_matches_transformers_fp64(golden, keys_shapes, case):
 def test_oracle_bf16_emulation_error_is_the_autocast_scale(golden, keys_shapes):
     """The bf16-operand emulation lands at the same error scale as transformers under CPU autocast (within 2x)."""
     sd = filled_state_dict(keys_shapes)
-    f64 = seanet_encoder_oracle.encode(sd, audio(2, 75))
-    fem = seanet_encoder_oracle.encode(sd, audio(2, 75), emulate_bf16=True)
+    f64 = seanet_oracle.encode(sd, audio(2, 75))
+    fem = seanet_oracle.encode(sd, audio(2, 75), emulate_bf16=True)
     rel = float((fem - f64).norm() / f64.norm())
     auto = float(golden["b2n75_err"][2])
     assert auto / 2 < rel < 2 * auto, (rel, auto)

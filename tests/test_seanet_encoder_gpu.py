@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from golden.make_golden_seanet_encoder import CASES, audio, codebooks, filled_state_dict
-import seanet_encoder_oracle
+import seanet_oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -59,8 +59,8 @@ def test_encoder_against_fp64_oracle_long_sequence(sd64, enc):
     B, N = 4, 1024
     x = audio(B, N).cuda()
     sdc = {k: v.cuda() for k, v in sd64.items()}
-    f64 = seanet_encoder_oracle.encode(sdc, x, dtype=torch.float64)
-    fem = seanet_encoder_oracle.encode(sdc, x, dtype=torch.float64, emulate_bf16=True)
+    f64 = seanet_oracle.encode(sdc, x, dtype=torch.float64)
+    fem = seanet_oracle.encode(sdc, x, dtype=torch.float64, emulate_bf16=True)
     f = enc(x.float())
     rel, mx = _err(f, f64)
     em_rel, em_max = _err(fem, f64)

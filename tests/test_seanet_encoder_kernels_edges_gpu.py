@@ -47,7 +47,7 @@ def _head_ref(x, sd, pad=None):
     if pad is not None:
         seanet_oracle.reflect_pad_left = pad
     try:
-        z0 = seanet_oracle._conv(x.double()[:, None], sd, "layers.0.conv", False)
+        z0 = seanet_oracle.conv(x.double()[:, None], sd, "layers.0.conv", False)
         z1 = seanet_oracle.resnet_block(z0, sd, "layers.1")
         y = seanet_oracle.reflect_pad_left(F.elu(z1), 2)
     finally:

@@ -200,7 +200,7 @@ def _tail_ref(x, sd, zero_pad=False):
         seanet_oracle.reflect_pad_left = lambda t, p: F.pad(t, (p, 0))
     try:
         z = seanet_oracle.resnet_block(xc, sd, "layers.13")
-        y = seanet_oracle._conv(F.elu(z), sd, "layers.15.conv", False)
+        y = seanet_oracle.conv(F.elu(z), sd, "layers.15.conv", False)
     finally:
         if zero_pad:
             seanet_oracle.reflect_pad_left = orig

@@ -20,7 +20,6 @@ sys.path.insert(0, str(ROOT / "tests"))
 import torch  # noqa: E402
 import torch.nn.functional as F  # noqa: E402
 
-import seanet_encoder_oracle  # noqa: E402
 import seanet_oracle  # noqa: E402
 from golden.make_golden_seanet import filled_state_dict  # noqa: E402
 from golden import make_golden_seanet_encoder as genc  # noqa: E402
@@ -38,14 +37,14 @@ def torch_decoder(sd, dtype):
 
     @torch.no_grad()
     def run(emb):
-        x = seanet_oracle._conv(emb.to(dtype).transpose(1, 2), sdd, "layers.0.conv", False)
+        x = seanet_oracle.conv(emb.to(dtype).transpose(1, 2), sdd, "layers.0.conv", False)
         xt = x.permute(2, 0, 1)
         x = (lstm(xt)[0] + xt).permute(1, 2, 0)
         for si, s in enumerate(seanet_oracle.RATIOS):
             i = 2 + 3 * si
             x = seanet_oracle._conv_t(F.elu(x), sdd, f"layers.{i + 1}.conv", s, False)
             x = seanet_oracle.resnet_block(x, sdd, f"layers.{i + 2}")
-        return seanet_oracle._conv(F.elu(x), sdd, "layers.15.conv", False).float()
+        return seanet_oracle.conv(F.elu(x), sdd, "layers.15.conv", False).float()
     return run
 
 
@@ -58,14 +57,14 @@ def torch_encoder(sd, dtype):
 
     @torch.no_grad()
     def run(audio):
-        x = seanet_encoder_oracle.conv(audio.to(dtype)[:, None], sdd, "layers.0.conv", False)
+        x = seanet_oracle.conv(audio.to(dtype)[:, None], sdd, "layers.0.conv", False)
         for si, s in enumerate(reversed(seanet_oracle.RATIOS)):
             i = 1 + 3 * si
             x = seanet_oracle.resnet_block(x, sdd, f"layers.{i}")
-            x = seanet_encoder_oracle.conv(F.elu(x), sdd, f"layers.{i + 2}.conv", False, stride=s)
+            x = seanet_oracle.conv(F.elu(x), sdd, f"layers.{i + 2}.conv", False, stride=s)
         xt = x.permute(2, 0, 1)
         x = (lstm(xt)[0] + xt).permute(1, 2, 0)
-        return seanet_encoder_oracle.conv(F.elu(x), sdd, "layers.15.conv", False).transpose(1, 2).float()
+        return seanet_oracle.conv(F.elu(x), sdd, "layers.15.conv", False).transpose(1, 2).float()
     return run
 
 

@@ -418,6 +418,29 @@ int ns2_add_rows_bcast(float* x, int32_t batch, int32_t rows, int32_t dim, const
                        ns2_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * 8c. Backward of the duration / pitch predictor (DurationPitchPredictor ns2.py:345-527, trained through the L1
+ *     losses of ns2.py:1579-1590).  Its k=3 "same" convs use ns2_gemm / ns2_wgrad (shifts +1..-1), its cross
+ *     attention and RMSNorm(gamma) section 8.  Both entries are deterministic: per-CTA partial sums in a caller-provided
+ *     workspace, then a second launch adds them in a fixed order (no atomics).
+ *    ns2_groupnorm_silu_bwd : backward of ns2_groupnorm_silu (without its residual, an identity the caller adds) given
+ *                             dy f32 (batch, rows, channels): with xh = (x - mean) * rstd (statistics recomputed as the
+ *                             forward computes them), z = xh * weight + bias, dz = dy * silu'(z), dxh = dz * weight,
+ *                               dx = rstd * (dxh - mean(dxh) - xh * mean(dxh * xh))   (means over the group of a sample)
+ *                             written as bf16; dweight[c] = sum dz * xh, dbias[c] = sum dz (overwritten).  channels /
+ *                             groups a multiple of 4 and <= 1024, batch <= 65535.  partial: 2 * batch * channels floats.
+ *    ns2_rowdot_bwd         : backward of ns2_rowdot with relu: dpre[r] = pred[r] > 0 ? dpred[r] : 0 (0 at pred == 0,
+ *                             as torch's threshold_backward); dx[r, :] += dpre[r] * w (f32, in place); dw[:] =
+ *                             sum_r dpre[r] * x[r, :], db[0] = sum_r dpre[r] (overwritten).  partial:
+ *                             ceil(rows / NS2_ROWDOT_BWD_ROWS) * (dim + 4) floats.
+ * ------------------------------------------------------------------------------------------------ */
+#define NS2_ROWDOT_BWD_ROWS 32
+int ns2_groupnorm_silu_bwd(const float* x, int32_t batch, int32_t rows, int32_t channels, int32_t groups,
+                           const float* weight, const float* bias, float eps, const float* dy, void* dx_bf16,
+                           float* partial, float* dweight, float* dbias, ns2_stream_t stream);
+int ns2_rowdot_bwd(const float* x, int64_t rows, int32_t dim, const float* w, const float* pred, const float* dpred,
+                   float* dx, float* partial, float* dw, float* db, ns2_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * 9. Monotonic alignment search: `maximum_path(value, mask)` of naturalspeech2_pytorch/aligner.py:88-122 (called from
  *    Aligner.forward aligner.py:214, reached from NaturalSpeech2.forward ns2.py:1578 in conditional training).
  *    value, mask: f32 (batch, t_x, t_y) contiguous (t_x text positions <= 1024, t_y mel frames); mask holds 0/1.

@@ -20,6 +20,7 @@ NS2_GEMM_FLAG_SKIP_EPILOGUE, NS2_GEMM_FLAG_SILU = 1, 4
 NS2_ELU_PAD_ELU, NS2_ELU_PAD_RAW = 1, 2
 NS2_SEANET_TAIL_PARAMS = 3348
 NS2_SEANET_HEAD_PARAMS = 3376
+NS2_ROWDOT_BWD_ROWS = 32
 NS2_ABI_VERSION = 7
 
 
@@ -131,6 +132,8 @@ SIGNATURES = {
     "ns2_embedding_bwd": (C.c_int, [_P, _I64, _P, _I32, _I32, _I32, _P, _P]),
     "ns2_expand_encodings_bwd": (C.c_int, [_P, _I64, _P, _I32, _P, _I32, _I32, _I32, _I32, _P, _P, _P]),
     "ns2_add_rows_bcast": (C.c_int, [_P, _I32, _I32, _I32, _P, _F, _P]),
+    "ns2_groupnorm_silu_bwd": (C.c_int, [_P, _I32, _I32, _I32, _I32, _P, _P, _F, _P, _P, _P, _P, _P, _P]),
+    "ns2_rowdot_bwd": (C.c_int, [_P, _I64, _I32, _P, _P, _P, _P, _P, _P, _P, _P]),
     "ns2_rvq_prepare": (C.c_int, [_P, _I32, _I32, _I32, _P, _P, _P, _P]),
     "ns2_rvq_encode": (C.c_int, [_P, _I64, _I32, _P, _P, _P, _P, _I32, _I32, _P, _P, _P]),
     "ns2_rvq_decode": (C.c_int, [_P, _I64, _I32, _I32, _I32, _P, _P, _P]),
@@ -167,7 +170,11 @@ def load() -> C.CDLL:
             "`python -c 'import __graft_entry__ as g; g.build()'` (needs nvcc). There is no fallback path.")
     lib = C.CDLL(str(_LIB_PATH))
     for name, (res, args) in SIGNATURES.items():
-        fn = getattr(lib, name)  # AttributeError here means header / library mismatch
+        try:
+            fn = getattr(lib, name)
+        except AttributeError:
+            raise Ns2Error(f"ABI mismatch: {_LIB_PATH} does not export {name} (a library built from older sources); "
+                           "rebuild it with `python -m naturalspeech2_pytorch_b200.build --force`") from None
         fn.restype = res
         fn.argtypes = args
     if lib.ns2_abi_version() != NS2_ABI_VERSION:

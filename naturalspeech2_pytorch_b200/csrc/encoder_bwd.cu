@@ -11,7 +11,11 @@
 //   add_rows_bcast         d prompt of the prompt FiLM vector's mean-pool (Reduce 'b n d -> b d' mean, ns2.py:858-862)
 //   dropout_f32            the phoneme encoder's conv dropout (nn.Dropout after the causal conv's SiLU, ns2.py:258) on
 //                          the forward activation and, with the same mask, on its gradient (philox.cuh element stream)
-// All HBM-bound.  The scatters accumulate with fp32 atomics, so their summation order is not fixed.
+// and those of the duration / pitch predictor (ns2.py:345-527), trained through its L1 losses (ns2.py:1579-1590):
+//   groupnorm_silu_bwd     Block's GroupNorm + SiLU (ns2.py:345-365); the ResnetBlock residual (399-401) is the caller's
+//   rowdot_bwd             the Linear(dim, 1) + ReLU heads (ns2.py:451-455)
+// All HBM-bound.  The scatters accumulate with fp32 atomics, so their summation order is not fixed; the predictor's
+// parameter sums go through per-CTA partials and a fixed-order second pass, so they are.
 #include "host_common.h"
 #include "philox.cuh"
 #include "../../include/ns2_b200.h"
@@ -147,6 +151,178 @@ unsigned grid_cap(long long n) {
   return static_cast<unsigned>(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
+// ---- duration / pitch predictor (ns2.py:345-527) ----
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// The 256-thread block sum of groupnorm_silu_kernel (elementwise.cu), so that the recomputed statistics are the
+// forward's bit for bit.
+__device__ __forceinline__ float block_sum_256(float v, float* red) {
+  v = warp_sum(v);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  __syncthreads();
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  float t = (lane < 8) ? red[lane] : 0.f;
+  t = warp_sum(t);
+  return t;
+}
+
+// d z of y = silu(z), z = xh * w + b, and d xh = d z * w (fp32; __expf like the forward).
+__device__ __forceinline__ float gn_silu_dz(float xh, float w, float b, float dy) {
+  const float z = xh * w + b;
+  const float s = 1.0f / (1.0f + __expf(-z));
+  return dy * s * (1.0f + z * (1.0f - s));
+}
+
+// Backward of groupnorm_silu_kernel.  One CTA per (group, batch element), like the forward:
+//   passes 1-2  mean and rstd, the forward's code and summation order
+//   pass 3      each thread owns one channel quad (c4 = tid % v4) and walks rows r0, r0 + rstep, ...: per-channel
+//               sums of dz * xh and dz (d gamma / d beta of this sample) and the group sums of dxh and dxh * xh
+//   pass 4      dx = rstd * (dxh - mean(dxh) - xh * mean(dxh * xh)), written as bf16
+// The per-channel sums of the CTA's threads are added in a fixed order through shared memory and written to
+// partial[b][0 / 1][channel]; sum_parts_kernel reduces them over the batch.  No atomics anywhere.
+__global__ void __launch_bounds__(256) groupnorm_silu_bwd_kernel(const float* __restrict__ x, int rows, int channels,
+                                                                 int cpg, const float* __restrict__ weight,
+                                                                 const float* __restrict__ bias, float eps,
+                                                                 const float* __restrict__ dy,
+                                                                 __nv_bfloat16* __restrict__ dx,
+                                                                 float* __restrict__ partial) {
+  __shared__ float red[8];
+  __shared__ float4 s_dg[256], s_db[256];
+  const int g = blockIdx.x, b = blockIdx.y;
+  const int v4 = cpg / 4;
+  const long long base = (static_cast<long long>(b) * rows) * channels + g * cpg;
+  const int total = rows * v4;
+  float s = 0.f;
+  for (int e = threadIdx.x; e < total; e += 256) {
+    const float4 v = __ldg(reinterpret_cast<const float4*>(x + base + static_cast<long long>(e / v4) * channels) + e % v4);
+    s += (v.x + v.y) + (v.z + v.w);
+  }
+  const float n = static_cast<float>(rows) * cpg;
+  const float mean = block_sum_256(s, red) / n;
+  float q = 0.f;
+  for (int e = threadIdx.x; e < total; e += 256) {
+    const float4 v = __ldg(reinterpret_cast<const float4*>(x + base + static_cast<long long>(e / v4) * channels) + e % v4);
+    const float a = v.x - mean, c = v.y - mean, d = v.z - mean, f = v.w - mean;
+    q += (a * a + c * c) + (d * d + f * f);
+  }
+  const float rstd = rsqrtf(block_sum_256(q, red) / n + eps);
+
+  const int rstep = 256 / v4;                  // v4 <= 256 (checked on the host)
+  const int c4 = threadIdx.x % v4, r0 = threadIdx.x / v4;
+  float4 dg = make_float4(0.f, 0.f, 0.f, 0.f), db = dg;
+  float s1 = 0.f, s2 = 0.f;
+  if (r0 < rstep) {
+    const float4 w = __ldg(reinterpret_cast<const float4*>(weight + g * cpg) + c4);
+    const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + g * cpg) + c4);
+    for (int r = r0; r < rows; r += rstep) {
+      const long long off = base + static_cast<long long>(r) * channels + c4 * 4;
+      const float4 v = __ldg(reinterpret_cast<const float4*>(x + off));
+      const float4 d = __ldg(reinterpret_cast<const float4*>(dy + off));
+      const float h0 = (v.x - mean) * rstd, h1 = (v.y - mean) * rstd, h2 = (v.z - mean) * rstd, h3 = (v.w - mean) * rstd;
+      const float z0 = gn_silu_dz(h0, w.x, bb.x, d.x), z1 = gn_silu_dz(h1, w.y, bb.y, d.y);
+      const float z2 = gn_silu_dz(h2, w.z, bb.z, d.z), z3 = gn_silu_dz(h3, w.w, bb.w, d.w);
+      dg.x += z0 * h0; dg.y += z1 * h1; dg.z += z2 * h2; dg.w += z3 * h3;
+      db.x += z0; db.y += z1; db.z += z2; db.w += z3;
+      const float e0 = z0 * w.x, e1 = z1 * w.y, e2 = z2 * w.z, e3 = z3 * w.w;
+      s1 += (e0 + e1) + (e2 + e3);
+      s2 += (e0 * h0 + e1 * h1) + (e2 * h2 + e3 * h3);
+    }
+  }
+  s_dg[threadIdx.x] = dg;
+  s_db[threadIdx.x] = db;
+  const float m1 = block_sum_256(s1, red) / n;   // its __syncthreads also publishes s_dg / s_db
+  const float m2 = block_sum_256(s2, red) / n;
+  if (threadIdx.x < v4) {
+    float4 tg = s_dg[threadIdx.x], tb = s_db[threadIdx.x];
+    for (int j = 1; j < rstep; ++j) {
+      const float4 ug = s_dg[j * v4 + threadIdx.x], ub = s_db[j * v4 + threadIdx.x];
+      tg.x += ug.x; tg.y += ug.y; tg.z += ug.z; tg.w += ug.w;
+      tb.x += ub.x; tb.y += ub.y; tb.z += ub.z; tb.w += ub.w;
+    }
+    const long long p = static_cast<long long>(b) * 2 * channels + g * cpg + threadIdx.x * 4;
+    *reinterpret_cast<float4*>(partial + p) = tg;
+    *reinterpret_cast<float4*>(partial + p + channels) = tb;
+  }
+
+  for (int e = threadIdx.x; e < total; e += 256) {
+    const int r = e / v4, k4 = e % v4;
+    const long long off = base + static_cast<long long>(r) * channels + k4 * 4;
+    const float4 v = __ldg(reinterpret_cast<const float4*>(x + off));
+    const float4 d = __ldg(reinterpret_cast<const float4*>(dy + off));
+    const float4 w = __ldg(reinterpret_cast<const float4*>(weight + g * cpg) + k4);
+    const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + g * cpg) + k4);
+    const float h0 = (v.x - mean) * rstd, h1 = (v.y - mean) * rstd, h2 = (v.z - mean) * rstd, h3 = (v.w - mean) * rstd;
+    const float o0 = rstd * (gn_silu_dz(h0, w.x, bb.x, d.x) * w.x - m1 - h0 * m2);
+    const float o1 = rstd * (gn_silu_dz(h1, w.y, bb.y, d.y) * w.y - m1 - h1 * m2);
+    const float o2 = rstd * (gn_silu_dz(h2, w.z, bb.z, d.z) * w.z - m1 - h2 * m2);
+    const float o3 = rstd * (gn_silu_dz(h3, w.w, bb.w, d.w) * w.w - m1 - h3 * m2);
+    uint2 pk;
+    pk.x = f2_bf2(o0, o1);
+    pk.y = f2_bf2(o2, o3);
+    *reinterpret_cast<uint2*>(dx + off) = pk;
+  }
+}
+
+// out[i] = sum over j = 0 .. parts-1 of partial[j * stride + i], in that order (the fixed-order second level of the
+// predictor's deterministic reductions).  Columns [0, split) go to out0, [split, cols) to out1.
+__global__ void __launch_bounds__(256) sum_parts_kernel(const float* __restrict__ partial, long long parts,
+                                                        long long stride, int cols, int split, float* __restrict__ out0,
+                                                        float* __restrict__ out1) {
+  const int i = blockIdx.x * 256 + threadIdx.x;
+  if (i >= cols) return;
+  float s = 0.f;
+  for (long long j = 0; j < parts; ++j) s += __ldg(partial + j * stride + i);
+  if (i < split) out0[i] = s;
+  else out1[i - split] = s;
+}
+
+// Backward of rowdot_kernel with ReLU: dpre[r] = pred[r] > 0 ? dpred[r] : 0 (0 at an exact zero, as torch's
+// threshold_backward).  One CTA per NS2_ROWDOT_BWD_ROWS rows: dx[r, :] += dpre[r] * w, and this chunk's
+// sum_r dpre[r] * x[r, :] and sum_r dpre[r] (rows in order) to partial[chunk, 0 .. dim] (rows of dim + 4 floats, so
+// that every row starts 16-byte aligned).
+__global__ void __launch_bounds__(256) rowdot_bwd_kernel(const float* __restrict__ x, long long rows, int dim,
+                                                         const float* __restrict__ w, const float* __restrict__ pred,
+                                                         const float* __restrict__ dpred, float* __restrict__ dx,
+                                                         float* __restrict__ partial) {
+  __shared__ float s_d[NS2_ROWDOT_BWD_ROWS];
+  const long long r0 = static_cast<long long>(blockIdx.x) * NS2_ROWDOT_BWD_ROWS;
+  const int nr = static_cast<int>(rows - r0 < NS2_ROWDOT_BWD_ROWS ? rows - r0 : NS2_ROWDOT_BWD_ROWS);
+  if (threadIdx.x < NS2_ROWDOT_BWD_ROWS) {
+    float d = 0.f;
+    if (threadIdx.x < nr) {
+      const long long r = r0 + threadIdx.x;
+      d = __ldg(pred + r) > 0.f ? __ldg(dpred + r) : 0.f;
+    }
+    s_d[threadIdx.x] = d;
+  }
+  __syncthreads();
+  float* prow = partial + static_cast<long long>(blockIdx.x) * (dim + 4);
+  for (int c4 = threadIdx.x; c4 < dim / 4; c4 += 256) {
+    const float4 wv = __ldg(reinterpret_cast<const float4*>(w) + c4);
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int i = 0; i < nr; ++i) {
+      const float d = s_d[i];
+      const long long off = (r0 + i) * dim + c4 * 4;
+      const float4 xv = __ldg(reinterpret_cast<const float4*>(x + off));
+      acc.x += d * xv.x; acc.y += d * xv.y; acc.z += d * xv.z; acc.w += d * xv.w;
+      float4 o = *reinterpret_cast<float4*>(dx + off);
+      o.x += d * wv.x; o.y += d * wv.y; o.z += d * wv.z; o.w += d * wv.w;
+      *reinterpret_cast<float4*>(dx + off) = o;
+    }
+    *reinterpret_cast<float4*>(prow + c4 * 4) = acc;
+  }
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+    for (int i = 0; i < nr; ++i) s += s_d[i];
+    prow[dim] = s;
+  }
+}
+
 }  // namespace
 }  // namespace ns2
 
@@ -220,6 +396,60 @@ extern "C" int ns2_dropout_f32(float* x, int64_t n, const ns2_dropout* dropout, 
   NS2_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "dropout_f32: x must be 16-byte aligned");
   dropout_f32_kernel<<<grid_cap((n + 3) / 4), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, n, d);
   g_launches.fetch_add(1, std::memory_order_relaxed);
+  NS2_CUDA_CHECK(cudaGetLastError());
+  return kOk;
+}
+
+extern "C" int ns2_groupnorm_silu_bwd(const float* x, int32_t batch, int32_t rows, int32_t channels, int32_t groups,
+                                      const float* weight, const float* bias, float eps, const float* dy, void* dx_bf16,
+                                      float* partial, float* dweight, float* dbias, ns2_stream_t stream) {
+  NS2_REQUIRE(batch >= 0 && rows >= 0 && channels > 0 && groups > 0 && channels % groups == 0,
+              "groupnorm_silu_bwd: bad sizes");
+  NS2_REQUIRE((channels / groups) % 4 == 0 && channels / groups <= 1024,
+              "groupnorm_silu_bwd: channels per group (%d) must be a multiple of 4 and <= 1024", channels / groups);
+  NS2_REQUIRE(batch <= 65535, "groupnorm_silu_bwd: batch %d > 65535", batch);
+  NS2_REQUIRE(dweight && dbias, "groupnorm_silu_bwd: null pointer");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (batch == 0 || rows == 0) {   // no element: zero parameter gradients
+    NS2_CUDA_CHECK(cudaMemsetAsync(dweight, 0, sizeof(float) * channels, st));
+    NS2_CUDA_CHECK(cudaMemsetAsync(dbias, 0, sizeof(float) * channels, st));
+    return kOk;
+  }
+  NS2_REQUIRE(x && weight && bias && dy && dx_bf16 && partial, "groupnorm_silu_bwd: null pointer");
+  NS2_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(weight) | reinterpret_cast<uintptr_t>(bias) |
+                reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(partial)) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(dx_bf16) & 7) == 0,
+              "groupnorm_silu_bwd: pointers must be 16-byte aligned (dx 8-byte)");
+  groupnorm_silu_bwd_kernel<<<dim3(groups, batch), 256, 0, st>>>(x, rows, channels, channels / groups, weight, bias, eps,
+                                                                 dy, static_cast<__nv_bfloat16*>(dx_bf16), partial);
+  NS2_CUDA_CHECK(cudaGetLastError());
+  sum_parts_kernel<<<(2 * channels + 255) / 256, 256, 0, st>>>(partial, batch, 2LL * channels, 2 * channels, channels,
+                                                               dweight, dbias);
+  g_launches.fetch_add(2, std::memory_order_relaxed);
+  NS2_CUDA_CHECK(cudaGetLastError());
+  return kOk;
+}
+
+extern "C" int ns2_rowdot_bwd(const float* x, int64_t rows, int32_t dim, const float* w, const float* pred,
+                              const float* dpred, float* dx, float* partial, float* dw, float* db, ns2_stream_t stream) {
+  NS2_REQUIRE(rows >= 0 && dim > 0 && dim % 4 == 0, "rowdot_bwd: bad sizes");
+  NS2_REQUIRE(dw && db, "rowdot_bwd: null pointer");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (rows == 0) {
+    NS2_CUDA_CHECK(cudaMemsetAsync(dw, 0, sizeof(float) * dim, st));
+    NS2_CUDA_CHECK(cudaMemsetAsync(db, 0, sizeof(float), st));
+    return kOk;
+  }
+  NS2_REQUIRE(x && w && pred && dpred && dx && partial, "rowdot_bwd: null pointer");
+  NS2_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(dx) |
+                reinterpret_cast<uintptr_t>(partial)) & 15) == 0,
+              "rowdot_bwd: x, w, dx and partial must be 16-byte aligned");
+  const long long chunks = (rows + NS2_ROWDOT_BWD_ROWS - 1) / NS2_ROWDOT_BWD_ROWS;
+  NS2_REQUIRE(chunks <= 0x7fffffffLL, "rowdot_bwd: too many rows");
+  rowdot_bwd_kernel<<<static_cast<unsigned>(chunks), 256, 0, st>>>(x, rows, dim, w, pred, dpred, dx, partial);
+  NS2_CUDA_CHECK(cudaGetLastError());
+  sum_parts_kernel<<<(dim + 1 + 255) / 256, 256, 0, st>>>(partial, chunks, dim + 4LL, dim + 1, dim, dw, db);
+  g_launches.fetch_add(2, std::memory_order_relaxed);
   NS2_CUDA_CHECK(cudaGetLastError());
   return kOk;
 }

@@ -60,7 +60,7 @@ class NaturalSpeech2(nn.Module):
     def __init__(self, model: Model, codec=None, *, tokenizer=None, target_sample_hz=None, timesteps=1000,
                  use_ddim=True, noise_schedule="sigmoid", objective="v", schedule_kwargs: dict = dict(),
                  time_difference=0., min_snr_loss_weight=True, min_snr_gamma=5, train_prob_self_cond=0.9,
-                 rvq_cross_entropy_loss_weight=0., scale=1.,
+                 rvq_cross_entropy_loss_weight=0., scale=1., duration_loss_weight=1., pitch_loss_weight=1.,
                  conditioner: Optional[Callable] = None, cuda_graphs: bool = True, **conditioning_kwargs):
         super().__init__()
         if not isinstance(model, Model):
@@ -92,6 +92,7 @@ class NaturalSpeech2(nn.Module):
         self.min_snr_loss_weight = min_snr_loss_weight
         self.min_snr_gamma = min_snr_gamma
         self.rvq_cross_entropy_loss_weight = rvq_cross_entropy_loss_weight
+        self.duration_loss_weight, self.pitch_loss_weight = duration_loss_weight, pitch_loss_weight   # ns2.py:1193-1194
         self.conditioner = conditioner
         self.cuda_graphs = cuda_graphs  # sampling loop: replay one captured CUDA graph per sampling step
         self._sampler_graphs = OrderedDict()
@@ -250,17 +251,23 @@ class NaturalSpeech2(nn.Module):
         """ns2.py:1503-1684 -> scalar diffusion loss (the only term the reference returns, SURVEY T11).
         Extra keyword-only arguments: `prompt_enc`/`cond` (precomputed conditioning), `times`/`noise`
         (inject the two random draws of ns2.py:1621,1625 — used by the parity tests) and `duration` (per-phoneme frame
-        counts, handed to the conditioner only when given: encoders.Conditioner takes them in place of an aligner)."""
+        counts, handed to the conditioner only when given: encoders.Conditioner takes them in place of an aligner).
+        A conditioner that returns (prompt_enc, cond, duration_loss, pitch_loss) (encoders.Conditioner with
+        train_duration_pitch=True) adds duration_loss_weight * duration_loss + pitch_loss_weight * pitch_loss to the
+        returned loss, the `aux_loss` of ns2.py:1600-1602 that the reference adds at 1684."""
         is_raw_audio = audio.ndim == 2
+        aux_loss = None
         if self.conditional and not (_exists(prompt_enc) and _exists(cond)):
             if not _exists(self.conditioner):
                 raise NotImplementedError(
                     "conditional training needs prompt_enc= and cond= or a `conditioner` callable (the "
                     "reference's encoders + aligner are outside the accelerated path)")
             extra = {} if duration is None else {"duration": duration}
-            prompt_enc, cond = self.conditioner(audio=audio, text=text, text_lens=text_lens, mel=mel,
-                                                mel_lens=mel_lens, prompt=self.process_prompt(prompt),
-                                                pitch=pitch, mode="train", **extra)
+            out = self.conditioner(audio=audio, text=text, text_lens=text_lens, mel=mel, mel_lens=mel_lens,
+                                   prompt=self.process_prompt(prompt), pitch=pitch, mode="train", **extra)
+            prompt_enc, cond = out[:2]
+            if len(out) == 4:   # the duration / pitch predictor's L1 losses (ns2.py:1587-1602)
+                aux_loss = self.duration_loss_weight * out[2] + self.pitch_loss_weight * out[3]
         assert not (is_raw_audio and not _exists(self.codec)), \
             "codec must be passed in if one were to train on raw audio"
         if is_raw_audio:
@@ -302,7 +309,7 @@ class NaturalSpeech2(nn.Module):
             loss_weight = clipped / (snr + 1)
         loss = (loss * loss_weight).mean()
         if self.rvq_cross_entropy_loss_weight == 0 or not _exists(codes):   # ns2.py:1670-1671
-            return loss
+            return loss if aux_loss is None else loss + aux_loss
         # cross entropy of the predicted x_start against the codec's codes (ns2.py:1673-1684)
         if pred.requires_grad and isinstance(self.codec, EncodecRVQ):
             ce_loss = XStartCrossEntropyFunction.apply(pred, audio, alpha, sigma, self.codec, codes, self.objective)
@@ -310,7 +317,8 @@ class NaturalSpeech2(nn.Module):
             x_start = torch.empty_like(audio)
             ops.x_start_from_pred(audio, pred.detach(), alpha, sigma, x_start, objective=self.objective)
             _, ce_loss = self.codec.rq(x_start, codes)
-        return loss + self.rvq_cross_entropy_loss_weight * ce_loss
+        loss = loss + self.rvq_cross_entropy_loss_weight * ce_loss
+        return loss if aux_loss is None else loss + aux_loss
 
     p_losses = forward  # the name BASELINE.json's north_star uses; the reference inlines it in forward
 

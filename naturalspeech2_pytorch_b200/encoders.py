@@ -32,6 +32,16 @@ attention drops softmax probabilities with p = `attn_dropout` (SpeechPromptEncod
 call from torch's default CPU generator (no device sync; torch.manual_seed reproduces it); site 0 is the conv, site
 1 + l the attention of layer l.  The backward regenerates them from the seed in the record.  Without train_dropout, in
 eval() mode, or with p = 0 nothing is drawn and the kernels are those of inference.
+`DurationPitchPredictor.forward` records one node the same way, for both outputs (duration_pred, pitch_pred) and both
+inputs (phoneme encodings or token ids, encoded prompts); its backward walks each trunk in reverse:
+  Linear(dim, 1) + ReLU  ops.rowdot_bwd (d x into the trunk's fp32 residual-stream gradient)
+  cross attention        training.attention_backward with the keys [RMSNorm(x) ; prompts]: d ctx = d kv Wkv is split
+                         into the queries' rows (joining d RMSNorm(x) before rmsnorm_film_bwd) and the prompts' rows
+                         (accumulated in fp32 over both trunks and all layers)
+  ResnetBlock            per Block in reverse ops.groupnorm_silu_bwd on the saved conv output, then training.
+                         conv_backward ("same" k=3: shifts +1..-1); the first Block's d x is added to the identity path
+A prediction that gets no gradient skips its trunk (its parameters get None); d x of both trunks is summed, or
+scattered into the token table.  The predictor's dropout (p = 0.2 in every Block and Attention) is not drawn.
 Attention masks are not supported (`mask=None` is what NaturalSpeech2.forward / .sample pass, ns2.py:1475-1476,
 1538-1539).  Numerics follow the denoiser: bf16 tensor-core operands, fp32 accumulation, fp32 residual stream and norm
 statistics.
@@ -48,7 +58,7 @@ from . import _lib, ops
 from .ops import conv_segs as _conv_segs
 from .model import (_AttentionParams, _NoParam, _PackedCache, _RMSNormParams, _bf, _feedforward_params, _pack_conv,
                     _pack_geglu, _records_graph, _transpose_conv)
-from .training import attention_backward, conv_backward, ff_backward, param_grads
+from .training import attention_backward, conv_backward, ff_backward, linear_backward, param_grads
 
 _SILU = _lib.NS2_GEMM_FLAG_SILU
 
@@ -65,24 +75,34 @@ class _PlainTransformerParams(nn.Module):
         self.norm = _RMSNormParams(dim) if final_norm else nn.Identity()
 
 
+_INPUT_GRADS = "<inputs>"   # key of `_train_backward`'s result holding the gradients of the node's inputs
+
+
 class _EncoderFunction(torch.autograd.Function):
     """One autograd node for a whole encoder: forward = the inference kernels keeping activations, backward = the
-    hand-written kernels (`_train_backward`).  `reducer` (parallel.GradReducer or None) receives the parameter
-    gradients when the backward ends."""
+    hand-written kernels (`_train_backward`).  apply(enc, reducer, *inputs, *enc.parameters()): the arguments before
+    the parameters are the module's inputs, handed to `_train_forward`; its output may be one tensor or a tuple.
+    `_train_backward(record, *d_outs)` gets None for an output that received no gradient, and returns the parameter
+    gradients (None for parameters it did not reach) and, under _INPUT_GRADS, a tuple of the inputs' gradients (absent:
+    none).  `reducer` (parallel.GradReducer or None) receives the parameter gradients when the backward ends."""
 
     @staticmethod
-    def forward(ctx, enc, reducer, x, *params):
+    def forward(ctx, enc, reducer, *args):
+        n_in = len(args) - sum(1 for _ in enc.parameters())
+        ctx.set_materialize_grads(False)
         with torch.no_grad():
-            out, saved = enc._train_forward(x)
-        ctx.enc, ctx.reducer, ctx.saved = enc, reducer, saved
+            out, saved = enc._train_forward(*args[:n_in])
+        ctx.enc, ctx.reducer, ctx.saved, ctx.n_in = enc, reducer, saved, n_in
         return out
 
     @staticmethod
-    def backward(ctx, d_out):
+    def backward(ctx, *d_outs):
         with torch.no_grad():
-            grads = ctx.enc._train_backward(ctx.saved, d_out)
+            grads = ctx.enc._train_backward(ctx.saved, *d_outs)
         ctx.saved = None
-        return (None, None, None, *param_grads(ctx.enc, grads, ctx.reducer))
+        d_in = grads.pop(_INPUT_GRADS, None) or (None,) * ctx.n_in
+        d_in = [d if need else None for d, need in zip(d_in, ctx.needs_input_grad[2:2 + ctx.n_in])]
+        return (None, None, *d_in, *param_grads(ctx.enc, grads, ctx.reducer))
 
 
 class _EncoderBase(_PackedCache):
@@ -469,49 +489,132 @@ class DurationPitchPredictor(_EncoderBase):
             P["emb"] = self.phoneme_token_emb.weight.detach().float().contiguous()
         return P
 
-    def _trunk(self, name: str, trunk: _TrunkParams, P, x0: torch.Tensor, prompts_bf: torch.Tensor) -> torch.Tensor:
+    def _pack_transposed(self, P) -> Dict[str, torch.Tensor]:
+        T = {}
+        for name, trunk in (("p", self.to_pitch_pred), ("d", self.to_duration_pred)):
+            for l, (convs, _, _) in enumerate(trunk.layers):
+                for r, rb in enumerate(convs):
+                    for c in range(len(rb.blocks)):
+                        k = f"{name}{l}_{r}_{c}_w"
+                        T[k] = _transpose_conv(P[k], self.kernel_size)
+                for w in ("q", "kv", "o"):
+                    T[f"{name}{l}_{w}"] = P[f"{name}{l}_{w}"].t().contiguous()
+        return T
+
+    @staticmethod
+    def _norm_config(trunk: _TrunkParams):
+        """(groups, eps) of the trunk's GroupNorms (every Block of a trunk is built alike)."""
+        if not len(trunk.layers):
+            return 8, 1e-5
+        norm = trunk.layers[0][0][0].blocks[0].norm
+        return norm.num_groups, norm.eps
+
+    def _trunk(self, name: str, trunk: _TrunkParams, P, x0: torch.Tensor, prompts_bf: torch.Tensor,
+               saved: Optional[dict] = None) -> torch.Tensor:
+        """DurationPitchPredictorTrunk.forward (ns2.py:457-466).  With `saved` the activations `_trunk_backward` reads
+        go to saved[name] in fresh tensors (same kernels, same output)."""
+        keep = saved is not None
         B, T, D = x0.shape
         Np = prompts_bf.shape[1]
         dev, bf, H = x0.device, torch.bfloat16, self.heads
         inner = H * 64
-        groups = trunk.layers[0][0][0].blocks[0].norm.num_groups if len(trunk.layers) else 8
-        eps = trunk.layers[0][0][0].blocks[0].norm.eps if len(trunk.layers) else 1e-5
+        groups, eps = self._norm_config(trunk)
         segs = _conv_segs(D, self.kernel_size, self.kernel_size // 2)
+        e = lambda *s, dt=bf: torch.empty(*s, device=dev, dtype=dt)  # noqa: E731
         x = x0.clone()                                               # fp32 stream of this trunk
-        x_bf = ops.cast_bf16(x, torch.empty(B, T, D, device=dev, dtype=bf))
-        c = torch.empty(B, T, D, device=dev, dtype=torch.float32)
-        h_bf = torch.empty(B, T, D, device=dev, dtype=bf)
-        ctx = torch.empty(B, T + Np, D, device=dev, dtype=bf)        # [norm(x) ; encoded prompts] (ns2.py:1060-1061)
-        ctx[:, T:].copy_(prompts_bf)
-        nx = torch.empty(B, T, D, device=dev, dtype=bf)
-        q = torch.empty(B, T, inner, device=dev, dtype=bf)
-        kv = torch.empty(B, T + Np, 2 * inner, device=dev, dtype=bf)
-        o = torch.empty(B, T, inner, device=dev, dtype=bf)
+        x_bf = ops.cast_bf16(x, e(B, T, D))
+        c = e(B, T, D, dt=torch.float32)
+        h_bf = e(B, T, D)
+        layers = []
         for l, (convs, _, _) in enumerate(trunk.layers):
+            if keep or l == 0:   # inference reuses the first layer's buffers
+                ctx = e(B, T + Np, D)                                # [norm(x) ; encoded prompts] (ns2.py:1060-1061)
+                ctx[:, T:].copy_(prompts_bf)
+                L = {"nx": e(B, T, D), "q": e(B, T, inner), "kv": e(B, T + Np, 2 * inner), "o": e(B, T, inner),
+                     "ctx": ctx, "lse": e(B, H, T, dt=torch.float32) if keep else None, "blocks": []}
             for r, rb in enumerate(convs):
                 nb = len(rb.blocks)
                 src = x_bf
                 for ci in range(nb):
                     k = f"{name}{l}_{r}_{ci}"
                     ops.gemm(src, P[k + "_w"], c, n=D, epilogue=ops.EPI_F32, segs=segs, bias=P[k + "_b"])
+                    if keep:
+                        L["blocks"].append((src.clone(), c.clone()))   # conv input (bf16), GroupNorm input (fp32)
                     if ci < nb - 1:
                         ops.groupnorm_silu(c, P[k + "_gw"], P[k + "_gb"], groups, eps=eps, out_bf16=h_bf)
                         src = h_bf
                     else:   # out = blocks(x) + res_conv(x), res_conv = Identity (ns2.py:399-401)
                         ops.groupnorm_silu(c, P[k + "_gw"], P[k + "_gb"], groups, eps=eps, resid=x, out_f32=x,
                                            out_bf16=x_bf)
+            if keep:
+                L["x_mid"] = x.clone()
+                layers.append(L)
+            nx, q, kv, o, ctx = L["nx"], L["q"], L["kv"], L["o"], L["ctx"]
             ops.rmsnorm_film(x, nx, gamma=P[f"{name}{l}_g"])
             ctx[:, :T].copy_(nx)
             ops.gemm(nx, P[f"{name}{l}_q"], q, n=inner, epilogue=ops.EPI_BF16)
             ops.gemm(ctx, P[f"{name}{l}_kv"], kv, n=2 * inner, epilogue=ops.EPI_BF16)
-            ops.attention(q, kv[:, :, :inner], kv[:, :, inner:], o, heads=H)
+            ops.attention(q, kv[:, :, :inner], kv[:, :, inner:], o, heads=H, lse=L["lse"])
             ops.gemm(o, P[f"{name}{l}_o"], x, n=D, epilogue=ops.EPI_F32, resid=x)   # attn(norm(x), prompts) + x
             ops.cast_bf16(x, x_bf)
-        pred = torch.empty(B, T, device=dev, dtype=torch.float32)
+        pred = e(B, T, dt=torch.float32)
         ops.rowdot(x, P[f"{name}_pw"], P[f"{name}_pb"], pred, relu=True)            # Linear(dim, 1) + ReLU
+        if keep:
+            saved[name] = {"layers": layers, "x": x, "pred": pred.clone()}
         return pred
 
-    @torch.no_grad()
+    def _trunk_backward(self, name: str, trunk: _TrunkParams, P, T, S: dict, d_pred: torch.Tensor,
+                        d_prompts: torch.Tensor, grads: Dict[str, torch.Tensor], pfx: str) -> torch.Tensor:
+        """Backward of `_trunk` from d pred (B, T): parameter gradients go to `grads` under pfx + the reference's names,
+        d prompts (B, Np, D) f32 is accumulated in place; returns d x0 (B, T, D) f32."""
+        x = S["x"]
+        B, Tn, D = x.shape
+        Np = d_prompts.shape[1]
+        dev, bf, H = x.device, torch.bfloat16, self.heads
+        inner = H * 64
+        k, half = self.kernel_size, self.kernel_size // 2
+        groups, eps = self._norm_config(trunk)
+        dgrad_segs = ops.conv_dgrad_segs(D, k, half)
+        e = lambda *s, dt=bf: torch.empty(*s, device=dev, dtype=dt)  # noqa: E731
+        dxr = torch.zeros_like(x)                     # fp32 gradient of the trunk's residual stream
+        dxr_bf, dh, d_c = e(B, Tn, D), e(B, Tn, D), e(B, Tn, D)
+        d_kv = e(B, Tn + Np, 2 * inner)
+        # ---- to_pred: ReLU(Linear(dim, 1)) (ns2.py:451-455) ----
+        grads[pfx + "to_pred.0.weight"], grads[pfx + "to_pred.0.bias"] = ops.rowdot_bwd(
+            x, P[f"{name}_pw"], S["pred"], d_pred.float().contiguous(), dxr)
+        for l in reversed(range(len(trunk.layers))):
+            L = S["layers"][l]
+            lp = f"{pfx}layers.{l}."
+            # ---- x += Wo attn(Wq nx, Wkv [nx ; prompts]), nx = RMSNorm(x): the keys include the queries ----
+            ops.cast_bf16(dxr, dxr_bf)
+            d_nx, _ = attention_backward(dxr_bf, L["nx"], L["o"], L["lse"], L["q"], L["kv"], T[f"{name}{l}_o"],
+                                         T[f"{name}{l}_q"], H, grads, lp + "2.", d_kv=d_kv)
+            linear_backward(d_kv, L["ctx"], grads, lp + "2.to_kv", bias=False)
+            # d ctx = d kv Wkv, split: the first Tn rows join the query path's d nx, the rest is d prompts
+            d_nx32 = ops.gemm(d_kv[:, :Tn], T[f"{name}{l}_kv"], e(B, Tn, D, dt=torch.float32), n=D, epilogue=ops.EPI_F32)
+            ops.gemm(d_kv[:, Tn:], T[f"{name}{l}_kv"], d_prompts, n=D, epilogue=ops.EPI_F32, resid=d_prompts)
+            ops.accum_bf16(d_nx32, d_nx, dh)
+            grads[lp + "1.gamma"] = dgamma = torch.zeros(D, device=dev)
+            ops.rmsnorm_film_bwd(L["x_mid"], dh, dxr, dxr_bf, rows_per_batch=Tn, gamma=P[f"{name}{l}_g"], dgamma=dgamma)
+            # ---- ResnetBlocks in reverse: out = blocks(x) + x (ns2.py:397-401) ----
+            convs = trunk.layers[l][0]
+            i = len(L["blocks"])
+            for r in reversed(range(len(convs))):
+                dy = dxr                              # d out of the last Block; the identity keeps dxr as it is
+                for ci in reversed(range(len(convs[r].blocks))):
+                    i -= 1
+                    src, c = L["blocks"][i]
+                    key, bp = f"{name}{l}_{r}_{ci}", f"{lp}0.{r}.blocks.{ci}."
+                    grads[bp + "norm.weight"], grads[bp + "norm.bias"] = ops.groupnorm_silu_bwd(
+                        c, P[key + "_gw"], P[key + "_gb"], groups, dy, d_c, eps=eps)
+                    conv_backward(d_c, src, grads, bp + "proj", None, k, half)
+                    if ci > 0:
+                        dy = ops.gemm(d_c, T[key + "_w"], e(B, Tn, D, dt=torch.float32), n=D, epilogue=ops.EPI_F32,
+                                      segs=dgrad_segs)
+                    else:   # the first conv reads the ResnetBlock's input: its d x joins the identity path's
+                        ops.gemm(d_c, T[key + "_w"], dxr, n=D, epilogue=ops.EPI_F32, segs=dgrad_segs, resid=dxr)
+        return dxr
+
     def forward(self, x, encoded_prompts: torch.Tensor, prompt_mask=None):
         if prompt_mask is not None:
             raise NotImplementedError("DurationPitchPredictor: prompt masks are not supported by the sm_90a attention kernel")
@@ -520,20 +623,58 @@ class DurationPitchPredictor(_EncoderBase):
             x = self.tokenizer.texts_to_tensor_ids(x).to(encoded_prompts.device)
         if not (x.is_cuda and encoded_prompts.is_cuda):
             raise ValueError("DurationPitchPredictor: inputs must be CUDA tensors (the ns2_b200 ops have no CPU path)")
+        if _records_graph(self):
+            return _EncoderFunction.apply(self, self.grad_reducer, x, encoded_prompts, *self.parameters())
+        with torch.no_grad():
+            return self._forward(x, encoded_prompts)
+
+    def _train_forward(self, x: torch.Tensor, encoded_prompts: torch.Tensor):
+        saved = {"x_dtype": x.dtype, "prompts_dtype": encoded_prompts.dtype}
+        return self._forward(x, encoded_prompts, saved), saved
+
+    def _forward(self, x: torch.Tensor, encoded_prompts: torch.Tensor, saved: Optional[dict] = None):
+        """The forward; with `saved` it also records what `_train_backward` reads (same kernels, same output)."""
         P = self.packed()
         dev, bf = x.device, torch.bfloat16
         if "emb" in P:
             B, T = x.shape
-            e = ops.embedding_bf16(x.long().contiguous(), P["emb"],
-                                   torch.empty(B, T, self.dim_hidden, device=dev, dtype=bf), 0)
+            ids = x.long().contiguous()
+            e = ops.embedding_bf16(ids, P["emb"], torch.empty(B, T, self.dim_hidden, device=dev, dtype=bf), 0)
             x = e.float()
+            if saved is not None:
+                saved["ids"] = ids
         x = x.float().contiguous()
         B, Np, Dp = encoded_prompts.shape
         assert x.shape[-1] == self.dim_hidden and Dp == self.dim_hidden
         prompts_bf = ops.cast_bf16(encoded_prompts.float().contiguous(), torch.empty(B, Np, Dp, device=dev, dtype=bf))
-        duration = self._trunk("d", self.to_duration_pred, P, x, prompts_bf)
-        pitch = self._trunk("p", self.to_pitch_pred, P, x, prompts_bf)
+        duration = self._trunk("d", self.to_duration_pred, P, x, prompts_bf, saved)
+        pitch = self._trunk("p", self.to_pitch_pred, P, x, prompts_bf, saved)
         return duration, pitch
+
+    def _train_backward(self, S, d_duration: Optional[torch.Tensor], d_pitch: Optional[torch.Tensor]):
+        """Gradients of every parameter and of (x, encoded_prompts) given d duration_pred / d pitch_pred; a trunk whose
+        prediction received no gradient is skipped and its parameters get None."""
+        P, T = self.packed(), self.packed_transposed()
+        grads: Dict[str, Optional[torch.Tensor]] = {}
+        x = S["d"]["x"]
+        B, Tn, D = x.shape
+        Np = S["d"]["layers"][0]["ctx"].shape[1] - Tn if len(self.to_duration_pred.layers) else 0
+        d_prompts = torch.zeros(B, Np, D, device=x.device)
+        dx = None
+        for name, trunk, pfx, d in (("d", self.to_duration_pred, "to_duration_pred.", d_duration),
+                                    ("p", self.to_pitch_pred, "to_pitch_pred.", d_pitch)):
+            if d is None:
+                grads.update({pfx + n: None for n, _ in trunk.named_parameters()})
+                continue
+            dx_t = self._trunk_backward(name, trunk, P, T, S[name], d, d_prompts, grads, pfx)
+            dx = dx_t if dx is None else dx.add_(dx_t)          # x feeds both trunks
+        if "emb" in P:   # the ids get no gradient; the table does (pad id 0, as `_forward` gathers)
+            grads["phoneme_token_emb.weight"] = ops.embedding_bwd(S["ids"], dx, torch.zeros_like(P["emb"]), 0)
+            d_x = None
+        else:
+            d_x = dx.to(S["x_dtype"])
+        grads[_INPUT_GRADS] = (d_x, d_prompts.to(S["prompts_dtype"]))
+        return grads
 
 
 # --------------------------------------------------------------------------------------------------
@@ -629,22 +770,31 @@ class Conditioner(nn.Module):
 
     mode="train" takes the durations from the caller: `duration` (B, T) frame counts per phoneme (the reference
     aligner's `aln_hard`, from an external aligner or the reference's Aligner) and frame-level `pitch` (B, L) /
-    (B, 1, L).  The aligner network, its losses and the duration / pitch predictor are not run: in the reference they
-    only feed `aux_loss`, which is never returned (ns2.py:1600-1602), so the diffusion loss is the only gradient path
-    into the prompt encoder, the phoneme encoder and `pitch_emb`.  `grad_reducer` (parallel.GradReducer) all-reduces
+    (B, 1, L).  The aligner network and its losses are not run; the duration / pitch predictor only with
+    train_duration_pitch (below): in the reference they only feed `aux_loss`, which is never returned (ns2.py:1600-1602),
+    so by default the diffusion loss is the only gradient path into the prompt encoder, the phoneme encoder and
+    `pitch_emb`.  `grad_reducer` (parallel.GradReducer) all-reduces
     their gradients in data-parallel training.
 
     train_dropout=True makes training draw the reference's dropout in both encoders (their `train_dropout`; see the
-    module docstring).  The default False keeps them deterministic, as before the option existed."""
+    module docstring).  The default False keeps them deterministic, as before the option existed.
+
+    train_duration_pitch=True also trains the duration / pitch predictor: mode="train" runs it on the same encoder
+    outputs and returns (prompt_enc, cond, duration_loss, pitch_loss), the reference's L1 losses against the given
+    durations and the per-phoneme pitch (ns2.py:1579-1590).  Their gradients reach the predictor and, through its
+    inputs, both encoders; NaturalSpeech2.forward weights and adds them (duration_loss_weight, pitch_loss_weight)."""
+
+    train_duration_pitch = False
 
     def __init__(self, *, dim_codebook=128, num_phoneme_tokens=None, tokenizer=None, duration_pitch_dim=512,
-                 pitch_emb_dim=256, pitch_emb_pp_hidden_dim=512, train_dropout=False):
+                 pitch_emb_dim=256, pitch_emb_pp_hidden_dim=512, train_dropout=False, train_duration_pitch=False):
         super().__init__()
         self.phoneme_enc = PhonemeEncoder(tokenizer=tokenizer, num_tokens=num_phoneme_tokens)
         self.prompt_enc = SpeechPromptEncoder(dim_codebook=dim_codebook)
         self.phoneme_enc.train_dropout = self.prompt_enc.train_dropout = bool(train_dropout)
         self.duration_pitch = DurationPitchPredictor(dim=duration_pitch_dim)
         self.pitch_emb = nn.Embedding(pitch_emb_dim, pitch_emb_pp_hidden_dim)
+        self.train_duration_pitch = bool(train_duration_pitch)
         self.grad_reducer = None
 
     @property
@@ -654,8 +804,9 @@ class Conditioner(nn.Module):
     @grad_reducer.setter
     def grad_reducer(self, reducer):
         self._grad_reducer = reducer
-        self.prompt_enc.grad_reducer = reducer
-        self.phoneme_enc.grad_reducer = reducer
+        for name in ("prompt_enc", "phoneme_enc", "duration_pitch"):
+            if name in self._modules:   # a Conditioner may be assembled around some of them
+                self._modules[name].grad_reducer = reducer
 
     def forward(self, prompt=None, text=None, text_lens=None, mode="sample", pitch=None, duration=None, **unused):
         if mode == "train":
@@ -703,4 +854,9 @@ class Conditioner(nn.Module):
             ph_pitch = average_over_durations(pitch.float(), duration)[:, 0]      # (B, T), ns2.py:1581
         cond = expand_encodings(phoneme_enc, duration, ph_pitch, self.pitch_emb.weight, length=L,
                                 reducer=self._grad_reducer)
-        return prompt_enc, cond
+        if not self.train_duration_pitch:
+            return prompt_enc, cond
+        duration_pred, pitch_pred = self.duration_pitch(phoneme_enc, prompt_enc)
+        duration_loss = F.l1_loss(duration.float(), duration_pred)                # ns2.py:1587
+        pitch_loss = F.l1_loss(ph_pitch, pitch_pred)                              # ns2.py:1589-1590
+        return prompt_enc, cond, duration_loss, pitch_loss

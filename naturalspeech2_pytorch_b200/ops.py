@@ -844,6 +844,47 @@ def embedding_bwd(ids: torch.Tensor, de: torch.Tensor, dtable: torch.Tensor, pad
     return dtable
 
 
+def groupnorm_silu_bwd(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, groups: int, dy: torch.Tensor,
+                       dx: torch.Tensor, *, eps: float = 1e-5) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Backward of `groupnorm_silu` (without its residual): x, dy f32 (B, N, C) contiguous -> dx bf16 (B, N, C) written,
+    returns (d weight, d bias) f32 (C,), reduced over the batch in a fixed order (bit-reproducible)."""
+    lib = _lib.load()
+    for name, t, dt in (("x", x, torch.float32), ("dy", dy, torch.float32), ("dx", dx, torch.bfloat16)):
+        _req(t, dt, name)
+        if t.shape != x.shape or not t.is_contiguous() or t.dim() != 3:
+            raise ValueError(f"{name} must be a contiguous (B, N, C) tensor of x's shape")
+    B, N, Cn = x.shape
+    _req_flat(weight, torch.float32, "weight", Cn)
+    _req_flat(bias, torch.float32, "bias", Cn)
+    partial = torch.empty(2 * B * Cn, device=x.device)
+    dw, db = torch.empty(Cn, device=x.device), torch.empty(Cn, device=x.device)
+    check(lib.ns2_groupnorm_silu_bwd(x.data_ptr(), B, N, Cn, int(groups), weight.data_ptr(), bias.data_ptr(), float(eps),
+                                     dy.data_ptr(), dx.data_ptr(), partial.data_ptr(), dw.data_ptr(), db.data_ptr(),
+                                     _stream(x)), "ns2_groupnorm_silu_bwd")
+    return dw, db
+
+
+def rowdot_bwd(x: torch.Tensor, w: torch.Tensor, pred: torch.Tensor, dpred: torch.Tensor,
+               dx: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Backward of `rowdot(..., relu=True)` from its output `pred`: dx (f32, x's shape) += d pre * w in place, returns
+    (d w (dim,), d bias (1,)) f32, reduced in a fixed order.  d pre = d pred where pred > 0, else 0."""
+    lib = _lib.load()
+    for name, t in (("x", x), ("w", w), ("pred", pred), ("dpred", dpred), ("dx", dx)):
+        _req(t, torch.float32, name)
+        if not t.is_contiguous():
+            raise ValueError(f"rowdot_bwd: {name} must be contiguous")
+    dim = x.shape[-1]
+    rows = pred.numel()
+    if rows * dim != x.numel() or dpred.numel() != rows or dx.shape != x.shape or w.numel() != dim:
+        raise ValueError("rowdot_bwd needs x (..., dim), w (dim,), pred / dpred one value per row, dx of x's shape")
+    chunks = (rows + _lib.NS2_ROWDOT_BWD_ROWS - 1) // _lib.NS2_ROWDOT_BWD_ROWS
+    partial = torch.empty(max(chunks, 1) * (dim + 4), device=x.device)
+    dw, db = torch.empty(dim, device=x.device), torch.empty(1, device=x.device)
+    check(lib.ns2_rowdot_bwd(x.data_ptr(), rows, dim, w.data_ptr(), pred.data_ptr(), dpred.data_ptr(), dx.data_ptr(),
+                             partial.data_ptr(), dw.data_ptr(), db.data_ptr(), _stream(x)), "ns2_rowdot_bwd")
+    return dw, db
+
+
 def expand_encodings_bwd(dcond: torch.Tensor, coarse: torch.Tensor, idx: torch.Tensor, dphon: Optional[torch.Tensor],
                          dtable: Optional[torch.Tensor]):
     """Backward of `expand_encodings` given d cond TOKEN-MAJOR (B, L, D) f32 (unit channel stride, uniform row stride):

@@ -383,15 +383,15 @@ def _conditioning_backward_tokens(model, S, T, d_xkv, grads, want_prompt: bool):
 
 def param_grads(module: torch.nn.Module, grads: Dict[str, torch.Tensor], reducer=None) -> list:
     """The gradients of `module.parameters()` from a hand-written backward's `grads` (keys of `named_parameters()`), in
-    the parameters' shapes and dtypes; raises when one is missing.  `reducer` (parallel.GradReducer) all-reduces them
-    first."""
+    the parameters' shapes and dtypes; raises when one is missing.  A None entry (a part of the module the loss does
+    not reach) stays None, as torch autograd leaves it.  `reducer` (parallel.GradReducer) all-reduces them first."""
     missing = [n for n, _ in module.named_parameters() if n not in grads]
     if missing:
         raise RuntimeError(f"{type(module).__name__} backward produced no gradient for {missing[:4]}...")
     if reducer is not None:
-        reducer.reduce_all(grads)
+        reducer.reduce_all({n: g for n, g in grads.items() if g is not None})
         reducer.finish()
-    return [grads[n].reshape(p.shape).to(p.dtype) for n, p in module.named_parameters()]
+    return [None if grads[n] is None else grads[n].reshape(p.shape).to(p.dtype) for n, p in module.named_parameters()]
 
 
 class DenoiserFunction(torch.autograd.Function):

@@ -1,13 +1,18 @@
 #!/usr/bin/env python
 """Conditional training step with the conditioning front end in the loop, timed beside the same step without it.
 
-    python tools/train_cond_bench.py [--steps K] [--warmup W]
+    python tools/train_cond_bench.py [--steps K] [--warmup W] [--duration-pitch]
 
   cond_e2e   configs[4] training step (cfg3 denoiser Model(512, depth 12, heads 8, dim_prompt 512), B=32, N=1024) with
              SpeechPromptEncoder(dim_codebook=128) on (32, 103, 128) prompt latents, PhonemeEncoder on 100 phoneme ids
              per sample, durations summing to <= 1024 frames, backward through everything (encoders, pitch embedding,
              the denoiser's input gradients) and fused AdamW over the trained parameters
   cfg5       the same denoiser step on precomputed (prompt_enc, cond) — bench.py's secondary train_cfg5 workload
+  --duration-pitch  adds cond_e2e_dp: the same step with Conditioner(train_duration_pitch=True), i.e. the duration /
+             pitch predictor (dim 512, depth 10, both trunks) run on the encoders' outputs and trained through its L1
+             losses, timed alternately with cond_e2e (two rounds each); and dpp_alone: the predictor's forward +
+             backward on its own at B 32 x T 100 x Np 103 (CUDA events per call, median of --calls calls, two rounds)
+             with the peak memory of one training call
 Prints one JSON line: ms / steps per second of both, the encoders' measured share of the step (1 - cfg5 / cond_e2e),
 the card name and its enforced power limit (part of every number).
 """
@@ -58,6 +63,9 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--train-dropout", action="store_true",
                     help="train the encoders with the reference's dropout (Conditioner(train_dropout=True))")
+    ap.add_argument("--duration-pitch", action="store_true",
+                    help="also time the step with the duration / pitch predictor trained, and the predictor alone")
+    ap.add_argument("--calls", type=int, default=20, help="predictor-alone calls per round (median)")
     args = ap.parse_args()
     dev = torch.device("cuda", 0)
     torch.manual_seed(0)
@@ -101,12 +109,88 @@ def main():
         return loss.detach()
 
     ms_e2e, loss_e2e = timed(step_e2e, args.steps, args.warmup)
-    print(json.dumps({
+    res = {
         "cond_e2e": {"ms_per_step": round(ms_e2e, 3), "steps_per_s": round(1e3 / ms_e2e, 3), "loss": round(loss_e2e, 5)},
         "cfg5": {"ms_per_step": round(ms5, 3), "steps_per_s": round(1e3 / ms5, 3), "loss": round(loss5, 5)},
         "encoder_share_of_step": round(1.0 - ms5 / ms_e2e, 4), "train_dropout": args.train_dropout,
         "steps": args.steps, "warmup": args.warmup,
-        "batch": B, "card": card(dev)}))
+        "batch": B, "card": card(dev)}
+    if args.duration_pitch:
+        res.update(duration_pitch_legs(args, ns, cond_net, opt, step_e2e, trained, lat, text, prompt, pitch, dur))
+    print(json.dumps(res))
+
+
+def duration_pitch_legs(args, ns, cond_net, opt, step_e2e, trained, lat, text, prompt, pitch, dur):
+    """cond_e2e with and without the predictor trained (alternated), and the predictor's forward + backward alone."""
+    dev = lat.device
+    opt_dp = torch.optim.AdamW([*trained, *cond_net.duration_pitch.parameters()], lr=1e-4, fused=True)
+
+    def step_dp():
+        opt_dp.zero_grad(set_to_none=True)
+        loss = ns(lat, text=text, prompt=prompt, pitch=pitch, duration=dur)
+        loss.backward()
+        opt_dp.step()
+        return loss.detach()
+
+    rounds = {"cond_e2e": [], "cond_e2e_dp": []}
+    for _ in range(2):
+        cond_net.train_duration_pitch = False
+        rounds["cond_e2e"].append(timed(step_e2e, args.steps, args.warmup)[0])
+        cond_net.train_duration_pitch = True
+        rounds["cond_e2e_dp"].append(timed(step_dp, args.steps, args.warmup)[0])
+    cond_net.train_duration_pitch = False
+    # the predictor alone: phoneme encodings and prompts as the encoders hand them over
+    dp = cond_net.duration_pitch
+    g = torch.Generator().manual_seed(300)
+    x = torch.randn(B, T, 512, generator=g).to(dev).requires_grad_(True)
+    pr = torch.randn(B, NP, 512, generator=g).to(dev).requires_grad_(True)
+    d_dur, d_pitch = (torch.randn(B, T, generator=g).to(dev) for _ in range(2))
+
+    def call():
+        dp.zero_grad(set_to_none=True)
+        x.grad = pr.grad = None
+        dur_p, pitch_p = dp(x, pr)
+        torch.autograd.backward([dur_p, pitch_p], [d_dur, d_pitch])
+
+    for _ in range(3):
+        call()
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats(dev)
+    base = torch.cuda.memory_allocated(dev)
+    call()
+    torch.cuda.synchronize()
+    peak_mb = (torch.cuda.max_memory_allocated(dev) - base) / 2 ** 20
+    alone = []
+    for _ in range(2):
+        ms = []
+        for _ in range(args.calls):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            call()
+            e1.record()
+            torch.cuda.synchronize()
+            ms.append(e0.elapsed_time(e1))
+        alone.append(sorted(ms)[len(ms) // 2])
+    dp.eval()
+    with torch.no_grad():
+        launches_fwd = _launches(lambda: dp(x.detach(), pr.detach()))
+    dp.train()
+    launches_train = _launches(call)
+    return {"duration_pitch": {
+        "cond_e2e_ms_rounds": [round(v, 3) for v in rounds["cond_e2e"]],
+        "cond_e2e_dp_ms_rounds": [round(v, 3) for v in rounds["cond_e2e_dp"]],
+        "predictor_share_of_step": round(1.0 - sum(rounds["cond_e2e"]) / sum(rounds["cond_e2e_dp"]), 4),
+        "alone_fwd_bwd_median_ms_rounds": [round(v, 3) for v in alone], "alone_calls_per_round": args.calls,
+        "alone_shape": [B, T, NP], "alone_peak_extra_mib": round(peak_mb, 1),
+        "launches_inference_fwd": launches_fwd, "launches_fwd_bwd": launches_train}}
+
+
+def _launches(fn):
+    from naturalspeech2_pytorch_b200 import ops
+    n0 = ops.launch_count()
+    fn()
+    torch.cuda.synchronize()
+    return ops.launch_count() - n0
 
 
 if __name__ == "__main__":

@@ -316,7 +316,9 @@ int ns2_x_start(const float* x, const float* pred, const float* alpha, const flo
  *    ns2_rvq_encode  : frames f32 (F, d) -> codes int64 (F, Q); residual chain in fp32, nearest
  *                      codeword by exact squared L2 distance, ties -> lowest index.  d must be 128,
  *                      K a multiple of 128.
- *    ns2_rvq_decode  : emb f32 (F, d) = sum_q codebooks[q, codes[f,q], :]  (summed in order q = 0..Q-1)
+ *    ns2_rvq_decode  : emb f32 (F, d) = sum_q codebooks[q, codes[f,q], :]  (summed in order q = 0..Q-1); a code
+ *                      outside [0, K) reads the nearest valid codeword (< 0 -> 0, >= K -> K - 1).  d must be 128;
+ *                      codebooks and emb 16-byte aligned.
  * ------------------------------------------------------------------------------------------------ */
 #define NS2_RVQ_PREPARED_HALFS(q, k, d) ((long long)(q) * (k) * ((d) + 16))
 #define NS2_RVQ_STATS_LEN 4
@@ -334,7 +336,8 @@ int ns2_rvq_decode(const int64_t* codes, int64_t num_frames, int32_t q, int32_t 
  *                      vector-quantize-pytorch ResidualVQ.forward(x, indices)).  Per stage the logits are the negative
  *                      Euclidean distances -||r_q - c_k||; loss = sum_q mean_{f: target != -1} CE(logits, target[f,q]);
  *                      the residual chain follows `own_codes` (the codec's own nearest codewords, from ns2_rvq_encode).
- *                      ce_scratch: num_frames * q floats; loss: 1 float. */
+ *                      d must be 128, k >= 32.  ce_scratch: num_frames * q floats, left holding each frame's CE of
+ *                      each stage at [f * q + stage] (0 where the target is -1); loss: 1 float. */
 int ns2_rvq_ce(const float* frames, int64_t num_frames, int32_t d, const float* codebooks,
                const float* cb_norm2, int32_t q, int32_t k, const int64_t* own_codes,
                const int64_t* target_codes, float* ce_scratch, float* loss, ns2_stream_t stream);

@@ -89,8 +89,14 @@ class EncodecRVQ(nn.Module):
 
     @torch.no_grad()
     def get_emb_from_indices(self, codes: torch.Tensor) -> torch.Tensor:
+        """codes (..., Q) integer -> emb (..., 128) fp32, the sum of the indexed codewords."""
+        if codes.is_floating_point() or codes.dim() == 0 or codes.shape[-1] != self.num_quantizers:
+            raise ValueError(f"codes must be integer (..., {self.num_quantizers}), got {codes.dtype} "
+                             f"{tuple(codes.shape)}")
         shp = codes.shape[:-1]
-        emb = ops.rvq_decode(codes.reshape(-1, self.num_quantizers), self.codebooks)
+        if codes.numel() == 0:  # nothing to launch, as in `quantize`
+            return torch.empty(*shp, 128, dtype=torch.float32, device=codes.device)
+        emb = ops.rvq_decode(codes.reshape(-1, self.num_quantizers).to(torch.int64).contiguous(), self.codebooks)
         return emb.view(*shp, 128)
 
     @torch.no_grad()

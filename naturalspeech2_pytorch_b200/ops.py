@@ -585,31 +585,69 @@ def rvq_encode(frames: torch.Tensor, codebooks: torch.Tensor, prepared, codes: O
     return codes
 
 
+def _req_dense(t: torch.Tensor, dtype: torch.dtype, shape: Tuple[Optional[int], ...], name: str) -> None:
+    """dtype, shape (None = any size) and contiguity: the checks that need no device, so they fail the same way on a
+    machine without a GPU."""
+    if t.dtype != dtype:
+        raise ValueError(f"{name} must be {dtype}, got {t.dtype}")
+    if t.dim() != len(shape) or any(s is not None and s != n for s, n in zip(shape, t.shape)):
+        want = ", ".join("*" if s is None else str(s) for s in shape)
+        raise ValueError(f"{name} must have shape ({want}), got {tuple(t.shape)}")
+    if not t.is_contiguous():
+        raise ValueError(f"{name} must be contiguous")
+
+
+def _req_device(device: torch.device, **tensors: torch.Tensor) -> None:
+    """Every tensor is a CUDA tensor on `device`."""
+    for name, t in tensors.items():
+        if not t.is_cuda:
+            raise ValueError(f"{name} must be a CUDA tensor (the ns2_b200 ops have no CPU path)")
+        if t.device != device:
+            raise ValueError(f"{name} is on {t.device}, expected {device}")
+
+
 def rvq_decode(codes: torch.Tensor, codebooks: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """codes (F, Q) int64 -> emb (F, 128) f32 = sum_q codebooks[q, codes[:, q]], added in order q = 0..Q-1.  Codes
+    outside [0, K) are clamped to 0 / K - 1.  `out` (optional) is a contiguous (F, 128) f32 tensor."""
     lib = _lib.load()
+    _req_dense(codebooks, torch.float32, (None, None, 128), "codebooks")
     cb = codebooks.contiguous()
     Q, K, D = cb.shape
-    cd = codes.contiguous()
-    F = cd.shape[0]
+    _req_dense(codes, torch.int64, (None, Q), "codes")
+    F = codes.shape[0]
     if out is None:
-        out = torch.empty((F, D), device=cb.device, dtype=torch.float32)
-    check(lib.ns2_rvq_decode(cd.data_ptr(), F, Q, K, D, cb.data_ptr(), out.data_ptr(), _stream()),
+        out = torch.empty((F, D), device=codes.device, dtype=torch.float32)
+    _req_dense(out, torch.float32, (F, D), "out")
+    _req_device(codes.device, codes=codes, codebooks=cb, out=out)
+    for name, t in (("codebooks", cb), ("out", out)):   # read / written as float4
+        if t.data_ptr() % 16:
+            raise ValueError(f"{name} must be 16-byte aligned")
+    check(lib.ns2_rvq_decode(codes.data_ptr(), F, Q, K, D, cb.data_ptr(), out.data_ptr(), _stream(codes)),
           "ns2_rvq_decode")
     return out
 
 
+def _rvq_ce_args(frames, codebooks, cn2, own_codes, target_codes):
+    """Checks shared by rvq_ce and rvq_ce_bwd; returns (frames, codebooks) contiguous and F, Q, K."""
+    fr, cb = frames.contiguous(), codebooks.contiguous()
+    _req_dense(fr, torch.float32, (None, 128), "frames")
+    _req_dense(cb, torch.float32, (None, None, 128), "codebooks")
+    F = fr.shape[0]
+    Q, K, _ = cb.shape
+    _req_dense(cn2, torch.float32, (Q, K), "cn2")
+    _req_dense(own_codes, torch.int64, (F, Q), "own_codes")
+    _req_dense(target_codes, torch.int64, (F, Q), "target_codes")
+    _req_device(fr.device, frames=fr, codebooks=cb, cn2=cn2, own_codes=own_codes, target_codes=target_codes)
+    return fr, cb, F, Q, K
+
+
 def rvq_ce(frames: torch.Tensor, codebooks: torch.Tensor, cn2: torch.Tensor, own_codes: torch.Tensor,
            target_codes: torch.Tensor) -> torch.Tensor:
-    """Cross-entropy head of the residual VQ (`codec.rq`): frames (F, 128) f32, codes (F, Q) int64 -> 0-d loss."""
+    """Cross-entropy head of the residual VQ (`codec.rq`): frames (F, 128) f32, codebooks (Q, K, 128) f32, their
+    squared norms cn2 (Q, K) f32, codes (F, Q) int64 -> 0-d loss."""
     lib = _lib.load()
-    _req(frames, torch.float32, "frames")
-    cb = codebooks.contiguous()
-    Q, K, D = cb.shape
-    fr = frames.contiguous()
-    F = fr.shape[0]
-    for name, t in (("own_codes", own_codes), ("target_codes", target_codes)):
-        if not (t.is_cuda and t.dtype == torch.int64 and t.is_contiguous() and tuple(t.shape) == (F, Q)):
-            raise ValueError(f"{name} must be a contiguous CUDA int64 tensor of shape (F, Q)")
+    fr, cb, F, Q, K = _rvq_ce_args(frames, codebooks, cn2, own_codes, target_codes)
+    D = 128
     scratch = torch.empty(F * Q, device=fr.device, dtype=torch.float32)
     loss = torch.empty((), device=fr.device, dtype=torch.float32)
     check(lib.ns2_rvq_ce(fr.data_ptr(), F, D, cb.data_ptr(), cn2.data_ptr(), Q, K, own_codes.data_ptr(),
@@ -624,15 +662,9 @@ def rvq_ce_bwd(frames: torch.Tensor, codebooks: torch.Tensor, cn2: torch.Tensor,
     `row_scale` (optional, F / rows_per_sample f32) multiplies each sample's rows; `out` may be a (F, >= 128) f32 view
     with unit column stride (only its first 128 columns are written)."""
     lib = _lib.load()
-    _req(frames, torch.float32, "frames")
+    fr, cb, F, Q, K = _rvq_ce_args(frames, codebooks, cn2, own_codes, target_codes)
+    D = 128
     _req(d_loss, torch.float32, "d_loss")
-    cb = codebooks.contiguous()
-    Q, K, D = cb.shape
-    fr = frames.contiguous()
-    F = fr.shape[0]
-    for name, t in (("own_codes", own_codes), ("target_codes", target_codes)):
-        if not (t.is_cuda and t.dtype == torch.int64 and t.is_contiguous() and tuple(t.shape) == (F, Q)):
-            raise ValueError(f"{name} must be a contiguous CUDA int64 tensor of shape (F, Q)")
     if d_loss.numel() != 1:
         raise ValueError("d_loss must hold one element")
     if row_scale is not None:

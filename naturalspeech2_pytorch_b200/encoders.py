@@ -41,7 +41,14 @@ inputs (phoneme encodings or token ids, encoded prompts); its backward walks eac
   ResnetBlock            per Block in reverse ops.groupnorm_silu_bwd on the saved conv output, then training.
                          conv_backward ("same" k=3: shifts +1..-1); the first Block's d x is added to the identity path
 A prediction that gets no gradient skips its trunk (its parameters get None); d x of both trunks is summed, or
-scattered into the token table.  The predictor's dropout (p = 0.2 in every Block and Attention) is not drawn.
+scattered into the token table.
+The predictor's dropout: its constructor's `dropout` (0.2 by default) is what the reference hands to every layer's
+cross Attention (ns2.py:438-446): attention dropout on the softmax probabilities (Attend, attend.py:106 / 149), in the
+flash kernels.  The trunk builds its ResnetBlocks without a dropout argument (ns2.py:430, 435), so every Block's
+nn.Dropout has the default p = 0 (ns2.py:352, 374) and draws nothing.  With `train_dropout` (default False;
+`Conditioner(duration_pitch_dropout=True)` sets it) the attention dropout is drawn exactly as in the encoders: one seed
+per call in train() mode, none in eval(), without train_dropout or with p = 0.  The cross attention of layer l of trunk
+t (0 duration, 1 pitch; forward order) is site t depth + l.  The record keeps the seed, no mask.
 Attention masks are not supported (`mask=None` is what NaturalSpeech2.forward / .sample pass, ns2.py:1475-1476,
 1538-1539).  Numerics follow the denoiser: bf16 tensor-core operands, fp32 accumulation, fp32 residual stream and norm
 statistics.
@@ -462,6 +469,9 @@ class DurationPitchPredictor(_EncoderBase):
         if num_phoneme_tokens is not None and dim != dim_hidden:
             raise NotImplementedError("the token table width must equal dim_hidden")
         self.dim_hidden, self.heads, self.kernel_size = dim_hidden, heads, kernel_size
+        # the reference's `dropout` goes to every cross Attention only (ns2.py:438-446); its Blocks keep p = 0
+        # (conv_dropout stays 0); drawn only with train_dropout, see the module docstring
+        self.attn_dropout, self.depth = float(dropout), depth
         self.phoneme_token_emb = nn.Embedding(num_phoneme_tokens, dim) if num_phoneme_tokens is not None else nn.Identity()
         mk = lambda: _TrunkParams(dim_hidden, depth, kernel_size, dim_encoded_prompts, heads, dim_head,  # noqa: E731
                                   num_convs_per_resnet_block, num_convolutions_per_block)
@@ -509,10 +519,16 @@ class DurationPitchPredictor(_EncoderBase):
         norm = trunk.layers[0][0][0].blocks[0].norm
         return norm.num_groups, norm.eps
 
+    def _cross_attn_dropout(self, seed: Optional[int], name: str, l: int):
+        """(seed, site, p) of the cross attention of layer l of trunk `name`: site t depth + l, t = 0 for the duration
+        trunk and 1 for the pitch trunk (None without a seed)."""
+        t = 0 if name == "d" else 1
+        return None if seed is None else (seed, t * self.depth + l, self.attn_dropout)
+
     def _trunk(self, name: str, trunk: _TrunkParams, P, x0: torch.Tensor, prompts_bf: torch.Tensor,
-               saved: Optional[dict] = None) -> torch.Tensor:
+               saved: Optional[dict] = None, seed: Optional[int] = None) -> torch.Tensor:
         """DurationPitchPredictorTrunk.forward (ns2.py:457-466).  With `saved` the activations `_trunk_backward` reads
-        go to saved[name] in fresh tensors (same kernels, same output)."""
+        go to saved[name] in fresh tensors (same kernels, same output).  seed: the call's dropout seed (None = none)."""
         keep = saved is not None
         B, T, D = x0.shape
         Np = prompts_bf.shape[1]
@@ -554,7 +570,8 @@ class DurationPitchPredictor(_EncoderBase):
             ctx[:, :T].copy_(nx)
             ops.gemm(nx, P[f"{name}{l}_q"], q, n=inner, epilogue=ops.EPI_BF16)
             ops.gemm(ctx, P[f"{name}{l}_kv"], kv, n=2 * inner, epilogue=ops.EPI_BF16)
-            ops.attention(q, kv[:, :, :inner], kv[:, :, inner:], o, heads=H, lse=L["lse"])
+            ops.attention(q, kv[:, :, :inner], kv[:, :, inner:], o, heads=H, lse=L["lse"],
+                          dropout=self._cross_attn_dropout(seed, name, l))
             ops.gemm(o, P[f"{name}{l}_o"], x, n=D, epilogue=ops.EPI_F32, resid=x)   # attn(norm(x), prompts) + x
             ops.cast_bf16(x, x_bf)
         pred = e(B, T, dt=torch.float32)
@@ -564,9 +581,11 @@ class DurationPitchPredictor(_EncoderBase):
         return pred
 
     def _trunk_backward(self, name: str, trunk: _TrunkParams, P, T, S: dict, d_pred: torch.Tensor,
-                        d_prompts: torch.Tensor, grads: Dict[str, torch.Tensor], pfx: str) -> torch.Tensor:
+                        d_prompts: torch.Tensor, grads: Dict[str, torch.Tensor], pfx: str,
+                        seed: Optional[int] = None) -> torch.Tensor:
         """Backward of `_trunk` from d pred (B, T): parameter gradients go to `grads` under pfx + the reference's names,
-        d prompts (B, Np, D) f32 is accumulated in place; returns d x0 (B, T, D) f32."""
+        d prompts (B, Np, D) f32 is accumulated in place; returns d x0 (B, T, D) f32.  seed: the forward's dropout seed
+        (its masks are regenerated)."""
         x = S["x"]
         B, Tn, D = x.shape
         Np = d_prompts.shape[1]
@@ -588,7 +607,8 @@ class DurationPitchPredictor(_EncoderBase):
             # ---- x += Wo attn(Wq nx, Wkv [nx ; prompts]), nx = RMSNorm(x): the keys include the queries ----
             ops.cast_bf16(dxr, dxr_bf)
             d_nx, _ = attention_backward(dxr_bf, L["nx"], L["o"], L["lse"], L["q"], L["kv"], T[f"{name}{l}_o"],
-                                         T[f"{name}{l}_q"], H, grads, lp + "2.", d_kv=d_kv)
+                                         T[f"{name}{l}_q"], H, grads, lp + "2.", d_kv=d_kv,
+                                         dropout=self._cross_attn_dropout(seed, name, l))
             linear_backward(d_kv, L["ctx"], grads, lp + "2.to_kv", bias=False)
             # d ctx = d kv Wkv, split: the first Tn rows join the query path's d nx, the rest is d prompts
             d_nx32 = ops.gemm(d_kv[:, :Tn], T[f"{name}{l}_kv"], e(B, Tn, D, dt=torch.float32), n=D, epilogue=ops.EPI_F32)
@@ -647,8 +667,11 @@ class DurationPitchPredictor(_EncoderBase):
         B, Np, Dp = encoded_prompts.shape
         assert x.shape[-1] == self.dim_hidden and Dp == self.dim_hidden
         prompts_bf = ops.cast_bf16(encoded_prompts.float().contiguous(), torch.empty(B, Np, Dp, device=dev, dtype=bf))
-        duration = self._trunk("d", self.to_duration_pred, P, x, prompts_bf, saved)
-        pitch = self._trunk("p", self.to_pitch_pred, P, x, prompts_bf, saved)
+        seed = self._dropout_seed()
+        if saved is not None:
+            saved["dropout_seed"] = seed
+        duration = self._trunk("d", self.to_duration_pred, P, x, prompts_bf, saved, seed)
+        pitch = self._trunk("p", self.to_pitch_pred, P, x, prompts_bf, saved, seed)
         return duration, pitch
 
     def _train_backward(self, S, d_duration: Optional[torch.Tensor], d_pitch: Optional[torch.Tensor]):
@@ -666,7 +689,7 @@ class DurationPitchPredictor(_EncoderBase):
             if d is None:
                 grads.update({pfx + n: None for n, _ in trunk.named_parameters()})
                 continue
-            dx_t = self._trunk_backward(name, trunk, P, T, S[name], d, d_prompts, grads, pfx)
+            dx_t = self._trunk_backward(name, trunk, P, T, S[name], d, d_prompts, grads, pfx, S["dropout_seed"])
             dx = dx_t if dx is None else dx.add_(dx_t)          # x feeds both trunks
         if "emb" in P:   # the ids get no gradient; the table does (pad id 0, as `_forward` gathers)
             grads["phoneme_token_emb.weight"] = ops.embedding_bwd(S["ids"], dx, torch.zeros_like(P["emb"]), 0)
@@ -778,6 +801,8 @@ class Conditioner(nn.Module):
 
     train_dropout=True makes training draw the reference's dropout in both encoders (their `train_dropout`; see the
     module docstring).  The default False keeps them deterministic, as before the option existed.
+    duration_pitch_dropout=True does the same for the duration / pitch predictor (its cross attentions' dropout, the
+    only dropout of the reference's predictor with p > 0); train_dropout leaves the predictor deterministic.
 
     train_duration_pitch=True also trains the duration / pitch predictor: mode="train" runs it on the same encoder
     outputs and returns (prompt_enc, cond, duration_loss, pitch_loss), the reference's L1 losses against the given
@@ -787,12 +812,14 @@ class Conditioner(nn.Module):
     train_duration_pitch = False
 
     def __init__(self, *, dim_codebook=128, num_phoneme_tokens=None, tokenizer=None, duration_pitch_dim=512,
-                 pitch_emb_dim=256, pitch_emb_pp_hidden_dim=512, train_dropout=False, train_duration_pitch=False):
+                 pitch_emb_dim=256, pitch_emb_pp_hidden_dim=512, train_dropout=False, train_duration_pitch=False,
+                 duration_pitch_dropout=False):
         super().__init__()
         self.phoneme_enc = PhonemeEncoder(tokenizer=tokenizer, num_tokens=num_phoneme_tokens)
         self.prompt_enc = SpeechPromptEncoder(dim_codebook=dim_codebook)
         self.phoneme_enc.train_dropout = self.prompt_enc.train_dropout = bool(train_dropout)
         self.duration_pitch = DurationPitchPredictor(dim=duration_pitch_dim)
+        self.duration_pitch.train_dropout = bool(duration_pitch_dropout)
         self.pitch_emb = nn.Embedding(pitch_emb_dim, pitch_emb_pp_hidden_dim)
         self.train_duration_pitch = bool(train_duration_pitch)
         self.grad_reducer = None

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Conditional training step with the conditioning front end in the loop, timed beside the same step without it.
 
-    python tools/train_cond_bench.py [--steps K] [--warmup W] [--duration-pitch]
+    python tools/train_cond_bench.py [--steps K] [--warmup W] [--duration-pitch] [--duration-pitch-dropout]
 
   cond_e2e   configs[4] training step (cfg3 denoiser Model(512, depth 12, heads 8, dim_prompt 512), B=32, N=1024) with
              SpeechPromptEncoder(dim_codebook=128) on (32, 103, 128) prompt latents, PhonemeEncoder on 100 phoneme ids
@@ -13,6 +13,9 @@
              losses, timed alternately with cond_e2e (two rounds each); and dpp_alone: the predictor's forward +
              backward on its own at B 32 x T 100 x Np 103 (CUDA events per call, median of --calls calls, two rounds)
              with the peak memory of one training call
+  --duration-pitch-dropout  (implies --duration-pitch) also times cond_e2e_dp with the predictor's dropout drawn
+             (Conditioner(duration_pitch_dropout=True): p = 0.2 on its 20 cross attentions) alternately
+             with cond_e2e_dp without it (two rounds each), and the predictor alone with it
 Prints one JSON line: ms / steps per second of both, the encoders' measured share of the step (1 - cfg5 / cond_e2e),
 the card name and its enforced power limit (part of every number).
 """
@@ -65,8 +68,11 @@ def main():
                     help="train the encoders with the reference's dropout (Conditioner(train_dropout=True))")
     ap.add_argument("--duration-pitch", action="store_true",
                     help="also time the step with the duration / pitch predictor trained, and the predictor alone")
+    ap.add_argument("--duration-pitch-dropout", action="store_true",
+                    help="also time the --duration-pitch step and the predictor alone with the predictor's dropout")
     ap.add_argument("--calls", type=int, default=20, help="predictor-alone calls per round (median)")
     args = ap.parse_args()
+    args.duration_pitch |= args.duration_pitch_dropout
     dev = torch.device("cuda", 0)
     torch.manual_seed(0)
     model = Model(**CFG3).to(dev).train()
@@ -138,9 +144,18 @@ def duration_pitch_legs(args, ns, cond_net, opt, step_e2e, trained, lat, text, p
         rounds["cond_e2e"].append(timed(step_e2e, args.steps, args.warmup)[0])
         cond_net.train_duration_pitch = True
         rounds["cond_e2e_dp"].append(timed(step_dp, args.steps, args.warmup)[0])
+    dp = cond_net.duration_pitch
+    if args.duration_pitch_dropout:   # the predictor's step with and without its dropout, alternated
+        cond_net.train_duration_pitch = True
+        rounds["cond_e2e_dp_no_dropout"], rounds["cond_e2e_dp_dropout"] = [], []
+        for _ in range(2):
+            dp.train_dropout = False
+            rounds["cond_e2e_dp_no_dropout"].append(timed(step_dp, args.steps, args.warmup)[0])
+            dp.train_dropout = True
+            rounds["cond_e2e_dp_dropout"].append(timed(step_dp, args.steps, args.warmup)[0])
+        dp.train_dropout = False
     cond_net.train_duration_pitch = False
     # the predictor alone: phoneme encodings and prompts as the encoders hand them over
-    dp = cond_net.duration_pitch
     g = torch.Generator().manual_seed(300)
     x = torch.randn(B, T, 512, generator=g).to(dev).requires_grad_(True)
     pr = torch.randn(B, NP, 512, generator=g).to(dev).requires_grad_(True)
@@ -160,8 +175,7 @@ def duration_pitch_legs(args, ns, cond_net, opt, step_e2e, trained, lat, text, p
     call()
     torch.cuda.synchronize()
     peak_mb = (torch.cuda.max_memory_allocated(dev) - base) / 2 ** 20
-    alone = []
-    for _ in range(2):
+    def median_call_ms():
         ms = []
         for _ in range(args.calls):
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -170,13 +184,32 @@ def duration_pitch_legs(args, ns, cond_net, opt, step_e2e, trained, lat, text, p
             e1.record()
             torch.cuda.synchronize()
             ms.append(e0.elapsed_time(e1))
-        alone.append(sorted(ms)[len(ms) // 2])
+        return sorted(ms)[len(ms) // 2]
+
+    alone, alone_dropout = [], []
+    for _ in range(2):
+        alone.append(median_call_ms())
+        if args.duration_pitch_dropout:
+            dp.train_dropout = True
+            alone_dropout.append(median_call_ms())
+            dp.train_dropout = False
     dp.eval()
     with torch.no_grad():
         launches_fwd = _launches(lambda: dp(x.detach(), pr.detach()))
     dp.train()
     launches_train = _launches(call)
-    return {"duration_pitch": {
+    extra = {}
+    if args.duration_pitch_dropout:
+        dp.train_dropout = True
+        extra = {"dropout": {
+            "cond_e2e_dp_no_dropout_ms_rounds": [round(v, 3) for v in rounds["cond_e2e_dp_no_dropout"]],
+            "cond_e2e_dp_dropout_ms_rounds": [round(v, 3) for v in rounds["cond_e2e_dp_dropout"]],
+            "dropout_share_of_dp_step": round(1.0 - sum(rounds["cond_e2e_dp_no_dropout"])
+                                              / sum(rounds["cond_e2e_dp_dropout"]), 4),
+            "alone_fwd_bwd_median_ms_rounds": [round(v, 3) for v in alone_dropout], "p": dp.attn_dropout,
+            "launches_fwd_bwd": _launches(call)}}
+        dp.train_dropout = False
+    return {"duration_pitch": {**extra,
         "cond_e2e_ms_rounds": [round(v, 3) for v in rounds["cond_e2e"]],
         "cond_e2e_dp_ms_rounds": [round(v, 3) for v in rounds["cond_e2e_dp"]],
         "predictor_share_of_step": round(1.0 - sum(rounds["cond_e2e"]) / sum(rounds["cond_e2e_dp"]), 4),

@@ -200,6 +200,9 @@ __global__ void __launch_bounds__(ab::THREADS, 1) attn_bwd_kernel(const __grid_c
             pv[e] = pp;
             dv[e] = pp * (dp[4 * jj + e] - Dl[t]) * p.scale;
           }
+          // a softmax over one key is the constant 1: dS = 0 exactly, not the rounding left of dP - D (dP and
+          // D = rowsum(dO * O) are summed in different orders), so dQ and dK come out as exact zeros
+          if (p.kv_len == 1) dv[e] = 0.f;
         }
         pa[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(pv[0], pv[1]);
         pa[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(pv[2], pv[3]);

@@ -213,6 +213,7 @@ class _TransformerParams(nn.Module):
 class _PerceiverParams(nn.Module):
     def __init__(self, dim, depth, dim_context, num_latents, dim_head, heads, ff_mult=4):
         super().__init__()
+        self.ff_inner = int(dim * ff_mult * 2 / 3)   # its own feed-forward width: the reference keeps ff_mult=4 here
         self.proj_context = nn.Linear(dim_context, dim) if dim_context != dim else nn.Identity()
         self.latents = nn.Parameter(torch.randn(num_latents, dim))
         nn.init.normal_(self.latents, std=0.02)
@@ -473,7 +474,7 @@ class Model(_PackedCache):
         if "pr_proj_w" in P:
             proj = ops.gemm(p_bf, P["pr_proj_w"], e(B, Np, D), n=D, epilogue=ops.EPI_BF16, bias=P["pr_proj_b"])
         lat = pr.latents.detach().float().unsqueeze(0).expand(B, M, D).contiguous()
-        Dp = _round_up(self.ff_inner, 128)
+        Dp = _round_up(pr.ff_inner, 128)
         layers = []
         for i in range(len(pr.layers)):
             if keep or i == 0:   # inference reuses the first layer's buffers

@@ -108,6 +108,10 @@ def gemm(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, n: int, epilogu
     args.epilogue = epilogue
     if bias is not None:
         _req(bias, torch.float32, "bias")
+        # the epilogue reads bias[g * b_group_row_stride + col] for every output column col < n (and + bias1_off)
+        need = (groups - 1) * b_group_row_stride + n + (bias1_off if epilogue == EPI_WAVENET else 0)
+        if not bias.is_contiguous() or bias.numel() < need:
+            raise ValueError(f"bias must be contiguous with >= {need} elements for n={n}, got {bias.numel()}")
     args.bias = _ptr(bias)
     args.bias1_off = bias1_off
     args.out = out.data_ptr()

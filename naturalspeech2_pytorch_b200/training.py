@@ -366,7 +366,7 @@ def _conditioning_backward_tokens(model, S, T, d_xkv, grads, want_prompt: bool):
         L = S["pr_layers"][i]
         pfx = f"perceiver_resampler.layers.{i}."
         # feed-forward (no conv, no pre-norm): lat += W2 GEGLU(W1 lat)
-        ops.accum_bf16(dlat, ff_backward(dlat_bf, L["lat_bf2"], L["g"], None, P, T, f"pr{i}_ff_", model.ff_inner, grads,
+        ops.accum_bf16(dlat, ff_backward(dlat_bf, L["lat_bf2"], L["g"], None, P, T, f"pr{i}_ff_", pr.ff_inner, grads,
                                          pfx + "1."), dlat_bf)
         # attention over cat(latents, projected prompt): lat += Wo attn(Wq lat, Wkv cat)
         d_lat, d_cat = attention_backward(dlat_bf, L["lat_bf"], L["o"], L["lse"], L["q"], L["kv"], T[f"pr{i}_o"],

@@ -63,6 +63,9 @@ CASES = {
     "cond_samedim": (dict(dim=128, depth=1, heads=4, wavenet_layers=2, wavenet_stacks=2, dim_prompt=128,
                           condition_on_prompt=True, resampler_depth=2, num_latents_m=16), 3, 130, 25, 200),
     "readme_uncond": (dict(dim=128, depth=6), 1, 1024, None, None),
+    # ff_mult 2 in the denoiser while the perceiver keeps its own default ff_mult 4 (ns2.py:864-872); dim_cond_mult 2
+    "cond_ff2": (dict(dim=128, depth=2, heads=2, ff_mult=2, dim_cond_mult=2, wavenet_layers=3, wavenet_stacks=2,
+                      dim_prompt=192, condition_on_prompt=True), 2, 32, 12, 24),
 }
 
 # Slices of the BENCHMARKED configurations (BASELINE.json configs[1] / configs[2]: dim 512, heads 8, seq 1024) at

@@ -10,7 +10,7 @@ import torch
 from param_fill import fill_module
 
 GOLDEN = Path(__file__).resolve().parent / "golden"
-MODEL_CASES = ["uncond_small", "cond_small", "cond_samedim", "readme_uncond"]
+MODEL_CASES = ["uncond_small", "cond_small", "cond_samedim", "readme_uncond", "cond_ff2"]
 # slices of the benchmarked configurations (dim 512, heads 8, seq 1024, depth 2): inputs are regenerated from seeds,
 # outputs are stored on a row subsample (see tests/golden/make_golden.py BIG_CASES)
 BIG_MODEL_CASES = ["cfg2_slice", "cfg3_slice"]

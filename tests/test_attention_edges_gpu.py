@@ -183,3 +183,24 @@ def test_attention_bwd_determinism():
     assert torch.equal(a["dk"], b["dk"]) and torch.equal(a["dv"], b["dv"])
     ref = reference(q, k, v, d_o, H, 64 ** -0.5)
     assert_close(b["dq"], a["dq"], 2 * ref["b_dq"], RL2, "dq run-to-run")
+
+
+@pytest.mark.parametrize("dropout", [None, (7, 3, 0.25)], ids=["plain", "dropout"])
+@pytest.mark.parametrize("B,H,Nq", [(1, 1, 1), (2, 8, 300)])
+def test_attention_bwd_single_key_gives_exact_zero_dq_dk(B, H, Nq, dropout):
+    """kv_len = 1: the softmax is the constant 1, so dQ and dK are exactly zero (in float64 too: the cross attention
+    over one perceiver latent and a one-frame self-attention give exact-zero weight gradients), while dV = P^T dO."""
+    from naturalspeech2_pytorch_b200 import ops
+    q, k, v, d_o = _inputs(B, H, Nq, 1, seed=21 + Nq)
+    inner = H * 64
+    o = torch.empty(B, Nq, inner, device=dev, dtype=bf)
+    lse = torch.empty(B, H, Nq, device=dev)
+    ops.attention(q, k, v, o, heads=H, lse=lse, dropout=dropout)
+    dq = torch.zeros(B, Nq, inner, device=dev)
+    dk, dv = (torch.full((B, 1, inner), float("nan"), device=dev, dtype=bf) for _ in range(2))
+    ops.attention_bwd(q, k, v, o, d_o, lse, dq, dk, dv, heads=H, dropout=dropout)
+    assert int((dq != 0).sum()) == 0 and int((dk != 0).sum()) == 0
+    assert bool(torch.isfinite(dv).all())
+    if dropout is None:
+        ref = reference(q, k, v, d_o, H, 64 ** -0.5)
+        assert_close(dv, ref["dv"], ref["b_dv"], RL2, "dv, one key")

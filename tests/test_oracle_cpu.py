@@ -127,7 +127,7 @@ def test_rvq_oracle_matches_encodec_port():
     assert (rvq_oracle.encode(cbn[0, 7][None], cbn)[0, 0]) == 3
 
 
-@pytest.mark.parametrize("name", ["uncond_small", "cond_small", "cond_samedim"])
+@pytest.mark.parametrize("name", ["uncond_small", "cond_small", "cond_samedim", "cond_ff2"])
 def test_torch_port_matches_reference(name):
     """The torch-CPU port used for bench.py's reference arm reproduces the reference fp32/fp64 outputs."""
     from oracle import denoiser_torch_port as tp

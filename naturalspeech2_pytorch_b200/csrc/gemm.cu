@@ -7,7 +7,9 @@
 //   warpgroups 1-2 consumers: warpgroup w owns positions [64 (w-1), 64 w) of the tile, issues wgmma m64nBNk16 from the
 //                  shared-memory ring into register accumulators, then runs the epilogue (bias / residual / GEGLU /
 //                  FiLM + gate) in registers, stages the results in shared memory (two 8 KB boxes per warpgroup)
-//                  and writes them with TMA stores; the in-place fp32 residual is added by TMA reduce-add at L2
+//                  and writes them with TMA stores; the in-place fp32 residual is added by TMA reduce-add at L2.
+//                  The tile's column vectors (bias, FiLM) are copied into shared memory by cp.async while its
+//                  mainloop runs, so the epilogue reads them from there instead of waiting on global loads
 // Tiles are handed out by a static round robin, n fastest so co-resident CTAs share A rows in L2.
 //
 // Replaces, in the reference: nn.Linear GEMMs (ns2.py:1021,1024,1051-1053,783,613,731) and
@@ -72,6 +74,34 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmDev& p, int tile) {
 // residual update.  Thread (warp ww of the consumer warpgroup, lane l) holds rows 16 ww + l/4 + 8i of its warpgroup's
 // 64 rows, columns 8j + 2(l%4) + k:  acc[4j + 2i + k].
 // ------------------------------------------------------------------------------------------------
+// The tile's column vectors, fp32 in shared memory (vec), column c of the tile at:
+//   BF16 / F32  vec[c]                                    bias (not loaded without one)
+//   GEGLU       vec[c] value bias, vec[c + 128] gate bias
+//   WAVENET     vec[c] b0, vec[128 + c] b1 (bias1_off), vec[256 + c] FiLM gamma, vec[384 + c] FiLM beta
+template <int BN, int EPI>
+constexpr int tile_vec_floats() { return EPI == NS2_EPI_WAVENET ? 4 * BN : BN; }
+
+// Issue the copies of the tile's vectors: one 16-byte cp.async per consumer thread (ct in [0, 256)) at most.  Columns
+// at or past n are not read (n is a multiple of 32, so a 4-column piece is all in or all out).
+template <int BN, int EPI>
+__device__ __forceinline__ void load_tile_vectors(const GemmDev& p, const TileCoord& t, uint32_t vec, int ct) {
+  constexpr int PIECES = BN / 4;   // 16-byte pieces per vector
+  static_assert(tile_vec_floats<BN, EPI>() / 4 <= 256, "one piece per consumer thread");
+  const int v = ct / PIECES;
+  const int c = 4 * (ct - v * PIECES);
+  const int col = t.n_tile * BN + c;
+  if (ct >= tile_vec_floats<BN, EPI>() / 4 || col >= p.n) return;
+  const float* src;
+  if constexpr (EPI == NS2_EPI_WAVENET) {
+    src = v < 2 ? p.bias + t.g * p.b_grs + col + (v == 1 ? p.bias1_off : 0)
+                : p.film + t.b * p.film_bs + t.g * p.film_gs + col + (v == 3 ? p.n : 0);
+  } else {
+    if (p.bias == nullptr) return;
+    src = p.bias + t.g * p.b_grs + col;
+  }
+  cp_async_16(vec + 4 * (v * BN + c), src);
+}
+
 __device__ __forceinline__ float silu_f(float v) { return __fdividef(v, 1.0f + __expf(-v)); }
 
 // tanh(z) * sigmoid(z) with ONE MUFU: u = tanh(z/2); sigmoid = (1 + u)/2; tanh(z) = 2u / (1 + u^2), the reciprocal of
@@ -123,12 +153,15 @@ __device__ __forceinline__ void stage_f32(uint32_t buf, const float (&o)[16], in
   }
 }
 
-// One tile of one consumer warpgroup.  stg: its two staging boxes; nbox: boxes it has issued so far.  Only the
-// warpgroup's first thread (`leader`) issues and waits on bulk groups; the box written now was last read by the store
-// issued two boxes ago, which the leader waited for before the previous box's barrier.
+// One tile of one consumer warpgroup.  vec: the tile's column vectors in shared memory; stg: its two staging boxes;
+// nbox: boxes it has issued so far.  Only the warpgroup's first thread (`leader`) issues and waits on bulk groups; the
+// box written now was last read by the store issued two boxes ago, which the leader waited for before the previous
+// box's barrier.  (Waiting for that store only, just before the write, needs a second barrier per box and measured no
+// faster on H100; see DESIGN.md section 5.)
 template <int BN, int NACC, int EPI>
 __device__ __forceinline__ void epilogue_tile(const GemmDev& p, const TileCoord& t, const float (&acc)[NACC][BN / 2],
-                                              int cw, int ww, int lane, bool leader, uint32_t stg, uint32_t& nbox) {
+                                              const float* vec, int cw, int ww, int lane, bool leader, uint32_t stg,
+                                              uint32_t& nbox) {
   constexpr int CW = EPI == NS2_EPI_F32 ? 32 : 64;                   // output columns per staging box
   constexpr int OUT_COLS = EPI == NS2_EPI_GEGLU ? 128 : BN;         // output columns of the tile
   // First position of this warpgroup's rows.  When it is past a_rows the stores below are clipped away entirely; the
@@ -158,6 +191,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmDev& p, const TileCoord&
     for (int jj = 0; jj < CW / 8; ++jj) {
       const int j = q * (CW / 8) + jj;        // accumulator column group
       const int col = out_col0 + 8 * j + c2;  // output column of k = 0 (value column for GEGLU)
+      const int c = 8 * j + c2;               // its column inside the tile
       if (out_col0 + 8 * j >= out_n) {        // right half of a 64-column box past n: clipped by the TMA store
         put(jj, 0, 0.f, 0.f);
         put(jj, 1, 0.f, 0.f);
@@ -167,7 +201,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmDev& p, const TileCoord&
       }
       if constexpr (EPI == NS2_EPI_BF16 || EPI == NS2_EPI_F32) {
         float2 bb = make_float2(0.f, 0.f);
-        if (p.bias != nullptr) bb = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + col));
+        if (p.bias != nullptr) bb = *reinterpret_cast<const float2*>(vec + c);
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
           float v0 = acc[0][4 * j + 2 * i], v1 = acc[0][4 * j + 2 * i + 1];
@@ -192,21 +226,20 @@ __device__ __forceinline__ void epilogue_tile(const GemmDev& p, const TileCoord&
         }
       } else if constexpr (EPI == NS2_EPI_GEGLU) {
         static_assert(EPI != NS2_EPI_GEGLU || BN == 256, "GEGLU tiles pair 128 value + 128 gate rows");
-        const int c = 8 * j + c2;   // value column inside the tile; its gate is column c + 128 (fragment j + 16)
-        const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + t.n_tile * BN + c));
-        const float2 bg = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + t.n_tile * BN + c + 128));
+        // value column c, its gate column c + 128 (fragment j + 16)
+        const float2 bv = *reinterpret_cast<const float2*>(vec + c);
+        const float2 bg = *reinterpret_cast<const float2*>(vec + c + 128);
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
-          put(jj, i, (acc[0][4 * j + 2 * i] + bv.x) * gelu_erf(acc[0][4 * (j + 16) + 2 * i] + bg.x),
-              (acc[0][4 * j + 2 * i + 1] + bv.y) * gelu_erf(acc[0][4 * (j + 16) + 2 * i + 1] + bg.y));
+          put(jj, i, (acc[0][4 * j + 2 * i] + bv.x) * gelu_erf_fast(acc[0][4 * (j + 16) + 2 * i] + bg.x),
+              (acc[0][4 * j + 2 * i + 1] + bv.y) * gelu_erf_fast(acc[0][4 * (j + 16) + 2 * i + 1] + bg.y));
         }
       } else {  // NS2_EPI_WAVENET: y = tanh(z) sigmoid(z) + res, z = (conv + b0) * gamma + beta   (ns2.py:619-636)
         static_assert(EPI != NS2_EPI_WAVENET || NACC == 2, "wavenet block needs conv + res accumulators");
-        const float2 b0 = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + col));
-        const float2 b1 = __ldg(reinterpret_cast<const float2*>(p.bias + t.g * p.b_grs + col + p.bias1_off));
-        const float* fp = p.film + t.b * p.film_bs + t.g * p.film_gs + col;
-        const float2 ga = __ldg(reinterpret_cast<const float2*>(fp));
-        const float2 be = __ldg(reinterpret_cast<const float2*>(fp + p.n));
+        const float2 b0 = *reinterpret_cast<const float2*>(vec + c);
+        const float2 b1 = *reinterpret_cast<const float2*>(vec + BN + c);
+        const float2 ga = *reinterpret_cast<const float2*>(vec + 2 * BN + c);
+        const float2 be = *reinterpret_cast<const float2*>(vec + 3 * BN + c);
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
           const float z0 = fmaf(acc[0][4 * j + 2 * i] + b0.x, ga.x, be.x);
@@ -244,9 +277,13 @@ struct GemmCfg {
   static constexpr int THREADS = 384;
   static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
   static constexpr int STG_OFF = RING_BYTES;                        // 2 consumer warpgroups x 2 staging boxes
-  static constexpr int BAR_OFF = STG_OFF + 4 * STG_BYTES;
-  static constexpr int SMEM_BYTES = BAR_OFF + 1024 /*align slack*/ + 256 /*barriers*/;   // 225.25 KB of 227
+  static constexpr int VEC_OFF = STG_OFF + 4 * STG_BYTES;           // the tile's column vectors (tile_vec_floats)
+  static constexpr int BAR_OFF = VEC_OFF + (NACC == 2 ? 4 : 1) * BN * 4;
+  static constexpr int SMEM_BYTES = BAR_OFF + 256 /*barriers*/;     // 226.25 KB (WAVENET) of 227
+  static_assert(SMEM_BYTES <= 232448, "over the sm_90 per-block shared-memory limit");
 };
+
+constexpr int CONSUMER_BAR = 1;   // named barrier over the 256 consumer threads (warpgroup_bar uses 8 and 9)
 
 template <int BN>
 __device__ __forceinline__ void wgmma_tile_k16(float (&d)[BN / 2], uint64_t da, uint64_t db) {
@@ -257,9 +294,8 @@ __device__ __forceinline__ void wgmma_tile_k16(float (&d)[BN / 2], uint64_t da, 
 template <int BN, int NACC, int EPI>
 __global__ void __launch_bounds__(GemmCfg<BN, NACC>::THREADS, 1) gemm_kernel(const __grid_constant__ GemmDev p) {
   using Cfg = GemmCfg<BN, NACC>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
+  static_assert(Cfg::VEC_OFF / 4 + tile_vec_floats<BN, EPI>() <= Cfg::BAR_OFF / 4, "vector area too small");
+  extern __shared__ __align__(1024) uint8_t smem[];   // 128-byte swizzled TMA boxes need 1024-byte alignment
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::BAR_OFF);
   uint64_t* full_bar = bars;                 // [STAGES]
   uint64_t* empty_bar = bars + Cfg::STAGES;  // [STAGES] one arrive per consumer warp
@@ -268,6 +304,7 @@ __global__ void __launch_bounds__(GemmCfg<BN, NACC>::THREADS, 1) gemm_kernel(con
   const int lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
+    if ((smem_u32(smem) & 1023u) != 0) __trap();   // dynamic smem not 1024-byte aligned (no printf: see mbar_wait)
     tma_prefetch_desc(&p.tmA);
     tma_prefetch_desc(&p.tmB);
     tma_prefetch_desc(&p.tmOut);
@@ -316,11 +353,18 @@ __global__ void __launch_bounds__(GemmCfg<BN, NACC>::THREADS, 1) gemm_kernel(con
     const int ww = warp & 3;
     const bool leader = (threadIdx.x & 127) == 0;   // issues and waits on this warpgroup's bulk stores
     const uint32_t stg = smem_u32(smem + Cfg::STG_OFF + cw * 2 * STG_BYTES);
+    const float* vec = reinterpret_cast<const float*>(smem + Cfg::VEC_OFF);
+    // the epilogue reads column vectors (uniform over the grid): copy them in under each tile's mainloop
+    const bool tile_vecs = !p.skip_epilogue && (EPI == NS2_EPI_GEGLU || EPI == NS2_EPI_WAVENET || p.bias != nullptr);
     uint32_t nbox = 0;
     float acc[NACC][BN / 2];
     uint32_t it = 0;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       const TileCoord t = decode_tile(p, tile);
+      if (tile_vecs) {
+        named_bar(CONSUMER_BAR, 256);   // both warpgroups' epilogues of the previous tile are done reading vec
+        load_tile_vectors<BN, EPI>(p, t, smem_u32(vec), threadIdx.x - 128);
+      }
 #pragma unroll
       for (int a = 0; a < NACC; ++a)
 #pragma unroll
@@ -355,7 +399,11 @@ __global__ void __launch_bounds__(GemmCfg<BN, NACC>::THREADS, 1) gemm_kernel(con
 #pragma unroll
       for (int a = 0; a < NACC; ++a) wgmma_hold(acc[a]);
       if (prev_stage >= 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev_stage]));
-      if (!p.skip_epilogue) epilogue_tile<BN, NACC, EPI>(p, t, acc, cw, ww, lane, leader, stg, nbox);
+      if (tile_vecs) {
+        cp_async_wait_all();             // this thread's copies have landed
+        named_bar(CONSUMER_BAR, 256);   // and every other thread's
+      }
+      if (!p.skip_epilogue) epilogue_tile<BN, NACC, EPI>(p, t, acc, vec, cw, ww, lane, leader, stg, nbox);
     }
     if (leader) tma_store_wait_all();   // shared memory must outlive the reads of the last stores
   }

@@ -137,6 +137,13 @@ __device__ __forceinline__ void bulk_load_1d(uint32_t dst_smem, const void* src,
                : "memory");
 }
 
+// 16-byte global -> shared copy (LDGSTS, cached in L2 only): no register round trip; cp_async_wait_all completes it
+__device__ __forceinline__ void cp_async_16(uint32_t dst_smem, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst_smem), "l"(reinterpret_cast<uint64_t>(src))
+               : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void tma_store_wait_read() {  // smem of all but the N newest groups may be reused
@@ -191,6 +198,10 @@ __device__ __forceinline__ void st_shared_v2_f32(uint32_t addr, float a, float b
 __device__ __forceinline__ void warpgroup_bar(int wg) {
   asm volatile("bar.sync %0, 128;" ::"r"(8 + wg) : "memory");
 }
+// named barrier `id` over `count` threads (a multiple of 32); id 0 is __syncthreads
+__device__ __forceinline__ void named_bar(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 // ---------------------------------------------------------------------------------------------
 // small numeric helpers
@@ -211,7 +222,8 @@ __device__ __forceinline__ float tanh_fast(float x) {
   return y;
 }
 __device__ __forceinline__ float sigmoid_fast(float x) { return fmaf(tanh_fast(0.5f * x), 0.5f, 0.5f); }
-// exact-erf GELU with erf from Abramowitz-Stegun 7.1.26 (|error| <= 1.5e-7): one MUFU.EX2, one MUFU.RCP, 8 FMA
+// exact-erf GELU with erf from Abramowitz-Stegun 7.1.26 (|error| <= 1.5e-7; < 6e-7 as evaluated here in fp32, the
+// most near x = 0 where 1 - poly e cancels): one MUFU.EX2, one MUFU.RCP, 8 FMA.  The GEGLU GEMM epilogue uses it.
 __device__ __forceinline__ float gelu_erf_fast(float x) {
   const float z = fabsf(x) * 0.70710678118654752440f;
   float t;

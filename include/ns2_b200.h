@@ -149,6 +149,17 @@ typedef struct ns2_attn_args {
 
 int ns2_attn_fwd(const ns2_attn_args* args, ns2_stream_t stream);
 
+/* Key padding for a batch of sequences of different lengths: ns2_attn_fwd where sample b attends to keys
+ * [0, kv_lens[b]) only — Attend with a key-padding mask (attend.py:123-129, 140-142: masked scores -> -max, i.e.
+ * probability 0), the `mask` that PhonemeEncoder (ns2.py:275), SpeechPromptEncoder's Transformer (ns2.py:1110-1115)
+ * and the perceiver / predictor cross attentions (ns2.py:572-577, 457-466) would pass for padded batches.
+ *   kv_lens: device int32 (batches); each value is clamped to [1, kv_len] (callers should reject others).
+ *   K / V rows at or past kv_lens[b] are never weighted, but they must be FINITE: their probability is exactly 0 and
+ *   0 * V is still formed (V = NaN or inf there would reach the output).
+ *   Query rows are not masked: rows a caller treats as padding get finite, meaningless output.
+ *   Sample b's output rows are bit-identical to ns2_attn_fwd on that sample alone with kv_len = kv_lens[b]. */
+int ns2_attn_fwd_ragged(const ns2_attn_args* args, const int32_t* kv_lens, ns2_stream_t stream);
+
 /* Backward of the above (autograd of F.scaled_dot_product_attention, reached from loss.backward(), ns2.py:1886):
  *   dq_accum (batches, q_len, heads*64) f32, contiguous: dQ is ADDED to it (every key tile adds its share; zero it for
  *   a plain gradient);
@@ -236,12 +247,36 @@ int ns2_cast_bf16(const float* x, const float* add, int64_t count, void* out_bf1
                   ns2_stream_t stream);
 int ns2_mean_rows(const float* x, int32_t batch, int32_t n, int32_t dim, float* out,
                   ns2_stream_t stream);
+/*    ns2_mean_rows_ragged : out[b,:] = mean over n < lens[b] of x[b,n,:] (lens: device int32 (batch), clamped to [1, n];
+ *                           summed in ns2_mean_rows' order) — the prompt mean-pool (ns2.py:859) of a sample run alone
+ *    ns2_mask_rows        : x[b, r, 0:cols] = 0 for lens[b] <= r < rows (lens clamped to [0, rows]), in place; x is f32
+ *                           (f32 != 0) or bf16 with element strides row_stride / batch_stride — the zero padding past a
+ *                           sample's end that a "same" convolution (ns2.py:316-320, 345-365) reads
+ *    ns2_pack_rows_ragged : bf16 out[b, r, 0:cols] = a[b, r, :] for r < La, b[b, r - La, :] for La <= r < La + Lb,
+ *                           0 up to out_rows (La = a_lens[b] clamped to [0, a_rows], Lb = b_lens[b] clamped to
+ *                           [0, b_rows]; out_rows >= a_rows + b_rows): the keys [norm(x) ; prompts] of the predictor's
+ *                           cross attention (ns2.py:1060-1061) as one prefix of length La + Lb.  cols and every stride
+ *                           a multiple of 4, pointers 8-byte aligned. */
+int ns2_mean_rows_ragged(const float* x, int32_t batch, int32_t n, int32_t dim, const int32_t* lens, float* out,
+                         ns2_stream_t stream);
+int ns2_mask_rows(void* x, int32_t f32, int64_t row_stride, int64_t batch_stride, int32_t batch, int32_t rows,
+                  int32_t cols, const int32_t* lens, ns2_stream_t stream);
+int ns2_pack_rows_ragged(const void* a, int64_t a_row_stride, int64_t a_batch_stride, int32_t a_rows,
+                         const int32_t* a_lens, const void* b, int64_t b_row_stride, int64_t b_batch_stride,
+                         int32_t b_rows, const int32_t* b_lens, int32_t batch, int32_t cols, void* out,
+                         int64_t out_row_stride, int64_t out_batch_stride, int32_t out_rows, ns2_stream_t stream);
 /*    ns2_cond_inject      : out_bf16[b,n,:] = bf16(x[b,n,:] + c), c = 0 for n >= cond_len (zero padding, ns2.py:70-77),
  *                           null_cond[:] where drop_mask[b] (uint8, may be NULL = keep all), else cproj[b,n,:]
  *                           (cproj: projected aligned condition, token-major (batch, cond_len, dim) f32; ns2.py:978-992)
  *    ns2_select_rows      : out[b,:] = drop_mask[b] ? null_row[:] : src[b,:]  (f32 or bf16 out; ns2.py:954-968) */
 int ns2_cond_inject(const float* x, const float* cproj, const uint8_t* drop_mask, const float* null_cond,
                     int32_t batch, int32_t n, int32_t cond_len, int32_t dim, void* out_bf16, ns2_stream_t stream);
+/*    ns2_cond_inject_ragged : ns2_cond_inject where sample b's condition ends at min(cond_len, cond_lens[b]) (device
+ *                             int32 (batch), negative = 0): frames at or past it get nothing, null-substituted or not —
+ *                             the zero padding after the projection of a sample run alone (ns2.py:978-992) */
+int ns2_cond_inject_ragged(const float* x, const float* cproj, const uint8_t* drop_mask, const float* null_cond,
+                           int32_t batch, int32_t n, int32_t cond_len, int32_t dim, const int32_t* cond_lens,
+                           void* out_bf16, ns2_stream_t stream);
 int ns2_select_rows(const uint8_t* drop_mask, const float* null_row, const float* src, int64_t src_row_stride,
                     int32_t batch, int32_t row_len, void* out, int64_t out_row_stride, int32_t out_bf16,
                     ns2_stream_t stream);
@@ -262,6 +297,14 @@ int ns2_embedding_bf16(const int64_t* ids, int64_t rows, const float* table, int
 int ns2_groupnorm_silu(const float* x, int32_t batch, int32_t rows, int32_t channels, int32_t groups,
                        const float* weight, const float* bias, float eps, const float* resid, float* out_f32,
                        void* out_bf16, ns2_stream_t stream);
+/*    ns2_groupnorm_silu_ragged : ns2_groupnorm_silu where sample b has lens[b] rows (device int32 (batch), clamped to
+ *                           [1, rows]): the statistics cover rows [0, lens[b]) in the order ns2_groupnorm_silu walks a
+ *                           tensor of that many rows (bit-identical to it), and rows at or past lens[b] are written as
+ *                           exact zeros to out_f32 and out_bf16 (resid is not read there) — Block's GroupNorm over a
+ *                           sample's own phonemes (ns2.py:345-365) */
+int ns2_groupnorm_silu_ragged(const float* x, int32_t batch, int32_t rows, int32_t channels, int32_t groups,
+                              const float* weight, const float* bias, float eps, const float* resid, float* out_f32,
+                              void* out_bf16, const int32_t* lens, ns2_stream_t stream);
 int ns2_rowdot(const float* x, int64_t rows, int32_t dim, const float* w, const float* bias, int32_t relu, float* out,
                ns2_stream_t stream);
 /*    ns2_expand_encodings : length regulation, NaturalSpeech2.expand_encodings (ns2.py:1449-1455) with the hard alignment

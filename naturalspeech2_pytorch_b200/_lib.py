@@ -99,6 +99,7 @@ SIGNATURES = {
     "ns2_wgrad": (C.c_int, [C.POINTER(WgradArgs), _P]),
     "ns2_attn_fwd": (C.c_int, [C.POINTER(AttnArgs), _P]),
     "ns2_attn_bwd": (C.c_int, [C.POINTER(AttnBwdArgs), _P]),
+    "ns2_attn_fwd_ragged": (C.c_int, [C.POINTER(AttnArgs), _P, _P]),
     "ns2_attn_fwd_dropout": (C.c_int, [C.POINTER(AttnArgs), C.POINTER(Dropout), _P]),
     "ns2_attn_bwd_dropout": (C.c_int, [C.POINTER(AttnBwdArgs), C.POINTER(Dropout), _P]),
     "ns2_dropout_f32": (C.c_int, [_P, _I64, C.POINTER(Dropout), _P]),
@@ -108,12 +109,18 @@ SIGNATURES = {
     "ns2_small_linear": (C.c_int, [_P, _I64, _I32, _I32, _P, _P, _I32, _I32, _P, _I64, _P]),
     "ns2_cast_bf16": (C.c_int, [_P, _P, _I64, _P, _P]),
     "ns2_mean_rows": (C.c_int, [_P, _I32, _I32, _I32, _P, _P]),
+    "ns2_mean_rows_ragged": (C.c_int, [_P, _I32, _I32, _I32, _P, _P, _P]),
+    "ns2_mask_rows": (C.c_int, [_P, _I32, _I64, _I64, _I32, _I32, _I32, _P, _P]),
+    "ns2_pack_rows_ragged": (C.c_int, [_P, _I64, _I64, _I32, _P, _P, _I64, _I64, _I32, _P, _I32, _I32, _P, _I64, _I64,
+                                       _I32, _P]),
     "ns2_transpose_cast": (C.c_int, [_P, _I32, _I32, _I32, _P, _P]),
     "ns2_groupnorm_silu": (C.c_int, [_P, _I32, _I32, _I32, _I32, _P, _P, _F, _P, _P, _P, _P]),
+    "ns2_groupnorm_silu_ragged": (C.c_int, [_P, _I32, _I32, _I32, _I32, _P, _P, _F, _P, _P, _P, _P, _P]),
     "ns2_rowdot": (C.c_int, [_P, _I64, _I32, _P, _P, _I32, _P, _P]),
     "ns2_expand_encodings": (C.c_int, [_P, _P, _P, _I32, _P, _I32, _I32, _I32, _I32, _P, _P]),
     "ns2_embedding_bf16": (C.c_int, [_P, _I64, _P, _I32, _I32, _I32, _P, _P]),
     "ns2_cond_inject": (C.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P]),
+    "ns2_cond_inject_ragged": (C.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P, _P]),
     "ns2_select_rows": (C.c_int, [_P, _P, _P, _I64, _I32, _I32, _P, _I64, _I32, _P]),
     "ns2_q_sample": (C.c_int, [_P, _P, _P, _P, _I32, _I64, _P, _P, _I32, _P]),
     "ns2_mse_rows": (C.c_int, [_P, _P, _I32, _I64, _P, _P, _P, _P]),

@@ -14,6 +14,13 @@
 // sums l and the saved log-sum-exp use the undropped probabilities (lse is bit-identical to attn_fwd_kernel<false>'s),
 // each P element is multiplied by its keep bit before it becomes an A fragment of O += P V, and 1 / (1 - p) is applied
 // once, with 1 / l, when O is stored.
+//
+// attn_fwd_kernel<false, true> is the key-padding variant of sampling a batch of sequences of different lengths
+// (Attend with a key mask, attend.py:123-129 / 140-142, which the reference builds but never reaches, SURVEY T9):
+// sample b attends to keys [0, kv_lens[b]).  Both the producer and the softmax warpgroups take the key-tile count from
+// that length and the last tile masks the keys past it to -inf, exactly as keys past kv_len are masked; those keys'
+// P is 0, so their (finite) V rows add 0 to O.  A sample's output is therefore bit-identical to the plain kernel called
+// on its keys [0, kv_lens[b]) alone, whose padding keys are the TMA zero fill.
 #include "ptx.cuh"
 #include "philox.cuh"
 #include "host_common.h"
@@ -47,7 +54,8 @@ struct AttnDev {
   int q_len, kv_len;
   float scale_log2e;
   float* lse;   // optional (batches, heads, q_len): log2-domain log-sum-exp of the scaled scores, for the backward pass
-  DropoutDev drop;   // attn_fwd_kernel<true> only
+  DropoutDev drop;   // attn_fwd_kernel<true, false> only
+  const int* kv_lens;   // attn_fwd_kernel<false, true> only: (batches) key counts, clamped to [1, kv_len]
 };
 
 __device__ __forceinline__ float ex2_approx(float x) {
@@ -58,8 +66,9 @@ __device__ __forceinline__ float ex2_approx(float x) {
 
 __device__ __forceinline__ float keep_if(float x, uint32_t bits, int n) { return (bits >> n) & 1u ? x : 0.f; }
 
-template <bool DROPOUT>
+template <bool DROPOUT, bool RAGGED>
 __global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid_constant__ AttnDev p) {
+  static_assert(!(DROPOUT && RAGGED), "no dropout variant of the key-padding kernel");
   using namespace attn;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
@@ -71,7 +80,10 @@ __global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid
   const int q0 = blockIdx.x * BQ;
   const int head = blockIdx.y;
   const int b = blockIdx.z;
-  const int T = (p.kv_len + BKV - 1) / BKV;
+  // keys of this sample; the plain kernels read p.kv_len where they use it, which keeps their code as it was
+  const int kv_len_b = RAGGED ? min(max(__ldg(p.kv_lens + b), 1), p.kv_len) : 0;
+#define NS2_ATTN_KV_LEN (RAGGED ? kv_len_b : p.kv_len)
+  const int T = (NS2_ATTN_KV_LEN + BKV - 1) / BKV;
 
   if (threadIdx.x == 0) {
     if ((smem_u32(smem) & 1023u) != 0) __trap();   // dynamic smem not 1024-byte aligned (no printf: see mbar_wait)
@@ -148,7 +160,7 @@ __global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid
         wgmma_wait<0>();
         wgmma_hold(s);
       }
-      const int valid = p.kv_len - j * BKV;  // columns >= valid are padding keys (TMA zero-filled): excluded
+      const int valid = NS2_ATTN_KV_LEN - j * BKV;  // columns >= valid are padding keys (TMA zero-filled or past kv_lens[b])
       if (valid < BKV) {
 #pragma unroll
         for (int jj = 0; jj < BKV / 8; ++jj)
@@ -229,10 +241,12 @@ __global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid
       }
     }
   }
+#undef NS2_ATTN_KV_LEN
 }
 
-// drop == nullptr: the plain kernel; otherwise attn_fwd_kernel<true> with those dropout parameters.
-static int attn_fwd_launch(const ns2_attn_args* a, const DropoutDev* drop, cudaStream_t stream) {
+// drop == nullptr and kv_lens == nullptr: the plain kernel; drop: attn_fwd_kernel<true, false> with those dropout
+// parameters; kv_lens: attn_fwd_kernel<false, true> (never both).
+static int attn_fwd_launch(const ns2_attn_args* a, const DropoutDev* drop, const int* kv_lens, cudaStream_t stream) {
   NS2_REQUIRE(a != nullptr && a->q && a->k && a->v && a->out, "attn_fwd: NULL pointer");
   NS2_REQUIRE(a->dim_head == 64, "attn_fwd: dim_head=%d, only 64 is supported", a->dim_head);
   NS2_REQUIRE(a->batches > 0 && a->heads > 0 && a->q_len > 0 && a->kv_len > 0, "attn_fwd: empty problem");
@@ -266,13 +280,17 @@ static int attn_fwd_launch(const ns2_attn_args* a, const DropoutDev* drop, cudaS
   dev.scale_log2e = a->scale * 1.4426950408889634f;
   dev.lse = a->lse;
   dim3 grid((a->q_len + attn::BQ - 1) / attn::BQ, a->heads, a->batches);
-  if (drop == nullptr) {
-    NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<false>, attn::SMEM_BYTES));
-    attn_fwd_kernel<false><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
+  if (kv_lens != nullptr) {
+    dev.kv_lens = kv_lens;
+    NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<false, true>, attn::SMEM_BYTES));
+    attn_fwd_kernel<false, true><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
+  } else if (drop == nullptr) {
+    NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<false, false>, attn::SMEM_BYTES));
+    attn_fwd_kernel<false, false><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
   } else {
     dev.drop = *drop;
-    NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<true>, attn::SMEM_BYTES));
-    attn_fwd_kernel<true><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
+    NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<true, false>, attn::SMEM_BYTES));
+    attn_fwd_kernel<true, false><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
   }
   g_launches.fetch_add(1, std::memory_order_relaxed);
   NS2_CUDA_CHECK(cudaGetLastError());
@@ -282,7 +300,13 @@ static int attn_fwd_launch(const ns2_attn_args* a, const DropoutDev* drop, cudaS
 }  // namespace ns2
 
 extern "C" int ns2_attn_fwd(const ns2_attn_args* a, ns2_stream_t stream) {
-  return ns2::attn_fwd_launch(a, nullptr, static_cast<cudaStream_t>(stream));
+  return ns2::attn_fwd_launch(a, nullptr, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int ns2_attn_fwd_ragged(const ns2_attn_args* a, const int32_t* kv_lens, ns2_stream_t stream) {
+  using namespace ns2;
+  NS2_REQUIRE(kv_lens != nullptr, "attn_fwd_ragged: NULL kv_lens");
+  return ns2::attn_fwd_launch(a, nullptr, kv_lens, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int ns2_attn_fwd_dropout(const ns2_attn_args* a, const ns2_dropout* d, ns2_stream_t stream) {
@@ -291,5 +315,5 @@ extern "C" int ns2_attn_fwd_dropout(const ns2_attn_args* a, const ns2_dropout* d
   DropoutDev drop;
   NS2_REQUIRE(make_dropout_dev(d->seed, d->site, d->p, &drop), "attn_fwd_dropout: p=%g is not in [0, 1)",
               static_cast<double>(d->p));
-  return attn_fwd_launch(a, d->p == 0.0f ? nullptr : &drop, static_cast<cudaStream_t>(stream));
+  return attn_fwd_launch(a, d->p == 0.0f ? nullptr : &drop, nullptr, static_cast<cudaStream_t>(stream));
 }

@@ -232,18 +232,21 @@ __global__ void __launch_bounds__(256) cast_bf16_kernel(const float4* __restrict
 }
 
 // out[b, n, :] = bf16(x[b, n, :] + c) with c = 0 for n >= L (zero padding of pad_or_curtail_to_length, ns2.py:70-77),
-// null_cond[:] for a dropped sample, else cproj[b, n, :]   (torch.where(cond_drop_mask, null_cond, cond) + x, ns2.py:982-992)
+// null_cond[:] for a dropped sample, else cproj[b, n, :]   (torch.where(cond_drop_mask, null_cond, cond) + x, ns2.py:982-992).
+// cond_lens (optional): sample b's condition ends at min(L, cond_lens[b]) — the zero padding of a sample run alone.
 __global__ void __launch_bounds__(256) cond_inject_kernel(const float4* __restrict__ x, const float4* __restrict__ cproj,
                                                           const uint8_t* __restrict__ drop, const float4* __restrict__ null4,
-                                                          int n, int L, int d4, uint2* __restrict__ out) {
+                                                          int n, int L, const int* __restrict__ cond_lens, int d4,
+                                                          uint2* __restrict__ out) {
   const int b = blockIdx.y;
+  const int Lb = cond_lens != nullptr ? min(L, max(__ldg(cond_lens + b), 0)) : L;
   const bool dropped = drop != nullptr && drop[b] != 0;
   const long long per = static_cast<long long>(n) * d4;
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < per;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int pos = static_cast<int>(i / d4), c = static_cast<int>(i - static_cast<long long>(pos) * d4);
     float4 v = __ldg(x + b * per + i);
-    if (pos < L) {
+    if (pos < Lb) {
       const float4 a = dropped ? __ldg(null4 + c) : __ldg(cproj + (static_cast<long long>(b) * L + pos) * d4 + c);
       v.x += a.x; v.y += a.y; v.z += a.z; v.w += a.w;
     }
@@ -267,15 +270,52 @@ __global__ void __launch_bounds__(256) select_rows_kernel(const uint8_t* __restr
   }
 }
 
+// lens (optional): mean over rows [0, lens[b]) (clamped to [1, n]), summed in the same order as over n rows
 __global__ void __launch_bounds__(256) mean_rows_kernel(const float* __restrict__ x, int n, int dim,
-                                                        float* __restrict__ out) {
+                                                        const int* __restrict__ lens, float* __restrict__ out) {
   const int b = blockIdx.y;
   const int d = blockIdx.x * blockDim.x + threadIdx.x;
   if (d >= dim) return;
+  const int nb = lens != nullptr ? min(max(__ldg(lens + b), 1), n) : n;
   const float* p = x + static_cast<long long>(b) * n * dim + d;
   float s = 0.f;
-  for (int i = 0; i < n; ++i) s += p[static_cast<long long>(i) * dim];
-  out[static_cast<long long>(b) * dim + d] = s / static_cast<float>(n);
+  for (int i = 0; i < nb; ++i) s += p[static_cast<long long>(i) * dim];
+  out[static_cast<long long>(b) * dim + d] = s / static_cast<float>(nb);
+}
+
+// x[b, r, 0:cols] = 0 for r in [lens[b], rows) (lens clamped to [0, rows]); T = float or __nv_bfloat16
+template <typename T>
+__global__ void __launch_bounds__(256) mask_rows_kernel(T* __restrict__ x, long long rs, long long bs, int rows, int cols,
+                                                        const int* __restrict__ lens) {
+  const int b = blockIdx.y;
+  const int len = min(max(__ldg(lens + b), 0), rows);
+  const long long total = static_cast<long long>(rows - len) * cols;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long r = len + i / cols, c = i % cols;
+    x[b * bs + r * rs + c] = T(0.0f);
+  }
+}
+
+// out[b, r, :] = a[b, r, :] for r < La, bsrc[b, r - La, :] for La <= r < La + Lb, else 0 (bf16, 4 columns per thread);
+// La = a_lens[b] clamped to [0, a_rows], Lb likewise
+__global__ void __launch_bounds__(256) pack_rows_kernel(const uint2* __restrict__ a, long long a_rs, long long a_bs,
+                                                        int a_rows, const int* __restrict__ a_lens,
+                                                        const uint2* __restrict__ bsrc, long long b_rs, long long b_bs,
+                                                        int b_rows, const int* __restrict__ b_lens, int c4,
+                                                        uint2* __restrict__ out, long long o_rs, long long o_bs,
+                                                        int out_rows) {
+  const int b = blockIdx.y;
+  const int La = min(max(__ldg(a_lens + b), 0), a_rows), Lb = min(max(__ldg(b_lens + b), 0), b_rows);
+  const long long total = static_cast<long long>(out_rows) * c4;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int r = static_cast<int>(i / c4), c = static_cast<int>(i % c4);
+    uint2 v = make_uint2(0u, 0u);
+    if (r < La) v = __ldg(a + b * a_bs + r * a_rs + c);
+    else if (r < La + Lb) v = __ldg(bsrc + b * b_bs + static_cast<long long>(r - La) * b_rs + c);
+    out[b * o_bs + r * o_rs + c] = v;
+  }
 }
 
 // (B, C, L) f32 -> (B, L, C) bf16 through a 32x32 shared tile (coalesced on both sides)
@@ -467,23 +507,28 @@ __device__ __forceinline__ float block_sum_256(float v, float* red) {
   return t;
 }
 
+// RAGGED: sample b has lens[b] rows (clamped to [1, rows]): the statistics walk those rows exactly as the plain kernel
+// walks a tensor of that many rows, and rows at or past the length are written as zeros (the residual is not read)
+template <bool RAGGED>
 __global__ void __launch_bounds__(256) groupnorm_silu_kernel(const float* __restrict__ x, int rows, int channels,
                                                              int cpg, const float* __restrict__ weight,
                                                              const float* __restrict__ bias, float eps,
                                                              const float* __restrict__ resid,
                                                              float* __restrict__ out_f32,
-                                                             __nv_bfloat16* __restrict__ out_bf16) {
+                                                             __nv_bfloat16* __restrict__ out_bf16,
+                                                             const int* __restrict__ lens) {
   __shared__ float red[8];
   const int g = blockIdx.x, b = blockIdx.y;
   const int v4 = cpg / 4;                       // float4 per row of this group
   const long long base = (static_cast<long long>(b) * rows) * channels + g * cpg;
-  const int total = rows * v4;
+  const int len = RAGGED ? min(max(__ldg(lens + b), 1), rows) : rows;
+  const int total = len * v4;
   float s = 0.f;
   for (int e = threadIdx.x; e < total; e += 256) {
     const float4 v = __ldg(reinterpret_cast<const float4*>(x + base + static_cast<long long>(e / v4) * channels) + e % v4);
     s += (v.x + v.y) + (v.z + v.w);
   }
-  const float n = static_cast<float>(rows) * cpg;
+  const float n = static_cast<float>(len) * cpg;
   const float mean = block_sum_256(s, red) / n;
   float q = 0.f;
   for (int e = threadIdx.x; e < total; e += 256) {
@@ -512,6 +557,13 @@ __global__ void __launch_bounds__(256) groupnorm_silu_kernel(const float* __rest
       pk.x = pack_bf16x2(y[0], y[1]);
       pk.y = pack_bf16x2(y[2], y[3]);
       *reinterpret_cast<uint2*>(out_bf16 + off) = pk;
+    }
+  }
+  if constexpr (RAGGED) {   // rows [len, rows): exact zeros
+    for (int e = total + threadIdx.x; e < rows * v4; e += 256) {
+      const long long off = base + static_cast<long long>(e / v4) * channels + (e % v4) * 4;
+      if (out_f32 != nullptr) *reinterpret_cast<float4*>(out_f32 + off) = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (out_bf16 != nullptr) *reinterpret_cast<uint2*>(out_bf16 + off) = make_uint2(0u, 0u);
     }
   }
 }
@@ -588,9 +640,9 @@ extern "C" {
 
 int64_t ns2_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 
-int ns2_groupnorm_silu(const float* x, int32_t batch, int32_t rows, int32_t channels, int32_t groups,
-                       const float* weight, const float* bias, float eps, const float* resid, float* out_f32,
-                       void* out_bf16, ns2_stream_t stream) {
+static int groupnorm_silu_launch(const float* x, int32_t batch, int32_t rows, int32_t channels, int32_t groups,
+                                 const float* weight, const float* bias, float eps, const float* resid, float* out_f32,
+                                 void* out_bf16, const int32_t* lens, cudaStream_t stream) {
   NS2_REQUIRE(batch >= 0 && rows >= 0 && channels > 0 && groups > 0 && channels % groups == 0,
               "groupnorm_silu: bad sizes");
   NS2_REQUIRE((channels / groups) % 4 == 0, "groupnorm_silu: channels per group (%d) must be a multiple of 4",
@@ -602,8 +654,72 @@ int ns2_groupnorm_silu(const float* x, int32_t batch, int32_t rows, int32_t chan
                 reinterpret_cast<uintptr_t>(resid) | reinterpret_cast<uintptr_t>(out_f32)) & 15) == 0 &&
                   (reinterpret_cast<uintptr_t>(out_bf16) & 7) == 0,
               "groupnorm_silu: pointers must be 16-byte aligned");
-  groupnorm_silu_kernel<<<dim3(groups, batch), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      x, rows, channels, channels / groups, weight, bias, eps, resid, out_f32, static_cast<__nv_bfloat16*>(out_bf16));
+  const dim3 grid(groups, batch);
+  if (lens != nullptr)
+    groupnorm_silu_kernel<true><<<grid, 256, 0, stream>>>(x, rows, channels, channels / groups, weight, bias, eps, resid,
+                                                          out_f32, static_cast<__nv_bfloat16*>(out_bf16), lens);
+  else
+    groupnorm_silu_kernel<false><<<grid, 256, 0, stream>>>(x, rows, channels, channels / groups, weight, bias, eps,
+                                                           resid, out_f32, static_cast<__nv_bfloat16*>(out_bf16),
+                                                           nullptr);
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  NS2_CUDA_CHECK(cudaGetLastError());
+  return kOk;
+}
+
+int ns2_groupnorm_silu(const float* x, int32_t batch, int32_t rows, int32_t channels, int32_t groups,
+                       const float* weight, const float* bias, float eps, const float* resid, float* out_f32,
+                       void* out_bf16, ns2_stream_t stream) {
+  return groupnorm_silu_launch(x, batch, rows, channels, groups, weight, bias, eps, resid, out_f32, out_bf16, nullptr,
+                               static_cast<cudaStream_t>(stream));
+}
+
+int ns2_groupnorm_silu_ragged(const float* x, int32_t batch, int32_t rows, int32_t channels, int32_t groups,
+                              const float* weight, const float* bias, float eps, const float* resid, float* out_f32,
+                              void* out_bf16, const int32_t* lens, ns2_stream_t stream) {
+  NS2_REQUIRE(lens != nullptr, "groupnorm_silu_ragged: NULL lens");
+  return groupnorm_silu_launch(x, batch, rows, channels, groups, weight, bias, eps, resid, out_f32, out_bf16, lens,
+                               static_cast<cudaStream_t>(stream));
+}
+
+int ns2_mask_rows(void* x, int32_t f32, int64_t row_stride, int64_t batch_stride, int32_t batch, int32_t rows,
+                  int32_t cols, const int32_t* lens, ns2_stream_t stream) {
+  NS2_REQUIRE(batch >= 0 && rows >= 0 && cols >= 0 && row_stride >= cols && batch_stride >= 0, "mask_rows: bad sizes");
+  NS2_REQUIRE(batch <= 65535, "mask_rows: batch %d > 65535", batch);
+  if (batch == 0 || rows == 0 || cols == 0) return kOk;
+  NS2_REQUIRE(x && lens, "mask_rows: null pointer");
+  const dim3 grid(grid_for((static_cast<long long>(rows) * cols + 3) / 4) / (batch > 8 ? 4 : 1) + 1, batch);
+  if (f32)
+    mask_rows_kernel<float><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<float*>(x), row_stride, batch_stride, rows, cols, lens);
+  else
+    mask_rows_kernel<__nv_bfloat16><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<__nv_bfloat16*>(x), row_stride, batch_stride, rows, cols, lens);
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  NS2_CUDA_CHECK(cudaGetLastError());
+  return kOk;
+}
+
+int ns2_pack_rows_ragged(const void* a, int64_t a_row_stride, int64_t a_batch_stride, int32_t a_rows,
+                         const int32_t* a_lens, const void* b, int64_t b_row_stride, int64_t b_batch_stride,
+                         int32_t b_rows, const int32_t* b_lens, int32_t batch, int32_t cols, void* out,
+                         int64_t out_row_stride, int64_t out_batch_stride, int32_t out_rows, ns2_stream_t stream) {
+  NS2_REQUIRE(batch >= 0 && a_rows >= 0 && b_rows >= 0 && cols > 0 && out_rows >= 0, "pack_rows_ragged: bad sizes");
+  NS2_REQUIRE(out_rows >= a_rows + b_rows, "pack_rows_ragged: out_rows %d < %d + %d", out_rows, a_rows, b_rows);
+  NS2_REQUIRE(batch <= 65535, "pack_rows_ragged: batch %d > 65535", batch);
+  if (batch == 0 || out_rows == 0) return kOk;
+  NS2_REQUIRE(a && b && a_lens && b_lens && out, "pack_rows_ragged: null pointer");
+  NS2_REQUIRE(cols % 4 == 0 && a_row_stride % 4 == 0 && a_batch_stride % 4 == 0 && b_row_stride % 4 == 0 &&
+                  b_batch_stride % 4 == 0 && out_row_stride % 4 == 0 && out_batch_stride % 4 == 0 &&
+                  ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) |
+                    reinterpret_cast<uintptr_t>(out)) & 7) == 0,
+              "pack_rows_ragged: columns and strides must be multiples of 4, pointers 8-byte aligned");
+  const int c4 = cols / 4;
+  const dim3 grid(grid_for(static_cast<long long>(out_rows) * c4) / (batch > 8 ? 4 : 1) + 1, batch);
+  pack_rows_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint2*>(a), a_row_stride / 4, a_batch_stride / 4, a_rows, a_lens, static_cast<const uint2*>(b),
+      b_row_stride / 4, b_batch_stride / 4, b_rows, b_lens, c4, static_cast<uint2*>(out), out_row_stride / 4,
+      out_batch_stride / 4, out_rows);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   NS2_CUDA_CHECK(cudaGetLastError());
   return kOk;
@@ -717,8 +833,9 @@ int ns2_cast_bf16(const float* x, const float* add, int64_t count, void* out_bf1
   return kOk;
 }
 
-int ns2_cond_inject(const float* x, const float* cproj, const uint8_t* drop_mask, const float* null_cond,
-                    int32_t batch, int32_t n, int32_t cond_len, int32_t dim, void* out_bf16, ns2_stream_t stream) {
+static int cond_inject_launch(const float* x, const float* cproj, const uint8_t* drop_mask, const float* null_cond,
+                              int32_t batch, int32_t n, int32_t cond_len, int32_t dim, const int32_t* cond_lens,
+                              void* out_bf16, cudaStream_t stream) {
   NS2_REQUIRE(x && cproj && out_bf16 && batch > 0 && n > 0 && cond_len > 0 && dim > 0 && dim % 4 == 0,
               "cond_inject: bad arguments");
   NS2_REQUIRE(drop_mask == nullptr || null_cond != nullptr, "cond_inject: a drop mask needs null_cond");
@@ -726,12 +843,26 @@ int ns2_cond_inject(const float* x, const float* cproj, const uint8_t* drop_mask
                 reinterpret_cast<uintptr_t>(null_cond)) & 15) == 0, "cond_inject: pointers must be 16-byte aligned");
   const long long per4 = static_cast<long long>(n) * (dim / 4);
   dim3 grid(static_cast<unsigned>((per4 + 255) / 256 > 512 ? 512 : (per4 + 255) / 256), batch);
-  cond_inject_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+  cond_inject_kernel<<<grid, 256, 0, stream>>>(
       reinterpret_cast<const float4*>(x), reinterpret_cast<const float4*>(cproj), drop_mask,
-      reinterpret_cast<const float4*>(null_cond), n, cond_len, dim / 4, reinterpret_cast<uint2*>(out_bf16));
+      reinterpret_cast<const float4*>(null_cond), n, cond_len, cond_lens, dim / 4, reinterpret_cast<uint2*>(out_bf16));
   g_launches.fetch_add(1, std::memory_order_relaxed);
   NS2_CUDA_CHECK(cudaGetLastError());
   return kOk;
+}
+
+int ns2_cond_inject(const float* x, const float* cproj, const uint8_t* drop_mask, const float* null_cond,
+                    int32_t batch, int32_t n, int32_t cond_len, int32_t dim, void* out_bf16, ns2_stream_t stream) {
+  return cond_inject_launch(x, cproj, drop_mask, null_cond, batch, n, cond_len, dim, nullptr, out_bf16,
+                            static_cast<cudaStream_t>(stream));
+}
+
+int ns2_cond_inject_ragged(const float* x, const float* cproj, const uint8_t* drop_mask, const float* null_cond,
+                           int32_t batch, int32_t n, int32_t cond_len, int32_t dim, const int32_t* cond_lens,
+                           void* out_bf16, ns2_stream_t stream) {
+  NS2_REQUIRE(cond_lens != nullptr, "cond_inject_ragged: NULL cond_lens");
+  return cond_inject_launch(x, cproj, drop_mask, null_cond, batch, n, cond_len, dim, cond_lens, out_bf16,
+                            static_cast<cudaStream_t>(stream));
 }
 
 int ns2_select_rows(const uint8_t* drop_mask, const float* null_row, const float* src, int64_t src_row_stride,
@@ -746,14 +877,25 @@ int ns2_select_rows(const uint8_t* drop_mask, const float* null_row, const float
   return kOk;
 }
 
-int ns2_mean_rows(const float* x, int32_t batch, int32_t n, int32_t dim, float* out,
-                  ns2_stream_t stream) {
+static int mean_rows_launch(const float* x, int32_t batch, int32_t n, int32_t dim, const int32_t* lens, float* out,
+                            cudaStream_t stream) {
   NS2_REQUIRE(x && out && batch > 0 && n > 0 && dim > 0, "mean_rows: bad arguments");
   dim3 grid((dim + 255) / 256, batch);
-  mean_rows_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, n, dim, out);
+  mean_rows_kernel<<<grid, 256, 0, stream>>>(x, n, dim, lens, out);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   NS2_CUDA_CHECK(cudaGetLastError());
   return kOk;
+}
+
+int ns2_mean_rows(const float* x, int32_t batch, int32_t n, int32_t dim, float* out,
+                  ns2_stream_t stream) {
+  return mean_rows_launch(x, batch, n, dim, nullptr, out, static_cast<cudaStream_t>(stream));
+}
+
+int ns2_mean_rows_ragged(const float* x, int32_t batch, int32_t n, int32_t dim, const int32_t* lens, float* out,
+                         ns2_stream_t stream) {
+  NS2_REQUIRE(lens != nullptr, "mean_rows_ragged: NULL lens");
+  return mean_rows_launch(x, batch, n, dim, lens, out, static_cast<cudaStream_t>(stream));
 }
 
 int ns2_transpose_cast(const float* x, int32_t batch, int32_t channels, int32_t length,

@@ -178,9 +178,11 @@ class NaturalSpeech2(nn.Module):
         return entry
 
     @torch.no_grad()
-    def ddim_sample(self, shape, prompt=None, time_difference=None, cond_scale=1., cond=None, *, noise=None):
+    def ddim_sample(self, shape, prompt=None, time_difference=None, cond_scale=1., cond=None, *, noise=None,
+                    prompt_lens=None, cond_lens=None):
         """ns2.py:1379-1431.  `noise` (optional) fixes the initial latent instead of drawing it.
-        (`time_difference` only shifts a value the reference never reads again, ns2.py:1404-1406.)"""
+        (`time_difference` only shifts a value the reference never reads again, ns2.py:1404-1406.)
+        prompt_lens / cond_lens: per-sample lengths of the prompt and the condition (Model.precompute_conditioning)."""
         batch, device = shape[0], self.device
         # a dense, row-major copy: the eager loop updates it in place with ops.ddim_step, which reads flat arrays
         audio = torch.randn(shape, device=device) if noise is None else \
@@ -189,7 +191,8 @@ class NaturalSpeech2(nn.Module):
         if self.conditional:
             assert _exists(prompt) and _exists(cond)
             # timestep-invariant work (perceiver, prompt FiLM vector, aligned-condition projection) once
-            conditioning = self.model.precompute_conditioning(prompt, cond, shape[1])
+            conditioning = self.model.precompute_conditioning(prompt, cond, shape[1], prompt_lens=prompt_lens,
+                                                              cond_lens=cond_lens)
         times_tab, coef_tab = self._schedule_tables(batch, device)
         if self.cuda_graphs and audio.is_cuda and self.model._prof is None:
             entry = self._sampler_entry(shape, conditioning, cond_scale, device)
@@ -222,21 +225,42 @@ class NaturalSpeech2(nn.Module):
 
     @torch.no_grad()
     def sample(self, *, length, prompt=None, batch_size=1, cond_scale=1., text=None, text_lens=None,
-               prompt_enc=None, cond=None, noise=None):
-        """ns2.py:1457-1501.  Conditional models need (`prompt_enc`, `cond`) or a `conditioner`."""
+               prompt_enc=None, cond=None, noise=None, prompt_lens=None, phoneme_lens=None, cond_lens=None):
+        """ns2.py:1457-1501.  Conditional models need (`prompt_enc`, `cond`) or a `conditioner`.
+        `text_lens` is accepted and ignored, as in the reference.  A batch of prompts and texts of different lengths,
+        padded at their ends, is sampled as if each sample ran alone with `prompt_lens` (prompt latent frames) and
+        `phoneme_lens` (phonemes), given to the conditioner, whose condition lengths then follow; with precomputed
+        `prompt_enc=` / `cond=` pass `prompt_lens` and `cond_lens` (condition frames) instead.  With lengths the
+        prompt must be encoded latents (B, Np, dim): a raw-audio prompt would be curtailed by the batch's length."""
         if self.use_ddim is False:
             raise NotImplementedError("ddpm_sample is dead code in the reference (NameError: expm1, SURVEY T8)")
+        ragged = prompt_lens is not None or phoneme_lens is not None or cond_lens is not None
+        if ragged and not self.conditional:
+            raise ValueError("prompt_lens / phoneme_lens / cond_lens apply to conditional models")
         if self.conditional:
             if not (_exists(prompt_enc) and _exists(cond)):
                 if not _exists(self.conditioner):
                     raise NotImplementedError(
                         "conditional sampling needs prompt_enc= and cond= (outputs of the reference's "
                         "SpeechPromptEncoder / duration-pitch expansion) or a `conditioner` callable")
-                prompt_enc, cond = self.conditioner(prompt=self.process_prompt(prompt), text=text,
-                                                    text_lens=text_lens, mode="sample")
+                if not ragged:
+                    prompt_enc, cond = self.conditioner(prompt=self.process_prompt(prompt), text=text,
+                                                        text_lens=text_lens, mode="sample")
+                else:
+                    if cond_lens is not None:
+                        raise ValueError("cond_lens goes with precomputed prompt_enc= / cond=; the conditioner "
+                                         "computes it from phoneme_lens")
+                    if prompt is None or prompt.ndim != 3:
+                        raise ValueError("with prompt_lens / phoneme_lens the prompt must be encoded latents (B, Np, dim): "
+                                         "a raw-audio prompt is curtailed from the left by the batch's length")
+                    prompt_enc, cond, cond_lens = self.conditioner(
+                        prompt=prompt, text=text, text_lens=text_lens, mode="sample", prompt_lens=prompt_lens,
+                        phoneme_lens=phoneme_lens)
+            elif phoneme_lens is not None:
+                raise ValueError("phoneme_lens goes to the conditioner; with prompt_enc= / cond= pass cond_lens")
             batch_size = prompt_enc.shape[0]
         audio = self.ddim_sample((batch_size, length, self.dim), prompt=prompt_enc, cond=cond,
-                                 cond_scale=cond_scale, noise=noise)
+                                 cond_scale=cond_scale, noise=noise, prompt_lens=prompt_lens, cond_lens=cond_lens)
         if _exists(self.codec):
             audio = self.codec.decode(audio)
             if audio.ndim == 3 and audio.shape[1] == 1:

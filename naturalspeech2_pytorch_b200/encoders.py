@@ -50,7 +50,11 @@ nn.Dropout has the default p = 0 (ns2.py:352, 374) and draws nothing.  With `tra
 per call in train() mode, none in eval(), without train_dropout or with p = 0.  The cross attention of layer l of trunk
 t (0 duration, 1 pitch; forward order) is site t depth + l.  The record keeps the seed, no mask.
 Attention masks are not supported (`mask=None` is what NaturalSpeech2.forward / .sample pass, ns2.py:1475-1476,
-1538-1539).  Numerics follow the denoiser: bf16 tensor-core operands, fp32 accumulation, fp32 residual stream and norm
+1538-1539).  A batch of sequences of different lengths, each padded at its end, is sampled with per-sample lengths
+instead (`lengths=` / `prompt_lens=`, inference only): the "same" convolutions read zeros past each sample's end, the
+attentions take only a sample's own keys (ops.attention kv_lens), the predictor's GroupNorms take only its own rows, and
+padded output rows are exact zeros, so every sample's output is bit-identical to running it alone, unpadded.  What the
+padded input rows hold is never read into a valid row.  Numerics follow the denoiser: bf16 tensor-core operands, fp32 accumulation, fp32 residual stream and norm
 statistics.
 """
 from __future__ import annotations
@@ -154,10 +158,12 @@ class _EncoderBase(_PackedCache):
             P["final_g"] = tr.norm.gamma.detach().float().contiguous()
 
     def _transformer(self, x: torch.Tensor, tr: _PlainTransformerParams, P, heads: int,
-                     saved: Optional[dict] = None, seed: Optional[int] = None) -> torch.Tensor:
+                     saved: Optional[dict] = None, seed: Optional[int] = None,
+                     kv_lens: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Transformer.forward (ns2.py:1110-1115) on the fp32 residual stream x (B, N, D), updated in place.  With `saved`
         every layer's activations go to saved["layers"] in fresh tensors (`_transformer_backward` reads them).
-        seed: the call's dropout seed (None = no attention dropout)."""
+        seed: the call's dropout seed (None = no attention dropout).  kv_lens: per-sample lengths (keys past them are
+        not attended to; the rows past them hold finite values the caller ignores)."""
         keep = saved is not None
         if keep and "final_g" in P:
             raise NotImplementedError("training a Transformer with final_norm=True is not supported")
@@ -178,7 +184,7 @@ class _EncoderBase(_PackedCache):
             ops.rmsnorm_film(x, L["h1"], gamma=P[f"l{l}_g1"])
             qkv = ops.gemm(L["h1"], P[f"l{l}_qkv"], L["qkv"], n=3 * inner, epilogue=ops.EPI_BF16)
             ops.attention(qkv[:, :, :inner], qkv[:, :, inner:2 * inner], qkv[:, :, 2 * inner:], L["ao"], heads=heads,
-                          lse=L["lse"], dropout=self._attn_dropout(seed, l))
+                          lse=L["lse"], dropout=self._attn_dropout(seed, l), kv_lens=kv_lens)
             ops.gemm(L["ao"], P[f"l{l}_o"], x, n=D, epilogue=ops.EPI_F32, resid=x)
             if keep:
                 L["x_mid"] = x.clone()
@@ -229,6 +235,15 @@ class _EncoderBase(_PackedCache):
         ops.silu_bwd(pre, d_out)                                                                  # pre <- d pre
         return conv_backward(pre, x_in, grads, name, w_t, k, first_shift, dtype=dtype)
 
+    def _ragged_lengths(self, lengths, batch: int, n: int, device, name: str) -> Optional[torch.Tensor]:
+        """Validated int32 device lengths of a sampling call (None stays None).  Lengths are for inference only."""
+        if lengths is None:
+            return None
+        if _records_graph(self) or (self.training and self.train_dropout):
+            raise NotImplementedError(f"{type(self).__name__}: {name} are supported for sampling only (no autograd, no "
+                                      "dropout)")
+        return ops.lengths(lengths, batch, n, device=device, name=name)
+
     def _start_backward(self, d_out: torch.Tensor):
         dxr = d_out.float().contiguous().clone()        # fp32 residual-stream gradient, updated in place
         return dxr, ops.cast_bf16(dxr, torch.empty(dxr.shape, device=dxr.device, dtype=torch.bfloat16))
@@ -242,7 +257,8 @@ def _check_transformer_dims(dim: int, dim_head: int):
 
 
 class SpeechPromptEncoder(_EncoderBase):
-    """ns2.py:289-341.  forward(x: (B, Np, dim_codebook)) -> (B, Np, dims[-1]) fp32."""
+    """ns2.py:289-341.  forward(x: (B, Np, dim_codebook)) -> (B, Np, dims[-1]) fp32.
+    forward(x, lengths=(B,)): sample b is x[b, :lengths[b]] (see the module docstring); rows past it come out as zeros."""
 
     def __init__(self, dim_codebook, dims: Tuple[int, ...] = (256, 2048, 2048, 2048, 2048, 512, 512, 512), *,
                  depth=6, heads=8, dim_head=64, dropout=0.2, kernel_size=9, padding=4, use_flash_attn=True):
@@ -281,21 +297,25 @@ class SpeechPromptEncoder(_EncoderBase):
         self._pack_transposed_transformer(P, T, len(self.transformer.layers))
         return T
 
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
+    def forward(self, x: torch.Tensor, *, lengths=None) -> torch.Tensor:
         assert x.shape[-1] == self.dim
         if not x.is_cuda:
             raise ValueError("SpeechPromptEncoder: input must be a CUDA tensor (the ns2_b200 ops have no CPU path)")
+        lens = self._ragged_lengths(lengths, x.shape[0], x.shape[1], x.device, "lengths")
         if _records_graph(self):
             return _EncoderFunction.apply(self, self.grad_reducer, x, *self.parameters())
         with torch.no_grad():
-            return self._forward(x)
+            return self._forward(x, lens=lens)
 
-    def _forward(self, x: torch.Tensor, saved: Optional[dict] = None) -> torch.Tensor:
-        """The forward; with `saved` it also records the activations `_train_backward` reads (same kernels, same output)."""
+    def _forward(self, x: torch.Tensor, saved: Optional[dict] = None, lens: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The forward; with `saved` it also records the activations `_train_backward` reads (same kernels, same output).
+        lens: per-sample lengths; every conv input is zero past them, as the "same" padding of a sample run alone."""
         P = self.packed()
         B, N, _ = x.shape
         dev, bf = x.device, torch.bfloat16
         h = ops.cast_bf16(x.float().contiguous(), torch.empty(B, N, self.dim, device=dev, dtype=bf))
+        if lens is not None:
+            ops.mask_rows(h, lens)
         convs = self._convs()
         conv_in = []
         for i, c in enumerate(convs):
@@ -303,13 +323,16 @@ class SpeechPromptEncoder(_EncoderBase):
             out = torch.empty(B, N, c.out_channels, device=dev, dtype=torch.float32 if last else bf)
             ops.gemm(h, P[f"c{i}_w"], out, n=c.out_channels, epilogue=ops.EPI_F32 if last else ops.EPI_BF16,
                      segs=_conv_segs(c.in_channels, self.kernel_size, self.padding), bias=P[f"c{i}_b"], flags=_SILU)
+            if lens is not None:
+                ops.mask_rows(out, lens)
             if saved is not None:
                 conv_in.append(h)
             h = out
         seed = self._dropout_seed()
         if saved is not None:
             saved.update(conv_in=conv_in, dropout_seed=seed)
-        return self._transformer(h, self.transformer, P, self.heads, saved, seed)
+        out = self._transformer(h, self.transformer, P, self.heads, saved, seed, kv_lens=lens)
+        return out if lens is None else ops.mask_rows(out, lens)
 
     def _train_backward(self, S, d_out: torch.Tensor) -> Dict[str, torch.Tensor]:
         P, T = self.packed(), self.packed_transposed()
@@ -327,7 +350,8 @@ class SpeechPromptEncoder(_EncoderBase):
 
 class PhonemeEncoder(_EncoderBase):
     """ns2.py:228-287.  forward(x: (B, T) int64 phoneme ids, negative = padding) -> (B, T, dim_hidden) fp32.
-    A tokenizer (List[str] input) is used exactly like the reference when one is given."""
+    A tokenizer (List[str] input) is used exactly like the reference when one is given.
+    forward(x, lengths=(B,)): sample b is x[b, :lengths[b]] (see the module docstring); rows past it come out as zeros."""
 
     def __init__(self, *, tokenizer=None, num_tokens=None, dim=512, dim_hidden=512, kernel_size=9, depth=6,
                  dim_head=64, heads=8, conv_dropout=0.2, attn_dropout=0., use_flash=False):
@@ -361,7 +385,7 @@ class PhonemeEncoder(_EncoderBase):
         self._pack_transposed_transformer(P, T, len(self.transformer.layers))
         return T
 
-    def forward(self, x, mask=None) -> torch.Tensor:
+    def forward(self, x, mask=None, *, lengths=None) -> torch.Tensor:
         if mask is not None:
             raise NotImplementedError("PhonemeEncoder: attention masks are not supported by the sm_90a attention kernel")
         if isinstance(x, (list, tuple)):
@@ -369,12 +393,13 @@ class PhonemeEncoder(_EncoderBase):
             x = self.tokenizer.texts_to_tensor_ids(x).to(self.token_emb.weight.device)
         if not x.is_cuda:
             raise ValueError("PhonemeEncoder: input must be a CUDA tensor (the ns2_b200 ops have no CPU path)")
+        lens = self._ragged_lengths(lengths, x.shape[0], x.shape[1], x.device, "lengths")
         if _records_graph(self):
             return _EncoderFunction.apply(self, self.grad_reducer, x, *self.parameters())
         with torch.no_grad():
-            return self._forward(x)
+            return self._forward(x, lens=lens)
 
-    def _forward(self, x: torch.Tensor, saved: Optional[dict] = None) -> torch.Tensor:
+    def _forward(self, x: torch.Tensor, saved: Optional[dict] = None, lens: Optional[torch.Tensor] = None) -> torch.Tensor:
         """The forward; with `saved` it also records the activations `_train_backward` reads (same kernels, same output)."""
         P = self.packed()
         B, T = x.shape
@@ -390,7 +415,9 @@ class PhonemeEncoder(_EncoderBase):
             ops.dropout_(h, dropout=(seed, 0, self.conv_dropout))                   # nn.Dropout(conv_dropout), ns2.py:258
         if saved is not None:
             saved.update(ids=ids, emb=e, dropout_seed=seed)
-        return self._transformer(h, self.transformer, P, self.heads, saved, seed)
+        # the conv is causal: a valid row never reads a padded one, only the attention needs the lengths
+        out = self._transformer(h, self.transformer, P, self.heads, saved, seed, kv_lens=lens)
+        return out if lens is None else ops.mask_rows(out, lens)
 
     def _train_backward(self, S, d_out: torch.Tensor) -> Dict[str, torch.Tensor]:
         P, T = self.packed(), self.packed_transposed()
@@ -448,7 +475,9 @@ class _TrunkParams(nn.Module):
 
 class DurationPitchPredictor(_EncoderBase):
     """ns2.py:468-527.  forward(x: (B, T, dim_hidden) phoneme encodings [or (B, T) ids with a token table],
-    encoded_prompts: (B, Np, dim_encoded_prompts)) -> (duration_pred (B, T), pitch_pred (B, T)), both fp32 >= 0."""
+    encoded_prompts: (B, Np, dim_encoded_prompts)) -> (duration_pred (B, T), pitch_pred (B, T)), both fp32 >= 0.
+    forward(..., lengths=(B,), prompt_lens=(B,)): sample b is x[b, :lengths[b]] with the prompt encoded_prompts[b,
+    :prompt_lens[b]] (see the module docstring); its predictions past lengths[b] are exact zeros."""
 
     def __init__(self, *, dim, num_phoneme_tokens=None, tokenizer=None, dim_encoded_prompts=None,
                  num_convolutions_per_block=3, use_resnet_block=True, num_convs_per_resnet_block=2, depth=10,
@@ -526,9 +555,12 @@ class DurationPitchPredictor(_EncoderBase):
         return None if seed is None else (seed, t * self.depth + l, self.attn_dropout)
 
     def _trunk(self, name: str, trunk: _TrunkParams, P, x0: torch.Tensor, prompts_bf: torch.Tensor,
-               saved: Optional[dict] = None, seed: Optional[int] = None) -> torch.Tensor:
+               saved: Optional[dict] = None, seed: Optional[int] = None, ragged: Optional[tuple] = None) -> torch.Tensor:
         """DurationPitchPredictorTrunk.forward (ns2.py:457-466).  With `saved` the activations `_trunk_backward` reads
-        go to saved[name] in fresh tensors (same kernels, same output).  seed: the call's dropout seed (None = none)."""
+        go to saved[name] in fresh tensors (same kernels, same output).  seed: the call's dropout seed (None = none).
+        ragged: (lengths, prompt_lens, lengths + prompt_lens) of a batch of different lengths; x0 must be zero past
+        the lengths.  Then the stream's bf16 copy that the "same" convs read is kept zero there (the GroupNorms write
+        zeros), the keys are the packed prefix [norm(x)[:T_b] ; prompts[:Np_b]], and the predictions past T_b are 0."""
         keep = saved is not None
         B, T, D = x0.shape
         Np = prompts_bf.shape[1]
@@ -537,6 +569,7 @@ class DurationPitchPredictor(_EncoderBase):
         groups, eps = self._norm_config(trunk)
         segs = _conv_segs(D, self.kernel_size, self.kernel_size // 2)
         e = lambda *s, dt=bf: torch.empty(*s, device=dev, dtype=dt)  # noqa: E731
+        lens, plens, kv_lens = ragged if ragged is not None else (None, None, None)
         x = x0.clone()                                               # fp32 stream of this trunk
         x_bf = ops.cast_bf16(x, e(B, T, D))
         c = e(B, T, D, dt=torch.float32)
@@ -545,7 +578,8 @@ class DurationPitchPredictor(_EncoderBase):
         for l, (convs, _, _) in enumerate(trunk.layers):
             if keep or l == 0:   # inference reuses the first layer's buffers
                 ctx = e(B, T + Np, D)                                # [norm(x) ; encoded prompts] (ns2.py:1060-1061)
-                ctx[:, T:].copy_(prompts_bf)
+                if ragged is None:
+                    ctx[:, T:].copy_(prompts_bf)
                 L = {"nx": e(B, T, D), "q": e(B, T, inner), "kv": e(B, T + Np, 2 * inner), "o": e(B, T, inner),
                      "ctx": ctx, "lse": e(B, H, T, dt=torch.float32) if keep else None, "blocks": []}
             for r, rb in enumerate(convs):
@@ -557,25 +591,32 @@ class DurationPitchPredictor(_EncoderBase):
                     if keep:
                         L["blocks"].append((src.clone(), c.clone()))   # conv input (bf16), GroupNorm input (fp32)
                     if ci < nb - 1:
-                        ops.groupnorm_silu(c, P[k + "_gw"], P[k + "_gb"], groups, eps=eps, out_bf16=h_bf)
+                        ops.groupnorm_silu(c, P[k + "_gw"], P[k + "_gb"], groups, eps=eps, out_bf16=h_bf, lens=lens)
                         src = h_bf
                     else:   # out = blocks(x) + res_conv(x), res_conv = Identity (ns2.py:399-401)
                         ops.groupnorm_silu(c, P[k + "_gw"], P[k + "_gb"], groups, eps=eps, resid=x, out_f32=x,
-                                           out_bf16=x_bf)
+                                           out_bf16=x_bf, lens=lens)
             if keep:
                 L["x_mid"] = x.clone()
                 layers.append(L)
             nx, q, kv, o, ctx = L["nx"], L["q"], L["kv"], L["o"], L["ctx"]
             ops.rmsnorm_film(x, nx, gamma=P[f"{name}{l}_g"])
-            ctx[:, :T].copy_(nx)
+            if ragged is None:
+                ctx[:, :T].copy_(nx)
+            else:
+                ops.pack_rows(nx, lens, prompts_bf, plens, ctx)
             ops.gemm(nx, P[f"{name}{l}_q"], q, n=inner, epilogue=ops.EPI_BF16)
             ops.gemm(ctx, P[f"{name}{l}_kv"], kv, n=2 * inner, epilogue=ops.EPI_BF16)
             ops.attention(q, kv[:, :, :inner], kv[:, :, inner:], o, heads=H, lse=L["lse"],
-                          dropout=self._cross_attn_dropout(seed, name, l))
+                          dropout=self._cross_attn_dropout(seed, name, l), kv_lens=kv_lens)
             ops.gemm(o, P[f"{name}{l}_o"], x, n=D, epilogue=ops.EPI_F32, resid=x)   # attn(norm(x), prompts) + x
             ops.cast_bf16(x, x_bf)
+            if ragged is not None:   # the next ResnetBlock's first conv reads it
+                ops.mask_rows(x_bf, lens)
         pred = e(B, T, dt=torch.float32)
         ops.rowdot(x, P[f"{name}_pw"], P[f"{name}_pb"], pred, relu=True)            # Linear(dim, 1) + ReLU
+        if ragged is not None:
+            ops.mask_rows(pred.view(B, T, 1), lens)
         if keep:
             saved[name] = {"layers": layers, "x": x, "pred": pred.clone()}
         return pred
@@ -635,7 +676,7 @@ class DurationPitchPredictor(_EncoderBase):
                         ops.gemm(d_c, T[key + "_w"], dxr, n=D, epilogue=ops.EPI_F32, segs=dgrad_segs, resid=dxr)
         return dxr
 
-    def forward(self, x, encoded_prompts: torch.Tensor, prompt_mask=None):
+    def forward(self, x, encoded_prompts: torch.Tensor, prompt_mask=None, *, lengths=None, prompt_lens=None):
         if prompt_mask is not None:
             raise NotImplementedError("DurationPitchPredictor: prompt masks are not supported by the sm_90a attention kernel")
         if isinstance(x, (list, tuple)):
@@ -643,26 +684,40 @@ class DurationPitchPredictor(_EncoderBase):
             x = self.tokenizer.texts_to_tensor_ids(x).to(encoded_prompts.device)
         if not (x.is_cuda and encoded_prompts.is_cuda):
             raise ValueError("DurationPitchPredictor: inputs must be CUDA tensors (the ns2_b200 ops have no CPU path)")
+        ragged = None
+        if lengths is not None or prompt_lens is not None:
+            B, T = x.shape[:2]
+            Np = encoded_prompts.shape[1]
+            lens = self._ragged_lengths(lengths if lengths is not None else [T] * B, B, T, x.device, "lengths")
+            plens = self._ragged_lengths(prompt_lens if prompt_lens is not None else [Np] * B, B, Np, x.device,
+                                         "prompt_lens")
+            ragged = (lens, plens, lens + plens)
         if _records_graph(self):
             return _EncoderFunction.apply(self, self.grad_reducer, x, encoded_prompts, *self.parameters())
         with torch.no_grad():
-            return self._forward(x, encoded_prompts)
+            return self._forward(x, encoded_prompts, ragged=ragged)
 
     def _train_forward(self, x: torch.Tensor, encoded_prompts: torch.Tensor):
         saved = {"x_dtype": x.dtype, "prompts_dtype": encoded_prompts.dtype}
         return self._forward(x, encoded_prompts, saved), saved
 
-    def _forward(self, x: torch.Tensor, encoded_prompts: torch.Tensor, saved: Optional[dict] = None):
-        """The forward; with `saved` it also records what `_train_backward` reads (same kernels, same output)."""
+    def _forward(self, x: torch.Tensor, encoded_prompts: torch.Tensor, saved: Optional[dict] = None,
+                 ragged: Optional[tuple] = None):
+        """The forward; with `saved` it also records what `_train_backward` reads (same kernels, same output).
+        ragged: see `_trunk`; the input rows past the lengths are replaced by zeros (a copy, the input is not touched)."""
         P = self.packed()
         dev, bf = x.device, torch.bfloat16
         if "emb" in P:
             B, T = x.shape
             ids = x.long().contiguous()
             e = ops.embedding_bf16(ids, P["emb"], torch.empty(B, T, self.dim_hidden, device=dev, dtype=bf), 0)
+            if ragged is not None:
+                ops.mask_rows(e, ragged[0])
             x = e.float()
             if saved is not None:
                 saved["ids"] = ids
+        elif ragged is not None:
+            x = ops.mask_rows(x.float().clone(memory_format=torch.contiguous_format), ragged[0])
         x = x.float().contiguous()
         B, Np, Dp = encoded_prompts.shape
         assert x.shape[-1] == self.dim_hidden and Dp == self.dim_hidden
@@ -670,8 +725,8 @@ class DurationPitchPredictor(_EncoderBase):
         seed = self._dropout_seed()
         if saved is not None:
             saved["dropout_seed"] = seed
-        duration = self._trunk("d", self.to_duration_pred, P, x, prompts_bf, saved, seed)
-        pitch = self._trunk("p", self.to_pitch_pred, P, x, prompts_bf, saved, seed)
+        duration = self._trunk("d", self.to_duration_pred, P, x, prompts_bf, saved, seed, ragged)
+        pitch = self._trunk("p", self.to_pitch_pred, P, x, prompts_bf, saved, seed, ragged)
         return duration, pitch
 
     def _train_backward(self, S, d_duration: Optional[torch.Tensor], d_pitch: Optional[torch.Tensor]):
@@ -835,18 +890,33 @@ class Conditioner(nn.Module):
             if name in self._modules:   # a Conditioner may be assembled around some of them
                 self._modules[name].grad_reducer = reducer
 
-    def forward(self, prompt=None, text=None, text_lens=None, mode="sample", pitch=None, duration=None, **unused):
+    def forward(self, prompt=None, text=None, text_lens=None, mode="sample", pitch=None, duration=None, *,
+                prompt_lens=None, phoneme_lens=None, **unused):
+        """`text_lens` is accepted and ignored, as in the reference (ns2.py:1462).  mode="sample" with `prompt_lens` /
+        `phoneme_lens` (per-sample lengths of a batch padded at the end) returns (prompt_enc, cond, cond_lens): each
+        sample's outputs are those of running it alone, zero past its lengths; cond_lens (B,) int32 is each sample's
+        total predicted duration in frames (cond is zero past it)."""
+        ragged = prompt_lens is not None or phoneme_lens is not None
         if mode == "train":
+            if ragged:
+                raise NotImplementedError("Conditioner(mode='train') does not take prompt_lens / phoneme_lens")
             return self._forward_train(prompt, text, pitch, duration)
         if mode != "sample":
             raise NotImplementedError(f"Conditioner: unknown mode {mode!r} (sample | train)")
         assert prompt is not None and text is not None
         with torch.no_grad():
-            prompt_enc = self.prompt_enc(prompt)
-            phoneme_enc = self.phoneme_enc(text)
-            duration, pitch = self.duration_pitch(phoneme_enc, prompt_enc)
+            if not ragged:
+                prompt_enc = self.prompt_enc(prompt)
+                phoneme_enc = self.phoneme_enc(text)
+                duration, pitch = self.duration_pitch(phoneme_enc, prompt_enc)
+                cond = expand_encodings(phoneme_enc, duration, pitch, self.pitch_emb.weight)
+                return prompt_enc, cond
+            prompt_enc = self.prompt_enc(prompt, lengths=prompt_lens)
+            phoneme_enc = self.phoneme_enc(text, lengths=phoneme_lens)
+            duration, pitch = self.duration_pitch(phoneme_enc, prompt_enc, lengths=phoneme_lens, prompt_lens=prompt_lens)
             cond = expand_encodings(phoneme_enc, duration, pitch, self.pitch_emb.weight)
-        return prompt_enc, cond
+            cond_lens = duration.int().sum(dim=-1, dtype=torch.int32)   # the frames frames_to_text_index fills
+        return prompt_enc, cond, cond_lens
 
     def _forward_train(self, prompt, text, pitch, duration):
         """ns2.py:1538-1583 with the aligner's hard durations given: prompt_enc = prompt_enc(prompt), cond =

@@ -460,9 +460,11 @@ class Model(_PackedCache):
     # ----------------------------------------------------------------------------------------------
     # conditioning (timestep-invariant; cache across sampling steps via `precompute_conditioning`)
     # ----------------------------------------------------------------------------------------------
-    def _perceiver(self, prompt: torch.Tensor, P: Dict[str, torch.Tensor], saved: Optional[dict] = None) -> torch.Tensor:
+    def _perceiver(self, prompt: torch.Tensor, P: Dict[str, torch.Tensor], saved: Optional[dict] = None,
+                   prompt_lens: Optional[torch.Tensor] = None) -> torch.Tensor:
         """PerceiverResampler.forward (ns2.py:568-579) -> (B, M, D) fp32.  With `saved`, every layer's activations are
-        kept (fresh buffers per layer) for `training._conditioning_backward_tokens`."""
+        kept (fresh buffers per layer) for `training._conditioning_backward_tokens`.  prompt_lens: validated per-sample
+        prompt lengths; the keys [latents ; prompt] of sample b are then its first M + prompt_lens[b]."""
         D, M, inner, H = self.dim, self.num_latents_m, self.inner, self.heads
         pr = self.perceiver_resampler
         B, Np, _ = prompt.shape
@@ -470,10 +472,15 @@ class Model(_PackedCache):
         e = lambda *s, dt=torch.bfloat16: torch.empty(*s, device=dev, dtype=dt)  # noqa: E731
         keep = saved is not None
         p_bf = ops.cast_bf16(prompt.contiguous().float(), e(B, Np, self.dim_prompt))
+        kv_lens = None
+        if prompt_lens is not None:   # padded rows are never attended to, but their keys must be finite
+            ops.mask_rows(p_bf, prompt_lens)
+            kv_lens = prompt_lens + M
         proj = p_bf
         if "pr_proj_w" in P:
             proj = ops.gemm(p_bf, P["pr_proj_w"], e(B, Np, D), n=D, epilogue=ops.EPI_BF16, bias=P["pr_proj_b"])
-        lat = pr.latents.detach().float().unsqueeze(0).expand(B, M, D).contiguous()
+        # a copy: updated in place below, and for B = 1 `.contiguous()` would hand back the parameter's own storage
+        lat = pr.latents.detach().float().unsqueeze(0).expand(B, M, D).clone(memory_format=torch.contiguous_format)
         Dp = _round_up(pr.ff_inner, 128)
         layers = []
         for i in range(len(pr.layers)):
@@ -487,7 +494,8 @@ class Model(_PackedCache):
             L["cat"][:, :M].copy_(L["lat_bf"])  # cross_attn_include_queries: keys = cat(latents, context) (ns2.py:1060-1061)
             ops.gemm(L["lat_bf"], P[f"pr{i}_q"], L["q"], n=inner, epilogue=ops.EPI_BF16)
             ops.gemm(L["cat"], P[f"pr{i}_kv"], L["kv"], n=2 * inner, epilogue=ops.EPI_BF16)
-            ops.attention(L["q"], L["kv"][:, :, :inner], L["kv"][:, :, inner:], L["o"], heads=H, lse=L["lse"])
+            ops.attention(L["q"], L["kv"][:, :, :inner], L["kv"][:, :, inner:], L["o"], heads=H, lse=L["lse"],
+                          kv_lens=kv_lens)
             ops.gemm(L["o"], P[f"pr{i}_o"], lat, n=D, epilogue=ops.EPI_F32, resid=lat)
             ops.cast_bf16(lat, L["lat_bf2"])
             ops.gemm(L["lat_bf2"], P[f"pr{i}_ff_w1"], L["g"], n=2 * Dp, epilogue=ops.EPI_GEGLU, bias=P[f"pr{i}_ff_b1"])
@@ -499,21 +507,28 @@ class Model(_PackedCache):
         return out
 
     def precompute_conditioning(self, prompt: torch.Tensor, cond: torch.Tensor, length: int,
-                                saved: Optional[dict] = None) -> dict:
+                                saved: Optional[dict] = None, *, prompt_lens=None, cond_lens=None) -> dict:
         """Everything in `forward` that depends on (prompt, cond) but not on the timestep or x:
         prompt FiLM vector, perceiver latents, projected aligned condition (ns2.py:947-992).  `saved`: see
-        `_forward_impl`."""
+        `_forward_impl`.
+        prompt_lens (B,): sample b's prompt is prompt[b, :prompt_lens[b]] (the mean, the perceiver's keys); cond_lens (B,):
+        its condition ends at frame cond_lens[b] (kept in the result as "cond_lens" for `forward`).  With them each
+        sample's conditioning is that of the sample alone, and nothing in the padded rows is read."""
         assert self.condition_on_prompt
         P, D = self.packed(), self.dim
         B = prompt.shape[0]
         dev = prompt.device
+        if saved is not None and (prompt_lens is not None or cond_lens is not None):
+            raise NotImplementedError("prompt_lens / cond_lens are supported for sampling only")
+        plens = None if prompt_lens is None else ops.lengths(prompt_lens, B, prompt.shape[1], device=dev,
+                                                             name="prompt_lens")
         prompt = prompt.float().contiguous()
-        mean = ops.mean_rows(prompt, torch.empty(B, self.dim_prompt, device=dev))
+        mean = ops.mean_rows(prompt, torch.empty(B, self.dim_prompt, device=dev), lens=plens)
         lin = self.to_prompt_cond[1]
         prompt_cond = ops.small_linear(mean, lin.weight.detach().float().contiguous(),
                                        lin.bias.detach().float().contiguous(),
                                        torch.empty(B, self.dim_time, device=dev), act=1)
-        tokens = self._perceiver(prompt, P, saved)
+        tokens = self._perceiver(prompt, P, saved, plens)
         L = cond.shape[-1]
         cond_bf = ops.transpose_cast(cond.float().contiguous(), torch.empty(B, L, self.dim_prompt, device=dev,
                                                                             dtype=torch.bfloat16))
@@ -521,7 +536,10 @@ class Model(_PackedCache):
                              bias=P["cond_b"])
         if saved is not None:
             saved.update(prompt_mean=mean, cond_bf=cond_bf, Lc=L)
-        return Conditioning(prompt_cond=prompt_cond, tokens=tokens, cond_proj=cond_proj, length=length)
+        c = Conditioning(prompt_cond=prompt_cond, tokens=tokens, cond_proj=cond_proj, length=length)
+        if cond_lens is not None:
+            c["cond_lens"] = ops.lengths(cond_lens, B, None, device=dev, name="cond_lens", lo=0)
+        return c
 
     def _run(self, name, fn, *args, **kwargs):
         """Call one kernel wrapper; when profiling is on, bracket it with CUDA events on the current stream."""
@@ -546,7 +564,8 @@ class Model(_PackedCache):
         return ops.cfg_combine(logits, null_logits, cond_scale, logits)   # in place into the (fresh) first output
 
     def forward(self, x, times, prompt=None, prompt_mask=None, cond=None, cond_drop_prob=None, *,
-                out: Optional[torch.Tensor] = None, _conditioning: Optional[dict] = None):
+                out: Optional[torch.Tensor] = None, _conditioning: Optional[dict] = None, prompt_lens=None,
+                cond_lens=None):
         """x (B, N, dim) fp32, times (B,) in [0, 1] -> (B, N, dim) fp32   (ns2.py:929-1000).
 
         Returns a fresh tensor, like the reference; pass `out=` (contiguous fp32 (B, N, dim)) to have the prediction
@@ -556,13 +575,26 @@ class Model(_PackedCache):
 
         With `use_cuda_graphs` the whole step (every kernel launch below) is captured once per
         (B, N, drop-prob, conditioning shapes) and replayed; eligible when no RNG draw and no per-call host work is
-        involved, i.e. unconditional models or cached conditioning with cond_drop_prob in {0, 1}."""
+        involved, i.e. unconditional models or cached conditioning with cond_drop_prob in {0, 1}.
+
+        prompt_lens / cond_lens (B,) (inference only): per-sample prompt lengths and condition lengths of a batch padded
+        at the end, see `precompute_conditioning`; cached conditioning carries its own."""
+        ragged = prompt_lens is not None or cond_lens is not None
+        if ragged and _conditioning is not None:
+            raise ValueError("prompt_lens / cond_lens go to precompute_conditioning when the conditioning is cached")
         if _records_graph(self):
             # training: one autograd node whose backward runs the hand-written kernels (training.py)
             from .training import DenoiserFunction
-            if prompt_mask is not None or out is not None or _conditioning is not None:
-                raise NotImplementedError("training mode takes (x, times[, prompt, cond]): no out=, prompt_mask or cached conditioning")
+            if prompt_mask is not None or out is not None or _conditioning is not None or ragged:
+                raise NotImplementedError("training mode takes (x, times[, prompt, cond]): no out=, prompt_mask, lengths or "
+                                          "cached conditioning")
             return DenoiserFunction.apply(self, x, times, prompt, cond, cond_drop_prob, *self.parameters())
+        if ragged:
+            if not self.condition_on_prompt:
+                raise ValueError("prompt_lens / cond_lens apply to models with condition_on_prompt=True")
+            with torch.no_grad():   # eager: the prompt work is per call anyway
+                return self._forward_impl(x, times, prompt, prompt_mask, cond, cond_drop_prob, None, out,
+                                          prompt_lens=prompt_lens, cond_lens=cond_lens)
         with torch.no_grad():
             return self._forward_nograd(x, times, prompt, prompt_mask, cond, cond_drop_prob, out, _conditioning)
 
@@ -584,6 +616,7 @@ class Model(_PackedCache):
         cond_sig = None
         if conditioning is not None:
             cond_sig = tuple(tuple(conditioning[k].shape) for k in ("prompt_cond", "tokens", "cond_proj"))
+            cond_sig += (conditioning.get("cond_lens") is not None,)   # a different cond_inject launch
         key = (B, N, float(p_eff), cond_sig, str(x.device))
         entry = self._graphs.get(key)
         if entry is None:
@@ -627,7 +660,7 @@ class Model(_PackedCache):
     @torch.no_grad()
     def _forward_impl(self, x, times, prompt=None, prompt_mask=None, cond=None, cond_drop_prob=None,
                       _conditioning: Optional[dict] = None, out: Optional[torch.Tensor] = None,
-                      saved: Optional[dict] = None):
+                      saved: Optional[dict] = None, prompt_lens=None, cond_lens=None):
         """The denoiser's forward.  Without `saved` every intermediate lives in the per-shape workspace, so the call can
         be captured in a CUDA graph.  With `saved` (a dict; the training forward of `training.DenoiserFunction`) the
         workspace is not touched: each activation `training.train_backward` reads goes to a fresh tensor recorded
@@ -663,7 +696,8 @@ class Model(_PackedCache):
             if _conditioning is None:
                 assert _exists(prompt), "prompt is required when condition_on_prompt=True"
                 assert _exists(cond), "cond is required when condition_on_prompt=True"
-                _conditioning = self.precompute_conditioning(prompt, cond, N, saved)
+                _conditioning = self.precompute_conditioning(prompt, cond, N, saved, prompt_lens=prompt_lens,
+                                                             cond_lens=cond_lens)
             # two independent draws, in the reference's order (ns2.py:950, 980): kept in torch for RNG-stream parity
             drop_mask = _prob_mask_like((B,), cond_drop_prob, dev)
             cond_drop_mask = _prob_mask_like((B,), cond_drop_prob, dev)
@@ -685,7 +719,8 @@ class Model(_PackedCache):
             # x + pad_or_curtail(where(cond_drop_mask, null_cond, cond_proj)) -> bf16 in one pass (ns2.py:982-992)
             x_bf = self._run("cast", ops.cond_inject, x.float().contiguous(), _conditioning["cond_proj"],
                              buf("x_bf", B, N, D), drop_mask=cond_drop_mask,
-                             null_cond=self.null_cond.detach().float().reshape(-1))
+                             null_cond=self.null_cond.detach().float().reshape(-1),
+                             cond_lens=_conditioning.get("cond_lens"))
         else:
             x_bf = self._run("cast", ops.cast_bf16, x.float().contiguous(), buf("x_bf", B, N, D))
         h0 = self._run("wn_init", ops.gemm, x_bf, P["wn_init_w"], buf("h", B, N, D), n=D, epilogue=ops.EPI_BF16,

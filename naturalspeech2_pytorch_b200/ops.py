@@ -211,18 +211,110 @@ def dropout_(x: torch.Tensor, *, dropout: Optional[DropoutSpec]) -> torch.Tensor
 
 
 # --------------------------------------------------------------------------------------------------
+# per-sample lengths: a batch of sequences padded at the end to the longest one
+# --------------------------------------------------------------------------------------------------
+def lengths(lens, batch: int, max_len: Optional[int], *, device, name: str = "lengths", lo: int = 1) -> torch.Tensor:
+    """`lens` (a sequence of ints, or an integer tensor anywhere) as the contiguous int32 CUDA tensor the ragged kernels
+    read, after checking it holds `batch` values in [lo, max_len] (max_len None: no upper bound)."""
+    if isinstance(lens, torch.Tensor):
+        if lens.is_floating_point() or lens.is_complex() or lens.dtype == torch.bool:
+            raise ValueError(f"{name} must hold integers, got {lens.dtype}")
+        host = lens.detach().reshape(-1).tolist() if lens.dim() <= 1 else None
+    else:
+        host = [int(v) for v in lens]
+    if host is None or len(host) != batch:
+        raise ValueError(f"{name} must hold one length per sample ({batch}), got {host if host is None else len(host)}")
+    _check_range(name, min(host), max(host), lo, max_len)
+    out = torch.tensor(host, dtype=torch.int32).to(device)
+    out._ns2_range = (out._version, min(host), max(host))
+    return out
+
+
+def _check_range(name: str, mn: int, mx: int, lo: int, hi: Optional[int]) -> None:
+    if mn < lo or (hi is not None and mx > hi):
+        raise ValueError(f"{name} must lie in [{lo}, {hi if hi is not None else 'inf'}], got values in [{mn}, {mx}]")
+
+
+def _check_lens(lens: torch.Tensor, batch: int, lo: int, hi: Optional[int], name: str) -> int:
+    """Check per-sample lengths before a ragged launch: an int32 CUDA tensor of `batch` values in [lo, hi] on the current
+    device.  The range is read once per tensor version (one device sync) and remembered on the tensor; while a CUDA graph
+    is being captured values cannot be read, and the kernels clamp them instead.  Returns the data pointer."""
+    if not isinstance(lens, torch.Tensor) or not lens.is_cuda:
+        raise ValueError(f"{name} must be a CUDA int32 tensor")
+    if lens.dtype != torch.int32:
+        raise ValueError(f"{name} must be int32, got {lens.dtype}")
+    if lens.dim() != 1 or lens.numel() != batch or not lens.is_contiguous():
+        raise ValueError(f"{name} must be a contiguous ({batch},) tensor, got {tuple(lens.shape)}")
+    _stream(lens)
+    rng = getattr(lens, "_ns2_range", None)
+    if rng is None or rng[0] != lens._version:
+        if torch.cuda.is_current_stream_capturing():
+            return lens.data_ptr()
+        mn, mx = torch.stack((lens.min(), lens.max())).tolist()
+        rng = lens._ns2_range = (lens._version, mn, mx)
+    _check_range(name, rng[1], rng[2], lo, hi)
+    return lens.data_ptr()
+
+
+def mask_rows(x: torch.Tensor, lens: torch.Tensor) -> torch.Tensor:
+    """x (B, N, C) f32 or bf16, in place: rows r >= lens[b] of sample b become exact zeros.  Row- and batch-strided
+    views are fine (channels contiguous); lens in [0, N]."""
+    lib = _lib.load()
+    if x.dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError(f"x must be float32 or bfloat16, got {x.dtype}")
+    _req(x, x.dtype, "x")
+    if x.dim() != 3:
+        raise ValueError(f"x must be (B, N, C), got {tuple(x.shape)}")
+    B, N, Cc = x.shape
+    lp = _check_lens(lens, B, 0, N, "lens")
+    check(lib.ns2_mask_rows(x.data_ptr(), int(x.dtype == torch.float32), x.stride(1), x.stride(0), B, N, Cc, lp,
+                            _stream(x)), "ns2_mask_rows")
+    return x
+
+
+def pack_rows(a: torch.Tensor, a_lens: torch.Tensor, b: torch.Tensor, b_lens: torch.Tensor,
+              out: torch.Tensor) -> torch.Tensor:
+    """bf16 out[s] = [a[s, :a_lens[s]] ; b[s, :b_lens[s]] ; 0]: two end-padded segments (B, Na, C), (B, Nb, C) as one
+    prefix of length a_lens + b_lens of out (B, No >= Na + Nb, C).  Row- and batch-strided views are fine."""
+    lib = _lib.load()
+    for name, t in (("a", a), ("b", b), ("out", out)):
+        _req(t, torch.bfloat16, name)
+        if t.dim() != 3:
+            raise ValueError(f"{name} must be (B, N, C), got {tuple(t.shape)}")
+    B, Na, Cc = a.shape
+    if b.shape[0] != B or out.shape[0] != B or b.shape[2] != Cc or out.shape[2] != Cc:
+        raise ValueError(f"pack_rows: inconsistent shapes {tuple(a.shape)}, {tuple(b.shape)}, {tuple(out.shape)}")
+    Nb, No = b.shape[1], out.shape[1]
+    if No < Na + Nb:
+        raise ValueError(f"out holds {No} rows, fewer than {Na} + {Nb}")
+    ap = _check_lens(a_lens, B, 0, Na, "a_lens")
+    bp = _check_lens(b_lens, B, 0, Nb, "b_lens")
+    check(lib.ns2_pack_rows_ragged(a.data_ptr(), a.stride(1), a.stride(0), Na, ap, b.data_ptr(), b.stride(1),
+                                   b.stride(0), Nb, bp, B, Cc, out.data_ptr(), out.stride(1), out.stride(0), No,
+                                   _stream(out)), "ns2_pack_rows_ragged")
+    return out
+
+
+# --------------------------------------------------------------------------------------------------
 # attention
 # --------------------------------------------------------------------------------------------------
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tensor, *, heads: int,
               scale: Optional[float] = None, lse: Optional[torch.Tensor] = None,
-              dropout: Optional[DropoutSpec] = None) -> torch.Tensor:
+              dropout: Optional[DropoutSpec] = None, kv_lens: Optional[torch.Tensor] = None) -> torch.Tensor:
     """q: (B, Nq, heads*64), k/v: (B, Nk, heads*64) bf16 (strided views into a fused projection are fine).
-    dropout=(seed, site, p): attention dropout on the softmax probabilities (lse stays that of the undropped ones)."""
+    dropout=(seed, site, p): attention dropout on the softmax probabilities (lse stays that of the undropped ones).
+    kv_lens: int32 CUDA (B,) in [1, Nk]: sample b attends to its keys [0, kv_lens[b]) only (K / V rows past it must be
+    finite); its output is bit-identical to the call on that sample's keys alone.  No dropout with kv_lens."""
     lib = _lib.load()
     for name, t in (("q", q), ("k", k), ("v", v), ("out", out)):
         _req(t, torch.bfloat16, name)
         if t.dim() != 3 or t.shape[2] != heads * 64:
             raise ValueError(f"{name} must be (B, N, heads*64), got {tuple(t.shape)}")
+    lens_ptr = None
+    if kv_lens is not None:
+        if dropout is not None:
+            raise ValueError("attention: dropout with kv_lens is not supported")
+        lens_ptr = _check_lens(kv_lens, q.shape[0], 1, k.shape[1], "kv_lens")
     args = AttnArgs()
     args.q, args.q_row_stride, args.q_batch_stride = q.data_ptr(), q.stride(1), q.stride(0)
     args.k, args.k_row_stride, args.k_batch_stride = k.data_ptr(), k.stride(1), k.stride(0)
@@ -237,7 +329,9 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tens
             raise ValueError("lse must be a contiguous (B, heads, Nq) float tensor")
     args.lse = _ptr(lse)
     d = _dropout_args(dropout)
-    if d is None:
+    if lens_ptr is not None:
+        check(lib.ns2_attn_fwd_ragged(C.byref(args), lens_ptr, _stream(out)), "ns2_attn_fwd_ragged")
+    elif d is None:
         check(lib.ns2_attn_fwd(C.byref(args), _stream(out)), "ns2_attn_fwd")
     else:
         check(lib.ns2_attn_fwd_dropout(C.byref(args), C.byref(d), _stream(out)), "ns2_attn_fwd_dropout")
@@ -334,8 +428,9 @@ def cast_bf16(x: torch.Tensor, out: torch.Tensor, add: Optional[torch.Tensor] = 
 
 
 def cond_inject(x: torch.Tensor, cproj: torch.Tensor, out: torch.Tensor, drop_mask: Optional[torch.Tensor] = None,
-                null_cond: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """out (B, N, D) bf16 = x (B, N, D) f32 + [padded / curtailed, null-substituted] cproj (B, L, D) f32."""
+                null_cond: Optional[torch.Tensor] = None, *, cond_lens: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out (B, N, D) bf16 = x (B, N, D) f32 + [padded / curtailed, null-substituted] cproj (B, L, D) f32.
+    cond_lens: int32 CUDA (B,) >= 0: sample b's condition ends at frame min(L, cond_lens[b])."""
     lib = _lib.load()
     _req(x, torch.float32, "x")
     _req(cproj, torch.float32, "cproj")
@@ -350,8 +445,13 @@ def cond_inject(x: torch.Tensor, cproj: torch.Tensor, out: torch.Tensor, drop_ma
         _req(null_cond, torch.float32, "null_cond")
         if null_cond.numel() != D or not null_cond.is_contiguous():
             raise ValueError("null_cond must be a contiguous (D,) float tensor")
-    check(lib.ns2_cond_inject(x.data_ptr(), cproj.data_ptr(), _ptr(drop_mask), _ptr(null_cond), B, N, cproj.shape[1], D,
-                              out.data_ptr(), _stream(out)), "ns2_cond_inject")
+    if cond_lens is None:
+        check(lib.ns2_cond_inject(x.data_ptr(), cproj.data_ptr(), _ptr(drop_mask), _ptr(null_cond), B, N, cproj.shape[1],
+                                  D, out.data_ptr(), _stream(out)), "ns2_cond_inject")
+        return out
+    lp = _check_lens(cond_lens, B, 0, None, "cond_lens")
+    check(lib.ns2_cond_inject_ragged(x.data_ptr(), cproj.data_ptr(), _ptr(drop_mask), _ptr(null_cond), B, N,
+                                     cproj.shape[1], D, lp, out.data_ptr(), _stream(out)), "ns2_cond_inject_ragged")
     return out
 
 
@@ -377,13 +477,22 @@ def select_rows(drop_mask: torch.Tensor, null_row: torch.Tensor, src: torch.Tens
     return out
 
 
-def mean_rows(x: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+def mean_rows(x: torch.Tensor, out: torch.Tensor, *, lens: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out (B, D) = mean over the rows of x (B, N, D) f32; lens: int32 CUDA (B,) in [1, N], the mean of sample b over
+    its rows [0, lens[b])."""
     lib = _lib.load()
     _req(x, torch.float32, "x")
     _req(out, torch.float32, "out")
     B, N, D = x.shape
-    check(lib.ns2_mean_rows(x.contiguous().data_ptr(), B, N, D, out.data_ptr(), _stream()),
-          "ns2_mean_rows")
+    if lens is None:
+        check(lib.ns2_mean_rows(x.contiguous().data_ptr(), B, N, D, out.data_ptr(), _stream()),
+              "ns2_mean_rows")
+        return out
+    lp = _check_lens(lens, B, 1, N, "lens")
+    if not out.is_contiguous() or tuple(out.shape) != (B, D):
+        raise ValueError(f"out must be a contiguous ({B}, {D}) tensor")
+    check(lib.ns2_mean_rows_ragged(x.contiguous().data_ptr(), B, N, D, lp, out.data_ptr(), _stream()),
+          "ns2_mean_rows_ragged")
     return out
 
 
@@ -406,8 +515,10 @@ OBJECTIVES = {"v": _lib.NS2_OBJ_V, "eps": _lib.NS2_OBJ_EPS, "x0": _lib.NS2_OBJ_X
 
 def groupnorm_silu(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, groups: int, *, eps: float = 1e-5,
                    resid: Optional[torch.Tensor] = None, out_f32: Optional[torch.Tensor] = None,
-                   out_bf16: Optional[torch.Tensor] = None):
-    """silu(GroupNorm(groups)(x)) (+ resid) for token-major x (B, N, C) f32 -> out_f32 and/or out_bf16 (B, N, C)."""
+                   out_bf16: Optional[torch.Tensor] = None, lens: Optional[torch.Tensor] = None):
+    """silu(GroupNorm(groups)(x)) (+ resid) for token-major x (B, N, C) f32 -> out_f32 and/or out_bf16 (B, N, C).
+    lens: int32 CUDA (B,) in [1, N]: sample b is normalised over its rows [0, lens[b]) (bit-identical to the call on
+    those rows alone); its rows past that are written as zeros."""
     lib = _lib.load()
     _req(x, torch.float32, "x")
     _req(weight, torch.float32, "weight")
@@ -423,8 +534,14 @@ def groupnorm_silu(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, gr
     if out_f32 is None and out_bf16 is None:
         raise ValueError("groupnorm_silu needs at least one output")
     B, N, Cn = x.shape
-    check(lib.ns2_groupnorm_silu(x.data_ptr(), B, N, Cn, int(groups), weight.data_ptr(), bias.data_ptr(), float(eps),
-                                 _ptr(resid), _ptr(out_f32), _ptr(out_bf16), _stream(x)), "ns2_groupnorm_silu")
+    if lens is None:
+        check(lib.ns2_groupnorm_silu(x.data_ptr(), B, N, Cn, int(groups), weight.data_ptr(), bias.data_ptr(), float(eps),
+                                     _ptr(resid), _ptr(out_f32), _ptr(out_bf16), _stream(x)), "ns2_groupnorm_silu")
+        return out_f32, out_bf16
+    lp = _check_lens(lens, B, 1, N, "lens")
+    check(lib.ns2_groupnorm_silu_ragged(x.data_ptr(), B, N, Cn, int(groups), weight.data_ptr(), bias.data_ptr(),
+                                        float(eps), _ptr(resid), _ptr(out_f32), _ptr(out_bf16), lp, _stream(x)),
+          "ns2_groupnorm_silu_ragged")
     return out_f32, out_bf16
 
 

@@ -131,6 +131,19 @@ typedef struct ns2_wgrad_args {
 int ns2_wgrad(const ns2_wgrad_args* args, ns2_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * 1c. A conv followed by a Linear with nothing between them, folded into one conv pack: the transformer feed-forward's
+ *     CausalConv1d and output projection (FeedForward, ns2.py:1019-1024).  For each of `layers` stacked layers
+ *        out[l][o, t*i_pad + c] = bf16( sum_d w2[l][o, d] * wc[l][d, c, t] )   (0 for i <= c < i_pad)
+ *        bias_out[l][o]         = sum_d w2[l][o, d] * bc[l][d] + b2[l][o]
+ *     w2 (layers, o, k), wc (layers, k, i, taps) (Conv1d's (out, in, taps) layout), bc (layers, k), b2 (layers, o):
+ *     contiguous fp32.  out: bf16 (layers, o, taps*i_pad), tap-major like every conv pack; bias_out fp32 (layers, o).
+ *     fp32 FMA accumulation (no TF32), one rounding to bf16.
+ * ------------------------------------------------------------------------------------------------ */
+int ns2_fold_conv_linear(const float* w2, const float* wc, const float* bc, const float* b2, int32_t layers, int32_t o,
+                         int32_t k, int32_t i, int32_t taps, int32_t i_pad, void* out_bf16, float* bias_out,
+                         ns2_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * 2. Non-causal, unmasked flash attention forward (Attend.forward, attend.py:112-155 with mask=None,
  *    causal=False, dropout=0 — the only configuration the hot path uses, SURVEY T9).
  *    q/k/v: bf16, head h lives in columns [h*64, h*64+64) of each row; dim_head must be 64.

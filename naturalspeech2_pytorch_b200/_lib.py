@@ -97,6 +97,7 @@ SIGNATURES = {
     "ns2_launch_count": (C.c_int64, []),
     "ns2_gemm": (C.c_int, [C.POINTER(GemmArgs), _P]),
     "ns2_wgrad": (C.c_int, [C.POINTER(WgradArgs), _P]),
+    "ns2_fold_conv_linear": (C.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P]),
     "ns2_attn_fwd": (C.c_int, [C.POINTER(AttnArgs), _P]),
     "ns2_attn_bwd": (C.c_int, [C.POINTER(AttnBwdArgs), _P]),
     "ns2_attn_fwd_ragged": (C.c_int, [C.POINTER(AttnArgs), _P, _P]),

@@ -21,7 +21,7 @@ LIB_PATH = LIB_DIR / "libns2b200.so"
 OBJ_DIR = PKG_DIR / "build" / "obj"
 
 SOURCES = ["host_common.cu", "elementwise.cu", "gemm.cu", "attn.cu", "rvq.cu", "rvq_ce.cu", "wgrad.cu", "backward.cu", "attn_bwd.cu", "align.cu",
-           "encoder_bwd.cu", "seanet.cu"]
+           "encoder_bwd.cu", "seanet.cu", "fold.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

@@ -214,7 +214,7 @@ class _EncoderBase(_PackedCache):
             L = layers[l]
             pfx = f"transformer.layers.{l}."
             # ---- feed-forward: x += W2 GEGLU(W1 RMSNorm(x) + b1) + b2 ----
-            dh2 = ff_backward(dxr_bf, L["h2"], L["ff_g"], None, P, T, f"l{l}_", tr.layers[l][3][-1].weight.shape[1],
+            dh2 = ff_backward(dxr_bf, L["h2"], L["ff_g"], P, T, f"l{l}_", tr.layers[l][3][-1].weight.shape[1],
                               grads, pfx + "3.")
             norm_backward(L["x_mid"], dh2, P[f"l{l}_g2"], pfx + "2.gamma")
             # ---- attention: x += Wo attn(Wqkv RMSNorm(x)) ----

@@ -11,7 +11,8 @@ never called); the math runs through `ops` (libns2b200.so):
                      skip sum as one K=8*dim GEMM, final conv                              ns2.py:597-725
   Transformer layer  RMSNorm+FiLM -> fused QKV GEMM -> flash attention -> out-proj(+residual)
                      [-> cross attention over the perceiver latents]
-                     -> RMSNorm+FiLM -> GEGLU GEMM -> causal k=3 conv GEMM -> out GEMM(+residual)   ns2.py:786-809
+                     -> RMSNorm+FiLM -> GEGLU GEMM -> causal k=3 conv GEMM with the out projection folded
+                     into its taps (+residual)                                             ns2.py:786-809
 Numerics: bf16 tensor-core operands, fp32 accumulation, fp32 residual stream / norm statistics / softmax,
 fp32 output (the protocol of SURVEY section 7, H1).
 """
@@ -69,6 +70,26 @@ def _pack_conv(w: torch.Tensor, i_pad: Optional[int] = None, o_pad: Optional[int
     out = w.new_zeros(o_pad, k, i_pad)
     out[:O, :, :I] = w.detach().permute(0, 2, 1)
     return _bf(out.view(o_pad, k * i_pad))
+
+
+def _fold_conv_linear(convs, lins, i_pad: int):
+    """Each conv followed by a Linear with nothing between them (FeedForward's causal conv and output projection,
+    ns2.py:1019-1024) as ONE conv from the conv's input straight to the Linear's output:
+    tap t = W2 @ Wc[:, :, t], bias = W2 @ bc + b2.  Returns per pair (the `_pack_conv` layout, input width zero-padded to
+    i_pad; the fp32 bias).  On CUDA one `ops.fold_conv_linear` launch folds every pair (fp32 accumulation, no TF32,
+    rounded to bf16 once); parameters on the CPU, where no kernel runs, are folded in float64."""
+    st = lambda ts: torch.stack([t.detach().float() for t in ts]).contiguous()  # noqa: E731
+    if convs[0].weight.is_cuda:
+        wo, bo = ops.fold_conv_linear(st(l.weight for l in lins), st(c.weight for c in convs),
+                                      st(c.bias for c in convs), st(l.bias for l in lins), i_pad)
+        return list(zip(wo.unbind(0), bo.unbind(0)))
+    out = []
+    for conv, lin in zip(convs, lins):
+        w2 = lin.weight.detach().double()
+        w = torch.einsum("od,dit->oit", w2, conv.weight.detach().double())    # (D, Di, 3)
+        b = w2 @ conv.bias.detach().double() + lin.bias.detach().double()
+        out.append((_pack_conv(w, i_pad), b.float().contiguous()))
+    return out
 
 
 def _transpose_conv(w: torch.Tensor, kernel: int) -> torch.Tensor:
@@ -373,6 +394,11 @@ class Model(_PackedCache):
             P[f"l{l}_ff_wc"] = _pack_conv(conv.weight, Dp, Dp)
             P[f"l{l}_ff_bc"] = torch.zeros(Dp, device=conv.bias.device)
             P[f"l{l}_ff_bc"][:self.ff_inner] = conv.bias
+        # the forward runs each FFN's conv and output projection as one conv (wc / bc / w2 stay for the backward)
+        ffs = [layer[5] for layer in self.transformer.layers]
+        folded = _fold_conv_linear([ff[2][1] for ff in ffs], [ff[-1] for ff in ffs], P["l0_ff_w2"].shape[1])
+        for l, (wo, bo) in enumerate(folded):
+            P[f"l{l}_ff_wo"], P[f"l{l}_ff_bo"] = wo, bo                     # (D, 3*Dp), (D,)
         if kv_all:
             P["x_kv_all"] = _bf(torch.cat(kv_all, dim=0))  # (depth*2*inner, D): cross K/V of all layers
         P["pred_gamma"] = self.transformer.to_pred[0].gamma.detach().float().contiguous()
@@ -409,6 +435,7 @@ class Model(_PackedCache):
             T[f"l{l}_ff_w1"] = t(P[f"l{l}_ff_w1"])                          # (D, 2*Dp)
             T[f"l{l}_ff_wc"] = _transpose_conv(P[f"l{l}_ff_wc"], 3)         # (Dp, 3*Dp)
             T[f"l{l}_ff_w2"] = t(P[f"l{l}_ff_w2"])                          # (Dp, D)
+            T[f"l{l}_ff_wo"] = _transpose_conv(P[f"l{l}_ff_wo"], 3)         # (Dp, 3*D)
         T["pred_w"] = t(P["pred_w"])
         T["wn_init_w"] = _transpose_conv(P["wn_init_w"], 3)
         if self.condition_on_prompt:
@@ -448,7 +475,7 @@ class Model(_PackedCache):
             "wn_a": e(B, N, G * D), "wn_b": e(B, N, G * D),
             "x_res": e(B, N, D, dt=f32),
             "qkv": e(B, N, 3 * inner), "attn_o": e(B, N, inner),
-            "ff_g": e(B, N, Dp), "ff_c": e(B, N, Dp),
+            "ff_g": e(B, N, Dp),
         }
         if self.condition_on_prompt:
             M = self.num_latents_m
@@ -780,10 +807,9 @@ class Model(_PackedCache):
             L["h2"] = self._run("norm", ops.rmsnorm_film, xr, buf("h", B, N, D), film=film[:, fo3:fo3 + 2 * D])
             L["ff_g"] = self._run("ff_in", ops.gemm, L["h2"], P[f"l{l}_ff_w1"], buf("ff_g", B, N, Dp), n=2 * Dp,
                                   epilogue=ops.EPI_GEGLU, bias=P[f"l{l}_ff_b1"])
-            L["ff_c"] = self._run("ff_conv", ops.gemm, L["ff_g"], P[f"l{l}_ff_wc"], buf("ff_c", B, N, Dp), n=Dp,
-                                  epilogue=ops.EPI_BF16, bias=P[f"l{l}_ff_bc"], segs=ops.conv3_segs(Dp))
-            self._run("ff_out", ops.gemm, L["ff_c"], P[f"l{l}_ff_w2"], xr, n=D, epilogue=ops.EPI_F32,
-                      bias=P[f"l{l}_ff_b2"], resid=xr)
+            # causal conv with the output projection folded in: x += W' * g + b' straight from the GEGLU output
+            self._run("ff_conv", ops.gemm, L["ff_g"], P[f"l{l}_ff_wo"], xr, n=D, epilogue=ops.EPI_F32,
+                      bias=P[f"l{l}_ff_bo"], resid=xr, segs=ops.conv3_segs(Dp))
             layers.append(L)
         hf = self._run("norm", ops.rmsnorm_film, xr, buf("h", B, N, D), gamma=P["pred_gamma"])
         if keep:

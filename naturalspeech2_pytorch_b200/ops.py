@@ -161,6 +161,29 @@ def wgrad(dy: torch.Tensor, x: torch.Tensor, dw: torch.Tensor, *, n: int, k: int
     return dw
 
 
+def fold_conv_linear(w2: torch.Tensor, wc: torch.Tensor, bc: torch.Tensor, b2: torch.Tensor, i_pad: int):
+    """Stacked (conv, Linear) pairs with nothing between them as one conv each (include/ns2_b200.h section 1c):
+    w2 (L, O, K), wc (L, K, I, taps), bc (L, K), b2 (L, O) fp32 -> (bf16 (L, O, taps*i_pad) tap-major pack of the taps
+    w2 @ wc[..., t], zero-padded from I to i_pad; fp32 (L, O) bias w2 @ bc + b2)."""
+    lib = _lib.load()
+    for t, name in ((w2, "w2"), (wc, "wc"), (bc, "bc"), (b2, "b2")):
+        _req(t, torch.float32, name)
+        if not t.is_contiguous():
+            raise ValueError(f"{name} must be contiguous")
+    if w2.dim() != 3 or wc.dim() != 4 or bc.dim() != 2 or b2.dim() != 2:
+        raise ValueError("fold_conv_linear: w2 (L, O, K), wc (L, K, I, taps), bc (L, K), b2 (L, O)")
+    L, O, K = w2.shape
+    _, _, I, taps = wc.shape
+    if wc.shape[:2] != (L, K) or bc.shape != (L, K) or b2.shape != (L, O) or i_pad < I:
+        raise ValueError(f"fold_conv_linear: shapes w2 {tuple(w2.shape)}, wc {tuple(wc.shape)}, bc {tuple(bc.shape)}, "
+                         f"b2 {tuple(b2.shape)}, i_pad {i_pad} do not fit")
+    out = torch.empty(L, O, taps * i_pad, device=w2.device, dtype=torch.bfloat16)
+    bias = torch.empty(L, O, device=w2.device, dtype=torch.float32)
+    check(lib.ns2_fold_conv_linear(w2.data_ptr(), wc.data_ptr(), bc.data_ptr(), b2.data_ptr(), L, O, K, I, taps, i_pad,
+                                   out.data_ptr(), bias.data_ptr(), _stream(out)), "ns2_fold_conv_linear")
+    return out, bias
+
+
 def conv_segs(c_in: int, kernel: int, first_shift: int) -> list:
     """Segments of a stride-1 convolution whose packed weight holds tap t at columns [t*c_in, (t+1)*c_in): tap t reads
     x[n - (first_shift - t) * dilation].  Causal k=3 (CausalConv1d, ns2.py:583-595): first_shift = 2; "same" padding p:

@@ -9,7 +9,8 @@ fresh tensors.  Its backward walks the network in reverse and launches, per laye
   * attention bwd   ns2_attn_bwd (wgmma flash backward from the saved log-sum-exp),
   * the element-wise backward kernels of csrc/backward.cu (RMSNorm+FiLM, GEGLU, Wavenet gate, bias column sums).
 Pre-activations that the fused forward epilogues never materialise (GEGLU's value/gate pair, the Wavenet conv output
-before FiLM) are recomputed with plain-epilogue GEMMs instead of being stored.  Gradients come out in the packed bf16
+before FiLM) and the feed-forward's conv output, which the forward folds into the output projection and never
+computes, are recomputed with plain-epilogue GEMMs instead of being stored.  Gradients come out in the packed bf16
 layouts' fp32 twins, under the state_dict's keys; `param_grads` gives them the parameters' shapes.
 Each building block has one implementation, shared by the denoiser, the perceiver and the encoders (encoders.py):
 `linear_backward`, `conv_backward`, `ff_backward` (with `geglu_backward`) and `attention_backward`.
@@ -107,14 +108,23 @@ def geglu_backward(h, d_g, w1, b1, w1_t, Di: int, grads: Dict[str, torch.Tensor]
     return _dgrad(pre, w1_t)
 
 
-def ff_backward(dy, h, g, c, P, T, pk: str, Di: int, grads: Dict[str, torch.Tensor], name: str) -> torch.Tensor:
+def ff_backward(dy, h, g, P, T, pk: str, Di: int, grads: Dict[str, torch.Tensor], name: str,
+                causal_conv: bool = False) -> torch.Tensor:
     """Backward of FeedForward (ns2.py:1009-1025) y = W2 [causal conv](GEGLU(W1 h + b1)) + b2 from the saved GEGLU output
-    g and, when the layer has the causal k=3 conv, its output c (None without it).  Weights are P / T[pk + "w1" / "b1" /
-    "wc" / "w2"], the inner width Di padded in the packs; gradients go to grads[name + Sequential index + ...].  Returns
-    d h (bf16)."""
-    d_g = linear_backward(dy, g if c is None else c, grads, name + ("2" if c is None else "3"), T[pk + "w2"], width=Di)
-    if c is not None:
-        d_g = conv_backward(d_g, g, grads, name + "2.1", T[pk + "wc"], 3, 2, width=Di)
+    g.  Weights are P / T[pk + "w1" / "b1" / "wc" / "bc" / "w2" / "wo"], the inner width Di padded in the packs;
+    gradients go to grads[name + Sequential index + ...].  Returns d h (bf16).
+    With the causal k=3 conv the forward ran conv and W2 as one folded conv (pack "wo", `model._fold_conv_linear`) and
+    kept no conv output: c = conv(g) + bc is recomputed for W2's gradient alone, d c = dy W2 gives the conv's
+    gradients, and d g is the folded conv's dgrad straight from dy (K = 3 D instead of 3 Dp)."""
+    if not causal_conv:
+        d_g = linear_backward(dy, g, grads, name + "2", T[pk + "w2"], width=Di)
+    else:
+        Dp = g.shape[-1]
+        c = ops.gemm(g, P[pk + "wc"], torch.empty_like(g), n=Dp, epilogue=ops.EPI_BF16, bias=P[pk + "bc"],
+                     segs=ops.conv3_segs(Dp))
+        d_c = linear_backward(dy, c, grads, name + "3", T[pk + "w2"], width=Di)
+        conv_backward(d_c, g, grads, name + "2.1", None, 3, 2, width=Di)
+        d_g = _dgrad(dy, T[pk + "wo"], segs=ops.conv_dgrad_segs(dy.shape[-1], 3, 2))
     return geglu_backward(h, d_g, P[pk + "w1"], P[pk + "b1"], T[pk + "w1"], Di, grads, name + "0")
 
 
@@ -199,7 +209,7 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grad
         pfx = f"transformer.layers.{l}."
         fo = model._film_tr_off + l * npl * 2 * D
         # ---- feed-forward branch: x += W2 conv(GEGLU(W1 h2)) ----
-        dh2 = ff_backward(dxr_bf, L["h2"], L["ff_g"], L["ff_c"], P, T, f"l{l}_ff_", Di, grads, pfx + "5.")
+        dh2 = ff_backward(dxr_bf, L["h2"], L["ff_g"], P, T, f"l{l}_ff_", Di, grads, pfx + "5.", causal_conv=True)
         norm_backward(L["x_mid"], dh2, fo + (npl - 1) * 2 * D)
         # ---- cross-attention branch: x += Wxo attn(Wxq h_x, Wxkv c); Wxkv's gradient is taken for all layers at once ----
         if conditional:
@@ -366,7 +376,7 @@ def _conditioning_backward_tokens(model, S, T, d_xkv, grads, want_prompt: bool):
         L = S["pr_layers"][i]
         pfx = f"perceiver_resampler.layers.{i}."
         # feed-forward (no conv, no pre-norm): lat += W2 GEGLU(W1 lat)
-        ops.accum_bf16(dlat, ff_backward(dlat_bf, L["lat_bf2"], L["g"], None, P, T, f"pr{i}_ff_", pr.ff_inner, grads,
+        ops.accum_bf16(dlat, ff_backward(dlat_bf, L["lat_bf2"], L["g"], P, T, f"pr{i}_ff_", pr.ff_inner, grads,
                                          pfx + "1."), dlat_bf)
         # attention over cat(latents, projected prompt): lat += Wo attn(Wq lat, Wkv cat)
         d_lat, d_cat = attention_backward(dlat_bf, L["lat_bf"], L["o"], L["lse"], L["q"], L["kv"], T[f"pr{i}_o"],

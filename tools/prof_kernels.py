@@ -6,7 +6,11 @@ Every GEMM shape is timed twice in the same process: the full kernel, and the ma
 epilogue costs on top of the MMAs.  Prints the GPU name and power limit first, because every number below
 depends on them.
 
-    python tools/prof_kernels.py [conv attn wavenet ffin ffout attnout qkv norm rvq sweep]
+    python tools/prof_kernels.py [conv fold attn wavenet ffin ffout attnout qkv norm rvq sweep]
+
+"conv" is the unfolded FFN causal conv (1408 -> 1408, BF16 out), kept to compare with "fold": the conv with the
+output projection folded into its taps, 1408 -> 512, F32 + residual in place, the launch the model runs.  "conv"'s
+rate counts the unpadded conv's FLOPs (1365 wide), "fold"'s the FLOPs the launch executes, padding included.
 """
 import os
 import subprocess
@@ -21,7 +25,7 @@ from naturalspeech2_pytorch_b200 import ops  # noqa: E402
 B, N, D, H, Di, Dp = 32, 1024, 512, 8, 1365, 1408
 dev = "cuda"
 bf = torch.bfloat16
-which = set(sys.argv[1:]) or {"conv", "attn", "wavenet", "ffin", "ffout", "attnout", "qkv", "norm", "rvq"}
+which = set(sys.argv[1:]) or {"conv", "fold", "attn", "wavenet", "ffin", "ffout", "attnout", "qkv", "norm", "rvq"}
 reps = int(os.environ.get("NS2_PROF_REPS", "20"))
 SKIP_EPILOGUE = 1   # NS2_GEMM_FLAG_SKIP_EPILOGUE
 
@@ -80,6 +84,13 @@ if "conv" in which:
     out = torch.empty(B, N, Dp, device=dev, dtype=bf)
     time_gemm("ff_conv gemm<256,1,BF16>", 2.0 * B * N * Di * 3 * Di, a=g, w=wc, out=out, n=Dp,
               epilogue=ops.EPI_BF16, bias=bc, segs=ops.conv3_segs(Dp))
+if "fold" in which:
+    g = (torch.randn(B, N, Dp, device=dev) * 0.5).to(bf)
+    wo = (torch.randn(D, 3 * Dp, device=dev) * 0.02).to(bf)
+    bo = torch.randn(D, device=dev)
+    xr = torch.randn(B, N, D, device=dev)
+    time_gemm("ff_conv folded gemm<256,1,F32+resid in place> K=3x1408", 2.0 * B * N * D * 3 * Dp, a=g, w=wo, out=xr,
+              n=D, epilogue=ops.EPI_F32, bias=bo, resid=xr, segs=ops.conv3_segs(Dp))
 if "attn" in which:
     qkv = torch.randn(B, N, 3 * H * 64, device=dev).to(bf)
     o = torch.empty(B, N, H * 64, device=dev, dtype=bf)

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define NS2_ABI_VERSION 7
+#define NS2_ABI_VERSION 8
 
 typedef void* ns2_stream_t; /* cudaStream_t */
 
@@ -143,11 +143,32 @@ int ns2_fold_conv_linear(const float* w2, const float* wc, const float* bc, cons
                          int32_t k, int32_t i, int32_t taps, int32_t i_pad, void* out_bf16, float* bias_out,
                          ns2_stream_t stream);
 
+/* One dropout site's parameters (training only): seed, site and drop probability p.  The attention calls of section 2
+ * take them through a pointer in their argument structs (NULL = no dropout); section 2b gives the keep rule. */
+typedef struct ns2_dropout {
+  uint64_t seed;
+  uint32_t site;
+  float p;
+} ns2_dropout;
+
 /* ------------------------------------------------------------------------------------------------
- * 2. Non-causal, unmasked flash attention forward (Attend.forward, attend.py:112-155 with mask=None,
- *    causal=False, dropout=0 — the only configuration the hot path uses, SURVEY T9).
+ * 2. Non-causal flash attention forward (Attend.forward, attend.py:112-155 with causal=False).
  *    q/k/v: bf16, head h lives in columns [h*64, h*64+64) of each row; dim_head must be 64.
  *    out[b, i, h*64:(h+1)*64] = softmax_j(q_i . k_j * scale) @ v   (bf16)
+ *    With kv_lens == NULL and dropout == NULL (a zero-initialised struct's optional fields) this is the unmasked,
+ *    dropout-free attention the denoiser runs (mask=None, dropout=0, SURVEY T9).
+ *  kv_lens: key padding for a batch of sequences of different lengths: sample b attends to keys [0, kv_lens[b]) only —
+ *    Attend with a key-padding mask (attend.py:123-129, 140-142: masked scores -> -max, i.e. probability 0), the `mask`
+ *    that PhonemeEncoder (ns2.py:275), SpeechPromptEncoder's Transformer (ns2.py:1110-1115) and the perceiver /
+ *    predictor cross attentions (ns2.py:572-577, 457-466) would pass for padded batches.
+ *    Device int32 (batches); each value is clamped to [1, kv_len] (callers should reject others).
+ *    K / V rows at or past kv_lens[b] are never weighted, but they must be FINITE: their probability is exactly 0 and
+ *    0 * V is still formed (V = NaN or inf there would reach the output).
+ *    Query rows are not masked: rows a caller treats as padding get finite, meaningless output.
+ *    Sample b's output rows are bit-identical to a call on that sample alone with kv_len = kv_lens[b] and no kv_lens.
+ *  dropout: dropout on the softmax probabilities (Attend, attend.py:106 SDPA dropout_p, attend.py:149 attn_dropout):
+ *    out = ((P (.) M) V) / (1 - p); lse as without dropout (undropped probabilities, bit-identical).  p = 0 gives the
+ *    bits of dropout == NULL.  kv_lens together with a dropout of p > 0 is an error (nothing is launched).
  * ------------------------------------------------------------------------------------------------ */
 typedef struct ns2_attn_args {
   const void* q; int64_t q_row_stride, q_batch_stride;
@@ -158,25 +179,19 @@ typedef struct ns2_attn_args {
   float scale;
   float* lse;    /* optional (batches, heads, q_len) f32: log2-domain log-sum-exp of the scaled score rows,
                     saved for ns2_attn_bwd */
+  const int32_t* kv_lens;       /* optional (batches) key counts; NULL = every key */
+  const ns2_dropout* dropout;   /* optional; NULL = no dropout */
 } ns2_attn_args;
 
 int ns2_attn_fwd(const ns2_attn_args* args, ns2_stream_t stream);
 
-/* Key padding for a batch of sequences of different lengths: ns2_attn_fwd where sample b attends to keys
- * [0, kv_lens[b]) only — Attend with a key-padding mask (attend.py:123-129, 140-142: masked scores -> -max, i.e.
- * probability 0), the `mask` that PhonemeEncoder (ns2.py:275), SpeechPromptEncoder's Transformer (ns2.py:1110-1115)
- * and the perceiver / predictor cross attentions (ns2.py:572-577, 457-466) would pass for padded batches.
- *   kv_lens: device int32 (batches); each value is clamped to [1, kv_len] (callers should reject others).
- *   K / V rows at or past kv_lens[b] are never weighted, but they must be FINITE: their probability is exactly 0 and
- *   0 * V is still formed (V = NaN or inf there would reach the output).
- *   Query rows are not masked: rows a caller treats as padding get finite, meaningless output.
- *   Sample b's output rows are bit-identical to ns2_attn_fwd on that sample alone with kv_len = kv_lens[b]. */
-int ns2_attn_fwd_ragged(const ns2_attn_args* args, const int32_t* kv_lens, ns2_stream_t stream);
-
 /* Backward of the above (autograd of F.scaled_dot_product_attention, reached from loss.backward(), ns2.py:1886):
  *   dq_accum (batches, q_len, heads*64) f32, contiguous: dQ is ADDED to it (every key tile adds its share; zero it for
  *   a plain gradient);
- *   dk / dv: bf16, same layout conventions as k / v;  lse from ns2_attn_fwd;  delta: scratch (batches, heads, q_len) f32. */
+ *   dk / dv: bf16, same layout conventions as k / v;  lse from ns2_attn_fwd;  delta: scratch (batches, heads, q_len) f32.
+ *   dropout: the forward's dropout parameters; the mask is regenerated from (seed, site, b, h, q, k):
+ *   dV = (P (.) M)^T dO / (1 - p), dP = (dO V^T) (.) M / (1 - p), dS = P (.) (dP - D), D from the dropped output o.
+ *   p = 0 gives the bits of dropout == NULL. */
 typedef struct ns2_attn_bwd_args {
   const void* q; int64_t q_row_stride, q_batch_stride;
   const void* k; int64_t k_row_stride, k_batch_stride;
@@ -190,6 +205,7 @@ typedef struct ns2_attn_bwd_args {
   void* dv; int64_t dv_row_stride, dv_batch_stride;
   int32_t batches, heads, q_len, kv_len, dim_head;
   float scale;
+  const ns2_dropout* dropout;   /* optional; NULL = no dropout */
 } ns2_attn_bwd_args;
 
 int ns2_attn_bwd(const ns2_attn_bwd_args* args, ns2_stream_t stream);
@@ -198,28 +214,14 @@ int ns2_attn_bwd(const ns2_attn_bwd_args* args, ns2_stream_t stream);
  * 2b. Dropout (training only).  One site's parameters: a 64-bit seed (Philox4x32-10 key = its low / high 32 bits),
  *     the site number (one per dropout site of a forward call, reused by its backward) and the drop probability p.
  *     An element is kept iff its Philox word is >= min(floor(p 2^32 + 0.5), 2^32 - 1) (computed in double from the
- *     float p); kept values are scaled by (float)(1 / (1 - p)).  p must be in [0, 1); p = 0 runs the plain entry point.
+ *     float p); kept values are scaled by (float)(1 / (1 - p)).  p must be in [0, 1); p = 0 is the same as no dropout.
  *     Counter layouts (csrc/philox.cuh):
  *       attention element (b, h, q, k), q' = q & ~8, k' = k & ~8:  ctr = ((k' >> 4) 8 + (k' & 7), (q' >> 4) 8 + (q' & 7),
  *           b heads + h, site); its four words belong to (q', k'), (q', k' + 8), (q' + 8, k'), (q' + 8, k' + 8)
  *       element-wise element i:  ctr = ((i >> 2) & 0xffffffff, i >> 34, 0xffffffff, site); word i & 3
- *    ns2_attn_fwd_dropout : ns2_attn_fwd with dropout on the softmax probabilities (Attend, attend.py:106 SDPA
- *                           dropout_p, attend.py:149 attn_dropout): out = ((P (.) M) V) / (1 - p); lse as without
- *                           dropout (undropped probabilities, bit-identical)
- *    ns2_attn_bwd_dropout : ns2_attn_bwd of that forward, the mask regenerated from (seed, site, b, h, q, k):
- *                           dV = (P (.) M)^T dO / (1 - p), dP = (dO V^T) (.) M / (1 - p), dS = P (.) (dP - D), D from the
- *                           dropped output o
  *    ns2_dropout_f32      : x (n f32, in place) = x * keep * scale — the phoneme encoder's conv dropout
  *                           (nn.Dropout, ns2.py:258) and its backward on the gradient
  * ------------------------------------------------------------------------------------------------ */
-typedef struct ns2_dropout {
-  uint64_t seed;
-  uint32_t site;
-  float p;
-} ns2_dropout;
-
-int ns2_attn_fwd_dropout(const ns2_attn_args* args, const ns2_dropout* dropout, ns2_stream_t stream);
-int ns2_attn_bwd_dropout(const ns2_attn_bwd_args* args, const ns2_dropout* dropout, ns2_stream_t stream);
 int ns2_dropout_f32(float* x, int64_t n, const ns2_dropout* dropout, ns2_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
@@ -253,43 +255,39 @@ int ns2_small_linear(const float* x, int64_t x_row_stride, int32_t batch, int32_
 /* ------------------------------------------------------------------------------------------------
  * 5. Layout / cast helpers (what `rearrange` + autocast do in the reference, ns2.py:972-997).
  *    ns2_cast_bf16        : out_bf16 = (bf16) (x [+ add]) ; add is broadcast over nothing (same shape) or NULL
- *    ns2_mean_rows        : out[b,:] = mean over n of x[b,n,:]   (Reduce('b n d -> b d','mean'), ns2.py:859)
+ *    ns2_mean_rows        : out[b,:] = mean over n < L_b of x[b,n,:]   (Reduce('b n d -> b d','mean'), ns2.py:859);
+ *                           L_b = n when lens is NULL, else lens[b] (device int32 (batch), clamped to [1, n]), summed
+ *                           in row order either way — with lens, the prompt mean-pool of each sample run alone
  *    ns2_transpose_cast   : (B, C, L) f32 channel-first -> (B, L, C) bf16 token-major
  * ------------------------------------------------------------------------------------------------ */
 int ns2_cast_bf16(const float* x, const float* add, int64_t count, void* out_bf16,
                   ns2_stream_t stream);
-int ns2_mean_rows(const float* x, int32_t batch, int32_t n, int32_t dim, float* out,
+int ns2_mean_rows(const float* x, int32_t batch, int32_t n, int32_t dim, float* out, const int32_t* lens,
                   ns2_stream_t stream);
-/*    ns2_mean_rows_ragged : out[b,:] = mean over n < lens[b] of x[b,n,:] (lens: device int32 (batch), clamped to [1, n];
- *                           summed in ns2_mean_rows' order) — the prompt mean-pool (ns2.py:859) of a sample run alone
- *    ns2_mask_rows        : x[b, r, 0:cols] = 0 for lens[b] <= r < rows (lens clamped to [0, rows]), in place; x is f32
+/*    ns2_mask_rows        : x[b, r, 0:cols] = 0 for lens[b] <= r < rows (lens clamped to [0, rows]), in place; x is f32
  *                           (f32 != 0) or bf16 with element strides row_stride / batch_stride — the zero padding past a
  *                           sample's end that a "same" convolution (ns2.py:316-320, 345-365) reads
- *    ns2_pack_rows_ragged : bf16 out[b, r, 0:cols] = a[b, r, :] for r < La, b[b, r - La, :] for La <= r < La + Lb,
+ *    ns2_pack_rows        : bf16 out[b, r, 0:cols] = a[b, r, :] for r < La, b[b, r - La, :] for La <= r < La + Lb,
  *                           0 up to out_rows (La = a_lens[b] clamped to [0, a_rows], Lb = b_lens[b] clamped to
  *                           [0, b_rows]; out_rows >= a_rows + b_rows): the keys [norm(x) ; prompts] of the predictor's
  *                           cross attention (ns2.py:1060-1061) as one prefix of length La + Lb.  cols and every stride
  *                           a multiple of 4, pointers 8-byte aligned. */
-int ns2_mean_rows_ragged(const float* x, int32_t batch, int32_t n, int32_t dim, const int32_t* lens, float* out,
-                         ns2_stream_t stream);
 int ns2_mask_rows(void* x, int32_t f32, int64_t row_stride, int64_t batch_stride, int32_t batch, int32_t rows,
                   int32_t cols, const int32_t* lens, ns2_stream_t stream);
-int ns2_pack_rows_ragged(const void* a, int64_t a_row_stride, int64_t a_batch_stride, int32_t a_rows,
-                         const int32_t* a_lens, const void* b, int64_t b_row_stride, int64_t b_batch_stride,
-                         int32_t b_rows, const int32_t* b_lens, int32_t batch, int32_t cols, void* out,
-                         int64_t out_row_stride, int64_t out_batch_stride, int32_t out_rows, ns2_stream_t stream);
-/*    ns2_cond_inject      : out_bf16[b,n,:] = bf16(x[b,n,:] + c), c = 0 for n >= cond_len (zero padding, ns2.py:70-77),
+int ns2_pack_rows(const void* a, int64_t a_row_stride, int64_t a_batch_stride, int32_t a_rows, const int32_t* a_lens,
+                  const void* b, int64_t b_row_stride, int64_t b_batch_stride, int32_t b_rows, const int32_t* b_lens,
+                  int32_t batch, int32_t cols, void* out, int64_t out_row_stride, int64_t out_batch_stride,
+                  int32_t out_rows, ns2_stream_t stream);
+/*    ns2_cond_inject      : out_bf16[b,n,:] = bf16(x[b,n,:] + c), c = 0 for n >= L_b (zero padding, ns2.py:70-77),
  *                           null_cond[:] where drop_mask[b] (uint8, may be NULL = keep all), else cproj[b,n,:]
- *                           (cproj: projected aligned condition, token-major (batch, cond_len, dim) f32; ns2.py:978-992)
+ *                           (cproj: projected aligned condition, token-major (batch, cond_len, dim) f32; ns2.py:978-992).
+ *                           L_b = cond_len when cond_lens is NULL, else min(cond_len, cond_lens[b]) (device int32
+ *                           (batch), negative = 0): sample b's frames at or past it get nothing, null-substituted or
+ *                           not — the zero padding after the projection of a sample run alone (ns2.py:978-992)
  *    ns2_select_rows      : out[b,:] = drop_mask[b] ? null_row[:] : src[b,:]  (f32 or bf16 out; ns2.py:954-968) */
 int ns2_cond_inject(const float* x, const float* cproj, const uint8_t* drop_mask, const float* null_cond,
-                    int32_t batch, int32_t n, int32_t cond_len, int32_t dim, void* out_bf16, ns2_stream_t stream);
-/*    ns2_cond_inject_ragged : ns2_cond_inject where sample b's condition ends at min(cond_len, cond_lens[b]) (device
- *                             int32 (batch), negative = 0): frames at or past it get nothing, null-substituted or not —
- *                             the zero padding after the projection of a sample run alone (ns2.py:978-992) */
-int ns2_cond_inject_ragged(const float* x, const float* cproj, const uint8_t* drop_mask, const float* null_cond,
-                           int32_t batch, int32_t n, int32_t cond_len, int32_t dim, const int32_t* cond_lens,
-                           void* out_bf16, ns2_stream_t stream);
+                    int32_t batch, int32_t n, int32_t cond_len, int32_t dim, void* out_bf16, const int32_t* cond_lens,
+                    ns2_stream_t stream);
 int ns2_select_rows(const uint8_t* drop_mask, const float* null_row, const float* src, int64_t src_row_stride,
                     int32_t batch, int32_t row_len, void* out, int64_t out_row_stride, int32_t out_bf16,
                     ns2_stream_t stream);
@@ -304,20 +302,16 @@ int ns2_embedding_bf16(const int64_t* ids, int64_t rows, const float* table, int
  *                           statistics per (batch element, group) over rows x channels/groups values, biased variance,
  *                           eps inside the square root, per-channel affine (nn.GroupNorm) - Block.forward of the
  *                           duration / pitch predictor (ns2.py:345-365) with the ResnetBlock residual (ns2.py:399-401).
- *                           Writes out_f32 and/or out_bf16 (either may be NULL).
+ *                           Writes out_f32 and/or out_bf16 (either may be NULL).  lens: NULL = every row, or sample b
+ *                           has lens[b] rows (device int32 (batch), clamped to [1, rows]): the statistics cover rows
+ *                           [0, lens[b]) in the order a call on a tensor of that many rows walks them (bit-identical to
+ *                           it), and rows at or past lens[b] are written as exact zeros to out_f32 and out_bf16 (resid
+ *                           is not read there) — Block's GroupNorm over a sample's own phonemes (ns2.py:345-365)
  *    ns2_rowdot           : out[r] = (relu ?) max(0, .) : (.) of dot(x[r,:], w) + bias[0] - Linear(dim, 1) + ReLU heads
  *                           (ns2.py:452-456) */
 int ns2_groupnorm_silu(const float* x, int32_t batch, int32_t rows, int32_t channels, int32_t groups,
                        const float* weight, const float* bias, float eps, const float* resid, float* out_f32,
-                       void* out_bf16, ns2_stream_t stream);
-/*    ns2_groupnorm_silu_ragged : ns2_groupnorm_silu where sample b has lens[b] rows (device int32 (batch), clamped to
- *                           [1, rows]): the statistics cover rows [0, lens[b]) in the order ns2_groupnorm_silu walks a
- *                           tensor of that many rows (bit-identical to it), and rows at or past lens[b] are written as
- *                           exact zeros to out_f32 and out_bf16 (resid is not read there) — Block's GroupNorm over a
- *                           sample's own phonemes (ns2.py:345-365) */
-int ns2_groupnorm_silu_ragged(const float* x, int32_t batch, int32_t rows, int32_t channels, int32_t groups,
-                              const float* weight, const float* bias, float eps, const float* resid, float* out_f32,
-                              void* out_bf16, const int32_t* lens, ns2_stream_t stream);
+                       void* out_bf16, const int32_t* lens, ns2_stream_t stream);
 int ns2_rowdot(const float* x, int64_t rows, int32_t dim, const float* w, const float* bias, int32_t relu, float* out,
                ns2_stream_t stream);
 /*    ns2_expand_encodings : length regulation, NaturalSpeech2.expand_encodings (ns2.py:1449-1455) with the hard alignment

@@ -21,7 +21,7 @@ NS2_ELU_PAD_ELU, NS2_ELU_PAD_RAW = 1, 2
 NS2_SEANET_TAIL_PARAMS = 3348
 NS2_SEANET_HEAD_PARAMS = 3376
 NS2_ROWDOT_BWD_ROWS = 32
-NS2_ABI_VERSION = 7
+NS2_ABI_VERSION = 8
 
 
 class GemmSeg(C.Structure):
@@ -57,6 +57,10 @@ class WgradArgs(C.Structure):
     ]
 
 
+class Dropout(C.Structure):
+    _fields_ = [("seed", C.c_uint64), ("site", C.c_uint32), ("p", C.c_float)]
+
+
 class AttnArgs(C.Structure):
     _fields_ = [
         ("q", C.c_void_p), ("q_row_stride", C.c_int64), ("q_batch_stride", C.c_int64),
@@ -65,6 +69,7 @@ class AttnArgs(C.Structure):
         ("out", C.c_void_p), ("o_row_stride", C.c_int64), ("o_batch_stride", C.c_int64),
         ("batches", C.c_int32), ("heads", C.c_int32), ("q_len", C.c_int32), ("kv_len", C.c_int32),
         ("dim_head", C.c_int32), ("scale", C.c_float), ("lse", C.c_void_p),
+        ("kv_lens", C.c_void_p), ("dropout", C.POINTER(Dropout)),
     ]
 
 
@@ -79,12 +84,8 @@ class AttnBwdArgs(C.Structure):
         ("dk", C.c_void_p), ("dk_row_stride", C.c_int64), ("dk_batch_stride", C.c_int64),
         ("dv", C.c_void_p), ("dv_row_stride", C.c_int64), ("dv_batch_stride", C.c_int64),
         ("batches", C.c_int32), ("heads", C.c_int32), ("q_len", C.c_int32), ("kv_len", C.c_int32),
-        ("dim_head", C.c_int32), ("scale", C.c_float),
+        ("dim_head", C.c_int32), ("scale", C.c_float), ("dropout", C.POINTER(Dropout)),
     ]
-
-
-class Dropout(C.Structure):
-    _fields_ = [("seed", C.c_uint64), ("site", C.c_uint32), ("p", C.c_float)]
 
 
 _P, _I32, _I64, _F = C.c_void_p, C.c_int32, C.c_int64, C.c_float
@@ -100,28 +101,22 @@ SIGNATURES = {
     "ns2_fold_conv_linear": (C.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P]),
     "ns2_attn_fwd": (C.c_int, [C.POINTER(AttnArgs), _P]),
     "ns2_attn_bwd": (C.c_int, [C.POINTER(AttnBwdArgs), _P]),
-    "ns2_attn_fwd_ragged": (C.c_int, [C.POINTER(AttnArgs), _P, _P]),
-    "ns2_attn_fwd_dropout": (C.c_int, [C.POINTER(AttnArgs), C.POINTER(Dropout), _P]),
-    "ns2_attn_bwd_dropout": (C.c_int, [C.POINTER(AttnBwdArgs), C.POINTER(Dropout), _P]),
     "ns2_dropout_f32": (C.c_int, [_P, _I64, C.POINTER(Dropout), _P]),
     "ns2_rmsnorm_film": (C.c_int, [_P, _I64, _I64, _I32, _I32, _P, _P, _I64, _P, _I64, _P]),
     "ns2_rmsnorm_f32": (C.c_int, [_P, _I64, _I64, _I32, _P, _P, _I64, _P]),
     "ns2_time_cond": (C.c_int, [_P, _I32, _P, _I32, _P, _P, _I32, _P, _I64, _P]),
     "ns2_small_linear": (C.c_int, [_P, _I64, _I32, _I32, _P, _P, _I32, _I32, _P, _I64, _P]),
     "ns2_cast_bf16": (C.c_int, [_P, _P, _I64, _P, _P]),
-    "ns2_mean_rows": (C.c_int, [_P, _I32, _I32, _I32, _P, _P]),
-    "ns2_mean_rows_ragged": (C.c_int, [_P, _I32, _I32, _I32, _P, _P, _P]),
+    "ns2_mean_rows": (C.c_int, [_P, _I32, _I32, _I32, _P, _P, _P]),
     "ns2_mask_rows": (C.c_int, [_P, _I32, _I64, _I64, _I32, _I32, _I32, _P, _P]),
-    "ns2_pack_rows_ragged": (C.c_int, [_P, _I64, _I64, _I32, _P, _P, _I64, _I64, _I32, _P, _I32, _I32, _P, _I64, _I64,
-                                       _I32, _P]),
+    "ns2_pack_rows": (C.c_int, [_P, _I64, _I64, _I32, _P, _P, _I64, _I64, _I32, _P, _I32, _I32, _P, _I64, _I64, _I32,
+                                _P]),
     "ns2_transpose_cast": (C.c_int, [_P, _I32, _I32, _I32, _P, _P]),
-    "ns2_groupnorm_silu": (C.c_int, [_P, _I32, _I32, _I32, _I32, _P, _P, _F, _P, _P, _P, _P]),
-    "ns2_groupnorm_silu_ragged": (C.c_int, [_P, _I32, _I32, _I32, _I32, _P, _P, _F, _P, _P, _P, _P, _P]),
+    "ns2_groupnorm_silu": (C.c_int, [_P, _I32, _I32, _I32, _I32, _P, _P, _F, _P, _P, _P, _P, _P]),
     "ns2_rowdot": (C.c_int, [_P, _I64, _I32, _P, _P, _I32, _P, _P]),
     "ns2_expand_encodings": (C.c_int, [_P, _P, _P, _I32, _P, _I32, _I32, _I32, _I32, _P, _P]),
     "ns2_embedding_bf16": (C.c_int, [_P, _I64, _P, _I32, _I32, _I32, _P, _P]),
-    "ns2_cond_inject": (C.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P]),
-    "ns2_cond_inject_ragged": (C.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P, _P]),
+    "ns2_cond_inject": (C.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P, _P]),
     "ns2_select_rows": (C.c_int, [_P, _P, _P, _I64, _I32, _I32, _P, _I64, _I32, _P]),
     "ns2_q_sample": (C.c_int, [_P, _P, _P, _P, _I32, _I64, _P, _P, _I32, _P]),
     "ns2_mse_rows": (C.c_int, [_P, _P, _I32, _I64, _P, _P, _P, _P]),

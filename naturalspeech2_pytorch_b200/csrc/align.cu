@@ -19,11 +19,7 @@
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
 
-#include <atomic>
-
 namespace ns2 {
-
-extern std::atomic<long long> g_launches;
 
 namespace {
 
@@ -248,7 +244,6 @@ int ns2_maximum_path(const float* value, const float* mask, int32_t batch, int32
   else if (t_x <= 512) rc = launch_dp<16>(value, mask, batch, t_x, t_y, neg_const, dirw, idx, st);
   else rc = launch_dp<32>(value, mask, batch, t_x, t_y, neg_const, dirw, idx, st);
   if (rc != kOk) return rc;
-  g_launches.fetch_add(1, std::memory_order_relaxed);
   if (path != nullptr) {
     const long long total = static_cast<long long>(batch) * t_x * t_y;
     const bool vec = (t_y % 4 == 0) && ((reinterpret_cast<uintptr_t>(mask) | reinterpret_cast<uintptr_t>(path) |
@@ -259,10 +254,8 @@ int ns2_maximum_path(const float* value, const float* mask, int32_t batch, int32
     if (grid > cap) grid = cap;
     if (vec) mas_expand_kernel<4><<<static_cast<unsigned>(grid), 256, 0, st>>>(idx, mask, t_x, t_y, total, path);
     else mas_expand_kernel<1><<<static_cast<unsigned>(grid), 256, 0, st>>>(idx, mask, t_x, t_y, total, path);
-    NS2_CUDA_CHECK(cudaGetLastError());
-    g_launches.fetch_add(1, std::memory_order_relaxed);
   }
-  return kOk;
+  return launched(path != nullptr ? 2 : 1);
 }
 
 }  // extern "C"

@@ -26,11 +26,7 @@
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
 
-#include <atomic>
-
 namespace ns2 {
-
-extern std::atomic<long long> g_launches;
 
 namespace attn {
 constexpr int BQ = 128;   // queries per CTA (64 per softmax warpgroup)
@@ -244,15 +240,27 @@ __global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid
 #undef NS2_ATTN_KV_LEN
 }
 
-// drop == nullptr and kv_lens == nullptr: the plain kernel; drop: attn_fwd_kernel<true, false> with those dropout
-// parameters; kv_lens: attn_fwd_kernel<false, true> (never both).
-static int attn_fwd_launch(const ns2_attn_args* a, const DropoutDev* drop, const int* kv_lens, cudaStream_t stream) {
-  NS2_REQUIRE(a != nullptr && a->q && a->k && a->v && a->out, "attn_fwd: NULL pointer");
+}  // namespace ns2
+
+using namespace ns2;
+
+// No dropout (or p = 0) and no kv_lens: the plain kernel; dropout with p > 0: attn_fwd_kernel<true, false>; kv_lens:
+// attn_fwd_kernel<false, true> (never both).
+extern "C" int ns2_attn_fwd(const ns2_attn_args* a, ns2_stream_t stream_) {
+  NS2_REQUIRE(a != nullptr, "attn_fwd: NULL args");
+  const ns2_dropout* d = a->dropout;
+  DropoutDev drop;
+  NS2_REQUIRE(d == nullptr || make_dropout_dev(d->seed, d->site, d->p, &drop), "attn_fwd: dropout p=%g is not in [0, 1)",
+              static_cast<double>(d->p));
+  const bool dropout = d != nullptr && d->p != 0.0f;
+  NS2_REQUIRE(!(dropout && a->kv_lens), "attn_fwd: kv_lens with dropout p > 0 is not supported");
+  NS2_REQUIRE(a->q && a->k && a->v && a->out, "attn_fwd: NULL pointer");
   NS2_REQUIRE(a->dim_head == 64, "attn_fwd: dim_head=%d, only 64 is supported", a->dim_head);
   NS2_REQUIRE(a->batches > 0 && a->heads > 0 && a->q_len > 0 && a->kv_len > 0, "attn_fwd: empty problem");
   NS2_REQUIRE(a->o_row_stride % 8 == 0 && a->o_batch_stride % 8 == 0 &&
                   (reinterpret_cast<uintptr_t>(a->out) & 15) == 0,
               "attn_fwd: out must be 16-byte aligned with strides multiple of 8");
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   AttnDev dev;
   memset(&dev, 0, sizeof(dev));
   const uint32_t box[3] = {64, attn::BQ, 1};
@@ -280,40 +288,17 @@ static int attn_fwd_launch(const ns2_attn_args* a, const DropoutDev* drop, const
   dev.scale_log2e = a->scale * 1.4426950408889634f;
   dev.lse = a->lse;
   dim3 grid((a->q_len + attn::BQ - 1) / attn::BQ, a->heads, a->batches);
-  if (kv_lens != nullptr) {
-    dev.kv_lens = kv_lens;
+  if (a->kv_lens != nullptr) {
+    dev.kv_lens = a->kv_lens;
     NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<false, true>, attn::SMEM_BYTES));
     attn_fwd_kernel<false, true><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
-  } else if (drop == nullptr) {
+  } else if (!dropout) {
     NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<false, false>, attn::SMEM_BYTES));
     attn_fwd_kernel<false, false><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
   } else {
-    dev.drop = *drop;
+    dev.drop = drop;
     NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<true, false>, attn::SMEM_BYTES));
     attn_fwd_kernel<true, false><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
   }
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
-}
-
-}  // namespace ns2
-
-extern "C" int ns2_attn_fwd(const ns2_attn_args* a, ns2_stream_t stream) {
-  return ns2::attn_fwd_launch(a, nullptr, nullptr, static_cast<cudaStream_t>(stream));
-}
-
-extern "C" int ns2_attn_fwd_ragged(const ns2_attn_args* a, const int32_t* kv_lens, ns2_stream_t stream) {
-  using namespace ns2;
-  NS2_REQUIRE(kv_lens != nullptr, "attn_fwd_ragged: NULL kv_lens");
-  return ns2::attn_fwd_launch(a, nullptr, kv_lens, static_cast<cudaStream_t>(stream));
-}
-
-extern "C" int ns2_attn_fwd_dropout(const ns2_attn_args* a, const ns2_dropout* d, ns2_stream_t stream) {
-  using namespace ns2;
-  NS2_REQUIRE(d != nullptr, "attn_fwd_dropout: NULL dropout parameters");
-  DropoutDev drop;
-  NS2_REQUIRE(make_dropout_dev(d->seed, d->site, d->p, &drop), "attn_fwd_dropout: p=%g is not in [0, 1)",
-              static_cast<double>(d->p));
-  return attn_fwd_launch(a, d->p == 0.0f ? nullptr : &drop, nullptr, static_cast<cudaStream_t>(stream));
+  return launched(1);
 }

@@ -25,11 +25,7 @@
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
 
-#include <atomic>
-
 namespace ns2 {
-
-extern std::atomic<long long> g_launches;
 
 namespace ab {
 constexpr int BQ = 64, BKV = 128, DH = 64;
@@ -291,12 +287,23 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const __nv_bfloat16* __
   }
 }
 
-// drop == nullptr: the plain kernel; otherwise attn_bwd_kernel<true> with those dropout parameters.
-static int attn_bwd_launch(const ns2_attn_bwd_args* a, const DropoutDev* drop, cudaStream_t stream) {
-  NS2_REQUIRE(a != nullptr && a->q && a->k && a->v && a->o && a->d_o && a->lse && a->delta && a->dq_accum && a->dk && a->dv,
+}  // namespace ns2
+
+using namespace ns2;
+
+// No dropout (or p = 0): the plain kernel; otherwise attn_bwd_kernel<true> with those dropout parameters.
+extern "C" int ns2_attn_bwd(const ns2_attn_bwd_args* a, ns2_stream_t stream_) {
+  NS2_REQUIRE(a != nullptr, "attn_bwd: NULL args");
+  const ns2_dropout* d = a->dropout;
+  DropoutDev drop;
+  NS2_REQUIRE(d == nullptr || make_dropout_dev(d->seed, d->site, d->p, &drop), "attn_bwd: dropout p=%g is not in [0, 1)",
+              static_cast<double>(d->p));
+  const bool dropout = d != nullptr && d->p != 0.0f;
+  NS2_REQUIRE(a->q && a->k && a->v && a->o && a->d_o && a->lse && a->delta && a->dq_accum && a->dk && a->dv,
               "attn_bwd: NULL pointer");
   NS2_REQUIRE(a->dim_head == 64, "attn_bwd: dim_head=%d, only 64 is supported", a->dim_head);
   NS2_REQUIRE(a->batches > 0 && a->heads > 0 && a->q_len > 0 && a->kv_len > 0, "attn_bwd: empty problem");
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   // 1. delta = rowsum(dO * O)
   {
     const long long rows = static_cast<long long>(a->batches) * a->q_len;
@@ -334,30 +341,13 @@ static int attn_bwd_launch(const ns2_attn_bwd_args* a, const DropoutDev* drop, c
   dev.scale = a->scale;
   dev.scale_log2e = a->scale * 1.4426950408889634f;
   dim3 grid((a->kv_len + ab::BKV - 1) / ab::BKV, a->heads, a->batches);
-  if (drop == nullptr) {
+  if (!dropout) {
     NS2_CUDA_CHECK(set_max_smem_once(attn_bwd_kernel<false>, ab::SMEM_BYTES));
     attn_bwd_kernel<false><<<grid, ab::THREADS, ab::SMEM_BYTES, stream>>>(dev);
   } else {
-    dev.drop = *drop;
+    dev.drop = drop;
     NS2_CUDA_CHECK(set_max_smem_once(attn_bwd_kernel<true>, ab::SMEM_BYTES_DROPOUT));
     attn_bwd_kernel<true><<<grid, ab::THREADS, ab::SMEM_BYTES_DROPOUT, stream>>>(dev);
   }
-  g_launches.fetch_add(2, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
-}
-
-}  // namespace ns2
-
-extern "C" int ns2_attn_bwd(const ns2_attn_bwd_args* a, ns2_stream_t stream) {
-  return ns2::attn_bwd_launch(a, nullptr, static_cast<cudaStream_t>(stream));
-}
-
-extern "C" int ns2_attn_bwd_dropout(const ns2_attn_bwd_args* a, const ns2_dropout* d, ns2_stream_t stream) {
-  using namespace ns2;
-  NS2_REQUIRE(d != nullptr, "attn_bwd_dropout: NULL dropout parameters");
-  DropoutDev drop;
-  NS2_REQUIRE(make_dropout_dev(d->seed, d->site, d->p, &drop), "attn_bwd_dropout: p=%g is not in [0, 1)",
-              static_cast<double>(d->p));
-  return attn_bwd_launch(a, d->p == 0.0f ? nullptr : &drop, static_cast<cudaStream_t>(stream));
+  return launched(2);
 }

@@ -6,13 +6,10 @@
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
 
-#include <atomic>
 #include <cuda_bf16.h>
 #include <math.h>
 
 namespace ns2 {
-
-extern std::atomic<long long> g_launches;
 
 __device__ __forceinline__ float bwd_warp_sum(float v) {
 #pragma unroll
@@ -405,18 +402,14 @@ extern "C" int ns2_rmsnorm_film_bwd(const float* x, const void* dh_bf16, int64_t
     default: return set_error(kErrInvalidArg, "rmsnorm_film_bwd: unsupported dim %d", dim);
   }
 #undef NS2_CASE
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 extern "C" int ns2_geglu_bwd(void* pre_bf16, const void* dg_bf16, int64_t rows, int32_t dp, ns2_stream_t stream_) {
   NS2_REQUIRE(pre_bf16 && dg_bf16 && rows > 0 && dp > 0 && dp % 128 == 0, "geglu_bwd: bad arguments");
   geglu_bwd_kernel<<<grid_1d(rows * (dp / 2)), 256, 0, static_cast<cudaStream_t>(stream_)>>>(
       reinterpret_cast<uint32_t*>(pre_bf16), reinterpret_cast<const uint32_t*>(dg_bf16), rows, dp);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 extern "C" int ns2_wavenet_gate_bwd(const void* c_bf16, int64_t c_row_stride, const void* dy_bf16, int64_t dy_row_stride,
@@ -435,9 +428,7 @@ extern "C" int ns2_wavenet_gate_bwd(const void* c_bf16, int64_t c_row_stride, co
       reinterpret_cast<const uint2*>(c_bf16), c_row_stride / 4, reinterpret_cast<const uint2*>(dy_bf16), dy_row_stride / 4,
       reinterpret_cast<uint2*>(dc_bf16), dc_row_stride / 4, rows_per_batch, dim, groups, film, film_batch_stride,
       film_group_stride, dfilm, dfilm_batch_stride);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 extern "C" int ns2_colsum_bf16(const void* t_bf16, int64_t rows, int32_t cols, int64_t row_stride, float* out,
@@ -446,9 +437,7 @@ extern "C" int ns2_colsum_bf16(const void* t_bf16, int64_t rows, int32_t cols, i
   dim3 grid((cols / 2 + 255) / 256, static_cast<unsigned>((rows + 255) / 256));
   colsum_bf16_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream_)>>>(reinterpret_cast<const uint32_t*>(t_bf16), rows,
                                                                           cols, row_stride / 2, out);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 extern "C" int ns2_group_sum_bf16(const void* t_bf16, int64_t rows, int32_t dim, int32_t groups, void* out_bf16,
@@ -456,9 +445,7 @@ extern "C" int ns2_group_sum_bf16(const void* t_bf16, int64_t rows, int32_t dim,
   NS2_REQUIRE(t_bf16 && out_bf16 && rows > 0 && dim > 0 && dim % 2 == 0 && groups > 0, "group_sum_bf16: bad arguments");
   group_sum_kernel<<<grid_1d(rows * (dim / 2)), 256, 0, static_cast<cudaStream_t>(stream_)>>>(
       reinterpret_cast<const uint32_t*>(t_bf16), rows, dim / 2, groups, reinterpret_cast<uint32_t*>(out_bf16));
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 extern "C" int ns2_mse_bwd(const float* pred, const float* target, const float* coef, int32_t batch, int64_t per_sample,
@@ -469,18 +456,14 @@ extern "C" int ns2_mse_bwd(const float* pred, const float* target, const float* 
                                                                       reinterpret_cast<const float4*>(target), coef,
                                                                       per_sample / 4, reinterpret_cast<uint2*>(out_bf16),
                                                                       reinterpret_cast<float4*>(out_f32));
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 extern "C" int ns2_accum_bf16(float* acc, const void* t_bf16, int64_t count, void* acc_bf16, ns2_stream_t stream_) {
   NS2_REQUIRE(acc && t_bf16 && count > 0 && count % 4 == 0, "accum_bf16: bad arguments");
   accum_bf16_kernel<<<grid_1d(count / 4), 256, 0, static_cast<cudaStream_t>(stream_)>>>(
       reinterpret_cast<float4*>(acc), reinterpret_cast<const uint2*>(t_bf16), count / 4, reinterpret_cast<uint2*>(acc_bf16));
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 extern "C" int ns2_film_wgrad(const float* dfilm, int64_t dfilm_batch_stride, const float* t, int32_t batch, int64_t rows,
@@ -493,7 +476,5 @@ extern "C" int ns2_film_wgrad(const float* dfilm, int64_t dfilm_batch_stride, co
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (accumulate) film_wgrad_kernel<true><<<grid, 256, smem, st>>>(dfilm, dfilm_batch_stride, t, batch, rows, cols, dw);
   else film_wgrad_kernel<false><<<grid, 256, smem, st>>>(dfilm, dfilm_batch_stride, t, batch, rows, cols, dw);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }

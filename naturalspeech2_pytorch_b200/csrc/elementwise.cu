@@ -6,11 +6,7 @@
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
 
-#include <atomic>
-
 namespace ns2 {
-
-std::atomic<long long> g_launches{0};
 
 // CTAs per SM of the streaming RMSNorm grid: 76 registers -> 3 resident
 // (19.5 us vs 20.1 at 3, 20.5 at 4, 23.3 for one CTA per 8 rows; 32768 x 512 rows, profiles/r02j_rmsnorm_stream.txt)
@@ -147,9 +143,7 @@ static int launch_rmsnorm(const float* x, long long x_rs, long long rows, int di
     NS2_RMS_CASE(7) NS2_RMS_CASE(8)
   }
 #undef NS2_RMS_CASE
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -638,11 +632,9 @@ using namespace ns2;
 
 extern "C" {
 
-int64_t ns2_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
-
-static int groupnorm_silu_launch(const float* x, int32_t batch, int32_t rows, int32_t channels, int32_t groups,
-                                 const float* weight, const float* bias, float eps, const float* resid, float* out_f32,
-                                 void* out_bf16, const int32_t* lens, cudaStream_t stream) {
+int ns2_groupnorm_silu(const float* x, int32_t batch, int32_t rows, int32_t channels, int32_t groups,
+                       const float* weight, const float* bias, float eps, const float* resid, float* out_f32,
+                       void* out_bf16, const int32_t* lens, ns2_stream_t stream_) {
   NS2_REQUIRE(batch >= 0 && rows >= 0 && channels > 0 && groups > 0 && channels % groups == 0,
               "groupnorm_silu: bad sizes");
   NS2_REQUIRE((channels / groups) % 4 == 0, "groupnorm_silu: channels per group (%d) must be a multiple of 4",
@@ -655,6 +647,7 @@ static int groupnorm_silu_launch(const float* x, int32_t batch, int32_t rows, in
                   (reinterpret_cast<uintptr_t>(out_bf16) & 7) == 0,
               "groupnorm_silu: pointers must be 16-byte aligned");
   const dim3 grid(groups, batch);
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (lens != nullptr)
     groupnorm_silu_kernel<true><<<grid, 256, 0, stream>>>(x, rows, channels, channels / groups, weight, bias, eps, resid,
                                                           out_f32, static_cast<__nv_bfloat16*>(out_bf16), lens);
@@ -662,24 +655,7 @@ static int groupnorm_silu_launch(const float* x, int32_t batch, int32_t rows, in
     groupnorm_silu_kernel<false><<<grid, 256, 0, stream>>>(x, rows, channels, channels / groups, weight, bias, eps,
                                                            resid, out_f32, static_cast<__nv_bfloat16*>(out_bf16),
                                                            nullptr);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
-}
-
-int ns2_groupnorm_silu(const float* x, int32_t batch, int32_t rows, int32_t channels, int32_t groups,
-                       const float* weight, const float* bias, float eps, const float* resid, float* out_f32,
-                       void* out_bf16, ns2_stream_t stream) {
-  return groupnorm_silu_launch(x, batch, rows, channels, groups, weight, bias, eps, resid, out_f32, out_bf16, nullptr,
-                               static_cast<cudaStream_t>(stream));
-}
-
-int ns2_groupnorm_silu_ragged(const float* x, int32_t batch, int32_t rows, int32_t channels, int32_t groups,
-                              const float* weight, const float* bias, float eps, const float* resid, float* out_f32,
-                              void* out_bf16, const int32_t* lens, ns2_stream_t stream) {
-  NS2_REQUIRE(lens != nullptr, "groupnorm_silu_ragged: NULL lens");
-  return groupnorm_silu_launch(x, batch, rows, channels, groups, weight, bias, eps, resid, out_f32, out_bf16, lens,
-                               static_cast<cudaStream_t>(stream));
+  return launched(1);
 }
 
 int ns2_mask_rows(void* x, int32_t f32, int64_t row_stride, int64_t batch_stride, int32_t batch, int32_t rows,
@@ -695,34 +671,30 @@ int ns2_mask_rows(void* x, int32_t f32, int64_t row_stride, int64_t batch_stride
   else
     mask_rows_kernel<__nv_bfloat16><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
         static_cast<__nv_bfloat16*>(x), row_stride, batch_stride, rows, cols, lens);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
-int ns2_pack_rows_ragged(const void* a, int64_t a_row_stride, int64_t a_batch_stride, int32_t a_rows,
-                         const int32_t* a_lens, const void* b, int64_t b_row_stride, int64_t b_batch_stride,
-                         int32_t b_rows, const int32_t* b_lens, int32_t batch, int32_t cols, void* out,
-                         int64_t out_row_stride, int64_t out_batch_stride, int32_t out_rows, ns2_stream_t stream) {
-  NS2_REQUIRE(batch >= 0 && a_rows >= 0 && b_rows >= 0 && cols > 0 && out_rows >= 0, "pack_rows_ragged: bad sizes");
-  NS2_REQUIRE(out_rows >= a_rows + b_rows, "pack_rows_ragged: out_rows %d < %d + %d", out_rows, a_rows, b_rows);
-  NS2_REQUIRE(batch <= 65535, "pack_rows_ragged: batch %d > 65535", batch);
+int ns2_pack_rows(const void* a, int64_t a_row_stride, int64_t a_batch_stride, int32_t a_rows, const int32_t* a_lens,
+                  const void* b, int64_t b_row_stride, int64_t b_batch_stride, int32_t b_rows, const int32_t* b_lens,
+                  int32_t batch, int32_t cols, void* out, int64_t out_row_stride, int64_t out_batch_stride,
+                  int32_t out_rows, ns2_stream_t stream) {
+  NS2_REQUIRE(batch >= 0 && a_rows >= 0 && b_rows >= 0 && cols > 0 && out_rows >= 0, "pack_rows: bad sizes");
+  NS2_REQUIRE(out_rows >= a_rows + b_rows, "pack_rows: out_rows %d < %d + %d", out_rows, a_rows, b_rows);
+  NS2_REQUIRE(batch <= 65535, "pack_rows: batch %d > 65535", batch);
   if (batch == 0 || out_rows == 0) return kOk;
-  NS2_REQUIRE(a && b && a_lens && b_lens && out, "pack_rows_ragged: null pointer");
+  NS2_REQUIRE(a && b && a_lens && b_lens && out, "pack_rows: null pointer");
   NS2_REQUIRE(cols % 4 == 0 && a_row_stride % 4 == 0 && a_batch_stride % 4 == 0 && b_row_stride % 4 == 0 &&
                   b_batch_stride % 4 == 0 && out_row_stride % 4 == 0 && out_batch_stride % 4 == 0 &&
                   ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) |
                     reinterpret_cast<uintptr_t>(out)) & 7) == 0,
-              "pack_rows_ragged: columns and strides must be multiples of 4, pointers 8-byte aligned");
+              "pack_rows: columns and strides must be multiples of 4, pointers 8-byte aligned");
   const int c4 = cols / 4;
   const dim3 grid(grid_for(static_cast<long long>(out_rows) * c4) / (batch > 8 ? 4 : 1) + 1, batch);
   pack_rows_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const uint2*>(a), a_row_stride / 4, a_batch_stride / 4, a_rows, a_lens, static_cast<const uint2*>(b),
       b_row_stride / 4, b_batch_stride / 4, b_rows, b_lens, c4, static_cast<uint2*>(out), out_row_stride / 4,
       out_batch_stride / 4, out_rows);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 int ns2_rowdot(const float* x, int64_t rows, int32_t dim, const float* w, const float* bias, int32_t relu, float* out,
@@ -733,9 +705,7 @@ int ns2_rowdot(const float* x, int64_t rows, int32_t dim, const float* w, const 
   NS2_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w)) & 15) == 0, "rowdot: x and w must be 16-byte aligned");
   rowdot_kernel<<<static_cast<unsigned>((rows + 7) / 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, rows, dim, w, bias,
                                                                                                   relu, out);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 int ns2_expand_encodings(const float* phon, const int32_t* coarse, const float* pitch_table, int32_t table_rows,
@@ -749,9 +719,7 @@ int ns2_expand_encodings(const float* phon, const int32_t* coarse, const float* 
   NS2_REQUIRE(grid.y <= 65535, "expand_encodings: dim too large");
   expand_encodings_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(phon, coarse, pitch_table, table_rows, idx,
                                                                               t_text, dim, length, out);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 int ns2_embedding_bf16(const int64_t* ids, int64_t rows, const float* table, int32_t num_rows, int32_t dim,
@@ -765,9 +733,7 @@ int ns2_embedding_bf16(const int64_t* ids, int64_t rows, const float* table, int
   embedding_bf16_kernel<<<grid_for(rows * (dim / 4)), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const long long*>(ids), rows, table, dim, num_rows, pad_id,
       static_cast<__nv_bfloat16*>(out_bf16));
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 int ns2_rmsnorm_film(const float* x, int64_t x_row_stride, int64_t rows, int32_t dim,
@@ -797,9 +763,7 @@ int ns2_small_linear(const float* x, int64_t x_row_stride, int32_t batch, int32_
   NS2_CUDA_CHECK(configure_small_linear());
   small_linear_kernel<<<(n_out + 7) / 8, 256, smem, static_cast<cudaStream_t>(stream)>>>(
       x, x_row_stride, batch, k, nullptr, W, bias, n_out, act, out, out_row_stride);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 int ns2_time_cond(const float* times, int32_t batch, const float* freqs, int32_t half_dim,
@@ -816,9 +780,7 @@ int ns2_time_cond(const float* times, int32_t batch, const float* freqs, int32_t
   // per 1024-thread CTA = one wave of 64 CTAs at n_out = 2048 instead of two waves of 8-feature CTAs (77 -> ~20 us)
   small_linear_kernel<<<(n_out + 31) / 32, 1024, smem, static_cast<cudaStream_t>(stream)>>>(
       times, 1, batch, k, freqs, W, bias, n_out, /*SiLU*/ 1, out, out_row_stride);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 int ns2_cast_bf16(const float* x, const float* add, int64_t count, void* out_bf16,
@@ -828,14 +790,12 @@ int ns2_cast_bf16(const float* x, const float* add, int64_t count, void* out_bf1
   cast_bf16_kernel<<<grid_for(n4), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const float4*>(x), reinterpret_cast<const float4*>(add), n4,
       reinterpret_cast<uint2*>(out_bf16));
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
-static int cond_inject_launch(const float* x, const float* cproj, const uint8_t* drop_mask, const float* null_cond,
-                              int32_t batch, int32_t n, int32_t cond_len, int32_t dim, const int32_t* cond_lens,
-                              void* out_bf16, cudaStream_t stream) {
+int ns2_cond_inject(const float* x, const float* cproj, const uint8_t* drop_mask, const float* null_cond,
+                    int32_t batch, int32_t n, int32_t cond_len, int32_t dim, void* out_bf16, const int32_t* cond_lens,
+                    ns2_stream_t stream) {
   NS2_REQUIRE(x && cproj && out_bf16 && batch > 0 && n > 0 && cond_len > 0 && dim > 0 && dim % 4 == 0,
               "cond_inject: bad arguments");
   NS2_REQUIRE(drop_mask == nullptr || null_cond != nullptr, "cond_inject: a drop mask needs null_cond");
@@ -843,26 +803,10 @@ static int cond_inject_launch(const float* x, const float* cproj, const uint8_t*
                 reinterpret_cast<uintptr_t>(null_cond)) & 15) == 0, "cond_inject: pointers must be 16-byte aligned");
   const long long per4 = static_cast<long long>(n) * (dim / 4);
   dim3 grid(static_cast<unsigned>((per4 + 255) / 256 > 512 ? 512 : (per4 + 255) / 256), batch);
-  cond_inject_kernel<<<grid, 256, 0, stream>>>(
+  cond_inject_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const float4*>(x), reinterpret_cast<const float4*>(cproj), drop_mask,
       reinterpret_cast<const float4*>(null_cond), n, cond_len, cond_lens, dim / 4, reinterpret_cast<uint2*>(out_bf16));
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
-}
-
-int ns2_cond_inject(const float* x, const float* cproj, const uint8_t* drop_mask, const float* null_cond,
-                    int32_t batch, int32_t n, int32_t cond_len, int32_t dim, void* out_bf16, ns2_stream_t stream) {
-  return cond_inject_launch(x, cproj, drop_mask, null_cond, batch, n, cond_len, dim, nullptr, out_bf16,
-                            static_cast<cudaStream_t>(stream));
-}
-
-int ns2_cond_inject_ragged(const float* x, const float* cproj, const uint8_t* drop_mask, const float* null_cond,
-                           int32_t batch, int32_t n, int32_t cond_len, int32_t dim, const int32_t* cond_lens,
-                           void* out_bf16, ns2_stream_t stream) {
-  NS2_REQUIRE(cond_lens != nullptr, "cond_inject_ragged: NULL cond_lens");
-  return cond_inject_launch(x, cproj, drop_mask, null_cond, batch, n, cond_len, dim, cond_lens, out_bf16,
-                            static_cast<cudaStream_t>(stream));
+  return launched(1);
 }
 
 int ns2_select_rows(const uint8_t* drop_mask, const float* null_row, const float* src, int64_t src_row_stride,
@@ -872,30 +816,15 @@ int ns2_select_rows(const uint8_t* drop_mask, const float* null_row, const float
   dim3 grid((row_len + 255) / 256 > 64 ? 64 : (row_len + 255) / 256, batch);
   select_rows_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(drop_mask, null_row, src, src_row_stride,
                                                                           row_len, out, out_row_stride, out_bf16);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
-static int mean_rows_launch(const float* x, int32_t batch, int32_t n, int32_t dim, const int32_t* lens, float* out,
-                            cudaStream_t stream) {
+int ns2_mean_rows(const float* x, int32_t batch, int32_t n, int32_t dim, float* out, const int32_t* lens,
+                  ns2_stream_t stream) {
   NS2_REQUIRE(x && out && batch > 0 && n > 0 && dim > 0, "mean_rows: bad arguments");
   dim3 grid((dim + 255) / 256, batch);
-  mean_rows_kernel<<<grid, 256, 0, stream>>>(x, n, dim, lens, out);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
-}
-
-int ns2_mean_rows(const float* x, int32_t batch, int32_t n, int32_t dim, float* out,
-                  ns2_stream_t stream) {
-  return mean_rows_launch(x, batch, n, dim, nullptr, out, static_cast<cudaStream_t>(stream));
-}
-
-int ns2_mean_rows_ragged(const float* x, int32_t batch, int32_t n, int32_t dim, const int32_t* lens, float* out,
-                         ns2_stream_t stream) {
-  NS2_REQUIRE(lens != nullptr, "mean_rows_ragged: NULL lens");
-  return mean_rows_launch(x, batch, n, dim, lens, out, static_cast<cudaStream_t>(stream));
+  mean_rows_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, n, dim, lens, out);
+  return launched(1);
 }
 
 int ns2_transpose_cast(const float* x, int32_t batch, int32_t channels, int32_t length,
@@ -904,9 +833,7 @@ int ns2_transpose_cast(const float* x, int32_t batch, int32_t channels, int32_t 
   dim3 grid((length + 31) / 32, (channels + 31) / 32, batch);
   transpose_cast_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       x, channels, length, reinterpret_cast<__nv_bfloat16*>(out_bf16));
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 int ns2_q_sample(const float* x0, const float* noise, const float* alpha, const float* sigma,
@@ -919,9 +846,7 @@ int ns2_q_sample(const float* x0, const float* noise, const float* alpha, const 
   q_sample_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const float4*>(x0), reinterpret_cast<const float4*>(noise), alpha, sigma,
       per_sample / 4, reinterpret_cast<float4*>(x_t), reinterpret_cast<float4*>(target), objective);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 int ns2_mse_rows(const float* pred, const float* target, int32_t batch, int64_t per_sample,
@@ -933,13 +858,8 @@ int ns2_mse_rows(const float* pred, const float* target, int32_t batch, int64_t 
       reinterpret_cast<const float4*>(pred), reinterpret_cast<const float4*>(target), per_sample / 4,
       partial);
   mse_final_kernel<<<batch, 64, 0, static_cast<cudaStream_t>(stream)>>>(partial, per_sample, out);
-  g_launches.fetch_add(2, std::memory_order_relaxed);
-  if (mean_out != nullptr) {
-    batch_mean_kernel<<<1, 256, 0, static_cast<cudaStream_t>(stream)>>>(out, batch, mean_out);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-  }
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  if (mean_out != nullptr) batch_mean_kernel<<<1, 256, 0, static_cast<cudaStream_t>(stream)>>>(out, batch, mean_out);
+  return launched(mean_out != nullptr ? 3 : 2);
 }
 
 int ns2_ddim_step(float* x, const float* v, const float* alpha, const float* sigma,
@@ -952,9 +872,7 @@ int ns2_ddim_step(float* x, const float* v, const float* alpha, const float* sig
   ddim_step_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<float4*>(x), reinterpret_cast<const float4*>(v), alpha, sigma, alpha_next,
       sigma_next, per_sample / 4, objective);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 int ns2_x_start(const float* x, const float* pred, const float* alpha, const float* sigma, int32_t batch,
@@ -966,9 +884,7 @@ int ns2_x_start(const float* x, const float* pred, const float* alpha, const flo
   x_start_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const float4*>(x), reinterpret_cast<const float4*>(pred), alpha, sigma, per_sample / 4,
       reinterpret_cast<float4*>(out), objective);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 int ns2_cfg_combine(const float* cond, const float* null_, float scale, int64_t count, float* out,
@@ -977,9 +893,7 @@ int ns2_cfg_combine(const float* cond, const float* null_, float scale, int64_t 
   cfg_combine_kernel<<<grid_for(count / 4), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const float4*>(cond), reinterpret_cast<const float4*>(null_), scale, count / 4,
       reinterpret_cast<float4*>(out));
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 }  // extern "C"

@@ -20,13 +20,10 @@
 #include "philox.cuh"
 #include "../../include/ns2_b200.h"
 
-#include <atomic>
 #include <cuda_bf16.h>
 #include <math.h>
 
 namespace ns2 {
-
-extern std::atomic<long long> g_launches;
 
 namespace {
 
@@ -338,9 +335,7 @@ extern "C" int ns2_silu_bwd(const void* pre_bf16, const void* dout_bf16, int64_t
   silu_bwd_kernel<<<grid_cap(count / 2), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const uint32_t*>(pre_bf16), static_cast<const uint32_t*>(dout_bf16), count / 2,
       static_cast<uint32_t*>(dpre_bf16));
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 extern "C" int ns2_embedding_bwd(const int64_t* ids, int64_t rows, const float* de, int32_t num_rows, int32_t dim,
@@ -351,9 +346,7 @@ extern "C" int ns2_embedding_bwd(const int64_t* ids, int64_t rows, const float* 
   NS2_REQUIRE(ids && de && dtable, "embedding_bwd: null pointer");
   embedding_bwd_kernel<<<grid_cap(rows * dim), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const long long*>(ids), rows, de, dim, num_rows, pad_id, dtable);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 extern "C" int ns2_expand_encodings_bwd(const float* dcond, int64_t dcond_row_stride, const int32_t* coarse,
@@ -368,9 +361,7 @@ extern "C" int ns2_expand_encodings_bwd(const float* dcond, int64_t dcond_row_st
   NS2_REQUIRE(grid.y <= 65535, "expand_encodings_bwd: dim too large");
   expand_encodings_bwd_kernel<<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(
       dcond, dcond_row_stride, dcond_row_stride * length, coarse, table_rows, idx, t_text, dim, length, dphon, dtable);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 extern "C" int ns2_add_rows_bcast(float* x, int32_t batch, int32_t rows, int32_t dim, const float* v, float scale,
@@ -380,9 +371,7 @@ extern "C" int ns2_add_rows_bcast(float* x, int32_t batch, int32_t rows, int32_t
   if (total == 0) return kOk;
   NS2_REQUIRE(x && v, "add_rows_bcast: null pointer");
   add_rows_bcast_kernel<<<grid_cap(total), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, rows, dim, v, scale, total);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 extern "C" int ns2_dropout_f32(float* x, int64_t n, const ns2_dropout* dropout, ns2_stream_t stream) {
@@ -395,9 +384,7 @@ extern "C" int ns2_dropout_f32(float* x, int64_t n, const ns2_dropout* dropout, 
   NS2_REQUIRE(x != nullptr, "dropout_f32: null pointer");
   NS2_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "dropout_f32: x must be 16-byte aligned");
   dropout_f32_kernel<<<grid_cap((n + 3) / 4), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, n, d);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 extern "C" int ns2_groupnorm_silu_bwd(const float* x, int32_t batch, int32_t rows, int32_t channels, int32_t groups,
@@ -425,9 +412,7 @@ extern "C" int ns2_groupnorm_silu_bwd(const float* x, int32_t batch, int32_t row
   NS2_CUDA_CHECK(cudaGetLastError());
   sum_parts_kernel<<<(2 * channels + 255) / 256, 256, 0, st>>>(partial, batch, 2LL * channels, 2 * channels, channels,
                                                                dweight, dbias);
-  g_launches.fetch_add(2, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(2);
 }
 
 extern "C" int ns2_rowdot_bwd(const float* x, int64_t rows, int32_t dim, const float* w, const float* pred,
@@ -449,7 +434,5 @@ extern "C" int ns2_rowdot_bwd(const float* x, int64_t rows, int32_t dim, const f
   rowdot_bwd_kernel<<<static_cast<unsigned>(chunks), 256, 0, st>>>(x, rows, dim, w, pred, dpred, dx, partial);
   NS2_CUDA_CHECK(cudaGetLastError());
   sum_parts_kernel<<<(dim + 1 + 255) / 256, 256, 0, st>>>(partial, chunks, dim + 4LL, dim + 1, dim, dw, db);
-  g_launches.fetch_add(2, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(2);
 }

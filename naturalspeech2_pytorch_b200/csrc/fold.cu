@@ -8,12 +8,9 @@
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
 
-#include <atomic>
 #include <cuda_bf16.h>
 
 namespace ns2 {
-
-extern std::atomic<long long> g_launches;
 
 namespace {
 
@@ -134,7 +131,5 @@ extern "C" int ns2_fold_conv_linear(const float* w2, const float* wc, const floa
             static_cast<unsigned>(layers));
   fold_conv_linear_kernel<<<grid, 256, 0, stream>>>(w2, wc, bc, b2, reinterpret_cast<__nv_bfloat16*>(out_bf16), bias_out,
                                                     o, k, i, taps, i_pad);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }

@@ -18,12 +18,9 @@
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
 
-#include <atomic>
 #include <type_traits>
 
 namespace ns2 {
-
-extern std::atomic<long long> g_launches;
 
 constexpr int BM = 128;
 constexpr int BK = 64;
@@ -419,9 +416,7 @@ static int launch_gemm(const GemmDev& dev, cudaStream_t stream) {
   NS2_CUDA_CHECK(set_max_smem_once(kern, Cfg::SMEM_BYTES));
   const int grid = dev.num_tiles < num_sms() ? dev.num_tiles : num_sms();
   kern<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(dev);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 }  // namespace ns2

@@ -10,6 +10,8 @@
 
 namespace ns2 {
 
+std::atomic<long long> g_launches{0};
+
 static thread_local char g_err[512] = "";
 
 int set_error(int code, const char* fmt, ...) {
@@ -116,4 +118,5 @@ int ns2_set_sm_limit(int sms) {
   const int prev = ns2::g_sm_limit.exchange(sms < 0 ? 0 : (sms & ~1), std::memory_order_relaxed);
   return prev;
 }
+int64_t ns2_launch_count(void) { return ns2::g_launches.load(std::memory_order_relaxed); }
 }

@@ -1,4 +1,4 @@
-// Host-side helpers shared by the C-ABI entry points: error reporting and TMA tensor-map encoding.
+// Host-side helpers shared by the C-ABI entry points: error reporting, launch accounting and TMA tensor-map encoding.
 // The driver API is reached through cudaGetDriverEntryPoint so the library has no link-time dependency
 // on libcuda (it must load, and export its symbols, on a box without a GPU driver).
 #pragma once
@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdarg.h>
+#include <atomic>
 #include <stdio.h>
 
 namespace ns2 {
@@ -42,6 +43,16 @@ int make_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* 
   do {                                                                                        \
     if (!(cond)) return ns2::set_error(ns2::kErrInvalidArg, __VA_ARGS__);                     \
   } while (0)
+
+// Kernel launches issued through the library since load (ns2_launch_count).
+extern std::atomic<long long> g_launches;
+
+// How every entry point ends: count the k kernels it launched, then report a launch that failed.
+inline int launched(int k) {
+  g_launches.fetch_add(k, std::memory_order_relaxed);
+  NS2_CUDA_CHECK(cudaGetLastError());
+  return kOk;
+}
 
 // SM count of the CURRENT device (cached per device ordinal).
 int num_sms();

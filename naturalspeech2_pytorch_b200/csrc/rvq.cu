@@ -27,11 +27,7 @@
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
 
-#include <atomic>
-
 namespace ns2 {
-
-extern std::atomic<long long> g_launches;
 
 namespace rvq {
 constexpr int D = 128;        // latent dimension
@@ -707,9 +703,7 @@ int ns2_rvq_prepare(const float* codebooks, int32_t q, int32_t k, int32_t d, voi
   __half* cb16 = reinterpret_cast<__half*>(cb_f16);
   rvq_prepare_kernel<<<q, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       codebooks, k, d, cb16, cb16 + static_cast<long long>(q) * k * d, cb_norm2, cb_meta);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 int ns2_rvq_encode(const float* frames, int64_t num_frames, int32_t d, const float* codebooks,
@@ -743,9 +737,7 @@ int ns2_rvq_encode(const float* frames, int64_t num_frames, int32_t d, const flo
   NS2_REQUIRE(grid <= 0x7fffffffLL, "rvq_encode: too many frames");
   NS2_CUDA_CHECK(set_max_smem_once(rvq_encode_kernel, rvq::SMEM_BYTES));
   rvq_encode_kernel<<<static_cast<unsigned>(grid), 320, rvq::SMEM_BYTES, static_cast<cudaStream_t>(stream)>>>(dev);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 int ns2_rvq_decode(const int64_t* codes, int64_t num_frames, int32_t q, int32_t k, int32_t d,
@@ -755,9 +747,7 @@ int ns2_rvq_decode(const int64_t* codes, int64_t num_frames, int32_t q, int32_t 
   const long long grid = (num_frames + 7) / 8;
   rvq_decode_kernel<<<static_cast<unsigned>(grid), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const long long*>(codes), num_frames, q, k, codebooks, emb);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 }  // extern "C"

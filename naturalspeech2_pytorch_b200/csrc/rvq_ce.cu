@@ -12,12 +12,9 @@
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
 
-#include <atomic>
 #include <math.h>
 
 namespace ns2 {
-
-extern std::atomic<long long> g_launches;
 
 namespace rvqce {
 constexpr int D = 128;
@@ -428,9 +425,7 @@ extern "C" int ns2_rvq_ce(const float* frames, int64_t num_frames, int32_t d, co
       reinterpret_cast<const long long*>(target_codes), ce_scratch);
   rvq_ce_reduce_kernel<<<1, 256, 0, stream>>>(ce_scratch, reinterpret_cast<const long long*>(target_codes),
                                              num_frames, q, loss);
-  g_launches.fetch_add(2, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(2);
 }
 
 extern "C" int ns2_rvq_ce_bwd(const float* frames, int64_t num_frames, int32_t d, const float* codebooks,
@@ -456,7 +451,5 @@ extern "C" int ns2_rvq_ce_bwd(const float* frames, int64_t num_frames, int32_t d
   rvq_ce_bwd_kernel<<<static_cast<unsigned>(grid), 256, rvqce::SMEM_BWD_BYTES, stream>>>(
       frames, num_frames, codebooks, cb_norm2, q, k, reinterpret_cast<const long long*>(own_codes),
       reinterpret_cast<const long long*>(target_codes), coef_scratch, row_scale, rows_per_sample, d_frames, out_stride);
-  g_launches.fetch_add(2, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(2);
 }

@@ -13,11 +13,7 @@
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
 
-#include <atomic>
-
 namespace ns2 {
-
-extern std::atomic<long long> g_launches;
 
 // ------------------------------------------------------------------------------------------------
 // cluster / distributed shared memory plumbing
@@ -252,9 +248,7 @@ static int launch_lstm(const LstmDev& p, int groups, cudaStream_t stream) {
                      "ns2_lstm_seq: no %d-CTA cluster with %d bytes of shared memory per CTA fits on this device",
                      kLstmCluster, smem);
   NS2_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, p));
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -556,9 +550,7 @@ extern "C" int ns2_elu_pad(const float* x, int64_t x_row_stride, int64_t x_batch
   elu_pad_kernel<<<static_cast<unsigned>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       x, x_row_stride, x_batch_stride, batch, length, channels, pad, flags, static_cast<__nv_bfloat16*>(out_bf16),
       out_row_stride, out_batch_stride);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 extern "C" int ns2_seanet_tail(const float* x, int64_t x_row_stride, int64_t x_batch_stride, int32_t batch,
@@ -578,9 +570,7 @@ extern "C" int ns2_seanet_tail(const float* x, int64_t x_row_stride, int64_t x_b
   seanet_tail_kernel<<<grid, kTailThreads, smem, static_cast<cudaStream_t>(stream)>>>(x, x_row_stride, x_batch_stride,
                                                                                       length, params, out,
                                                                                       out_batch_stride);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }
 
 extern "C" int ns2_seanet_head(const float* x, int64_t x_batch_stride, int32_t batch, int32_t length,
@@ -605,7 +595,5 @@ extern "C" int ns2_seanet_head(const float* x, int64_t x_batch_stride, int32_t b
   const dim3 grid((length + kHeadOut - 1) / kHeadOut, batch);
   seanet_head_kernel<<<grid, kHeadThreads, smem, static_cast<cudaStream_t>(stream)>>>(
       x, x_batch_stride, length, params, static_cast<__nv_bfloat16*>(out_bf16), out_row_stride, out_batch_stride);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }

@@ -20,11 +20,7 @@
 #include "host_common.h"
 #include "../../include/ns2_b200.h"
 
-#include <atomic>
-
 namespace ns2 {
-
-extern std::atomic<long long> g_launches;
 
 namespace wg {
 constexpr int BM = 128;           // dW rows per tile (output channels n)
@@ -224,7 +220,5 @@ extern "C" int ns2_wgrad(const ns2_wgrad_args* a, ns2_stream_t stream_) {
     NS2_CUDA_CHECK(set_max_smem_once(wgrad_kernel<128>, wg::Cfg<128>::SMEM_BYTES));
     wgrad_kernel<128><<<grid, wg::THREADS, wg::Cfg<128>::SMEM_BYTES, stream>>>(dev);
   }
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  NS2_CUDA_CHECK(cudaGetLastError());
-  return kOk;
+  return launched(1);
 }

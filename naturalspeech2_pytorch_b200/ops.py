@@ -209,7 +209,7 @@ DropoutSpec = Tuple[int, int, float]   # (64-bit seed, site, p)
 
 
 def _dropout_args(dropout: Optional[DropoutSpec]) -> Optional["_lib.Dropout"]:
-    """ctypes parameters of `dropout`, or None when it draws nothing (None or p = 0: the plain entry point runs)."""
+    """ctypes parameters of `dropout`, or None when it draws nothing (None or p = 0: no dropout)."""
     if dropout is None:
         return None
     seed, site, p = dropout
@@ -312,9 +312,8 @@ def pack_rows(a: torch.Tensor, a_lens: torch.Tensor, b: torch.Tensor, b_lens: to
         raise ValueError(f"out holds {No} rows, fewer than {Na} + {Nb}")
     ap = _check_lens(a_lens, B, 0, Na, "a_lens")
     bp = _check_lens(b_lens, B, 0, Nb, "b_lens")
-    check(lib.ns2_pack_rows_ragged(a.data_ptr(), a.stride(1), a.stride(0), Na, ap, b.data_ptr(), b.stride(1),
-                                   b.stride(0), Nb, bp, B, Cc, out.data_ptr(), out.stride(1), out.stride(0), No,
-                                   _stream(out)), "ns2_pack_rows_ragged")
+    check(lib.ns2_pack_rows(a.data_ptr(), a.stride(1), a.stride(0), Na, ap, b.data_ptr(), b.stride(1), b.stride(0), Nb,
+                            bp, B, Cc, out.data_ptr(), out.stride(1), out.stride(0), No, _stream(out)), "ns2_pack_rows")
     return out
 
 
@@ -350,14 +349,10 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tens
         _req(lse, torch.float32, "lse")
         if not lse.is_contiguous() or tuple(lse.shape) != (q.shape[0], heads, q.shape[1]):
             raise ValueError("lse must be a contiguous (B, heads, Nq) float tensor")
-    args.lse = _ptr(lse)
+    args.lse, args.kv_lens = _ptr(lse), lens_ptr
     d = _dropout_args(dropout)
-    if lens_ptr is not None:
-        check(lib.ns2_attn_fwd_ragged(C.byref(args), lens_ptr, _stream(out)), "ns2_attn_fwd_ragged")
-    elif d is None:
-        check(lib.ns2_attn_fwd(C.byref(args), _stream(out)), "ns2_attn_fwd")
-    else:
-        check(lib.ns2_attn_fwd_dropout(C.byref(args), C.byref(d), _stream(out)), "ns2_attn_fwd_dropout")
+    args.dropout = None if d is None else C.pointer(d)
+    check(lib.ns2_attn_fwd(C.byref(args), _stream(out)), "ns2_attn_fwd")
     return out
 
 
@@ -468,13 +463,9 @@ def cond_inject(x: torch.Tensor, cproj: torch.Tensor, out: torch.Tensor, drop_ma
         _req(null_cond, torch.float32, "null_cond")
         if null_cond.numel() != D or not null_cond.is_contiguous():
             raise ValueError("null_cond must be a contiguous (D,) float tensor")
-    if cond_lens is None:
-        check(lib.ns2_cond_inject(x.data_ptr(), cproj.data_ptr(), _ptr(drop_mask), _ptr(null_cond), B, N, cproj.shape[1],
-                                  D, out.data_ptr(), _stream(out)), "ns2_cond_inject")
-        return out
-    lp = _check_lens(cond_lens, B, 0, None, "cond_lens")
-    check(lib.ns2_cond_inject_ragged(x.data_ptr(), cproj.data_ptr(), _ptr(drop_mask), _ptr(null_cond), B, N,
-                                     cproj.shape[1], D, lp, out.data_ptr(), _stream(out)), "ns2_cond_inject_ragged")
+    lp = None if cond_lens is None else _check_lens(cond_lens, B, 0, None, "cond_lens")
+    check(lib.ns2_cond_inject(x.data_ptr(), cproj.data_ptr(), _ptr(drop_mask), _ptr(null_cond), B, N, cproj.shape[1], D,
+                              out.data_ptr(), lp, _stream(out)), "ns2_cond_inject")
     return out
 
 
@@ -507,15 +498,10 @@ def mean_rows(x: torch.Tensor, out: torch.Tensor, *, lens: Optional[torch.Tensor
     _req(x, torch.float32, "x")
     _req(out, torch.float32, "out")
     B, N, D = x.shape
-    if lens is None:
-        check(lib.ns2_mean_rows(x.contiguous().data_ptr(), B, N, D, out.data_ptr(), _stream()),
-              "ns2_mean_rows")
-        return out
-    lp = _check_lens(lens, B, 1, N, "lens")
+    lp = None if lens is None else _check_lens(lens, B, 1, N, "lens")
     if not out.is_contiguous() or tuple(out.shape) != (B, D):
         raise ValueError(f"out must be a contiguous ({B}, {D}) tensor")
-    check(lib.ns2_mean_rows_ragged(x.contiguous().data_ptr(), B, N, D, lp, out.data_ptr(), _stream()),
-          "ns2_mean_rows_ragged")
+    check(lib.ns2_mean_rows(x.contiguous().data_ptr(), B, N, D, out.data_ptr(), lp, _stream()), "ns2_mean_rows")
     return out
 
 
@@ -557,14 +543,9 @@ def groupnorm_silu(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, gr
     if out_f32 is None and out_bf16 is None:
         raise ValueError("groupnorm_silu needs at least one output")
     B, N, Cn = x.shape
-    if lens is None:
-        check(lib.ns2_groupnorm_silu(x.data_ptr(), B, N, Cn, int(groups), weight.data_ptr(), bias.data_ptr(), float(eps),
-                                     _ptr(resid), _ptr(out_f32), _ptr(out_bf16), _stream(x)), "ns2_groupnorm_silu")
-        return out_f32, out_bf16
-    lp = _check_lens(lens, B, 1, N, "lens")
-    check(lib.ns2_groupnorm_silu_ragged(x.data_ptr(), B, N, Cn, int(groups), weight.data_ptr(), bias.data_ptr(),
-                                        float(eps), _ptr(resid), _ptr(out_f32), _ptr(out_bf16), lp, _stream(x)),
-          "ns2_groupnorm_silu_ragged")
+    lp = None if lens is None else _check_lens(lens, B, 1, N, "lens")
+    check(lib.ns2_groupnorm_silu(x.data_ptr(), B, N, Cn, int(groups), weight.data_ptr(), bias.data_ptr(), float(eps),
+                                 _ptr(resid), _ptr(out_f32), _ptr(out_bf16), lp, _stream(x)), "ns2_groupnorm_silu")
     return out_f32, out_bf16
 
 
@@ -858,10 +839,8 @@ def attention_bwd(q, k, v, o, d_o, lse, dq_accum, dk, dv, *, heads: int, scale: 
     a.batches, a.heads, a.q_len, a.kv_len, a.dim_head = B, heads, Nq, Nk, 64
     a.scale = float(scale if scale is not None else 64 ** -0.5)
     d = _dropout_args(dropout)
-    if d is None:
-        check(lib.ns2_attn_bwd(C.byref(a), _stream(dq_accum)), "ns2_attn_bwd")
-    else:
-        check(lib.ns2_attn_bwd_dropout(C.byref(a), C.byref(d), _stream(dq_accum)), "ns2_attn_bwd_dropout")
+    a.dropout = None if d is None else C.pointer(d)
+    check(lib.ns2_attn_bwd(C.byref(a), _stream(dq_accum)), "ns2_attn_bwd")
     return dq_accum, dk, dv
 
 

@@ -59,7 +59,7 @@ def test_argument_validation_without_gpu(lib):
     assert lib.ns2_maximum_path(1, 1, 2, 2000, 16, float("-inf"), 1, 1 << 20, 1, None, None) < 0
     assert b"1024" in lib.ns2_last_error()
     assert lib.ns2_maximum_path(None, None, 0, 10, 10, float("-inf"), None, 0, None, None, None) == 0   # empty batch
-    assert lib.ns2_groupnorm_silu(None, 2, 8, 100, 8, None, None, 1e-5, None, None, None, None) < 0       # 100 % 8 != 0
+    assert lib.ns2_groupnorm_silu(None, 2, 8, 100, 8, None, None, 1e-5, None, None, None, None, None) < 0  # 100 % 8 != 0
     assert lib.ns2_rowdot(None, 4, 10, None, None, 0, None, None) < 0                                     # dim % 4 != 0
     assert lib.ns2_embedding_bf16(None, 4, None, 10, 128, 10, None, None) < 0                             # pad_id outside
     assert lib.ns2_film_wgrad(None, 8, None, 33, 8, 8, None, 0, None) < 0
@@ -84,11 +84,15 @@ def test_rvq_rejects_unsupported_codebook_size_before_launch(lib, k):
 def test_struct_layout_matches_header():
     """ctypes mirrors of the C structs: sizes are what a C compiler produces for include/ns2_b200.h."""
     import subprocess, tempfile, textwrap
-    from naturalspeech2_pytorch_b200._lib import GemmArgs, AttnArgs, GemmSeg
+    from naturalspeech2_pytorch_b200._lib import GemmArgs, AttnArgs, AttnBwdArgs, GemmSeg
     src = textwrap.dedent('''
         #include <stdio.h>
         #include "ns2_b200.h"
-        int main(void) { printf("%zu %zu %zu\\n", sizeof(ns2_gemm_seg), sizeof(ns2_gemm_args), sizeof(ns2_attn_args)); return 0; }
+        int main(void) {
+          printf("%zu %zu %zu %zu\\n", sizeof(ns2_gemm_seg), sizeof(ns2_gemm_args), sizeof(ns2_attn_args),
+                 sizeof(ns2_attn_bwd_args));
+          return 0;
+        }
     ''')
     with tempfile.TemporaryDirectory() as d:
         c = Path(d) / "t.c"
@@ -96,7 +100,8 @@ def test_struct_layout_matches_header():
         exe = Path(d) / "t"
         subprocess.run(["gcc", "-I", str(ROOT / "include"), str(c), "-o", str(exe)], check=True)
         out = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()
-    assert [int(v) for v in out] == [ctypes.sizeof(GemmSeg), ctypes.sizeof(GemmArgs), ctypes.sizeof(AttnArgs)]
+    assert [int(v) for v in out] == [ctypes.sizeof(GemmSeg), ctypes.sizeof(GemmArgs), ctypes.sizeof(AttnArgs),
+                                     ctypes.sizeof(AttnBwdArgs)]
 
 
 def test_ops_reject_cpu_tensors():

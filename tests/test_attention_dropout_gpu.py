@@ -205,7 +205,7 @@ def test_sensitivity_shifted_mask_and_wrong_site():
 
 
 def _raw_calls(q, k, v, o, d_o, lse, dq, dk, dv, H, drop):
-    """ns2_attn_fwd_dropout / ns2_attn_bwd_dropout called directly (ops routes p = 0 to the plain entry points)."""
+    """ns2_attn_fwd / ns2_attn_bwd called directly with the dropout field set (ops passes NULL for p = 0)."""
     from naturalspeech2_pytorch_b200 import _lib
     lib = _lib.load()
     stream = torch.cuda.current_stream().cuda_stream
@@ -217,7 +217,8 @@ def _raw_calls(q, k, v, o, d_o, lse, dq, dk, dv, H, drop):
     a.batches, a.heads, a.q_len, a.kv_len, a.dim_head, a.scale = q.shape[0], H, q.shape[1], k.shape[1], 64, 0.125
     a.lse = lse.data_ptr()
     d = _lib.Dropout(*drop)
-    _lib.check(lib.ns2_attn_fwd_dropout(ctypes.byref(a), ctypes.byref(d), stream), "ns2_attn_fwd_dropout")
+    a.dropout = ctypes.pointer(d)
+    _lib.check(lib.ns2_attn_fwd(ctypes.byref(a), stream), "ns2_attn_fwd")
     g = _lib.AttnBwdArgs()
     for n, t in (("q", q), ("k", k), ("v", v), ("o", o), ("d_o", d_o)):
         setattr(g, n, t.data_ptr())
@@ -231,11 +232,12 @@ def _raw_calls(q, k, v, o, d_o, lse, dq, dk, dv, H, drop):
     g.dk, g.dk_row_stride, g.dk_batch_stride = dk.data_ptr(), dk.stride(1), dk.stride(0)
     g.dv, g.dv_row_stride, g.dv_batch_stride = dv.data_ptr(), dv.stride(1), dv.stride(0)
     g.batches, g.heads, g.q_len, g.kv_len, g.dim_head, g.scale = q.shape[0], H, q.shape[1], k.shape[1], 64, 0.125
-    _lib.check(lib.ns2_attn_bwd_dropout(ctypes.byref(g), ctypes.byref(d), stream), "ns2_attn_bwd_dropout")
+    g.dropout = ctypes.pointer(d)
+    _lib.check(lib.ns2_attn_bwd(ctypes.byref(g), stream), "ns2_attn_bwd")
 
 
 def test_p0_entry_points_bit_identical_and_repeatable():
-    """p = 0 through the dropout entry points = the plain kernels; the same dropout arguments twice = the same bits."""
+    """dropout p = 0 = no dropout, bit for bit; the same dropout arguments twice = the same bits."""
     B, H, Nq, Nk = 2, 4, 300, 257
     q, k, v, d_o = _inputs(B, H, Nq, Nk, seed=8)
     plain = _run(q, k, v, d_o, H, None)

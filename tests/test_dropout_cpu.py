@@ -75,9 +75,9 @@ def test_entry_points_reject_bad_p_before_launch(lib):
     before = lib.ns2_launch_count()
     for p in (-0.5, 1.0, float("nan")):
         d = Dropout(1, 0, p)
-        assert lib.ns2_attn_fwd_dropout(ctypes.byref(AttnArgs()), ctypes.byref(d), None) < 0
+        assert lib.ns2_attn_fwd(ctypes.byref(AttnArgs(dropout=ctypes.pointer(d))), None) < 0
         assert b"[0, 1)" in lib.ns2_last_error()
-        assert lib.ns2_attn_bwd_dropout(ctypes.byref(AttnBwdArgs()), ctypes.byref(d), None) < 0
+        assert lib.ns2_attn_bwd(ctypes.byref(AttnBwdArgs(dropout=ctypes.pointer(d))), None) < 0
         assert b"[0, 1)" in lib.ns2_last_error()
         assert lib.ns2_dropout_f32(16, 4, ctypes.byref(d), None) < 0
         assert b"[0, 1)" in lib.ns2_last_error()
@@ -105,7 +105,7 @@ def test_dropout_struct_matches_header():
         subprocess.run(["gcc", "-I", str(ROOT / "include"), str(c), "-o", str(exe)], check=True)
         out = [int(v) for v in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
     assert out[:4] == [ctypes.sizeof(Dropout), Dropout.seed.offset, Dropout.site.offset, Dropout.p.offset]
-    assert out[4] == 7
+    assert out[4] == 8
 
 
 def test_train_dropout_defaults_off_and_conditioner_plumbs_it():

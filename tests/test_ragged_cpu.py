@@ -16,27 +16,31 @@ def lib():
 def test_entry_points_reject_bad_arguments(lib):
     from naturalspeech2_pytorch_b200._lib import AttnArgs
     before = lib.ns2_launch_count()
-    a = AttnArgs()
-    assert lib.ns2_attn_fwd_ragged(ctypes.byref(a), None, None) < 0
-    assert b"kv_lens" in lib.ns2_last_error()
-    assert lib.ns2_attn_fwd_ragged(ctypes.byref(a), 16, None) < 0          # NULL q / k / v / out
-    assert lib.ns2_attn_fwd_ragged(None, 16, None) < 0
-    assert lib.ns2_groupnorm_silu_ragged(16, 2, 8, 64, 8, 16, 16, 1e-5, None, 16, None, None, None) < 0
-    assert b"lens" in lib.ns2_last_error()
-    assert lib.ns2_groupnorm_silu_ragged(16, 2, 8, 100, 8, 16, 16, 1e-5, None, 16, None, 16, None) < 0   # 100 % 8
-    assert lib.ns2_mean_rows_ragged(16, 2, 8, 64, None, 16, None) < 0
-    assert lib.ns2_mean_rows_ragged(None, 2, 8, 64, 16, 16, None) < 0
-    assert lib.ns2_cond_inject_ragged(16, 16, None, None, 2, 8, 8, 64, None, 16, None) < 0
-    assert lib.ns2_cond_inject_ragged(16, 16, 16, None, 2, 8, 8, 64, 16, 16, None) < 0   # drop mask without null_cond
+    a = AttnArgs(kv_lens=16)
+    assert lib.ns2_attn_fwd(ctypes.byref(a), None) < 0                     # NULL q / k / v / out
+    assert lib.ns2_attn_fwd(None, None) < 0
+    assert lib.ns2_groupnorm_silu(16, 2, 8, 100, 8, 16, 16, 1e-5, None, 16, None, 16, None) < 0   # 100 % 8
+    assert lib.ns2_mean_rows(None, 2, 8, 64, 16, 16, None) < 0
+    assert lib.ns2_cond_inject(16, 16, 16, None, 2, 8, 8, 64, 16, 16, None) < 0   # drop mask without null_cond
     assert lib.ns2_mask_rows(16, 1, 64, 512, 2, 8, 64, None, None) < 0
     assert lib.ns2_mask_rows(16, 1, 32, 512, 2, 8, 64, 16, None) < 0                    # row stride < cols
     assert lib.ns2_mask_rows(None, 1, 64, 512, 0, 8, 64, None, None) == 0               # empty: nothing to do
     args = (16, 64, 640, 10, 16, 16, 64, 640, 10, 16, 2, 64, 16, 64, 1280)
-    assert lib.ns2_pack_rows_ragged(*args, 19, None) < 0                                 # out_rows < 10 + 10
-    assert lib.ns2_pack_rows_ragged(*args[:4], None, *args[5:], 20, None) < 0            # NULL a_lens
+    assert lib.ns2_pack_rows(*args, 19, None) < 0                                        # out_rows < 10 + 10
+    assert lib.ns2_pack_rows(*args[:4], None, *args[5:], 20, None) < 0                   # NULL a_lens
     bad_cols = args[:11] + (62,) + args[12:]
-    assert lib.ns2_pack_rows_ragged(*bad_cols, 20, None) < 0
+    assert lib.ns2_pack_rows(*bad_cols, 20, None) < 0
     assert b"multiples of 4" in lib.ns2_last_error()
+    assert lib.ns2_launch_count() == before
+
+
+def test_attention_rejects_kv_lens_with_dropout(lib):
+    """Key padding has no dropout kernel: ns2_attn_fwd refuses kv_lens with a dropout of p > 0 before it launches."""
+    from naturalspeech2_pytorch_b200._lib import AttnArgs, Dropout
+    before = lib.ns2_launch_count()
+    d = Dropout(1, 0, 0.5)
+    assert lib.ns2_attn_fwd(ctypes.byref(AttnArgs(kv_lens=16, dropout=ctypes.pointer(d))), None) < 0
+    assert b"kv_lens" in lib.ns2_last_error()
     assert lib.ns2_launch_count() == before
 
 

@@ -13,16 +13,17 @@ unchanged; the module tree only HOLDS parameters, the math goes through `ops` (l
   Transformer layer               RMSNorm kernel -> fused QKV GEMM -> flash attention -> out-proj GEMM (+residual,
                                   fp32 stream) -> RMSNorm -> GEGLU GEMM -> out GEMM (+residual)
 
-Training: in `train()` mode with gradients enabled (and parameters that require them) `SpeechPromptEncoder.forward` and
-`PhonemeEncoder.forward` record ONE autograd node each (`_EncoderFunction`, the pattern of training.DenoiserFunction).
-Its forward is the inference forward (`_forward` and `_transformer`) given a `saved` dict, which keeps the activations
-the backward needs (bit-identical output); its backward walks the encoder in reverse:
+Training: in `train()` mode with gradients enabled (and parameters or a float input that require them)
+`SpeechPromptEncoder.forward` and `PhonemeEncoder.forward` record ONE autograd node each (`_EncoderFunction`, the
+pattern of training.DenoiserFunction).  Its forward is the inference forward (`_forward` and `_transformer`) given a
+`saved` dict, which keeps the activations the backward needs (bit-identical output); its backward walks the encoder in
+reverse:
   plain Transformer      training.ff_backward and training.attention_backward (shared with the denoiser's backward)
                          on the transposed packs, rmsnorm_film_bwd(gamma=...)
   k=9 conv + SiLU        pre-activation recomputed with a plain-epilogue GEMM, ops.silu_bwd, then training.conv_backward:
                          one ops.wgrad per tap ("same" padding: shifts +4..-4, causal: 8..0), dgrad = one nine-segment
-                         GEMM with mirrored shifts (the prompt encoder's first conv needs none: its input comes from the
-                         codec)
+                         GEMM with mirrored shifts (the prompt encoder's first conv only when the prompt requires grad:
+                         it usually comes from the codec)
   nn.Embedding           ops.embedding_bwd (scatter-add; the pad row receives gradient, as in the reference)
 Dropout: with `train_dropout` set (default False; `Conditioner(train_dropout=True)` sets it on both encoders) a call
 in train() mode - with or without autograd, like nn.Dropout - draws the reference's dropout: every transformer layer's
@@ -235,11 +236,17 @@ class _EncoderBase(_PackedCache):
         ops.silu_bwd(pre, d_out)                                                                  # pre <- d pre
         return conv_backward(pre, x_in, grads, name, w_t, k, first_shift, dtype=dtype)
 
-    def _ragged_lengths(self, lengths, batch: int, n: int, device, name: str) -> Optional[torch.Tensor]:
+    def _records(self, *inputs) -> bool:
+        """Whether a call records the `_EncoderFunction` node: train mode with gradients on, and a parameter or an input
+        that requires grad (with every parameter frozen the node still carries the inputs' gradients)."""
+        return _records_graph(self) or (self.training and torch.is_grad_enabled() and
+                                        any(t.requires_grad for t in inputs))
+
+    def _ragged_lengths(self, lengths, batch: int, n: int, device, name: str, *inputs) -> Optional[torch.Tensor]:
         """Validated int32 device lengths of a sampling call (None stays None).  Lengths are for inference only."""
         if lengths is None:
             return None
-        if _records_graph(self) or (self.training and self.train_dropout):
+        if self._records(*inputs) or (self.training and self.train_dropout):
             raise NotImplementedError(f"{type(self).__name__}: {name} are supported for sampling only (no autograd, no "
                                       "dropout)")
         return ops.lengths(lengths, batch, n, device=device, name=name)
@@ -293,7 +300,7 @@ class SpeechPromptEncoder(_EncoderBase):
         return P
 
     def _pack_transposed(self, P) -> Dict[str, torch.Tensor]:
-        T = {f"c{i}_w": _transpose_conv(P[f"c{i}_w"], self.kernel_size) for i in range(1, len(self._convs()))}
+        T = {f"c{i}_w": _transpose_conv(P[f"c{i}_w"], self.kernel_size) for i in range(len(self._convs()))}
         self._pack_transposed_transformer(P, T, len(self.transformer.layers))
         return T
 
@@ -301,8 +308,8 @@ class SpeechPromptEncoder(_EncoderBase):
         assert x.shape[-1] == self.dim
         if not x.is_cuda:
             raise ValueError("SpeechPromptEncoder: input must be a CUDA tensor (the ns2_b200 ops have no CPU path)")
-        lens = self._ragged_lengths(lengths, x.shape[0], x.shape[1], x.device, "lengths")
-        if _records_graph(self):
+        lens = self._ragged_lengths(lengths, x.shape[0], x.shape[1], x.device, "lengths", x)
+        if self._records(x):
             return _EncoderFunction.apply(self, self.grad_reducer, x, *self.parameters())
         with torch.no_grad():
             return self._forward(x, lens=lens)
@@ -334,6 +341,10 @@ class SpeechPromptEncoder(_EncoderBase):
         out = self._transformer(h, self.transformer, P, self.heads, saved, seed, kv_lens=lens)
         return out if lens is None else ops.mask_rows(out, lens)
 
+    def _train_forward(self, x: torch.Tensor):
+        saved = {"x_requires_grad": x.requires_grad, "x_dtype": x.dtype}
+        return self._forward(x, saved), saved
+
     def _train_backward(self, S, d_out: torch.Tensor) -> Dict[str, torch.Tensor]:
         P, T = self.packed(), self.packed_transposed()
         grads: Dict[str, torch.Tensor] = {}
@@ -341,10 +352,16 @@ class SpeechPromptEncoder(_EncoderBase):
         self._transformer_backward(S["layers"], self.transformer, P, T, self.heads, dxr, dxr_bf, grads,
                                    S["dropout_seed"])
         d_h = dxr_bf                        # gradient of the last conv's (SiLU) output
+        need_dx = S["x_requires_grad"]
         for i in reversed(range(len(self._convs()))):
-            # conv i is module conv.{2i+1} (Rearrange, then [Conv1d, SiLU] pairs); its input needs no gradient for i = 0
-            d_h = self._conv_silu_backward(S["conv_in"][i], P[f"c{i}_w"], T.get(f"c{i}_w"), P[f"c{i}_b"], d_h,
-                                           self.padding, grads, f"conv.{2 * i + 1}")
+            # conv i is module conv.{2i+1} (Rearrange, then [Conv1d, SiLU] pairs); conv 0's d x (fp32) only when the
+            # prompt requires grad (it usually comes from the codec)
+            first = i == 0
+            w_t = T[f"c{i}_w"] if need_dx or not first else None
+            d_h = self._conv_silu_backward(S["conv_in"][i], P[f"c{i}_w"], w_t, P[f"c{i}_b"], d_h, self.padding, grads,
+                                           f"conv.{2 * i + 1}", dtype=torch.float32 if first else torch.bfloat16)
+        if need_dx:
+            grads[_INPUT_GRADS] = (d_h.to(S["x_dtype"]),)
         return grads
 
 
@@ -394,7 +411,7 @@ class PhonemeEncoder(_EncoderBase):
         if not x.is_cuda:
             raise ValueError("PhonemeEncoder: input must be a CUDA tensor (the ns2_b200 ops have no CPU path)")
         lens = self._ragged_lengths(lengths, x.shape[0], x.shape[1], x.device, "lengths")
-        if _records_graph(self):
+        if self._records():   # ids have no gradient
             return _EncoderFunction.apply(self, self.grad_reducer, x, *self.parameters())
         with torch.no_grad():
             return self._forward(x, lens=lens)
@@ -688,11 +705,12 @@ class DurationPitchPredictor(_EncoderBase):
         if lengths is not None or prompt_lens is not None:
             B, T = x.shape[:2]
             Np = encoded_prompts.shape[1]
-            lens = self._ragged_lengths(lengths if lengths is not None else [T] * B, B, T, x.device, "lengths")
+            lens = self._ragged_lengths(lengths if lengths is not None else [T] * B, B, T, x.device, "lengths", x,
+                                        encoded_prompts)
             plens = self._ragged_lengths(prompt_lens if prompt_lens is not None else [Np] * B, B, Np, x.device,
-                                         "prompt_lens")
+                                         "prompt_lens", x, encoded_prompts)
             ragged = (lens, plens, lens + plens)
-        if _records_graph(self):
+        if self._records(x, encoded_prompts):
             return _EncoderFunction.apply(self, self.grad_reducer, x, encoded_prompts, *self.parameters())
         with torch.no_grad():
             return self._forward(x, encoded_prompts, ragged=ragged)

@@ -88,15 +88,15 @@ def _predictor(table):
     return m
 
 
-def _oracle(x, prompts, table, groups=8, trunk=None):
+def _oracle(x, prompts, table, groups=8, trunk=None, heads=HEADS):
     """Restatement -> fwd(P, dtype) = {"duration": ..., "pitch": ...}; `x` are ids when `table`."""
     trunk = trunk or eo._trunk
 
     def fwd(P, dtype):
         h = P["phoneme_token_emb.weight"][x] if table else x.to(dtype)
         sub = lambda pfx: {k: v for k, v in P.items() if k.startswith(pfx)}  # noqa: E731
-        return {"duration": trunk(sub(TRUNKS[0]), TRUNKS[0], h, prompts.to(dtype), HEADS, groups=groups),
-                "pitch": trunk(sub(TRUNKS[1]), TRUNKS[1], h, prompts.to(dtype), HEADS, groups=groups)}
+        return {"duration": trunk(sub(TRUNKS[0]), TRUNKS[0], h, prompts.to(dtype), heads, groups=groups),
+                "pitch": trunk(sub(TRUNKS[1]), TRUNKS[1], h, prompts.to(dtype), heads, groups=groups)}
     return fwd
 
 
@@ -157,13 +157,13 @@ def _with_leaves(x, prompts, table, **kw):
     return fwd
 
 
-def _set_head_biases(m, x, prompts, table):
+def _set_head_biases(m, x, prompts, table, heads=HEADS):
     """Head biases (bf16 values) that keep every fp64 pre-activation away from 0; returns them per trunk."""
     P = {n: p.detach().double() for n, p in m.named_parameters()}
     for t in TRUNKS:
         P[t + "to_pred.0.bias"] = torch.full_like(P[t + "to_pred.0.bias"], 1e3)
     with torch.backends.cudnn.flags(enabled=False):
-        outs = _oracle(x, prompts, table)(P, torch.float64)
+        outs = _oracle(x, prompts, table, heads=heads)(P, torch.float64)
     biases = {}
     for t, key in zip(TRUNKS, ("duration", "pitch")):
         pre = (outs[key] - 1e3).flatten().sort().values           # pre-activations without the bias

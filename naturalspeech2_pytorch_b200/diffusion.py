@@ -37,10 +37,12 @@ def simple_linear_schedule(t, clip_min=1e-9):
 
 
 def cosine_schedule(t, start=0, end=1, tau=1, clip_min=1e-9):
+    """ns2.py:1136-1142 on tensors (the reference's `math.cos` raises on them, SURVEY T12).  The cosine is clamped at
+    0 before the power: in fp32 cos(pi/2) is -4.4e-8, which a fractional power (non-integer 2 tau) turns into NaN."""
     power = 2 * tau
     v_start = math.cos(start * math.pi / 2) ** power
     v_end = math.cos(end * math.pi / 2) ** power
-    output = torch.cos((t * (end - start) + start) * math.pi / 2) ** power
+    output = torch.cos((t * (end - start) + start) * math.pi / 2).clamp(min=0) ** power
     output = (v_end - output) / (v_end - v_start)
     return output.clamp(min=clip_min)
 

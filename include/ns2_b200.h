@@ -210,6 +210,15 @@ typedef struct ns2_attn_bwd_args {
 
 int ns2_attn_bwd(const ns2_attn_bwd_args* args, ns2_stream_t stream);
 
+/* The backward of ns2_attn_fwd with kv_lens (key padding): the same arguments, plus the forward's kv_lens (device int32
+ * (batches), each value clamped to [1, kv_len]).  Sample b's dk / dv rows [0, kv_lens[b]) are bit-identical to a call
+ * on that sample alone with kv_len = kv_lens[b]; its rows past kv_lens[b] are written as exact zeros, and nothing from
+ * them reaches dq_accum.  K / V rows past kv_lens[b] must be finite (as for the forward).  kv_lens == NULL is exactly
+ * ns2_attn_bwd, which forwards to this call.  kv_lens together with a dropout of p > 0 is an error (nothing is
+ * launched).  kv_lens is an argument rather than a field of ns2_attn_bwd_args so that the struct's layout stays that of
+ * ABI version 8; it moves into the struct at the next ABI version. */
+int ns2_attn_bwd_kv_lens(const ns2_attn_bwd_args* args, const int32_t* kv_lens, ns2_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * 2b. Dropout (training only).  One site's parameters: a 64-bit seed (Philox4x32-10 key = its low / high 32 bits),
  *     the site number (one per dropout site of a forward call, reused by its backward) and the drop probability p.

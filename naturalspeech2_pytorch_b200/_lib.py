@@ -101,6 +101,7 @@ SIGNATURES = {
     "ns2_fold_conv_linear": (C.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P]),
     "ns2_attn_fwd": (C.c_int, [C.POINTER(AttnArgs), _P]),
     "ns2_attn_bwd": (C.c_int, [C.POINTER(AttnBwdArgs), _P]),
+    "ns2_attn_bwd_kv_lens": (C.c_int, [C.POINTER(AttnBwdArgs), _P, _P]),
     "ns2_dropout_f32": (C.c_int, [_P, _I64, C.POINTER(Dropout), _P]),
     "ns2_rmsnorm_film": (C.c_int, [_P, _I64, _I64, _I32, _I32, _P, _P, _I64, _P, _I64, _P]),
     "ns2_rmsnorm_f32": (C.c_int, [_P, _I64, _I64, _I32, _P, _P, _I64, _P]),

@@ -20,6 +20,13 @@
 // regenerates M from (seed, site, b, h, q, k) with Philox (philox.cuh) while the S^T / dP^T wgmma run:
 //   dV = (P * M)^T dO s (s applied when dV is stored)    dP = (dO V^T) * M s    dS = P * (dP - D) * scale
 // with D = rowsum(dO * O) of the dropped output O, so attn_delta_kernel is unchanged.
+//
+// attn_bwd_kernel<false, true> is the backward of attn_fwd_kernel<false, true> (key padding: sample b attends to keys
+// [0, kv_lens[b]) only).  A CTA whose key tile starts at or past kv_lens[b] writes its dK / dV rows as exact zeros and
+// exits: no TMA, nothing added to dQ.  The last valid tile masks P and dS^T to 0 for the keys past kv_lens[b], exactly
+// as keys past kv_len are masked; those K / V rows hold finite data (not the TMA zero fill), and forcing dS^T to 0
+// keeps junk in them out of dK, while their dK / dV rows come out as exact zeros.  The forward's lse covers only the
+// valid keys, so sample b's dK / dV are bit-identical to the plain kernel called on its keys alone.
 #include "ptx.cuh"
 #include "philox.cuh"
 #include "host_common.h"
@@ -52,7 +59,8 @@ struct AttnBwdDev {
   long long dk_rs, dk_bs, dv_rs, dv_bs;
   int q_len, kv_len, heads;
   float scale, scale_log2e;
-  DropoutDev drop;      // attn_bwd_kernel<true> only
+  DropoutDev drop;      // attn_bwd_kernel<true, false> only
+  const int* kv_lens;   // attn_bwd_kernel<false, true> only: (batches) key counts, clamped to [1, kv_len]
 };
 
 __device__ __forceinline__ float ab_ex2(float x) {
@@ -63,8 +71,9 @@ __device__ __forceinline__ float ab_ex2(float x) {
 
 __device__ __forceinline__ float ab_keep_if(float x, uint32_t bits, int n) { return (bits >> n) & 1u ? x : 0.f; }
 
-template <bool DROPOUT>
+template <bool DROPOUT, bool RAGGED>
 __global__ void __launch_bounds__(ab::THREADS, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdDev p) {
+  static_assert(!(DROPOUT && RAGGED), "no dropout variant of the key-padding kernel");
   using namespace ab;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
@@ -75,6 +84,21 @@ __global__ void __launch_bounds__(ab::THREADS, 1) attn_bwd_kernel(const __grid_c
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int j = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
   const int TQ = (p.q_len + BQ - 1) / BQ;
+  // keys of this sample; the plain kernels read p.kv_len where they use it, which keeps their code as it was
+  const int kv_len_b = RAGGED ? min(max(__ldg(p.kv_lens + b), 1), p.kv_len) : 0;
+#define NS2_ATTN_BWD_KV_LEN (RAGGED ? kv_len_b : p.kv_len)
+  if constexpr (RAGGED) {
+    if (j * BKV >= kv_len_b) {   // every key of the tile is padding: dK = dV = 0, nothing else to do
+      const int rows = min(BKV, p.kv_len - j * BKV);
+      for (int idx = threadIdx.x; idx < rows * (DH / 2); idx += THREADS) {
+        const long long key = j * BKV + idx / (DH / 2);
+        const int col = head * DH + 2 * (idx % (DH / 2));
+        *reinterpret_cast<uint32_t*>(p.dk + b * p.dk_bs + key * p.dk_rs + col) = 0u;
+        *reinterpret_cast<uint32_t*>(p.dv + b * p.dv_bs + key * p.dv_rs + col) = 0u;
+      }
+      return;
+    }
+  }
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmQ);
@@ -118,7 +142,7 @@ __global__ void __launch_bounds__(ab::THREADS, 1) attn_bwd_kernel(const __grid_c
     const int w = (warp >> 2) - 1;
     const int kr0 = 64 * w + 16 * (warp & 3) + (lane >> 2);   // this thread's key rows (in the tile): kr0, kr0 + 8
     const int c2 = 2 * (lane & 3);
-    const int valid = p.kv_len - j * BKV;   // keys of this tile that exist
+    const int valid = NS2_ATTN_BWD_KV_LEN - j * BKV;   // keys of this tile that exist (or are not past kv_lens[b])
     const uint32_t k_s = smem_u32(smem + OFF_K) + w * (64 * 128), v_s = smem_u32(smem + OFF_V) + w * (64 * 128);
     const uint32_t ds_s = smem_u32(smem + OFF_DS) + w * (64 * 128);
     uint8_t* ds_rows = smem + OFF_DS;
@@ -188,7 +212,8 @@ __global__ void __launch_bounds__(ab::THREADS, 1) attn_bwd_kernel(const __grid_c
         for (int e = 0; e < 4; ++e) {   // e = 2 r + t: key row kr0 + 8 r, query column qc + t
           const int r = e >> 1, t = e & 1;
           float pp = ab_ex2(fmaf(s[4 * jj + e], p.scale_log2e, -L[t]));
-          if (kr0 + 8 * r >= valid) pp = 0.f;
+          const bool pad_key = kr0 + 8 * r >= valid;
+          if (pad_key) pp = 0.f;
           if constexpr (DROPOUT) {
             pv[e] = ab_keep_if(pp, keep, 4 * jj + e);
             dv[e] = pp * (ab_keep_if(dp[4 * jj + e], keep, 4 * jj + e) * p.drop.scale - Dl[t]) * p.scale;
@@ -198,7 +223,9 @@ __global__ void __launch_bounds__(ab::THREADS, 1) attn_bwd_kernel(const __grid_c
           }
           // a softmax over one key is the constant 1: dS = 0 exactly, not the rounding left of dP - D (dP and
           // D = rowsum(dO * O) are summed in different orders), so dQ and dK come out as exact zeros
-          if (p.kv_len == 1) dv[e] = 0.f;
+          if (NS2_ATTN_BWD_KV_LEN == 1) dv[e] = 0.f;
+          // a padding key's dP is formed from its finite but arbitrary V row: dS = 0 outright, not 0 * dP
+          if (RAGGED && pad_key) dv[e] = 0.f;
         }
         pa[jj >> 1][(jj & 1) * 2 + 0] = pack_bf16x2(pv[0], pv[1]);
         pa[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(pv[2], pv[3]);
@@ -259,11 +286,17 @@ __global__ void __launch_bounds__(ab::THREADS, 1) attn_bwd_kernel(const __grid_c
       __nv_bfloat16* pk = p.dk + static_cast<long long>(b) * p.dk_bs + static_cast<long long>(key) * p.dk_rs + head * DH + c2;
 #pragma unroll
       for (int jj = 0; jj < DH / 8; ++jj) {
+        if (RAGGED && key >= kv_len_b) {   // a padding key: exact zeros (its P and dS were 0 already)
+          *reinterpret_cast<uint32_t*>(pv + 8 * jj) = 0u;
+          *reinterpret_cast<uint32_t*>(pk + 8 * jj) = 0u;
+          continue;
+        }
         *reinterpret_cast<uint32_t*>(pv + 8 * jj) = pack_bf16x2(dv_acc[4 * jj + 2 * r], dv_acc[4 * jj + 2 * r + 1]);
         *reinterpret_cast<uint32_t*>(pk + 8 * jj) = pack_bf16x2(dk_acc[4 * jj + 2 * r], dk_acc[4 * jj + 2 * r + 1]);
       }
     }
   }
+#undef NS2_ATTN_BWD_KV_LEN
 }
 
 // delta[b, h, q] = sum_d dO[b, q, h*64 + d] * O[b, q, h*64 + d]; one warp per (b, q) row, lanes over the heads' columns
@@ -291,14 +324,16 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const __nv_bfloat16* __
 
 using namespace ns2;
 
-// No dropout (or p = 0): the plain kernel; otherwise attn_bwd_kernel<true> with those dropout parameters.
-extern "C" int ns2_attn_bwd(const ns2_attn_bwd_args* a, ns2_stream_t stream_) {
+// No dropout (or p = 0) and no kv_lens: the plain kernel; dropout with p > 0: attn_bwd_kernel<true, false>; kv_lens:
+// attn_bwd_kernel<false, true> (never both).
+extern "C" int ns2_attn_bwd_kv_lens(const ns2_attn_bwd_args* a, const int32_t* kv_lens, ns2_stream_t stream_) {
   NS2_REQUIRE(a != nullptr, "attn_bwd: NULL args");
   const ns2_dropout* d = a->dropout;
   DropoutDev drop;
   NS2_REQUIRE(d == nullptr || make_dropout_dev(d->seed, d->site, d->p, &drop), "attn_bwd: dropout p=%g is not in [0, 1)",
               static_cast<double>(d->p));
   const bool dropout = d != nullptr && d->p != 0.0f;
+  NS2_REQUIRE(!(dropout && kv_lens), "attn_bwd: kv_lens with dropout p > 0 is not supported");
   NS2_REQUIRE(a->q && a->k && a->v && a->o && a->d_o && a->lse && a->delta && a->dq_accum && a->dk && a->dv,
               "attn_bwd: NULL pointer");
   NS2_REQUIRE(a->dim_head == 64, "attn_bwd: dim_head=%d, only 64 is supported", a->dim_head);
@@ -341,13 +376,21 @@ extern "C" int ns2_attn_bwd(const ns2_attn_bwd_args* a, ns2_stream_t stream_) {
   dev.scale = a->scale;
   dev.scale_log2e = a->scale * 1.4426950408889634f;
   dim3 grid((a->kv_len + ab::BKV - 1) / ab::BKV, a->heads, a->batches);
-  if (!dropout) {
-    NS2_CUDA_CHECK(set_max_smem_once(attn_bwd_kernel<false>, ab::SMEM_BYTES));
-    attn_bwd_kernel<false><<<grid, ab::THREADS, ab::SMEM_BYTES, stream>>>(dev);
+  if (kv_lens != nullptr) {
+    dev.kv_lens = kv_lens;
+    NS2_CUDA_CHECK(set_max_smem_once(attn_bwd_kernel<false, true>, ab::SMEM_BYTES));
+    attn_bwd_kernel<false, true><<<grid, ab::THREADS, ab::SMEM_BYTES, stream>>>(dev);
+  } else if (!dropout) {
+    NS2_CUDA_CHECK(set_max_smem_once(attn_bwd_kernel<false, false>, ab::SMEM_BYTES));
+    attn_bwd_kernel<false, false><<<grid, ab::THREADS, ab::SMEM_BYTES, stream>>>(dev);
   } else {
     dev.drop = drop;
-    NS2_CUDA_CHECK(set_max_smem_once(attn_bwd_kernel<true>, ab::SMEM_BYTES_DROPOUT));
-    attn_bwd_kernel<true><<<grid, ab::THREADS, ab::SMEM_BYTES_DROPOUT, stream>>>(dev);
+    NS2_CUDA_CHECK(set_max_smem_once(attn_bwd_kernel<true, false>, ab::SMEM_BYTES_DROPOUT));
+    attn_bwd_kernel<true, false><<<grid, ab::THREADS, ab::SMEM_BYTES_DROPOUT, stream>>>(dev);
   }
   return launched(2);
+}
+
+extern "C" int ns2_attn_bwd(const ns2_attn_bwd_args* a, ns2_stream_t stream) {
+  return ns2_attn_bwd_kv_lens(a, nullptr, stream);
 }

@@ -273,27 +273,43 @@ class NaturalSpeech2(nn.Module):
     # training loss (differentiable: `loss.backward()` runs the hand-written backward kernels)
     # ------------------------------------------------------------------------------------------
     def forward(self, audio, text=None, text_lens=None, mel=None, mel_lens=None, codes=None, prompt=None,
-                pitch=None, *args, prompt_enc=None, cond=None, times=None, noise=None, duration=None, **kwargs):
+                pitch=None, *args, prompt_enc=None, cond=None, times=None, noise=None, duration=None, prompt_lens=None,
+                phoneme_lens=None, **kwargs):
         """ns2.py:1503-1684 -> scalar diffusion loss (the only term the reference returns, SURVEY T11).
         Extra keyword-only arguments: `prompt_enc`/`cond` (precomputed conditioning), `times`/`noise`
         (inject the two random draws of ns2.py:1621,1625 — used by the parity tests) and `duration` (per-phoneme frame
         counts, handed to the conditioner only when given: encoders.Conditioner takes them in place of an aligner).
         A conditioner that returns (prompt_enc, cond, duration_loss, pitch_loss) (encoders.Conditioner with
         train_duration_pitch=True) adds duration_loss_weight * duration_loss + pitch_loss_weight * pitch_loss to the
-        returned loss, the `aux_loss` of ns2.py:1600-1602 that the reference adds at 1684."""
+        returned loss, the `aux_loss` of ns2.py:1600-1602 that the reference adds at 1684.
+        A batch of prompts and texts of different lengths, padded at their ends, trains as if each sample ran alone with
+        `prompt_lens` (prompt latent frames) and `phoneme_lens` (phonemes), given to the conditioner, and prompt_lens to
+        the model; with precomputed `prompt_enc=` / `cond=` only prompt_lens (to the model).  The latents and pitch share
+        one length.  Each sample's MSE row is then that of the sample alone; the loss, as in the reference, is
+        mean(mse) * mean(weight) over the batch (ns2.py:1651-1666), not the mean of the per-sample losses."""
         is_raw_audio = audio.ndim == 2
         aux_loss = None
+        ragged = prompt_lens is not None or phoneme_lens is not None
+        if ragged and not self.conditional:
+            raise ValueError("prompt_lens / phoneme_lens apply to conditional models")
         if self.conditional and not (_exists(prompt_enc) and _exists(cond)):
             if not _exists(self.conditioner):
                 raise NotImplementedError(
                     "conditional training needs prompt_enc= and cond= or a `conditioner` callable (the "
                     "reference's encoders + aligner are outside the accelerated path)")
             extra = {} if duration is None else {"duration": duration}
+            if ragged:
+                if prompt is None or prompt.ndim != 3:
+                    raise ValueError("with prompt_lens / phoneme_lens the prompt must be encoded latents (B, Np, dim): "
+                                     "a raw-audio prompt is curtailed from the left by the batch's length")
+                extra.update(prompt_lens=prompt_lens, phoneme_lens=phoneme_lens)
             out = self.conditioner(audio=audio, text=text, text_lens=text_lens, mel=mel, mel_lens=mel_lens,
                                    prompt=self.process_prompt(prompt), pitch=pitch, mode="train", **extra)
             prompt_enc, cond = out[:2]
             if len(out) == 4:   # the duration / pitch predictor's L1 losses (ns2.py:1587-1602)
                 aux_loss = self.duration_loss_weight * out[2] + self.pitch_loss_weight * out[3]
+        elif phoneme_lens is not None:
+            raise ValueError("phoneme_lens goes to the conditioner; with prompt_enc= / cond= pass prompt_lens only")
         assert not (is_raw_audio and not _exists(self.codec)), \
             "codec must be passed in if one were to train on raw audio"
         if is_raw_audio:
@@ -314,7 +330,8 @@ class NaturalSpeech2(nn.Module):
         noised = torch.empty_like(audio)
         target = torch.empty_like(audio)
         ops.q_sample(audio, noise, alpha, sigma, noised, target, objective=self.objective)  # ns2.py:1631-1644
-        pred = self.model(noised, times, prompt=prompt_enc, cond=cond)  # ns2.py:1635
+        lens = {} if prompt_lens is None else {"prompt_lens": prompt_lens}
+        pred = self.model(noised, times, prompt=prompt_enc, cond=cond, **lens)  # ns2.py:1635
         if pred.requires_grad:
             from .training import MseRowsFunction
             loss = MseRowsFunction.apply(pred, target)                  # ns2.py:1646-1647, with a backward kernel

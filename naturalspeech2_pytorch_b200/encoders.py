@@ -51,11 +51,18 @@ nn.Dropout has the default p = 0 (ns2.py:352, 374) and draws nothing.  With `tra
 per call in train() mode, none in eval(), without train_dropout or with p = 0.  The cross attention of layer l of trunk
 t (0 duration, 1 pitch; forward order) is site t depth + l.  The record keeps the seed, no mask.
 Attention masks are not supported (`mask=None` is what NaturalSpeech2.forward / .sample pass, ns2.py:1475-1476,
-1538-1539).  A batch of sequences of different lengths, each padded at its end, is sampled with per-sample lengths
-instead (`lengths=` / `prompt_lens=`, inference only): the "same" convolutions read zeros past each sample's end, the
+1538-1539).  A batch of sequences of different lengths, each padded at its end, is run with per-sample lengths
+instead (`lengths=` / `prompt_lens=`): the "same" convolutions read zeros past each sample's end, the
 attentions take only a sample's own keys (ops.attention kv_lens), the predictor's GroupNorms take only its own rows, and
 padded output rows are exact zeros, so every sample's output is bit-identical to running it alone, unpadded.  What the
-padded input rows hold is never read into a valid row.  Numerics follow the denoiser: bf16 tensor-core operands, fp32 accumulation, fp32 residual stream and norm
+padded input rows hold is never read into a valid row.
+The two encoders also train with lengths (not with train_dropout: the attention has no key-padded dropout kernel).  The
+record keeps the lengths and the backward undoes each row mask of the forward on the gradient (ops.mask_rows), runs the
+attention backward with the same key counts (ops.attention_bwd kv_lens: d K / d V rows past them are exact zeros), and
+so every parameter gradient is the sum of the per-sample-alone gradients (up to the fp32 summation order of the dQ and
+weight-gradient reductions), every input gradient is the alone one, and the gradient of a padded prompt row - or of a
+token-table row that only padded ids reach - is exactly zero.  The duration / pitch predictor takes lengths for
+sampling only.  Numerics follow the denoiser: bf16 tensor-core operands, fp32 accumulation, fp32 residual stream and norm
 statistics.
 """
 from __future__ import annotations
@@ -112,7 +119,8 @@ class _EncoderFunction(torch.autograd.Function):
         with torch.no_grad():
             grads = ctx.enc._train_backward(ctx.saved, *d_outs)
         ctx.saved = None
-        d_in = grads.pop(_INPUT_GRADS, None) or (None,) * ctx.n_in
+        d_in = tuple(grads.pop(_INPUT_GRADS, None) or ())
+        d_in += (None,) * (ctx.n_in - len(d_in))   # inputs without a gradient (ids, lengths) may be left out
         d_in = [d if need else None for d, need in zip(d_in, ctx.needs_input_grad[2:2 + ctx.n_in])]
         return (None, None, *d_in, *param_grads(ctx.enc, grads, ctx.reducer))
 
@@ -141,10 +149,10 @@ class _EncoderBase(_PackedCache):
             for k in ("qkv", "o", "w1", "w2"):
                 T[f"l{l}_{k}"] = P[f"l{l}_{k}"].t().contiguous()
 
-    def _train_forward(self, x: torch.Tensor):
+    def _train_forward(self, x: torch.Tensor, lens: Optional[torch.Tensor] = None):
         """`_forward` keeping the activations `_train_backward` reads -> (output, record)."""
-        saved = {}
-        return self._forward(x, saved), saved
+        saved = {"lens": lens}
+        return self._forward(x, saved, lens), saved
 
     # ---- transformer ----
     def _pack_transformer(self, P: Dict[str, torch.Tensor], tr: _PlainTransformerParams, dim: int) -> None:
@@ -201,10 +209,13 @@ class _EncoderBase(_PackedCache):
         return x
 
     def _transformer_backward(self, layers: list, tr: _PlainTransformerParams, P, T, heads: int, dxr: torch.Tensor,
-                              dxr_bf: torch.Tensor, grads: Dict[str, torch.Tensor], seed: Optional[int] = None) -> None:
+                              dxr_bf: torch.Tensor, grads: Dict[str, torch.Tensor], seed: Optional[int] = None,
+                              kv_lens: Optional[torch.Tensor] = None) -> None:
         """Transformer backward (ns2.py:1110-1115): dxr (fp32 gradient of the output, updated in place) becomes the
         gradient of the input; dxr_bf its bf16 copy.  Parameter gradients go to `grads` under the reference's names.
-        seed: the forward's dropout seed (its attention masks are regenerated)."""
+        seed: the forward's dropout seed (its attention masks are regenerated).  kv_lens: the forward's per-sample
+        lengths; rows of dxr past them that come in as zeros stay exact zeros (the layers are row-wise but for the
+        attention, whose d K / d V rows past them are zeros, and a padded query with d O = 0 has dS = 0)."""
         _, N, D = dxr.shape
 
         def norm_backward(x_in, dh, gamma, key):
@@ -220,7 +231,7 @@ class _EncoderBase(_PackedCache):
             norm_backward(L["x_mid"], dh2, P[f"l{l}_g2"], pfx + "2.gamma")
             # ---- attention: x += Wo attn(Wqkv RMSNorm(x)) ----
             dh1, _ = attention_backward(dxr_bf, L["h1"], L["ao"], L["lse"], L["qkv"], None, T[f"l{l}_o"], T[f"l{l}_qkv"],
-                                        heads, grads, pfx + "1.", dropout=self._attn_dropout(seed, l))
+                                        heads, grads, pfx + "1.", dropout=self._attn_dropout(seed, l), kv_lens=kv_lens)
             norm_backward(L["x_in"], dh1, P[f"l{l}_g1"], pfx + "0.gamma")
 
     def _conv_silu_backward(self, x_in: torch.Tensor, w: torch.Tensor, w_t: Optional[torch.Tensor], bias: torch.Tensor,
@@ -242,17 +253,19 @@ class _EncoderBase(_PackedCache):
         return _records_graph(self) or (self.training and torch.is_grad_enabled() and
                                         any(t.requires_grad for t in inputs))
 
-    def _ragged_lengths(self, lengths, batch: int, n: int, device, name: str, *inputs) -> Optional[torch.Tensor]:
-        """Validated int32 device lengths of a sampling call (None stays None).  Lengths are for inference only."""
+    def _ragged_lengths(self, lengths, batch: int, n: int, device, name: str) -> Optional[torch.Tensor]:
+        """Validated int32 device lengths of a call (None stays None).  Not with train_dropout in train mode: the
+        attention has no key-padded dropout kernel, and the phoneme conv dropout's counter is the flat element index."""
         if lengths is None:
             return None
-        if self._records(*inputs) or (self.training and self.train_dropout):
-            raise NotImplementedError(f"{type(self).__name__}: {name} are supported for sampling only (no autograd, no "
-                                      "dropout)")
+        if self.training and self.train_dropout:
+            raise NotImplementedError(f"{type(self).__name__}: {name} are not supported together with train_dropout")
         return ops.lengths(lengths, batch, n, device=device, name=name)
 
-    def _start_backward(self, d_out: torch.Tensor):
+    def _start_backward(self, d_out: torch.Tensor, lens: Optional[torch.Tensor] = None):
         dxr = d_out.float().contiguous().clone()        # fp32 residual-stream gradient, updated in place
+        if lens is not None:                            # the forward zeroed the output rows past the lengths
+            ops.mask_rows(dxr, lens)
         return dxr, ops.cast_bf16(dxr, torch.empty(dxr.shape, device=dxr.device, dtype=torch.bfloat16))
 
 
@@ -265,7 +278,8 @@ def _check_transformer_dims(dim: int, dim_head: int):
 
 class SpeechPromptEncoder(_EncoderBase):
     """ns2.py:289-341.  forward(x: (B, Np, dim_codebook)) -> (B, Np, dims[-1]) fp32.
-    forward(x, lengths=(B,)): sample b is x[b, :lengths[b]] (see the module docstring); rows past it come out as zeros."""
+    forward(x, lengths=(B,)): sample b is x[b, :lengths[b]] (see the module docstring); rows past it come out as zeros,
+    in training too (then d x rows past it are exact zeros)."""
 
     def __init__(self, dim_codebook, dims: Tuple[int, ...] = (256, 2048, 2048, 2048, 2048, 512, 512, 512), *,
                  depth=6, heads=8, dim_head=64, dropout=0.2, kernel_size=9, padding=4, use_flash_attn=True):
@@ -308,9 +322,9 @@ class SpeechPromptEncoder(_EncoderBase):
         assert x.shape[-1] == self.dim
         if not x.is_cuda:
             raise ValueError("SpeechPromptEncoder: input must be a CUDA tensor (the ns2_b200 ops have no CPU path)")
-        lens = self._ragged_lengths(lengths, x.shape[0], x.shape[1], x.device, "lengths", x)
+        lens = self._ragged_lengths(lengths, x.shape[0], x.shape[1], x.device, "lengths")
         if self._records(x):
-            return _EncoderFunction.apply(self, self.grad_reducer, x, *self.parameters())
+            return _EncoderFunction.apply(self, self.grad_reducer, x, lens, *self.parameters())
         with torch.no_grad():
             return self._forward(x, lens=lens)
 
@@ -341,16 +355,17 @@ class SpeechPromptEncoder(_EncoderBase):
         out = self._transformer(h, self.transformer, P, self.heads, saved, seed, kv_lens=lens)
         return out if lens is None else ops.mask_rows(out, lens)
 
-    def _train_forward(self, x: torch.Tensor):
-        saved = {"x_requires_grad": x.requires_grad, "x_dtype": x.dtype}
-        return self._forward(x, saved), saved
+    def _train_forward(self, x: torch.Tensor, lens: Optional[torch.Tensor] = None):
+        saved = {"x_requires_grad": x.requires_grad, "x_dtype": x.dtype, "lens": lens}
+        return self._forward(x, saved, lens), saved
 
     def _train_backward(self, S, d_out: torch.Tensor) -> Dict[str, torch.Tensor]:
         P, T = self.packed(), self.packed_transposed()
         grads: Dict[str, torch.Tensor] = {}
-        dxr, dxr_bf = self._start_backward(d_out)
+        lens = S["lens"]
+        dxr, dxr_bf = self._start_backward(d_out, lens)
         self._transformer_backward(S["layers"], self.transformer, P, T, self.heads, dxr, dxr_bf, grads,
-                                   S["dropout_seed"])
+                                   S["dropout_seed"], kv_lens=lens)
         d_h = dxr_bf                        # gradient of the last conv's (SiLU) output
         need_dx = S["x_requires_grad"]
         for i in reversed(range(len(self._convs()))):
@@ -358,9 +373,13 @@ class SpeechPromptEncoder(_EncoderBase):
             # prompt requires grad (it usually comes from the codec)
             first = i == 0
             w_t = T[f"c{i}_w"] if need_dx or not first else None
+            if lens is not None:            # the forward zeroed this conv's output past the lengths
+                ops.mask_rows(d_h, lens)
             d_h = self._conv_silu_backward(S["conv_in"][i], P[f"c{i}_w"], w_t, P[f"c{i}_b"], d_h, self.padding, grads,
                                            f"conv.{2 * i + 1}", dtype=torch.float32 if first else torch.bfloat16)
         if need_dx:
+            if lens is not None:            # ... and its input (the "same" conv's dgrad spreads into the padding)
+                ops.mask_rows(d_h, lens)
             grads[_INPUT_GRADS] = (d_h.to(S["x_dtype"]),)
         return grads
 
@@ -368,7 +387,8 @@ class SpeechPromptEncoder(_EncoderBase):
 class PhonemeEncoder(_EncoderBase):
     """ns2.py:228-287.  forward(x: (B, T) int64 phoneme ids, negative = padding) -> (B, T, dim_hidden) fp32.
     A tokenizer (List[str] input) is used exactly like the reference when one is given.
-    forward(x, lengths=(B,)): sample b is x[b, :lengths[b]] (see the module docstring); rows past it come out as zeros."""
+    forward(x, lengths=(B,)): sample b is x[b, :lengths[b]] (see the module docstring); rows past it come out as zeros,
+    in training too (then the token-table rows that only padded ids reach get exact-zero gradients)."""
 
     def __init__(self, *, tokenizer=None, num_tokens=None, dim=512, dim_hidden=512, kernel_size=9, depth=6,
                  dim_head=64, heads=8, conv_dropout=0.2, attn_dropout=0., use_flash=False):
@@ -412,7 +432,7 @@ class PhonemeEncoder(_EncoderBase):
             raise ValueError("PhonemeEncoder: input must be a CUDA tensor (the ns2_b200 ops have no CPU path)")
         lens = self._ragged_lengths(lengths, x.shape[0], x.shape[1], x.device, "lengths")
         if self._records():   # ids have no gradient
-            return _EncoderFunction.apply(self, self.grad_reducer, x, *self.parameters())
+            return _EncoderFunction.apply(self, self.grad_reducer, x, lens, *self.parameters())
         with torch.no_grad():
             return self._forward(x, lens=lens)
 
@@ -439,9 +459,12 @@ class PhonemeEncoder(_EncoderBase):
     def _train_backward(self, S, d_out: torch.Tensor) -> Dict[str, torch.Tensor]:
         P, T = self.packed(), self.packed_transposed()
         grads: Dict[str, torch.Tensor] = {}
-        dxr, dxr_bf = self._start_backward(d_out)
+        # with lengths: the output gradient is masked like the output; the causal conv and the zero d K / d V rows keep
+        # every padded row's gradient an exact zero from there on, so embedding_bwd adds nothing for padded ids
+        dxr, dxr_bf = self._start_backward(d_out, S["lens"])
         seed = S["dropout_seed"]
-        self._transformer_backward(S["layers"], self.transformer, P, T, self.heads, dxr, dxr_bf, grads, seed)
+        self._transformer_backward(S["layers"], self.transformer, P, T, self.heads, dxr, dxr_bf, grads, seed,
+                                   kv_lens=S["lens"])
         if seed is not None and self.conv_dropout > 0:   # the conv's dropout mask, on the fp32 gradient
             ops.cast_bf16(ops.dropout_(dxr, dropout=(seed, 0, self.conv_dropout)), dxr_bf)
         d_e = self._conv_silu_backward(S["emb"], P["c_w"], T["c_w"], P["c_b"], dxr_bf, self.kernel_size - 1, grads,
@@ -705,10 +728,12 @@ class DurationPitchPredictor(_EncoderBase):
         if lengths is not None or prompt_lens is not None:
             B, T = x.shape[:2]
             Np = encoded_prompts.shape[1]
-            lens = self._ragged_lengths(lengths if lengths is not None else [T] * B, B, T, x.device, "lengths", x,
-                                        encoded_prompts)
+            if self._records(x, encoded_prompts):
+                raise NotImplementedError("DurationPitchPredictor: lengths / prompt_lens are supported for sampling only "
+                                          "(no autograd)")
+            lens = self._ragged_lengths(lengths if lengths is not None else [T] * B, B, T, x.device, "lengths")
             plens = self._ragged_lengths(prompt_lens if prompt_lens is not None else [Np] * B, B, Np, x.device,
-                                         "prompt_lens", x, encoded_prompts)
+                                         "prompt_lens")
             ragged = (lens, plens, lens + plens)
         if self._records(x, encoded_prompts):
             return _EncoderFunction.apply(self, self.grad_reducer, x, encoded_prompts, *self.parameters())
@@ -880,7 +905,13 @@ class Conditioner(nn.Module):
     train_duration_pitch=True also trains the duration / pitch predictor: mode="train" runs it on the same encoder
     outputs and returns (prompt_enc, cond, duration_loss, pitch_loss), the reference's L1 losses against the given
     durations and the per-phoneme pitch (ns2.py:1579-1590).  Their gradients reach the predictor and, through its
-    inputs, both encoders; NaturalSpeech2.forward weights and adds them (duration_loss_weight, pitch_loss_weight)."""
+    inputs, both encoders; NaturalSpeech2.forward weights and adds them (duration_loss_weight, pitch_loss_weight).
+
+    mode="train" with prompt_lens / phoneme_lens (a batch padded at its ends): sample b is prompt[b, :prompt_lens[b]]
+    and text[b, :phoneme_lens[b]] with its durations, which must be 0 past phoneme_lens[b].  Each sample's prompt_enc
+    and cond are those of the sample alone (zero past its prompt length and its total duration), and the gradients
+    reaching the encoders are the sums of the per-sample-alone ones (see the module docstring).  Not together with
+    train_dropout or train_duration_pitch."""
 
     train_duration_pitch = False
 
@@ -916,9 +947,7 @@ class Conditioner(nn.Module):
         total predicted duration in frames (cond is zero past it)."""
         ragged = prompt_lens is not None or phoneme_lens is not None
         if mode == "train":
-            if ragged:
-                raise NotImplementedError("Conditioner(mode='train') does not take prompt_lens / phoneme_lens")
-            return self._forward_train(prompt, text, pitch, duration)
+            return self._forward_train(prompt, text, pitch, duration, prompt_lens, phoneme_lens)
         if mode != "sample":
             raise NotImplementedError(f"Conditioner: unknown mode {mode!r} (sample | train)")
         assert prompt is not None and text is not None
@@ -936,9 +965,10 @@ class Conditioner(nn.Module):
             cond_lens = duration.int().sum(dim=-1, dtype=torch.int32)   # the frames frames_to_text_index fills
         return prompt_enc, cond, cond_lens
 
-    def _forward_train(self, prompt, text, pitch, duration):
+    def _forward_train(self, prompt, text, pitch, duration, prompt_lens=None, phoneme_lens=None):
         """ns2.py:1538-1583 with the aligner's hard durations given: prompt_enc = prompt_enc(prompt), cond =
-        expand_encodings(phoneme_enc(text), durations, average_over_durations(pitch, durations)) with L = pitch frames."""
+        expand_encodings(phoneme_enc(text), durations, average_over_durations(pitch, durations)) with L = pitch frames.
+        prompt_lens / phoneme_lens: per-sample lengths, see the class docstring."""
         if duration is None:
             raise NotImplementedError(
                 "Conditioner(mode='train') needs duration=(B, T) frame counts per phoneme (the aligner's aln_hard): the "
@@ -963,8 +993,20 @@ class Conditioner(nn.Module):
         total = duration.long().sum(dim=-1)
         if bool((total > L).any()):
             raise ValueError(f"durations sum to {int(total.max())} frames, past the {L} frames of pitch")
-        prompt_enc = self.prompt_enc(prompt)
-        phoneme_enc = self.phoneme_enc(text)
+        if phoneme_lens is not None:   # host-side checks: nothing is launched for a refused call
+            lens = ops.lengths(phoneme_lens, B, T, device=duration.device, name="phoneme_lens")
+            past = torch.arange(T, device=duration.device)[None, :] >= lens[:, None].long()
+            if bool(((duration != 0) & past).any()):
+                raise ValueError("duration must be 0 past phoneme_lens (padded phonemes take no frames)")
+        if prompt_lens is not None or phoneme_lens is not None:
+            if self.train_duration_pitch:
+                raise NotImplementedError("Conditioner(train_duration_pitch=True) does not take prompt_lens / "
+                                          "phoneme_lens: the duration / pitch predictor trains without lengths")
+            if self.training and (self.prompt_enc.train_dropout or self.phoneme_enc.train_dropout):
+                raise NotImplementedError("Conditioner(train_dropout=True) does not take prompt_lens / phoneme_lens: "
+                                          "the attention has no key-padded dropout")
+        prompt_enc = self.prompt_enc(prompt, lengths=prompt_lens)
+        phoneme_enc = self.phoneme_enc(text, lengths=phoneme_lens)
         with torch.no_grad():
             ph_pitch = average_over_durations(pitch.float(), duration)[:, 0]      # (B, T), ns2.py:1581
         cond = expand_encodings(phoneme_enc, duration, ph_pitch, self.pitch_emb.weight, length=L,

@@ -540,13 +540,14 @@ class Model(_PackedCache):
         `_forward_impl`.
         prompt_lens (B,): sample b's prompt is prompt[b, :prompt_lens[b]] (the mean, the perceiver's keys); cond_lens (B,):
         its condition ends at frame cond_lens[b] (kept in the result as "cond_lens" for `forward`).  With them each
-        sample's conditioning is that of the sample alone, and nothing in the padded rows is read."""
+        sample's conditioning is that of the sample alone, and nothing in the padded rows is read.  With `saved` (the
+        training forward) prompt_lens is recorded for the backward; cond_lens is for sampling only."""
         assert self.condition_on_prompt
         P, D = self.packed(), self.dim
         B = prompt.shape[0]
         dev = prompt.device
-        if saved is not None and (prompt_lens is not None or cond_lens is not None):
-            raise NotImplementedError("prompt_lens / cond_lens are supported for sampling only")
+        if saved is not None and cond_lens is not None:
+            raise NotImplementedError("cond_lens is supported for sampling only")
         plens = None if prompt_lens is None else ops.lengths(prompt_lens, B, prompt.shape[1], device=dev,
                                                              name="prompt_lens")
         prompt = prompt.float().contiguous()
@@ -562,7 +563,7 @@ class Model(_PackedCache):
         cond_proj = ops.gemm(cond_bf, P["cond_w"], torch.empty(B, L, D, device=dev), n=D, epilogue=ops.EPI_F32,
                              bias=P["cond_b"])
         if saved is not None:
-            saved.update(prompt_mean=mean, cond_bf=cond_bf, Lc=L)
+            saved.update(prompt_mean=mean, cond_bf=cond_bf, Lc=L, prompt_lens=plens)
         c = Conditioning(prompt_cond=prompt_cond, tokens=tokens, cond_proj=cond_proj, length=length)
         if cond_lens is not None:
             c["cond_lens"] = ops.lengths(cond_lens, B, None, device=dev, name="cond_lens", lo=0)
@@ -604,21 +605,23 @@ class Model(_PackedCache):
         (B, N, drop-prob, conditioning shapes) and replayed; eligible when no RNG draw and no per-call host work is
         involved, i.e. unconditional models or cached conditioning with cond_drop_prob in {0, 1}.
 
-        prompt_lens / cond_lens (B,) (inference only): per-sample prompt lengths and condition lengths of a batch padded
-        at the end, see `precompute_conditioning`; cached conditioning carries its own."""
+        prompt_lens / cond_lens (B,): per-sample prompt lengths and condition lengths of a batch padded at the end, see
+        `precompute_conditioning`; cached conditioning carries its own.  Training takes prompt_lens (each sample's
+        prediction and gradients are those of the sample alone, d prompt is zero past its length); cond_lens is for
+        inference only: in training the condition spans the latents' frames, zero past each sample's durations."""
         ragged = prompt_lens is not None or cond_lens is not None
         if ragged and _conditioning is not None:
             raise ValueError("prompt_lens / cond_lens go to precompute_conditioning when the conditioning is cached")
+        if ragged and not self.condition_on_prompt:
+            raise ValueError("prompt_lens / cond_lens apply to models with condition_on_prompt=True")
         if _records_graph(self):
             # training: one autograd node whose backward runs the hand-written kernels (training.py)
             from .training import DenoiserFunction
-            if prompt_mask is not None or out is not None or _conditioning is not None or ragged:
-                raise NotImplementedError("training mode takes (x, times[, prompt, cond]): no out=, prompt_mask, lengths or "
-                                          "cached conditioning")
-            return DenoiserFunction.apply(self, x, times, prompt, cond, cond_drop_prob, *self.parameters())
+            if prompt_mask is not None or out is not None or _conditioning is not None or cond_lens is not None:
+                raise NotImplementedError("training mode takes (x, times[, prompt, cond, prompt_lens]): no out=, "
+                                          "prompt_mask, cond_lens or cached conditioning")
+            return DenoiserFunction.apply(self, x, times, prompt, cond, cond_drop_prob, prompt_lens, *self.parameters())
         if ragged:
-            if not self.condition_on_prompt:
-                raise ValueError("prompt_lens / cond_lens apply to models with condition_on_prompt=True")
             with torch.no_grad():   # eager: the prompt work is per call anyway
                 return self._forward_impl(x, times, prompt, prompt_mask, cond, cond_drop_prob, None, out,
                                           prompt_lens=prompt_lens, cond_lens=cond_lens)

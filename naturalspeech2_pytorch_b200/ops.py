@@ -736,10 +736,15 @@ def rvq_ce_bwd(frames: torch.Tensor, codebooks: torch.Tensor, cn2: torch.Tensor,
 # backward pass
 # --------------------------------------------------------------------------------------------------
 def attention_bwd(q, k, v, o, d_o, lse, dq_accum, dk, dv, *, heads: int, scale: Optional[float] = None,
-                  delta: Optional[torch.Tensor] = None, dropout: Optional[DropoutSpec] = None):
+                  delta: Optional[torch.Tensor] = None, dropout: Optional[DropoutSpec] = None,
+                  kv_lens: Optional[torch.Tensor] = None):
     """(dq_accum f32 (B, Nq, inner) += dQ, dk, dv bf16) of softmax(q k^T scale) v given d_o; zero dq_accum for a plain dQ.
-    dropout: the forward's (seed, site, p); the mask is regenerated, not stored."""
+    dropout: the forward's (seed, site, p); the mask is regenerated, not stored.
+    kv_lens: the forward's int32 CUDA (B,) key counts in [1, Nk] (see `attention`): dk / dv rows past them come out as
+    exact zeros, and sample b's dk / dv are bit-identical to the call on its keys alone.  No dropout with kv_lens."""
     lib = _lib.load()
+    if kv_lens is not None and dropout is not None:
+        raise ValueError("attention_bwd: dropout with kv_lens is not supported")
     inner = heads * 64
     B, Nq, _ = q.shape
     _, Nk, _ = k.shape
@@ -748,7 +753,9 @@ def attention_bwd(q, k, v, o, d_o, lse, dq_accum, dk, dv, *, heads: int, scale: 
     qs, ks = (B, Nq, inner), (B, Nk, inner)
     _check(("q", q, BF16, qs, LAST), ("k", k, BF16, ks, LAST), ("v", v, BF16, ks, LAST), ("o", o, BF16, qs, LAST),
            ("d_o", d_o, BF16, qs, LAST), ("lse", lse, F32, (B, heads, Nq), DENSE), ("dq_accum", dq_accum, F32, qs, DENSE),
-           ("dk", dk, BF16, ks, LAST), ("dv", dv, BF16, ks, LAST), ("delta", delta, F32, (B, heads, Nq), DENSE))
+           ("dk", dk, BF16, ks, LAST), ("dv", dv, BF16, ks, LAST), ("delta", delta, F32, (B, heads, Nq), DENSE),
+           ("kv_lens", kv_lens, I32, (B,), DENSE))
+    lens_ptr = _check_lens(kv_lens, 1, Nk, "kv_lens")
     a = _lib.AttnBwdArgs()
     a.q, a.q_row_stride, a.q_batch_stride = q.data_ptr(), q.stride(1), q.stride(0)
     a.k, a.k_row_stride, a.k_batch_stride = k.data_ptr(), k.stride(1), k.stride(0)
@@ -762,7 +769,7 @@ def attention_bwd(q, k, v, o, d_o, lse, dq_accum, dk, dv, *, heads: int, scale: 
     a.scale = float(scale if scale is not None else 64 ** -0.5)
     d = _dropout_args(dropout)
     a.dropout = None if d is None else C.pointer(d)
-    check(lib.ns2_attn_bwd(C.byref(a), _stream()), "ns2_attn_bwd")
+    check(lib.ns2_attn_bwd_kv_lens(C.byref(a), lens_ptr, _stream()), "ns2_attn_bwd_kv_lens")
     return dq_accum, dk, dv
 
 

@@ -25,6 +25,10 @@ When autograd asks for them (an encoder upstream: encoders.Conditioner in train 
 d loss / d prompt (perceiver context projection dgrad + the mean-pool's share, spread by ops.add_rows_bcast) and
 d loss / d cond (one dgrad GEMM through the aligned-condition projection, token-major, handed over as a channel-first
 view); otherwise nothing extra runs.  `x` and `times` stay non-differentiable (latents come from the codec).
+With per-sample prompt lengths (`Model.forward(prompt_lens=)`) the perceiver's attention backward takes the forward's
+key counts M + prompt_lens (ops.attention_bwd kv_lens) and the mean-pool's share of d prompt is d mean[b] / prompt_lens[b]
+over the rows [0, prompt_lens[b]): d prompt rows past a sample's length are exact zeros.  The latent sequence needs no
+lengths: the WaveNet and feed-forward convs are causal and the batch shares one latent length.
 """
 from __future__ import annotations
 
@@ -129,14 +133,15 @@ def ff_backward(dy, h, g, P, T, pk: str, Di: int, grads: Dict[str, torch.Tensor]
 
 
 def attention_backward(dy, x, o, lse, q, kv, w_o_t, w_q_t, heads: int, grads: Dict[str, torch.Tensor], name: str,
-                       d_kv=None, x_kv=None, w_kv_t=None, dropout=None):
+                       d_kv=None, x_kv=None, w_kv_t=None, dropout=None, kv_lens=None):
     """Backward of y = Wo attn(Wq x, Wkv x_kv) (Attention, ns2.py:1029-1053, bias-free) from the forward's attention
     output o and log-sum-exp.  to_out / to_q / to_kv gradients go to grads[name + ...]; returns (d x, d x_kv), bf16.
       * self-attention: kv is None and q is the fused (B, N, 3*inner) qkv of one GEMM on x (transposed pack w_q_t),
         so one wgrad and one dgrad cover q, k and v;
       * cross-attention: d kv goes to `d_kv` (a fresh buffer when None).  Given the context x_kv and its transposed pack
         w_kv_t, to_kv's gradient and d x_kv are computed too; otherwise d x_kv is None and to_kv is the caller's.
-    `dropout`: the forward's attention dropout (seed, site, p), or None (see ops.attention)."""
+    `dropout`: the forward's attention dropout (seed, site, p), or None (see ops.attention).  `kv_lens`: the forward's
+    per-sample key counts, or None (see ops.attention_bwd): d kv rows past them come out as exact zeros."""
     B, N = dy.shape[:2]
     inner = heads * 64
     dev = dy.device
@@ -150,7 +155,7 @@ def attention_backward(dy, x, o, lse, q, kv, w_o_t, w_q_t, heads: int, grads: Di
         d_kv = torch.empty(B, kv.shape[1], 2 * inner, device=dev, dtype=bf)
     dq = torch.zeros(B, N, inner, device=dev)
     ops.attention_bwd(q, kv[:, :, :inner], kv[:, :, inner:], o, d_o, lse, dq, d_kv[:, :, :inner], d_kv[:, :, inner:],
-                      heads=heads, dropout=dropout)
+                      heads=heads, dropout=dropout, kv_lens=kv_lens)
     if fused:
         d_q[:, :, :inner].copy_(dq)   # fp32 accumulator -> bf16 slot (layout glue)
         dw = _wgrad(d_q, x)
@@ -316,7 +321,12 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grad
             F.silu(F.linear(mean, lw, lb)).backward(d_pc * (~S["drop"])[:, None])
         grads["to_prompt_cond.1.weight"], grads["to_prompt_cond.1.bias"] = lw.grad, lb.grad
         if want_prompt:   # d prompt, term (b): the mean-pool spreads d mean evenly over the prompt rows
-            ops.add_rows_bcast(input_grads["prompt"], mean.grad.contiguous(), 1.0 / S["pr_Np"])
+            plens = S["prompt_lens"]
+            if plens is None:
+                ops.add_rows_bcast(input_grads["prompt"], mean.grad.contiguous(), 1.0 / S["pr_Np"])
+            else:         # ... over each sample's own rows: d mean[b] / prompt_lens[b] on [0, prompt_lens[b]), zero past
+                ops.add_rows_bcast(input_grads["prompt"], (mean.grad * (1.0 / plens.double()).float()[:, None]).contiguous())
+                ops.mask_rows(input_grads["prompt"], plens)
         dt = dt[:, :model.dim_time]
     off = 0
     for s in range(nst):
@@ -371,6 +381,7 @@ def _conditioning_backward_tokens(model, S, T, d_xkv, grads, want_prompt: bool):
                          dgamma=dgam)
     grads["perceiver_resampler.norm.gamma"] = dgam
     Np = S["pr_Np"]
+    kv_lens = None if S["prompt_lens"] is None else S["prompt_lens"] + M   # keys [latents ; prompt[:prompt_lens]]
     d_proj = z(B, Np, D)
     for i in reversed(range(len(pr.layers))):
         L = S["pr_layers"][i]
@@ -380,7 +391,8 @@ def _conditioning_backward_tokens(model, S, T, d_xkv, grads, want_prompt: bool):
                                          pfx + "1."), dlat_bf)
         # attention over cat(latents, projected prompt): lat += Wo attn(Wq lat, Wkv cat)
         d_lat, d_cat = attention_backward(dlat_bf, L["lat_bf"], L["o"], L["lse"], L["q"], L["kv"], T[f"pr{i}_o"],
-                                          T[f"pr{i}_q"], H, grads, pfx + "0.", x_kv=L["cat"], w_kv_t=T[f"pr{i}_kv"])
+                                          T[f"pr{i}_q"], H, grads, pfx + "0.", x_kv=L["cat"], w_kv_t=T[f"pr{i}_kv"],
+                                          kv_lens=kv_lens)
         ops.accum_bf16(dlat, d_lat)
         ops.accum_bf16(dlat, d_cat[:, :M].contiguous(), dlat_bf)
         ops.accum_bf16(d_proj, d_cat[:, M:].contiguous())
@@ -408,9 +420,10 @@ class DenoiserFunction(torch.autograd.Function):
     """One autograd node for the whole denoiser: forward saves activations, backward runs the kernels above."""
 
     @staticmethod
-    def forward(ctx, model, x, times, prompt, cond, cond_drop_prob, *params):
+    def forward(ctx, model, x, times, prompt, cond, cond_drop_prob, prompt_lens, *params):
         saved = {}
-        out = model._forward_impl(x, times, prompt, cond=cond, cond_drop_prob=cond_drop_prob, saved=saved)
+        out = model._forward_impl(x, times, prompt, cond=cond, cond_drop_prob=cond_drop_prob, saved=saved,
+                                  prompt_lens=prompt_lens)
         ctx.model, ctx.saved = model, saved
         ctx.in_dtypes = (prompt.dtype if prompt is not None else None, cond.dtype if cond is not None else None)
         return out
@@ -428,7 +441,7 @@ class DenoiserFunction(torch.autograd.Function):
             d_prompt = d_prompt.to(ctx.in_dtypes[0])
         if d_cond is not None:
             d_cond = d_cond.to(ctx.in_dtypes[1])
-        return (None, None, None, d_prompt, d_cond, None, *param_grads(ctx.model, grads))
+        return (None, None, None, d_prompt, d_cond, None, None, *param_grads(ctx.model, grads))
 
 
 class MseRowsFunction(torch.autograd.Function):

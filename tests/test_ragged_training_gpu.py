@@ -256,7 +256,7 @@ def test_conditioner_train(mods, inputs):
 def test_natural_speech2_forward(mods, inputs, monkeypatch):
     """Each sample's MSE row is bit-identical to its alone run.  The loss is not the mean of the alone losses: the
     reference's min-SNR weighting broadcasts the (B,) MSE rows against (B, 1, 1) weights (ns2.py:1651-1666), so the
-    loss is mean(mse) * mean(weight)."""
+    loss is mean(mse) * mean(weight).  Its gradients are checked in test_ragged_training_fp64_gpu.py."""
     from naturalspeech2_pytorch_b200 import NaturalSpeech2, training
     from naturalspeech2_pytorch_b200.diffusion import gamma_to_alpha_sigma
     cn, model = mods
@@ -276,7 +276,6 @@ def test_natural_speech2_forward(mods, inputs, monkeypatch):
     common = dict(pitch=inputs["pitch"], times=times, noise=noise)
     loss = ns(audio, text=inputs["text"], prompt=inputs["prompt"], duration=inputs["duration"],
               prompt_lens=PROMPT_LENS, phoneme_lens=TEXT_LENS, **common)
-    loss.backward()
     batch_rows = rows[-1]
     for b, (n, t) in enumerate(zip(PROMPT_LENS, TEXT_LENS)):
         ns(audio[b:b + 1], text=inputs["text"][b:b + 1, :t], prompt=inputs["prompt"][b:b + 1, :n],
@@ -289,8 +288,3 @@ def test_natural_speech2_forward(mods, inputs, monkeypatch):
     assert ns.objective == "v"
     want = batch_rows.double().mean() * weight.double().mean()
     assert abs(loss.item() - want.item()) <= 1e-5 * abs(want.item()), (loss.item(), want.item())
-    for name, p in cn.named_parameters():
-        if p.grad is not None:
-            assert bool(torch.isfinite(p.grad).all()), name
-    for name, p in model.named_parameters():
-        assert p.grad is not None and bool(torch.isfinite(p.grad).all()), name

@@ -92,6 +92,80 @@ def nan_buf(shape, dtype=torch.float32, pad: int = 40, device: str = "cuda"):
     return buf, buf[:n].view(shape)
 
 
+# ---- the flash attention reference (tests/test_attention_edges_gpu.py and the ragged attention suites) ----
+LOG2E = 1.4426950408889634
+ATTN_RL2 = 2.0 ** -6   # relative L2 of every attention output: a few bf16 roundings of P, dS and the stored result
+
+
+def _attn_heads(t, B, H):
+    return t.double().reshape(B, t.shape[1], H, 64).transpose(1, 2)   # (B, H, N, 64)
+
+
+def _attn_merge(t):
+    B, H, N, _ = t.shape
+    return t.transpose(1, 2).reshape(B, N, H * 64)
+
+
+def attention_reference(q, k, v, d_o, H, scale, drop_key_tile=None):
+    """The attention edge suites' reference of softmax(q k^T scale) v on (B, N, H x 64) bf16 operands: float64 o, lse
+    (log2 domain), dq, dk, dv and their element-wise error bounds for the kernel's arithmetic.
+    drop_key_tile: leave keys [128 t, 128 t + 128) out (sensitivity check)."""
+    B = q.shape[0]
+    qh, kh, vh, doh = (_attn_heads(t, B, H) for t in (q, k, v, d_o))
+    if drop_key_tile is not None:
+        keep = torch.ones(kh.shape[2], dtype=torch.bool, device=qh.device)
+        keep[128 * drop_key_tile:128 * (drop_key_tile + 1)] = False
+        kh, vh = kh[:, :, keep], vh[:, :, keep]
+    s = qh @ kh.transpose(-1, -2) * scale
+    p = torch.softmax(s, dim=-1)
+    o = p @ vh
+    lse = torch.logsumexp(s, dim=-1) * LOG2E
+    nq, nk = qh.shape[2], kh.shape[2]
+    # score error: fp32 sum of 64 bf16 products, in log2 units after the scale
+    ds = acc_eps(64) * (qh.abs() @ kh.abs().transpose(-1, -2)).amax(-1) * abs(scale) * LOG2E        # (B, H, Nq)
+    # lse = m + log2(l): score error, fp32 sum of nk exponentials in l, fp32 rounding of m + log2(l)
+    dlse = ds + acc_eps(nk) * LOG2E + 2.0 ** -18 * (1.0 + lse.abs())
+    # relative error of each P element as the kernels form it: bf16 rounding of P + score and lse errors through exp2
+    ep = 2.0 ** -9 + math.log(2.0) * (ds + dlse)                                                      # (B, H, Nq)
+    pv = p @ vh.abs()
+    # o: P's error on both the numerator (P V, an fp32 sum of nk terms) and the normaliser, + bf16 rounding of o
+    b_o = 2 * (ep[..., None] + acc_eps(nk)) * (pv + o.abs()) + U_BF16 * o.abs()
+    dp = doh @ vh.transpose(-1, -2)
+    D = (doh * o).sum(-1, keepdim=True)
+    dS = p * (dp - D)
+    dv = p.transpose(-1, -2) @ doh
+    dk = dS.transpose(-1, -2) @ qh * scale
+    dq = dS @ kh * scale
+    # dS error: P's relative error on |dP - D|; D from the bf16-rounded o (2^-8 of sum |dO||o|); dP's fp32 sum of 64
+    # products; bf16 rounding of dS itself
+    dD = U_BF16 * (doh.abs() * o.abs()).sum(-1, keepdim=True) + acc_eps(64) * (doh.abs() * o.abs()).sum(-1, keepdim=True)
+    e_p = ep[..., None] * p
+    e_dS = (e_p * (dp - D).abs() + p * (acc_eps(64) * (doh.abs() @ vh.abs().transpose(-1, -2)) + dD)
+            + 2.0 ** -9 * dS.abs()) * abs(scale)
+    b_dv = 2 * (e_p.transpose(-1, -2) @ doh.abs() + acc_eps(nq) * (p.transpose(-1, -2) @ doh.abs())) + U_BF16 * dv.abs()
+    b_dk = 2 * (e_dS.transpose(-1, -2) @ qh.abs() + acc_eps(nq) * (dS.abs().transpose(-1, -2) @ qh.abs()) * abs(scale)) \
+        + U_BF16 * dk.abs()
+    b_dq = 2 * (e_dS @ kh.abs() + acc_eps(nk) * (dS.abs() @ kh.abs()) * abs(scale))
+    return dict(o=_attn_merge(o), lse=lse, dq=_attn_merge(dq), dk=_attn_merge(dk), dv=_attn_merge(dv),
+                b_o=_attn_merge(b_o), b_lse=dlse, b_dq=_attn_merge(b_dq), b_dk=_attn_merge(b_dk), b_dv=_attn_merge(b_dv))
+
+
+def attention_inputs(B, H, Nq, Nk, seed, growing_max=False):
+    """q / k / v as column windows of one fused (B, N, 3 inner) projection, d_o as a window of a wider buffer."""
+    inner = H * 64
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    qkv = torch.randn(B, max(Nq, Nk), 3 * inner, device="cuda", generator=g)
+    if growing_max:
+        # scores grow along the key axis (the row maximum moves by far more than 2^8 between key tiles), alternating
+        # signs, and 64 queries of sample 1 with all-equal (zero) scores
+        qkv[:, :Nk, inner:2 * inner] *= torch.linspace(0.2, 12.0, Nk, device="cuda")[None, :, None]
+        qkv[:, :Nk:7, inner:2 * inner] *= -1.0
+        qkv[1, :64, :inner] = 0.0
+    qkv = qkv.to(torch.bfloat16)
+    do_full = torch.randn(B, Nq, inner + 64, device="cuda", generator=g).to(torch.bfloat16)
+    return qkv[:, :Nq, :inner], qkv[:, :Nk, inner:2 * inner], qkv[:, :Nk, 2 * inner:], do_full[..., :inner]
+
+
 @contextmanager
 def sm_limit(sms: int):
     """Every kernel's persistent grid sized for at most `sms` SMs (0 = all) inside the block; yields the previous

@@ -5,88 +5,15 @@ Tile geometry: the forward runs 128 queries x 128-key tiles per CTA (64 query ro
 runs one 128-key tile per CTA (64 keys per warpgroup) over 64-query tiles.  Keys past kv_len in the last tile are
 zero-filled and masked; dQ is summed with fp32 atomics over the key tiles; dK / dV stay in registers.
 """
-import math
-
 import pytest
 import torch
 
-from kernel_check import U_BF16, U_F32, acc_eps, assert_close, assert_nan, assert_rejects
+from kernel_check import (ATTN_RL2, U_F32, assert_close, assert_nan, assert_rejects, attention_inputs,
+                          attention_reference)
 
 pytestmark = pytest.mark.gpu
 bf = torch.bfloat16
 dev = "cuda"
-LOG2E = 1.4426950408889634
-RL2 = 2.0 ** -6   # relative L2 of every attention output: a few bf16 roundings of P, dS and the stored result
-
-
-def _heads(t, B, H):
-    return t.double().reshape(B, t.shape[1], H, 64).transpose(1, 2)   # (B, H, N, 64)
-
-
-def _merge(t):
-    B, H, N, _ = t.shape
-    return t.transpose(1, 2).reshape(B, N, H * 64)
-
-
-def reference(q, k, v, d_o, H, scale, drop_key_tile=None):
-    """float64 o, lse (log2 domain), dq, dk, dv and their element-wise error bounds for the kernel's arithmetic.
-    drop_key_tile: leave keys [128 t, 128 t + 128) out (sensitivity check)."""
-    B = q.shape[0]
-    qh, kh, vh, doh = (_heads(t, B, H) for t in (q, k, v, d_o))
-    if drop_key_tile is not None:
-        keep = torch.ones(kh.shape[2], dtype=torch.bool, device=dev)
-        keep[128 * drop_key_tile:128 * (drop_key_tile + 1)] = False
-        kh, vh = kh[:, :, keep], vh[:, :, keep]
-    s = qh @ kh.transpose(-1, -2) * scale
-    p = torch.softmax(s, dim=-1)
-    o = p @ vh
-    lse = torch.logsumexp(s, dim=-1) * LOG2E
-    nq, nk = qh.shape[2], kh.shape[2]
-    # score error: fp32 sum of 64 bf16 products, in log2 units after the scale
-    ds = acc_eps(64) * (qh.abs() @ kh.abs().transpose(-1, -2)).amax(-1) * abs(scale) * LOG2E        # (B, H, Nq)
-    # lse = m + log2(l): score error, fp32 sum of nk exponentials in l, fp32 rounding of m + log2(l)
-    dlse = ds + acc_eps(nk) * LOG2E + 2.0 ** -18 * (1.0 + lse.abs())
-    # relative error of each P element as the kernels form it: bf16 rounding of P + score and lse errors through exp2
-    ep = 2.0 ** -9 + math.log(2.0) * (ds + dlse)                                                      # (B, H, Nq)
-    pv = p @ vh.abs()
-    # o: P's error on both the numerator (P V, an fp32 sum of nk terms) and the normaliser, + bf16 rounding of o
-    b_o = 2 * (ep[..., None] + acc_eps(nk)) * (pv + o.abs()) + U_BF16 * o.abs()
-    dp = doh @ vh.transpose(-1, -2)
-    D = (doh * o).sum(-1, keepdim=True)
-    dS = p * (dp - D)
-    dv = p.transpose(-1, -2) @ doh
-    dk = dS.transpose(-1, -2) @ qh * scale
-    dq = dS @ kh * scale
-    # dS error: P's relative error on |dP - D|; D from the bf16-rounded o (2^-8 of sum |dO||o|); dP's fp32 sum of 64
-    # products; bf16 rounding of dS itself
-    dD = U_BF16 * (doh.abs() * o.abs()).sum(-1, keepdim=True) + acc_eps(64) * (doh.abs() * o.abs()).sum(-1, keepdim=True)
-    e_p = ep[..., None] * p
-    e_dS = (e_p * (dp - D).abs() + p * (acc_eps(64) * (doh.abs() @ vh.abs().transpose(-1, -2)) + dD)
-            + 2.0 ** -9 * dS.abs()) * abs(scale)
-    b_dv = 2 * (e_p.transpose(-1, -2) @ doh.abs() + acc_eps(nq) * (p.transpose(-1, -2) @ doh.abs())) + U_BF16 * dv.abs()
-    b_dk = 2 * (e_dS.transpose(-1, -2) @ qh.abs() + acc_eps(nq) * (dS.abs().transpose(-1, -2) @ qh.abs()) * abs(scale)) \
-        + U_BF16 * dk.abs()
-    b_dq = 2 * (e_dS @ kh.abs() + acc_eps(nk) * (dS.abs() @ kh.abs()) * abs(scale))
-    return dict(o=_merge(o), lse=lse, dq=_merge(dq), dk=_merge(dk), dv=_merge(dv),
-                b_o=_merge(b_o), b_lse=dlse, b_dq=_merge(b_dq), b_dk=_merge(b_dk), b_dv=_merge(b_dv))
-
-
-def _inputs(B, H, Nq, Nk, seed, growing_max=False):
-    """q / k / v as column windows of one fused (B, N, 3 inner) projection, d_o as a window of a wider buffer."""
-    inner = H * 64
-    g = torch.Generator(device=dev).manual_seed(seed)
-    qkv = torch.randn(B, max(Nq, Nk), 3 * inner, device=dev, generator=g)
-    if growing_max:
-        # scores grow along the key axis (the row maximum moves by far more than 2^8 between key tiles), alternating
-        # signs, and 64 queries of sample 1 with all-equal (zero) scores
-        qkv[:, :Nk, inner:2 * inner] *= torch.linspace(0.2, 12.0, Nk, device=dev)[None, :, None]
-        qkv[:, :Nk:7, inner:2 * inner] *= -1.0
-        qkv[1, :64, :inner] = 0.0
-    qkv = qkv.to(bf)
-    do_full = torch.randn(B, Nq, inner + 64, device=dev, generator=g).to(bf)
-    return qkv[:, :Nq, :inner], qkv[:, :Nk, inner:2 * inner], qkv[:, :Nk, 2 * inner:], do_full[..., :inner]
-
-
 def _wide(B, N, inner, dtype):
     """NaN-filled (B, N, inner + 64) buffer plus one spare row block: outputs go to its first `inner` columns."""
     store = torch.full((B * N + 64, inner + 64), float("nan"), device=dev, dtype=dtype)
@@ -112,16 +39,16 @@ def _run(q, k, v, d_o, H, scale, dq_start=None):
 
 
 def _check(got, ref, what, dq_start=None):
-    assert_close(got["o"], ref["o"], ref["b_o"], RL2, f"{what} o")
-    assert_close(got["lse"], ref["lse"], ref["b_lse"], RL2, f"{what} lse")
+    assert_close(got["o"], ref["o"], ref["b_o"], ATTN_RL2, f"{what} o")
+    assert_close(got["lse"], ref["lse"], ref["b_lse"], ATTN_RL2, f"{what} lse")
     dq = got["dq"].double()
     b_dq = ref["b_dq"]
     if dq_start is not None:   # the call adds into dq_accum: compare the increment (fp32 rounding of the sum)
         dq = dq - dq_start.double()
         b_dq = b_dq + U_F32 * (got["dq"].double().abs() + dq_start.double().abs())
-    assert_close(dq, ref["dq"], b_dq, RL2, f"{what} dq")
-    assert_close(got["dk"], ref["dk"], ref["b_dk"], RL2, f"{what} dk")
-    assert_close(got["dv"], ref["dv"], ref["b_dv"], RL2, f"{what} dv")
+    assert_close(dq, ref["dq"], b_dq, ATTN_RL2, f"{what} dq")
+    assert_close(got["dk"], ref["dk"], ref["b_dk"], ATTN_RL2, f"{what} dk")
+    assert_close(got["dv"], ref["dv"], ref["b_dv"], ATTN_RL2, f"{what} dv")
 
 
 SHAPES = [
@@ -140,49 +67,49 @@ SHAPES = [
 @pytest.mark.parametrize("scale", [None, 0.05, 0.5], ids=["default", "0.05", "0.5"])
 @pytest.mark.parametrize("B,H,Nq,Nk", SHAPES)
 def test_attention_fwd_bwd(B, H, Nq, Nk, scale):
-    q, k, v, d_o = _inputs(B, H, Nq, Nk, seed=B * 1000 + Nq + Nk)
+    q, k, v, d_o = attention_inputs(B, H, Nq, Nk, seed=B * 1000 + Nq + Nk)
     s = 64 ** -0.5 if scale is None else scale
     # dq_accum starts non-zero: the call must add dQ to it
     dq_start = torch.randn(B, Nq, H * 64, device=dev, generator=torch.Generator(device=dev).manual_seed(1))
     got = _run(q, k, v, d_o, H, scale, dq_start=dq_start)
-    _check(got, reference(q, k, v, d_o, H, s), f"B{B} H{H} Nq{Nq} Nk{Nk} scale {s:.4g}", dq_start=dq_start)
+    _check(got, attention_reference(q, k, v, d_o, H, s), f"B{B} H{H} Nq{Nq} Nk{Nk} scale {s:.4g}", dq_start=dq_start)
 
 
 def test_attention_growing_max_fwd_bwd():
     """The adversarial online-softmax inputs of the forward check also go through the backward."""
     B, H, Nq, Nk = 2, 2, 384, 640
-    q, k, v, d_o = _inputs(B, H, Nq, Nk, seed=4, growing_max=True)
+    q, k, v, d_o = attention_inputs(B, H, Nq, Nk, seed=4, growing_max=True)
     got = _run(q, k, v, d_o, H, None)
-    _check(got, reference(q, k, v, d_o, H, 64 ** -0.5), "growing max")
+    _check(got, attention_reference(q, k, v, d_o, H, 64 ** -0.5), "growing max")
 
 
 def test_attention_sensitivity_omit_key_tile():
     """The forward and backward tolerances reject a reference that leaves out key tile 1 of 3 (dK / dV compared on
     the keys both references have)."""
     B, H, Nq, Nk = 2, 4, 64, 300
-    q, k, v, d_o = _inputs(B, H, Nq, Nk, seed=12)
+    q, k, v, d_o = attention_inputs(B, H, Nq, Nk, seed=12)
     got = _run(q, k, v, d_o, H, None)
-    ref = reference(q, k, v, d_o, H, 64 ** -0.5)
+    ref = attention_reference(q, k, v, d_o, H, 64 ** -0.5)
     _check(got, ref, "exact reference")
-    wrong = reference(q, k, v, d_o, H, 64 ** -0.5, drop_key_tile=1)
-    assert_rejects(got["o"], wrong["o"], ref["b_o"], RL2, "o without key tile 1")
-    assert_rejects(got["dq"], wrong["dq"], ref["b_dq"], RL2, "dq without key tile 1")
+    wrong = attention_reference(q, k, v, d_o, H, 64 ** -0.5, drop_key_tile=1)
+    assert_rejects(got["o"], wrong["o"], ref["b_o"], ATTN_RL2, "o without key tile 1")
+    assert_rejects(got["dq"], wrong["dq"], ref["b_dq"], ATTN_RL2, "dq without key tile 1")
     keep = torch.cat([torch.arange(0, 128), torch.arange(256, Nk)]).to(dev)
     for name in ("dk", "dv"):
-        assert_rejects(got[name][:, keep], wrong[name], ref["b_" + name][:, keep], RL2, f"{name} without key tile 1")
+        assert_rejects(got[name][:, keep], wrong[name], ref["b_" + name][:, keep], ATTN_RL2, f"{name} without key tile 1")
 
 
 def test_attention_bwd_determinism():
     """dK / dV are register-resident and stored once: bit-identical across runs.  dQ (fp32 atomics) only within
     tolerance of the first run."""
     B, H, Nq, Nk = 2, 4, 513, 385
-    q, k, v, d_o = _inputs(B, H, Nq, Nk, seed=6)
+    q, k, v, d_o = attention_inputs(B, H, Nq, Nk, seed=6)
     a = _run(q, k, v, d_o, H, None)
     b = _run(q, k, v, d_o, H, None)
     assert torch.equal(a["o"], b["o"]) and torch.equal(a["lse"], b["lse"])
     assert torch.equal(a["dk"], b["dk"]) and torch.equal(a["dv"], b["dv"])
-    ref = reference(q, k, v, d_o, H, 64 ** -0.5)
-    assert_close(b["dq"], a["dq"], 2 * ref["b_dq"], RL2, "dq run-to-run")
+    ref = attention_reference(q, k, v, d_o, H, 64 ** -0.5)
+    assert_close(b["dq"], a["dq"], 2 * ref["b_dq"], ATTN_RL2, "dq run-to-run")
 
 
 @pytest.mark.parametrize("dropout", [None, (7, 3, 0.25)], ids=["plain", "dropout"])
@@ -191,7 +118,7 @@ def test_attention_bwd_single_key_gives_exact_zero_dq_dk(B, H, Nq, dropout):
     """kv_len = 1: the softmax is the constant 1, so dQ and dK are exactly zero (in float64 too: the cross attention
     over one perceiver latent and a one-frame self-attention give exact-zero weight gradients), while dV = P^T dO."""
     from naturalspeech2_pytorch_b200 import ops
-    q, k, v, d_o = _inputs(B, H, Nq, 1, seed=21 + Nq)
+    q, k, v, d_o = attention_inputs(B, H, Nq, 1, seed=21 + Nq)
     inner = H * 64
     o = torch.empty(B, Nq, inner, device=dev, dtype=bf)
     lse = torch.empty(B, H, Nq, device=dev)
@@ -202,5 +129,5 @@ def test_attention_bwd_single_key_gives_exact_zero_dq_dk(B, H, Nq, dropout):
     assert int((dq != 0).sum()) == 0 and int((dk != 0).sum()) == 0
     assert bool(torch.isfinite(dv).all())
     if dropout is None:
-        ref = reference(q, k, v, d_o, H, 64 ** -0.5)
-        assert_close(dv, ref["dv"], ref["b_dv"], RL2, "dv, one key")
+        ref = attention_reference(q, k, v, d_o, H, 64 ** -0.5)
+        assert_close(dv, ref["dv"], ref["b_dv"], ATTN_RL2, "dv, one key")

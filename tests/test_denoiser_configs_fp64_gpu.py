@@ -8,9 +8,10 @@ at other depths and norm counts, the batch splits of the conditioning-vector ker
 differs from the denoiser's (the perceiver keeps the reference's ff_mult 4 whatever the denoiser's is).
 
 Reference and protocol are those of the backward module: the float64 torch port (`oracle.denoiser_torch_port`) on the
-GPU, every parameter and input rounded to bf16 in place; a tensor passes when
-  (i)   rel-L2 <= C_AUTOCAST x the rel-L2 of the port in fp32 under torch.autocast("cuda", bfloat16) + REL_FLOOR,
-  (ii)  rel-L2 <= REL_CEILING,
+GPU, every parameter and input rounded to bf16 in place; a tensor passes when, with the denoiser's family of
+tests/fp64_check.py,
+  (i)   rel-L2 <= C x the rel-L2 of the port in fp32 under torch.autocast("cuda", bfloat16) + floor,
+  (ii)  rel-L2 <= ceiling,
   (iii) it is exactly zero wherever the fp64 value is exactly zero, and finite everywhere.
 Per case: the inference forward (two calls bit-identical), the classifier-free-guided forward (cond_scale 3) of the
 conditional ones, CUDA-graph replay against the eager launches, and the training backward (every parameter gradient,
@@ -31,7 +32,7 @@ tensor, and the tightest use of a bound:
   n1_b33     transformer.layers.0.5.0.weight             7.2e-3 / 1.2e-2   53 % (to_pred gamma)
 The whole output of the inference forward sits at 3.7e-3 ... 4.7e-3 (autocast-bf16 7.0e-3 ... 9.4e-3), the guided one
 at 6.0e-3 ... 6.5e-3 (1.1e-2 ... 1.2e-2).  On every tensor of every case ours / autocast-bf16 <= 0.80, hence
-C_AUTOCAST = 1 and the ceiling of the backward module; the tightest tensor uses 73 % of its bound.  The wrong
+C = 1 and the ceiling of the backward module; the tightest tensor uses 73 % of its bound.  The wrong
 references sit at rel-L2 0.56 - 0.67 (perceiver tile) and 1.17 (dilation).  The whole module takes ~25 s, w1024_b50
 (320 M parameters) ~6 s of it.
 """
@@ -40,38 +41,17 @@ import time
 import pytest
 import torch
 
+from fp64_check import DENOISER, assert_rejected, bf, bound, compare, over, round_params
 from helpers import build_model, oracle_config
 from oracle import denoiser_torch_port as tp
-from test_denoiser_backward_fp64_gpu import _drop_masks, _port_grads
+from restatements import DENOISER_CASES as CASES
+from restatements import drop_masks, port_grads
 
 pytestmark = pytest.mark.gpu
 
-C_AUTOCAST = 1.0     # measured ratio ours / autocast-bf16 <= 0.80 on every tensor of every case
-REL_FLOOR = 2e-3
-REL_CEILING = 1.5e-2  # measured worst 1.1e-2 (g5_d3)
-
-COND = dict(condition_on_prompt=True)
-CASES = {
-    # name: (model kwargs, B, N, prompt length, cond frames, cond_drop_prob)
-    "g1_h1": (dict(dim=256, depth=1, heads=1, wavenet_layers=1, wavenet_stacks=1), 3, 200, None, None, 0.),
-    "g5_d3": (dict(dim=384, depth=3, heads=5, wavenet_layers=5, wavenet_stacks=3, dim_cond_mult=2), 2, 129, None, None, 0.),
-    "ff2_cond": (dict(dim=128, depth=2, heads=2, ff_mult=2, wavenet_layers=3, wavenet_stacks=2, dim_prompt=192, **COND),
-                 3, 160, 40, 150, .5),
-    "ff8_cond": (dict(dim=128, depth=1, heads=4, ff_mult=8, dim_cond_mult=1, wavenet_layers=2, wavenet_stacks=2,
-                      dim_prompt=128, **COND), 2, 97, 25, 200, 0.),
-    "w640_m1": (dict(dim=640, depth=2, heads=10, wavenet_layers=7, wavenet_stacks=2, dim_cond_mult=3, dim_prompt=64,
-                     num_latents_m=1, resampler_depth=1, **COND), 2, 300, 1, 300, 0.),
-    "w1024_b50": (dict(dim=1024, depth=1, heads=16, wavenet_layers=8, wavenet_stacks=1, dim_prompt=1088, num_latents_m=33,
-                       resampler_depth=3, **COND), 50, 37, 19, 20, 0.),
-    "n1_b33": (dict(dim=128, depth=1, heads=2, wavenet_layers=8, wavenet_stacks=2), 33, 1, None, None, 0.),
-}
 # cases whose parameters, inputs and gradients are kept for the sensitivity tests
 KEEP = {"ff2_cond": ("perceiver_resampler.layers.0.1.0.weight", "perceiver_resampler.layers.1.1.0.weight"),
         "g5_d3": ("wavenet.stacks.2.blocks.4.conv.weight",)}
-
-
-def _rel(got, ref):
-    return float((got.double() - ref).norm() / ref.norm())
 
 
 def _port_out(params, kwargs, inp, drop, dtype=torch.float64, autocast=False):
@@ -92,18 +72,6 @@ def _guided_ref(params, kwargs, inp, **kw):
     return n + 3.0 * (c - n)
 
 
-def _stat(o, r, r_ac):
-    """(rel-L2 ours, rel-L2 autocast twin, non-zero count where the reference is exactly zero, count of those zeros,
-    finite) of one tensor."""
-    o = o.reshape(r.shape)
-    zero = r == 0
-    nz = int((o[zero] != 0).sum()) if bool(zero.any()) else 0
-    finite = bool(torch.isfinite(o).all())
-    if bool(zero.all()) or not finite:
-        return (0.0, 0.0, nz, int(zero.sum()), finite)
-    return (_rel(o, r), _rel(r_ac, r), nz, int(zero.sum()), finite)
-
-
 _CACHE = {}
 
 
@@ -115,22 +83,26 @@ def _case(name):
     kwargs, B, N, Np, Lc, p = CASES[name]
     t0 = time.perf_counter()
     model = build_model(kwargs, 1234, device="cuda")
-    with torch.no_grad():
-        for prm in model.parameters():
-            prm.copy_(prm.bfloat16().float())        # the packs hold exactly these values
+    round_params(model)
     D = kwargs["dim"]
     g = torch.Generator().manual_seed(20)
-    bf = lambda *s: torch.randn(*s, generator=g).bfloat16().float().cuda()  # noqa: E731
-    inp = {"x": bf(B, N, D), "times": torch.rand(B, generator=g).cuda()}
+    inp = {"x": bf(g, B, N, D), "times": torch.rand(B, generator=g).cuda()}
     cond = Np is not None
     if cond:
-        inp["prompt"], inp["cond"] = bf(B, Np, kwargs["dim_prompt"]), bf(B, kwargs["dim_prompt"], Lc)
-    d_out = bf(B, N, D)
-    seed, dp, dc = _drop_masks(B, p)
+        inp["prompt"], inp["cond"] = bf(g, B, Np, kwargs["dim_prompt"]), bf(g, B, kwargs["dim_prompt"], Lc)
+    d_out = bf(g, B, N, D)
+    seed, dp, dc = drop_masks(B, p)
     drop = (dp, dc) if cond else (None, None)
     fkw = dict(prompt=inp["prompt"], cond=inp["cond"], cond_drop_prob=p) if cond else {}
     params = {n: prm.detach() for n, prm in model.named_parameters()}
-    res = dict(kwargs=kwargs, stats={}, checks={})
+    res = dict(kwargs=kwargs, stats={}, fails=[], checks={})
+
+    def stat(n, o, r, r_ac):
+        s = compare(o, r, r_ac)
+        if isinstance(s, str):
+            res["fails"].append((n, s))
+        elif s is not None:
+            res["stats"][n] = s
 
     def reseed():
         if seed is not None:
@@ -143,14 +115,14 @@ def _case(name):
     reseed()
     out2 = model(inp["x"], inp["times"], **fkw)
     res["checks"]["repeat bit-identical"] = torch.equal(out, out2)
-    res["stats"]["forward"] = _stat(out, _port_out(params, kwargs, inp, drop),
-                                    _port_out(params, kwargs, inp, drop, torch.float32, autocast=True))
+    stat("forward", out, _port_out(params, kwargs, inp, drop),
+         _port_out(params, kwargs, inp, drop, torch.float32, autocast=True))
     # ---- classifier-free guidance ----
     if cond:
         guided = model.forward_with_cond_scale(inp["x"], inp["times"], prompt=inp["prompt"], cond=inp["cond"],
                                                cond_scale=3.)
-        res["stats"]["guided forward"] = _stat(guided, _guided_ref(params, kwargs, inp),
-                                               _guided_ref(params, kwargs, inp, dtype=torch.float32, autocast=True))
+        stat("guided forward", guided, _guided_ref(params, kwargs, inp),
+             _guided_ref(params, kwargs, inp, dtype=torch.float32, autocast=True))
     # ---- CUDA graphs: replay against the eager launches (cached conditioning, no drop) ----
     gkw = {}
     if cond:
@@ -176,12 +148,12 @@ def _case(name):
     ours.update({f"d {k}": v.grad for k, v in X.items()})
     del tout, X, out
 
-    ref = _port_grads(params, kwargs, inp, drop, d_out)
-    ac = _port_grads(params, kwargs, inp, drop, d_out, dtype=torch.float32, autocast=True)
+    ref = port_grads(params, kwargs, inp, drop, d_out)
+    ac = port_grads(params, kwargs, inp, drop, d_out, autocast=True)
     assert set(ref) == set(ours)
     for n, r in ref.items():
         assert ours[n] is not None, n
-        res["stats"][n] = _stat(ours[n], r, ac[n])
+        stat(n, ours[n], r, ac[n])
     if name in KEEP:
         res.update(params={n: v.clone() for n, v in params.items()}, inp=inp, d_out=d_out, drop=drop,
                    ours={n: ours[n].clone() for n in KEEP[name]})
@@ -195,34 +167,27 @@ def _case(name):
     return res
 
 
-def _bound(rel_ac):
-    return min(C_AUTOCAST * rel_ac + REL_FLOOR, REL_CEILING)
-
-
 @pytest.mark.parametrize("name", list(CASES))
 def test_config_matches_fp64(name):
     r = _case(name)
     stats = r["stats"]
-    compared = {n: s for n, s in stats.items() if s[0] > 0}
-    ranked = sorted(compared.items(), key=lambda kv: kv[1][0] / _bound(kv[1][1]), reverse=True)
-    worst = max(compared.items(), key=lambda kv: kv[1][0])
-    ratio = max(s[0] / s[1] for s in compared.values())
+    compared = {n: s for n, s in stats.items() if s.rel > 0}
+    ranked = sorted(compared.items(), key=lambda kv: kv[1].rel / bound(DENOISER, kv[1].rel_ac), reverse=True)
+    worst = max(compared.items(), key=lambda kv: kv[1].rel)
+    ratio = max(s.rel / s.rel_ac for s in compared.values())
     print(f"\n{name}: {len(compared)} tensors compared in {r['seconds']:.1f} s; worst rel-L2 {worst[0]}: ours "
-          f"{worst[1][0]:.3e} autocast-bf16 {worst[1][1]:.3e}; max ratio ours / autocast-bf16 {ratio:.2f}; "
-          f"tightest {ranked[0][0]} at {ranked[0][1][0] / _bound(ranked[0][1][1]):.0%} of its bound")
-    for n, (rel, rel_ac, nz, zeros, _) in ranked[:6]:
-        print(f"  {n}: rel-L2 ours {rel:.3e} / autocast-bf16 {rel_ac:.3e} (bound {_bound(rel_ac):.3e}), "
-              f"{zeros} exact zeros")
+          f"{worst[1].rel:.3e} autocast-bf16 {worst[1].rel_ac:.3e}; max ratio ours / autocast-bf16 {ratio:.2f}; "
+          f"tightest {ranked[0][0]} at {ranked[0][1].rel / bound(DENOISER, ranked[0][1].rel_ac):.0%} of its bound")
+    for n, s in ranked[:6]:
+        print(f"  {n}: rel-L2 ours {s.rel:.3e} / autocast-bf16 {s.rel_ac:.3e} (bound {bound(DENOISER, s.rel_ac):.3e}), "
+              f"{s.zeros} exact zeros")
     for n in ("forward", "guided forward"):
         if n in stats:
-            print(f"  {n}: rel-L2 ours {stats[n][0]:.3e} / autocast-bf16 {stats[n][1]:.3e}")
+            print(f"  {n}: rel-L2 ours {stats[n].rel:.3e} / autocast-bf16 {stats[n].rel_ac:.3e}")
     bad_checks = [k for k, ok in r["checks"].items() if not ok]
     assert not bad_checks, bad_checks
-    nonfinite = [n for n, s in stats.items() if not s[4]]
-    assert not nonfinite, nonfinite[:8]
-    zero_fail = [(n, s[2], s[3]) for n, s in stats.items() if s[2]]
-    assert not zero_fail, f"non-zero where the fp64 value is exactly zero (name, count, zeros): {zero_fail[:8]}"
-    bad = [(n, s[0], s[1]) for n, s in ranked if s[0] > _bound(s[1])]
+    assert not r["fails"], f"non-finite, or non-zero where the fp64 value is exactly zero: {r['fails'][:8]}"
+    bad = [(n, s.rel, s.rel_ac) for n, s in ranked if over(DENOISER, s)]
     assert not bad, f"{len(bad)} tensors over the bound (name, rel-L2, autocast rel-L2): {bad[:8]}"
 
 
@@ -243,11 +208,7 @@ def test_single_frame_conv_taps_are_exact_zeros():
 
 
 def _assert_rejected(r, wrong, names):
-    for n in names:
-        rel = _rel(r["ours"][n].reshape(wrong[n].shape), wrong[n])
-        b = _bound(r["stats"][n][1])
-        print(f"  {n}: rel-L2 vs the wrong reference {rel:.3e} (bound {b:.3e})")
-        assert rel > b, f"{n}: the bound accepts a wrong reference (rel-L2 {rel:.3e})"
+    assert_rejected(r["ours"], wrong, r["stats"], names, DENOISER)
 
 
 def test_rejects_perceiver_feedforward_missing_its_last_tile():
@@ -261,7 +222,7 @@ def test_rejects_perceiver_feedforward_missing_its_last_tile():
         params[key] = params[key].clone()
         params[key][:, 256:] = 0
     names = list(KEEP["ff2_cond"])
-    wrong = _port_grads(params, r["kwargs"], r["inp"], r["drop"], r["d_out"], only=names)
+    wrong = port_grads(params, r["kwargs"], r["inp"], r["drop"], r["d_out"], only=names)
     _assert_rejected(r, wrong, names)
 
 
@@ -272,5 +233,5 @@ def test_rejects_reference_with_one_dilation_off():
     dil = [[2 ** i for i in range(kw["wavenet_layers"])] for _ in range(kw["wavenet_stacks"])]
     dil[-1][4] = 8
     names = list(KEEP["g5_d3"])
-    wrong = _port_grads(r["params"], kw, r["inp"], r["drop"], r["d_out"], dilations=dil, only=names)
+    wrong = port_grads(r["params"], kw, r["inp"], r["drop"], r["d_out"], dilations=dil, only=names)
     _assert_rejected(r, wrong, names)

@@ -6,9 +6,9 @@ The reference is `oracle.encoders_oracle.duration_pitch_predictor`, pinned to th
 tests/test_encoders_cpu.py (and, with a token table, the table gathered in front of it).  Both sides see the same
 operands: every parameter is rounded to bf16 in place, inputs, prompts and upstream gradients are bf16-representable.
 The fp64 reference runs with cuDNN off, so conv taps that only read the zero padding get exactly zero gradients.
-Every parameter gradient, d x (or the token table's gradient) and d prompts are compared whole, with the bounds of
-tests/test_conditioning_backward_fp64_gpu.py: rel-L2 <= C_AUTOCAST x the rel-L2 of the same restatement under bf16
-autocast + REL_FLOOR, and <= REL_CEILING; exact zeros where fp64 is zero; nothing non-finite.  to_q needs no bound of
+Every parameter gradient, d x (or the token table's gradient) and d prompts are compared whole, with the predictor's
+family of tests/fp64_check.py (the encoders' numbers): rel-L2 <= C x the rel-L2 of the same restatement under bf16
+autocast + floor, and <= ceiling; exact zeros where fp64 is zero; nothing non-finite.  to_q needs no bound of
 its own here: the conditioning test bounds it relative to the fused q / kv gradient because nearly flat self-attention
 leaves its exact gradient below the rounding of D = rowsum(dO * O); with the prompts among the keys the predictor's
 attention is not that flat, and to_q meets the common bound (ours at most 1.1 x its autocast twin).  Its error as a
@@ -38,16 +38,16 @@ import time
 import pytest
 import torch
 
+from fp64_check import MARGIN, PREDICTOR, assert_rejected, autograd, bf, bound, compare, over, round_params
 from oracle import encoders_oracle as eo
 from param_fill import fill_module
+from restatements import DPP_DEPTH as DEPTH
+from restatements import DPP_DIM as DIM
+from restatements import DPP_HEADS as HEADS
+from restatements import TRUNKS, predictor_fwd, set_head_biases
 
 pytestmark = pytest.mark.gpu
 
-C_AUTOCAST = 1.5
-REL_FLOOR = 2e-3
-REL_CEILING = 2e-2
-MARGIN = 20.0
-DIM, HEADS, DEPTH = 512, 8, 10
 NUM_TOKENS = 100
 CASES = {
     # name: (B, T, Np, token table, which predictions get a gradient)
@@ -57,23 +57,10 @@ CASES = {
     "table": (2, 50, 40, True, "both"),
     "dur_only": (2, 40, 30, False, "duration"),
 }
-TRUNKS = ("to_duration_pred.", "to_pitch_pred.")
-
-
-def _rel(got, ref):
-    return float((got.double() - ref).norm() / ref.norm())
 
 
 def _is_q(name):
     return name.endswith(".2.to_q.weight")
-
-
-def _rel_qkv(got, ref, ref_kv):
-    return float((got.double() - ref).norm() / torch.cat((ref, ref_kv)).norm())
-
-
-def _bf(g, *shape, scale=1.0):
-    return (torch.randn(*shape, generator=g) * scale).bfloat16().float().cuda()
 
 
 def _predictor(table):
@@ -81,23 +68,9 @@ def _predictor(table):
     m = DurationPitchPredictor(dim=DIM, num_phoneme_tokens=NUM_TOKENS if table else None)
     fill_module(m, 4321)
     m.cuda()
-    with torch.no_grad():
-        for p in m.parameters():
-            p.copy_(p.bfloat16().float())
+    round_params(m)
     assert (m.heads, len(m.to_duration_pred.layers), len(m.to_duration_pred.layers[0][0])) == (HEADS, DEPTH, 3)
     return m
-
-
-def _oracle(x, prompts, table, groups=8, trunk=None, heads=HEADS):
-    """Restatement -> fwd(P, dtype) = {"duration": ..., "pitch": ...}; `x` are ids when `table`."""
-    trunk = trunk or eo._trunk
-
-    def fwd(P, dtype):
-        h = P["phoneme_token_emb.weight"][x] if table else x.to(dtype)
-        sub = lambda pfx: {k: v for k, v in P.items() if k.startswith(pfx)}  # noqa: E731
-        return {"duration": trunk(sub(TRUNKS[0]), TRUNKS[0], h, prompts.to(dtype), heads, groups=groups),
-                "pitch": trunk(sub(TRUNKS[1]), TRUNKS[1], h, prompts.to(dtype), heads, groups=groups)}
-    return fwd
 
 
 def _trunk_without_query_keys(P, pre, x, prompts, heads, groups=8, eps=1e-5):
@@ -124,64 +97,6 @@ def _trunk_without_query_keys(P, pre, x, prompts, heads, groups=8, eps=1e-5):
     return F.relu(x @ P[pre + "to_pred.0.weight"].T + P[pre + "to_pred.0.bias"]).squeeze(-1)
 
 
-def _ref_grads(fwd, params, inputs, d_outs, autocast=False, only=None):
-    """{name: gradient} of `fwd` in fp64 (or fp32 under bf16 autocast) w.r.t. the parameters and the float inputs."""
-    dtype = torch.float32 if autocast else torch.float64
-    P = {n: p.detach().to(dtype).requires_grad_(True) for n, p in params.items()}
-    leaves = dict(P)
-    for n, t in inputs.items():
-        if t.is_floating_point():
-            leaves[n] = t.detach().to(dtype).requires_grad_(True)
-    names = list(leaves) if only is None else list(only)
-    with torch.backends.cudnn.flags(enabled=False):
-        with torch.autocast("cuda", dtype=torch.bfloat16, enabled=autocast):
-            outs = _call(fwd, P, leaves, dtype)
-        used = [(o, d_outs[k]) for k, o in outs.items() if d_outs.get(k) is not None]
-        g = torch.autograd.grad([o for o, _ in used], [leaves[n] for n in names],
-                                [d.to(o.dtype) for o, d in used], allow_unused=True)
-    res = {n: torch.zeros_like(leaves[n]) if gi is None else gi.detach() for n, gi in zip(names, g)}
-    if only is None:
-        res.update({"out " + k: o.detach() for k, o in outs.items()})
-    return res
-
-
-def _call(fwd, P, leaves, dtype):
-    return fwd(P, dtype, leaves) if getattr(fwd, "takes_leaves", False) else fwd(P, dtype)
-
-
-def _with_leaves(x, prompts, table, **kw):
-    """The oracle on the (differentiable) input leaves "x" / "prompts" when present."""
-    def fwd(P, dtype, leaves):
-        return _oracle(leaves.get("x", x), leaves.get("prompts", prompts), table, **kw)(P, dtype)
-    fwd.takes_leaves = True
-    return fwd
-
-
-def _set_head_biases(m, x, prompts, table, heads=HEADS):
-    """Head biases (bf16 values) that keep every fp64 pre-activation away from 0; returns them per trunk."""
-    P = {n: p.detach().double() for n, p in m.named_parameters()}
-    for t in TRUNKS:
-        P[t + "to_pred.0.bias"] = torch.full_like(P[t + "to_pred.0.bias"], 1e3)
-    with torch.backends.cudnn.flags(enabled=False):
-        outs = _oracle(x, prompts, table, heads=heads)(P, torch.float64)
-    biases = {}
-    for t, key in zip(TRUNKS, ("duration", "pitch")):
-        pre = (outs[key] - 1e3).flatten().sort().values           # pre-activations without the bias
-        spread = float(pre[-1] - pre[0]) + 1e-3
-        lo, hi = int(0.2 * pre.numel()), int(0.8 * pre.numel())
-        gaps = pre[lo + 1:hi + 1] - pre[lo:hi] if hi > lo else pre[:0]
-        if gaps.numel() and float(gaps.max()) > 0.2 * spread:     # room for dead and live rows on both sides
-            i = lo + int(gaps.argmax())
-            b = -0.5 * float(pre[i] + pre[i + 1])
-        else:                                                       # every row alive
-            b = 0.25 * spread - float(pre[0])
-        biases[t] = torch.tensor(b).bfloat16().float().item()
-        with torch.no_grad():
-            m.get_submodule(t[:-1]).to_pred[0].bias.fill_(biases[t])
-    m.invalidate_packed()
-    return biases
-
-
 _CACHE = {}
 
 
@@ -192,10 +107,10 @@ def _case(name):
     B, T, Np, table, which = CASES[name]
     m = _predictor(table)
     g = torch.Generator().manual_seed(7 + list(CASES).index(name))
-    x = torch.randint(0, NUM_TOKENS, (B, T), generator=g).cuda() if table else _bf(g, B, T, DIM)
-    prompts = _bf(g, B, Np, DIM)
-    biases = _set_head_biases(m, x, prompts, table)
-    d_outs = {"duration": _bf(g, B, T, scale=0.05), "pitch": _bf(g, B, T, scale=0.05) if which == "both" else None}
+    x = torch.randint(0, NUM_TOKENS, (B, T), generator=g).cuda() if table else bf(g, B, T, DIM)
+    prompts = bf(g, B, Np, DIM)
+    biases = set_head_biases(m, x, prompts, table)
+    d_outs = {"duration": bf(g, B, T, scale=0.05), "pitch": bf(g, B, T, scale=0.05) if which == "both" else None}
 
     # ours
     m.train()
@@ -216,9 +131,10 @@ def _case(name):
 
     params = {n: p.detach() for n, p in m.named_parameters()}
     inputs = {"prompts": prompts} if table else {"x": x, "prompts": prompts}
-    fwd = _with_leaves(x, prompts, table)
-    ref = _ref_grads(fwd, params, inputs, d_outs)
-    ac = _ref_grads(fwd, params, inputs, d_outs, autocast=True)
+    fwd = predictor_fwd(x, prompts, table)
+    # cuDNN off for both runs: conv taps that only read the zero padding get exact zeros
+    ref = autograd(fwd, params, d_outs, inputs=inputs, cudnn=False, out_prefix="out ")
+    ac = autograd(fwd, params, d_outs, autocast=True, inputs=inputs, cudnn=False, out_prefix="out ")
 
     # the ReLU margin: every fp64 pre-activation at least MARGIN x our forward's max-abs error away from 0
     fwd_err = max(float((ours["out " + k].double() - ref["out " + k]).abs().max()) for k in ("duration", "pitch"))
@@ -226,27 +142,23 @@ def _case(name):
     for t in TRUNKS:
         P64[t + "to_pred.0.bias"] = P64[t + "to_pred.0.bias"] + 1e3
     with torch.backends.cudnn.flags(enabled=False):
-        pre = _oracle(x, prompts, table)(P64, torch.float64)
+        pre = predictor_fwd(x, prompts, table)(P64, torch.float64)
     min_pre = min(float((pre[k] - 1e3).abs().min()) for k in ("duration", "pitch"))
     dead = sum(int((pre[k] - 1e3 < 0).sum()) for k in ("duration", "pitch"))
 
-    stats, zero_fail, nonfinite, none_ok = {}, [], [], True
+    stats, fails, none_ok = {}, [], True
     for n, r in ref.items():
         o = ours.get(n)
         if which == "duration" and n.startswith(TRUNKS[1]):
             none_ok &= o is None
             continue
         assert o is not None and o.shape == r.shape, n
-        if not bool(torch.isfinite(o).all()):
-            nonfinite.append(n)
-            continue
-        zero = r == 0
-        if bool(zero.any()) and bool((o[zero] != 0).any()):
-            zero_fail.append((n, int((o[zero] != 0).sum()), int(zero.sum())))
-        if bool(zero.all()) or n.startswith("out "):
-            continue
-        stats[n] = (_rel(o, r), _rel(ac[n], r), _rel_qkv(o, r, ref[n.replace("to_q", "to_kv")]) if _is_q(n) else None)
-    res = dict(stats=stats, zero_fail=zero_fail, nonfinite=nonfinite, none_ok=none_ok, fwd_err=fwd_err,
+        s = compare(o, r, ac[n], ref[n.replace("to_q", "to_kv")] if _is_q(n) else None)
+        if isinstance(s, str):
+            fails.append((n, s))
+        elif s is not None and not n.startswith("out "):
+            stats[n] = s
+    res = dict(stats=stats, fails=fails, none_ok=none_ok, fwd_err=fwd_err,
                min_pre=min_pre, dead=dead, biases=biases, train_equals_eval=train_equals_eval, params=params,
                inputs=inputs, d_outs=d_outs, x=x, prompts=prompts, table=table,
                ours={n: ours[n].clone() for n in ("to_duration_pred.layers.0.0.0.blocks.0.proj.weight",
@@ -261,35 +173,25 @@ def _case(name):
     return res
 
 
-def _bound(rel_ac):
-    return min(C_AUTOCAST * rel_ac + REL_FLOOR, REL_CEILING)
-
-
-def _over(name, s):
-    return s[0] > _bound(s[1])
-
-
 @pytest.mark.parametrize("name", list(CASES))
 def test_backward_matches_fp64_autograd(name):
     r = _case(name)
     stats = r["stats"]
-    rest = stats
     q = {n: s for n, s in stats.items() if _is_q(n)}
-    worst = max(rest.items(), key=lambda kv: kv[1][0])
-    ratio = max(((n, s) for n, s in rest.items() if s[1] > 0), key=lambda kv: kv[1][0] / kv[1][1])
-    use = max(rest.items(), key=lambda kv: kv[1][0] / _bound(kv[1][1]))
-    worst_q = max(q.items(), key=lambda kv: kv[1][2])
-    print(f"\n{name}: {len(stats)} tensors in {r['seconds']:.1f} s; worst rel-L2 {worst[0]} ours {worst[1][0]:.3e} / "
-          f"autocast {worst[1][1]:.3e}; max ratio {ratio[1][0] / ratio[1][1]:.2f} ({ratio[0]}); tightest "
-          f"{use[0]} at {use[1][0] / _bound(use[1][1]):.0%} of its bound; worst to_q {worst_q[0]} {worst_q[1][2]:.3e}; "
-          f"forward max-abs {r['fwd_err']:.3e}, min |pre| {r['min_pre']:.3e}, dead rows {r['dead']}, "
-          f"head biases {r['biases']}")
+    worst = max(stats.items(), key=lambda kv: kv[1].rel)
+    ratio = max(((n, s) for n, s in stats.items() if s.rel_ac > 0), key=lambda kv: kv[1].rel / kv[1].rel_ac)
+    use = max(stats.items(), key=lambda kv: kv[1].rel / bound(PREDICTOR, kv[1].rel_ac))
+    worst_q = max(q.items(), key=lambda kv: kv[1].share)
+    print(f"\n{name}: {len(stats)} tensors in {r['seconds']:.1f} s; worst rel-L2 {worst[0]} ours {worst[1].rel:.3e} / "
+          f"autocast {worst[1].rel_ac:.3e}; max ratio {ratio[1].rel / ratio[1].rel_ac:.2f} ({ratio[0]}); tightest "
+          f"{use[0]} at {use[1].rel / bound(PREDICTOR, use[1].rel_ac):.0%} of its bound; worst to_q {worst_q[0]} "
+          f"{worst_q[1].share:.3e}; forward max-abs {r['fwd_err']:.3e}, min |pre| {r['min_pre']:.3e}, dead rows "
+          f"{r['dead']}, head biases {r['biases']}")
     assert r["min_pre"] >= MARGIN * r["fwd_err"], "fixture: a head pre-activation lies too close to 0"
     assert r["train_equals_eval"], "the training forward must be bit-identical to the inference forward"
     assert r["none_ok"], "a trunk without an upstream gradient must leave its parameters' .grad None"
-    assert not r["nonfinite"], r["nonfinite"][:8]
-    assert not r["zero_fail"], f"non-zero where the fp64 value is exactly zero: {r['zero_fail'][:8]}"
-    bad = [(n, s) for n, s in stats.items() if _over(n, s)]
+    assert not r["fails"], f"non-finite, or non-zero where the fp64 value is exactly zero: {r['fails'][:8]}"
+    bad = [(n, s) for n, s in stats.items() if over(PREDICTOR, s)]
     assert not bad, f"{len(bad)} tensors over the bound: {bad[:8]}"
 
 
@@ -303,42 +205,40 @@ def test_short_cases_cover_dead_rows_and_padding_taps():
 
 # ---- wrong references ----
 def _assert_rejected(r, wrong, names):
-    for n in names:
-        s = r["stats"][n]
-        rel = _rel(r["ours"][n], wrong[n])
-        print(f"  {n}: rel-L2 vs the wrong reference {rel:.3e} (bound {_bound(s[1]):.3e})")
-        assert rel > _bound(s[1]), f"the bound accepts a wrong reference for {n}"
+    assert_rejected(r["ours"], wrong, r["stats"], names, PREDICTOR)
+
+
+def _wrong(r, fwd, d_outs, names):
+    return autograd(fwd, r["params"], d_outs, inputs=r["inputs"], only=names, cudnn=False)
 
 
 def test_rejects_reversed_conv_taps():
     r = _case("main")
     key = "to_duration_pred.layers.0.0.0.blocks.0.proj.weight"
-    base = _with_leaves(r["x"], r["prompts"], r["table"])
+    base = predictor_fwd(r["x"], r["prompts"], r["table"])
 
-    def fwd(P, dtype, leaves):
-        return base(dict(P, **{key: P[key].flip(-1)}), dtype, leaves)
-    fwd.takes_leaves = True
-    _assert_rejected(r, _ref_grads(fwd, r["params"], r["inputs"], r["d_outs"], only=[key]), [key])
+    def fwd(P, dtype):
+        return base(dict(P, **{key: P[key].flip(-1)}), dtype)
+    _assert_rejected(r, _wrong(r, fwd, r["d_outs"], [key]), [key])
 
 
 def test_rejects_wrong_group_count():
     r = _case("main")
     names = ["to_duration_pred.layers.9.0.2.blocks.1.norm.weight"]
-    fwd = _with_leaves(r["x"], r["prompts"], r["table"], groups=4)
-    _assert_rejected(r, _ref_grads(fwd, r["params"], r["inputs"], r["d_outs"], only=names), names)
+    fwd = predictor_fwd(r["x"], r["prompts"], r["table"], groups=4)
+    _assert_rejected(r, _wrong(r, fwd, r["d_outs"], names), names)
 
 
 def test_rejects_keys_without_the_queries():
     r = _case("main")
     names = ["to_duration_pred.layers.9.2.to_kv.weight", "prompts"]
-    fwd = _with_leaves(r["x"], r["prompts"], r["table"], trunk=_trunk_without_query_keys)
-    _assert_rejected(r, _ref_grads(fwd, r["params"], r["inputs"], r["d_outs"], only=names), names)
+    fwd = predictor_fwd(r["x"], r["prompts"], r["table"], trunk=_trunk_without_query_keys)
+    _assert_rejected(r, _wrong(r, fwd, r["d_outs"], names), names)
 
 
 def test_rejects_swapped_trunks():
     r = _case("main")
     names = ["to_duration_pred.layers.0.0.0.blocks.0.proj.weight", "to_pitch_pred.layers.9.0.0.blocks.0.proj.weight"]
     d = r["d_outs"]
-    fwd = _with_leaves(r["x"], r["prompts"], r["table"])
-    wrong = _ref_grads(fwd, r["params"], r["inputs"], {"duration": d["pitch"], "pitch": d["duration"]}, only=names)
-    _assert_rejected(r, wrong, names)
+    fwd = predictor_fwd(r["x"], r["prompts"], r["table"])
+    _assert_rejected(r, _wrong(r, fwd, {"duration": d["pitch"], "pitch": d["duration"]}, names), names)

@@ -2,7 +2,7 @@
 by default) on the softmax probabilities of every layer's cross attention.  The reference's Blocks keep p = 0
 (tests/test_duration_pitch_dropout_cpu.py reads that from the reference module), so nothing else is dropped.
 
-The reference is `masked_trunk`, oracle.encoders_oracle._trunk with each layer's attention mask applied after its
+The reference is `restatements.masked_trunk`, oracle.encoders_oracle._trunk with each layer's attention mask applied after its
 softmax (attend.py:149), built from tests/dropout_oracle.py with the sites of the predictor's docstring and the seed the
 call drew (re-drawn with torch.manual_seed).  At the reference's default dims (dim 512, depth 10, 8 heads, both
 trunks) the GPU output, every parameter gradient, d x and d prompts are compared with fp64 autograd of it, with the
@@ -33,86 +33,15 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-import dropout_oracle as do
-from oracle import encoders_oracle as eo
 from param_fill import fill_module
+from restatements import DPP_DEPTH as DEPTH
+from restatements import DPP_DIM as DIM
+from restatements import (dpp_train_inputs, dpp_train_loss, drawn_seed, masked_predictor_fp64, masks_for,
+                          set_head_biases_masked, site)
 
 pytestmark = pytest.mark.gpu
-DIM, HEADS, DEPTH = 512, 8, 10
-TRUNKS = ("to_duration_pred.", "to_pitch_pred.")
 MARGIN = 20.0
-SEED_HIGH = 2 ** 63 - 1
 CASES = {"main": (4, 100, 103), "short": (3, 5, 3)}   # (B, T, Np)
-
-
-def site(t, l):
-    """Site of the cross attention of layer l of trunk t (0 duration, 1 pitch)."""
-    return t * DEPTH + l
-
-
-def masks_for(seed, p, B, T, Np, site_of=site, block_sites=None):
-    """{trunk: (block masks [l][j] (B, T, D) or None, attention masks [l] (B, H, T, T + Np))}, keep * scale in fp64 on
-    the GPU.  block_sites(t, l, j): sites for masks after every Block's SiLU (only the wrong reference has them)."""
-    out = {}
-    for t, pre in enumerate(TRUNKS):
-        blocks = None if block_sites is None else [
-            [do.mask_tensor(do.elementwise_mask(seed, block_sites(t, l, j), p, B * T * DIM).reshape(B, T, DIM), p)
-             .cuda() for j in range(6)] for l in range(DEPTH)]
-        attn = [do.mask_tensor(do.attention_mask(seed, site_of(t, l), p, B, HEADS, T, T + Np), p).cuda()
-                for l in range(DEPTH)]
-        out[pre] = (blocks, attn)
-    return out
-
-
-def masked_trunk(P, pre, x, prompts, heads, block_masks=None, attn_masks=None, groups=8, eps=1e-5):
-    """eo._trunk with the attention mask after the softmax (attend.py:149) and, for the wrong reference only, Block j's
-    mask after its SiLU; masks None = no dropout."""
-    for l in range(DEPTH):
-        lp = f"{pre}layers.{l}."
-        j = 0
-        for r in range(3):
-            h = x.transpose(1, 2)
-            for c in range(2):
-                bp = f"{lp}0.{r}.blocks.{c}."
-                w = P[bp + "proj.weight"]
-                h = F.conv1d(h, w, P[bp + "proj.bias"], padding=w.shape[-1] // 2)
-                h = F.silu(F.group_norm(h, groups, P[bp + "norm.weight"], P[bp + "norm.bias"], eps))
-                if block_masks is not None:
-                    h = h * block_masks[l][j].transpose(1, 2).to(h.dtype)
-                j += 1
-            x = h.transpose(1, 2) + x
-        nx = eo._rmsnorm(x, P[lp + "1.gamma"])
-        ctx = torch.cat((nx, prompts), dim=-2)
-        q = nx @ P[lp + "2.to_q.weight"].T
-        k, v = (ctx @ P[lp + "2.to_kv.weight"].T).chunk(2, dim=-1)
-        b, n, _ = q.shape
-        q, k, v = (t.view(b, t.shape[1], heads, -1).transpose(1, 2) for t in (q, k, v))
-        attn = (torch.einsum("bhid,bhjd->bhij", q, k) * (q.shape[-1] ** -0.5)).softmax(dim=-1)
-        if attn_masks is not None:
-            attn = attn * attn_masks[l].to(attn.dtype)
-        o = torch.einsum("bhij,bhjd->bhid", attn, v).transpose(1, 2).reshape(b, n, -1)
-        x = o @ P[lp + "2.to_out.weight"].T + x
-    return F.relu(x @ P[pre + "to_pred.0.weight"].T + P[pre + "to_pred.0.bias"]).squeeze(-1)
-
-
-def _fp64(params, x, prompts, d_outs, masks=None, only=None):
-    """fp64 autograd of the (masked) restatement -> {name: gradient} plus "out duration" / "out pitch"."""
-    P = {n: p.detach().double().requires_grad_(True) for n, p in params.items()}
-    leaves = dict(P, x=x.detach().double().requires_grad_(True), prompts=prompts.detach().double().requires_grad_(True))
-    outs = {}
-    with torch.backends.cudnn.flags(enabled=False):
-        for pre, key in zip(TRUNKS, ("duration", "pitch")):
-            sub = {k: v for k, v in P.items() if k.startswith(pre)}
-            bm, am = masks[pre] if masks is not None else (None, None)
-            outs[key] = masked_trunk(sub, pre, leaves["x"], leaves["prompts"], HEADS, bm, am)
-        if d_outs is None:
-            return {k: o.detach() for k, o in outs.items()}
-        names = list(leaves) if only is None else list(only)
-        g = torch.autograd.grad([outs["duration"], outs["pitch"]], [leaves[n] for n in names],
-                                [d_outs["duration"].double(), d_outs["pitch"].double()], allow_unused=True)
-    res = {n: torch.zeros_like(leaves[n]) if gi is None else gi.detach() for n, gi in zip(names, g)}
-    res.update({"out " + k: o.detach() for k, o in outs.items()})
-    return res
 
 
 def _predictor():
@@ -127,20 +56,6 @@ def _predictor():
     return m
 
 
-def _set_head_biases(m, params, x, prompts, masks):
-    """bf16 head biases that keep every fp64 pre-activation, with and without the masks, well above 0."""
-    P = dict(params)
-    for pre in TRUNKS:
-        P[pre + "to_pred.0.bias"] = torch.full_like(P[pre + "to_pred.0.bias"], 1e3)
-    outs = [_fp64(P, x, prompts, None, mk) for mk in (None, masks)]
-    for pre, key in zip(TRUNKS, ("duration", "pitch")):
-        pres = torch.cat([(o[key] - 1e3).flatten() for o in outs])   # pre-activations without the bias
-        b = 0.25 * float(pres.max() - pres.min()) + 1e-3 - float(pres.min())
-        with torch.no_grad():
-            m.get_submodule(pre[:-1]).to_pred[0].bias.fill_(torch.tensor(b).bfloat16().float().item())
-    m.invalidate_packed()
-
-
 def _gpu(m, x, prompts, d_outs):
     m.zero_grad(set_to_none=True)
     x_in, p_in = x.clone().requires_grad_(True), prompts.clone().requires_grad_(True)
@@ -149,11 +64,6 @@ def _gpu(m, x, prompts, d_outs):
     res = {n: prm.grad.clone() for n, prm in m.named_parameters()}
     res.update({"x": x_in.grad, "prompts": p_in.grad, "out duration": dur.detach(), "out pitch": pitch.detach()})
     return res
-
-
-def _drawn_seed(torch_seed):
-    torch.manual_seed(torch_seed)
-    return int(torch.randint(0, SEED_HIGH, ()))
 
 
 def _rel_cos(got, ref):
@@ -181,10 +91,10 @@ def _case(name, p):
     x, prompts = bf(B, T, DIM), bf(B, Np, DIM)
     d_outs = {"duration": bf(B, T, scale=0.05), "pitch": bf(B, T, scale=0.05)}
     torch_seed = 900 + int(p * 10) + 7 * list(CASES).index(name)
-    seed = _drawn_seed(torch_seed)
+    seed = drawn_seed(torch_seed)
     assert seed >> 32, "the drawn seed should use the key's high word"
     masks = masks_for(seed, p, B, T, Np)
-    _set_head_biases(m, {n: q.detach() for n, q in m.named_parameters()}, x, prompts, masks)
+    set_head_biases_masked(m, {n: q.detach() for n, q in m.named_parameters()}, x, prompts, masks)
     params = {n: q.detach() for n, q in m.named_parameters()}
     m.train()
     m.train_dropout = False
@@ -192,8 +102,8 @@ def _case(name, p):
     m.train_dropout = True
     torch.manual_seed(torch_seed)
     ours = _gpu(m, x, prompts, d_outs)
-    plain_ref = _fp64(params, x, prompts, d_outs)
-    ref = _fp64(params, x, prompts, d_outs, masks)
+    plain_ref = masked_predictor_fp64(params, x, prompts, d_outs)
+    ref = masked_predictor_fp64(params, x, prompts, d_outs, masks)
     fwd_err = max(float((ours[k] - ref[k]).abs().max()) for k in ("out duration", "out pitch"))
     min_pre = min(float(o[k].abs().min()) for o in (ref, plain_ref) for k in ("out duration", "out pitch"))
     stats = {}
@@ -236,7 +146,7 @@ def test_predictor_dropout_matches_fp64_autograd(name, p):
 
 
 def _assert_rejected(r, wrong_masks):
-    wrong = _fp64(r["params"], r["x"], r["prompts"], r["d_outs"], wrong_masks, only=WRONG_NAMES)
+    wrong = masked_predictor_fp64(r["params"], r["x"], r["prompts"], r["d_outs"], wrong_masks, only=WRONG_NAMES)
     for n in WRONG_NAMES:
         (rel, cos), (rel0, cos0) = r["stats"][n][:2]
         wrel, wcos = _rel_cos(r["ours"][n], wrong[n])
@@ -323,7 +233,6 @@ def test_conditional_training_with_predictor_dropout_lowers_both_losses():
     """AdamW steps with the predictor's dropout on lower both L1 losses, evaluated without dropout, on a fixed batch."""
     from naturalspeech2_pytorch_b200 import Model, NaturalSpeech2
     from naturalspeech2_pytorch_b200.encoders import Conditioner
-    from test_duration_pitch_training_gpu import _inputs, _loss
     torch.manual_seed(0)
     cond_net = Conditioner(dim_codebook=128, num_phoneme_tokens=50, train_duration_pitch=True,
                            duration_pitch_dropout=True)
@@ -337,7 +246,7 @@ def test_conditional_training_with_predictor_dropout_lowers_both_losses():
     cond_net.cuda().train()
     model.cuda().train()
     ns = NaturalSpeech2(model, target_sample_hz=24000, timesteps=4, conditioner=cond_net)
-    inp = _inputs()
+    inp = dpp_train_inputs()
     assert cond_net.duration_pitch.train_dropout and cond_net.duration_pitch.attn_dropout == 0.2
 
     def eval_losses():
@@ -354,7 +263,7 @@ def test_conditional_training_with_predictor_dropout_lowers_both_losses():
     losses = []
     for _ in range(6):
         opt.zero_grad(set_to_none=True)
-        loss = _loss(ns, inp)
+        loss = dpp_train_loss(ns, inp)
         loss.backward()
         opt.step()
         losses.append(float(loss.detach()))

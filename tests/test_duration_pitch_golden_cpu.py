@@ -8,14 +8,10 @@ import torch
 import torch.nn.functional as F
 
 from golden.make_golden_dpp_train import DPP_TRAIN_CASES, dpp_train_inputs
+from fp64_check import rel_l2
 from helpers import GOLDEN, build_encoder
 
 Z = np.load(GOLDEN / "grads_dpp_train.npz")
-
-
-def _rel(got, ref):
-    ref = torch.as_tensor(ref).double()
-    return float((got.detach().double() - ref).norm() / ref.norm())
 
 
 @pytest.mark.parametrize("name", list(DPP_TRAIN_CASES))
@@ -48,5 +44,5 @@ def test_oracle_fp64_autograd_matches_the_reference_golden(name):
     norms = np.array([P[n].grad.norm().item() for n in names])
     np.testing.assert_allclose(norms, Z[f"{name}::norms"], rtol=1e-9, atol=1e-12)
     d_in = P["phoneme_token_emb.weight"].grad if table else x.grad
-    assert _rel(d_in, Z[f"{name}::d_table" if table else f"{name}::d_x"]) < 1e-6       # stored as fp32
-    assert _rel(prompts.grad, Z[f"{name}::d_prompts"]) < 1e-6
+    assert rel_l2(d_in, Z[f"{name}::d_table" if table else f"{name}::d_x"]) < 1e-6       # stored as fp32
+    assert rel_l2(prompts.grad, Z[f"{name}::d_prompts"]) < 1e-6

@@ -6,9 +6,10 @@ import torch
 import torch.nn.functional as F
 
 from param_fill import fill_module
+from restatements import DPP_TRAIN_SHAPE, dpp_train_inputs, dpp_train_loss
 
 pytestmark = pytest.mark.gpu
-B, T_TEXT, NP, L = 2, 24, 40, 96
+B, T_TEXT, NP, L = DPP_TRAIN_SHAPE
 W_DUR, W_PITCH = 0.7, 0.3
 
 
@@ -32,23 +33,6 @@ def _setup(flag=True):
     return ns, cond_net, model
 
 
-def _inputs():
-    g = torch.Generator().manual_seed(5)
-    dur = torch.randint(1, 6, (B, T_TEXT), generator=g)
-    dur[:, -1] = 0
-    dur[0, 3] = 0
-    pitch = 100 + 200 * torch.rand(B, L, generator=g)
-    pitch[:, ::5] = 0.0                                              # unvoiced frames
-    return dict(latents=torch.randn(B, L, 128, generator=g).cuda(), prompt=torch.randn(B, NP, 128, generator=g).cuda(),
-                text=torch.randint(0, 50, (B, T_TEXT), generator=g).cuda(), duration=dur.cuda(), pitch=pitch.cuda(),
-                times=torch.rand(B, generator=g).cuda(), noise=torch.randn(B, L, 128, generator=g).cuda())
-
-
-def _loss(ns, inp):
-    return ns(inp["latents"], text=inp["text"], prompt=inp["prompt"], pitch=inp["pitch"], duration=inp["duration"],
-              times=inp["times"], noise=inp["noise"])
-
-
 def _capture(cond_net):
     """Hook that keeps the predictor's outputs."""
     seen = {}
@@ -60,12 +44,12 @@ def _capture(cond_net):
 
 def test_loss_adds_the_weighted_duration_and_pitch_losses():
     from naturalspeech2_pytorch_b200.encoders import average_over_durations
-    inp = _inputs()
+    inp = dpp_train_inputs()
     ns, cond_net, _ = _setup(flag=False)
-    loss_off = _loss(ns, inp)
+    loss_off = dpp_train_loss(ns, inp)
     cond_net.train_duration_pitch = True
     seen, h = _capture(cond_net)
-    loss_on = _loss(ns, inp)
+    loss_on = dpp_train_loss(ns, inp)
     h.remove()
     dur_pred, pitch_pred = seen["pred"]
     ph_pitch = average_over_durations(inp["pitch"][:, None].float(), inp["duration"])[:, 0]
@@ -77,7 +61,7 @@ def test_loss_adds_the_weighted_duration_and_pitch_losses():
 def test_encoder_outputs_receive_the_predictors_input_gradients():
     """With the flag, the gradient reaching each encoder's output is the flag-off one plus that of the weighted L1
     losses through the predictor's node (its d x / d prompts), and every predictor parameter gets a gradient."""
-    inp = _inputs()
+    inp = dpp_train_inputs()
     ns, cond_net, _ = _setup(flag=False)
     params = dict(cond_net.named_parameters())
     encs = ("phoneme_enc", "prompt_enc")
@@ -92,7 +76,7 @@ def test_encoder_outputs_receive_the_predictors_input_gradients():
         outs, hooks = outputs()
         got = {}
         cond_net.zero_grad(set_to_none=True)
-        loss = _loss(ns, inp)
+        loss = dpp_train_loss(ns, inp)
         for n in encs:
             outs[n].register_hook(lambda g, n=n: got.__setitem__(n, g.clone()))
         loss.backward()
@@ -122,13 +106,13 @@ def test_encoder_outputs_receive_the_predictors_input_gradients():
 
 
 def test_two_identical_steps_give_bit_identical_gradients():
-    inp = _inputs()
+    inp = dpp_train_inputs()
     ns, cond_net, model = _setup()
     runs = []
     for _ in range(2):
         cond_net.zero_grad(set_to_none=True)
         model.zero_grad(set_to_none=True)
-        _loss(ns, inp).backward()
+        dpp_train_loss(ns, inp).backward()
         runs.append({n: p.grad.clone() for n, p in cond_net.named_parameters() if n.startswith("duration_pitch.")})
     assert runs[0].keys() == runs[1].keys() and len(runs[0]) > 0
     assert all(torch.equal(runs[0][n], runs[1][n]) for n in runs[0])
@@ -136,14 +120,14 @@ def test_two_identical_steps_give_bit_identical_gradients():
 
 def test_adamw_steps_lower_both_losses():
     from naturalspeech2_pytorch_b200.encoders import average_over_durations
-    inp = _inputs()
+    inp = dpp_train_inputs()
     ns, cond_net, model = _setup()
     opt = torch.optim.AdamW(list(cond_net.parameters()) + list(model.parameters()), lr=1e-5)
     hist = []
     for _ in range(5):
         seen, h = _capture(cond_net)
         opt.zero_grad(set_to_none=True)
-        _loss(ns, inp).backward()
+        dpp_train_loss(ns, inp).backward()
         h.remove()
         ph_pitch = average_over_durations(inp["pitch"][:, None].float(), inp["duration"])[:, 0]
         hist.append((float(F.l1_loss(inp["duration"].float(), seen["pred"][0])),

@@ -13,16 +13,16 @@ more, and the host code turns each configuration into its own segment lists, pac
     384, 768, 1408 and 2816) and 1024 (no padding);
   * ResnetBlocks of 1 and 3 Blocks and layers of 1 and 2 ResnetBlocks (the backward's walk of the saved blocks).
 
-Reference and protocol are those of the two default-dims modules, whose bounds and helpers this module imports: every
-parameter is rounded to bf16 in place, inputs and upstream gradients are bf16-representable, and the reference is the
+Reference and protocol are those of the two default-dims modules, with the encoders' family of tests/fp64_check.py:
+every parameter is rounded to bf16 in place, inputs and upstream gradients are bf16-representable, and the reference is the
 float64 restatement (`oracle.encoders_oracle`, pinned to the reference modules at these knobs by
 tests/test_encoders_cpu.py and tests/golden/encoder_configs.npz) on the GPU with cuDNN off.  A tensor passes when
-  (i)   rel-L2 <= C_AUTOCAST x the rel-L2 of the same restatement in fp32 under torch.autocast("cuda", bfloat16)
-        + REL_FLOOR,
-  (ii)  rel-L2 <= REL_CEILING,
+  (i)   rel-L2 <= C x the rel-L2 of the same restatement in fp32 under torch.autocast("cuda", bfloat16) + floor,
+  (ii)  rel-L2 <= ceiling,
   (iii) it is exactly zero wherever the fp64 value is exactly zero, and nothing is non-finite.
 The self-attention to_q of the prompt and phoneme encoders is bounded by TO_Q_BOUND relative to the fused q / kv
-gradient, for the reason test_conditioning_backward_fp64_gpu.py gives; the predictor's to_q meets the common bound.
+gradient, for the reason test_conditioning_backward_fp64_gpu.py gives, under fp64_check.EITHER (below); the predictor's
+to_q meets the common bound.
 The predictor's head biases are chosen as in its module, away from the ReLU kink.
 
 Per run: (1) the inference forward against fp64, and two calls bit-identical; (2) the training forward (autograd in
@@ -45,7 +45,7 @@ Two findings shaped the comparison, neither a kernel error:
     to_q therefore passes under the common bound or under TO_Q_BOUND.
   * The predictor's output at T = 1 (dpp_128-T1): the pitch head has three values, and its head bias leaves live rows
     0.14 above the kink, where our 5.2e-3 absolute error (the twin's is 2.5x larger) is rel-L2 2.1e-2 of the pitch
-    alone, over REL_CEILING.  The predictor's output is compared whole, both predictions as one tensor (1.9e-3 there).
+    alone, over the ceiling.  The predictor's output is compared whole, both predictions as one tensor (1.9e-3 there).
 
 Measured on an H100 80GB HBM3 (700 W power limit).  Worst tensor per run, rel-L2 ours / autocast-bf16 of the same
 tensor, and the tightest use of a bound:
@@ -84,33 +84,14 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from fp64_check import (EITHER, ENCODERS, MARGIN, assert_rejected, autograd, bf, bound, compare, over,
+                        use)
 from oracle import encoders_oracle as eo
-from param_fill import fill_module
-from test_conditioning_backward_fp64_gpu import TO_Q_BOUND, _bound, _rel, _rel_qkv, _round_params
-from test_duration_pitch_backward_fp64_gpu import MARGIN, TRUNKS, _ref_grads, _set_head_biases, _with_leaves
+from restatements import DPP, PHON, SPE, TRUNKS, build_config, config_fwd, config_heads, set_head_biases
+from restatements import ENCODER_CONFIGS as CONFIGS
 
 pytestmark = pytest.mark.gpu
 
-SPE, PHON, DPP = "SpeechPromptEncoder", "PhonemeEncoder", "DurationPitchPredictor"
-CONFIGS = {
-    # name: (class, constructor kwargs, ragged lengths, ragged prompt lengths (predictor))
-    "spe_k3_narrow": (SPE, dict(dim_codebook=64, dims=(64, 192, 128), kernel_size=3, padding=1, depth=2, heads=3),
-                      (1, 129, 50), None),
-    "spe_k1_wide": (SPE, dict(dim_codebook=128, dims=(1024,), kernel_size=1, padding=0, depth=1, heads=16),
-                    (1, 300), None),
-    "spe_k11": (SPE, dict(dim_codebook=128, dims=(256, 384), kernel_size=11, padding=5, depth=1, heads=4),
-                (1, 103), None),
-    "phon_d64": (PHON, dict(num_tokens=30, dim=64, dim_hidden=384, kernel_size=3, depth=2, heads=5), (1, 37, 20), None),
-    "phon_k12": (PHON, dict(num_tokens=30, dim=256, dim_hidden=256, kernel_size=12, depth=1, heads=2), (1, 100), None),
-    "phon_k1": (PHON, dict(num_tokens=30, dim=512, dim_hidden=1024, kernel_size=1, depth=1, heads=8), (1, 64), None),
-    "dpp_128": (DPP, dict(dim=128, dim_hidden=128, kernel_size=5, depth=2, heads=2, num_convs_per_resnet_block=1,
-                          num_convolutions_per_block=2), (1, 40, 17), (7, 1, 4)),
-    "dpp_384": (DPP, dict(dim=384, dim_hidden=384, kernel_size=7, depth=1, heads=3, num_convs_per_resnet_block=3,
-                          num_convolutions_per_block=1), (1, 65), (129, 1)),
-    "dpp_640": (DPP, dict(dim=640, dim_hidden=640, kernel_size=1, depth=1, heads=10), (33, 1), (1, 64)),
-    "dpp_1024": (DPP, dict(dim=1024, dim_hidden=1024, kernel_size=3, depth=1, heads=16), (1, 100), (103, 1)),
-    "dpp_table": (DPP, dict(num_phoneme_tokens=60, dim=256, dim_hidden=256, kernel_size=3, depth=2), (1, 50), (40, 1)),
-}
 RUNS = {
     # name: (configuration, B, N (prompt frames / text length), predictor: Np / encoders: text lengths (-1 past),
     #        predictions that get a gradient)
@@ -138,64 +119,18 @@ RUNS = {
 RAGGED_RUN = {cfg: max((r for r in RUNS if RUNS[r][0] == cfg), key=lambda r: RUNS[r][2]) for cfg in CONFIGS}
 
 
-def _heads(cfg):
-    return CONFIGS[cfg][1].get("heads", 8)
-
-
 def _is_self_q(cls, name):
     return cls != DPP and name.endswith(".1.to_q.weight")
-
-
-def _bf(g, *shape, scale=1.0):
-    return (torch.randn(*shape, generator=g) * scale).bfloat16().float().cuda()
-
-
-def _build(cfg):
-    from naturalspeech2_pytorch_b200 import encoders
-    cls, kw, _, _ = CONFIGS[cfg]
-    m = getattr(encoders, cls)(**kw)
-    fill_module(m, 1234)
-    m.cuda()
-    _round_params(m)
-    return m
-
-
-def _restatement(cfg, x, prompts=None, **kw):
-    """fwd(P, dtype, leaves) of the configuration's oracle; x: prompt frames, ids (-1 = padding) or phoneme encodings."""
-    cls, ckw, _, _ = CONFIGS[cfg]
-    heads = _heads(cfg)
-    if cls == DPP:
-        return _with_leaves(x, prompts, "num_phoneme_tokens" in ckw, heads=heads, **kw)
-
-    def fwd(P, dtype, leaves):
-        if cls == SPE:
-            return {"encoding": eo.speech_prompt_encoder(P, leaves.get("x", x).to(dtype), heads=heads,
-                                                         padding=ckw["padding"])}
-        return {"encoding": eo.phoneme_encoder(P, x, heads=heads)}
-    fwd.takes_leaves = True
-    return fwd
 
 
 def _outputs(fwd, params, inputs, autocast=False):
     """The restatement's outputs (fp64 values) without gradients."""
     dtype = torch.float32 if autocast else torch.float64
     P = {n: p.detach().to(dtype) for n, p in params.items()}
-    leaves = dict(P, **{n: t.to(dtype) for n, t in inputs.items() if t.is_floating_point()})
+    P.update({n: t.to(dtype) for n, t in inputs.items() if t.is_floating_point()})
     with torch.no_grad(), torch.backends.cudnn.flags(enabled=False):
         with torch.autocast("cuda", dtype=torch.bfloat16, enabled=autocast):
-            return {k: o.double() for k, o in fwd(P, dtype, leaves).items()}
-
-
-def _compare(o, r, ac, share=None):
-    """(rel-L2 ours, rel-L2 autocast-bf16, q / kv share) of one tensor, or a failure string."""
-    if not bool(torch.isfinite(o).all()):
-        return "non-finite"
-    zero = r == 0
-    if bool(zero.any()) and bool((o[zero] != 0).any()):
-        return f"{int((o[zero] != 0).sum())} of {int(zero.sum())} exact zeros are not zero"
-    if bool(zero.all()):
-        return None
-    return (_rel(o, r), _rel(ac, r), share)
+            return {k: o.double() for k, o in fwd(P, dtype).items()}
 
 
 def _inputs(run):
@@ -203,7 +138,7 @@ def _inputs(run):
     cls, kw, _, _ = CONFIGS[cfg]
     g = torch.Generator().manual_seed(100 + list(RUNS).index(run))
     if cls == SPE:
-        return {"x": _bf(g, B, N, kw["dim_codebook"])}, g
+        return {"x": bf(g, B, N, kw["dim_codebook"])}, g
     if cls == PHON:
         ids = torch.randint(0, kw["num_tokens"], (B, N), generator=g)
         for b, n in enumerate(extra):
@@ -212,8 +147,8 @@ def _inputs(run):
     if "num_phoneme_tokens" in kw:
         x = torch.randint(0, kw["num_phoneme_tokens"], (B, N), generator=g).cuda()
     else:
-        x = _bf(g, B, N, kw["dim_hidden"])
-    return {"x": x, "prompts": _bf(g, B, extra, kw["dim_hidden"])}, g
+        x = bf(g, B, N, kw["dim_hidden"])
+    return {"x": x, "prompts": bf(g, B, extra, kw["dim_hidden"])}, g
 
 
 def _alive_biases(m, cfg, samples):
@@ -224,7 +159,7 @@ def _alive_biases(m, cfg, samples):
         params[t + "to_pred.0.bias"] = torch.full_like(params[t + "to_pred.0.bias"], 1e3)
     pre = {k: [] for k in ("duration", "pitch")}
     for x, p in samples:
-        for k, o in _outputs(_restatement(cfg, x, p), params, {}).items():
+        for k, o in _outputs(config_fwd(cfg, x, p), params, {}).items():
             pre[k].append(o.flatten() - 1e3)
     with torch.no_grad():
         for t, k in zip(TRUNKS, ("duration", "pitch")):
@@ -251,20 +186,20 @@ def _run(run):
     t0 = time.perf_counter()
     cfg, B, N, extra, which = RUNS[run]
     cls, kw, _, _ = CONFIGS[cfg]
-    m = _build(cfg)
+    m = build_config(cfg)
     inputs, g = _inputs(run)
     table = cls == DPP and "num_phoneme_tokens" in kw
     if cls == DPP:
         x, prompts = inputs["x"], inputs["prompts"]
-        biases = _set_head_biases(m, x, prompts, table, heads=_heads(cfg))
-        d_outs = {"duration": _bf(g, B, N, scale=0.05), "pitch": _bf(g, B, N, scale=0.05) if which == "both" else None}
-        fwd = _restatement(cfg, x, prompts)
+        biases = set_head_biases(m, x, prompts, table, heads=config_heads(cfg))
+        d_outs = {"duration": bf(g, B, N, scale=0.05), "pitch": bf(g, B, N, scale=0.05) if which == "both" else None}
+        fwd = config_fwd(cfg, x, prompts)
         args = (x, prompts)
     else:
         x = inputs.get("x", inputs.get("ids"))
         biases = None
-        d_outs = {"encoding": _bf(g, B, N, m.dim_out if cls == SPE else m.dim_hidden)}
-        fwd = _restatement(cfg, x)
+        d_outs = {"encoding": bf(g, B, N, m.dim_out if cls == SPE else m.dim_hidden)}
+        fwd = config_fwd(cfg, x)
         args = (x,)
     ref_inputs = {k: v for k, v in inputs.items() if v.is_floating_point()}
 
@@ -290,8 +225,8 @@ def _run(run):
     train_eq = all(torch.equal(a, b.detach()) for a, b in zip(inf[0], outs))
 
     params = {n: p.detach().clone() for n, p in m.named_parameters()}
-    ref = _ref_grads(fwd, params, ref_inputs, d_outs)
-    ac = _ref_grads(fwd, params, ref_inputs, d_outs, autocast=True)
+    ref = autograd(fwd, params, d_outs, inputs=ref_inputs, cudnn=False, out_prefix="out ")
+    ac = autograd(fwd, params, d_outs, autocast=True, inputs=ref_inputs, cudnn=False, out_prefix="out ")
 
     fails, stats, none_ok = [], {}, True
     if cls == DPP:   # the whole output: both predictions as one tensor
@@ -305,8 +240,7 @@ def _run(run):
         if o is None or o.shape != r.shape:
             fails.append((n, "missing" if o is None else f"shape {tuple(o.shape)} != {tuple(r.shape)}"))
             continue
-        share = _rel_qkv(o, r, ref[n.replace("to_q", "to_kv")]) if _is_self_q(cls, n) else None
-        s = _compare(o, r, ac[n], share)
+        s = compare(o, r, ac[n], ref[n.replace("to_q", "to_kv")] if _is_self_q(cls, n) else None)
         if isinstance(s, str):
             fails.append((n, s))
         elif s is not None:
@@ -354,11 +288,11 @@ def _ragged(m, cfg, inputs):
             got = torch.stack(m(xr, pr, lengths=list(lens), prompt_lens=list(plens)), -1)     # (B, T, 2)
             alone = [torch.stack(m(*a), -1)[0] for a in alone_in]
             params = {n: p.detach() for n, p in m.named_parameters()}
-            refs = [torch.stack(list(_outputs(_restatement(cfg, *a), params, {}).values()), -1)[0] for a in alone_in]
-            acs = [torch.stack(list(_outputs(_restatement(cfg, *a), params, {}, autocast=True).values()), -1)[0]
+            refs = [torch.stack(list(_outputs(config_fwd(cfg, *a), params, {}).values()), -1)[0] for a in alone_in]
+            acs = [torch.stack(list(_outputs(config_fwd(cfg, *a), params, {}, autocast=True).values()), -1)[0]
                    for a in alone_in]
             valid = [got[b, :n] for b, n in enumerate(lens)]
-            res["valid rows"] = _compare(torch.cat(valid), torch.cat(refs), torch.cat(acs))
+            res["valid rows"] = compare(torch.cat(valid), torch.cat(refs), torch.cat(acs))
         else:
             if cls == SPE:
                 xr = inputs["x"].clone()
@@ -373,39 +307,28 @@ def _ragged(m, cfg, inputs):
             valid = [got[b, :n] for b, n in enumerate(lens)]
             params = {n: p.detach() for n, p in m.named_parameters()}
             for b, a in enumerate(alone_in):
-                r = _outputs(_restatement(cfg, a), params, {"x": a} if cls == SPE else {})["encoding"][0]
-                ac = _outputs(_restatement(cfg, a), params, {"x": a} if cls == SPE else {}, autocast=True)["encoding"][0]
-                res[f"sample {b} (length {lens[b]})"] = _compare(valid[b], r, ac)
+                r = _outputs(config_fwd(cfg, a), params, {"x": a} if cls == SPE else {})["encoding"][0]
+                ac = _outputs(config_fwd(cfg, a), params, {"x": a} if cls == SPE else {}, autocast=True)["encoding"][0]
+                res[f"sample {b} (length {lens[b]})"] = compare(valid[b], r, ac)
     res["bit-identical to alone"] = all(torch.equal(v, a) for v, a in zip(valid, alone))
     res["padding zeros"] = all(int((got[b, n:] != 0).sum()) == 0 for b, n in enumerate(lens))
     return res
-
-
-def _over(s):
-    """Over the bound; a self-attention to_q (share given) passes under the common bound or under TO_Q_BOUND."""
-    rel, rel_ac, share = s
-    return rel > _bound(rel_ac) and (share is None or share > TO_Q_BOUND)
-
-
-def _use(s):
-    rel, rel_ac, share = s
-    return rel / _bound(rel_ac) if share is None else min(rel / _bound(rel_ac), share / TO_Q_BOUND)
 
 
 @pytest.mark.parametrize("run", list(RUNS))
 def test_matches_fp64(run):
     r = _run(run)
     stats = r["stats"]
-    rest = {n: s for n, s in stats.items() if s[2] is None}
-    worst = max(rest.items(), key=lambda kv: kv[1][0])
-    tight = max(stats.items(), key=lambda kv: _use(kv[1]))
-    ratio = max(((n, s) for n, s in rest.items() if s[1] > 0), key=lambda kv: kv[1][0] / kv[1][1])
-    q = [s[2] for s in stats.values() if s[2] is not None]
+    rest = {n: s for n, s in stats.items() if s.share is None}
+    worst = max(rest.items(), key=lambda kv: kv[1].rel)
+    tight = max(stats.items(), key=lambda kv: use(ENCODERS, kv[1], EITHER))
+    ratio = max(((n, s) for n, s in rest.items() if s.rel_ac > 0), key=lambda kv: kv[1].rel / kv[1].rel_ac)
+    q = [s.share for s in stats.values() if s.share is not None]
     outs = {n: s for n, s in stats.items() if n.startswith("out ")}
-    print(f"\n{run}: {len(stats)} tensors in {r['seconds']:.1f} s; worst {worst[0]} ours {worst[1][0]:.2e} / autocast "
-          f"{worst[1][1]:.2e}; max ratio {ratio[1][0] / ratio[1][1]:.2f} ({ratio[0]}); tightest {tight[0]} at "
-          f"{_use(tight[1]):.0%} of its bound" + (f"; worst to_q share {max(q):.2e}" if q else "") +
-          "; forward " + ", ".join(f"{n[4:]} {s[0]:.2e} / {s[1]:.2e}" for n, s in outs.items()) +
+    print(f"\n{run}: {len(stats)} tensors in {r['seconds']:.1f} s; worst {worst[0]} ours {worst[1].rel:.2e} / autocast "
+          f"{worst[1].rel_ac:.2e}; max ratio {ratio[1].rel / ratio[1].rel_ac:.2f} ({ratio[0]}); tightest {tight[0]} at "
+          f"{use(ENCODERS, tight[1], EITHER):.0%} of its bound" + (f"; worst to_q share {max(q):.2e}" if q else "") +
+          "; forward " + ", ".join(f"{n[4:]} {s.rel:.2e} / {s.rel_ac:.2e}" for n, s in outs.items()) +
           (f"; forward max-abs {r['fwd_err']:.2e}, min |pre| {r['min_pre']:.2e}, head biases {r['biases']}"
            if r["cls"] == DPP else ""))
     assert r["twice"], "two inference calls differ"
@@ -414,7 +337,7 @@ def test_matches_fp64(run):
     if r["cls"] == DPP:
         assert r["min_pre"] >= MARGIN * r["fwd_err"], "fixture: a head pre-activation lies too close to 0"
     assert not r["fails"], r["fails"][:8]
-    bad = [(n, s) for n, s in stats.items() if _over(s)]
+    bad = [(n, s) for n, s in stats.items() if over(ENCODERS, s, EITHER)]
     assert not bad, f"{len(bad)} tensors over the bound (rel-L2, autocast rel-L2, to_q share): {bad[:8]}"
 
 
@@ -428,7 +351,7 @@ def test_ragged_batch_matches_each_sample_alone(cfg):
     assert rg["padding zeros"], "padded output rows must be exact zeros"
     for k, v in checks.items():
         assert not isinstance(v, str), (k, v)
-        assert v is None or not _over(v), (k, v, _bound(v[1]))
+        assert v is None or not over(ENCODERS, v, EITHER), (k, v, bound(ENCODERS, v[1]))
 
 
 def test_input_grads_with_frozen_parameters():
@@ -436,9 +359,9 @@ def test_input_grads_with_frozen_parameters():
     and give the inputs the gradients of the run with trainable parameters, bit for bit."""
     for run in ("spe_k3_narrow-N129", "dpp_128-T40"):
         r = _run(run)
-        m = _build(r["cfg"])
+        m = build_config(r["cfg"])
         if r["cls"] == DPP:
-            _set_head_biases(m, r["inputs"]["x"], r["inputs"]["prompts"], False, heads=_heads(r["cfg"]))
+            set_head_biases(m, r["inputs"]["x"], r["inputs"]["prompts"], False, heads=config_heads(r["cfg"]))
         m.requires_grad_(False)
         m.train()
         leaves = [r["inputs"][k].clone().requires_grad_(True) for k in ("x", "prompts") if k in r["inputs"]]
@@ -453,16 +376,8 @@ def test_input_grads_with_frozen_parameters():
 # ---- wrong references ----
 def _assert_rejected(run, fwd, names):
     r = _run(run)
-    wrong = _ref_grads(fwd, r["params"], r["ref_inputs"], r["d_outs"], only=names)
-    for n in names:
-        s = r["stats"][n]
-        o = r["ours"][n]
-        rel = _rel(o, wrong[n])
-        share = _rel_qkv(o, wrong[n], wrong[n.replace("to_q", "to_kv")]) if s[2] is not None else None
-        print(f"  {run} {n}: rel-L2 vs the wrong reference {rel:.3e}" +
-              (f", q / kv share {share:.3e} (bound {TO_Q_BOUND:.1e})" if share is not None else
-               f" (bound {_bound(s[1]):.3e})"))
-        assert _over((rel, s[1], share)), f"the bound accepts a wrong reference for {n}"
+    wrong = autograd(fwd, r["params"], r["d_outs"], inputs=r["ref_inputs"], only=names, cudnn=False)
+    assert_rejected(r["ours"], wrong, r["stats"], names, ENCODERS, EITHER)
 
 
 def _group_norm_without_last_quad(h, groups, weight, bias, eps):
@@ -477,47 +392,44 @@ def _group_norm_without_last_quad(h, groups, weight, bias, eps):
 
 def test_rejects_group_norm_without_the_last_channel_quad():
     r = _run("dpp_384")
-    fwd = _restatement("dpp_384", r["inputs"]["x"], r["inputs"]["prompts"],
+    fwd = config_fwd("dpp_384", r["inputs"]["x"], r["inputs"]["prompts"],
                        trunk=functools.partial(eo._trunk, group_norm=_group_norm_without_last_quad))
     _assert_rejected("dpp_384", fwd, list(KEEP["dpp_384"]))
 
 
 def test_rejects_same_conv_taps_one_row_off():
     """spe_k11's convs padded (k//2 - 1, k//2 + 1): every tap reads one row later."""
-    k, heads = CONFIGS["spe_k11"][1]["kernel_size"], _heads("spe_k11")
+    k, heads = CONFIGS["spe_k11"][1]["kernel_size"], config_heads("spe_k11")
 
-    def fwd(P, dtype, leaves):
-        h = leaves["x"].to(dtype).transpose(1, 2)
+    def fwd(P, dtype):
+        h = P["x"].to(dtype).transpose(1, 2)
         for i in (1, 3):
             h = F.silu(F.conv1d(F.pad(h, (k // 2 - 1, k // 2 + 1)), P[f"conv.{i}.weight"], P[f"conv.{i}.bias"]))
         return {"encoding": eo.transformer(h.transpose(1, 2), P, "transformer.", heads)}
-    fwd.takes_leaves = True
     _assert_rejected("spe_k11-N103", fwd, list(KEEP["spe_k11-N103"]))
 
 
 def test_rejects_causal_conv_padded_one_short():
     """phon_k12's causal conv padded (k - 2, 1) instead of (k - 1, 0)."""
     r = _run("phon_k12-T100")
-    ids, heads = r["inputs"]["ids"], _heads("phon_k12")
+    ids, heads = r["inputs"]["ids"], config_heads("phon_k12")
 
-    def fwd(P, dtype, leaves):
+    def fwd(P, dtype):
         pad_id = P["token_emb.weight"].shape[0] - 1
         w = P["conv.1.weight"]
         h = P["token_emb.weight"][ids.masked_fill(ids < 0, pad_id)].transpose(1, 2)
         h = F.silu(F.conv1d(F.pad(h, (w.shape[-1] - 2, 1)), w, P["conv.1.bias"]))
         return {"encoding": eo.transformer(h.transpose(1, 2), P, "transformer.", heads)}
-    fwd.takes_leaves = True
     _assert_rejected("phon_k12-T100", fwd, list(KEEP["phon_k12-T100"]))
 
 
 def test_rejects_attention_scaled_by_the_attention_width():
     """spe_k3_narrow's attention scaled by (heads x 64)^-1/2: q scaled by heads^-1/2 inside the restatement."""
     r = _run("spe_k3_narrow-N129")
-    heads = _heads("spe_k3_narrow")
-    base = _restatement("spe_k3_narrow", r["inputs"]["x"])
+    heads = config_heads("spe_k3_narrow")
+    base = config_fwd("spe_k3_narrow", r["inputs"]["x"])
 
-    def fwd(P, dtype, leaves):
+    def fwd(P, dtype):
         q = {n: v * heads ** -0.5 for n, v in P.items() if n.endswith(".to_q.weight")}
-        return base(dict(P, **q), dtype, leaves)
-    fwd.takes_leaves = True
+        return base(dict(P, **q), dtype)
     _assert_rejected("spe_k3_narrow-N129", fwd, list(KEEP["spe_k3_narrow-N129"]))

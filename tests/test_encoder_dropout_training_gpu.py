@@ -7,9 +7,9 @@ import torch
 
 import dropout_oracle as do
 from helpers import build_encoder, encoder_case
+from restatements import drawn_seed, e2e_front_end, e2e_inputs, e2e_loss
 
 pytestmark = pytest.mark.gpu
-SEED_HIGH = 2 ** 63 - 1
 
 
 def _rel_cos(got, ref):
@@ -34,11 +34,6 @@ def _encoder(name, p, train_dropout=True):
     enc = build_encoder(cls, kw, device="cuda").train()
     enc.train_dropout = train_dropout
     return cls, kwargs, enc, x
-
-
-def _drawn_seed(torch_seed):
-    torch.manual_seed(torch_seed)
-    return int(torch.randint(0, SEED_HIGH, ()))
 
 
 def _fp64(cls, kwargs, enc, x, w, seed, p):
@@ -84,7 +79,7 @@ def test_encoder_dropout_matches_fp64_autograd(name, p):
     enc.train_dropout = True
     torch.manual_seed(torch_seed)
     out, g = _gpu(enc, x, w)
-    seed = _drawn_seed(torch_seed)
+    seed = drawn_seed(torch_seed)
     ref, rg = _fp64(cls, kwargs, enc, x, w, seed, p)
     _assert_tensor(out, ref, f"{name} p{p} output")
     assert _rel_cos(out, plain_ref)[0] > 0.05, "the output must differ from the undropped encoder's"
@@ -131,19 +126,18 @@ def test_conditional_training_with_dropout_lowers_the_loss():
     """AdamW steps over the denoiser and the front end with the encoders' dropout on lower the (dropout-free) loss on
     a fixed batch."""
     from naturalspeech2_pytorch_b200 import NaturalSpeech2
-    from test_conditional_training_gpu import _front_end, _inputs, _loss
-    mods, cond_net = _front_end("e2e_small")
+    mods, cond_net = e2e_front_end("e2e_small")
     for enc in (cond_net.prompt_enc, cond_net.phoneme_enc):
         enc.train_dropout = True
         assert enc.attn_dropout > 0 or enc.conv_dropout > 0
     ns = NaturalSpeech2(mods["model"], target_sample_hz=24000, timesteps=4, conditioner=cond_net)
-    inp = _inputs("e2e_small")
+    inp = e2e_inputs("e2e_small")
 
     def eval_loss():
         for m in mods.values():
             m.eval()
         with torch.no_grad():
-            v = float(_loss(ns, inp))
+            v = float(e2e_loss(ns, inp))
         for m in mods.values():
             m.train()
         return v
@@ -155,7 +149,7 @@ def test_conditional_training_with_dropout_lowers_the_loss():
     losses = []
     for _ in range(8):
         opt.zero_grad(set_to_none=True)
-        loss = _loss(ns, inp)
+        loss = e2e_loss(ns, inp)
         loss.backward()
         opt.step()
         losses.append(float(loss.detach()))

@@ -109,7 +109,7 @@ def test_encoder_constructors_accept_the_swept_configs_and_reject_their_neighbou
     """Every configuration of tests/test_encoder_configs_fp64_gpu.py constructs; the nearest unsupported ones raise
     NotImplementedError in the constructor, before any kernel could launch."""
     from naturalspeech2_pytorch_b200.encoders import DurationPitchPredictor, PhonemeEncoder, SpeechPromptEncoder
-    from test_encoder_configs_fp64_gpu import CONFIGS
+    from restatements import ENCODER_CONFIGS as CONFIGS
     from naturalspeech2_pytorch_b200 import encoders
     for cls, kw, _, _ in CONFIGS.values():
         getattr(encoders, cls)(**kw)

@@ -1,6 +1,6 @@
 """GPU: the key-padding attention backward (`ops.attention_bwd(kv_lens=)`, attn_bwd_kernel<false, true>) against a
-float64 reference of each sample's attention over its own keys [0, kv_lens[b]), under the bounds of
-test_attention_edges_gpu.py.
+float64 reference of each sample's attention over its own keys [0, kv_lens[b]), under the bounds of the attention
+edge suite (kernel_check.attention_reference).
 
 Lengths straddle the backward's 128-key tiles and its 64-key warpgroup halves ({1, 63, 64, 65, 127, 128, 129, Nk},
 those <= Nk), for self attention (Nq = Nk) and cross attention (Nq != Nk), 1 and 8 heads.  Besides the float64 bounds:
@@ -12,8 +12,7 @@ length of 1 gives exact-zero d Q and d K, as the plain kernel does at kv_len = 1
 import pytest
 import torch
 
-from kernel_check import assert_close
-from test_attention_edges_gpu import RL2, _inputs, reference
+from kernel_check import ATTN_RL2, assert_close, attention_inputs, attention_reference
 
 pytestmark = pytest.mark.gpu
 bf = torch.bfloat16
@@ -47,18 +46,18 @@ def test_attention_bwd_kv_lens(Nk, kind, H):
     lens = sorted({n for n in LENGTHS if n <= Nk} | {Nk})
     B = len(lens)
     Nq = Nk if kind == "self" else 77
-    q, k, v, d_o = _inputs(B, H, Nq, Nk, seed=Nk + Nq + H)
+    q, k, v, d_o = attention_inputs(B, H, Nq, Nk, seed=Nk + Nq + H)
     kl = _lens(lens)
     got = _run(q, k, v, d_o, H, kl)
     scale = 64 ** -0.5
     for b, n in enumerate(lens):
         what = f"Nk{Nk} {kind} H{H} sample {b} (kv_len {n})"
-        ref = reference(q[b:b + 1], k[b:b + 1, :n], v[b:b + 1, :n], d_o[b:b + 1], H, scale)
-        assert_close(got["o"][b:b + 1], ref["o"], ref["b_o"], RL2, f"{what} o")
-        assert_close(got["lse"][b:b + 1], ref["lse"], ref["b_lse"], RL2, f"{what} lse")
-        assert_close(got["dq"][b:b + 1], ref["dq"], ref["b_dq"], RL2, f"{what} dq")
-        assert_close(got["dk"][b:b + 1, :n], ref["dk"], ref["b_dk"], RL2, f"{what} dk")
-        assert_close(got["dv"][b:b + 1, :n], ref["dv"], ref["b_dv"], RL2, f"{what} dv")
+        ref = attention_reference(q[b:b + 1], k[b:b + 1, :n], v[b:b + 1, :n], d_o[b:b + 1], H, scale)
+        assert_close(got["o"][b:b + 1], ref["o"], ref["b_o"], ATTN_RL2, f"{what} o")
+        assert_close(got["lse"][b:b + 1], ref["lse"], ref["b_lse"], ATTN_RL2, f"{what} lse")
+        assert_close(got["dq"][b:b + 1], ref["dq"], ref["b_dq"], ATTN_RL2, f"{what} dq")
+        assert_close(got["dk"][b:b + 1, :n], ref["dk"], ref["b_dk"], ATTN_RL2, f"{what} dk")
+        assert_close(got["dv"][b:b + 1, :n], ref["dv"], ref["b_dv"], ATTN_RL2, f"{what} dv")
         for name in ("dk", "dv"):   # NaN-initialised: != 0 also catches rows left unwritten
             assert int((got[name][b, n:] != 0).sum()) == 0, (what, name, "padding")
         alone = _run(q[b:b + 1], k[b:b + 1, :n], v[b:b + 1, :n], d_o[b:b + 1], H)
@@ -77,8 +76,8 @@ def test_attention_bwd_kv_lens(Nk, kind, H):
     for name in ("o", "lse", "dk", "dv"):
         assert torch.equal(junk[name], got[name]), (name, "junk")
     for b, n in enumerate(lens):
-        ref = reference(q[b:b + 1], k[b:b + 1, :n], v[b:b + 1, :n], d_o[b:b + 1], H, scale)
-        assert_close(junk["dq"][b:b + 1], ref["dq"], ref["b_dq"], RL2, f"sample {b} dq with junk keys")
+        ref = attention_reference(q[b:b + 1], k[b:b + 1, :n], v[b:b + 1, :n], d_o[b:b + 1], H, scale)
+        assert_close(junk["dq"][b:b + 1], ref["dq"], ref["b_dq"], ATTN_RL2, f"sample {b} dq with junk keys")
 
     # lengths that cover every key: the plain call's d K / d V, bit for bit
     full = _run(q, k, v, d_o, H, _lens([Nk] * B))
@@ -93,7 +92,7 @@ def test_attention_bwd_kv_lens_strided_views():
     from naturalspeech2_pytorch_b200 import ops
     B, H, Nq, Nk = 3, 2, 70, 300
     inner = H * 64
-    q, k, v, d_o = _inputs(B, H, Nq, Nk, seed=5)
+    q, k, v, d_o = attention_inputs(B, H, Nq, Nk, seed=5)
     kl = _lens([1, 129, 300])
     o = torch.empty(B, Nq, inner, device=dev, dtype=bf)
     lse = torch.empty(B, H, Nq, device=dev)

@@ -4,13 +4,12 @@ Each ragged kernel must give every sample exactly what the plain kernel gives th
 not read what the padded rows hold: the attention over keys [0, kv_lens[b]) (`ops.attention(kv_lens=)`), the GroupNorm
 + SiLU over rows [0, lens[b]) (`ops.groupnorm_silu(lens=)`), the prompt mean, the row mask, the row pack of the
 predictor's keys and the condition injection with per-sample condition lengths.  The attention is also held to the
-fp64 bounds of tests/test_attention_edges_gpu.py, which reject a reference that attends to one key more.
+fp64 bounds of the attention edge suite (kernel_check.attention_reference), which reject a reference that attends to one key more.
 """
 import pytest
 import torch
 
-from kernel_check import assert_close, assert_rejects
-from test_attention_edges_gpu import RL2, _inputs, reference
+from kernel_check import ATTN_RL2, assert_close, assert_rejects, attention_inputs, attention_reference
 
 pytestmark = pytest.mark.gpu
 bf = torch.bfloat16
@@ -34,7 +33,7 @@ def test_attention_ragged(Nk, Nq, H):
     from naturalspeech2_pytorch_b200 import ops
     lens = [v for v in LENS if v < Nk] + [Nk]
     B, inner = len(lens), H * 64
-    q, k, v, d_o = _inputs(B, H, Nq, Nk, seed=Nk + 7 * Nq + H)      # windows of one fused projection
+    q, k, v, d_o = attention_inputs(B, H, Nq, Nk, seed=Nk + 7 * Nq + H)      # windows of one fused projection
     g = torch.Generator(device=dev).manual_seed(Nk * Nq)
     for b, n in enumerate(lens):
         if n < Nk:   # the first key past the length: score 0 and a large value, so attending to it shows
@@ -48,17 +47,17 @@ def test_attention_ragged(Nk, Nq, H):
         alone = torch.empty(1, Nq, inner, device=dev, dtype=bf)
         ops.attention(q[b:b + 1], k[b:b + 1, :n], v[b:b + 1, :n], alone, heads=H)
         assert torch.equal(out[b:b + 1], alone), (b, n)
-        ref = reference(q[b:b + 1], k[b:b + 1, :n], v[b:b + 1, :n], d_o[b:b + 1], H, 64 ** -0.5)
-        assert_close(out[b:b + 1], ref["o"], ref["b_o"], RL2, f"sample {b}, {n} keys")
+        ref = attention_reference(q[b:b + 1], k[b:b + 1, :n], v[b:b + 1, :n], d_o[b:b + 1], H, 64 ** -0.5)
+        assert_close(out[b:b + 1], ref["o"], ref["b_o"], ATTN_RL2, f"sample {b}, {n} keys")
         if n < Nk:   # attending to one key more (a ±1e4 garbage key) must fail the same bounds
-            wrong = reference(q[b:b + 1], k[b:b + 1, :n + 1], v[b:b + 1, :n + 1], d_o[b:b + 1], H, 64 ** -0.5)
-            assert_rejects(out[b:b + 1], wrong["o"], ref["b_o"], RL2, f"sample {b}, {n} + 1 keys")
+            wrong = attention_reference(q[b:b + 1], k[b:b + 1, :n + 1], v[b:b + 1, :n + 1], d_o[b:b + 1], H, 64 ** -0.5)
+            assert_rejects(out[b:b + 1], wrong["o"], ref["b_o"], ATTN_RL2, f"sample {b}, {n} + 1 keys")
 
 
 @pytest.mark.parametrize("B,H,Nq,Nk", [(2, 8, 300, 1024), (3, 2, 65, 129)])
 def test_attention_ragged_full_lengths_match_plain(B, H, Nq, Nk):
     from naturalspeech2_pytorch_b200 import ops
-    q, k, v, _ = _inputs(B, H, Nq, Nk, seed=3)
+    q, k, v, _ = attention_inputs(B, H, Nq, Nk, seed=3)
     a, p = (torch.empty(B, Nq, H * 64, device=dev, dtype=bf) for _ in range(2))
     ops.attention(q, k, v, a, heads=H, kv_lens=_lens([Nk] * B))
     ops.attention(q, k, v, p, heads=H)

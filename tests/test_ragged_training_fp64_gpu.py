@@ -6,11 +6,12 @@ never leave one key tile.  This module checks the same calls against the float64
 300 where every attention backward spans three 128-key tiles and five 64-query tiles, and across the configurations
 the constructors accept:
   * SpeechPromptEncoder / PhonemeEncoder(lengths=): `spe_k3_narrow`, `spe_k1_wide`, `spe_k11`, `phon_d64`, `phon_k12`
-    and `phon_k1` of test_encoder_configs_fp64_gpu.CONFIGS, and both encoders at their default dims;
+    and `phon_k1` of restatements.ENCODER_CONFIGS (test_encoder_configs_fp64_gpu.py), and both encoders at their
+    default dims;
   * Model(prompt_lens=): the conditional cases `ff2_cond` (cond_drop_prob 0.5: dropped and kept samples both carry
     lengths), `ff8_cond` (no perceiver projection), `w640_m1` (one latent) and `w1024_b50` (B 50, 33 latents, resampler
-    depth 3) of test_denoiser_configs_fp64_gpu.CASES with their prompts padded to 300 frames, and `bench` (dim 512,
-    8 heads, depth 2, 32 latents: M + length lands on 33, 128, 129, 256 and 332 keys);
+    depth 3) of restatements.DENOISER_CASES (test_denoiser_configs_fp64_gpu.py) with their prompts padded to 300
+    frames, and `bench` (dim 512, 8 heads, depth 2, 32 latents: M + length lands on 33, 128, 129, 256 and 332 keys);
   * Conditioner(mode="train", prompt_lens=, phoneme_lens=) at the encoders' default dims;
   * NaturalSpeech2.forward(prompt_lens=, phoneme_lens=).
 Each padded batch mixes lengths 1, 63 / 64 / 65, 127 / 128 / 129 and the full length, unsorted, with one length used
@@ -23,7 +24,7 @@ for the encoders and the Conditioner, `oracle.denoiser_torch_port.model_forward_
 one length run together, which for the restatement is the same computation).  With the loss sum_b <out_b, up_b> and
 bf16-representable upstream gradients, each sample's input gradient (d prompt rows, d cond, d x) is that sample's
 float64 gradient and each parameter gradient the sum over samples.  The autocast-bf16 twin is computed the same way, so
-the bounds of the default-dims modules apply unchanged: rel-L2 <= C_AUTOCAST x twin + REL_FLOOR and <= REL_CEILING
+the bounds of the default-dims modules apply unchanged: rel-L2 <= C x twin + floor and <= ceiling
 (the encoders' constants and to_q rule for the encoders and the Conditioner, the denoiser's for the Model), exact zeros
 wherever float64 is exactly zero, nothing non-finite.  Per case also:
   * forward: each sample's output is bit-identical to the alone call, and padded output rows are exact zeros;
@@ -73,7 +74,7 @@ with its rel-L2 ours / autocast-bf16 (a self-attention to_q under the to_q rule 
   bench          transformer.layers.0.1.to_q.weight               1.05e-2 / 1.76e-2   70 %   0.75
   Conditioner    prompt_enc.transformer.layers.4.1.to_q.weight (q) 3.1e2 / 5.6e-1    80 %   3.39
 The largest ratios (2.6 ... 6.7) are all on the last feed-forward bias of an encoder, where the twin's error is far
-below REL_FLOOR; every tensor is within its bound.  NaturalSpeech2.forward: the denoiser's gradients match the scaled
+below the floor; every tensor is within its bound.  NaturalSpeech2.forward: the denoiser's gradients match the scaled
 alone gradients to 8.6e-7, the conditioner's to 7.6e-3 (prompt_enc.conv.1.weight).  The wrong references sit at 106x
 the bound (perceiver to_kv; 204x on latents, 437x on d prompt), 4.7x (mean-pool over Np, on d prompt of the 224-frame sample; 781x on to_prompt_cond),
 21x (spe_k11 convs, on d x of the 129-frame sample; 59-65x on the conv weights) and 1.4x (phoneme attention over one
@@ -87,21 +88,19 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from fp64_check import DENOISER, EITHER, ENCODERS, assert_rejected, autograd, bf, compare, over, rel_qkv, round_params, use
 from helpers import build_encoder, build_model
 from oracle import denoiser_torch_port as tp
 from oracle import encoders_oracle as eo
 from param_fill import fill_module
-from test_conditioning_backward_fp64_gpu import REL_CEILING as REL_CEILING_ENC
-from test_conditioning_backward_fp64_gpu import (_bound, _conditioner_fwd, _encoder_fwd, _ref_grads, _rel,
-                                                 _rel_qkv, _round_params)
-from test_denoiser_backward_fp64_gpu import _drop_masks, _port_grads
-from test_denoiser_configs_fp64_gpu import C_AUTOCAST, CASES, REL_CEILING, REL_FLOOR
-from test_encoder_configs_fp64_gpu import CONFIGS, _build, _compare, _over, _restatement, _use
-from test_ragged_training_gpu import RTOL
+from restatements import DENOISER_CASES as CASES
+from restatements import ENCODER_CONFIGS as CONFIGS
+from restatements import RTOL, build_config, conditioner_fwd, config_fwd, drop_masks, encoder_fwd, port_grads
 
 pytestmark = pytest.mark.gpu
 
 SPE, PHON = "SpeechPromptEncoder", "PhonemeEncoder"
+FAMILY = {"enc": ENCODERS, "den": DENOISER}   # the Model's tensors take the denoiser's bounds, the rest the encoders'
 NPAD = 300                                              # padded prompt frames / phonemes
 LENS = (129, 1, 300, 64, 63, 128, 65, 40, 127, 64)      # unsorted, 64 twice
 LENS_K11 = (129, 4, 300, 64, 1, 63, 128, 65, 2, 127, 64)
@@ -135,14 +134,6 @@ DEN_CASES = {
 assert DEN_CASES["ff2_cond"][4] == 0.5
 
 
-def _dbound(rel_ac):
-    return min(C_AUTOCAST * rel_ac + REL_FLOOR, REL_CEILING)
-
-
-def _bf(g, *shape):
-    return torch.randn(*shape, generator=g).bfloat16().float().cuda()
-
-
 def _groups(lens):
     """{length: sample indices} (samples of one length run together in the restatement)."""
     out = {}
@@ -171,7 +162,7 @@ def _err(got, want):
     return 0.0 if d == 0 else (d / w if w > 0 else float("inf"))
 
 
-def _against(res, ours, ref, ac, names, zero_names=()):
+def _against(res, ours, ref, ac, names):
     """Stats of ours against fp64 (ref) and its twin (ac) into res["stats"], failures into res["fails"]."""
     for n in names:
         o, r, a = ours.get(n), ref[n], ac[n]
@@ -179,21 +170,11 @@ def _against(res, ours, ref, ac, names, zero_names=()):
             if bool((r != 0).any()):
                 res["fails"].append((n, "missing"))
             continue
-        o = o.reshape(r.shape)
-        share = _rel_qkv(o, r, ref[n.replace("to_q", "to_kv")]) if res["family"] == "enc" and _is_self_q(n) else None
-        s = _compare(o, r, a, share)
+        s = compare(o, r, a, ref[n.replace("to_q", "to_kv")] if res["family"] == "enc" and _is_self_q(n) else None)
         if isinstance(s, str):
             res["fails"].append((n, s))
         elif s is not None:
             res["stats"][n] = s
-
-
-def _over_case(res, s):
-    return _over(s) if res["family"] == "enc" else s[0] > _dbound(s[1])
-
-
-def _use_case(res, s):
-    return _use(s) if res["family"] == "enc" else s[0] / _dbound(s[1])
 
 
 def _alone_spread(res, got, again, alone, names):
@@ -204,7 +185,7 @@ def _alone_spread(res, got, again, alone, names):
     for n in names:
         share = None
         if res["family"] == "enc" and _is_self_q(n) and got[n] is not None:
-            share = _rel_qkv(got[n], alone[n], alone[n.replace("to_q", "to_kv")])
+            share = rel_qkv(got[n], alone[n], alone[n.replace("to_q", "to_kv")])
         res["alone_errs"][n] = (_err(got[n], alone.get(n)), share)
 
 
@@ -215,9 +196,9 @@ _CACHE = {}
 def _enc_module(case):
     cfg, _ = ENC_CASES[case]
     if cfg in CONFIGS:
-        return _build(cfg), CONFIGS[cfg][0]
+        return build_config(cfg), CONFIGS[cfg][0]
     m = build_encoder(cfg, DEFAULT_KW[cfg], seed=1234, device="cuda")
-    _round_params(m)
+    round_params(m)
     return m, cfg
 
 
@@ -225,11 +206,10 @@ def _enc_fwd(case, x, cls, heads, padding):
     """fwd(P, dtype) of the restatement on one group of samples; the prompt frames are the leaf P["x"]."""
     cfg = ENC_CASES[case][0]
     if cfg in CONFIGS:
-        base = _restatement(cfg, x)
-        return lambda P, dtype: base(P, dtype, P)
+        return config_fwd(cfg, x)
     if cls == SPE:
         return lambda P, dtype: {"encoding": eo.speech_prompt_encoder(P, P["x"].to(dtype), heads=heads, padding=padding)}
-    base = _encoder_fwd(cls, x, (None, None))
+    base = encoder_fwd(cls, x, (None, None))
     return lambda P, dtype: {"encoding": base(P, dtype)["out"]}
 
 
@@ -238,7 +218,7 @@ def _enc_inputs(case, m, cls):
     B = len(lens)
     g = torch.Generator().manual_seed(50 + list(ENC_CASES).index(case))
     if cls == SPE:
-        x = _bf(g, B, NPAD, m.dim)
+        x = bf(g, B, NPAD, m.dim)
         junk = x.clone()
         for b, n in enumerate(lens):
             x[b, n:] = float("nan")
@@ -249,7 +229,7 @@ def _enc_inputs(case, m, cls):
         for b, n in enumerate(lens):    # ids only the padding uses
             x[b, n:] = torch.randint(V // 2, V, (NPAD - n,), generator=g)
         x = junk = x.cuda()
-    up = _bf(g, B, NPAD, m.dim_out if cls == SPE else m.dim_hidden)
+    up = bf(g, B, NPAD, m.dim_out if cls == SPE else m.dim_hidden)
     return x, junk, up
 
 
@@ -340,8 +320,8 @@ def _enc_case(case):
         for n, idx in _groups(lens).items():
             xs = x[idx, :n]
             extra = {"x": xs} if cls == SPE else {}
-            gr = _ref_grads(_enc_fwd(case, xs, cls, heads, padding), dict(params, **extra),
-                            {"encoding": up[idx, :n]}, autocast=autocast, only=names + list(extra))
+            gr = autograd(_enc_fwd(case, xs, cls, heads, padding), dict(params, **extra), {"encoding": up[idx, :n]},
+                          autocast=autocast, only=names + list(extra), cudnn="twin")
             _acc(dst, gr, names)
             for i, b in enumerate(idx):
                 if cls == SPE:
@@ -364,7 +344,7 @@ def _alone_use(res):
     out = {}
     for n, (e, share) in res["alone_errs"].items():
         if n in res["stats"]:
-            out[n] = _use_case(res, (e, res["stats"][n][1], share))
+            out[n] = use(FAMILY[res["family"]], (e, res["stats"][n].rel_ac, share), EITHER)
         else:
             out[n] = 0.0 if e == 0 else float("inf")
     return out
@@ -372,13 +352,16 @@ def _alone_use(res):
 
 def _report(name, res):
     stats = res["stats"]
-    worst = max(stats.items(), key=lambda kv: kv[1][0])
-    tight = max(stats.items(), key=lambda kv: _use_case(res, kv[1]))
-    ratio = max(((n, s) for n, s in stats.items() if s[1] > 0 and s[2] is None), key=lambda kv: kv[1][0] / kv[1][1])
+    fam = FAMILY[res["family"]]
+    worst = max(stats.items(), key=lambda kv: kv[1].rel)
+    tight = max(stats.items(), key=lambda kv: use(fam, kv[1], EITHER))
+    ratio = max(((n, s) for n, s in stats.items() if s.rel_ac > 0 and s.share is None),
+                key=lambda kv: kv[1].rel / kv[1].rel_ac)
     alone = max(_alone_use(res).items(), key=lambda kv: kv[1])
-    print(f"\n{name}: {len(stats)} tensors in {res['seconds']:.1f} s; worst {worst[0]} ours {worst[1][0]:.2e} / "
-          f"autocast {worst[1][1]:.2e}; max ratio {ratio[1][0] / ratio[1][1]:.2f} ({ratio[0]}); tightest {tight[0]} at "
-          f"{_use_case(res, tight[1]):.0%} of its bound (ours {tight[1][0]:.2e} / autocast {tight[1][1]:.2e}); batch vs alone: largest {max(e for e, _ in res['alone_errs'].values()):.2e}, "
+    print(f"\n{name}: {len(stats)} tensors in {res['seconds']:.1f} s; worst {worst[0]} ours {worst[1].rel:.2e} / "
+          f"autocast {worst[1].rel_ac:.2e}; max ratio {ratio[1].rel / ratio[1].rel_ac:.2f} ({ratio[0]}); tightest "
+          f"{tight[0]} at {use(fam, tight[1], EITHER):.0%} of its bound (ours {tight[1].rel:.2e} / autocast "
+          f"{tight[1].rel_ac:.2e}); batch vs alone: largest {max(e for e, _ in res['alone_errs'].values()):.2e}, "
           f"tightest {alone[0]} at {alone[1]:.0%} of its bound; run to run {res['spread'][0]:.2e} ({res['spread'][1]})")
 
 
@@ -386,10 +369,10 @@ def _assert_case(res):
     bad_checks = [k for k, ok in res["checks"].items() if not ok]
     assert not bad_checks, bad_checks
     assert not res["fails"], res["fails"][:8]
-    bad = [(n, s) for n, s in res["stats"].items() if _over_case(res, s)]
+    bad = [(n, s) for n, s in res["stats"].items() if over(FAMILY[res["family"]], s, EITHER)]
     assert not bad, f"{len(bad)} tensors over the bound (rel-L2, autocast rel-L2, to_q share): {bad[:8]}"
-    over = [(n, res["alone_errs"][n], u) for n, u in _alone_use(res).items() if u > 1]
-    assert not over, f"batch vs the sum of the alone calls over the bound: {over[:8]}"
+    over_alone = [(n, res["alone_errs"][n], u) for n, u in _alone_use(res).items() if u > 1]
+    assert not over_alone, f"batch vs the sum of the alone calls over the bound: {over_alone[:8]}"
 
 
 @pytest.mark.parametrize("case", list(ENC_CASES))
@@ -427,17 +410,17 @@ def _den_case(case):
     kwargs, N, lens, Lc, p = DEN_CASES[case]
     B = len(lens)
     model = build_model(kwargs, 1234, device="cuda").train()
-    _round_params(model)
+    round_params(model)
     D, Dp = kwargs["dim"], kwargs["dim_prompt"]
     g = torch.Generator().manual_seed(60 + list(DEN_CASES).index(case))
-    inp = {"x": _bf(g, B, N, D), "times": torch.rand(B, generator=g).cuda(), "prompt": _bf(g, B, NPAD, Dp),
-           "cond": _bf(g, B, Dp, Lc)}
+    inp = {"x": bf(g, B, N, D), "times": torch.rand(B, generator=g).cuda(), "prompt": bf(g, B, NPAD, Dp),
+           "cond": bf(g, B, Dp, Lc)}
     junk = inp["prompt"].clone()
     for b, n in enumerate(lens):
         inp["prompt"][b, n:] = float("nan")
         junk[b, n:] = JUNK * torch.randn(NPAD - n, Dp, generator=g).sign().cuda()
-    d_out = _bf(g, B, N, D)
-    seed, dp, dc = _drop_masks(B, p)
+    d_out = bf(g, B, N, D)
+    seed, dp, dc = drop_masks(B, p)
     names = [n for n, _ in model.named_parameters()]
     params = {n: prm.detach() for n, prm in model.named_parameters()}
     res = dict(family="den", lens=lens, stats={}, fails=[], checks={})
@@ -476,11 +459,11 @@ def _den_case(case):
     _alone_spread(res, got, again, alone, names + in_names)
 
     ref, ac = {}, {}
-    for dst, kw in ((ref, {}), (ac, dict(dtype=torch.float32, autocast=True))):
+    for dst, kw in ((ref, {}), (ac, dict(autocast=True))):
         for n, idx in _groups(lens).items():
             sub = {"x": inp["x"][idx], "times": inp["times"][idx], "prompt": inp["prompt"][idx, :n],
                    "cond": inp["cond"][idx]}
-            gr = _port_grads(params, kwargs, sub, (dp[idx], dc[idx]), d_out[idx], **kw)
+            gr = port_grads(params, kwargs, sub, (dp[idx], dc[idx]), d_out[idx], **kw)
             _acc(dst, gr, names)
             for i, b in enumerate(idx):
                 dst[f"d prompt {b}"], dst[f"d cond {b}"] = gr["d prompt"][i].double(), gr["d cond"][i].double()
@@ -509,7 +492,7 @@ def test_model_prompt_lens_matches_fp64_per_sample(case):
 NUM_TOKENS, PITCH_BINS, L_FRAMES = 100, 256, 600
 NS_NP, NS_T, NS_L = 96, 64, 128                     # NaturalSpeech2.forward: every attention within one key tile
 NS_LENS, NS_PHON_LENS = (96, 1, 63, 64, 65, 40, 95, 64), (64, 1, 33, 63, 17, 40, 64, 5)
-NS_COND_BOUND = REL_CEILING_ENC   # the conditioner behind the denoiser: see the docstring of the test below
+NS_COND_BOUND = ENCODERS.ceiling   # the conditioner behind the denoiser: see the docstring of the test below
 
 
 def _cond_inputs(prompt_lens=LENS, phon_lens=PHON_LENS, Np=NPAD, T=NPAD, L=L_FRAMES):
@@ -518,7 +501,7 @@ def _cond_inputs(prompt_lens=LENS, phon_lens=PHON_LENS, Np=NPAD, T=NPAD, L=L_FRA
     rng = np.random.default_rng(11)
     B = len(prompt_lens)
     g = torch.Generator().manual_seed(12)
-    prompt = _bf(g, B, Np, 128)
+    prompt = bf(g, B, Np, 128)
     for b, n in enumerate(prompt_lens):
         prompt[b, n:] = float("nan")
     text = rng.integers(0, NUM_TOKENS // 2, (B, T))
@@ -545,7 +528,7 @@ def _conditioner():
     net = Conditioner(dim_codebook=128, num_phoneme_tokens=NUM_TOKENS)
     fill_module(net, 1234)
     net.cuda()
-    _round_params(net)
+    round_params(net)
     return net.train()
 
 
@@ -558,7 +541,7 @@ def _cond_case():
     B = len(LENS)
     text, duration, pitch = (torch.from_numpy(a).cuda() for a in (text_np, dur, pitch_np.astype(np.float32)))
     g = torch.Generator().manual_seed(13)
-    up = {"out prompt_enc": _bf(g, B, NPAD, 512), "out cond": _bf(g, B, 512, L_FRAMES)}
+    up = {"out prompt_enc": bf(g, B, NPAD, 512), "out cond": bf(g, B, 512, L_FRAMES)}
     names = [n for n, _ in net.named_parameters() if not n.startswith("duration_pitch.")]
     res = dict(family="enc", stats={}, fails=[], checks={})
 
@@ -598,10 +581,10 @@ def _cond_case():
         used[coarse[torch.from_numpy(d > 0)]] = True
         mask = eo.generate_mask_from_repeats(torch.from_numpy(d))
         mask = F.pad(mask, (0, L_FRAMES - mask.shape[-1])).cuda()
-        fwd = _conditioner_fwd(prompt[b:b + 1, :n], text[b:b + 1, :t], mask, F.one_hot(coarse, PITCH_BINS).cuda())
+        fwd = conditioner_fwd(prompt[b:b + 1, :n], text[b:b + 1, :t], mask, F.one_hot(coarse, PITCH_BINS).cuda())
         d_outs = {"out prompt_enc": up["out prompt_enc"][b:b + 1, :n], "out cond": up["out cond"][b:b + 1]}
         for dst, autocast in ((ref, False), (ac, True)):
-            _acc(dst, _ref_grads(fwd, params, d_outs, autocast=autocast, only=names), names)
+            _acc(dst, autograd(fwd, params, d_outs, autocast=autocast, only=names, cudnn="twin"), names)
     _against(res, got, ref, ac, names)
     res["checks"]["pitch rows without a valid frame are zeros"] = (
         int((got["pitch_emb.weight"].cpu()[~used] != 0).sum()) == 0 and 0 < int(used.sum()) < PITCH_BINS)
@@ -716,17 +699,7 @@ def test_cases_reach_the_key_and_query_tile_edges():
 
 # ---- wrong references: the same bounds must reject them ----
 def _assert_rejected(res, wrong, names):
-    margins = []
-    for n in names:
-        s = res["stats"][n]
-        o = res["ours"][n].reshape(wrong[n].shape)
-        rel = _rel(o, wrong[n])
-        share = _rel_qkv(o, wrong[n], wrong[n.replace("to_q", "to_kv")]) if s[2] is not None else None
-        b = _bound(s[1]) if res["family"] == "enc" else _dbound(s[1])
-        print(f"  {n}: rel-L2 vs the wrong reference {rel:.3e} (bound {b:.3e}, {rel / b:.1f}x)")
-        margins.append(rel / b)
-        assert _over_case(res, (rel, s[1], share)), f"the bound accepts a wrong reference for {n}"
-    return min(margins)
+    return assert_rejected(res["ours"], wrong, res["stats"], names, FAMILY[res["family"]], EITHER)[0]
 
 
 def _wrong_port(res, names, perceiver_rows, mean_rows):
@@ -748,7 +721,7 @@ def _wrong_port(res, names, perceiver_rows, mean_rows):
             return orig(P, cfg, torch.cat((prompt[:, :n], jrows.to(prompt.dtype)), 1))
         tp.perceiver_resampler = perceiver
         try:
-            gr = _port_grads(res["params"], res["kwargs"], sub, (dp[b:b + 1], dc[b:b + 1]), res["d_out"][b:b + 1],
+            gr = port_grads(res["params"], res["kwargs"], sub, (dp[b:b + 1], dc[b:b + 1]), res["d_out"][b:b + 1],
                              only=[k for k in names if not k.startswith("d ")] + ["d prompt"])
         finally:
             tp.perceiver_resampler = orig
@@ -795,7 +768,7 @@ def test_rejects_same_conv_reading_the_first_padded_rows():
                 h = F.silu(F.conv1d(h, P[f"conv.{i}.weight"], P[f"conv.{i}.bias"], padding=k // 2))
             return {"encoding": eo.transformer(h.transpose(1, 2)[:, :n], P, "transformer.", res["heads"])}
         up = res["up"][idx, :n]
-        gr = _ref_grads(fwd, dict(res["params"], x=xs), {"encoding": up}, only=names[:2] + ["x"])
+        gr = autograd(fwd, dict(res["params"], x=xs), {"encoding": up}, only=names[:2] + ["x"], cudnn="twin")
         _acc(wrong, gr, names[:2])
         for i, s in enumerate(idx):
             wrong[f"x {s}"] = gr["x"][i, :n]
@@ -814,5 +787,5 @@ def test_rejects_phoneme_attention_with_one_padded_token():
         up = torch.zeros(len(idx), ext, res["up"].shape[-1], device="cuda")
         up[:, :n] = res["up"][idx, :n]
         fwd = _enc_fwd("phon_default", res["x"][idx, :ext], PHON, res["heads"], None)
-        _acc(wrong, _ref_grads(fwd, res["params"], {"encoding": up}, only=names), names)
+        _acc(wrong, autograd(fwd, res["params"], {"encoding": up}, only=names, cudnn="twin"), names)
     print(f"\nphoneme attention with one padded token: smallest margin {_assert_rejected(res, wrong, names):.1f}x")

@@ -14,7 +14,7 @@ from torch import nn
 from helpers import GOLDEN
 from oracle import encoders_oracle as eo
 from param_fill import fill_module
-from test_training_objective_fp64_gpu import objective
+from restatements import objective
 
 
 @pytest.mark.parametrize("case", ["e2e_small", "e2e_wide"])

@@ -5,9 +5,9 @@ benchmark's training step (bench.py `train_step_dp`) at its own shape.
 
 The modules' float64 suites each feed one module random upstream gradients.  Here the reference is one float64
 autograd graph of the scalar an optimizer receives, composed from the pinned restatements only
-(`objective` below): `oracle.encoders_oracle` (prompt and phoneme encoders, the length regulator's alignment from
+(`restatements.objective`): `oracle.encoders_oracle` (prompt and phoneme encoders, the length regulator's alignment from
 generate_mask_from_repeats, the coarse pitch from f0_to_coarse, duration_pitch_predictor), with dropout the masked
-restatements of tests/dropout_oracle.py and test_duration_pitch_dropout_gpu.masked_trunk with the masks of the seeds
+restatements of tests/dropout_oracle.py and restatements.masked_trunk with the masks of the seeds
 the call drew; `oracle.denoiser_torch_port.model_forward_autograd` with the drop masks the call drew;
 `oracle.diffusion_oracle.diffusion_loss` with the wrapper's fp32 alpha / sigma; F.l1_loss of ns2.py:1587-1590 and
 tests/rvq_ce_restatement.residual_vq_ce on the objective's x_start with our own codes.  test_training_objective_cpu.py
@@ -25,12 +25,11 @@ Pitch sits at coarse-bin centres, so the bins agree exactly; the predictor's hea
 `_set_head_biases` on the float64 encodings, and durations that lie within DUR_GAP of a float64 duration prediction move
 by one frame.  The predictor's inputs carry the encoders' error, so MARGIN x its forward error is out of reach; instead
 the heads' ReLU branches and the signs of the L1 terms are asserted equal to float64's.
-Asserted: the loss and both L1 losses |ours - fp64| <= C_ENC x |twin - fp64| + REL_FLOOR_ENC x |fp64|; every parameter
-gradient of the five modules, d prompt_enc and d cond as the Model receives them and the total gradient at each
-encoder's output within its family's bound (`model.*` and the Model's inputs the denoiser's: C_DEN, REL_FLOOR,
-REL_CEILING of test_denoiser_configs_fp64_gpu; the rest the encoders': C_ENC, REL_FLOOR_ENC, their ceiling; every to_q
-may also pass under the encoders' to_q rule, TO_Q_BOUND of its share of the q / kv gradient), except the tensors
-EXCEPTIONS names; finite and exactly zero wherever float64 is (the Model's d prompt of prompt-dropped samples, its d
+Asserted, with the families of tests/fp64_check.py: the loss and both L1 losses |ours - fp64| <= C x |twin - fp64| +
+floor x |fp64| with the encoders' C and floor; every parameter gradient of the five modules, d prompt_enc and d cond as
+the Model receives them and the total gradient at each encoder's output within its family's bound (`model.*` and the
+Model's inputs the denoiser's, the rest the encoders'; every to_q may also pass under the to_q rule fp64_check.EITHER,
+TO_Q_BOUND of its share of the q / kv gradient), except the tensors EXCEPTIONS names; finite and exactly zero wherever float64 is (the Model's d prompt of prompt-dropped samples, its d
 cond of cond-dropped samples, the null parameters when nothing is dropped, pitch-table rows no frame reaches, token rows
 that never occur, the predictor's ReLU-dead rows); a bit-identical loss from two calls under one torch seed.
 Gradients are not required to be bit-identical: the attention backward adds dQ with fp32 atomics in an order that
@@ -41,7 +40,7 @@ prompt encoder's output as the prompt and the L1 terms' sign gradients upstream,
 suites' bounds, which were measured on random bf16 inputs and upstream gradients:
   * the Model's perceiver (every model.perceiver_resampler.* tensor) and d prompt_enc as the Model receives it: ours /
     twin up to 1.59 (ce_128 d prompt_enc: 5.43e-2 / 3.40e-2), 1.30 on the latents (5.46e-2 / 4.21e-2), 1.41 on layer
-    0's to_q; the twin itself reaches 5.3e-2, above REL_CEILING (1.5e-2) -> C = 2;
+    0's to_q; the twin itself reaches 5.3e-2, above the denoiser's ceiling (1.5e-2) -> C = 2;
   * the Model's transformer FiLM of the cross attention (layers.*.2.to_gamma_beta), its cross-attention to_q and its
     self-attention to_q: up to 1.34 (ce_128 layers.1.1.to_q, 1.49e-2 / 1.11e-2), above the ceiling where the twin is
     (full_512 layers.0.2.to_gamma_beta.weight 2.67e-2 / 3.59e-2) -> C = 1.5;
@@ -60,7 +59,7 @@ B: bench.py's training step (CFG3 = dim 512, depth 12; B 32, N 1024; prompt_enc 
 NaturalSpeech2 defaults) with rounded parameters and seeded inputs.  The float64 port cannot hold 32 samples at depth
 12, so it runs per chunk of BENCH_CHUNK samples from d mse_b = mean(w) / B (the batch's own weight) and accumulates
 in float64; so does the twin.  The loss, every parameter gradient, d prompt and d cond take the denoiser family's
-C_DEN x twin + REL_FLOOR, without the denoiser's REL_CEILING, which was measured at depth 2: at depth 12, 13 of our
+C x twin + floor, without the denoiser's ceiling, which was measured at depth 2: at depth 12, 13 of our
 tensors and 30 of the twin's exceed it.  Every to_q may also pass under the encoders' to_q rule (TO_Q_BOUND): the
 self-attention to_q of layers 1-11 have rel-L2 0.4 ... 5.8 on both sides (nearly flat attention), with shares of the
 q / kv gradient <= 3.5e-5.
@@ -92,24 +91,14 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-import dropout_oracle as do
+from fp64_check import DENOISER, EITHER, ENCODERS, assert_rejected, bf, compare, round_params, use
 from helpers import oracle_config
 from oracle import denoiser_torch_port as tp
 from oracle import diffusion_oracle as dfo
 from oracle import encoders_oracle as eo
 from param_fill import fill_module, rvq_fixture_inputs
-from rvq_ce_restatement import residual_vq_ce
-from test_conditioning_backward_fp64_gpu import C_AUTOCAST as C_ENC
-from test_conditioning_backward_fp64_gpu import REL_FLOOR as REL_FLOOR_ENC
-from test_conditioning_backward_fp64_gpu import TO_Q_BOUND, _bound, _encoder_masks, _rel, _rel_qkv, _round_params
-from test_denoiser_configs_fp64_gpu import C_AUTOCAST as C_DEN
-from test_denoiser_configs_fp64_gpu import REL_CEILING, REL_FLOOR
-from test_encoder_configs_fp64_gpu import _compare
-from test_denoiser_backward_fp64_gpu import _drop_masks
-from test_duration_pitch_backward_fp64_gpu import _set_head_biases
-from test_duration_pitch_dropout_gpu import _set_head_biases as _set_head_biases_masked
-from test_duration_pitch_dropout_gpu import masked_trunk, masks_for
-from test_ragged_training_fp64_gpu import _bf, _dbound
+from restatements import (drop_masks, encoder_masks, masks_for, objective, predict, set_head_biases,
+                          set_head_biases_masked)
 
 pytestmark = pytest.mark.gpu
 
@@ -139,75 +128,7 @@ BOUNDARY = {"d prompt_enc (model)": DEN, "d cond (model)": DEN, "d prompt_enc (t
             "d phoneme_enc (total)": ENC}
 
 
-# ---- the composed objective ----
-def objective(P, dtype, c, wrong=None):
-    """The scalar NaturalSpeech2.forward returns, as one graph over P ({"model." / "prompt_enc." / "phoneme_enc." /
-    "pitch_emb." / "duration_pitch." + name: tensor}) -> {"loss", "duration_loss", "pitch_loss"} and the boundary
-    tensors "pe" (prompt encoder output), "pe_model" (what the Model receives), "cond", "ph" (phoneme encodings).
-    `c` holds the inputs and host-side glue (alignment mask, coarse-pitch one-hot, per-phoneme pitch, alpha / sigma,
-    drop masks, dropout masks); `wrong` selects a deliberately wrong variant."""
-    sub = lambda pfx: {k[len(pfx):]: v for k, v in P.items() if k.startswith(pfx)}  # noqa: E731
-    attn, conv, pred_masks = c.get("masks", (None, None, None))
-    if attn is None:
-        pe = eo.speech_prompt_encoder(sub("prompt_enc."), c["prompt"].to(dtype), heads=c["heads"][0],
-                                      padding=c["padding"])
-    else:
-        pe = do.speech_prompt_encoder(sub("prompt_enc."), c["prompt"].to(dtype), heads=c["heads"][0],
-                                      padding=c["padding"], attn_masks=[m.to(dtype) for m in attn])
-    if conv is None:
-        ph = eo.phoneme_encoder(sub("phoneme_enc."), c["text"], heads=c["heads"][1])
-    else:
-        ph = do.phoneme_encoder(sub("phoneme_enc."), c["text"], heads=c["heads"][1], conv_mask=conv.to(dtype))
-    if "enc_values" in c:     # the downstream graph evaluated at given encoder outputs; gradients pass unchanged
-        pe = pe + (c["enc_values"][0].to(dtype) - pe).detach()
-        ph = ph + (c["enc_values"][1].to(dtype) - ph).detach()
-    # expand_encodings (ns2.py:1449-1455) with the alignment of the durations over L frames and the coarse pitch
-    m = c["mask"].to(dtype)
-    pitch = c["onehot"].to(dtype) @ P["pitch_emb.weight"]
-    cond = torch.einsum("btl,bdt->bdl", m, ph.transpose(1, 2)) + torch.einsum("btl,bdt->bdl", m, pitch.transpose(1, 2))
-    out = {"pe": pe, "ph": ph, "cond": cond}
-    if "duration_pitch.to_duration_pred.to_pred.0.bias" in P:
-        ph_in = ph.detach() if wrong == "predictor without phoneme stream" else ph
-        Pd = sub("duration_pitch.")
-        if wrong == "predictor on the null-substituted prompt":
-            dp = c["drop"][0]
-            null = P["model.null_prompt_tokens"][None].expand(int(dp.sum()), -1, -1)
-            keep, drop = _predict(Pd, ph_in[~dp], pe[~dp], c, None), _predict(Pd, ph_in[dp], null, c, None)
-            preds = [torch.empty(B, T, dtype=k.dtype, device=k.device).index_put((~dp,), k).index_put((dp,), d)
-                     for k, d in zip(keep, drop)]
-        else:
-            preds = _predict(Pd, ph_in, pe, c, pred_masks)
-        out["duration_loss"] = F.l1_loss(c["duration"].to(device=ph.device, dtype=dtype), preds[0].to(dtype))
-        out["pitch_loss"] = F.l1_loss(c["ph_pitch"].to(device=ph.device, dtype=dtype), preds[1].to(dtype))
-        out["duration_pred"], out["pitch_pred"] = preds
-    pe_model = pe.view_as(pe)              # the Model's share of d prompt_enc
-    cfg = c["cfg"]
-    a, s = c["alpha"].to(dtype), c["sigma"].to(dtype)
-    audio, noise = c["audio"].to(dtype), c["noise"].to(dtype)
-    noised = a[:, None, None] * audio + s[:, None, None] * noise
-    pred = tp.model_forward_autograd(sub("model."), oracle_config(c["model_kwargs"]), noised, c["times"].to(dtype),
-                                     pe_model, cond, drop_prompt=c["drop"][0], drop_cond=c["drop"][1]).to(dtype)
-    loss, _ = dfo.diffusion_loss(pred, audio, noise, a, s, cfg["objective"], cfg["min_snr_loss_weight"],
-                                 cfg["min_snr_gamma"])
-    if c.get("codebooks") is not None:
-        x_start = pred if wrong == "ce x_start = pred" else dfo.x_start_from_pred(audio, pred, a, s, cfg["objective"])
-        _, ce, _ = residual_vq_ce(x_start, c["codebooks"].to(dtype), c["codes"], own=c.get("own"))
-        loss = loss + cfg["ce_weight"] * ce
-    if "duration_loss" in out:
-        wd, wp = cfg["weights"][::-1] if wrong == "loss weights swapped" else cfg["weights"]
-        loss = loss + (wd * out["duration_loss"] + wp * out["pitch_loss"])
-    out.update(loss=loss, pe_model=pe_model)
-    return out
-
-
-def _predict(Pd, x, prompts, c, masks):
-    heads = c["heads"][2]
-    if masks is None:
-        return eo.duration_pitch_predictor(Pd, x, prompts, heads=heads)
-    return tuple(masked_trunk(Pd, pre, x, prompts, heads, None, [m.to(x.dtype) for m in masks[pre][1]])
-                 for pre in ("to_duration_pred.", "to_pitch_pred."))
-
-
+# ---- the composed objective (restatements.objective) ----
 def objective_grads(params, c, autocast=False, wrong=None, only=None):
     """({name: d loss / d name} over the parameters and the boundary tensors, {scalar name: value}) in fp64, or in fp32
     under bf16 autocast."""
@@ -239,7 +160,7 @@ def _modules(name):
     fill_module(cn, 1234)
     for m in (model, cn):
         m.cuda().train()
-        _round_params(m)
+        round_params(m)
     return model, cn
 
 
@@ -339,9 +260,9 @@ def _case(name):
     g = torch.Generator().manual_seed(41 + list(CASES).index(name))
     D = mkw["dim"]
     c = dict(model_kwargs=mkw, heads=(cn.prompt_enc.heads, cn.phoneme_enc.heads, cn.duration_pitch.heads),
-             padding=cn.prompt_enc.padding, prompt=_bf(g, B, NP, 128),
+             padding=cn.prompt_enc.padding, prompt=bf(g, B, NP, 128),
              text=torch.from_numpy(rng.integers(0, NUM_TOKENS // 2, (B, T))).cuda(),
-             times=torch.rand(B, generator=g).cuda(), noise=_bf(g, B, N, D))
+             times=torch.rand(B, generator=g).cuda(), noise=bf(g, B, N, D))
     codec = None
     if ce:
         cb, frames = rvq_fixture_inputs()
@@ -351,12 +272,12 @@ def _case(name):
         codec = EncodecRVQ(cb).cuda()
         c.update(audio=audio.view(B, N, D).bfloat16().float().cuda(), codes=codes, codebooks=codec.codebooks)
     else:
-        c["audio"] = _bf(g, B, N, D)
+        c["audio"] = bf(g, B, N, D)
     ns = NaturalSpeech2(model, codec, target_sample_hz=24000, timesteps=4, conditioner=cn, **nkw)
     c["cfg"] = dict(objective=ns.objective, min_snr_loss_weight=ns.min_snr_loss_weight, min_snr_gamma=ns.min_snr_gamma,
                     ce_weight=ns.rvq_cross_entropy_loss_weight, weights=(ns.duration_loss_weight, ns.pitch_loss_weight))
     c["alpha"], c["sigma"] = gamma_to_alpha_sigma(ns.gamma_schedule(c["times"]), ns.scale)
-    seed = _drop_masks(B, p)[0] if p > 0 else 5
+    seed = drop_masks(B, p)[0] if p > 0 else 5
     dur = _durations(rng)
     _host_glue(c, dur, _pitch(rng, dur)[0])
 
@@ -383,8 +304,8 @@ def _case(name):
         assert set(spy.seeds) == {"prompt_enc", "phoneme_enc", "duration_pitch"}, spy.seeds
         assert (cn.prompt_enc.attn_dropout, cn.phoneme_enc.conv_dropout) == (0.2, 0.2)
         pm = masks_for(spy.seeds["duration_pitch"], cn.duration_pitch.attn_dropout, B, T, NP)
-        c["masks"] = (_encoder_masks("SpeechPromptEncoder", spy.seeds["prompt_enc"], B, NP)[0],
-                      _encoder_masks("PhonemeEncoder", spy.seeds["phoneme_enc"], B, T)[1], pm)
+        c["masks"] = (encoder_masks("SpeechPromptEncoder", spy.seeds["prompt_enc"], B, NP)[0],
+                      encoder_masks("PhonemeEncoder", spy.seeds["phoneme_enc"], B, T)[1], pm)
     params = {f"model.{n}": q.detach() for n, q in model.named_parameters()}
     params.update({n: q.detach() for n, q in cn.named_parameters()})
     # the predictor's head biases from the float64 encodings, then durations away from the duration predictions
@@ -394,13 +315,13 @@ def _case(name):
         tmp = objective({k: v for k, v in P64.items() if not k.startswith("duration_pitch.")}, torch.float64, c)
         enc["pe"], enc["ph"] = tmp["pe"], tmp["ph"]
     if ckw:
-        _set_head_biases_masked(cn.duration_pitch, {n: q.detach() for n, q in cn.duration_pitch.named_parameters()},
+        set_head_biases_masked(cn.duration_pitch, {n: q.detach() for n, q in cn.duration_pitch.named_parameters()},
                                 enc["ph"], enc["pe"], c["masks"][2])
     else:
-        _set_head_biases(cn.duration_pitch, enc["ph"], enc["pe"], False, heads=c["heads"][2])
+        set_head_biases(cn.duration_pitch, enc["ph"], enc["pe"], False, heads=c["heads"][2])
     params.update({n: q.detach() for n, q in cn.named_parameters() if n.startswith("duration_pitch.")})
     with torch.no_grad(), torch.backends.cudnn.flags(enabled=False):
-        pred = _predict({k[15:]: v.double() for k, v in params.items() if k.startswith("duration_pitch.")},
+        pred = predict({k[15:]: v.double() for k, v in params.items() if k.startswith("duration_pitch.")},
                         enc["ph"], enc["pe"], c, c.get("masks", (None,) * 3)[2])[0].cpu().numpy()
     moved = 0
     for b in range(B):
@@ -413,7 +334,7 @@ def _case(name):
     with torch.no_grad(), torch.backends.cudnn.flags(enabled=False):
         shifted = {k[15:]: v.double() + (1e3 if k.endswith("to_pred.0.bias") else 0)
                    for k, v in params.items() if k.startswith("duration_pitch.")}
-        pre = _predict(shifted, enc["ph"], enc["pe"], c, c.get("masks", (None,) * 3)[2])
+        pre = predict(shifted, enc["ph"], enc["pe"], c, c.get("masks", (None,) * 3)[2])
     min_pre = min(float((v - 1e3).abs().min()) for v in pre)
     _host_glue(c, dur, _pitch(rng, dur)[0])
 
@@ -482,8 +403,7 @@ def _fill(res_den, res_enc, got, ref, ac, names):
             if bool((r != 0).any()):
                 res["fails"].append((n, "missing"))
             continue
-        share = _rel_qkv(o, r, ref[n.replace("to_q", "to_kv")]) if n.endswith("to_q.weight") else None
-        st = _compare(o.reshape(r.shape), r, ac[n], share)
+        st = compare(o, r, ac[n], ref[n.replace("to_q", "to_kv")] if n.endswith("to_q.weight") else None)
         if isinstance(st, str):
             res["fails"].append((n, st))
         elif st is not None:
@@ -498,30 +418,16 @@ _KEEP = ("prompt_enc.conv.1.weight", "prompt_enc.transformer.layers.5.3.2.weight
          "d phoneme_enc (total)")
 
 
-def _exception(n):
-    """The EXCEPTIONS entry that names tensor `n`, or None."""
-    return next((e for e in EXCEPTIONS if re.search(e[0], n)), None)
-
-
-def _rel_bound(n, res, rel_ac):
-    """rel-L2 bound of tensor `n`: its family's, or C x twin + the family's floor for a named exception."""
-    e = _exception(n)
-    if e is not None:
-        return e[1] * rel_ac + (REL_FLOOR_ENC if res["family"] == ENC else REL_FLOOR)
-    return _bound(rel_ac) if res["family"] == ENC else _dbound(rel_ac)
-
-
-def _use_of(res, s, n):
-    """Share of a tensor's bound: the rel-L2 bound, and for a to_q the smaller of that and its share of the q / kv
-    gradient against TO_Q_BOUND (the encoders' to_q rule)."""
-    rel, rel_ac, share = s
-    use = rel / _rel_bound(n, res, rel_ac)
-    return use if share is None else min(use, share / TO_Q_BOUND)
+def _family(n):
+    """The bounds of tensor `n`: its family's, or for a named exception C x twin + the family's floor, no ceiling."""
+    fam = DENOISER if n.startswith("model.") or BOUNDARY.get(n) == DEN else ENCODERS
+    e = next((e for e in EXCEPTIONS if re.search(e[0], n)), None)
+    return fam if e is None else fam.without_ceiling(e[1])
 
 
 def _scalar_excess(ours, r64, r32):
-    """|ours - fp64| / (C_ENC |twin - fp64| + REL_FLOOR_ENC |fp64|)."""
-    return abs(float(ours) - float(r64)) / (C_ENC * abs(float(r32) - float(r64)) + REL_FLOOR_ENC * abs(float(r64)))
+    """|ours - fp64| / (C |twin - fp64| + floor |fp64|) with the encoders' C and floor."""
+    return abs(float(ours) - float(r64)) / (ENCODERS.c * abs(float(r32) - float(r64)) + ENCODERS.floor * abs(float(r64)))
 
 
 def _report(name, r):
@@ -533,19 +439,19 @@ def _report(name, r):
                     f"({_scalar_excess(r['scal'][k], r['s64'][k], r['s32'][k]):.0%} of its bound)")
     for fam in ("den", "enc", "den_at", "enc_at"):
         res = r[fam]
-        rest = {n: st for n, st in res["stats"].items() if st[2] is None}
-        worst = max(rest.items(), key=lambda kv: kv[1][0])
-        ratio = max(((n, st) for n, st in rest.items() if st[1] > 0), key=lambda kv: kv[1][0] / kv[1][1])
-        tight = max(res["stats"].items(), key=lambda kv: _use_of(res, kv[1], kv[0]))
-        worst_q = max(((n, st) for n, st in res["stats"].items() if st[2] is not None), key=lambda kv: kv[1][2])
-        line.append(f"  {fam}: worst {worst[0]} ours {worst[1][0]:.2e} / autocast {worst[1][1]:.2e}; max ratio "
-                    f"{ratio[1][0] / ratio[1][1]:.2f} ({ratio[0]}); worst to_q share {worst_q[0]} {worst_q[1][2]:.2e} "
-                    f"({worst_q[1][0]:.2e} / {worst_q[1][1]:.2e}); tightest {tight[0]} at {_use_of(res, tight[1], tight[0]):.0%} "
-                    f"of its bound ({tight[1][0]:.2e} / {tight[1][1]:.2e})")
-        over = sorted(((n, st) for n, st in res["stats"].items() if _use_of(res, st, n) > 1),
-                      key=lambda kv: -_use_of(res, kv[1], kv[0]))
-        for n, st in over[:40]:
-            line.append(f"    over: {n} {st[0]:.2e} / {st[1]:.2e} share {st[2]} ({_use_of(res, st, n):.0%})")
+        u = {n: use(_family(n), st, EITHER) for n, st in res["stats"].items()}
+        rest = {n: st for n, st in res["stats"].items() if st.share is None}
+        worst = max(rest.items(), key=lambda kv: kv[1].rel)
+        ratio = max(((n, st) for n, st in rest.items() if st.rel_ac > 0), key=lambda kv: kv[1].rel / kv[1].rel_ac)
+        tight = max(res["stats"].items(), key=lambda kv: u[kv[0]])
+        worst_q = max(((n, st) for n, st in res["stats"].items() if st.share is not None), key=lambda kv: kv[1].share)
+        line.append(f"  {fam}: worst {worst[0]} ours {worst[1].rel:.2e} / autocast {worst[1].rel_ac:.2e}; max ratio "
+                    f"{ratio[1].rel / ratio[1].rel_ac:.2f} ({ratio[0]}); worst to_q share {worst_q[0]} "
+                    f"{worst_q[1].share:.2e} ({worst_q[1].rel:.2e} / {worst_q[1].rel_ac:.2e}); tightest {tight[0]} at "
+                    f"{u[tight[0]]:.0%} of its bound ({tight[1].rel:.2e} / {tight[1].rel_ac:.2e})")
+        over_bound = sorted(((n, st) for n, st in res["stats"].items() if u[n] > 1), key=lambda kv: -u[kv[0]])
+        for n, st in over_bound[:40]:
+            line.append(f"    over: {n} {st.rel:.2e} / {st.rel_ac:.2e} share {st.share} ({u[n]:.0%})")
     print("\n".join(line))
 
 
@@ -561,7 +467,7 @@ def test_objective_matches_fp64(name):
     for res in (r["den"], r["enc"]):
         assert not res["fails"], res["fails"][:8]
     for res in (r["den"], r["enc"]):
-        bad = [(n, s) for n, s in res["stats"].items() if _use_of(res, s, n) > 1]
+        bad = [(n, s) for n, s in res["stats"].items() if use(_family(n), s, EITHER) > 1]
         assert not bad, f"{len(bad)} tensors over the bound (rel-L2, autocast rel-L2, to_q share): {bad[:8]}"
     assert all(n in r[BOUNDARY[n]]["stats"] for n in BOUNDARY)
 
@@ -573,18 +479,11 @@ def test_full_case_drops_some_samples_and_keeps_others():
 
 # ---- wrong references ----
 def _assert_rejected(name, wrong, names):
+    """The bounds of each tensor's family (no to_q rule: no to_q is named) must reject the wrong variant."""
     r = _case(name)
     wg, ws = objective_grads(r["params"], r["c"], wrong=wrong, only=names)
-    margins = []
-    for n in names:
-        res = r["den"] if n.startswith("model.") or BOUNDARY.get(n) == DEN else r["enc"]
-        s = res["stats"][n]
-        rel = _rel(r["ours"][n].reshape(wg[n].shape), wg[n])
-        b = _rel_bound(n, res, s[1])
-        print(f"  {n}: rel-L2 vs the wrong reference {rel:.3e} (bound {b:.3e}, {rel / b:.1f}x)")
-        margins.append((rel / b, n))
-        assert rel > b, f"the bound accepts a wrong reference for {n}"
-    print(f"{name} / {wrong}: smallest margin {min(margins)[0]:.1f}x ({min(margins)[1]})")
+    m = assert_rejected(r["ours"], wg, dict(r["den"]["stats"], **r["enc"]["stats"]), names, _family)
+    print(f"{name} / {wrong}: smallest margin {m[0]:.1f}x ({m[1]})")
     return ws
 
 
@@ -648,11 +547,11 @@ def test_bench_training_step_matches_fp64():
     t0 = time.perf_counter()
     torch.manual_seed(0)
     model = Model(**bench.CFG3).cuda().train()
-    _round_params(model)
+    round_params(model)
     ns = NaturalSpeech2(model, target_sample_hz=24000)
     g = torch.Generator().manual_seed(100)
-    inp = {"lat": _bf(g, Bb, Nb, 512), "prompt": _bf(g, Bb, 103, 512), "cond": _bf(g, Bb, 512, Nb),
-           "times": torch.rand(Bb, generator=g).cuda(), "noise": _bf(g, Bb, Nb, 512)}
+    inp = {"lat": bf(g, Bb, Nb, 512), "prompt": bf(g, Bb, 103, 512), "cond": bf(g, Bb, 512, Nb),
+           "times": torch.rand(Bb, generator=g).cuda(), "noise": bf(g, Bb, Nb, 512)}
     X = {k: inp[k].clone().requires_grad_(True) for k in ("prompt", "cond")}
     torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats()
@@ -683,24 +582,24 @@ def test_bench_training_step_matches_fp64():
     peak = torch.cuda.max_memory_allocated() / 2 ** 30
     stats, fails = {}, []
     for n, r in ref.items():
-        q = n.endswith("to_q.weight")
-        s = _compare(got[n].reshape(r.shape), r, ac[n], _rel_qkv(got[n], r, ref[n.replace("to_q", "to_kv")]) if q else None)
+        s = compare(got[n], r, ac[n], ref[n.replace("to_q", "to_kv")] if n.endswith("to_q.weight") else None)
         if isinstance(s, str):
             fails.append((n, s))
         elif s is not None:
             stats[n] = s
-    rest = {n: s for n, s in stats.items() if s[2] is None}
-    worst = max(rest.items(), key=lambda kv: kv[1][0])
+    rest = {n: s for n, s in stats.items() if s.share is None}
+    worst = max(rest.items(), key=lambda kv: kv[1].rel)
     tight = max(stats.items(), key=lambda kv: _bench_use(kv[1]))
-    ratio = max(rest.items(), key=lambda kv: kv[1][0] / kv[1][1])
-    worst_q = max(((n, s) for n, s in stats.items() if s[2] is not None), key=lambda kv: kv[1][2])
+    ratio = max(rest.items(), key=lambda kv: kv[1].rel / kv[1].rel_ac)
+    worst_q = max(((n, s) for n, s in stats.items() if s.share is not None), key=lambda kv: kv[1].share)
     l64, l32 = tot[torch.float64], tot[torch.float32]
     le = _scalar_excess(loss.detach(), l64, l32)
     print(f"\nbench step: {len(stats)} tensors; loss ours {float(loss.detach()):.8g} fp64 {l64:.8g} twin {l32:.8g} "
-          f"({le:.0%} of its bound); worst {worst[0]} {worst[1][0]:.2e} / autocast {worst[1][1]:.2e}; max ratio "
-          f"{ratio[1][0] / ratio[1][1]:.2f} ({ratio[0]}); {sum(s[0] > REL_CEILING for s in rest.values())} tensors past "
-          f"the depth-2 ceiling (twin: {sum(s[1] > REL_CEILING for s in rest.values())}); worst to_q share {worst_q[0]} "
-          f"{worst_q[1][2]:.2e} (rel-L2 {worst_q[1][0]:.2e} / autocast {worst_q[1][1]:.2e}); tightest {tight[0]} at "
+          f"({le:.0%} of its bound); worst {worst[0]} {worst[1].rel:.2e} / autocast {worst[1].rel_ac:.2e}; max ratio "
+          f"{ratio[1].rel / ratio[1].rel_ac:.2f} ({ratio[0]}); {sum(s.rel > DENOISER.ceiling for s in rest.values())} "
+          f"tensors past the depth-2 ceiling (twin: {sum(s.rel_ac > DENOISER.ceiling for s in rest.values())}); worst "
+          f"to_q share {worst_q[0]} {worst_q[1].share:.2e} (rel-L2 {worst_q[1].rel:.2e} / autocast "
+          f"{worst_q[1].rel_ac:.2e}); tightest {tight[0]} at "
           f"{_bench_use(tight[1]):.0%} of its bound; peak memory {peak:.1f} GiB; ours {t_ours:.1f} s, fp64 {t_ref:.1f} s, "
           f"whole test {time.perf_counter() - t0:.1f} s")
     assert le <= 1, (float(loss.detach()), l64, l32)
@@ -710,8 +609,6 @@ def test_bench_training_step_matches_fp64():
 
 
 def _bench_use(s):
-    """B's bound: C_DEN x twin + REL_FLOOR without the denoiser's depth-2 ceiling (at depth 12 the twin itself exceeds
-    it on 30 tensors), and for a to_q the to_q rule."""
-    rel, rel_ac, share = s
-    use = rel / (C_DEN * rel_ac + REL_FLOOR)
-    return use if share is None else min(use, share / TO_Q_BOUND)
+    """B's bound: the denoiser's C x twin + floor without its depth-2 ceiling (at depth 12 the twin itself exceeds it
+    on 30 tensors), and for a to_q the to_q rule."""
+    return use(DENOISER.without_ceiling(), s, EITHER)

@@ -108,6 +108,21 @@ typedef struct ns2_gemm_args {
 
 int ns2_gemm(const ns2_gemm_args* args, ns2_stream_t stream);
 
+/* ns2_gemm over a batch of sequences of different lengths, padded at the end: batch b's rows [0, row_lens[b]) are the
+ * sample, the rest padding.  row_lens: device int32 (a_batches), each value clamped to [1, a_rows].  Only the 128-row
+ * tiles that start before row_lens[b] are computed and stored (ceil(row_lens[b] / 128) tiles of batch b per group and
+ * n-tile); every row of those tiles, including the rows at or past row_lens[b] inside the last one, is bit-identical to
+ * ns2_gemm's.  Rows of the other tiles are left untouched: neither written nor, with the F32 epilogue's in-place
+ * residual, reduce-added.  A computed row reads A rows of its own tile and, through causal shifts, earlier ones, so
+ * rows in untouched tiles (whatever they hold, NaN included) reach no computed row unless a negative shift_units (an
+ * anti-causal tap) reads past the tile; callers must not pass such segments with padding that is not finite.
+ * a_batches must be <= NS2_GEMM_ROW_LENS_MAX_BATCHES (the lengths and their prefix sums live in the kernel's shared
+ * memory); a larger batch is an error and nothing is launched.  row_lens == NULL is exactly ns2_gemm, which forwards to
+ * this call.  An argument rather than a field of ns2_gemm_args, so that the struct's layout stays that of ABI
+ * version 8. */
+#define NS2_GEMM_ROW_LENS_MAX_BATCHES 64
+int ns2_gemm_row_lens(const ns2_gemm_args* args, const int32_t* row_lens, ns2_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * 1b. Weight gradient of a Linear / CausalConv1d tap (autograd's grad_weight = grad_output^T @ input; the reference
  *     reaches it through loss.backward(), README.md:63, ns2.py:1886):
@@ -185,6 +200,16 @@ typedef struct ns2_attn_args {
 
 int ns2_attn_fwd(const ns2_attn_args* args, ns2_stream_t stream);
 
+/* ns2_attn_fwd with query lengths: sample b's queries [0, q_lens[b]) are the sample, the rest padding (device int32
+ * (batches), each value clamped to [1, q_len]).  A 128-query tile that starts at or past q_lens[b] does nothing: its out
+ * rows and lse entries are left untouched.  Every row of the other tiles, including rows at or past q_lens[b] inside
+ * the last one, is bit-identical to ns2_attn_fwd's with the same kv_lens (or none).  Self-attention over padded
+ * sequences passes the same lengths as kv_lens; cross-attention to unpadded keys passes q_lens only.  Q rows of skipped
+ * tiles are never loaded, so they may hold anything; K / V rows must be finite as for ns2_attn_fwd.  q_lens == NULL is
+ * exactly ns2_attn_fwd.  q_lens together with a dropout of p > 0 is an error (nothing is launched).  An argument rather
+ * than a field of ns2_attn_args, so that the struct's layout stays that of ABI version 8. */
+int ns2_attn_fwd_q_lens(const ns2_attn_args* args, const int32_t* q_lens, ns2_stream_t stream);
+
 /* Backward of the above (autograd of F.scaled_dot_product_attention, reached from loss.backward(), ns2.py:1886):
  *   dq_accum (batches, q_len, heads*64) f32, contiguous: dQ is ADDED to it (every key tile adds its share; zero it for
  *   a plain gradient);
@@ -243,6 +268,14 @@ int ns2_rmsnorm_film(const float* x, int64_t x_row_stride, int64_t rows, int32_t
                      int32_t rows_per_batch, const float* gamma, const float* film,
                      int64_t film_batch_stride, void* out_bf16, int64_t out_row_stride,
                      ns2_stream_t stream);
+
+/* ns2_rmsnorm_film with per-batch row counts: lens device int32 (rows / rows_per_batch), each value clamped to
+ * [1, rows_per_batch].  Row r of batch b = r / rows_per_batch is normalized only if r % rows_per_batch < lens[b], by the
+ * same per-row code as ns2_rmsnorm_film (bit-identical); the other rows are neither read nor written.  lens == NULL is
+ * exactly ns2_rmsnorm_film, which forwards to this call. */
+int ns2_rmsnorm_film_lens(const float* x, int64_t x_row_stride, int64_t rows, int32_t dim, int32_t rows_per_batch,
+                          const float* gamma, const float* film, int64_t film_batch_stride, void* out_bf16,
+                          int64_t out_row_stride, const int32_t* lens, ns2_stream_t stream);
 
 /* Same, fp32 output (PerceiverResampler.norm, ns2.py:566,579). */
 int ns2_rmsnorm_f32(const float* x, int64_t x_row_stride, int64_t rows, int32_t dim,
@@ -356,6 +389,14 @@ int ns2_mse_rows(const float* pred, const float* target, int32_t batch, int64_t 
                  float* scratch /* batch * NS2_MSE_SCRATCH_PER_SAMPLE floats */, float* out,
                  float* mean_out /* optional: mean over the batch of out[], ns2.py:1666 */,
                  ns2_stream_t stream);
+/*    ns2_mse_rows_lens : ns2_mse_rows over a batch padded at the end: sample b is its first lens[b] rows of row_elems
+ *                        elements (device int32 (batch), each clamped to [1, per_sample / row_elems]; row_elems a
+ *                        multiple of 4 dividing per_sample).  out[b] is the mean over those lens[b] * row_elems elements,
+ *                        reduced in the order a call on the unpadded sample uses: bit-identical to it.  Elements past
+ *                        them are not read (they may hold anything).  mean_out as for ns2_mse_rows.  lens == NULL is
+ *                        exactly ns2_mse_rows, which forwards to this call. */
+int ns2_mse_rows_lens(const float* pred, const float* target, int32_t batch, int64_t per_sample, float* scratch,
+                      float* out, float* mean_out, int64_t row_elems, const int32_t* lens, ns2_stream_t stream);
 int ns2_ddim_step(float* x, const float* v, const float* alpha, const float* sigma,
                   const float* alpha_next, const float* sigma_next, int32_t batch,
                   int64_t per_sample, int32_t objective, ns2_stream_t stream);
@@ -450,6 +491,12 @@ int ns2_film_wgrad(const float* dfilm, int64_t dfilm_batch_stride /* elements be
                    column window of the stacked FiLM gradient can be reduced as soon as its layer is final */,
                    const float* t, int32_t batch, int64_t rows, int32_t cols, float* dw,
                    int32_t accumulate /* 0: dw = ..., dw need not be initialised; 1: dw += ... */, ns2_stream_t stream);
+/*    ns2_mse_bwd_lens     : ns2_mse_bwd with the lengths of ns2_mse_rows_lens: the first lens[b] rows of row_elems
+ *                           elements of sample b are bit-identical to ns2_mse_bwd's, every element past them is written
+ *                           as an exact zero (pred / target are not read there).  lens == NULL is exactly ns2_mse_bwd,
+ *                           which forwards to this call. */
+int ns2_mse_bwd_lens(const float* pred, const float* target, const float* coef, int32_t batch, int64_t per_sample,
+                     void* out_bf16, float* out_f32, int64_t row_elems, const int32_t* lens, ns2_stream_t stream);
 /*    ns2_accum_bf16       : acc (f32) += t (bf16); acc_bf16 (optional) = bf16(acc)   (joins a branch gradient) */
 int ns2_accum_bf16(float* acc, const void* t_bf16, int64_t count, void* acc_bf16, ns2_stream_t stream);
 

@@ -52,6 +52,7 @@ struct AttnDev {
   float* lse;   // optional (batches, heads, q_len): log2-domain log-sum-exp of the scaled scores, for the backward pass
   DropoutDev drop;   // attn_fwd_kernel<true, false> only
   const int* kv_lens;   // attn_fwd_kernel<false, true> only: (batches) key counts, clamped to [1, kv_len]
+  const int* q_lens;    // attn_fwd_kernel<false, *, true> only: (batches) query counts, clamped to [1, q_len]
 };
 
 __device__ __forceinline__ float ex2_approx(float x) {
@@ -62,9 +63,12 @@ __device__ __forceinline__ float ex2_approx(float x) {
 
 __device__ __forceinline__ float keep_if(float x, uint32_t bits, int n) { return (bits >> n) & 1u ? x : 0.f; }
 
-template <bool DROPOUT, bool RAGGED>
+// attn_fwd_kernel<false, *, true> (ns2_attn_fwd_q_lens) adds query padding: a CTA whose query tile starts at or past
+// q_lens[b] returns before it touches anything, the others run exactly as attn_fwd_kernel<false, RAGGED>.
+template <bool DROPOUT, bool RAGGED, bool QLENS = false>
 __global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid_constant__ AttnDev p) {
   static_assert(!(DROPOUT && RAGGED), "no dropout variant of the key-padding kernel");
+  static_assert(!(DROPOUT && QLENS), "no dropout variant of the query-padding kernel");
   using namespace attn;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
@@ -76,6 +80,7 @@ __global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid
   const int q0 = blockIdx.x * BQ;
   const int head = blockIdx.y;
   const int b = blockIdx.z;
+  if (QLENS && q0 >= min(max(__ldg(p.q_lens + b), 1), p.q_len)) return;   // uniform over the CTA
   // keys of this sample; the plain kernels read p.kv_len where they use it, which keeps their code as it was
   const int kv_len_b = RAGGED ? min(max(__ldg(p.kv_lens + b), 1), p.kv_len) : 0;
 #define NS2_ATTN_KV_LEN (RAGGED ? kv_len_b : p.kv_len)
@@ -245,8 +250,10 @@ __global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid
 using namespace ns2;
 
 // No dropout (or p = 0) and no kv_lens: the plain kernel; dropout with p > 0: attn_fwd_kernel<true, false>; kv_lens:
-// attn_fwd_kernel<false, true> (never both).
-extern "C" int ns2_attn_fwd(const ns2_attn_args* a, ns2_stream_t stream_) {
+// attn_fwd_kernel<false, true> (never both); q_lens: attn_fwd_kernel<false, kv_lens != NULL, true>.
+extern "C" int ns2_attn_fwd(const ns2_attn_args* a, ns2_stream_t stream) { return ns2_attn_fwd_q_lens(a, nullptr, stream); }
+
+extern "C" int ns2_attn_fwd_q_lens(const ns2_attn_args* a, const int32_t* q_lens, ns2_stream_t stream_) {
   NS2_REQUIRE(a != nullptr, "attn_fwd: NULL args");
   const ns2_dropout* d = a->dropout;
   DropoutDev drop;
@@ -254,6 +261,7 @@ extern "C" int ns2_attn_fwd(const ns2_attn_args* a, ns2_stream_t stream_) {
               static_cast<double>(d->p));
   const bool dropout = d != nullptr && d->p != 0.0f;
   NS2_REQUIRE(!(dropout && a->kv_lens), "attn_fwd: kv_lens with dropout p > 0 is not supported");
+  NS2_REQUIRE(!(dropout && q_lens), "attn_fwd: q_lens with dropout p > 0 is not supported");
   NS2_REQUIRE(a->q && a->k && a->v && a->out, "attn_fwd: NULL pointer");
   NS2_REQUIRE(a->dim_head == 64, "attn_fwd: dim_head=%d, only 64 is supported", a->dim_head);
   NS2_REQUIRE(a->batches > 0 && a->heads > 0 && a->q_len > 0 && a->kv_len > 0, "attn_fwd: empty problem");
@@ -288,8 +296,15 @@ extern "C" int ns2_attn_fwd(const ns2_attn_args* a, ns2_stream_t stream_) {
   dev.scale_log2e = a->scale * 1.4426950408889634f;
   dev.lse = a->lse;
   dim3 grid((a->q_len + attn::BQ - 1) / attn::BQ, a->heads, a->batches);
-  if (a->kv_lens != nullptr) {
-    dev.kv_lens = a->kv_lens;
+  dev.kv_lens = a->kv_lens;
+  dev.q_lens = q_lens;
+  if (q_lens != nullptr && a->kv_lens != nullptr) {
+    NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<false, true, true>, attn::SMEM_BYTES));
+    attn_fwd_kernel<false, true, true><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
+  } else if (q_lens != nullptr) {
+    NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<false, false, true>, attn::SMEM_BYTES));
+    attn_fwd_kernel<false, false, true><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
+  } else if (a->kv_lens != nullptr) {
     NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<false, true>, attn::SMEM_BYTES));
     attn_fwd_kernel<false, true><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
   } else if (!dropout) {

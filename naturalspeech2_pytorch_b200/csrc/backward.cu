@@ -274,16 +274,23 @@ __global__ void __launch_bounds__(256) group_sum_kernel(const uint32_t* __restri
 }
 
 // d pred = coef[b] * (pred - target) -> fp32 residual-stream gradient seed and its bf16 copy  (MSE backward, ns2.py:1646-1666)
+// With lens (ns2_mse_bwd_lens): elements past sample b's first lens[b] rows of row4 float4s are written as exact zeros
+// (pred / target are not read there).
 __global__ void __launch_bounds__(256) mse_bwd_kernel(const float4* __restrict__ pred, const float4* __restrict__ target,
                                                       const float* __restrict__ coef, long long per4,
-                                                      uint2* __restrict__ out_bf, float4* __restrict__ out_f32) {
+                                                      uint2* __restrict__ out_bf, float4* __restrict__ out_f32,
+                                                      const int* __restrict__ lens, long long row4, int rows) {
   const int b = blockIdx.y;
   const float cf = coef[b];
   const long long base = static_cast<long long>(b) * per4;
+  const long long n4 = lens == nullptr ? per4 : static_cast<long long>(min(max(__ldg(lens + b), 1), rows)) * row4;
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < per4;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const float4 p = __ldg(pred + base + i), t = __ldg(target + base + i);
-    const float4 d = make_float4(cf * (p.x - t.x), cf * (p.y - t.y), cf * (p.z - t.z), cf * (p.w - t.w));
+    float4 d = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (i < n4) {
+      const float4 p = __ldg(pred + base + i), t = __ldg(target + base + i);
+      d = make_float4(cf * (p.x - t.x), cf * (p.y - t.y), cf * (p.z - t.z), cf * (p.w - t.w));
+    }
     if (out_bf != nullptr) out_bf[base + i] = make_uint2(f2_to_bf2(d.x, d.y), f2_to_bf2(d.z, d.w));
     if (out_f32 != nullptr) out_f32[base + i] = d;
   }
@@ -450,12 +457,24 @@ extern "C" int ns2_group_sum_bf16(const void* t_bf16, int64_t rows, int32_t dim,
 
 extern "C" int ns2_mse_bwd(const float* pred, const float* target, const float* coef, int32_t batch, int64_t per_sample,
                            void* out_bf16, float* out_f32, ns2_stream_t stream_) {
+  return ns2_mse_bwd_lens(pred, target, coef, batch, per_sample, out_bf16, out_f32, per_sample, nullptr, stream_);
+}
+
+extern "C" int ns2_mse_bwd_lens(const float* pred, const float* target, const float* coef, int32_t batch,
+                                int64_t per_sample, void* out_bf16, float* out_f32, int64_t row_elems,
+                                const int32_t* lens, ns2_stream_t stream_) {
   NS2_REQUIRE(pred && target && coef && (out_bf16 || out_f32) && batch > 0 && per_sample % 4 == 0, "mse_bwd: bad arguments");
+  NS2_REQUIRE(lens == nullptr || (row_elems > 0 && row_elems % 4 == 0 && per_sample % row_elems == 0),
+              "mse_bwd_lens: row_elems=%lld must be a positive multiple of 4 dividing per_sample=%lld",
+              static_cast<long long>(row_elems), static_cast<long long>(per_sample));
+  const long long row4 = lens == nullptr ? 0 : row_elems / 4;
+  const int rows = lens == nullptr ? 0 : static_cast<int>(per_sample / row_elems);
   dim3 grid(grid_1d(per_sample / 4, 64), batch);
   mse_bwd_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream_)>>>(reinterpret_cast<const float4*>(pred),
                                                                       reinterpret_cast<const float4*>(target), coef,
                                                                       per_sample / 4, reinterpret_cast<uint2*>(out_bf16),
-                                                                      reinterpret_cast<float4*>(out_f32));
+                                                                      reinterpret_cast<float4*>(out_f32), lens, row4,
+                                                                      rows);
   return launched(1);
 }
 

@@ -62,15 +62,24 @@ __device__ __forceinline__ void rmsnorm_row(const float4 (&v)[VEC], long long ro
 // RMSNorm (+gamma) (+FiLM): one warp per row, the row stays in registers between the reduction and the
 // scaled write (single HBM read of x, single write of the result).  DIM = 32 * 4 * VEC.
 // ------------------------------------------------------------------------------------------------
-template <int VEC, bool OUT_BF16>
+// LENS (ns2_rmsnorm_film_lens): row r of batch b = r / rows_per_batch is live iff r % rows_per_batch < lens[b] (clamped
+// to [1, rows_per_batch]); rows that are not live are neither read nor written.
+__device__ __forceinline__ bool rmsnorm_row_live(long long row, int rows_per_batch, const int* __restrict__ lens) {
+  const long long b = row / rows_per_batch;
+  return row - b * rows_per_batch < min(max(__ldg(lens + b), 1), rows_per_batch);
+}
+
+template <int VEC, bool OUT_BF16, bool LENS = false>
 __global__ void __launch_bounds__(256) rmsnorm_kernel(const float* __restrict__ x, long long x_rs,
                                                       long long rows, int dim, int rows_per_batch,
                                                       const float* __restrict__ gamma,
                                                       const float* __restrict__ film, long long film_bs,
-                                                      void* __restrict__ out, long long out_rs) {
+                                                      void* __restrict__ out, long long out_rs,
+                                                      const int* __restrict__ lens) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long row = static_cast<long long>(blockIdx.x) * 8 + warp;
   if (row >= rows) return;
+  if (LENS && !rmsnorm_row_live(row, rows_per_batch, lens)) return;
   const float4* xp = reinterpret_cast<const float4*>(x + row * x_rs);
   float4 v[VEC];
 #pragma unroll
@@ -84,18 +93,20 @@ __global__ void __launch_bounds__(256) rmsnorm_kernel(const float* __restrict__ 
 // each warp always has one row (dim * 4 bytes) in flight.  The one-row-per-warp kernel above leaves the memory
 // pipe idle while a warp reduces, fetches its FiLM vectors and stores, and between CTA generations: ncu showed
 // 2.9 TB/s of DRAM reads at 53 % active warps (profiles/r02g_rmsnorm_ncu.txt).
-template <int VEC, bool OUT_BF16>
+template <int VEC, bool OUT_BF16, bool LENS = false>
 __global__ void __launch_bounds__(256) rmsnorm_stream_kernel(const float* __restrict__ x, long long x_rs,
                                                              long long rows, int dim, int rows_per_batch,
                                                              const float* __restrict__ gamma,
                                                              const float* __restrict__ film, long long film_bs,
-                                                             void* __restrict__ out, long long out_rs) {
+                                                             void* __restrict__ out, long long out_rs,
+                                                             const int* __restrict__ lens) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long nwarps = static_cast<long long>(gridDim.x) * 8;
   long long row = static_cast<long long>(blockIdx.x) * 8 + warp;
   if (row >= rows) return;
   float4 cur[VEC], nxt[VEC];
-  {
+  bool live = !LENS || rmsnorm_row_live(row, rows_per_batch, lens);
+  if (live) {
     const float4* xp = reinterpret_cast<const float4*>(x + row * x_rs);
 #pragma unroll
     for (int i = 0; i < VEC; ++i) cur[i] = __ldg(xp + i * 32 + lane);
@@ -104,23 +115,25 @@ __global__ void __launch_bounds__(256) rmsnorm_stream_kernel(const float* __rest
   while (true) {
     const long long nrow = row + nwarps;
     const bool has_next = nrow < rows;
-    if (has_next) {
+    const bool next_live = has_next && (!LENS || rmsnorm_row_live(nrow, rows_per_batch, lens));
+    if (next_live) {
       const float4* xp = reinterpret_cast<const float4*>(x + nrow * x_rs);
 #pragma unroll
       for (int i = 0; i < VEC; ++i) nxt[i] = __ldg(xp + i * 32 + lane);
     }
-    rmsnorm_row<VEC, OUT_BF16>(cur, row, lane, dim, sqrt_dim, rows_per_batch, gamma, film, film_bs, out, out_rs);
+    if (live) rmsnorm_row<VEC, OUT_BF16>(cur, row, lane, dim, sqrt_dim, rows_per_batch, gamma, film, film_bs, out, out_rs);
     if (!has_next) break;
 #pragma unroll
     for (int i = 0; i < VEC; ++i) cur[i] = nxt[i];
     row = nrow;
+    live = next_live;
   }
 }
 
 template <bool OUT_BF16>
 static int launch_rmsnorm(const float* x, long long x_rs, long long rows, int dim, int rows_per_batch,
                           const float* gamma, const float* film, long long film_bs, void* out,
-                          long long out_rs, cudaStream_t stream) {
+                          long long out_rs, cudaStream_t stream, const int* lens = nullptr) {
   NS2_REQUIRE(x && out && rows > 0, "rmsnorm: NULL or empty input");
   NS2_REQUIRE(dim % 128 == 0 && dim <= 1024, "rmsnorm: dim=%d must be a multiple of 128, <= 1024", dim);
   NS2_REQUIRE(x_rs % 4 == 0 && out_rs % 4 == 0 && film_bs % 4 == 0, "rmsnorm: strides must be 16B-aligned");
@@ -129,20 +142,27 @@ static int launch_rmsnorm(const float* x, long long x_rs, long long rows, int di
   unsigned sgrid = static_cast<unsigned>(num_sms() * kRmsnormCtasPerSm);
   if (sgrid > grid / 4) sgrid = grid / 4;
   const bool stream_variant = grid >= static_cast<unsigned>(8 * num_sms());
-#define NS2_RMS_CASE(V)                                                                         \
-  case V:                                                                                       \
-    if (stream_variant)                                                                         \
-      rmsnorm_stream_kernel<V, OUT_BF16><<<sgrid, 256, 0, stream>>>(x, x_rs, rows, dim, rows_per_batch, gamma, film, \
-                                                                    film_bs, out, out_rs);      \
-    else                                                                                        \
-      rmsnorm_kernel<V, OUT_BF16><<<grid, 256, 0, stream>>>(x, x_rs, rows, dim, rows_per_batch, \
-                                                            gamma, film, film_bs, out, out_rs); \
+#define NS2_RMS_LAUNCH(V, L)                                                                                       \
+  if (stream_variant)                                                                                              \
+    rmsnorm_stream_kernel<V, OUT_BF16, L><<<sgrid, 256, 0, stream>>>(x, x_rs, rows, dim, rows_per_batch, gamma, film, \
+                                                                     film_bs, out, out_rs, lens);                  \
+  else                                                                                                             \
+    rmsnorm_kernel<V, OUT_BF16, L><<<grid, 256, 0, stream>>>(x, x_rs, rows, dim, rows_per_batch, gamma, film,        \
+                                                             film_bs, out, out_rs, lens);
+#define NS2_RMS_CASE(V)                                                                                            \
+  case V:                                                                                                          \
+    if (lens != nullptr) {                                                                                         \
+      NS2_RMS_LAUNCH(V, true)                                                                                      \
+    } else {                                                                                                       \
+      NS2_RMS_LAUNCH(V, false)                                                                                     \
+    }                                                                                                              \
     break;
   switch (dim / 128) {
     NS2_RMS_CASE(1) NS2_RMS_CASE(2) NS2_RMS_CASE(3) NS2_RMS_CASE(4) NS2_RMS_CASE(5) NS2_RMS_CASE(6)
     NS2_RMS_CASE(7) NS2_RMS_CASE(8)
   }
 #undef NS2_RMS_CASE
+#undef NS2_RMS_LAUNCH
   return launched(1);
 }
 
@@ -358,15 +378,23 @@ __global__ void __launch_bounds__(256) q_sample_kernel(const float4* __restrict_
   }
 }
 
-// per-sample mean squared error; deterministic two-level reduction (fixed grid, no atomics on floats)
+// per-sample mean squared error; deterministic two-level reduction (fixed grid, no atomics on floats).
+// With lens (ns2_mse_rows_lens) sample b covers its first lens[b] rows of row4 float4s: the same grid-stride walk over
+// those elements as a call on the unpadded sample, so the partial sums and the mean are bit-identical to it.
 constexpr int kMseBlocks = 64;
+__device__ __forceinline__ long long mse_count4(const int* __restrict__ lens, int b, long long row4, int rows,
+                                                long long per4) {
+  return lens == nullptr ? per4 : static_cast<long long>(min(max(__ldg(lens + b), 1), rows)) * row4;
+}
 __global__ void __launch_bounds__(256) mse_partial_kernel(const float4* __restrict__ pred,
                                                           const float4* __restrict__ target,
-                                                          long long per4, float* __restrict__ partial) {
+                                                          long long per4, float* __restrict__ partial,
+                                                          const int* __restrict__ lens, long long row4, int rows) {
   const int b = blockIdx.y;
   const long long base = static_cast<long long>(b) * per4;
+  const long long n4 = mse_count4(lens, b, row4, rows, per4);
   float s = 0.f;
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < per4;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n4;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const float4 p = __ldg(pred + base + i), t = __ldg(target + base + i);
     const float dx = p.x - t.x, dy = p.y - t.y, dz = p.z - t.z, dw = p.w - t.w;
@@ -383,8 +411,9 @@ __global__ void __launch_bounds__(256) mse_partial_kernel(const float4* __restri
   }
 }
 __global__ void mse_final_kernel(const float* __restrict__ partial, long long per_sample,
-                                 float* __restrict__ out) {
+                                 float* __restrict__ out, const int* __restrict__ lens, long long row4, int rows) {
   const int b = blockIdx.x;
+  if (lens != nullptr) per_sample = 4 * mse_count4(lens, b, row4, rows, per_sample / 4);
   float v = threadIdx.x < kMseBlocks ? partial[b * kMseBlocks + threadIdx.x] : 0.f;
   __shared__ float red[2];
   v = warp_sum(v);
@@ -740,10 +769,20 @@ int ns2_rmsnorm_film(const float* x, int64_t x_row_stride, int64_t rows, int32_t
                      int32_t rows_per_batch, const float* gamma, const float* film,
                      int64_t film_batch_stride, void* out_bf16, int64_t out_row_stride,
                      ns2_stream_t stream) {
+  return ns2_rmsnorm_film_lens(x, x_row_stride, rows, dim, rows_per_batch, gamma, film, film_batch_stride, out_bf16,
+                               out_row_stride, nullptr, stream);
+}
+
+int ns2_rmsnorm_film_lens(const float* x, int64_t x_row_stride, int64_t rows, int32_t dim, int32_t rows_per_batch,
+                          const float* gamma, const float* film, int64_t film_batch_stride, void* out_bf16,
+                          int64_t out_row_stride, const int32_t* lens, ns2_stream_t stream) {
   NS2_REQUIRE(rows_per_batch > 0, "rmsnorm_film: rows_per_batch must be positive");
+  NS2_REQUIRE(lens == nullptr || rows % rows_per_batch == 0,
+              "rmsnorm_film_lens: rows=%lld is not a whole number of batches of %d rows", static_cast<long long>(rows),
+              rows_per_batch);
   return launch_rmsnorm<true>(x, x_row_stride, rows, dim, rows_per_batch, gamma, film,
                               film_batch_stride, out_bf16, out_row_stride,
-                              static_cast<cudaStream_t>(stream));
+                              static_cast<cudaStream_t>(stream), lens);
 }
 
 int ns2_rmsnorm_f32(const float* x, int64_t x_row_stride, int64_t rows, int32_t dim,
@@ -851,13 +890,23 @@ int ns2_q_sample(const float* x0, const float* noise, const float* alpha, const 
 
 int ns2_mse_rows(const float* pred, const float* target, int32_t batch, int64_t per_sample,
                  float* partial, float* out, float* mean_out, ns2_stream_t stream) {
+  return ns2_mse_rows_lens(pred, target, batch, per_sample, partial, out, mean_out, per_sample, nullptr, stream);
+}
+
+int ns2_mse_rows_lens(const float* pred, const float* target, int32_t batch, int64_t per_sample, float* partial,
+                      float* out, float* mean_out, int64_t row_elems, const int32_t* lens, ns2_stream_t stream) {
   NS2_REQUIRE(pred && target && out && partial, "mse_rows: NULL pointer");
   NS2_REQUIRE(per_sample % 4 == 0 && batch > 0, "mse_rows: bad sizes");
+  NS2_REQUIRE(lens == nullptr || (row_elems > 0 && row_elems % 4 == 0 && per_sample % row_elems == 0),
+              "mse_rows_lens: row_elems=%lld must be a positive multiple of 4 dividing per_sample=%lld",
+              static_cast<long long>(row_elems), static_cast<long long>(per_sample));
+  const long long row4 = lens == nullptr ? 0 : row_elems / 4;
+  const int rows = lens == nullptr ? 0 : static_cast<int>(per_sample / row_elems);
   dim3 grid(kMseBlocks, batch);
   mse_partial_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const float4*>(pred), reinterpret_cast<const float4*>(target), per_sample / 4,
-      partial);
-  mse_final_kernel<<<batch, 64, 0, static_cast<cudaStream_t>(stream)>>>(partial, per_sample, out);
+      partial, lens, row4, rows);
+  mse_final_kernel<<<batch, 64, 0, static_cast<cudaStream_t>(stream)>>>(partial, per_sample, out, lens, row4, rows);
   if (mean_out != nullptr) batch_mean_kernel<<<1, 256, 0, static_cast<cudaStream_t>(stream)>>>(out, batch, mean_out);
   return launched(mean_out != nullptr ? 3 : 2);
 }

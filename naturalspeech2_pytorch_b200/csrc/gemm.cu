@@ -47,6 +47,10 @@ struct GemmDev {
   int film_gs;
   int act;            // BF16 / F32 epilogues: 0 = none, 1 = SiLU applied to acc + bias (ns2_gemm_args.flags & NS2_GEMM_FLAG_SILU)
   int skip_epilogue;  // measurement aid (ns2_gemm_args.flags & NS2_GEMM_FLAG_SKIP_EPILOGUE): mainloop-only timing
+  // gemm_kernel<..., true> only: per-batch row counts (a_batches <= NS2_GEMM_ROW_LENS_MAX_BATCHES values, each clamped
+  // to [1, a_rows]); the fields above keep their offsets, so the plain kernels read their parameters as before
+  const int* row_lens;
+  int batches;
 };
 
 struct TileCoord {
@@ -54,6 +58,7 @@ struct TileCoord {
 };
 
 __device__ __forceinline__ TileCoord decode_tile(const GemmDev& p, int tile) {
+  // every m-tile of every batch: tile = (g, b, m, n_tile) in row-major order, n fastest
   TileCoord t;
   const int per_group = p.tiles_m * p.tiles_n;
   t.g = tile / per_group;
@@ -62,6 +67,27 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmDev& p, int tile) {
   t.n_tile = r - m_tile * p.tiles_n;
   t.b = m_tile / p.tiles_per_batch;
   t.n0 = (m_tile - t.b * p.tiles_per_batch) * BM;
+  return t;
+}
+
+// Length-aware schedule: only the m-tiles that start before row_lens[b], numbered densely in the same (g, b, m, n_tile)
+// order, so the static round robin hands out computed tiles only and stays balanced.  pre[b] (shared memory) is the
+// number of such m-tiles in batches < b, pre[batches] their total per group.
+__device__ __forceinline__ TileCoord decode_tile_lens(const GemmDev& p, const int* pre, int tile) {
+  TileCoord t;
+  const int per_group = pre[p.batches] * p.tiles_n;
+  t.g = tile / per_group;
+  const int r = tile - t.g * per_group;
+  const int m_tile = r / p.tiles_n;
+  t.n_tile = r - m_tile * p.tiles_n;
+  int lo = 0, hi = p.batches;   // the batch b with pre[b] <= m_tile < pre[b + 1] (every batch has >= 1 m-tile)
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (pre[mid] <= m_tile) lo = mid;
+    else hi = mid;
+  }
+  t.b = lo;
+  t.n0 = (m_tile - pre[lo]) * BM;
   return t;
 }
 
@@ -278,6 +304,10 @@ struct GemmCfg {
   static constexpr int BAR_OFF = VEC_OFF + (NACC == 2 ? 4 : 1) * BN * 4;
   static constexpr int SMEM_BYTES = BAR_OFF + 256 /*barriers*/;     // 226.25 KB (WAVENET) of 227
   static_assert(SMEM_BYTES <= 232448, "over the sm_90 per-block shared-memory limit");
+  // length-aware kernels: the row counts (cp.async-staged) and their m-tile prefix sums after the barriers
+  static constexpr int LENS_OFF = SMEM_BYTES;
+  static constexpr int SMEM_BYTES_LENS = LENS_OFF + (2 * NS2_GEMM_ROW_LENS_MAX_BATCHES + 4) * 4;
+  static_assert(SMEM_BYTES_LENS <= 232448, "NS2_GEMM_ROW_LENS_MAX_BATCHES does not fit in shared memory");
 };
 
 constexpr int CONSUMER_BAR = 1;   // named barrier over the 256 consumer threads (warpgroup_bar uses 8 and 9)
@@ -288,7 +318,11 @@ __device__ __forceinline__ void wgmma_tile_k16(float (&d)[BN / 2], uint64_t da, 
   else wgmma_bf16_ss_n128<0, 0>(d, da, db, 1);
 }
 
-template <int BN, int NACC, int EPI>
+// gemm_kernel<BN, NACC, EPI, true>: the length-aware variant of ns2_gemm_row_lens.  Before the roles split, the first
+// a_batches threads copy row_lens into shared memory by cp.async (the kernels read no global memory through the
+// register path, see tests/test_gemm_epilogue_loads_cpu.py) and thread 0 forms the m-tile prefix sums; every role then
+// walks the same compacted tile list (decode_tile_lens).  A tile is computed and stored exactly as by the plain kernel.
+template <int BN, int NACC, int EPI, bool LENS = false>
 __global__ void __launch_bounds__(GemmCfg<BN, NACC>::THREADS, 1) gemm_kernel(const __grid_constant__ GemmDev p) {
   using Cfg = GemmCfg<BN, NACC>;
   static_assert(Cfg::VEC_OFF / 4 + tile_vec_floats<BN, EPI>() <= Cfg::BAR_OFF / 4, "vector area too small");
@@ -311,15 +345,37 @@ __global__ void __launch_bounds__(GemmCfg<BN, NACC>::THREADS, 1) gemm_kernel(con
     }
     fence_barrier_init();
   }
-  __syncthreads();
+  int num_tiles = p.num_tiles;
+  const int* pre = nullptr;
+  if constexpr (LENS) {
+    int* lens = reinterpret_cast<int*>(smem + Cfg::LENS_OFF);
+    int* pre_w = lens + NS2_GEMM_ROW_LENS_MAX_BATCHES;
+    if (threadIdx.x < p.batches) cp_async_4(smem_u32(lens + threadIdx.x), p.row_lens + threadIdx.x);
+    cp_async_wait_all();
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int acc = 0;
+      for (int b = 0; b < p.batches; ++b) {
+        pre_w[b] = acc;
+        acc += (min(max(lens[b], 1), p.a_rows) + BM - 1) / BM;
+      }
+      pre_w[p.batches] = acc;
+    }
+    __syncthreads();
+    pre = pre_w;
+    num_tiles = pre[p.batches] * p.tiles_n * p.groups;
+  } else {
+    __syncthreads();
+  }
+#define NS2_DECODE_TILE(tile) (LENS ? decode_tile_lens(p, pre, tile) : decode_tile(p, tile))
 
   if (warp < 4) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (warp == 0) {
       // =============================== TMA producer (converged, one elected lane issues) ===============================
       uint32_t it = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        const TileCoord t = decode_tile(p, tile);
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const TileCoord t = NS2_DECODE_TILE(tile);
         const int dil = p.dil[t.g];
         for (int s = 0; s < p.num_segs; ++s) {
           const ns2_gemm_seg sg = p.segs[s];
@@ -356,8 +412,8 @@ __global__ void __launch_bounds__(GemmCfg<BN, NACC>::THREADS, 1) gemm_kernel(con
     uint32_t nbox = 0;
     float acc[NACC][BN / 2];
     uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      const TileCoord t = decode_tile(p, tile);
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const TileCoord t = NS2_DECODE_TILE(tile);
       if (tile_vecs) {
         named_bar(CONSUMER_BAR, 256);   // both warpgroups' epilogues of the previous tile are done reading vec
         load_tile_vectors<BN, EPI>(p, t, smem_u32(vec), threadIdx.x - 128);
@@ -404,6 +460,7 @@ __global__ void __launch_bounds__(GemmCfg<BN, NACC>::THREADS, 1) gemm_kernel(con
     }
     if (leader) tma_store_wait_all();   // shared memory must outlive the reads of the last stores
   }
+#undef NS2_DECODE_TILE
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -412,19 +469,31 @@ __global__ void __launch_bounds__(GemmCfg<BN, NACC>::THREADS, 1) gemm_kernel(con
 template <int BN, int NACC, int EPI>
 static int launch_gemm(const GemmDev& dev, cudaStream_t stream) {
   using Cfg = GemmCfg<BN, NACC>;
-  auto kern = gemm_kernel<BN, NACC, EPI>;
-  NS2_CUDA_CHECK(set_max_smem_once(kern, Cfg::SMEM_BYTES));
+  // with row lengths the grid is sized for every tile: the CTAs past the compacted count exit at once
   const int grid = dev.num_tiles < num_sms() ? dev.num_tiles : num_sms();
-  kern<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(dev);
+  if (dev.row_lens != nullptr) {
+    auto kern = gemm_kernel<BN, NACC, EPI, true>;
+    NS2_CUDA_CHECK(set_max_smem_once(kern, Cfg::SMEM_BYTES_LENS));
+    kern<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES_LENS, stream>>>(dev);
+  } else {
+    auto kern = gemm_kernel<BN, NACC, EPI>;
+    NS2_CUDA_CHECK(set_max_smem_once(kern, Cfg::SMEM_BYTES));
+    kern<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(dev);
+  }
   return launched(1);
 }
 
 }  // namespace ns2
 
-extern "C" int ns2_gemm(const ns2_gemm_args* a, ns2_stream_t stream_) {
+extern "C" int ns2_gemm(const ns2_gemm_args* a, ns2_stream_t stream) { return ns2_gemm_row_lens(a, nullptr, stream); }
+
+extern "C" int ns2_gemm_row_lens(const ns2_gemm_args* a, const int32_t* row_lens, ns2_stream_t stream_) {
   using namespace ns2;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   NS2_REQUIRE(a != nullptr, "ns2_gemm: args is NULL");
+  NS2_REQUIRE(row_lens == nullptr || (a->a_batches >= 1 && a->a_batches <= NS2_GEMM_ROW_LENS_MAX_BATCHES),
+              "ns2_gemm_row_lens: a_batches=%d, row lengths take 1 to %d batches", a->a_batches,
+              NS2_GEMM_ROW_LENS_MAX_BATCHES);
   NS2_REQUIRE(a->A && a->B && a->out, "ns2_gemm: A, B and out must be non-NULL");
   NS2_REQUIRE(a->groups >= 1 && a->groups <= NS2_GEMM_MAX_GROUPS, "ns2_gemm: groups=%d out of range",
               a->groups);
@@ -532,6 +601,8 @@ extern "C" int ns2_gemm(const ns2_gemm_args* a, ns2_stream_t stream_) {
   NS2_REQUIRE(dev.act == 0 || a->epilogue == NS2_EPI_BF16 || a->epilogue == NS2_EPI_F32,
               "ns2_gemm: NS2_GEMM_FLAG_SILU only applies to the BF16 / F32 epilogues");
   dev.skip_epilogue = (a->flags & NS2_GEMM_FLAG_SKIP_EPILOGUE) ? 1 : 0;
+  dev.row_lens = row_lens;
+  dev.batches = a->a_batches;
 
   switch (a->epilogue) {
     case NS2_EPI_BF16:

@@ -142,6 +142,10 @@ __device__ __forceinline__ void cp_async_16(uint32_t dst_smem, const void* src) 
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst_smem), "l"(reinterpret_cast<uint64_t>(src))
                : "memory");
 }
+// 4-byte global -> shared copy (LDGSTS through L1): small per-launch tables such as per-batch lengths
+__device__ __forceinline__ void cp_async_4(uint32_t dst_smem, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst_smem), "l"(src) : "memory");
+}
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }

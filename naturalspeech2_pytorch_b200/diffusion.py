@@ -125,17 +125,21 @@ class NaturalSpeech2(nn.Module):
         times = t_all[:-1, None].expand(-1, batch).contiguous()
         return times, coef[:, :, None].expand(-1, -1, batch).contiguous()
 
-    def _sampler_entry(self, shape, conditioning, cond_scale, device):
+    def _sampler_entry(self, shape, conditioning, cond_scale, device, lens=None):
         """One captured CUDA graph = one whole sampling step: denoiser forward(s), guidance combine, DDIM update of the
-        static latent buffer.  Keyed on shapes only; conditioning is copied into static buffers."""
+        static latent buffer.  Keyed on shapes (and on whether latent lengths are given) only; conditioning and the
+        lengths are copied into static buffers."""
         guided = self.conditional and cond_scale != 1.
         cond_sig = None
         if conditioning is not None:
             cond_sig = tuple(tuple(v.shape) for v in conditioning.values() if torch.is_tensor(v))
-        key = (tuple(shape), cond_sig, float(cond_scale) if guided else None, self.objective, str(device))
+        key = (tuple(shape), cond_sig, float(cond_scale) if guided else None, self.objective, lens is not None,
+               str(device))
         entry = self._sampler_graphs.get(key)
         if entry is not None and entry["packed"] is self.model.packed():
             self._sampler_graphs.move_to_end(key)
+            if lens is not None:
+                entry["lens"].copy_(lens)
             if conditioning is not None:
                 for k, v in conditioning.items():
                     if torch.is_tensor(v):
@@ -155,11 +159,12 @@ class NaturalSpeech2(nn.Module):
             static_cond = type(conditioning)({k: (v.clone() if torch.is_tensor(v) else v)
                                               for k, v in conditioning.items()})
         p_cond = 0. if self.conditional else None
+        static_lens = None if lens is None else lens.clone()
 
         def step():
-            model._forward_impl(x, ts, None, None, None, p_cond, static_cond, v0)
+            model._forward_impl(x, ts, None, None, None, p_cond, static_cond, v0, lengths=static_lens)
             if guided:   # classifier-free guidance (ns2.py:914-927): conditional + null forward, lerp
-                model._forward_impl(x, ts, None, None, None, 1., static_cond, v1)
+                model._forward_impl(x, ts, None, None, None, 1., static_cond, v1, lengths=static_lens)
                 ops.cfg_combine(v0, v1, cond_scale, v0)
             ops.ddim_step(x, v0, coef[0], coef[1], coef[2], coef[3], objective=self.objective)
 
@@ -175,17 +180,21 @@ class NaturalSpeech2(nn.Module):
         # the entry owns every buffer the graph reads or writes: v0 / v1 are written by each replay, and a buffer freed
         # here would go back to the caching allocator while the graph still writes the prediction into it
         entry = {"graph": graph, "x": x, "ts": ts, "coef": coef, "v": (v0, v1), "cond": static_cond,
-                 "packed": model.packed()}
+                 "lens": static_lens, "packed": model.packed()}
         self._sampler_graphs[key] = entry
         return entry
 
     @torch.no_grad()
     def ddim_sample(self, shape, prompt=None, time_difference=None, cond_scale=1., cond=None, *, noise=None,
-                    prompt_lens=None, cond_lens=None):
+                    prompt_lens=None, cond_lens=None, latent_lens=None):
         """ns2.py:1379-1431.  `noise` (optional) fixes the initial latent instead of drawing it.
         (`time_difference` only shifts a value the reference never reads again, ns2.py:1404-1406.)
-        prompt_lens / cond_lens: per-sample lengths of the prompt and the condition (Model.precompute_conditioning)."""
+        prompt_lens / cond_lens: per-sample lengths of the prompt and the condition (Model.precompute_conditioning).
+        latent_lens: per-sample latent lengths (`Model.forward`'s `lengths`); the result is zero past them."""
         batch, device = shape[0], self.device
+        lens = None
+        if latent_lens is not None:
+            lens = self.model._latent_lens(latent_lens, torch.empty(shape[:2], device=device))
         # a dense, row-major copy: the eager loop updates it in place with ops.ddim_step, which reads flat arrays
         audio = torch.randn(shape, device=device) if noise is None else \
             noise.to(device).float().clone(memory_format=torch.contiguous_format)
@@ -197,22 +206,38 @@ class NaturalSpeech2(nn.Module):
                                                               cond_lens=cond_lens)
         times_tab, coef_tab = self._schedule_tables(batch, device)
         if self.cuda_graphs and audio.is_cuda and self.model._prof is None:
-            entry = self._sampler_entry(shape, conditioning, cond_scale, device)
+            entry = self._sampler_entry(shape, conditioning, cond_scale, device, lens)
             entry["x"].copy_(audio)
             for i in range(self.timesteps):
                 entry["ts"].copy_(times_tab[i])
                 entry["coef"].copy_(coef_tab[i])
                 entry["graph"].replay()
-            return entry["x"].clone()
+            audio = entry["x"].clone()
+            return audio if lens is None else ops.mask_rows(audio, lens)
+        extra = {} if lens is None else {"lengths": lens}
         for i in range(self.timesteps):
             if self.conditional:
                 v = self.model.forward_with_cond_scale(audio, times_tab[i], cond_scale=cond_scale,
-                                                       _conditioning=conditioning)
+                                                       _conditioning=conditioning, **extra)
             else:
-                v = self.model.forward_with_cond_scale(audio, times_tab[i], cond_scale=cond_scale)
+                v = self.model.forward_with_cond_scale(audio, times_tab[i], cond_scale=cond_scale, **extra)
             c = coef_tab[i]
             ops.ddim_step(audio, v, c[0], c[1], c[2], c[3], objective=self.objective)
-        return audio
+        return audio if lens is None else ops.mask_rows(audio, lens)
+
+    def _check_latent_lens_training(self, audio, codes):
+        """Refuse, before any launch, what `forward(latent_lens=)` does not support."""
+        if audio.ndim == 2:
+            raise ValueError("latent_lens needs encoded latents (B, N, dim): the codec's encoder takes no lengths")
+        if self.rvq_cross_entropy_loss_weight != 0 and codes is not None:
+            raise NotImplementedError("latent_lens with the RVQ cross-entropy term is not supported (its reduction over "
+                                      "frames has no lengths)")
+        cn = self.conditioner
+        if cn is not None and getattr(cn, "train_duration_pitch", False):
+            raise NotImplementedError("latent_lens with train_duration_pitch is not supported")
+        if cn is not None and isinstance(cn, torch.nn.Module) and cn.training and any(
+                getattr(m, "train_dropout", False) for m in cn.modules()):
+            raise NotImplementedError("latent_lens with training dropout (train_dropout) is not supported")
 
     def process_prompt(self, prompt=None):
         """ns2.py:1433-1447."""
@@ -227,13 +252,22 @@ class NaturalSpeech2(nn.Module):
 
     @torch.no_grad()
     def sample(self, *, length, prompt=None, batch_size=1, cond_scale=1., text=None, text_lens=None,
-               prompt_enc=None, cond=None, noise=None, prompt_lens=None, phoneme_lens=None, cond_lens=None):
+               prompt_enc=None, cond=None, noise=None, prompt_lens=None, phoneme_lens=None, cond_lens=None,
+               latent_lens=None):
         """ns2.py:1457-1501.  Conditional models need (`prompt_enc`, `cond`) or a `conditioner`.
         `text_lens` is accepted and ignored, as in the reference.  A batch of prompts and texts of different lengths,
         padded at their ends, is sampled as if each sample ran alone with `prompt_lens` (prompt latent frames) and
         `phoneme_lens` (phonemes), given to the conditioner, whose condition lengths then follow; with precomputed
         `prompt_enc=` / `cond=` pass `prompt_lens` and `cond_lens` (condition frames) instead.  With lengths the
-        prompt must be encoded latents (B, Np, dim): a raw-audio prompt would be curtailed by the batch's length."""
+        prompt must be encoded latents (B, Np, dim): a raw-audio prompt would be curtailed by the batch's length.
+
+        latent_lens (B,): sample b is `latent_lens[b]` latent frames long (`length` stays the padded length, at most 64
+        samples): each returned latent equals sampling that sample alone with length=latent_lens[b] and the first
+        latent_lens[b] frames of its noise, bit for bit, and is zero past it.  The denoiser skips the 128-frame tiles
+        wholly past each length.  With a codec, each waveform is zero past latent_lens[b] * hop samples; the SEANet
+        decoder is causal, so its prefix is the sample's waveform decoded alone provided latent_lens[b] >= 7 frames
+        (shorter inputs fall under Encodec's short-input padding rule when decoded alone, which a batch cannot
+        reproduce)."""
         if self.use_ddim is False:
             raise NotImplementedError("ddpm_sample is dead code in the reference (NameError: expm1, SURVEY T8)")
         ragged = prompt_lens is not None or phoneme_lens is not None or cond_lens is not None
@@ -261,12 +295,22 @@ class NaturalSpeech2(nn.Module):
             elif phoneme_lens is not None:
                 raise ValueError("phoneme_lens goes to the conditioner; with prompt_enc= / cond= pass cond_lens")
             batch_size = prompt_enc.shape[0]
+        if latent_lens is not None and prompt is not None and prompt.ndim == 2:
+            raise ValueError("latent_lens needs an encoded prompt (B, Np, dim) or prompt_enc=: a raw-audio prompt is "
+                             "curtailed from the left by the batch's length")
         audio = self.ddim_sample((batch_size, length, self.dim), prompt=prompt_enc, cond=cond,
-                                 cond_scale=cond_scale, noise=noise, prompt_lens=prompt_lens, cond_lens=cond_lens)
+                                 cond_scale=cond_scale, noise=noise, prompt_lens=prompt_lens, cond_lens=cond_lens,
+                                 latent_lens=latent_lens)
         if _exists(self.codec):
             audio = self.codec.decode(audio)
             if audio.ndim == 3 and audio.shape[1] == 1:
                 audio = audio[:, 0]
+            if latent_lens is not None and audio.ndim == 2:   # a waveform: zeros past each sample's frames
+                lens = self.model._latent_lens(latent_lens, torch.empty(batch_size, length, device=audio.device))
+                hop = audio.shape[-1] // length
+                if hop * length != audio.shape[-1]:
+                    raise ValueError(f"latent_lens: the codec returned {audio.shape[-1]} samples for {length} frames")
+                audio = ops.mask_rows(audio.contiguous().view(batch_size, length, hop), lens).view(batch_size, -1)
         return audio
 
     # ------------------------------------------------------------------------------------------
@@ -274,7 +318,7 @@ class NaturalSpeech2(nn.Module):
     # ------------------------------------------------------------------------------------------
     def forward(self, audio, text=None, text_lens=None, mel=None, mel_lens=None, codes=None, prompt=None,
                 pitch=None, *args, prompt_enc=None, cond=None, times=None, noise=None, duration=None, prompt_lens=None,
-                phoneme_lens=None, **kwargs):
+                phoneme_lens=None, latent_lens=None, **kwargs):
         """ns2.py:1503-1684 -> scalar diffusion loss (the only term the reference returns, SURVEY T11).
         Extra keyword-only arguments: `prompt_enc`/`cond` (precomputed conditioning), `times`/`noise`
         (inject the two random draws of ns2.py:1621,1625 — used by the parity tests) and `duration` (per-phoneme frame
@@ -286,9 +330,17 @@ class NaturalSpeech2(nn.Module):
         `prompt_lens` (prompt latent frames) and `phoneme_lens` (phonemes), given to the conditioner, and prompt_lens to
         the model; with precomputed `prompt_enc=` / `cond=` only prompt_lens (to the model).  The latents and pitch share
         one length.  Each sample's MSE row is then that of the sample alone; the loss, as in the reference, is
-        mean(mse) * mean(weight) over the batch (ns2.py:1651-1666), not the mean of the per-sample losses."""
+        mean(mse) * mean(weight) over the batch (ns2.py:1651-1666), not the mean of the per-sample losses.
+
+        latent_lens (B,): sample b's latents are audio[b, :latent_lens[b]] (encoded latents, padded at the end, at most
+        64 samples); its MSE row is the mean over those frames only, bit-identical to the sample alone, and its
+        gradients are those of the sample alone (rows past the length add exact zeros).  Combines with prompt_lens /
+        phoneme_lens.  Not with raw audio (the codec encoder takes no lengths), the RVQ cross-entropy term (its frame
+        reduction has no lengths), train_duration_pitch or training dropout."""
         is_raw_audio = audio.ndim == 2
         aux_loss = None
+        if latent_lens is not None:
+            self._check_latent_lens_training(audio, codes)
         ragged = prompt_lens is not None or phoneme_lens is not None
         if ragged and not self.conditional:
             raise ValueError("prompt_lens / phoneme_lens apply to conditional models")
@@ -331,12 +383,16 @@ class NaturalSpeech2(nn.Module):
         target = torch.empty_like(audio)
         ops.q_sample(audio, noise, alpha, sigma, noised, target, objective=self.objective)  # ns2.py:1631-1644
         lens = {} if prompt_lens is None else {"prompt_lens": prompt_lens}
+        llens = None
+        if latent_lens is not None:
+            llens = self.model._latent_lens(latent_lens, audio)
+            lens["lengths"] = llens
         pred = self.model(noised, times, prompt=prompt_enc, cond=cond, **lens)  # ns2.py:1635
         if pred.requires_grad:
             from .training import MseRowsFunction
-            loss = MseRowsFunction.apply(pred, target)                  # ns2.py:1646-1647, with a backward kernel
+            loss = MseRowsFunction.apply(pred, target, *(() if llens is None else (llens,)))   # ns2.py:1646-1647
         else:
-            loss = ops.mse_rows(pred, target, torch.empty(batch, device=device))
+            loss = ops.mse_rows(pred, target, torch.empty(batch, device=device), lens=llens)
         # min-SNR weight on (B,)-sized tensors, with the reference's exact broadcasting (ns2.py:1651-1666):
         # loss is (B,), loss_weight is (B,1,1) -> the product is (B,1,B) before .mean()
         a3, s3 = alpha.view(-1, 1, 1), sigma.view(-1, 1, 1)

@@ -593,7 +593,7 @@ class Model(_PackedCache):
 
     def forward(self, x, times, prompt=None, prompt_mask=None, cond=None, cond_drop_prob=None, *,
                 out: Optional[torch.Tensor] = None, _conditioning: Optional[dict] = None, prompt_lens=None,
-                cond_lens=None):
+                cond_lens=None, lengths=None):
         """x (B, N, dim) fp32, times (B,) in [0, 1] -> (B, N, dim) fp32   (ns2.py:929-1000).
 
         Returns a fresh tensor, like the reference; pass `out=` (contiguous fp32 (B, N, dim)) to have the prediction
@@ -608,7 +608,18 @@ class Model(_PackedCache):
         prompt_lens / cond_lens (B,): per-sample prompt lengths and condition lengths of a batch padded at the end, see
         `precompute_conditioning`; cached conditioning carries its own.  Training takes prompt_lens (each sample's
         prediction and gradients are those of the sample alone, d prompt is zero past its length); cond_lens is for
-        inference only: in training the condition spans the latents' frames, zero past each sample's durations."""
+        inference only: in training the condition spans the latents' frames, zero past each sample's durations.
+
+        lengths (B,): per-sample latent lengths of a batch padded at the end, in [1, N], at most 64 samples.  Sample b's
+        prediction rows [0, lengths[b]) are then bit-identical to the call on x[b:b+1, :lengths[b]] alone, rows past it
+        are exact zeros, and nothing in x's (or the condition's) padded rows is read.  In inference the GEMMs, the
+        attention and the norms skip the 128-row tiles that lie wholly in a sample's padding.  In training every row is
+        computed (the backward reads every saved activation) with the self-attention's keys limited to each sample's
+        length; the gradient rows past a length are exact zeros and add nothing to any parameter gradient, so
+        each sample's gradients are those of the sample alone."""
+        lens = None
+        if lengths is not None:
+            lens = self._latent_lens(lengths, x)
         ragged = prompt_lens is not None or cond_lens is not None
         if ragged and _conditioning is not None:
             raise ValueError("prompt_lens / cond_lens go to precompute_conditioning when the conditioning is cached")
@@ -620,15 +631,29 @@ class Model(_PackedCache):
             if prompt_mask is not None or out is not None or _conditioning is not None or cond_lens is not None:
                 raise NotImplementedError("training mode takes (x, times[, prompt, cond, prompt_lens]): no out=, "
                                           "prompt_mask, cond_lens or cached conditioning")
-            return DenoiserFunction.apply(self, x, times, prompt, cond, cond_drop_prob, prompt_lens, *self.parameters())
+            return DenoiserFunction.apply(self, x, times, prompt, cond, cond_drop_prob, prompt_lens, lens,
+                                          *self.parameters())
         if ragged:
             with torch.no_grad():   # eager: the prompt work is per call anyway
                 return self._forward_impl(x, times, prompt, prompt_mask, cond, cond_drop_prob, None, out,
-                                          prompt_lens=prompt_lens, cond_lens=cond_lens)
+                                          prompt_lens=prompt_lens, cond_lens=cond_lens, lengths=lens)
         with torch.no_grad():
-            return self._forward_nograd(x, times, prompt, prompt_mask, cond, cond_drop_prob, out, _conditioning)
+            return self._forward_nograd(x, times, prompt, prompt_mask, cond, cond_drop_prob, out, _conditioning, lens)
 
-    def _forward_nograd(self, x, times, prompt, prompt_mask, cond, cond_drop_prob, out, _conditioning):
+    def _latent_lens(self, lengths, x: torch.Tensor) -> torch.Tensor:
+        """`lengths` as the validated int32 CUDA (B,) tensor the kernels read.  A tensor that already is one is used as
+        it is (its range is read once per tensor version), so a sampling loop passes the same lengths every step
+        without a host round trip."""
+        B, N = x.shape[0], x.shape[1]
+        if B > ops._lib.NS2_GEMM_ROW_LENS_MAX_BATCHES:
+            raise ValueError(f"lengths: at most {ops._lib.NS2_GEMM_ROW_LENS_MAX_BATCHES} samples per call, got {B}")
+        if (isinstance(lengths, torch.Tensor) and lengths.dtype == torch.int32 and lengths.is_cuda
+                and lengths.is_contiguous() and tuple(lengths.shape) == (B,) and lengths.device == x.device):
+            ops._check_lens(lengths, 1, N, "lengths")
+            return lengths
+        return ops.lengths(lengths, B, N, device=x.device, name="lengths")
+
+    def _forward_nograd(self, x, times, prompt, prompt_mask, cond, cond_drop_prob, out, _conditioning, lens=None):
         if out is not None:
             if not (out.is_cuda and out.dtype == torch.float32 and out.is_contiguous()
                     and tuple(out.shape) == tuple(x.shape)):
@@ -637,17 +662,18 @@ class Model(_PackedCache):
         if (self.use_cuda_graphs and self._prof is None and prompt_mask is None and x.is_cuda
                 and not torch.cuda.is_current_stream_capturing()
                 and (not self.condition_on_prompt or (_conditioning is not None and p_eff in (0, 0., 1, 1.)))):
-            return self._forward_graphed(x, times, p_eff, _conditioning, out)
-        return self._forward_impl(x, times, prompt, prompt_mask, cond, cond_drop_prob, _conditioning, out)
+            return self._forward_graphed(x, times, p_eff, _conditioning, out, lens)
+        return self._forward_impl(x, times, prompt, prompt_mask, cond, cond_drop_prob, _conditioning, out, lengths=lens)
 
-    def _forward_graphed(self, x, times, p_eff, conditioning, out):
+    def _forward_graphed(self, x, times, p_eff, conditioning, out, lens=None):
         B, N, _ = x.shape
         self.packed()  # a parameter-version change invalidates the packed weights AND clears self._graphs
         cond_sig = None
         if conditioning is not None:
             cond_sig = tuple(tuple(conditioning[k].shape) for k in ("prompt_cond", "tokens", "cond_proj"))
             cond_sig += (conditioning.get("cond_lens") is not None,)   # a different cond_inject launch
-        key = (B, N, float(p_eff), cond_sig, str(x.device))
+        # lengths live in a static device buffer: one graph serves every set of lengths of a shape
+        key = (B, N, float(p_eff), cond_sig, lens is not None, str(x.device))
         entry = self._graphs.get(key)
         if entry is None:
             while len(self._graphs) >= 2 * self.max_cached_shapes:
@@ -655,6 +681,7 @@ class Model(_PackedCache):
             xs = torch.empty(B, N, self.dim, device=x.device, dtype=torch.float32)
             ts = torch.empty(B, device=x.device, dtype=torch.float32)
             static_out = torch.empty(B, N, self.dim, device=x.device, dtype=torch.float32)
+            static_lens = None if lens is None else lens.clone()
             static_cond = None
             if conditioning is not None:   # static copies: the graph must not pin (or depend on) the caller's tensors
                 static_cond = Conditioning({k: (v.clone() if torch.is_tensor(v) else v) for k, v in conditioning.items()})
@@ -663,13 +690,13 @@ class Model(_PackedCache):
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):   # warm-up outside capture: workspaces, packing, lazy CUDA init
-                self._forward_impl(xs, ts, None, None, None, p_eff, static_cond, static_out)
+                self._forward_impl(xs, ts, None, None, None, p_eff, static_cond, static_out, lengths=static_lens)
             torch.cuda.current_stream().wait_stream(side)
             graph = torch.cuda.CUDAGraph()
             # thread_local: other threads (e.g. the NCCL watchdog) may touch CUDA while this thread captures
             with torch.cuda.graph(graph, capture_error_mode="thread_local"):
-                self._forward_impl(xs, ts, None, None, None, p_eff, static_cond, static_out)
-            entry = {"graph": graph, "xs": xs, "ts": ts, "out": static_out, "cond": static_cond,
+                self._forward_impl(xs, ts, None, None, None, p_eff, static_cond, static_out, lengths=static_lens)
+            entry = {"graph": graph, "xs": xs, "ts": ts, "out": static_out, "cond": static_cond, "lens": static_lens,
                      "cond_ref": weakref.ref(conditioning) if isinstance(conditioning, Conditioning) else None}
             self._graphs[key] = entry
         else:
@@ -681,6 +708,8 @@ class Model(_PackedCache):
                 entry["cond_ref"] = weakref.ref(conditioning) if isinstance(conditioning, Conditioning) else None
         entry["xs"].copy_(x)
         entry["ts"].copy_(times)
+        if lens is not None:
+            entry["lens"].copy_(lens)
         entry["graph"].replay()
         if out is None:
             return entry["out"].clone()
@@ -690,11 +719,22 @@ class Model(_PackedCache):
     @torch.no_grad()
     def _forward_impl(self, x, times, prompt=None, prompt_mask=None, cond=None, cond_drop_prob=None,
                       _conditioning: Optional[dict] = None, out: Optional[torch.Tensor] = None,
-                      saved: Optional[dict] = None, prompt_lens=None, cond_lens=None):
+                      saved: Optional[dict] = None, prompt_lens=None, cond_lens=None, lengths=None):
         """The denoiser's forward.  Without `saved` every intermediate lives in the per-shape workspace, so the call can
         be captured in a CUDA graph.  With `saved` (a dict; the training forward of `training.DenoiserFunction`) the
         workspace is not touched: each activation `training.train_backward` reads goes to a fresh tensor recorded
-        there, together with the residual stream before each branch and the attention log-sum-exps."""
+        there, together with the residual stream before each branch and the attention log-sum-exps.
+
+        lengths: validated int32 CUDA (B,) latent lengths (see `forward`).  The input rows past them (x and condition)
+        are zeroed on entry, the self-attention takes them as key lengths, and the prediction's padded rows are zeroed
+        at the end.  Without `saved`, every GEMM over latent rows and every norm also skips the 128-row tiles (norm:
+        rows) wholly past a sample's length, and both attentions take them as query lengths.  With `saved` every row is
+        computed, so every saved activation is finite.  The workspace rows of the
+        skipped tiles keep whatever an earlier call left there.  No valid row reads them: the causal convs read only
+        earlier rows, the other GEMMs and the norms are per row, and the self-attention never loads a key tile past a
+        sample's length.  Rows past a length inside a computed tile are computed from the zeroed input and rows of the
+        same computed tiles (the norm's skipped rows keep this call's skip-conv output), so the keys the attention
+        masks there are finite."""
         if prompt_mask is not None:
             raise NotImplementedError("prompt_mask is unsupported (the reference itself fails on it, SURVEY T9)")
         if not x.is_cuda:
@@ -706,6 +746,7 @@ class Model(_PackedCache):
         G, inner, H = self.wavenet_layers, self.inner, self.heads
         Dp = _round_up(self.ff_inner, 128)
         keep = saved is not None
+        lens = None if keep else lengths   # tile skipping: inference only
         if keep:
             buf = lambda name, *s, dt=torch.bfloat16: torch.empty(*s, device=dev, dtype=dt)  # noqa: E731
         else:
@@ -753,8 +794,10 @@ class Model(_PackedCache):
                              cond_lens=_conditioning.get("cond_lens"))
         else:
             x_bf = self._run("cast", ops.cast_bf16, x.float().contiguous(), buf("x_bf", B, N, D))
+        if lengths is not None:   # the padded rows of x + condition: zeros, whatever the caller's padding holds
+            self._run("mask", ops.mask_rows, x_bf, lengths)
         h0 = self._run("wn_init", ops.gemm, x_bf, P["wn_init_w"], buf("h", B, N, D), n=D, epilogue=ops.EPI_BF16,
-                       bias=P["wn_init_b"], segs=ops.conv3_segs(D))
+                       bias=P["wn_init_b"], segs=ops.conv3_segs(D), row_lens=lens)
         segs = ops.conv3_segs(D) + [(0, 3 * D, D, 0, 1)]
         dil = [2 ** i for i in range(G)]
         src, stack_out = h0, []
@@ -763,13 +806,13 @@ class Model(_PackedCache):
             self._run("wn_stack", ops.gemm, src, P[f"wn{s}_w"], dst, n=D, epilogue=ops.EPI_WAVENET, bias=P[f"wn{s}_b"],
                      bias1_off=G * D, segs=segs, film=film[:, s * G * 2 * D:], film_group_stride=2 * D,
                      groups=G, a_group_col_stride=0 if s == 0 else D, b_group_row_stride=D,
-                     out_group_col_stride=D, dil=dil)
+                     out_group_col_stride=D, dil=dil, row_lens=lens)
             stack_out.append(dst)
             src = dst
         skip = self._run("wn_skip", ops.gemm, src, P["wn_skip_w"], buf("h", B, N, D), n=D, epilogue=ops.EPI_BF16,
-                         bias=P["wn_skip_b"])
+                         bias=P["wn_skip_b"], row_lens=lens)
         xr = self._run("wn_final", ops.gemm, skip, P["wn_final_w"], buf("x_res", B, N, D, dt=torch.float32), n=D,
-                       epilogue=ops.EPI_F32, bias=P["wn_final_b"])
+                       epilogue=ops.EPI_F32, bias=P["wn_final_b"], row_lens=lens)
         if keep:
             saved.update(B=B, N=N, times=times, t=t, film=film, x_bf=x_bf, h0=h0, stack_out=stack_out, skip=skip)
 
@@ -785,38 +828,46 @@ class Model(_PackedCache):
         for l in range(self.depth):
             fo = self._film_tr_off + l * npl * 2 * D
             L = {"x_in": xr.clone()} if keep else {}
-            L["h1"] = self._run("norm", ops.rmsnorm_film, xr, buf("h", B, N, D), film=film[:, fo:fo + 2 * D])
+            L["h1"] = self._run("norm", ops.rmsnorm_film, xr, buf("h", B, N, D), film=film[:, fo:fo + 2 * D], lens=lens)
             qkv = L["qkv"] = self._run("qkv", ops.gemm, L["h1"], P[f"l{l}_qkv"], buf("qkv", B, N, 3 * inner),
-                                       n=3 * inner, epilogue=ops.EPI_BF16)
+                                       n=3 * inner, epilogue=ops.EPI_BF16, row_lens=lens)
             L["lse"] = lse()
             L["ao"] = self._run("attn", ops.attention, qkv[:, :, :inner], qkv[:, :, inner:2 * inner],
-                                qkv[:, :, 2 * inner:], buf("attn_o", B, N, inner), heads=H, lse=L["lse"])
-            self._run("attn_out", ops.gemm, L["ao"], P[f"l{l}_o"], xr, n=D, epilogue=ops.EPI_F32, resid=xr)
+                                qkv[:, :, 2 * inner:], buf("attn_o", B, N, inner), heads=H, lse=L["lse"],
+                                kv_lens=lengths, q_lens=lens)
+            self._run("attn_out", ops.gemm, L["ao"], P[f"l{l}_o"], xr, n=D, epilogue=ops.EPI_F32, resid=xr,
+                      row_lens=lens)
             if c_tokens is not None:   # cross attention over the perceiver latents (ns2.py:800-803)
                 fo2 = fo + 2 * D
                 if keep:
                     L["x_c"] = xr.clone()
-                L["h_x"] = self._run("norm", ops.rmsnorm_film, xr, buf("h", B, N, D), film=film[:, fo2:fo2 + 2 * D])
+                L["h_x"] = self._run("norm", ops.rmsnorm_film, xr, buf("h", B, N, D), film=film[:, fo2:fo2 + 2 * D],
+                                     lens=lens)
                 L["xq"] = self._run("x_q", ops.gemm, L["h_x"], P[f"l{l}_xq"], buf("xq", B, N, inner), n=inner,
-                                    epilogue=ops.EPI_BF16)
+                                    epilogue=ops.EPI_BF16, row_lens=lens)
                 kv = xkv[:, :, l * 2 * inner:(l + 1) * 2 * inner]
                 L["lse2"] = lse()
                 L["ao2"] = self._run("x_attn", ops.attention, L["xq"], kv[:, :, :inner], kv[:, :, inner:],
-                                     buf("attn_o", B, N, inner), heads=H, lse=L["lse2"])
-                self._run("x_out", ops.gemm, L["ao2"], P[f"l{l}_xo"], xr, n=D, epilogue=ops.EPI_F32, resid=xr)
+                                     buf("attn_o", B, N, inner), heads=H, lse=L["lse2"], q_lens=lens)
+                self._run("x_out", ops.gemm, L["ao2"], P[f"l{l}_xo"], xr, n=D, epilogue=ops.EPI_F32, resid=xr,
+                          row_lens=lens)
             if keep:
                 L["x_mid"] = xr.clone()
             fo3 = fo + (npl - 1) * 2 * D
-            L["h2"] = self._run("norm", ops.rmsnorm_film, xr, buf("h", B, N, D), film=film[:, fo3:fo3 + 2 * D])
+            L["h2"] = self._run("norm", ops.rmsnorm_film, xr, buf("h", B, N, D), film=film[:, fo3:fo3 + 2 * D],
+                                lens=lens)
             L["ff_g"] = self._run("ff_in", ops.gemm, L["h2"], P[f"l{l}_ff_w1"], buf("ff_g", B, N, Dp), n=2 * Dp,
-                                  epilogue=ops.EPI_GEGLU, bias=P[f"l{l}_ff_b1"])
+                                  epilogue=ops.EPI_GEGLU, bias=P[f"l{l}_ff_b1"], row_lens=lens)
             # causal conv with the output projection folded in: x += W' * g + b' straight from the GEGLU output
             self._run("ff_conv", ops.gemm, L["ff_g"], P[f"l{l}_ff_wo"], xr, n=D, epilogue=ops.EPI_F32,
-                      bias=P[f"l{l}_ff_bo"], resid=xr, segs=ops.conv3_segs(Dp))
+                      bias=P[f"l{l}_ff_bo"], resid=xr, segs=ops.conv3_segs(Dp), row_lens=lens)
             layers.append(L)
-        hf = self._run("norm", ops.rmsnorm_film, xr, buf("h", B, N, D), gamma=P["pred_gamma"])
+        hf = self._run("norm", ops.rmsnorm_film, xr, buf("h", B, N, D), gamma=P["pred_gamma"], lens=lens)
         if keep:
-            saved.update(layers=layers, x_final=xr, hf=hf)
+            saved.update(layers=layers, x_final=xr, hf=hf, lens=lengths)
         if out is None:
             out = torch.empty(B, N, D, device=dev, dtype=torch.float32)   # fresh tensor, like the reference
-        return self._run("pred", ops.gemm, hf, P["pred_w"], out, n=D, epilogue=ops.EPI_F32)
+        self._run("pred", ops.gemm, hf, P["pred_w"], out, n=D, epilogue=ops.EPI_F32, row_lens=lens)
+        if lengths is not None:
+            self._run("mask", ops.mask_rows, out, lengths)
+        return out

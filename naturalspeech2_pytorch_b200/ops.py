@@ -105,18 +105,26 @@ def gemm(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, n: int, epilogu
          resid: Optional[torch.Tensor] = None, film: Optional[torch.Tensor] = None,
          film_group_stride: int = 0, bias1_off: int = 0, groups: int = 1,
          a_group_col_stride: int = 0, b_group_row_stride: int = 0, out_group_col_stride: int = 0,
-         dil: Optional[Sequence[int]] = None, flags: int = 0) -> torch.Tensor:
+         dil: Optional[Sequence[int]] = None, flags: int = 0,
+         row_lens: Optional[torch.Tensor] = None) -> torch.Tensor:
     """out = epilogue(segmented_gemm(a, w)).  `a`: (batches, rows, cols) bf16 (may be a strided view),
-    `w`: packed bf16 weight (rows, K).  See include/ns2_b200.h section 1 for the exact semantics."""
+    `w`: packed bf16 weight (rows, K).  See include/ns2_b200.h section 1 for the exact semantics.
+    row_lens: int32 CUDA (batches,) in [1, rows], at most NS2_GEMM_ROW_LENS_MAX_BATCHES batches: only the 128-row tiles
+    of batch b that start before row_lens[b] are computed (bit-identical to the call without it); rows of the other
+    tiles of `out` are left as they were."""
     lib = _lib.load()
     # the epilogue reads bias[g * b_group_row_stride + col] for every output column col < n (and + bias1_off)
     need = (groups - 1) * b_group_row_stride + n + (bias1_off if epilogue == EPI_WAVENET else 0)
     if bias is not None and bias.numel() < need:
         raise ValueError(f"bias must have >= {need} elements for n={n}, got {bias.numel()}")
     Ba, M, _ = a.shape
+    if row_lens is not None and Ba > _lib.NS2_GEMM_ROW_LENS_MAX_BATCHES:
+        raise ValueError(f"row_lens: at most {_lib.NS2_GEMM_ROW_LENS_MAX_BATCHES} batches, got {Ba}")
     _check(("a", a, BF16, None, LAST), ("w", w, BF16, (None, None), LAST),
            ("out", out, F32 if epilogue == EPI_F32 else BF16, (Ba, M, None), ROWS), ("bias", bias, F32, None, DENSE),
-           ("resid", resid, F32, out.shape, ROWS), ("film", film, F32, None, LAST))
+           ("resid", resid, F32, out.shape, ROWS), ("film", film, F32, None, LAST),
+           ("row_lens", row_lens, I32, (Ba,), DENSE))
+    lens_ptr = _check_lens(row_lens, 1, M, "row_lens")
     if segs is None:
         segs = [(0, 0, a.shape[2], 0, 0)]
     args = GemmArgs()
@@ -150,7 +158,7 @@ def gemm(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, n: int, epilogu
     args.film = _ptr(film)
     args.film_group_stride = film_group_stride
     args.flags = int(flags)
-    check(lib.ns2_gemm(C.byref(args), _stream()), "ns2_gemm")
+    check(lib.ns2_gemm_row_lens(C.byref(args), lens_ptr, _stream()), "ns2_gemm_row_lens")
     return out
 
 
@@ -324,21 +332,26 @@ def pack_rows(a: torch.Tensor, a_lens: torch.Tensor, b: torch.Tensor, b_lens: to
 # --------------------------------------------------------------------------------------------------
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tensor, *, heads: int,
               scale: Optional[float] = None, lse: Optional[torch.Tensor] = None,
-              dropout: Optional[DropoutSpec] = None, kv_lens: Optional[torch.Tensor] = None) -> torch.Tensor:
+              dropout: Optional[DropoutSpec] = None, kv_lens: Optional[torch.Tensor] = None,
+              q_lens: Optional[torch.Tensor] = None) -> torch.Tensor:
     """q: (B, Nq, heads*64), k/v: (B, Nk, heads*64) bf16 (strided views into a fused projection are fine).
     dropout=(seed, site, p): attention dropout on the softmax probabilities (lse stays that of the undropped ones).
     kv_lens: int32 CUDA (B,) in [1, Nk]: sample b attends to its keys [0, kv_lens[b]) only (K / V rows past it must be
-    finite); its output is bit-identical to the call on that sample's keys alone.  No dropout with kv_lens."""
+    finite); its output is bit-identical to the call on that sample's keys alone.  No dropout with kv_lens.
+    q_lens: int32 CUDA (B,) in [1, Nq]: the 128-query tiles of sample b that start at or past q_lens[b] are skipped
+    (their out rows and lse entries are left as they were); the other rows are bit-identical to the call without it.
+    No dropout with q_lens."""
     lib = _lib.load()
-    if kv_lens is not None and dropout is not None:
-        raise ValueError("attention: dropout with kv_lens is not supported")
+    if (kv_lens is not None or q_lens is not None) and dropout is not None:
+        raise ValueError("attention: dropout with kv_lens or q_lens is not supported")
     inner = heads * 64
     B, Nq, _ = q.shape
     _, Nk, _ = k.shape
     _check(("q", q, BF16, (B, Nq, inner), LAST), ("k", k, BF16, (B, Nk, inner), LAST), ("v", v, BF16, (B, Nk, inner), LAST),
            ("out", out, BF16, (B, Nq, inner), LAST), ("lse", lse, F32, (B, heads, Nq), DENSE),
-           ("kv_lens", kv_lens, I32, (B,), DENSE))
+           ("kv_lens", kv_lens, I32, (B,), DENSE), ("q_lens", q_lens, I32, (B,), DENSE))
     lens_ptr = _check_lens(kv_lens, 1, Nk, "kv_lens")
+    q_lens_ptr = _check_lens(q_lens, 1, Nq, "q_lens")
     args = AttnArgs()
     args.q, args.q_row_stride, args.q_batch_stride = q.data_ptr(), q.stride(1), q.stride(0)
     args.k, args.k_row_stride, args.k_batch_stride = k.data_ptr(), k.stride(1), k.stride(0)
@@ -350,7 +363,7 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tens
     args.lse, args.kv_lens = _ptr(lse), lens_ptr
     d = _dropout_args(dropout)
     args.dropout = None if d is None else C.pointer(d)
-    check(lib.ns2_attn_fwd(C.byref(args), _stream()), "ns2_attn_fwd")
+    check(lib.ns2_attn_fwd_q_lens(C.byref(args), q_lens_ptr, _stream()), "ns2_attn_fwd_q_lens")
     return out
 
 
@@ -358,17 +371,20 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tens
 # norms, small layers, casts
 # --------------------------------------------------------------------------------------------------
 def rmsnorm_film(x: torch.Tensor, out: torch.Tensor, *, gamma: Optional[torch.Tensor] = None,
-                 film: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """x: (B, N, D) f32 -> out (B, N, D) bf16.  film: (B, >=2D) f32 view whose row b holds [gamma_b | beta_b]."""
+                 film: Optional[torch.Tensor] = None, lens: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """x: (B, N, D) f32 -> out (B, N, D) bf16.  film: (B, >=2D) f32 view whose row b holds [gamma_b | beta_b].
+    lens: int32 CUDA (B,) in [1, N]: only rows [0, lens[b]) of sample b are normalized (bit-identical to the call without
+    it); the other rows of `out` are left as they were."""
     lib = _lib.load()
     B, N, D = x.shape
     if film is not None and film.shape[-1] < 2 * D:
         raise ValueError(f"film must have >= {2 * D} columns, got {tuple(film.shape)}")
     _check(("x", x, F32, None, DENSE), ("out", out, BF16, (B, N, D), DENSE), ("gamma", gamma, F32, (D,), DENSE),
-           ("film", film, F32, (B, None), LAST))
+           ("film", film, F32, (B, None), LAST), ("lens", lens, I32, (B,), DENSE))
+    lens_ptr = _check_lens(lens, 1, N, "lens")
     film_bs = 0 if film is None else film.stride(0)
-    check(lib.ns2_rmsnorm_film(x.data_ptr(), D, B * N, D, N, _ptr(gamma), _ptr(film), film_bs,
-                               out.data_ptr(), D, _stream()), "ns2_rmsnorm_film")
+    check(lib.ns2_rmsnorm_film_lens(x.data_ptr(), D, B * N, D, N, _ptr(gamma), _ptr(film), film_bs,
+                                    out.data_ptr(), D, lens_ptr, _stream()), "ns2_rmsnorm_film_lens")
     return out
 
 
@@ -570,8 +586,10 @@ def q_sample(x0, noise, alpha, sigma, x_t, target=None, objective: str = "v"):
     return x_t, target
 
 
-def mse_rows(pred, target, out, scratch=None, mean_out=None):
-    """out[b] = mean((pred[b] - target[b])^2); `mean_out` (0-d / 1-element f32) additionally receives out.mean()."""
+def mse_rows(pred, target, out, scratch=None, mean_out=None, lens=None):
+    """out[b] = mean((pred[b] - target[b])^2); `mean_out` (0-d / 1-element f32) additionally receives out.mean().
+    lens: int32 CUDA (B,) in [1, N] for pred (B, N, ...): out[b] is the mean over sample b's first lens[b] rows,
+    bit-identical to the call on pred[b:b+1, :lens[b]]; the rest is not read."""
     lib = _lib.load()
     B, n = pred.shape[0], pred.numel()
     if scratch is None:
@@ -581,10 +599,24 @@ def mse_rows(pred, target, out, scratch=None, mean_out=None):
     if mean_out is not None and mean_out.numel() != 1:
         raise ValueError(f"mean_out must hold one element, got {mean_out.numel()}")
     _check(("pred", pred, F32, None, DENSE), ("target", target, F32, tuple(pred.shape), DENSE),
-           ("out", out, F32, (B,), DENSE), ("scratch", scratch, F32, None, DENSE), ("mean_out", mean_out, F32, None, DENSE))
-    check(lib.ns2_mse_rows(pred.data_ptr(), target.data_ptr(), B, n // B, scratch.data_ptr(),
-                           out.data_ptr(), _ptr(mean_out), _stream()), "ns2_mse_rows")
+           ("out", out, F32, (B,), DENSE), ("scratch", scratch, F32, None, DENSE), ("mean_out", mean_out, F32, None, DENSE),
+           ("lens", lens, I32, (B,), DENSE))
+    rows, lp = _rows_lens(pred, lens)
+    check(lib.ns2_mse_rows_lens(pred.data_ptr(), target.data_ptr(), B, n // B, scratch.data_ptr(),
+                                out.data_ptr(), _ptr(mean_out), n // B // rows, lp, _stream()), "ns2_mse_rows_lens")
     return out
+
+
+def _rows_lens(pred: torch.Tensor, lens: Optional[torch.Tensor]) -> Tuple[int, Optional[int]]:
+    """(rows per sample, checked lengths pointer) of a (B, N, ...) tensor whose samples are lens[b] rows long."""
+    if lens is None:
+        return 1, None
+    if pred.dim() < 2:
+        raise ValueError(f"pred must be (B, N, ...) with lens, got {tuple(pred.shape)}")
+    rows = pred.shape[1]
+    if (pred.numel() // pred.shape[0] // rows) % 4:
+        raise ValueError(f"pred rows must hold a multiple of 4 elements with lens, got {tuple(pred.shape)}")
+    return rows, _check_lens(lens, 1, rows, "lens")
 
 
 def ddim_step(x, v, alpha, sigma, alpha_next, sigma_next, objective: str = "v"):
@@ -849,16 +881,19 @@ def group_sum(t, out, *, dim: int, groups: int):
     return out
 
 
-def mse_bwd(pred, target, coef, out_bf=None, out_f32=None):
-    """coef[b] * (pred - target) as bf16 and/or f32: the seed of the backward pass."""
+def mse_bwd(pred, target, coef, out_bf=None, out_f32=None, lens=None):
+    """coef[b] * (pred - target) as bf16 and/or f32: the seed of the backward pass.  lens: int32 CUDA (B,) in [1, N] for
+    pred (B, N, ...): rows past lens[b] of sample b are written as exact zeros, the others are as without lens."""
     lib = _lib.load()
     B, n = pred.shape[0], pred.numel()
     if any(t is not None and t.numel() != n for t in (target, out_bf, out_f32)) or coef.numel() != B:
         raise ValueError(f"target, out_bf and out_f32 must hold pred's {n} elements and coef {B}")
     _check(("pred", pred, F32, None, DENSE, 16), ("target", target, F32, None, DENSE, 16), ("coef", coef, F32, None, DENSE),
-           ("out_bf", out_bf, BF16, None, DENSE, 8), ("out_f32", out_f32, F32, None, DENSE, 16))
-    check(lib.ns2_mse_bwd(pred.data_ptr(), target.data_ptr(), coef.data_ptr(), B, n // B, _ptr(out_bf),
-                          _ptr(out_f32), _stream()), "ns2_mse_bwd")
+           ("out_bf", out_bf, BF16, None, DENSE, 8), ("out_f32", out_f32, F32, None, DENSE, 16),
+           ("lens", lens, I32, (B,), DENSE))
+    rows, lp = _rows_lens(pred, lens)
+    check(lib.ns2_mse_bwd_lens(pred.data_ptr(), target.data_ptr(), coef.data_ptr(), B, n // B, _ptr(out_bf),
+                               _ptr(out_f32), n // B // rows, lp, _stream()), "ns2_mse_bwd_lens")
     return out_bf if out_bf is not None else out_f32
 
 

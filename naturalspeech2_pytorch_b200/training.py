@@ -191,6 +191,9 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grad
     dil = [2 ** i for i in range(G)]
 
     # ---- to_pred: Linear (no bias) after RMSNorm(gamma) ----
+    lens = S.get("lens")
+    if lens is not None:   # the forward zeroed the prediction past each latent length: no gradient flows from there
+        d_out = ops.mask_rows(d_out.float().clone(memory_format=torch.contiguous_format), lens)
     dout_bf = ops.cast_bf16(d_out.float().contiguous(), e(B, N, D))
     dhf = linear_backward(dout_bf, S["hf"], grads, "transformer.to_pred.1", T["pred_w"], bias=False)
     dxr = z(B, N, D)                       # fp32 gradient of the residual stream
@@ -224,7 +227,7 @@ def train_backward(model, S: dict, d_out: torch.Tensor, reducer=None, input_grad
             norm_backward(L["x_c"], dh_x, fo + 2 * D)
         # ---- attention branch: x += Wo attn(Wqkv h1) ----
         dh1, _ = attention_backward(dxr_bf, L["h1"], L["ao"], L["lse"], L["qkv"], None, T[f"l{l}_o"], T[f"l{l}_qkv"], H,
-                                    grads, pfx + "1.")
+                                    grads, pfx + "1.", kv_lens=lens)
         norm_backward(L["x_in"], dh1, fo)
         # FiLM projections of this layer's norms: their rows of dfilm are final now, so the weight gradient (the largest
         # gradient buffers of the model) joins this layer's all-reduce instead of trailing the whole backward
@@ -420,10 +423,10 @@ class DenoiserFunction(torch.autograd.Function):
     """One autograd node for the whole denoiser: forward saves activations, backward runs the kernels above."""
 
     @staticmethod
-    def forward(ctx, model, x, times, prompt, cond, cond_drop_prob, prompt_lens, *params):
+    def forward(ctx, model, x, times, prompt, cond, cond_drop_prob, prompt_lens, lengths, *params):
         saved = {}
         out = model._forward_impl(x, times, prompt, cond=cond, cond_drop_prob=cond_drop_prob, saved=saved,
-                                  prompt_lens=prompt_lens)
+                                  prompt_lens=prompt_lens, lengths=lengths)
         ctx.model, ctx.saved = model, saved
         ctx.in_dtypes = (prompt.dtype if prompt is not None else None, cond.dtype if cond is not None else None)
         return out
@@ -441,21 +444,27 @@ class DenoiserFunction(torch.autograd.Function):
             d_prompt = d_prompt.to(ctx.in_dtypes[0])
         if d_cond is not None:
             d_cond = d_cond.to(ctx.in_dtypes[1])
-        return (None, None, None, d_prompt, d_cond, None, None, *param_grads(ctx.model, grads))
+        return (None, None, None, d_prompt, d_cond, None, None, None, *param_grads(ctx.model, grads))
 
 
 class MseRowsFunction(torch.autograd.Function):
-    """Per-sample mean squared error (ns2.py:1646-1647) with the hand-written forward / backward kernels."""
+    """Per-sample mean squared error (ns2.py:1646-1647) with the hand-written forward / backward kernels.  `lens`
+    (validated int32 CUDA (B,), optional): sample b is its first lens[b] rows; its mean and gradient are those of the
+    sample alone, and the gradient past them is exact zeros."""
 
     @staticmethod
-    def forward(ctx, pred, target):
+    def forward(ctx, pred, target, lens=None):
         pred, target = pred.contiguous(), target.contiguous()
         ctx.save_for_backward(pred, target)
-        return ops.mse_rows(pred, target, torch.empty(pred.shape[0], device=pred.device))
+        ctx.lens = lens
+        return ops.mse_rows(pred, target, torch.empty(pred.shape[0], device=pred.device), lens=lens)
 
     @staticmethod
     def backward(ctx, d_rows):
         pred, target = ctx.saved_tensors
         per = pred.numel() // pred.shape[0]
-        coef = (d_rows.float() * (2.0 / per)).contiguous()
-        return ops.mse_bwd(pred, target, coef, out_f32=torch.empty_like(pred)), None
+        if ctx.lens is None:
+            coef = (d_rows.float() * (2.0 / per)).contiguous()
+        else:   # 2 / (lens[b] * row elements), rounded to fp32 as the alone call's 2.0 / per is
+            coef = (d_rows.float() * (2.0 / (ctx.lens.double() * (per // pred.shape[1]))).float()).contiguous()
+        return ops.mse_bwd(pred, target, coef, out_f32=torch.empty_like(pred), lens=ctx.lens), None, None

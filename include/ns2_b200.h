@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define NS2_ABI_VERSION 8
+#define NS2_ABI_VERSION 9
 
 typedef void* ns2_stream_t; /* cudaStream_t */
 
@@ -60,10 +60,22 @@ int ns2_set_sm_limit(int sms);
  *                    gamma = film[b*film_batch_stride + g*film_group_stride + j], beta = gamma + n;
  *                    bias1 = bias + bias1_off.
  * All k_len must be multiples of 64 unless the segment ends at the last column of A and B.
+ *
+ * row_lens: a batch of sequences of different lengths, padded at the end: batch b's rows [0, row_lens[b]) are the
+ * sample, the rest padding.  Device int32 (a_batches), each value clamped to [1, a_rows]; NULL = every row.  Only the
+ * 128-row tiles that start before row_lens[b] are computed and stored (ceil(row_lens[b] / 128) tiles of batch b per
+ * group and n-tile); every row of those tiles, including the rows at or past row_lens[b] inside the last one, is
+ * bit-identical to the call without row_lens.  Rows of the other tiles are left untouched: neither written nor, with
+ * the F32 epilogue's in-place residual, reduce-added.  A computed row reads A rows of its own tile and, through causal
+ * shifts, earlier ones, so rows in untouched tiles (whatever they hold, NaN included) reach no computed row unless a
+ * negative shift_units (an anti-causal tap) reads past the tile; callers must not pass such segments with padding that
+ * is not finite.  With row_lens, a_batches must be <= NS2_GEMM_ROW_LENS_MAX_BATCHES (the lengths and their prefix sums
+ * live in the kernel's shared memory); a larger batch is an error and nothing is launched.
  * ------------------------------------------------------------------------------------------------ */
 enum { NS2_EPI_BF16 = 0, NS2_EPI_F32 = 1, NS2_EPI_GEGLU = 2, NS2_EPI_WAVENET = 3 };
 #define NS2_GEMM_MAX_SEGS 12 /* a k=9 convolution (SpeechPromptEncoder, ns2.py:316-320) is 9 segments */
 #define NS2_GEMM_MAX_GROUPS 8
+#define NS2_GEMM_ROW_LENS_MAX_BATCHES 64
 
 typedef struct ns2_gemm_seg {
   int32_t a_col_off;   /* first A column of this segment (within the group's column window) */
@@ -100,6 +112,7 @@ typedef struct ns2_gemm_args {
   int64_t film_batch_stride;
   int32_t film_group_stride;
   int32_t flags;           /* 0, or NS2_GEMM_FLAG_*; any other bit is an error */
+  const int32_t* row_lens; /* optional (a_batches) row counts; NULL = every row */
 } ns2_gemm_args;
 
 #define NS2_GEMM_FLAG_SKIP_EPILOGUE 1  /* measurement aid: run the TMA/MMA mainloop only, write nothing */
@@ -107,21 +120,6 @@ typedef struct ns2_gemm_args {
                                encoder (ns2.py:316-320) and CausalConv1d + SiLU of the phoneme encoder (ns2.py:255-257) */
 
 int ns2_gemm(const ns2_gemm_args* args, ns2_stream_t stream);
-
-/* ns2_gemm over a batch of sequences of different lengths, padded at the end: batch b's rows [0, row_lens[b]) are the
- * sample, the rest padding.  row_lens: device int32 (a_batches), each value clamped to [1, a_rows].  Only the 128-row
- * tiles that start before row_lens[b] are computed and stored (ceil(row_lens[b] / 128) tiles of batch b per group and
- * n-tile); every row of those tiles, including the rows at or past row_lens[b] inside the last one, is bit-identical to
- * ns2_gemm's.  Rows of the other tiles are left untouched: neither written nor, with the F32 epilogue's in-place
- * residual, reduce-added.  A computed row reads A rows of its own tile and, through causal shifts, earlier ones, so
- * rows in untouched tiles (whatever they hold, NaN included) reach no computed row unless a negative shift_units (an
- * anti-causal tap) reads past the tile; callers must not pass such segments with padding that is not finite.
- * a_batches must be <= NS2_GEMM_ROW_LENS_MAX_BATCHES (the lengths and their prefix sums live in the kernel's shared
- * memory); a larger batch is an error and nothing is launched.  row_lens == NULL is exactly ns2_gemm, which forwards to
- * this call.  An argument rather than a field of ns2_gemm_args, so that the struct's layout stays that of ABI
- * version 8. */
-#define NS2_GEMM_ROW_LENS_MAX_BATCHES 64
-int ns2_gemm_row_lens(const ns2_gemm_args* args, const int32_t* row_lens, ns2_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * 1b. Weight gradient of a Linear / CausalConv1d tap (autograd's grad_weight = grad_output^T @ input; the reference
@@ -170,7 +168,7 @@ typedef struct ns2_dropout {
  * 2. Non-causal flash attention forward (Attend.forward, attend.py:112-155 with causal=False).
  *    q/k/v: bf16, head h lives in columns [h*64, h*64+64) of each row; dim_head must be 64.
  *    out[b, i, h*64:(h+1)*64] = softmax_j(q_i . k_j * scale) @ v   (bf16)
- *    With kv_lens == NULL and dropout == NULL (a zero-initialised struct's optional fields) this is the unmasked,
+ *    With kv_lens, q_lens and dropout NULL (a zero-initialised struct's optional fields) this is the unmasked,
  *    dropout-free attention the denoiser runs (mask=None, dropout=0, SURVEY T9).
  *  kv_lens: key padding for a batch of sequences of different lengths: sample b attends to keys [0, kv_lens[b]) only —
  *    Attend with a key-padding mask (attend.py:123-129, 140-142: masked scores -> -max, i.e. probability 0), the `mask`
@@ -181,9 +179,16 @@ typedef struct ns2_dropout {
  *    0 * V is still formed (V = NaN or inf there would reach the output).
  *    Query rows are not masked: rows a caller treats as padding get finite, meaningless output.
  *    Sample b's output rows are bit-identical to a call on that sample alone with kv_len = kv_lens[b] and no kv_lens.
+ *  q_lens: query padding: sample b's queries [0, q_lens[b]) are the sample, the rest padding (device int32 (batches),
+ *    each value clamped to [1, q_len]).  A 128-query tile that starts at or past q_lens[b] does nothing: its out rows
+ *    and lse entries are left untouched.  Every row of the other tiles, including rows at or past q_lens[b] inside the
+ *    last one, is bit-identical to the call without q_lens and the same kv_lens (or none).  Self-attention over padded
+ *    sequences passes the same lengths as kv_lens and q_lens; cross-attention to unpadded keys passes q_lens only.
+ *    Q rows of skipped tiles are never loaded, so they may hold anything.
+ *  q_lens / kv_lens with a dropout of p > 0 is an error, nothing launched.
  *  dropout: dropout on the softmax probabilities (Attend, attend.py:106 SDPA dropout_p, attend.py:149 attn_dropout):
  *    out = ((P (.) M) V) / (1 - p); lse as without dropout (undropped probabilities, bit-identical).  p = 0 gives the
- *    bits of dropout == NULL.  kv_lens together with a dropout of p > 0 is an error (nothing is launched).
+ *    bits of dropout == NULL.
  * ------------------------------------------------------------------------------------------------ */
 typedef struct ns2_attn_args {
   const void* q; int64_t q_row_stride, q_batch_stride;
@@ -196,19 +201,10 @@ typedef struct ns2_attn_args {
                     saved for ns2_attn_bwd */
   const int32_t* kv_lens;       /* optional (batches) key counts; NULL = every key */
   const ns2_dropout* dropout;   /* optional; NULL = no dropout */
+  const int32_t* q_lens;        /* optional (batches) query counts; NULL = every query */
 } ns2_attn_args;
 
 int ns2_attn_fwd(const ns2_attn_args* args, ns2_stream_t stream);
-
-/* ns2_attn_fwd with query lengths: sample b's queries [0, q_lens[b]) are the sample, the rest padding (device int32
- * (batches), each value clamped to [1, q_len]).  A 128-query tile that starts at or past q_lens[b] does nothing: its out
- * rows and lse entries are left untouched.  Every row of the other tiles, including rows at or past q_lens[b] inside
- * the last one, is bit-identical to ns2_attn_fwd's with the same kv_lens (or none).  Self-attention over padded
- * sequences passes the same lengths as kv_lens; cross-attention to unpadded keys passes q_lens only.  Q rows of skipped
- * tiles are never loaded, so they may hold anything; K / V rows must be finite as for ns2_attn_fwd.  q_lens == NULL is
- * exactly ns2_attn_fwd.  q_lens together with a dropout of p > 0 is an error (nothing is launched).  An argument rather
- * than a field of ns2_attn_args, so that the struct's layout stays that of ABI version 8. */
-int ns2_attn_fwd_q_lens(const ns2_attn_args* args, const int32_t* q_lens, ns2_stream_t stream);
 
 /* Backward of the above (autograd of F.scaled_dot_product_attention, reached from loss.backward(), ns2.py:1886):
  *   dq_accum (batches, q_len, heads*64) f32, contiguous: dQ is ADDED to it (every key tile adds its share; zero it for
@@ -216,7 +212,10 @@ int ns2_attn_fwd_q_lens(const ns2_attn_args* args, const int32_t* q_lens, ns2_st
  *   dk / dv: bf16, same layout conventions as k / v;  lse from ns2_attn_fwd;  delta: scratch (batches, heads, q_len) f32.
  *   dropout: the forward's dropout parameters; the mask is regenerated from (seed, site, b, h, q, k):
  *   dV = (P (.) M)^T dO / (1 - p), dP = (dO V^T) (.) M / (1 - p), dS = P (.) (dP - D), D from the dropped output o.
- *   p = 0 gives the bits of dropout == NULL. */
+ *   p = 0 gives the bits of dropout == NULL.
+ *   kv_lens: the forward's kv_lens.  Sample b's dk / dv rows [0, kv_lens[b]) are bit-identical to a call on that sample
+ *   alone with kv_len = kv_lens[b]; its rows past kv_lens[b] are written as exact zeros, and nothing from them reaches
+ *   dq_accum.  K / V rows past kv_lens[b] must be finite (as for the forward).  With a dropout of p > 0 an error. */
 typedef struct ns2_attn_bwd_args {
   const void* q; int64_t q_row_stride, q_batch_stride;
   const void* k; int64_t k_row_stride, k_batch_stride;
@@ -231,18 +230,10 @@ typedef struct ns2_attn_bwd_args {
   int32_t batches, heads, q_len, kv_len, dim_head;
   float scale;
   const ns2_dropout* dropout;   /* optional; NULL = no dropout */
+  const int32_t* kv_lens;       /* optional (batches) key counts; NULL = every key */
 } ns2_attn_bwd_args;
 
 int ns2_attn_bwd(const ns2_attn_bwd_args* args, ns2_stream_t stream);
-
-/* The backward of ns2_attn_fwd with kv_lens (key padding): the same arguments, plus the forward's kv_lens (device int32
- * (batches), each value clamped to [1, kv_len]).  Sample b's dk / dv rows [0, kv_lens[b]) are bit-identical to a call
- * on that sample alone with kv_len = kv_lens[b]; its rows past kv_lens[b] are written as exact zeros, and nothing from
- * them reaches dq_accum.  K / V rows past kv_lens[b] must be finite (as for the forward).  kv_lens == NULL is exactly
- * ns2_attn_bwd, which forwards to this call.  kv_lens together with a dropout of p > 0 is an error (nothing is
- * launched).  kv_lens is an argument rather than a field of ns2_attn_bwd_args so that the struct's layout stays that of
- * ABI version 8; it moves into the struct at the next ABI version. */
-int ns2_attn_bwd_kv_lens(const ns2_attn_bwd_args* args, const int32_t* kv_lens, ns2_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * 2b. Dropout (training only).  One site's parameters: a 64-bit seed (Philox4x32-10 key = its low / high 32 bits),
@@ -263,19 +254,14 @@ int ns2_dropout_f32(float* x, int64_t n, const ns2_dropout* dropout, ns2_stream_
  *    out_bf16[r, :] = x[r,:] / max(||x[r,:]||_2, 1e-12) * sqrt(dim) * gamma * film_gamma[b] + film_beta[b]
  *    gamma may be NULL (=1); film may be NULL (no FiLM); b = r / rows_per_batch;
  *    film_gamma = film + b*film_batch_stride, film_beta = film_gamma + dim.
+ *    lens: NULL = every row, or per-batch row counts: device int32 (rows / rows_per_batch), each value clamped to
+ *    [1, rows_per_batch].  Row r of batch b is normalized only if r % rows_per_batch < lens[b], by the same per-row
+ *    code as without lens (bit-identical); the other rows are neither read nor written.
  * ------------------------------------------------------------------------------------------------ */
 int ns2_rmsnorm_film(const float* x, int64_t x_row_stride, int64_t rows, int32_t dim,
                      int32_t rows_per_batch, const float* gamma, const float* film,
                      int64_t film_batch_stride, void* out_bf16, int64_t out_row_stride,
-                     ns2_stream_t stream);
-
-/* ns2_rmsnorm_film with per-batch row counts: lens device int32 (rows / rows_per_batch), each value clamped to
- * [1, rows_per_batch].  Row r of batch b = r / rows_per_batch is normalized only if r % rows_per_batch < lens[b], by the
- * same per-row code as ns2_rmsnorm_film (bit-identical); the other rows are neither read nor written.  lens == NULL is
- * exactly ns2_rmsnorm_film, which forwards to this call. */
-int ns2_rmsnorm_film_lens(const float* x, int64_t x_row_stride, int64_t rows, int32_t dim, int32_t rows_per_batch,
-                          const float* gamma, const float* film, int64_t film_batch_stride, void* out_bf16,
-                          int64_t out_row_stride, const int32_t* lens, ns2_stream_t stream);
+                     const int32_t* lens, ns2_stream_t stream);
 
 /* Same, fp32 output (PerceiverResampler.norm, ns2.py:566,579). */
 int ns2_rmsnorm_f32(const float* x, int64_t x_row_stride, int64_t rows, int32_t dim,
@@ -372,7 +358,12 @@ int ns2_expand_encodings(const float* phon, const int32_t* coarse, const float* 
  *    ns2_q_sample   : x_t = alpha*x0 + sigma*noise ; target = alpha*noise - sigma*x0 (v) | noise (eps) | x0 (x0)
  *    ns2_mse_rows   : out[b] = mean((pred-target)^2) over the sample          (ns2.py:1646-1647);
  *                     deterministic two-level reduction through caller-provided scratch; optionally
- *                     also the batch mean of those per-sample values (one more tiny launch)
+ *                     also the batch mean of those per-sample values (one more tiny launch).
+ *                     lens: NULL = every element, or a batch padded at the end: sample b is its first lens[b] rows of
+ *                     row_elems elements (device int32 (batch), each clamped to [1, per_sample / row_elems]; row_elems
+ *                     a multiple of 4 dividing per_sample, read only with lens).  out[b] is the mean over those
+ *                     lens[b] * row_elems elements, reduced in the order a call on the unpadded sample uses:
+ *                     bit-identical to it.  Elements past them are not read (they may hold anything).
  *    ns2_ddim_step  : x0 = alpha*x - sigma*out (v) | (x - sigma*out)/max(alpha,1e-10) (eps) | out (x0) ;
  *                     eps = (x - alpha*x0)/max(sigma,1e-10) ;
  *                     x <- x0*alpha_next + eps*sigma_next                     (ns2.py:1420-1429)
@@ -388,15 +379,7 @@ int ns2_q_sample(const float* x0, const float* noise, const float* alpha, const 
 int ns2_mse_rows(const float* pred, const float* target, int32_t batch, int64_t per_sample,
                  float* scratch /* batch * NS2_MSE_SCRATCH_PER_SAMPLE floats */, float* out,
                  float* mean_out /* optional: mean over the batch of out[], ns2.py:1666 */,
-                 ns2_stream_t stream);
-/*    ns2_mse_rows_lens : ns2_mse_rows over a batch padded at the end: sample b is its first lens[b] rows of row_elems
- *                        elements (device int32 (batch), each clamped to [1, per_sample / row_elems]; row_elems a
- *                        multiple of 4 dividing per_sample).  out[b] is the mean over those lens[b] * row_elems elements,
- *                        reduced in the order a call on the unpadded sample uses: bit-identical to it.  Elements past
- *                        them are not read (they may hold anything).  mean_out as for ns2_mse_rows.  lens == NULL is
- *                        exactly ns2_mse_rows, which forwards to this call. */
-int ns2_mse_rows_lens(const float* pred, const float* target, int32_t batch, int64_t per_sample, float* scratch,
-                      float* out, float* mean_out, int64_t row_elems, const int32_t* lens, ns2_stream_t stream);
+                 int64_t row_elems, const int32_t* lens, ns2_stream_t stream);
 int ns2_ddim_step(float* x, const float* v, const float* alpha, const float* sigma,
                   const float* alpha_next, const float* sigma_next, int32_t batch,
                   int64_t per_sample, int32_t objective, ns2_stream_t stream);
@@ -471,7 +454,10 @@ int ns2_rvq_ce_bwd(const float* frames, int64_t num_frames, int32_t d, const flo
  *                           dfilm += [sum dz*c | sum dz] per batch / group
  *    ns2_colsum_bf16      : out[c] += sum_r t[r, c]            (bias gradients)
  *    ns2_group_sum_bf16   : out[r, c] = sum_g t[r, g*dim + c]  (gradient of an input shared by all dilation columns)
- *    ns2_mse_bwd          : out = coef[b] * (pred - target), bf16 and/or f32   (seed of the backward pass, ns2.py:1646-1666)
+ *    ns2_mse_bwd          : out = coef[b] * (pred - target), bf16 and/or f32   (seed of the backward pass, ns2.py:1646-1666);
+ *                           row_elems / lens as for ns2_mse_rows: the first lens[b] rows of row_elems elements of
+ *                           sample b are bit-identical to the call without lens, every element past them is written as
+ *                           an exact zero (pred / target are not read there)
  *    ns2_film_wgrad       : dw[r, c] (+)= sum_b dfilm[b, r] * t[b, c]  (FiLM projection weights; batch <= 32 per call)
  *    ns2_attn_bwd         : flash-attention backward (dq, dk, dv) from (q, k, v, o, lse, do)
  * ------------------------------------------------------------------------------------------------ */
@@ -486,17 +472,12 @@ int ns2_wavenet_gate_bwd(const void* c_bf16, int64_t c_row_stride, const void* d
 int ns2_colsum_bf16(const void* t_bf16, int64_t rows, int32_t cols, int64_t row_stride, float* out, ns2_stream_t stream);
 int ns2_group_sum_bf16(const void* t_bf16, int64_t rows, int32_t dim, int32_t groups, void* out_bf16, ns2_stream_t stream);
 int ns2_mse_bwd(const float* pred, const float* target, const float* coef, int32_t batch, int64_t per_sample,
-                void* out_bf16 /* optional */, float* out_f32 /* optional */, ns2_stream_t stream);
+                void* out_bf16 /* optional */, float* out_f32 /* optional */, int64_t row_elems, const int32_t* lens,
+                ns2_stream_t stream);
 int ns2_film_wgrad(const float* dfilm, int64_t dfilm_batch_stride /* elements between batch rows of dfilm (>= rows): a
                    column window of the stacked FiLM gradient can be reduced as soon as its layer is final */,
                    const float* t, int32_t batch, int64_t rows, int32_t cols, float* dw,
                    int32_t accumulate /* 0: dw = ..., dw need not be initialised; 1: dw += ... */, ns2_stream_t stream);
-/*    ns2_mse_bwd_lens     : ns2_mse_bwd with the lengths of ns2_mse_rows_lens: the first lens[b] rows of row_elems
- *                           elements of sample b are bit-identical to ns2_mse_bwd's, every element past them is written
- *                           as an exact zero (pred / target are not read there).  lens == NULL is exactly ns2_mse_bwd,
- *                           which forwards to this call. */
-int ns2_mse_bwd_lens(const float* pred, const float* target, const float* coef, int32_t batch, int64_t per_sample,
-                     void* out_bf16, float* out_f32, int64_t row_elems, const int32_t* lens, ns2_stream_t stream);
 /*    ns2_accum_bf16       : acc (f32) += t (bf16); acc_bf16 (optional) = bf16(acc)   (joins a branch gradient) */
 int ns2_accum_bf16(float* acc, const void* t_bf16, int64_t count, void* acc_bf16, ns2_stream_t stream);
 

@@ -22,7 +22,7 @@ NS2_SEANET_TAIL_PARAMS = 3348
 NS2_SEANET_HEAD_PARAMS = 3376
 NS2_ROWDOT_BWD_ROWS = 32
 NS2_GEMM_ROW_LENS_MAX_BATCHES = 64
-NS2_ABI_VERSION = 8
+NS2_ABI_VERSION = 9
 
 
 class GemmSeg(C.Structure):
@@ -43,7 +43,7 @@ class GemmArgs(C.Structure):
         ("out", C.c_void_p), ("out_row_stride", C.c_int64),
         ("resid", C.c_void_p), ("resid_row_stride", C.c_int64),
         ("film", C.c_void_p), ("film_batch_stride", C.c_int64), ("film_group_stride", C.c_int32),
-        ("flags", C.c_int32),
+        ("flags", C.c_int32), ("row_lens", C.c_void_p),
     ]
 
 
@@ -70,7 +70,7 @@ class AttnArgs(C.Structure):
         ("out", C.c_void_p), ("o_row_stride", C.c_int64), ("o_batch_stride", C.c_int64),
         ("batches", C.c_int32), ("heads", C.c_int32), ("q_len", C.c_int32), ("kv_len", C.c_int32),
         ("dim_head", C.c_int32), ("scale", C.c_float), ("lse", C.c_void_p),
-        ("kv_lens", C.c_void_p), ("dropout", C.POINTER(Dropout)),
+        ("kv_lens", C.c_void_p), ("dropout", C.POINTER(Dropout)), ("q_lens", C.c_void_p),
     ]
 
 
@@ -85,7 +85,7 @@ class AttnBwdArgs(C.Structure):
         ("dk", C.c_void_p), ("dk_row_stride", C.c_int64), ("dk_batch_stride", C.c_int64),
         ("dv", C.c_void_p), ("dv_row_stride", C.c_int64), ("dv_batch_stride", C.c_int64),
         ("batches", C.c_int32), ("heads", C.c_int32), ("q_len", C.c_int32), ("kv_len", C.c_int32),
-        ("dim_head", C.c_int32), ("scale", C.c_float), ("dropout", C.POINTER(Dropout)),
+        ("dim_head", C.c_int32), ("scale", C.c_float), ("dropout", C.POINTER(Dropout)), ("kv_lens", C.c_void_p),
     ]
 
 
@@ -98,16 +98,12 @@ SIGNATURES = {
     "ns2_set_sm_limit": (C.c_int, [C.c_int]),
     "ns2_launch_count": (C.c_int64, []),
     "ns2_gemm": (C.c_int, [C.POINTER(GemmArgs), _P]),
-    "ns2_gemm_row_lens": (C.c_int, [C.POINTER(GemmArgs), _P, _P]),
     "ns2_wgrad": (C.c_int, [C.POINTER(WgradArgs), _P]),
     "ns2_fold_conv_linear": (C.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P]),
     "ns2_attn_fwd": (C.c_int, [C.POINTER(AttnArgs), _P]),
-    "ns2_attn_fwd_q_lens": (C.c_int, [C.POINTER(AttnArgs), _P, _P]),
     "ns2_attn_bwd": (C.c_int, [C.POINTER(AttnBwdArgs), _P]),
-    "ns2_attn_bwd_kv_lens": (C.c_int, [C.POINTER(AttnBwdArgs), _P, _P]),
     "ns2_dropout_f32": (C.c_int, [_P, _I64, C.POINTER(Dropout), _P]),
-    "ns2_rmsnorm_film": (C.c_int, [_P, _I64, _I64, _I32, _I32, _P, _P, _I64, _P, _I64, _P]),
-    "ns2_rmsnorm_film_lens": (C.c_int, [_P, _I64, _I64, _I32, _I32, _P, _P, _I64, _P, _I64, _P, _P]),
+    "ns2_rmsnorm_film": (C.c_int, [_P, _I64, _I64, _I32, _I32, _P, _P, _I64, _P, _I64, _P, _P]),
     "ns2_rmsnorm_f32": (C.c_int, [_P, _I64, _I64, _I32, _P, _P, _I64, _P]),
     "ns2_time_cond": (C.c_int, [_P, _I32, _P, _I32, _P, _P, _I32, _P, _I64, _P]),
     "ns2_small_linear": (C.c_int, [_P, _I64, _I32, _I32, _P, _P, _I32, _I32, _P, _I64, _P]),
@@ -124,8 +120,7 @@ SIGNATURES = {
     "ns2_cond_inject": (C.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P, _P]),
     "ns2_select_rows": (C.c_int, [_P, _P, _P, _I64, _I32, _I32, _P, _I64, _I32, _P]),
     "ns2_q_sample": (C.c_int, [_P, _P, _P, _P, _I32, _I64, _P, _P, _I32, _P]),
-    "ns2_mse_rows": (C.c_int, [_P, _P, _I32, _I64, _P, _P, _P, _P]),
-    "ns2_mse_rows_lens": (C.c_int, [_P, _P, _I32, _I64, _P, _P, _P, _I64, _P, _P]),
+    "ns2_mse_rows": (C.c_int, [_P, _P, _I32, _I64, _P, _P, _P, _I64, _P, _P]),
     "ns2_ddim_step": (C.c_int, [_P, _P, _P, _P, _P, _P, _I32, _I64, _I32, _P]),
     "ns2_cfg_combine": (C.c_int, [_P, _P, _F, _I64, _P, _P]),
     "ns2_x_start": (C.c_int, [_P, _P, _P, _P, _I32, _I64, _P, _I32, _P]),
@@ -134,8 +129,7 @@ SIGNATURES = {
     "ns2_wavenet_gate_bwd": (C.c_int, [_P, _I64, _P, _I64, _P, _I64, _I32, _I32, _I32, _I32, _P, _I64, _I32, _P, _I64, _P]),
     "ns2_colsum_bf16": (C.c_int, [_P, _I64, _I32, _I64, _P, _P]),
     "ns2_group_sum_bf16": (C.c_int, [_P, _I64, _I32, _I32, _P, _P]),
-    "ns2_mse_bwd": (C.c_int, [_P, _P, _P, _I32, _I64, _P, _P, _P]),
-    "ns2_mse_bwd_lens": (C.c_int, [_P, _P, _P, _I32, _I64, _P, _P, _I64, _P, _P]),
+    "ns2_mse_bwd": (C.c_int, [_P, _P, _P, _I32, _I64, _P, _P, _I64, _P, _P]),
     "ns2_film_wgrad": (C.c_int, [_P, _I64, _P, _I32, _I64, _I32, _P, _I32, _P]),
     "ns2_accum_bf16": (C.c_int, [_P, _P, _I64, _P, _P]),
     "ns2_silu_bwd": (C.c_int, [_P, _P, _I64, _P, _P]),

@@ -63,7 +63,7 @@ __device__ __forceinline__ float ex2_approx(float x) {
 
 __device__ __forceinline__ float keep_if(float x, uint32_t bits, int n) { return (bits >> n) & 1u ? x : 0.f; }
 
-// attn_fwd_kernel<false, *, true> (ns2_attn_fwd_q_lens) adds query padding: a CTA whose query tile starts at or past
+// attn_fwd_kernel<false, *, true> (ns2_attn_args.q_lens) adds query padding: a CTA whose query tile starts at or past
 // q_lens[b] returns before it touches anything, the others run exactly as attn_fwd_kernel<false, RAGGED>.
 template <bool DROPOUT, bool RAGGED, bool QLENS = false>
 __global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid_constant__ AttnDev p) {
@@ -245,15 +245,20 @@ __global__ void __launch_bounds__(attn::THREADS, 1) attn_fwd_kernel(const __grid
 #undef NS2_ATTN_KV_LEN
 }
 
+template <bool DROPOUT, bool RAGGED, bool QLENS>
+static int launch(const AttnDev& dev, dim3 grid, cudaStream_t stream) {
+  NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<DROPOUT, RAGGED, QLENS>, attn::SMEM_BYTES));
+  attn_fwd_kernel<DROPOUT, RAGGED, QLENS><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
+  return launched(1);
+}
+
 }  // namespace ns2
 
 using namespace ns2;
 
-// No dropout (or p = 0) and no kv_lens: the plain kernel; dropout with p > 0: attn_fwd_kernel<true, false>; kv_lens:
-// attn_fwd_kernel<false, true> (never both); q_lens: attn_fwd_kernel<false, kv_lens != NULL, true>.
-extern "C" int ns2_attn_fwd(const ns2_attn_args* a, ns2_stream_t stream) { return ns2_attn_fwd_q_lens(a, nullptr, stream); }
-
-extern "C" int ns2_attn_fwd_q_lens(const ns2_attn_args* a, const int32_t* q_lens, ns2_stream_t stream_) {
+// No dropout (or p = 0) and no lengths: the plain kernel; dropout with p > 0: attn_fwd_kernel<true, false>; kv_lens:
+// attn_fwd_kernel<false, true> (never with dropout); q_lens: attn_fwd_kernel<false, kv_lens != NULL, true>.
+extern "C" int ns2_attn_fwd(const ns2_attn_args* a, ns2_stream_t stream_) {
   NS2_REQUIRE(a != nullptr, "attn_fwd: NULL args");
   const ns2_dropout* d = a->dropout;
   DropoutDev drop;
@@ -261,7 +266,7 @@ extern "C" int ns2_attn_fwd_q_lens(const ns2_attn_args* a, const int32_t* q_lens
               static_cast<double>(d->p));
   const bool dropout = d != nullptr && d->p != 0.0f;
   NS2_REQUIRE(!(dropout && a->kv_lens), "attn_fwd: kv_lens with dropout p > 0 is not supported");
-  NS2_REQUIRE(!(dropout && q_lens), "attn_fwd: q_lens with dropout p > 0 is not supported");
+  NS2_REQUIRE(!(dropout && a->q_lens), "attn_fwd: q_lens with dropout p > 0 is not supported");
   NS2_REQUIRE(a->q && a->k && a->v && a->out, "attn_fwd: NULL pointer");
   NS2_REQUIRE(a->dim_head == 64, "attn_fwd: dim_head=%d, only 64 is supported", a->dim_head);
   NS2_REQUIRE(a->batches > 0 && a->heads > 0 && a->q_len > 0 && a->kv_len > 0, "attn_fwd: empty problem");
@@ -297,23 +302,12 @@ extern "C" int ns2_attn_fwd_q_lens(const ns2_attn_args* a, const int32_t* q_lens
   dev.lse = a->lse;
   dim3 grid((a->q_len + attn::BQ - 1) / attn::BQ, a->heads, a->batches);
   dev.kv_lens = a->kv_lens;
-  dev.q_lens = q_lens;
-  if (q_lens != nullptr && a->kv_lens != nullptr) {
-    NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<false, true, true>, attn::SMEM_BYTES));
-    attn_fwd_kernel<false, true, true><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
-  } else if (q_lens != nullptr) {
-    NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<false, false, true>, attn::SMEM_BYTES));
-    attn_fwd_kernel<false, false, true><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
-  } else if (a->kv_lens != nullptr) {
-    NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<false, true>, attn::SMEM_BYTES));
-    attn_fwd_kernel<false, true><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
-  } else if (!dropout) {
-    NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<false, false>, attn::SMEM_BYTES));
-    attn_fwd_kernel<false, false><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
-  } else {
-    dev.drop = drop;
-    NS2_CUDA_CHECK(set_max_smem_once(attn_fwd_kernel<true, false>, attn::SMEM_BYTES));
-    attn_fwd_kernel<true, false><<<grid, attn::THREADS, attn::SMEM_BYTES, stream>>>(dev);
-  }
-  return launched(1);
+  dev.q_lens = a->q_lens;
+  if (a->q_lens != nullptr)
+    return a->kv_lens != nullptr ? launch<false, true, true>(dev, grid, stream)
+                                 : launch<false, false, true>(dev, grid, stream);
+  if (a->kv_lens != nullptr) return launch<false, true, false>(dev, grid, stream);
+  if (!dropout) return launch<false, false, false>(dev, grid, stream);
+  dev.drop = drop;
+  return launch<true, false, false>(dev, grid, stream);
 }

@@ -320,20 +320,29 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const __nv_bfloat16* __
   }
 }
 
+// attn_bwd_kernel<DROPOUT, RAGGED> over the key tiles; its caller has already launched attn_delta_kernel
+template <bool DROPOUT, bool RAGGED>
+static int launch(const AttnBwdDev& dev, dim3 grid, cudaStream_t stream) {
+  constexpr int smem = DROPOUT ? ab::SMEM_BYTES_DROPOUT : ab::SMEM_BYTES;
+  NS2_CUDA_CHECK(set_max_smem_once(attn_bwd_kernel<DROPOUT, RAGGED>, smem));
+  attn_bwd_kernel<DROPOUT, RAGGED><<<grid, ab::THREADS, smem, stream>>>(dev);
+  return launched(2);
+}
+
 }  // namespace ns2
 
 using namespace ns2;
 
 // No dropout (or p = 0) and no kv_lens: the plain kernel; dropout with p > 0: attn_bwd_kernel<true, false>; kv_lens:
 // attn_bwd_kernel<false, true> (never both).
-extern "C" int ns2_attn_bwd_kv_lens(const ns2_attn_bwd_args* a, const int32_t* kv_lens, ns2_stream_t stream_) {
+extern "C" int ns2_attn_bwd(const ns2_attn_bwd_args* a, ns2_stream_t stream_) {
   NS2_REQUIRE(a != nullptr, "attn_bwd: NULL args");
   const ns2_dropout* d = a->dropout;
   DropoutDev drop;
   NS2_REQUIRE(d == nullptr || make_dropout_dev(d->seed, d->site, d->p, &drop), "attn_bwd: dropout p=%g is not in [0, 1)",
               static_cast<double>(d->p));
   const bool dropout = d != nullptr && d->p != 0.0f;
-  NS2_REQUIRE(!(dropout && kv_lens), "attn_bwd: kv_lens with dropout p > 0 is not supported");
+  NS2_REQUIRE(!(dropout && a->kv_lens), "attn_bwd: kv_lens with dropout p > 0 is not supported");
   NS2_REQUIRE(a->q && a->k && a->v && a->o && a->d_o && a->lse && a->delta && a->dq_accum && a->dk && a->dv,
               "attn_bwd: NULL pointer");
   NS2_REQUIRE(a->dim_head == 64, "attn_bwd: dim_head=%d, only 64 is supported", a->dim_head);
@@ -376,21 +385,9 @@ extern "C" int ns2_attn_bwd_kv_lens(const ns2_attn_bwd_args* a, const int32_t* k
   dev.scale = a->scale;
   dev.scale_log2e = a->scale * 1.4426950408889634f;
   dim3 grid((a->kv_len + ab::BKV - 1) / ab::BKV, a->heads, a->batches);
-  if (kv_lens != nullptr) {
-    dev.kv_lens = kv_lens;
-    NS2_CUDA_CHECK(set_max_smem_once(attn_bwd_kernel<false, true>, ab::SMEM_BYTES));
-    attn_bwd_kernel<false, true><<<grid, ab::THREADS, ab::SMEM_BYTES, stream>>>(dev);
-  } else if (!dropout) {
-    NS2_CUDA_CHECK(set_max_smem_once(attn_bwd_kernel<false, false>, ab::SMEM_BYTES));
-    attn_bwd_kernel<false, false><<<grid, ab::THREADS, ab::SMEM_BYTES, stream>>>(dev);
-  } else {
-    dev.drop = drop;
-    NS2_CUDA_CHECK(set_max_smem_once(attn_bwd_kernel<true, false>, ab::SMEM_BYTES_DROPOUT));
-    attn_bwd_kernel<true, false><<<grid, ab::THREADS, ab::SMEM_BYTES_DROPOUT, stream>>>(dev);
-  }
-  return launched(2);
-}
-
-extern "C" int ns2_attn_bwd(const ns2_attn_bwd_args* a, ns2_stream_t stream) {
-  return ns2_attn_bwd_kv_lens(a, nullptr, stream);
+  dev.kv_lens = a->kv_lens;
+  if (a->kv_lens != nullptr) return launch<false, true>(dev, grid, stream);
+  if (!dropout) return launch<false, false>(dev, grid, stream);
+  dev.drop = drop;
+  return launch<true, false>(dev, grid, stream);
 }

@@ -274,7 +274,7 @@ __global__ void __launch_bounds__(256) group_sum_kernel(const uint32_t* __restri
 }
 
 // d pred = coef[b] * (pred - target) -> fp32 residual-stream gradient seed and its bf16 copy  (MSE backward, ns2.py:1646-1666)
-// With lens (ns2_mse_bwd_lens): elements past sample b's first lens[b] rows of row4 float4s are written as exact zeros
+// With lens: elements past sample b's first lens[b] rows of row4 float4s are written as exact zeros
 // (pred / target are not read there).
 __global__ void __launch_bounds__(256) mse_bwd_kernel(const float4* __restrict__ pred, const float4* __restrict__ target,
                                                       const float* __restrict__ coef, long long per4,
@@ -456,16 +456,10 @@ extern "C" int ns2_group_sum_bf16(const void* t_bf16, int64_t rows, int32_t dim,
 }
 
 extern "C" int ns2_mse_bwd(const float* pred, const float* target, const float* coef, int32_t batch, int64_t per_sample,
-                           void* out_bf16, float* out_f32, ns2_stream_t stream_) {
-  return ns2_mse_bwd_lens(pred, target, coef, batch, per_sample, out_bf16, out_f32, per_sample, nullptr, stream_);
-}
-
-extern "C" int ns2_mse_bwd_lens(const float* pred, const float* target, const float* coef, int32_t batch,
-                                int64_t per_sample, void* out_bf16, float* out_f32, int64_t row_elems,
-                                const int32_t* lens, ns2_stream_t stream_) {
+                           void* out_bf16, float* out_f32, int64_t row_elems, const int32_t* lens, ns2_stream_t stream_) {
   NS2_REQUIRE(pred && target && coef && (out_bf16 || out_f32) && batch > 0 && per_sample % 4 == 0, "mse_bwd: bad arguments");
   NS2_REQUIRE(lens == nullptr || (row_elems > 0 && row_elems % 4 == 0 && per_sample % row_elems == 0),
-              "mse_bwd_lens: row_elems=%lld must be a positive multiple of 4 dividing per_sample=%lld",
+              "mse_bwd: row_elems=%lld must be a positive multiple of 4 dividing per_sample=%lld",
               static_cast<long long>(row_elems), static_cast<long long>(per_sample));
   const long long row4 = lens == nullptr ? 0 : row_elems / 4;
   const int rows = lens == nullptr ? 0 : static_cast<int>(per_sample / row_elems);

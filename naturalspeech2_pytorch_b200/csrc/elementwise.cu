@@ -62,8 +62,8 @@ __device__ __forceinline__ void rmsnorm_row(const float4 (&v)[VEC], long long ro
 // RMSNorm (+gamma) (+FiLM): one warp per row, the row stays in registers between the reduction and the
 // scaled write (single HBM read of x, single write of the result).  DIM = 32 * 4 * VEC.
 // ------------------------------------------------------------------------------------------------
-// LENS (ns2_rmsnorm_film_lens): row r of batch b = r / rows_per_batch is live iff r % rows_per_batch < lens[b] (clamped
-// to [1, rows_per_batch]); rows that are not live are neither read nor written.
+// LENS (lens != NULL): row r of batch b = r / rows_per_batch is live iff r % rows_per_batch < lens[b] (clamped to
+// [1, rows_per_batch]); rows that are not live are neither read nor written.
 __device__ __forceinline__ bool rmsnorm_row_live(long long row, int rows_per_batch, const int* __restrict__ lens) {
   const long long b = row / rows_per_batch;
   return row - b * rows_per_batch < min(max(__ldg(lens + b), 1), rows_per_batch);
@@ -379,8 +379,8 @@ __global__ void __launch_bounds__(256) q_sample_kernel(const float4* __restrict_
 }
 
 // per-sample mean squared error; deterministic two-level reduction (fixed grid, no atomics on floats).
-// With lens (ns2_mse_rows_lens) sample b covers its first lens[b] rows of row4 float4s: the same grid-stride walk over
-// those elements as a call on the unpadded sample, so the partial sums and the mean are bit-identical to it.
+// With lens, sample b covers its first lens[b] rows of row4 float4s: the same grid-stride walk over those elements as a
+// call on the unpadded sample, so the partial sums and the mean are bit-identical to it.
 constexpr int kMseBlocks = 64;
 __device__ __forceinline__ long long mse_count4(const int* __restrict__ lens, int b, long long row4, int rows,
                                                 long long per4) {
@@ -765,20 +765,12 @@ int ns2_embedding_bf16(const int64_t* ids, int64_t rows, const float* table, int
   return launched(1);
 }
 
-int ns2_rmsnorm_film(const float* x, int64_t x_row_stride, int64_t rows, int32_t dim,
-                     int32_t rows_per_batch, const float* gamma, const float* film,
-                     int64_t film_batch_stride, void* out_bf16, int64_t out_row_stride,
-                     ns2_stream_t stream) {
-  return ns2_rmsnorm_film_lens(x, x_row_stride, rows, dim, rows_per_batch, gamma, film, film_batch_stride, out_bf16,
-                               out_row_stride, nullptr, stream);
-}
-
-int ns2_rmsnorm_film_lens(const float* x, int64_t x_row_stride, int64_t rows, int32_t dim, int32_t rows_per_batch,
-                          const float* gamma, const float* film, int64_t film_batch_stride, void* out_bf16,
-                          int64_t out_row_stride, const int32_t* lens, ns2_stream_t stream) {
+int ns2_rmsnorm_film(const float* x, int64_t x_row_stride, int64_t rows, int32_t dim, int32_t rows_per_batch,
+                     const float* gamma, const float* film, int64_t film_batch_stride, void* out_bf16,
+                     int64_t out_row_stride, const int32_t* lens, ns2_stream_t stream) {
   NS2_REQUIRE(rows_per_batch > 0, "rmsnorm_film: rows_per_batch must be positive");
   NS2_REQUIRE(lens == nullptr || rows % rows_per_batch == 0,
-              "rmsnorm_film_lens: rows=%lld is not a whole number of batches of %d rows", static_cast<long long>(rows),
+              "rmsnorm_film: rows=%lld is not a whole number of batches of %d rows", static_cast<long long>(rows),
               rows_per_batch);
   return launch_rmsnorm<true>(x, x_row_stride, rows, dim, rows_per_batch, gamma, film,
                               film_batch_stride, out_bf16, out_row_stride,
@@ -888,17 +880,12 @@ int ns2_q_sample(const float* x0, const float* noise, const float* alpha, const 
   return launched(1);
 }
 
-int ns2_mse_rows(const float* pred, const float* target, int32_t batch, int64_t per_sample,
-                 float* partial, float* out, float* mean_out, ns2_stream_t stream) {
-  return ns2_mse_rows_lens(pred, target, batch, per_sample, partial, out, mean_out, per_sample, nullptr, stream);
-}
-
-int ns2_mse_rows_lens(const float* pred, const float* target, int32_t batch, int64_t per_sample, float* partial,
-                      float* out, float* mean_out, int64_t row_elems, const int32_t* lens, ns2_stream_t stream) {
+int ns2_mse_rows(const float* pred, const float* target, int32_t batch, int64_t per_sample, float* partial,
+                 float* out, float* mean_out, int64_t row_elems, const int32_t* lens, ns2_stream_t stream) {
   NS2_REQUIRE(pred && target && out && partial, "mse_rows: NULL pointer");
   NS2_REQUIRE(per_sample % 4 == 0 && batch > 0, "mse_rows: bad sizes");
   NS2_REQUIRE(lens == nullptr || (row_elems > 0 && row_elems % 4 == 0 && per_sample % row_elems == 0),
-              "mse_rows_lens: row_elems=%lld must be a positive multiple of 4 dividing per_sample=%lld",
+              "mse_rows: row_elems=%lld must be a positive multiple of 4 dividing per_sample=%lld",
               static_cast<long long>(row_elems), static_cast<long long>(per_sample));
   const long long row4 = lens == nullptr ? 0 : row_elems / 4;
   const int rows = lens == nullptr ? 0 : static_cast<int>(per_sample / row_elems);

@@ -318,10 +318,10 @@ __device__ __forceinline__ void wgmma_tile_k16(float (&d)[BN / 2], uint64_t da, 
   else wgmma_bf16_ss_n128<0, 0>(d, da, db, 1);
 }
 
-// gemm_kernel<BN, NACC, EPI, true>: the length-aware variant of ns2_gemm_row_lens.  Before the roles split, the first
-// a_batches threads copy row_lens into shared memory by cp.async (the kernels read no global memory through the
-// register path, see tests/test_gemm_epilogue_loads_cpu.py) and thread 0 forms the m-tile prefix sums; every role then
-// walks the same compacted tile list (decode_tile_lens).  A tile is computed and stored exactly as by the plain kernel.
+// gemm_kernel<BN, NACC, EPI, true>: ns2_gemm with row_lens.  Before the roles split, the first a_batches threads copy
+// row_lens into shared memory by cp.async (the kernels read no global memory through the register path, see
+// tests/test_gemm_epilogue_loads_cpu.py) and thread 0 forms the m-tile prefix sums; every role then walks the same
+// compacted tile list (decode_tile_lens).  A tile is computed and stored exactly as by the plain kernel.
 template <int BN, int NACC, int EPI, bool LENS = false>
 __global__ void __launch_bounds__(GemmCfg<BN, NACC>::THREADS, 1) gemm_kernel(const __grid_constant__ GemmDev p) {
   using Cfg = GemmCfg<BN, NACC>;
@@ -485,14 +485,12 @@ static int launch_gemm(const GemmDev& dev, cudaStream_t stream) {
 
 }  // namespace ns2
 
-extern "C" int ns2_gemm(const ns2_gemm_args* a, ns2_stream_t stream) { return ns2_gemm_row_lens(a, nullptr, stream); }
-
-extern "C" int ns2_gemm_row_lens(const ns2_gemm_args* a, const int32_t* row_lens, ns2_stream_t stream_) {
+extern "C" int ns2_gemm(const ns2_gemm_args* a, ns2_stream_t stream_) {
   using namespace ns2;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   NS2_REQUIRE(a != nullptr, "ns2_gemm: args is NULL");
-  NS2_REQUIRE(row_lens == nullptr || (a->a_batches >= 1 && a->a_batches <= NS2_GEMM_ROW_LENS_MAX_BATCHES),
-              "ns2_gemm_row_lens: a_batches=%d, row lengths take 1 to %d batches", a->a_batches,
+  NS2_REQUIRE(a->row_lens == nullptr || (a->a_batches >= 1 && a->a_batches <= NS2_GEMM_ROW_LENS_MAX_BATCHES),
+              "ns2_gemm: a_batches=%d, row lengths take 1 to %d batches", a->a_batches,
               NS2_GEMM_ROW_LENS_MAX_BATCHES);
   NS2_REQUIRE(a->A && a->B && a->out, "ns2_gemm: A, B and out must be non-NULL");
   NS2_REQUIRE(a->groups >= 1 && a->groups <= NS2_GEMM_MAX_GROUPS, "ns2_gemm: groups=%d out of range",
@@ -601,7 +599,7 @@ extern "C" int ns2_gemm_row_lens(const ns2_gemm_args* a, const int32_t* row_lens
   NS2_REQUIRE(dev.act == 0 || a->epilogue == NS2_EPI_BF16 || a->epilogue == NS2_EPI_F32,
               "ns2_gemm: NS2_GEMM_FLAG_SILU only applies to the BF16 / F32 epilogues");
   dev.skip_epilogue = (a->flags & NS2_GEMM_FLAG_SKIP_EPILOGUE) ? 1 : 0;
-  dev.row_lens = row_lens;
+  dev.row_lens = a->row_lens;
   dev.batches = a->a_batches;
 
   switch (a->epilogue) {

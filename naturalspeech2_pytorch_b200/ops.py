@@ -158,7 +158,8 @@ def gemm(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, n: int, epilogu
     args.film = _ptr(film)
     args.film_group_stride = film_group_stride
     args.flags = int(flags)
-    check(lib.ns2_gemm_row_lens(C.byref(args), lens_ptr, _stream()), "ns2_gemm_row_lens")
+    args.row_lens = lens_ptr
+    check(lib.ns2_gemm(C.byref(args), _stream()), "ns2_gemm")
     return out
 
 
@@ -360,10 +361,10 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tens
     args.batches, args.heads = q.shape[0], heads
     args.q_len, args.kv_len, args.dim_head = q.shape[1], k.shape[1], 64
     args.scale = float(scale if scale is not None else 64 ** -0.5)
-    args.lse, args.kv_lens = _ptr(lse), lens_ptr
+    args.lse, args.kv_lens, args.q_lens = _ptr(lse), lens_ptr, q_lens_ptr
     d = _dropout_args(dropout)
     args.dropout = None if d is None else C.pointer(d)
-    check(lib.ns2_attn_fwd_q_lens(C.byref(args), q_lens_ptr, _stream()), "ns2_attn_fwd_q_lens")
+    check(lib.ns2_attn_fwd(C.byref(args), _stream()), "ns2_attn_fwd")
     return out
 
 
@@ -383,8 +384,8 @@ def rmsnorm_film(x: torch.Tensor, out: torch.Tensor, *, gamma: Optional[torch.Te
            ("film", film, F32, (B, None), LAST), ("lens", lens, I32, (B,), DENSE))
     lens_ptr = _check_lens(lens, 1, N, "lens")
     film_bs = 0 if film is None else film.stride(0)
-    check(lib.ns2_rmsnorm_film_lens(x.data_ptr(), D, B * N, D, N, _ptr(gamma), _ptr(film), film_bs,
-                                    out.data_ptr(), D, lens_ptr, _stream()), "ns2_rmsnorm_film_lens")
+    check(lib.ns2_rmsnorm_film(x.data_ptr(), D, B * N, D, N, _ptr(gamma), _ptr(film), film_bs,
+                               out.data_ptr(), D, lens_ptr, _stream()), "ns2_rmsnorm_film")
     return out
 
 
@@ -602,8 +603,8 @@ def mse_rows(pred, target, out, scratch=None, mean_out=None, lens=None):
            ("out", out, F32, (B,), DENSE), ("scratch", scratch, F32, None, DENSE), ("mean_out", mean_out, F32, None, DENSE),
            ("lens", lens, I32, (B,), DENSE))
     rows, lp = _rows_lens(pred, lens)
-    check(lib.ns2_mse_rows_lens(pred.data_ptr(), target.data_ptr(), B, n // B, scratch.data_ptr(),
-                                out.data_ptr(), _ptr(mean_out), n // B // rows, lp, _stream()), "ns2_mse_rows_lens")
+    check(lib.ns2_mse_rows(pred.data_ptr(), target.data_ptr(), B, n // B, scratch.data_ptr(),
+                           out.data_ptr(), _ptr(mean_out), n // B // rows, lp, _stream()), "ns2_mse_rows")
     return out
 
 
@@ -801,7 +802,8 @@ def attention_bwd(q, k, v, o, d_o, lse, dq_accum, dk, dv, *, heads: int, scale: 
     a.scale = float(scale if scale is not None else 64 ** -0.5)
     d = _dropout_args(dropout)
     a.dropout = None if d is None else C.pointer(d)
-    check(lib.ns2_attn_bwd_kv_lens(C.byref(a), lens_ptr, _stream()), "ns2_attn_bwd_kv_lens")
+    a.kv_lens = lens_ptr
+    check(lib.ns2_attn_bwd(C.byref(a), _stream()), "ns2_attn_bwd")
     return dq_accum, dk, dv
 
 
@@ -892,8 +894,8 @@ def mse_bwd(pred, target, coef, out_bf=None, out_f32=None, lens=None):
            ("out_bf", out_bf, BF16, None, DENSE, 8), ("out_f32", out_f32, F32, None, DENSE, 16),
            ("lens", lens, I32, (B,), DENSE))
     rows, lp = _rows_lens(pred, lens)
-    check(lib.ns2_mse_bwd_lens(pred.data_ptr(), target.data_ptr(), coef.data_ptr(), B, n // B, _ptr(out_bf),
-                               _ptr(out_f32), n // B // rows, lp, _stream()), "ns2_mse_bwd_lens")
+    check(lib.ns2_mse_bwd(pred.data_ptr(), target.data_ptr(), coef.data_ptr(), B, n // B, _ptr(out_bf),
+                          _ptr(out_f32), n // B // rows, lp, _stream()), "ns2_mse_bwd")
     return out_bf if out_bf is not None else out_f32
 
 

@@ -82,15 +82,20 @@ def test_rvq_rejects_unsupported_codebook_size_before_launch(lib, k):
 
 
 def test_struct_layout_matches_header():
-    """ctypes mirrors of the C structs: sizes are what a C compiler produces for include/ns2_b200.h."""
+    """ctypes mirrors of the C structs: sizes, and the offsets of the optional pointer fields, are what a C compiler
+    produces for include/ns2_b200.h (equal sizes alone would not catch two pointers swapped)."""
     import subprocess, tempfile, textwrap
     from naturalspeech2_pytorch_b200._lib import GemmArgs, AttnArgs, AttnBwdArgs, GemmSeg
     src = textwrap.dedent('''
+        #include <stddef.h>
         #include <stdio.h>
         #include "ns2_b200.h"
         int main(void) {
           printf("%zu %zu %zu %zu\\n", sizeof(ns2_gemm_seg), sizeof(ns2_gemm_args), sizeof(ns2_attn_args),
                  sizeof(ns2_attn_bwd_args));
+          printf("%zu %zu %zu %zu %zu %zu\\n", offsetof(ns2_gemm_args, row_lens), offsetof(ns2_attn_args, kv_lens),
+                 offsetof(ns2_attn_args, dropout), offsetof(ns2_attn_args, q_lens),
+                 offsetof(ns2_attn_bwd_args, dropout), offsetof(ns2_attn_bwd_args, kv_lens));
           return 0;
         }
     ''')
@@ -101,7 +106,9 @@ def test_struct_layout_matches_header():
         subprocess.run(["gcc", "-I", str(ROOT / "include"), str(c), "-o", str(exe)], check=True)
         out = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()
     assert [int(v) for v in out] == [ctypes.sizeof(GemmSeg), ctypes.sizeof(GemmArgs), ctypes.sizeof(AttnArgs),
-                                     ctypes.sizeof(AttnBwdArgs)]
+                                     ctypes.sizeof(AttnBwdArgs),
+                                     GemmArgs.row_lens.offset, AttnArgs.kv_lens.offset, AttnArgs.dropout.offset,
+                                     AttnArgs.q_lens.offset, AttnBwdArgs.dropout.offset, AttnBwdArgs.kv_lens.offset]
 
 
 def test_ops_reject_cpu_tensors():

@@ -86,7 +86,7 @@ def test_entry_points_reject_bad_p_before_launch(lib):
     assert lib.ns2_launch_count() == before
 
 
-def test_dropout_struct_matches_header():
+def test_dropout_struct_and_abi_version_match_header():
     from naturalspeech2_pytorch_b200._lib import Dropout
     src = textwrap.dedent('''
         #include <stddef.h>
@@ -105,7 +105,7 @@ def test_dropout_struct_matches_header():
         subprocess.run(["gcc", "-I", str(ROOT / "include"), str(c), "-o", str(exe)], check=True)
         out = [int(v) for v in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
     assert out[:4] == [ctypes.sizeof(Dropout), Dropout.seed.offset, Dropout.site.offset, Dropout.p.offset]
-    assert out[4] == 8
+    assert out[4] == 9
 
 
 def test_train_dropout_defaults_off_and_conditioner_plumbs_it():

@@ -1,9 +1,10 @@
 """CPU: the C entry points and Python front ends of per-sample latent lengths refuse malformed calls before any launch,
 and the length-aware GEMM instantiations keep the epilogue's load discipline.
 
-- ns2_gemm_row_lens, ns2_attn_fwd_q_lens, ns2_rmsnorm_film_lens, ns2_mse_rows_lens and ns2_mse_bwd_lens are declared in include/ns2_b200.h, bound in `_lib`
-  and exported by the library; NULL arguments, a batch over NS2_GEMM_ROW_LENS_MAX_BATCHES and q_lens with dropout are
-  refused with nothing launched.
+- include/ns2_b200.h declares the lengths where the other optional inputs live: `row_lens` in ns2_gemm_args, `q_lens`
+  in ns2_attn_args and a trailing `lens` argument of ns2_rmsnorm_film, ns2_mse_rows and ns2_mse_bwd; no `_lens` twin
+  of an entry point is declared, bound or exported.  NULL arguments, a batch over NS2_GEMM_ROW_LENS_MAX_BATCHES and
+  q_lens with dropout are refused with nothing launched.
 - `ops.gemm(row_lens=)`, `ops.attention(q_lens=)`, `ops.rmsnorm_film(lens=)`, `ops.mse_rows(lens=)` and
   `ops.mse_bwd(lens=)` reject lengths of the wrong dtype or shape before the device check, `Model.forward(lengths=)`
   rejects batches over the cap, and `NaturalSpeech2.forward(latent_lens=)` refuses raw audio and the RVQ
@@ -22,7 +23,10 @@ import torch
 from naturalspeech2_pytorch_b200 import _lib, build as _build, ops
 
 ROOT = Path(__file__).resolve().parent.parent
-NEW = ["ns2_gemm_row_lens", "ns2_attn_fwd_q_lens", "ns2_rmsnorm_film_lens", "ns2_mse_rows_lens", "ns2_mse_bwd_lens"]
+# the entry points' former length-taking twins (entry point + suffix)
+TWINS = [entry + suffix for entry, suffix in [("ns2_gemm", "_row_lens"), ("ns2_attn_fwd", "_q_lens"),
+                                              ("ns2_attn_bwd", "_kv_lens"), ("ns2_rmsnorm_film", "_lens"),
+                                              ("ns2_mse_rows", "_lens"), ("ns2_mse_bwd", "_lens")]]
 
 
 @pytest.fixture(scope="module")
@@ -31,39 +35,56 @@ def lib():
     return _lib.load()
 
 
-def test_entry_points_are_declared_bound_and_exported(lib):
+def _struct(header, name):
+    return re.search(rf"typedef struct {name} \{{([^}}]*)\}} {name};", header).group(1)
+
+
+def test_lengths_are_fields_or_trailing_arguments_of_the_entry_points(lib):
     header = (ROOT / "include" / "ns2_b200.h").read_text()
-    for name in NEW:
-        assert re.search(rf"\bint {name}\(", header), name
-        assert name in _lib.SIGNATURES, name
+    assert re.search(r"\bconst int32_t\* row_lens;", _struct(header, "ns2_gemm_args"))
+    assert re.search(r"\bconst int32_t\* q_lens;", _struct(header, "ns2_attn_args"))
+    assert "row_lens" in dict(_lib.GemmArgs._fields_) and "q_lens" in dict(_lib.AttnArgs._fields_)
+    for name, tail in [("ns2_rmsnorm_film", r"const int32_t\* lens"),
+                       ("ns2_mse_rows", r"int64_t row_elems, const int32_t\* lens"),
+                       ("ns2_mse_bwd", r"int64_t row_elems, const int32_t\* lens")]:
+        assert re.search(rf"\bint {name}\([^;]*{tail},\s+ns2_stream_t stream\);", header), name
+        params = re.sub(r"/\*.*?\*/", "", re.search(rf"\bint {name}\(([^;]*)\);", header).group(1), flags=re.S)
+        assert len(_lib.SIGNATURES[name][1]) == len(params.split(",")), name
         assert getattr(lib, name) is not None
+    assert not re.findall(r"\b(ns2_\w+_lens)\s*\(", header)
+    assert not [name for name in _lib.SIGNATURES if name.endswith("_lens")]
+    for name in TWINS:
+        assert not re.search(rf"\b{name}\b", header), name
+        assert name not in _lib.SIGNATURES, name
+        assert not hasattr(lib, name), name
     assert re.search(rf"#define NS2_GEMM_ROW_LENS_MAX_BATCHES {_lib.NS2_GEMM_ROW_LENS_MAX_BATCHES}\b", header)
 
 
-def test_null_and_malformed_calls_are_refused(lib):
+def test_length_calls_refuse_null_and_malformed_arguments(lib):
     before = lib.ns2_launch_count()
     lens = (ctypes.c_int32 * 4)(1, 2, 3, 4)
-    assert lib.ns2_gemm_row_lens(None, lens, None) < 0
-    a = _lib.GemmArgs(a_batches=1)
-    assert lib.ns2_gemm_row_lens(ctypes.byref(a), lens, None) < 0               # NULL A / B / out
+    lens_ptr = ctypes.addressof(lens)
+    assert lib.ns2_gemm(None, None) < 0
+    a = _lib.GemmArgs(a_batches=1, row_lens=lens_ptr)
+    assert lib.ns2_gemm(ctypes.byref(a), None) < 0                              # NULL A / B / out
     assert b"non-NULL" in lib.ns2_last_error()
     a.A = a.B = a.out = 16
     a.a_batches = _lib.NS2_GEMM_ROW_LENS_MAX_BATCHES + 1
-    assert lib.ns2_gemm_row_lens(ctypes.byref(a), lens, None) < 0
+    assert lib.ns2_gemm(ctypes.byref(a), None) < 0
     assert b"batches" in lib.ns2_last_error()
-    assert lib.ns2_attn_fwd_q_lens(None, lens, None) < 0
-    assert lib.ns2_attn_fwd_q_lens(ctypes.byref(_lib.AttnArgs()), lens, None) < 0   # NULL q / k / v / out
+    assert lib.ns2_attn_fwd(None, None) < 0
+    assert lib.ns2_attn_fwd(ctypes.byref(_lib.AttnArgs(q_lens=lens_ptr)), None) < 0   # NULL q / k / v / out
     d = _lib.Dropout(1, 0, 0.5)
     t = _lib.AttnArgs(q=16, k=16, v=16, out=16, batches=1, heads=1, q_len=8, kv_len=8, dim_head=64,
-                      dropout=ctypes.pointer(d))
-    assert lib.ns2_attn_fwd_q_lens(ctypes.byref(t), lens, None) < 0
+                      dropout=ctypes.pointer(d), q_lens=lens_ptr)
+    assert lib.ns2_attn_fwd(ctypes.byref(t), None) < 0
     assert b"q_lens" in lib.ns2_last_error()
-    assert lib.ns2_rmsnorm_film_lens(None, 128, 8, 128, 4, None, None, 0, None, 128, lens, None) < 0
-    assert lib.ns2_rmsnorm_film_lens(16, 128, 9, 128, 4, None, None, 0, 16, 128, lens, None) < 0   # 9 rows, 4 per batch
-    assert lib.ns2_mse_rows_lens(None, 16, 2, 64, 16, 16, None, 32, lens, None) < 0
-    assert lib.ns2_mse_rows_lens(16, 16, 2, 64, 16, 16, None, 24, lens, None) < 0     # 24 does not divide 64
-    assert lib.ns2_mse_bwd_lens(16, 16, 16, 2, 64, None, None, 32, lens, None) < 0    # no output
-    assert lib.ns2_mse_bwd_lens(16, 16, 16, 2, 64, None, 16, 6, lens, None) < 0       # row not a multiple of 4
+    assert lib.ns2_rmsnorm_film(None, 128, 8, 128, 4, None, None, 0, None, 128, lens, None) < 0
+    assert lib.ns2_rmsnorm_film(16, 128, 9, 128, 4, None, None, 0, 16, 128, lens, None) < 0   # 9 rows, 4 per batch
+    assert lib.ns2_mse_rows(None, 16, 2, 64, 16, 16, None, 32, lens, None) < 0
+    assert lib.ns2_mse_rows(16, 16, 2, 64, 16, 16, None, 24, lens, None) < 0     # 24 does not divide 64
+    assert lib.ns2_mse_bwd(16, 16, 16, 2, 64, None, None, 32, lens, None) < 0    # no output
+    assert lib.ns2_mse_bwd(16, 16, 16, 2, 64, None, 16, 6, lens, None) < 0       # row not a multiple of 4
     assert lib.ns2_launch_count() == before
 
 

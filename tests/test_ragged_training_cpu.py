@@ -18,32 +18,34 @@ def lib():
     return _lib.load()
 
 
-def test_entry_point_is_declared_and_bound(lib):
+def test_attn_bwd_args_carry_kv_lens(lib):
     from naturalspeech2_pytorch_b200 import _lib
     header = (ROOT / "include" / "ns2_b200.h").read_text()
-    assert re.search(r"int ns2_attn_bwd_kv_lens\(const ns2_attn_bwd_args\* args, const int32_t\* kv_lens, "
-                     r"ns2_stream_t stream\);", header)
-    assert "ns2_attn_bwd_kv_lens" in _lib.SIGNATURES
-    assert hasattr(lib, "ns2_attn_bwd_kv_lens")
+    fields = re.search(r"typedef struct ns2_attn_bwd_args \{([^}]*)\} ns2_attn_bwd_args;", header).group(1)
+    assert re.search(r"\bconst int32_t\* kv_lens;", fields)
+    assert "kv_lens" in dict(_lib.AttnBwdArgs._fields_)
+    assert re.search(r"int ns2_attn_bwd\(const ns2_attn_bwd_args\* args, ns2_stream_t stream\);", header)
+    assert _lib.SIGNATURES["ns2_attn_bwd"][1][0] is ctypes.POINTER(_lib.AttnBwdArgs)
+    assert hasattr(lib, "ns2_attn_bwd")
 
 
-def test_entry_point_rejects_null_arguments(lib):
+def test_attn_bwd_with_kv_lens_rejects_null_arguments(lib):
     from naturalspeech2_pytorch_b200._lib import AttnBwdArgs
     before = lib.ns2_launch_count()
-    assert lib.ns2_attn_bwd_kv_lens(None, 16, None) < 0
+    assert lib.ns2_attn_bwd(None, None) < 0
     assert b"NULL" in lib.ns2_last_error()
-    assert lib.ns2_attn_bwd_kv_lens(ctypes.byref(AttnBwdArgs()), 16, None) < 0      # NULL q / k / v / ...
+    assert lib.ns2_attn_bwd(ctypes.byref(AttnBwdArgs(kv_lens=16)), None) < 0      # NULL q / k / v / ...
     assert b"NULL" in lib.ns2_last_error()
-    assert lib.ns2_attn_bwd_kv_lens(ctypes.byref(AttnBwdArgs()), None, None) < 0    # = ns2_attn_bwd
+    assert lib.ns2_attn_bwd(ctypes.byref(AttnBwdArgs()), None) < 0                # without kv_lens
     assert lib.ns2_launch_count() == before
 
 
-def test_kv_lens_with_dropout_is_refused(lib):
+def test_attn_bwd_refuses_kv_lens_with_dropout(lib):
     from naturalspeech2_pytorch_b200 import ops
     from naturalspeech2_pytorch_b200._lib import AttnBwdArgs, Dropout
     before = lib.ns2_launch_count()
     d = Dropout(1, 0, 0.5)
-    assert lib.ns2_attn_bwd_kv_lens(ctypes.byref(AttnBwdArgs(dropout=ctypes.pointer(d))), 16, None) < 0
+    assert lib.ns2_attn_bwd(ctypes.byref(AttnBwdArgs(dropout=ctypes.pointer(d), kv_lens=16)), None) < 0
     assert b"kv_lens" in lib.ns2_last_error()
     B, N = 2, 8
     q = torch.zeros(B, N, 64, dtype=torch.bfloat16)

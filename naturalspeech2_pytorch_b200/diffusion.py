@@ -15,7 +15,6 @@ backward hands d pred to the denoiser's, as the reference's autograd does.
 from __future__ import annotations
 
 import math
-from collections import OrderedDict
 from functools import partial
 from typing import Callable, Optional
 
@@ -97,7 +96,6 @@ class NaturalSpeech2(nn.Module):
         self.duration_loss_weight, self.pitch_loss_weight = duration_loss_weight, pitch_loss_weight   # ns2.py:1193-1194
         self.conditioner = conditioner
         self.cuda_graphs = cuda_graphs  # sampling loop: replay one captured CUDA graph per sampling step
-        self._sampler_graphs = OrderedDict()
         self.conditioning_kwargs = conditioning_kwargs  # accepted for signature parity (encoder hyper-parameters)
 
     @property
@@ -128,60 +126,37 @@ class NaturalSpeech2(nn.Module):
     def _sampler_entry(self, shape, conditioning, cond_scale, device, lens=None):
         """One captured CUDA graph = one whole sampling step: denoiser forward(s), guidance combine, DDIM update of the
         static latent buffer.  Keyed on shapes (and on whether latent lengths are given) only; conditioning and the
-        lengths are copied into static buffers."""
+        lengths are copied into static buffers.  It replays on the model's workspace, so the model caches it."""
         guided = self.conditional and cond_scale != 1.
         cond_sig = None
         if conditioning is not None:
             cond_sig = tuple(tuple(v.shape) for v in conditioning.values() if torch.is_tensor(v))
-        key = (tuple(shape), cond_sig, float(cond_scale) if guided else None, self.objective, lens is not None,
-               str(device))
-        entry = self._sampler_graphs.get(key)
-        if entry is not None and entry["packed"] is self.model.packed():
-            self._sampler_graphs.move_to_end(key)
-            if lens is not None:
-                entry["lens"].copy_(lens)
-            if conditioning is not None:
-                for k, v in conditioning.items():
-                    if torch.is_tensor(v):
-                        entry["cond"][k].copy_(v)
-            return entry
-        while len(self._sampler_graphs) >= 4:
-            self._sampler_graphs.popitem(last=False)
-        B = shape[0]
-        model = self.model
-        x = torch.empty(shape, device=device, dtype=torch.float32)
-        ts = torch.zeros(B, device=device, dtype=torch.float32)
-        coef = torch.ones(4, B, device=device, dtype=torch.float32)
-        v0 = torch.empty_like(x)
-        v1 = torch.empty_like(x) if guided else None
-        static_cond = None
-        if conditioning is not None:
-            static_cond = type(conditioning)({k: (v.clone() if torch.is_tensor(v) else v)
-                                              for k, v in conditioning.items()})
-        p_cond = 0. if self.conditional else None
-        static_lens = None if lens is None else lens.clone()
+        key = ("sample", tuple(shape), cond_sig, float(cond_scale) if guided else None, self.objective,
+               lens is not None, str(device))
+        model, B = self.model, shape[0]
 
-        def step():
-            model._forward_impl(x, ts, None, None, None, p_cond, static_cond, v0, lengths=static_lens)
-            if guided:   # classifier-free guidance (ns2.py:914-927): conditional + null forward, lerp
-                model._forward_impl(x, ts, None, None, None, 1., static_cond, v1, lengths=static_lens)
-                ops.cfg_combine(v0, v1, cond_scale, v0)
-            ops.ddim_step(x, v0, coef[0], coef[1], coef[2], coef[3], objective=self.objective)
+        def build(cond):
+            x = torch.empty(shape, device=device, dtype=torch.float32)
+            ts = torch.zeros(B, device=device, dtype=torch.float32)
+            coef = torch.ones(4, B, device=device, dtype=torch.float32)
+            v0 = torch.empty_like(x)
+            v1 = torch.empty_like(x) if guided else None
+            p_cond = 0. if self.conditional else None
+            static_lens = None if lens is None else lens.clone()
 
-        x.normal_()
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):   # warm-up outside capture (workspaces, packing)
-            step()
-        torch.cuda.current_stream().wait_stream(side)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph, capture_error_mode="thread_local"):
-            step()
-        # the entry owns every buffer the graph reads or writes: v0 / v1 are written by each replay, and a buffer freed
-        # here would go back to the caching allocator while the graph still writes the prediction into it
-        entry = {"graph": graph, "x": x, "ts": ts, "coef": coef, "v": (v0, v1), "cond": static_cond,
-                 "lens": static_lens, "packed": model.packed()}
-        self._sampler_graphs[key] = entry
+            def step():
+                model._forward_impl(x, ts, cond_drop_prob=p_cond, _conditioning=cond, out=v0, lengths=static_lens)
+                if guided:   # classifier-free guidance (ns2.py:914-927): conditional + null forward, lerp
+                    model._forward_impl(x, ts, cond_drop_prob=1., _conditioning=cond, out=v1, lengths=static_lens)
+                    ops.cfg_combine(v0, v1, cond_scale, v0)
+                ops.ddim_step(x, v0, coef[0], coef[1], coef[2], coef[3], objective=self.objective)
+
+            x.normal_()
+            return {"x": x, "ts": ts, "coef": coef, "v": (v0, v1), "lens": static_lens}, step
+
+        entry = model._captured(key, model._ws_key(B, shape[1], device), conditioning, build)
+        if lens is not None:
+            entry["lens"].copy_(lens)
         return entry
 
     @torch.no_grad()

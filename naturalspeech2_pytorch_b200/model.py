@@ -98,6 +98,20 @@ def _transpose_conv(w: torch.Tensor, kernel: int) -> torch.Tensor:
     return w.view(O, kernel, -1).permute(2, 1, 0).reshape(-1, kernel * O).contiguous()
 
 
+def _capture(step) -> torch.cuda.CUDAGraph:
+    """Warm `step` up on a side stream (workspaces, packing, lazy CUDA init), then capture it into a CUDA graph."""
+    side = torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        step()
+    torch.cuda.current_stream().wait_stream(side)
+    graph = torch.cuda.CUDAGraph()
+    # thread_local: other threads (e.g. the NCCL watchdog) may touch CUDA while this thread captures
+    with torch.cuda.graph(graph, capture_error_mode="thread_local"):
+        step()
+    return graph
+
+
 def _records_graph(m: nn.Module) -> bool:
     """Whether a call of `m` records its hand-written autograd node: train mode, gradients on, a trainable parameter."""
     return m.training and torch.is_grad_enabled() and any(p.requires_grad for p in m.parameters())
@@ -128,9 +142,10 @@ class _PackedCache(nn.Module):
     def packed(self) -> Dict[str, torch.Tensor]:
         sig = tuple((p.data_ptr(), p._version) for p in self.parameters())
         if self._packed is None or sig != self._packed_sig:
+            self.invalidate_packed()   # and whatever a subclass built on the old packs
             with torch.no_grad():
                 self._packed = self._pack()
-            self._packed_sig, self._packed_T = sig, None
+            self._packed_sig = sig
         return self._packed
 
     def packed_transposed(self) -> Dict[str, torch.Tensor]:
@@ -316,8 +331,8 @@ class Model(_PackedCache):
         self.freeze_packed = False  # set True to skip the per-call parameter-version check (inference loops)
         self._prof = None           # bench.py: list collecting (op name, start event, end event)
         self.use_cuda_graphs = False  # replay one captured CUDA graph per problem shape instead of ~110 launches
-        self._graphs: "OrderedDict[tuple, dict]" = OrderedDict()
-        self.max_cached_shapes = 4  # LRU bound on per-(B, N) workspaces (~1.3 GB each at cfg2) and captured graphs
+        self._graphs: "OrderedDict[tuple, dict]" = OrderedDict()   # `_captured`: model and sampler steps
+        self.max_cached_shapes = 4  # LRU bound on per-(B, N) workspaces (~1.3 GB each at cfg2); graphs: twice that
 
     @property
     def device(self):
@@ -454,15 +469,19 @@ class Model(_PackedCache):
     # ----------------------------------------------------------------------------------------------
     # workspaces (stable addresses per problem shape so a forward can be captured in a CUDA graph)
     # ----------------------------------------------------------------------------------------------
+    @staticmethod
+    def _ws_key(B: int, N: int, dev) -> tuple:
+        return (B, N, str(dev))
+
     def _workspace(self, B: int, N: int, dev) -> Dict[str, torch.Tensor]:
-        key = (B, N, str(dev))
+        key = self._ws_key(B, N, dev)
         ws = self._ws.get(key)
         if ws is not None:
             self._ws.move_to_end(key)
             return ws
         while len(self._ws) >= self.max_cached_shapes:   # LRU: variable-length serving must not grow without bound
             old_key, _ = self._ws.popitem(last=False)
-            for gk in [k for k in self._graphs if k[:2] == old_key[:2] and k[-1] == old_key[-1]]:
+            for gk in [k for k, e in self._graphs.items() if e["ws_key"] == old_key]:
                 del self._graphs[gk]                      # graphs captured on the evicted workspace die with it
         D, G, inner = self.dim, self.wavenet_layers, self.inner
         Dp = _round_up(self.ff_inner, 128)
@@ -483,6 +502,30 @@ class Model(_PackedCache):
                        "xkv": e(B, M, self.depth * 2 * inner)})
         self._ws[key] = ws
         return ws
+
+    def _captured(self, key, ws_key, conditioning, build) -> dict:
+        """The one cache of the CUDA graphs that replay on this model's workspaces (its forward, the sampler's step).
+        The entry for `key` holds "graph" and every buffer the graph reads or writes.  On a miss, `build(cond)` takes
+        the static copy of `conditioning` and returns (buffers, step), and the step is captured on workspace `ws_key`.
+        An entry goes with that workspace, with a repack, or as the least recent of 2 * max_cached_shapes."""
+        self.packed()   # a parameter-version change repacks, which drops every entry
+        entry = self._graphs.get(key)
+        if entry is None:
+            while len(self._graphs) >= 2 * self.max_cached_shapes:
+                self._graphs.popitem(last=False)
+            cond = None
+            if conditioning is not None:   # static copies: the graph must not pin (or depend on) the caller's tensors
+                cond = Conditioning({k: (v.clone() if torch.is_tensor(v) else v) for k, v in conditioning.items()})
+            entry, step = build(cond)
+            entry.update(graph=_capture(step), cond=cond, ws_key=ws_key)
+            self._graphs[key] = entry
+        elif conditioning is not None and (entry["cond_ref"] is None or entry["cond_ref"]() is not conditioning):
+            for k, v in conditioning.items():    # a different (prompt, cond) of the same shapes: refresh the copies
+                if torch.is_tensor(v):
+                    entry["cond"][k].copy_(v)
+        self._graphs.move_to_end(key)
+        entry["cond_ref"] = weakref.ref(conditioning) if isinstance(conditioning, Conditioning) else None
+        return entry
 
     # ----------------------------------------------------------------------------------------------
     # conditioning (timestep-invariant; cache across sampling steps via `precompute_conditioning`)
@@ -667,45 +710,26 @@ class Model(_PackedCache):
 
     def _forward_graphed(self, x, times, p_eff, conditioning, out, lens=None):
         B, N, _ = x.shape
-        self.packed()  # a parameter-version change invalidates the packed weights AND clears self._graphs
+        dev = x.device
         cond_sig = None
         if conditioning is not None:
             cond_sig = tuple(tuple(conditioning[k].shape) for k in ("prompt_cond", "tokens", "cond_proj"))
             cond_sig += (conditioning.get("cond_lens") is not None,)   # a different cond_inject launch
-        # lengths live in a static device buffer: one graph serves every set of lengths of a shape
-        key = (B, N, float(p_eff), cond_sig, lens is not None, str(x.device))
-        entry = self._graphs.get(key)
-        if entry is None:
-            while len(self._graphs) >= 2 * self.max_cached_shapes:
-                self._graphs.popitem(last=False)
-            xs = torch.empty(B, N, self.dim, device=x.device, dtype=torch.float32)
-            ts = torch.empty(B, device=x.device, dtype=torch.float32)
-            static_out = torch.empty(B, N, self.dim, device=x.device, dtype=torch.float32)
+
+        def build(cond):
+            xs = torch.empty(B, N, self.dim, device=dev, dtype=torch.float32)
+            ts = torch.empty(B, device=dev, dtype=torch.float32)
+            static_out = torch.empty(B, N, self.dim, device=dev, dtype=torch.float32)
             static_lens = None if lens is None else lens.clone()
-            static_cond = None
-            if conditioning is not None:   # static copies: the graph must not pin (or depend on) the caller's tensors
-                static_cond = Conditioning({k: (v.clone() if torch.is_tensor(v) else v) for k, v in conditioning.items()})
             xs.copy_(x)
             ts.copy_(times)
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):   # warm-up outside capture: workspaces, packing, lazy CUDA init
-                self._forward_impl(xs, ts, None, None, None, p_eff, static_cond, static_out, lengths=static_lens)
-            torch.cuda.current_stream().wait_stream(side)
-            graph = torch.cuda.CUDAGraph()
-            # thread_local: other threads (e.g. the NCCL watchdog) may touch CUDA while this thread captures
-            with torch.cuda.graph(graph, capture_error_mode="thread_local"):
-                self._forward_impl(xs, ts, None, None, None, p_eff, static_cond, static_out, lengths=static_lens)
-            entry = {"graph": graph, "xs": xs, "ts": ts, "out": static_out, "cond": static_cond, "lens": static_lens,
-                     "cond_ref": weakref.ref(conditioning) if isinstance(conditioning, Conditioning) else None}
-            self._graphs[key] = entry
-        else:
-            self._graphs.move_to_end(key)
-            if conditioning is not None and (entry["cond_ref"] is None or entry["cond_ref"]() is not conditioning):
-                for k, v in conditioning.items():    # a different (prompt, cond) of the same shapes: refresh the copies
-                    if torch.is_tensor(v):
-                        entry["cond"][k].copy_(v)
-                entry["cond_ref"] = weakref.ref(conditioning) if isinstance(conditioning, Conditioning) else None
+            step = lambda: self._forward_impl(xs, ts, cond_drop_prob=p_eff, _conditioning=cond,  # noqa: E731
+                                              out=static_out, lengths=static_lens)
+            return {"xs": xs, "ts": ts, "out": static_out, "lens": static_lens}, step
+
+        # lengths live in a static device buffer: one graph serves every set of lengths of a shape
+        key = (B, N, float(p_eff), cond_sig, lens is not None, str(dev))
+        entry = self._captured(key, self._ws_key(B, N, dev), conditioning, build)
         entry["xs"].copy_(x)
         entry["ts"].copy_(times)
         if lens is not None:

@@ -431,10 +431,11 @@ def test_gpu_schedule_tables_match_reference_coefficients(name):
                 assert torch.equal(c, expected), (name, T)
 
 
-def test_second_configuration_reuses_the_captured_graph():
+def test_second_configuration_reuses_the_model_cached_graph():
     """Swap another schedule and scale (same objective and shape) into a wrapper whose graph is captured: the
-    graph is reused and the sample equals the eager loop of that configuration."""
+    graph in the model's cache is reused and the sample equals the eager loop of that configuration."""
     model = _model("uncond_small")[0]
+    model._graphs.clear()   # the module's models are shared: count this test's captures only
     noise = torch.randn(B_SAMPLE, N_SAMPLE, 128, generator=torch.Generator().manual_seed(32)).cuda()
     ns = _wrapper("sig_v", 7, model, cuda_graphs=True)
     first = _sample(ns, noise, 1., {})
@@ -443,7 +444,7 @@ def test_second_configuration_reuses_the_captured_graph():
         o = _wrapper(other, 7, model, cuda_graphs=False)
         ns.gamma_schedule, ns.scale = o.gamma_schedule, o.scale
         got = _sample(ns, noise, 1., {})
-        assert len(ns._sampler_graphs) == 1
+        assert len(model._graphs) == 1
         assert torch.equal(got, _sample(o, noise, 1., {})), other
         assert not torch.equal(got, first), other
 

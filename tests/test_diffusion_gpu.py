@@ -86,12 +86,12 @@ def test_conditional_requires_conditioning():
     assert out.shape == (2, 160, 128) and torch.isfinite(out).all()
 
 
-def test_sampler_graph_matches_eager_loop():
+def test_sampler_graph_in_the_model_cache_matches_eager_loop():
     """The captured sampling step (forward(s) + guidance + DDIM update in one CUDA graph, schedule tables) gives the
     same latents as the eager per-step loop, for unconditional and guided conditional sampling, whatever the order of
     eager and graph calls on one model, and for the same noise passed as a transposed (B, D, N)-ordered view.  The graph
-    writes only into buffers its sampler owns: memory handed out by the caching allocator after the capture (the
-    sentinels) is never written by a later replay."""
+    writes only into buffers its cache entry owns: memory handed out by the caching allocator after the capture (the
+    sentinels) is never written by a later replay.  The step is the one entry of the model's graph cache."""
     from naturalspeech2_pytorch_b200 import NaturalSpeech2
     for name, kw in (("uncond_small", {}), ("cond_small", dict(cond_scale=2.0))):
         z, kwargs, seed = load_model_golden(name)
@@ -115,7 +115,7 @@ def test_sampler_graph_matches_eager_loop():
         assert all(bool((t == 7.0).all()) for t in sentinels), (name, "a replay wrote into memory it does not own")
         # a second call with other noise reuses the captured graph
         ns.sample(length=160, batch_size=2, **extra, **kw)
-        assert len(ns._sampler_graphs) == 1
+        assert len(model._graphs) == 1
 
 
 def test_loss_with_rvq_cross_entropy_term():

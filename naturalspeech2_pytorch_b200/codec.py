@@ -17,6 +17,7 @@ import torch
 from torch import nn
 
 from . import ops
+from .seanet import frame_lengths
 
 
 class EncodecRVQ(nn.Module):
@@ -59,20 +60,42 @@ class EncodecRVQ(nn.Module):
         return self._prepared
 
     @torch.no_grad()
-    def quantize(self, frames: torch.Tensor, stats: Optional[torch.Tensor] = None):
-        """frames (..., 128) fp32 -> (codes (..., Q) int64, emb (..., 128) fp32 = sum of the chosen codewords)."""
+    def quantize(self, frames: torch.Tensor, stats: Optional[torch.Tensor] = None, *, lengths=None):
+        """frames (..., 128) fp32 -> (codes (..., Q) int64, emb (..., 128) fp32 = sum of the chosen codewords).
+        lengths (B,) (optional, frames (B, N, 128) padded at the end, in [1, N], at most
+        NS2_GEMM_ROW_LENS_MAX_BATCHES samples): sample b's codes and emb past lengths[b] are -1 and exact zeros, and
+        its frames there are not read into any valid output."""
         shp = frames.shape[:-1]
+        host = None
+        if lengths is not None:
+            if frames.dim() != 3:
+                raise ValueError(f"quantize with lengths takes (B, N, 128) frames, got {tuple(frames.shape)}")
+            host = frame_lengths(lengths, frames.shape[0], frames.shape[1], device=frames.device, lo=1)
         if frames.numel() == 0:  # empty batch: nothing to launch (the reference returns empty tensors too)
             return (torch.empty(*shp, self.num_quantizers, dtype=torch.int64, device=frames.device),
                     torch.empty(*shp, 128, dtype=torch.float32, device=frames.device))
-        flat = frames.reshape(-1, 128).float().contiguous()
+        flat = frames.reshape(-1, 128).float()
+        if host is not None:   # zero (a copy of) the padding first: the search then meets only finite frames
+            flat_lens = ops.lengths(host, len(host), None, device=frames.device)
+            flat = ops.mask_rows(flat.clone(memory_format=torch.contiguous_format).view(*shp, 128), flat_lens)
+        flat = flat.reshape(-1, 128).contiguous()
         codes = ops.rvq_encode(flat, self.codebooks, self._prep(), stats=stats)
         emb = ops.rvq_decode(codes, self.codebooks)
-        return codes.view(*shp, self.num_quantizers), emb.view(*shp, 128)
+        codes, emb = codes.view(*shp, self.num_quantizers), emb.view(*shp, 128)
+        if host is not None:
+            ops.mask_rows(emb, flat_lens)
+            codes = codes_past_lengths(codes, host)
+        return codes, emb
 
     @torch.no_grad()
-    def forward(self, x, return_encoded: bool = False, curtail_from_left: bool = False, **kwargs):
-        """Mirror of EncodecWrapper.forward's return convention: (emb (B,N,128), codes (B,N,Q), None)."""
+    def forward(self, x, return_encoded: bool = False, curtail_from_left: bool = False, *, lengths=None,
+                **kwargs):
+        """Mirror of EncodecWrapper.forward's return convention: (emb (B,N,128), codes (B,N,Q), None).
+        lengths (B,) (optional, frames): a batch padded at the end.  For raw audio (B, T), sample b is
+        x[b, :320 lengths[b]], lengths in [seanet.MIN_FRAMES, T // 320]; nothing is curtailed (curtail_from_left is
+        ignored) and the result has T // 320 frames.  Sample b's frames, emb and codes are bit-identical to encoding
+        that waveform alone, and past lengths[b] emb is zero and codes are -1.  For frames (B, N, 128) see
+        `quantize`."""
         if x.ndim == 2:
             if self.encoder is None:
                 raise NotImplementedError(
@@ -80,9 +103,13 @@ class EncodecRVQ(nn.Module):
                     "EncodecRVQ.from_state_dict); pass encoder-output frames (B, N, 128) instead")
             m = self.seq_len_multiple_of
             T = x.shape[-1] // m * m
-            x = x[..., -T:] if curtail_from_left else x[..., :T]
-            x = self.encoder(x)
-        codes, emb = self.quantize(x)
+            if lengths is not None:
+                frame_lengths(lengths, x.shape[0], T // m, device=x.device)   # refuse before the encoder runs
+                x = self.encoder(x[..., :T], lengths=lengths)
+            else:
+                x = x[..., -T:] if curtail_from_left else x[..., :T]
+                x = self.encoder(x)
+        codes, emb = self.quantize(x, lengths=lengths)
         if not return_encoded:
             return codes
         return emb, codes, None
@@ -126,6 +153,19 @@ class EncodecRVQ(nn.Module):
         with torch.no_grad():
             emb = ops.rvq_decode(own, self.codebooks)
         return emb.view(*shp, 128), loss
+
+
+def codes_past_lengths(codes: torch.Tensor, lengths) -> torch.Tensor:
+    """codes (B, N, Q) int64 -> a new contiguous copy whose rows past lengths[b] (host ints in [0, N]) are -1, the
+    `ignore_index` of the RVQ cross-entropy: one `ops.pack_rows` of [codes[b, :len] ; -1 rows], which copies 64-bit
+    words, into rows [0, 2N) of a buffer whose first N rows are the result."""
+    B, N, Q = codes.shape
+    dev = codes.device
+    words = torch.empty(B, 2 * N, Q, dtype=torch.int64, device=dev)
+    fill = torch.full((1, N, Q), -1, dtype=torch.int64, device=dev).view(torch.bfloat16).expand(B, -1, -1)
+    ops.pack_rows(codes.contiguous().view(torch.bfloat16), ops.lengths(lengths, B, N, device=dev, lo=0), fill,
+                  ops.lengths([N - n for n in lengths], B, N, device=dev, lo=0), words.view(torch.bfloat16))
+    return words[:, :N].contiguous()
 
 
 class RqCrossEntropyFunction(torch.autograd.Function):

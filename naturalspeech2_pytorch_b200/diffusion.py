@@ -22,7 +22,8 @@ import torch
 from torch import nn
 
 from . import ops
-from .codec import EncodecRVQ
+from .codec import EncodecRVQ, codes_past_lengths
+from .seanet import frame_lengths
 from .model import Model
 
 
@@ -200,13 +201,31 @@ class NaturalSpeech2(nn.Module):
             ops.ddim_step(audio, v, c[0], c[1], c[2], c[3], objective=self.objective)
         return audio if lens is None else ops.mask_rows(audio, lens)
 
-    def _check_latent_lens_training(self, audio, codes):
+    def _encodes_lengths(self) -> bool:
+        """Whether the codec encodes a padded batch of waveforms with per-sample lengths (an EncodecRVQ with an
+        encoder, e.g. SEANetEncoder)."""
+        return isinstance(self.codec, EncodecRVQ) and self.codec.encoder is not None
+
+    def _encode_prompt(self, prompt, prompt_lens):
+        """A raw-audio prompt batch (B, T) with per-sample lengths (frames) -> its latents (B, T // hop, dim), each
+        sample's bit-identical to encoding its waveform alone and zero past its length.  Anything else is returned
+        as it is."""
+        if prompt is not None and prompt.ndim == 2 and prompt_lens is not None and self._encodes_lengths():
+            prompt, _, _ = self.codec(prompt, return_encoded=True, lengths=prompt_lens)
+        return prompt
+
+    def _check_latent_lens_training(self, audio, codes, latent_lens):
         """Refuse, before any launch, what `forward(latent_lens=)` does not support."""
         if audio.ndim == 2:
-            raise ValueError("latent_lens needs encoded latents (B, N, dim): the codec's encoder takes no lengths")
-        if self.rvq_cross_entropy_loss_weight != 0 and codes is not None:
-            raise NotImplementedError("latent_lens with the RVQ cross-entropy term is not supported (its reduction over "
-                                      "frames has no lengths)")
+            if not self._encodes_lengths():
+                raise ValueError("latent_lens needs encoded latents (B, N, dim) unless the codec is an EncodecRVQ with "
+                                 "an encoder: this codec's encoder takes no lengths")
+            frame_lengths(latent_lens, audio.shape[0], audio.shape[-1] // self.codec.seq_len_multiple_of,
+                          device=audio.device)
+        if self.rvq_cross_entropy_loss_weight != 0 and (codes is not None or audio.ndim == 2) and \
+                not isinstance(self.codec, EncodecRVQ):
+            raise NotImplementedError("latent_lens with the RVQ cross-entropy term needs an EncodecRVQ codec (the -1 "
+                                      "targets past each length are its ignore_index)")
         cn = self.conditioner
         if cn is not None and getattr(cn, "train_duration_pitch", False):
             raise NotImplementedError("latent_lens with train_duration_pitch is not supported")
@@ -234,7 +253,9 @@ class NaturalSpeech2(nn.Module):
         padded at their ends, is sampled as if each sample ran alone with `prompt_lens` (prompt latent frames) and
         `phoneme_lens` (phonemes), given to the conditioner, whose condition lengths then follow; with precomputed
         `prompt_enc=` / `cond=` pass `prompt_lens` and `cond_lens` (condition frames) instead.  With lengths the
-        prompt must be encoded latents (B, Np, dim): a raw-audio prompt would be curtailed by the batch's length.
+        prompt is encoded latents (B, Np, dim), or raw audio (B, T) with `prompt_lens` when the codec is an EncodecRVQ
+        with an encoder: sample b's prompt is then prompt[b, :prompt_lens[b] * hop] (at least 7 frames), encoded as if
+        alone (`EncodecRVQ.forward(lengths=)`).  Other raw-audio prompts would be curtailed by the batch's length.
 
         latent_lens (B,): sample b is `latent_lens[b]` latent frames long (`length` stays the padded length, at most 64
         samples): each returned latent equals sampling that sample alone with length=latent_lens[b] and the first
@@ -249,6 +270,7 @@ class NaturalSpeech2(nn.Module):
         if ragged and not self.conditional:
             raise ValueError("prompt_lens / phoneme_lens / cond_lens apply to conditional models")
         if self.conditional:
+            prompt = self._encode_prompt(prompt, prompt_lens)
             if not (_exists(prompt_enc) and _exists(cond)):
                 if not _exists(self.conditioner):
                     raise NotImplementedError(
@@ -303,23 +325,30 @@ class NaturalSpeech2(nn.Module):
         returned loss, the `aux_loss` of ns2.py:1600-1602 that the reference adds at 1684.
         A batch of prompts and texts of different lengths, padded at their ends, trains as if each sample ran alone with
         `prompt_lens` (prompt latent frames) and `phoneme_lens` (phonemes), given to the conditioner, and prompt_lens to
-        the model; with precomputed `prompt_enc=` / `cond=` only prompt_lens (to the model).  The latents and pitch share
-        one length.  Each sample's MSE row is then that of the sample alone; the loss, as in the reference, is
-        mean(mse) * mean(weight) over the batch (ns2.py:1651-1666), not the mean of the per-sample losses.
+        the model; with precomputed `prompt_enc=` / `cond=` only prompt_lens (to the model).  A raw-audio prompt (B, T)
+        with prompt_lens is encoded with those lengths when the codec is an EncodecRVQ with an encoder, as in `sample`.
+        The latents and pitch share one length.  Each sample's MSE row is then that of the sample alone; the loss, as in
+        the reference, is mean(mse) * mean(weight) over the batch (ns2.py:1651-1666), not the mean of the per-sample
+        losses.
 
         latent_lens (B,): sample b's latents are audio[b, :latent_lens[b]] (encoded latents, padded at the end, at most
         64 samples); its MSE row is the mean over those frames only, bit-identical to the sample alone, and its
         gradients are those of the sample alone (rows past the length add exact zeros).  Combines with prompt_lens /
-        phoneme_lens.  Not with raw audio (the codec encoder takes no lengths), the RVQ cross-entropy term (its frame
-        reduction has no lengths), train_duration_pitch or training dropout."""
+        phoneme_lens.  Raw audio (B, T) takes latent_lens in frames when the codec is an EncodecRVQ with an encoder:
+        sample b is audio[b, :latent_lens[b] * hop] (at least 7 frames), encoded as if alone
+        (`EncodecRVQ.forward(lengths=)`), and the latents (B, T // hop, dim) then take the path above.  With the RVQ
+        cross-entropy term (EncodecRVQ codecs only) the targets past each length are -1, the reference's ignore_index,
+        so each stage's term is the mean over the batch's valid frames.  Not with train_duration_pitch or training
+        dropout."""
         is_raw_audio = audio.ndim == 2
         aux_loss = None
         if latent_lens is not None:
-            self._check_latent_lens_training(audio, codes)
+            self._check_latent_lens_training(audio, codes, latent_lens)
         ragged = prompt_lens is not None or phoneme_lens is not None
         if ragged and not self.conditional:
             raise ValueError("prompt_lens / phoneme_lens apply to conditional models")
         if self.conditional and not (_exists(prompt_enc) and _exists(cond)):
+            prompt = self._encode_prompt(prompt, prompt_lens)
             if not _exists(self.conditioner):
                 raise NotImplementedError(
                     "conditional training needs prompt_enc= and cond= or a `conditioner` callable (the "
@@ -340,7 +369,8 @@ class NaturalSpeech2(nn.Module):
         assert not (is_raw_audio and not _exists(self.codec)), \
             "codec must be passed in if one were to train on raw audio"
         if is_raw_audio:
-            audio, codes, _ = self.codec(audio, return_encoded=True)
+            extra = {} if latent_lens is None else {"lengths": latent_lens}
+            audio, codes, _ = self.codec(audio, return_encoded=True, **extra)
         audio = audio.float().contiguous()
         batch, n, d = audio.shape
         device = self.device
@@ -384,12 +414,18 @@ class NaturalSpeech2(nn.Module):
         loss = (loss * loss_weight).mean()
         if self.rvq_cross_entropy_loss_weight == 0 or not _exists(codes):   # ns2.py:1670-1671
             return loss if aux_loss is None else loss + aux_loss
-        # cross entropy of the predicted x_start against the codec's codes (ns2.py:1673-1684)
+        # cross entropy of the predicted x_start against the codec's codes (ns2.py:1673-1684); with latent_lens the
+        # targets past each length are -1 (ignored) and x_start is zero there
+        if llens is not None:
+            codes = codes_past_lengths(codes.reshape(batch, n, -1).to(torch.int64), llens.tolist())
         if pred.requires_grad and isinstance(self.codec, EncodecRVQ):
-            ce_loss = XStartCrossEntropyFunction.apply(pred, audio, alpha, sigma, self.codec, codes, self.objective)
+            ce_loss = XStartCrossEntropyFunction.apply(pred, audio, alpha, sigma, self.codec, codes, self.objective,
+                                                       llens)
         else:   # no gradient wanted, or a codec other than EncodecRVQ (its `rq` gets a constant x_start)
             x_start = torch.empty_like(audio)
             ops.x_start_from_pred(audio, pred.detach(), alpha, sigma, x_start, objective=self.objective)
+            if llens is not None:
+                ops.mask_rows(x_start, llens)
             _, ce_loss = self.codec.rq(x_start, codes)
         loss = loss + self.rvq_cross_entropy_loss_weight * ce_loss
         return loss if aux_loss is None else loss + aux_loss
@@ -414,9 +450,12 @@ class XStartCrossEntropyFunction(torch.autograd.Function):
     so it returns d pred directly."""
 
     @staticmethod
-    def forward(ctx, pred, audio, alpha, sigma, codec, codes, objective):
+    def forward(ctx, pred, audio, alpha, sigma, codec, codes, objective, lens=None):
         x_start = torch.empty_like(audio)
         ops.x_start_from_pred(audio, pred.detach(), alpha, sigma, x_start, objective=objective)
+        if lens is not None:   # latent lengths: frames past them (targets -1) are zero, whatever the padding held
+            ops.mask_rows(x_start, lens)
+        ctx.lens = lens
         flat = x_start.view(-1, 128)
         tgt = codes.reshape(-1, codec.num_quantizers).to(torch.int64).contiguous()
         prep = codec._prep()
@@ -433,4 +472,7 @@ class XStartCrossEntropyFunction(torch.autograd.Function):
         d_pred = ops.rvq_ce_bwd(flat, codebooks, cn2, own, tgt, d_loss.float().reshape(1).contiguous(), row_scale=coef,
                                 rows_per_sample=ctx.rows_per_sample)
         n = ctx.rows_per_sample
-        return d_pred.view(flat.shape[0] // n, n, 128), None, None, None, None, None, None
+        d_pred = d_pred.view(flat.shape[0] // n, n, 128)
+        if ctx.lens is not None:   # frames whose targets are all -1 get nothing; written as +0 whatever the row scale
+            ops.mask_rows(d_pred, ctx.lens)
+        return d_pred, None, None, None, None, None, None, None

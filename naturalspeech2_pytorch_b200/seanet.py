@@ -35,6 +35,42 @@ SUPPORTED = dict(audio_channels=1, num_filters=32, upsampling_ratios=(8, 5, 4, 2
                  trim_right_ratio=1.0, use_conv_shortcut=True)
 
 
+# The shortest waveform, in frames, that the encoder reads as a prefix of a longer one.  Every conv pads on the left by
+# reflection, and Encodec reflects an input no longer than the pad around appended zeros instead.  The binding stage is
+# the last conv (k7, pad 6) at the frame rate: n frames need n > 6.  The others pad at most 8 rows at 8 or more rows
+# per frame (pads 6, 2, 2 at 320; 2, 4 at 160; 2, 5 at 40; 2, 8 at 8), so n >= 2 satisfies them.
+MIN_FRAMES = 7
+
+
+def frame_lengths(lengths, batch: int, frames: int, *, device, lo: int = MIN_FRAMES) -> list:
+    """Per-sample frame counts of a batch padded at the end, checked before anything runs: one integer per sample (a
+    sequence, or an integer tensor on the CPU or on `device`), each in [lo, frames], at most
+    NS2_GEMM_ROW_LENS_MAX_BATCHES samples.  Returns them as a list of ints."""
+    if isinstance(lengths, torch.Tensor):
+        if lengths.is_floating_point() or lengths.is_complex() or lengths.dtype == torch.bool:
+            raise ValueError(f"lengths must hold integers, got {lengths.dtype}")
+        if lengths.device.type != "cpu" and lengths.device != torch.device(device):
+            raise ValueError(f"lengths must be on the CPU or on the audio's device {device}, got {lengths.device}")
+        if lengths.dim() > 1:
+            raise ValueError(f"lengths must be one-dimensional, got shape {tuple(lengths.shape)}")
+        host = [int(v) for v in lengths.tolist()] if lengths.dim() == 1 else [int(lengths)]
+    else:
+        host = [int(v) for v in lengths]
+    if len(host) != batch:
+        raise ValueError(f"lengths must hold one length per sample ({batch}), got {len(host)}")
+    cap = _lib.NS2_GEMM_ROW_LENS_MAX_BATCHES
+    if batch > cap:
+        raise ValueError(f"lengths: at most {cap} samples per call, got {batch}")
+    if host and min(host) < lo:
+        why = " (shorter waveforms fall under Encodec's short-input padding rule when encoded alone)" \
+            if lo == MIN_FRAMES else ""
+        raise ValueError(f"lengths must be >= {lo} frames{why}, got {min(host)}")
+    if host and max(host) > frames:
+        raise ValueError(f"the input holds {frames} frames, fewer than the longest length {max(host)} "
+                         f"(lengths count frames of 320 samples)")
+    return host
+
+
 def lstm_gate_perm() -> torch.Tensor:
     """Row order of the packed LSTM weights (include/ns2_b200.h section 10): packed row 128 c + 64 hf + 16 w + 8 i + q
     is PyTorch row (2 hf + i) * 512 + 32 c + 8 w + q (gate 2 hf + i of hidden unit 32 c + 8 w + q)."""
@@ -251,24 +287,27 @@ class _SEANet(_PackedCache):
     # stages
     # ----------------------------------------------------------------------------------------------
     @staticmethod
-    def _lstm_stage(P, ws, y: torch.Tensor, out: torch.Tensor) -> None:
-        """out = lstm(y)[0] + y, y and out (B, N, 512) fp32."""
+    def _lstm_stage(P, ws, y: torch.Tensor, out: torch.Tensor, row_lens=None) -> None:
+        """out = lstm(y)[0] + y, y and out (B, N, 512) fp32.  row_lens (optional): the input projections compute only
+        the 128-row tiles that start before them; the recurrence runs over every row (it is causal)."""
         ops.elu_pad(y, ws["xb"], pad=0, elu=False)
-        ops.gemm(ws["xb"], P["l0_wih"], ws["xp"], n=2048, epilogue=ops.EPI_F32, bias=P["l0_b"])
+        ops.gemm(ws["xb"], P["l0_wih"], ws["xp"], n=2048, epilogue=ops.EPI_F32, bias=P["l0_b"], row_lens=row_lens)
         ops.lstm_seq(ws["xp"], P["l0_whh"], out_bf16=ws["xb"])
-        ops.gemm(ws["xb"], P["l1_wih"], ws["xp"], n=2048, epilogue=ops.EPI_F32, bias=P["l1_b"])
+        ops.gemm(ws["xb"], P["l1_wih"], ws["xp"], n=2048, epilogue=ops.EPI_F32, bias=P["l1_b"], row_lens=row_lens)
         ops.lstm_seq(ws["xp"], P["l1_whh"], skip=y, out=out)
 
     @staticmethod
-    def _resblock_stage(P, ws, si: int, x: torch.Tensor, c: int) -> torch.Tensor:
-        """ResnetBlock(c, hidden c / 2) of x (B, L, c) fp32 -> (B, L, c) fp32, a view of `z{si}`."""
+    def _resblock_stage(P, ws, si: int, x: torch.Tensor, c: int, row_lens=None) -> torch.Tensor:
+        """ResnetBlock(c, hidden c / 2) of x (B, L, c) fp32 -> (B, L, c) fp32, a view of `z{si}`.  row_lens (optional):
+        per-sample row counts of the padded (B, L + 2) buffers, passed to both GEMMs."""
         h = c // 2
         blk, hb, zo = ws[f"blk{si}"], ws[f"h{si}"], ws[f"z{si}"]
         ops.elu_pad(x, blk, pad=2, elu=True, raw=True)              # [ELU(x) | x], reflect-padded by 2
-        ops.gemm(blk, P[f"r{si}_w3"], hb, n=h, epilogue=ops.EPI_F32, segs=ops.conv_segs(c, 3, 2), bias=P[f"r{si}_b3"])
+        ops.gemm(blk, P[f"r{si}_w3"], hb, n=h, epilogue=ops.EPI_F32, segs=ops.conv_segs(c, 3, 2), bias=P[f"r{si}_b3"],
+                 row_lens=row_lens)
         ops.elu_pad(hb[:, 2:], blk[:, 2:, 2 * c:], pad=0, elu=True)
         ops.gemm(blk, P[f"r{si}_w1"], zo, n=c, epilogue=ops.EPI_F32,
-                 segs=[(c, 0, c, 0, 0), (2 * c, c, h, 0, 0)], bias=P[f"r{si}_b1"])
+                 segs=[(c, 0, c, 0, 0), (2 * c, c, h, 0, 0)], bias=P[f"r{si}_b1"], row_lens=row_lens)
         return zo[:, 2:]
 
 
@@ -420,8 +459,14 @@ class SEANetEncoder(_SEANet):
         return ws
 
     @torch.no_grad()
-    def forward(self, audio: torch.Tensor) -> torch.Tensor:
-        """audio (B, T) or (B, 1, T), T % 320 == 0 -> frames (B, T / 320, 128) fp32, a new tensor per call."""
+    def forward(self, audio: torch.Tensor, *, lengths=None) -> torch.Tensor:
+        """audio (B, T) or (B, 1, T), T % 320 == 0 -> frames (B, T / 320, 128) fp32, a new tensor per call.
+
+        lengths (B,) (optional, frames, in [MIN_FRAMES, T / 320], at most NS2_GEMM_ROW_LENS_MAX_BATCHES samples): a
+        batch of waveforms padded at the end, sample b being audio[b, :320 lengths[b]].  Its frames [0, lengths[b]) are
+        then bit-identical to encoding that waveform alone, whatever the padding holds (NaN included), and its frames
+        past it are exact zeros.  Every conv GEMM computes only the 128-row tiles that start before a sample's length
+        at its rate; the full-rate head, the operand preparation and the LSTM recurrence run over the padded rows."""
         if audio.dim() == 3 and audio.shape[1] == 1:
             audio = audio[:, 0]
         if audio.dim() != 2:
@@ -431,15 +476,27 @@ class SEANetEncoder(_SEANet):
             raise ValueError(f"SEANetEncoder needs T % 320 == 0 (the product of the strides), got T={T}")
         dev = audio.device
         N = T // 320
+        host_lens = None if lengths is None else frame_lengths(lengths, B, N, device=dev)
         if B == 0 or T == 0:
             return torch.empty(B, N, 128, device=dev, dtype=torch.float32)
         frames = torch.empty(B, N + 6, 128, device=dev, dtype=torch.float32)
         with torch.cuda.device(dev):
+            strides = tuple(reversed(RATIOS))
+            rl = {}   # per-stage GEMM row counts: padded buffers hold 1 (strided), 2 (ResnetBlock) or 6 leading rows
+            if host_lens is not None:
+                def rows(pad, rate, name):
+                    return ops.lengths([pad + n * rate for n in host_lens], B, None, device=dev, name=name)
+                rate = 320
+                for si, s in enumerate(strides):
+                    rate //= s
+                    rl[f"s{si}"] = rows(1, rate, f"stride {s} conv rows")
+                    if si < len(strides) - 1:
+                        rl[f"r{si}"] = rows(2, rate, f"ResnetBlock {si} rows")
+                rl["lstm"], rl["c15"] = rows(0, 1, "frames"), rows(6, 1, "last conv rows")
             P, ws = self.packed(), self._workspace(B, T, dev)
             x = audio.float()
             if x.stride(1) != 1:
                 x = x.contiguous()
-            strides = tuple(reversed(RATIOS))
             a, L, c_in = ws["a0"], T, 32
             ops.seanet_head(x, P["head"], a)                       # bf16(ELU(z1)) reflect-padded by 2
             for si, s in enumerate(strides):
@@ -447,15 +504,18 @@ class SEANetEncoder(_SEANet):
                 L //= s
                 y = ws[f"y{si}"]
                 ops.gemm(a.view(B, L + 1, s * c_in), P[f"s{si}_w"], y, n=c_out, epilogue=ops.EPI_F32,
-                         segs=strided_conv_segs(s, c_in), bias=P[f"s{si}_b"])
+                         segs=strided_conv_segs(s, c_in), bias=P[f"s{si}_b"], row_lens=rl.get(f"s{si}"))
                 y = y[:, 1:]
                 if si == len(strides) - 1:
                     break
                 a = ws[f"a{si + 1}"]
-                ops.elu_pad(self._resblock_stage(P, ws, si, y, c_out), a, pad=strides[si + 1], elu=True)
+                ops.elu_pad(self._resblock_stage(P, ws, si, y, c_out, row_lens=rl.get(f"r{si}")), a,
+                            pad=strides[si + 1], elu=True)
                 c_in = c_out
-            self._lstm_stage(P, ws, y, ws["lz"])
+            self._lstm_stage(P, ws, y, ws["lz"], row_lens=rl.get("lstm"))
             ops.elu_pad(ws["lz"], ws["a15"], pad=6, elu=True)
             ops.gemm(ws["a15"], P["c15_w"], frames, n=128, epilogue=ops.EPI_F32, segs=ops.conv_segs(512, 7, 6),
-                     bias=P["c15_b"])
+                     bias=P["c15_b"], row_lens=rl.get("c15"))
+            if host_lens is not None:
+                ops.mask_rows(frames[:, 6:], rl["lstm"])
         return frames[:, 6:]

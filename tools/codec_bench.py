@@ -1,11 +1,15 @@
 """Timing of SEANetDecoder and SEANetEncoder (Encodec 24 kHz decoder and encoder on the sm_90a kernels) against
 PyTorch (cuDNN LSTM and convs) in fp32 and bf16 on the same GPU:
-    python tools/codec_bench.py [--batch 32] [--frames 1024] [--reps 5] [--legs decode,encode] [--out codec_bench.json]
+    python tools/codec_bench.py [--batch 32] [--frames 1024] [--reps 5] [--legs decode,encode,ragged]
+                                [--min-frames 256] [--out codec_bench.json]
 Decodes (batch, frames, 128) latents and encodes (batch, 320 frames) samples of audio = batch x frames / 75 s of 24 kHz
 audio.  Reports ms per call (CUDA events around each call after warm-up, runs of the three implementations
 alternated, median), audio seconds per second, the output difference against the PyTorch fp32 path, and a per-stage
 split from a separate torch.profiler run; for the encoder also the head kernel's achieved FP32 rate (3,296 MACs per
-sample, from shapes).
+sample, from shapes).  The `ragged` leg encodes the same batch padded at the end, with per-sample lengths drawn
+uniformly from [--min-frames, frames] (seeded), through `SEANetEncoder(lengths=)` against the call without lengths
+(which computes every padded tile), alternated the same way; it reports the share of padded frames and checks that each
+sample's frames equal the unpadded call's prefix.
 """
 import argparse
 import json
@@ -84,6 +88,7 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--out", default=None)
     ap.add_argument("--legs", default="decode,encode")
+    ap.add_argument("--min-frames", type=int, default=256, help="ragged leg: shortest length drawn (>= 7)")
     a = ap.parse_args()
     B, N = a.batch, a.frames
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
@@ -91,7 +96,10 @@ def main():
     print(f"card: {card}")
     res = {"card": card, "batch": B, "frames": N, "audio_seconds": B * N / 75.0}
     for leg in a.legs.split(","):
-        res[leg] = {"decode": decode_leg, "encode": encode_leg}[leg](B, N, a.reps)
+        if leg == "ragged":
+            res[leg] = ragged_leg(B, N, a.reps, a.min_frames)
+        else:
+            res[leg] = {"decode": decode_leg, "encode": encode_leg}[leg](B, N, a.reps)
     if a.out:
         Path(a.out).parent.mkdir(parents=True, exist_ok=True)
         Path(a.out).write_text(json.dumps(res, indent=1))
@@ -152,6 +160,37 @@ def encode_leg(B, N, reps):
     print("stage split (ms, profiled call): " + ", ".join(f"{k} {v:.2f}" for k, v in split.items() if k != "tail"))
     print(f"head: {HEAD_MACS_PER_SAMPLE} MAC/sample, {res['head_tflops_fp32']:.1f} TFLOP/s FP32 achieved "
           f"(against the 67 TFLOP/s data-sheet FP32 peak)")
+    return res
+
+
+def _seeded_encoder():
+    keys_shapes = [(k, tuple(v.shape)) for k, v in SEANetEncoder().state_dict().items()]
+    enc = SEANetEncoder()
+    enc.load_state_dict({k: v.float() for k, v in genc.filled_state_dict(keys_shapes).items()})
+    return enc.cuda().eval()
+
+
+def ragged_leg(B, N, reps, min_frames):
+    lens = torch.randint(min_frames, N + 1, (B,), generator=torch.Generator().manual_seed(0)).tolist()
+    padded = 1.0 - sum(lens) / (B * N)
+    print(f"ragged encode: ({B}, {320 * N}) samples, lengths in [{min(lens)}, {max(lens)}] frames, "
+          f"{100 * padded:.1f} % padding")
+    enc = _seeded_encoder()
+    audio = genc.audio(B, N).float().cuda()
+    impls = {"no_lengths": enc, "lengths": lambda x: enc(x, lengths=lens)}
+    outs = {k: f(audio) for k, f in impls.items()}     # warm-up
+    for b, n in enumerate(lens):
+        assert torch.equal(outs["lengths"][b, :n], outs["no_lengths"][b, :n]), b
+    times = {k: [] for k in impls}
+    for _ in range(reps):
+        for k, f in impls.items():
+            times[k].append(time_ms(f, audio))
+    res = {"lengths": lens, "padded_share": padded}
+    for k in impls:
+        ms = sorted(times[k])[len(times[k]) // 2]
+        res[k] = {"ms_median": ms, "ms_all": times[k], "audio_s_per_s": sum(lens) / 75.0 / (ms / 1e3)}
+        print(f"{k:>11}: {ms:8.2f} ms/encode  {res[k]['audio_s_per_s']:9.0f} unpadded audio s/s  "
+              f"runs {[round(t, 2) for t in times[k]]}")
     return res
 
 
